@@ -1,9 +1,9 @@
-"""attention-lvcsr_b200 -- B200-native hot path of rizar/attention-lvcsr.
+"""attention-lvcsr_b200 -- H100-native hot path of rizar/attention-lvcsr.
 
 The directory name contains a hyphen (it is the contract's name); import it through
 ``__graft_entry__.load_package()`` which registers it as ``attention_lvcsr_b200``.
 
-Only what the path needs lives here: ``csrc/`` (sm_100a kernels + the C ABI of
+Only what the path needs lives here: ``csrc/`` (sm_90a kernels + the C ABI of
 include/lvsr_b200.h) and the host-side mirror of the reference's operator surface
 (``SpeechRecognizer``, ``BeamSearch``, initialisation/config tokens).
 """

@@ -1,4 +1,4 @@
-// C ABI of the B200-native attention-lvcsr hot path (see include/lvsr_b200.h).
+// C ABI of the H100-native attention-lvcsr hot path (see include/lvsr_b200.h).
 //
 // Host-side orchestration only: which kernel runs when, on which buffers.  The
 // compiled-function seam it replaces is SURVEY.md section 8b tier b3
@@ -285,7 +285,7 @@ int lvsr_model_create(const lvsr_config* cfg, lvsr_model** out) {
   LVSR_CHECK(cfg->num_phonemes >= 1 && cfg->num_phonemes <= 128, "num_phonemes out of range");
   int dev_count = 0;
   LVSR_CUDA_OK(cudaGetDeviceCount(&dev_count));
-  LVSR_CHECK(dev_count > 0, "no CUDA device: the B200 path has no CPU fallback");
+  LVSR_CHECK(dev_count > 0, "no CUDA device: the GPU path has no CPU fallback");
   lvsr_model* m = new lvsr_model();
   m->cfg = *cfg;
   LVSR_CUDA_OK(cudaGetDevice(&m->device));
@@ -412,8 +412,8 @@ int lvsr_model_finalize(lvsr_model* m) {
 namespace lvsr {
 // fp16 head/tail operands for the projections that read BiGRU outputs (|h| <= 1): layers >= 1 and preprocess.
 // Allocated and split at their first use after a parameter change, i.e. AFTER the caller has reserved the workspace arena:
-// the arena keeps the device pages it gets without these buffers (the persistent decoder's step time moves by up to 10 %
-// with the physical placement of its buffers, profiles/r2k_summary.md).
+// the arena keeps the device pages it gets without these buffers (the persistent decoder's step time can move with the
+// physical placement of its buffers).
 int ensure_h16(lvsr_model* m, cudaStream_t st) {
   if (!m->use_tc || !m->use_h16 || !m->h16_stale) return 0;
   const lvsr_config& c = m->cfg;
@@ -534,9 +534,8 @@ int finalize_on_stream(lvsr_model* m, cudaStream_t st, bool synchronise) {
       if (int rc = split_weight_tf32(m->P(std::string(ATT) + "/preprocess.W"), m->E, c.dim_matcher, m->Wp_hi, m->Wp_lo, st))
         return rc;
     // fp16 head/tail operands of the same weights: re-split lazily at their next use (ensure_h16).  Opt-in
-    // (LVSR_F16_GEMM=1): the GEMM class drops from 1.89 to 1.63 ms at the metric batch, but the extra device allocations move
-    // the workspace to other physical pages, and the persistent decoder happened to lose more than that on the benchmarked
-    // allocation sequence (51.2 -> 55.3 us per step; placement sweep in profiles/r2k_summary.md).
+    // (LVSR_F16_GEMM=1): half the operand bytes of the GEMMs, but extra device allocations that move the workspace to other
+    // physical pages, which the persistent decoder's step time is sensitive to.
     m->use_h16 = getenv("LVSR_F16_GEMM") != nullptr && atoi(getenv("LVSR_F16_GEMM")) != 0;
     m->h16_stale = true;
   }

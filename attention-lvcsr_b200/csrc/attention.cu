@@ -6,7 +6,7 @@
 // (:98-114), normaliser (:191-213), weighted average (B/bricks/attention.py:235-256)
 // and the paste back into [R, T'] (:177-181).
 //
-// B200 mapping: a row's P/H slices (T' x (M+E) floats, ~1 MB) are streamed once per
+// Mapping: a row's P/H slices (T' x (M+E) floats, ~1 MB) are streamed once per
 // step; a thread-block CLUSTER of `cs` CTAs splits the window of one row along time,
 // each CTA produces a local (max, sum, weighted partial context) triple and the
 // cluster combines them through distributed shared memory (online-softmax merge) --

@@ -4,15 +4,14 @@
 // (dec_scan.cu).  Math follows lvsr/bricks/attention.py:98-114,120-183,191-213 and
 // libs/blocks/blocks/bricks/attention.py:235-256.
 //
-// r1d -> r1e (profiles/): the first version spent 8.7 us in the conv, 13 us in the energies
-// (issue/latency bound: ~17 instructions per (t,m) element) and 4.5 us in the context pass.
-// Now:
+// A plain FFMA version is issue/latency bound in the energies (~17 instructions per (t,m) element).
+// Hence:
 //   * conv: each thread owns one position and a quarter of the taps for ALL filters
 //     (2.5 FMA per shared-memory load instead of 1.4), quarters meet by two shuffles;
 //   * energies: match = P + q + F.Wh runs on the tensor cores -- mma.sync m16n8k16 bf16 with
 //     fp32 accumulate, P (+q) is the accumulator init (so P and q stay exact fp32), and the
 //     K<=16 handler product uses a 3-term hi/lo bf16 split of both operands (error ~2^-17 of
-//     the location term only).  tcgen05 does not apply: K = 10, the accumulator is consumed
+//     the location term only).  wgmma does not apply: K = 10, the accumulator is consumed
 //     immediately by tanh in registers, and each warp owns a private 16x32 strip;
 //   * tanh = 1 - 2/(1+2^(2x log2e)): 2 MUFU + 3 FP32 instructions, |err| ~ 2e-7;
 //   * context: 8 independent 16-byte loads in flight per thread, 512 threads.

@@ -5,7 +5,7 @@
 // child of Bidirectional (B/bricks/recurrent.py:224-231, 608-620, 655-663) plus the
 // x[::k] subsampling of Encoder.apply (lvsr/bricks/__init__.py:75-77).
 //
-// B200 mapping (two DEPENDENT [rows,D]x[D,*] products per step, T sequential steps):
+// Mapping (two DEPENDENT [rows,D]x[D,*] products per step, T sequential steps):
 //   * batch rows are independent -> a thread-block CLUSTER of CS CTAs owns RB = 4 rows of one
 //     direction; clusters never talk to each other (no grid-wide barrier).
 //   * inside a cluster the hidden units are split: CTA `rank` owns UC = D/CS units, each of its
@@ -21,12 +21,9 @@
 //   * the fork pre-activations of step t+1 are prefetched into registers during step t.
 //   * TAPE (training): the gates / candidate overwrite the pre-activations they were computed from and every
 //     frame of h is kept (hext), for the reverse-time scan of bigru_bwd.cu; compiled out of the inference kernel.
-// History (profiles/): r1a 4-byte remote stores + barrier.cluster (30 % of the kernel in the fence, 8.6 us/step)
-// -> bulk DSMEM copies + mbarrier (3.07 us) -> k over 8 lanes, FFMA2 (2.76 us) -> k over 16 lanes, 4 CTAs x 16 warps,
-// st.async from registers (2.34 us in the loop, 2.67 us/step with launch and staging): the products are bound by the
-// shared-memory return path of the h loads, the rest is lock-step latency (profiles/r1g_summary.md)
-// -> round 2: hidden size 256 runs bigru_mma_kernel below (mma.sync on fp16 head/tail splits, weights as the M dimension,
-// warp-specialised): 1.40 us per step (profiles/r2i_summary.md); the FFMA kernel stays for the other hidden sizes.
+// The FFMA products are bound by the shared-memory return path of the h loads, the rest is lock-step latency.  Hidden
+// size 256 runs bigru_mma_kernel below (mma.sync on fp16 head/tail splits, weights as the M dimension, warp-specialised);
+// the FFMA kernel stays for the other hidden sizes and as the reference the tensor-core kernel is tested against.
 #include <cuda_fp16.h>
 
 #include "kernels.h"
@@ -96,15 +93,15 @@ __device__ __forceinline__ void st_async_v4(uint32_t remote_addr, float x, float
 //                       reset gates) and half of its candidate columns.
 // A lane accumulates RB x 4 gate sums and RB x 2 candidate sums over its D/16 k values; the
 // cross-lane reduction runs over the 16 kg-lanes: 15 + 8 exchanges per step.  The split is a
-// measured trade (LVSR_BIGRU_TRACE): every lane must read its k range of h for all rows, and the
-// shared-memory RETURN path (128 B/clk/SM, 4 cycles per warp-wide 16-byte load) is what bounds a
-// phase -- k over 8 lanes: 72 loads per warp and step, 4.6 k cycles; k over 32 lanes: 24 loads but
-// 46 exchanges and ~1000 instructions per warp and step (issue-bound); 16 lanes sits between.
+// trade: every lane must read its k range of h for all rows, and the shared-memory RETURN path
+// (128 B/clk/SM, 4 cycles per warp-wide 16-byte load) is what bounds a phase -- k over 8 lanes:
+// 72 loads per warp and step; k over 32 lanes: 24 loads but 46 exchanges and ~1000 instructions
+// per warp and step (issue-bound); 16 lanes sits between.
 //
 // Two shapes: <D, 8 or 4 CTAs, 8 warps> = 256 threads, two CTAs (two different clusters) per SM,
 // and <256, 4 CTAs, 16 warps> = 512 threads, one CTA per SM.  At the metric batch the second wins:
 // with two clusters sharing every SM any stall of one CTA delays its whole 8-CTA cluster twice per
-// step (1.73 us per step when a narrow CTA owns its SM vs 3.07 us when two share one).
+// step.
 // TAPE: training forward (stores c / z / r over the pre-activations and every frame of h); compiled out for inference
 template <int D, int CS, int NWARP, bool TAPE>
 __global__ void __launch_bounds__(NWARP * 32, NWARP == 8 ? 2 : 1)
@@ -126,7 +123,7 @@ bigru_kernel(BiGruArgs a) {
 
   // h and h*r of all units, in chunks of 32 units: chunk c holds [RB][32] floats + 16 bytes of pad.
   // The 8 kg lanes of a warp read 8 different chunks (or half chunks) at the same offset; without
-  // the pad that is an 8-way bank conflict on every load (measured: 2x the step time).
+  // the pad that is an 8-way bank conflict on every load.
   constexpr int CH = 32, NCH = D / CH, SLOT = RB * CH + 4;
   __shared__ __align__(128) float hbuf[NCH][SLOT];
   __shared__ __align__(128) float hrbuf[NCH][SLOT];
@@ -153,17 +150,17 @@ bigru_kernel(BiGruArgs a) {
 
   // ---- weights -> registers / shared memory (once) -----------------------------------
   // gate column cl of the warp (0..NC1): cl < NC2 -> update gate of unit u_warp + cl, else reset gate
-  // packed pairs (k, k+1): one FFMA2 (fma.rn.f32x2) advances the even-k and the odd-k partial sum
-  // of a column at once -- h arrives as (k, k+1) register pairs from the 16-byte loads anyway
-  unsigned long long w1[CPL1][KPG / 2];
+  // pairs (k, k+1): the even-k and the odd-k partial sum of a column advance side by side (fma2) --
+  // h arrives as (k, k+1) register pairs from the 16-byte loads anyway
+  float2 w1[CPL1][KPG / 2];
 #pragma unroll
   for (int j = 0; j < CPL1; ++j) {
     const int cl = cg * CPL1 + j;
     const int col = (cl < NC2) ? (u_warp + cl) : (D + u_warp + (cl - NC2));
 #pragma unroll
     for (int kk = 0; kk < KPG / 2; ++kk)
-      w1[j][kk] = pack_f32x2(Wg[(long long)(kg * KPG + 2 * kk) * (2 * D) + col],
-                             Wg[(long long)(kg * KPG + 2 * kk + 1) * (2 * D) + col]);
+      w1[j][kk] = make_float2(Wg[(long long)(kg * KPG + 2 * kk) * (2 * D) + col],
+                              Wg[(long long)(kg * KPG + 2 * kk + 1) * (2 * D) + col]);
   }
 #pragma unroll
   for (int q = 0; q < KQ; ++q)
@@ -278,25 +275,25 @@ bigru_kernel(BiGruArgs a) {
     // ---- phase 1: gates of the owned units -----------------------------------------
     float acc1[N1];
     {
-      unsigned long long ap[N1];
+      float2 ap[N1];
 #pragma unroll
-      for (int i = 0; i < N1; ++i) ap[i] = 0ull;
+      for (int i = 0; i < N1; ++i) ap[i] = make_float2(0.f, 0.f);
 #pragma unroll
       for (int q = 0; q < KQ; ++q) {
 #pragma unroll
         for (int r = 0; r < RB; ++r) {
-          const ulonglong2 v = *reinterpret_cast<const ulonglong2*>(&hbuf[kpeer][r * CH + koff + q * 4]);
+          const float4 v = *reinterpret_cast<const float4*>(&hbuf[kpeer][r * CH + koff + q * 4]);
 #pragma unroll
           for (int j = 0; j < CPL1; ++j) {
-            unsigned long long sacc = ap[r * CPL1 + j];
-            sacc = ffma2(v.x, w1[j][q * 2 + 0], sacc);
-            sacc = ffma2(v.y, w1[j][q * 2 + 1], sacc);
+            float2 sacc = ap[r * CPL1 + j];
+            sacc = fma2(make_float2(v.x, v.y), w1[j][q * 2 + 0], sacc);
+            sacc = fma2(make_float2(v.z, v.w), w1[j][q * 2 + 1], sacc);
             ap[r * CPL1 + j] = sacc;
           }
         }
       }
 #pragma unroll
-      for (int i = 0; i < N1; ++i) acc1[i] = sum_f32x2(ap[i]);
+      for (int i = 0; i < N1; ++i) acc1[i] = sum2(ap[i]);
     }
     BG_STAMP(1);
     warp_reduce_scatter<N1, CG>(acc1, lane);
@@ -318,28 +315,28 @@ bigru_kernel(BiGruArgs a) {
     BG_STAMP(3);
     float acc2[N2];
     {
-      unsigned long long ap[N2];
+      float2 ap[N2];
 #pragma unroll
-      for (int i = 0; i < N2; ++i) ap[i] = 0ull;
+      for (int i = 0; i < N2; ++i) ap[i] = make_float2(0.f, 0.f);
 #pragma unroll
       for (int q = 0; q < KQ; ++q) {
-        ulonglong2 w[CPL2];
+        float4 w[CPL2];
 #pragma unroll
-        for (int c2 = 0; c2 < CPL2; ++c2) w[c2] = *reinterpret_cast<const ulonglong2*>(&w2s[warp][q][c2][lane][0]);
+        for (int c2 = 0; c2 < CPL2; ++c2) w[c2] = *reinterpret_cast<const float4*>(&w2s[warp][q][c2][lane][0]);
 #pragma unroll
         for (int r = 0; r < RB; ++r) {
-          const ulonglong2 v = *reinterpret_cast<const ulonglong2*>(&hrbuf[kpeer][r * CH + koff + q * 4]);
+          const float4 v = *reinterpret_cast<const float4*>(&hrbuf[kpeer][r * CH + koff + q * 4]);
 #pragma unroll
           for (int c2 = 0; c2 < CPL2; ++c2) {
-            unsigned long long sacc = ap[r * CPL2 + c2];
-            sacc = ffma2(v.x, w[c2].x, sacc);
-            sacc = ffma2(v.y, w[c2].y, sacc);
+            float2 sacc = ap[r * CPL2 + c2];
+            sacc = fma2(make_float2(v.x, v.y), make_float2(w[c2].x, w[c2].y), sacc);
+            sacc = fma2(make_float2(v.z, v.w), make_float2(w[c2].z, w[c2].w), sacc);
             ap[r * CPL2 + c2] = sacc;
           }
         }
       }
 #pragma unroll
-      for (int i = 0; i < N2; ++i) acc2[i] = sum_f32x2(ap[i]);
+      for (int i = 0; i < N2; ++i) acc2[i] = sum2(ap[i]);
     }
     BG_STAMP(4);
     warp_reduce_scatter<N2, CG>(acc2, lane);
@@ -433,8 +430,8 @@ int launch_bigru_t(const BiGruArgs& a, cudaStream_t stream) {
 // fp32 accuracy from fp16 operands: every operand is split into an fp16 head and an fp16 tail scaled by
 // 2^11 (x = head + tail / 2048; both exact to ~2^-22 of x) and
 //     head_w * head_h + (head_w * tail_h + tail_w * head_h) / 2048
-// is accumulated in fp32 -- the error class of the 3xTF32 GEMMs at twice the MAC rate of tf32 (measured: 2.0 cycles
-// per m16n8k8-tf32 or m16n8k16-f16 MMA and SM, tools/micro/mma_rate.cu).  It takes TWO MMAs per 16 k, not three: the
+// is accumulated in fp32 -- the error class of the 3xTF32 GEMMs with an m16n8k16 fp16 MMA covering twice the k of an
+// m16n8k8 tf32 one.  It takes TWO MMAs per 16 k, not three: the
 // N columns 0..3 of the B operand carry the heads of the four rows and the columns 4..7 their tails, so
 // A = head_w yields head*head and head*tail in one instruction; the second one has A = tail_w.
 // Weights are split once and stay in registers as ready-made A fragments (192 per lane).  h and h*r are split by the
@@ -1003,7 +1000,7 @@ int bigru_layer(const BiGruArgs& a, cudaStream_t stream) {
   bool wide = a.D == 256 && 8 * groups * 2 > bigru_sm_count() && groups * 2 <= wide_clusters_resident();
   if (const char* e = getenv("LVSR_BIGRU_WIDE")) wide = a.D == 256 && atoi(e) != 0;
   // hidden size 256: tensor-core products.  Clusters never talk to each other, so a batch with more clusters than the
-  // device holds at once (mma_clusters_resident: 33 on a B200, i.e. more than 66 rows) simply runs in waves -- still
+  // device holds at once (mma_clusters_resident, from the occupancy query) simply runs in waves -- still
   // ahead of the FFMA kernels, which would have to put two or more CTAs on every SM for such a batch.
   bool mma = a.D == 256 && mma_clusters_resident<256>() > 0;
   if (const char* e = getenv("LVSR_BIGRU_MMA")) mma = a.D == 256 && atoi(e) != 0;

@@ -14,7 +14,7 @@
 // saved c, z, r) and h*r for every step, and the caller turns them into four large GEMMs
 // (dW_fork = X^T dPre, dX = dPre W_fork^T, dW_s = (h*r)^T dA, dW_g = H_prev^T [dGz|dGr]).
 //
-// B200 mapping: a cluster of CS CTAs owns RB = 4 batch rows of one direction, CTA `rank` owns 32
+// Mapping: a cluster of CS CTAs owns RB = 4 batch rows of one direction, CTA `rank` owns 32
 // hidden units.  Per step the owned dA (then [dGz|dGr]) of all 4 rows travel as ONE 16-byte
 // `st.async` per unit and peer into the receivers' shared memory, crediting the receiver's
 // mbarrier -- the all-gather machinery of the forward kernel.  W_s^T slice in registers, W_g^T

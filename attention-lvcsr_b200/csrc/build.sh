@@ -1,9 +1,16 @@
 #!/bin/bash
-# Build liblvsr_b200.so (sm_100a only) in-tree.  Usage: build.sh [extra nvcc flags]
+# Build liblvsr_b200.so (sm_90a only) in-tree.  Usage: build.sh [extra nvcc flags]
 set -euo pipefail
 cd "$(dirname "$0")"
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
-FLAGS="-gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -I../../include -I."
+ARCH="-gencode arch=compute_90a,code=sm_90a"
+FLAGS="$ARCH -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -I../../include -I."
+# objects built with other flags (another architecture, say) are stale too
+STAMP=build.flags
+if [ ! -f $STAMP ] || [ "$(cat $STAMP)" != "$FLAGS $*" ]; then
+  rm -f ./*.o
+  echo "$FLAGS $*" > $STAMP
+fi
 OBJS=()
 for f in gemm gemm_tc bigru bigru_bwd attention decoder dec_scan train search api; do
   stale=0
@@ -16,5 +23,5 @@ for f in gemm gemm_tc bigru bigru_bwd attention decoder dec_scan train search ap
   fi
   OBJS+=("$f.o")
 done
-$NVCC -gencode arch=compute_100a,code=sm_100a -shared -o liblvsr_b200.so "${OBJS[@]}" -lcudart
+$NVCC $ARCH -shared -o liblvsr_b200.so "${OBJS[@]}" -lcudart
 echo "built $(pwd)/liblvsr_b200.so"

@@ -1,4 +1,4 @@
-// Shared helpers for the sm_100a kernels of the attention-lvcsr hot path.
+// Shared helpers for the sm_90a kernels of the attention-lvcsr hot path.
 #pragma once
 #include <cuda_runtime.h>
 #include <cooperative_groups.h>
@@ -60,7 +60,7 @@ static inline int device_sm_count() {
   const int dev = current_device();
   if (sms[dev] == 0) {
     cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev);
-    if (sms[dev] <= 0) sms[dev] = 148;
+    if (sms[dev] <= 0) sms[dev] = 132;
   }
   return sms[dev];
 }
@@ -165,22 +165,11 @@ __device__ __forceinline__ float4 ld_flow_f4(const float* p) {
   return make_float4(__uint_as_float(x), __uint_as_float(y), __uint_as_float(z), __uint_as_float(w));
 }
 
-// Packed fp32 pair arithmetic (Blackwell FFMA2): d = a * b + c on both halves of a 64-bit register.
-__device__ __forceinline__ unsigned long long ffma2(unsigned long long a, unsigned long long b, unsigned long long c) {
-  unsigned long long d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+// fp32 pair arithmetic: two independent FFMA chains (even k in .x, odd k in .y), summed once at the end.
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
+  return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
 }
-__device__ __forceinline__ unsigned long long pack_f32x2(float lo, float hi) {
-  unsigned long long d;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(d) : "f"(lo), "f"(hi));
-  return d;
-}
-__device__ __forceinline__ float sum_f32x2(unsigned long long v) {
-  float lo, hi;
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-  return lo + hi;
-}
+__device__ __forceinline__ float sum2(float2 v) { return v.x + v.y; }
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

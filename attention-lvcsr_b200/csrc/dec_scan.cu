@@ -3,7 +3,7 @@
 // whole batch -- take_glimpses -> Distribute -> GatedRecurrent step -- i.e. the scan inside
 // BaseSequenceGenerator.evaluate (libs/blocks/blocks/bricks/sequence_generators.py:254-311).
 //
-// B200 mapping
+// Mapping
 //   * one CTA per SM, resident for the whole sequence; the GRU / state-transform weight
 //     slices of each CTA stay in SHARED MEMORY across all steps (2.75 MB spread over the
 //     grid), as do the attention constants (conv filters, handler, energy vector).

@@ -28,7 +28,7 @@ inline GemmArgs make_gemm(const float* A, int M, int K, const float* W, int N, c
   return g;
 }
 
-// ---- gemm_tc.cu: tcgen05 / TMEM / TMA path (3xTF32 split) ------------------------------
+// ---- gemm_tc.cu: wgmma / TMA path (3xTF32 split) -----------------------------------------
 bool gemm_tc_supported(int M, int N, int K);
 int gemm_tc_kpad(int K);                 // contraction dimension as stored in the hi/lo operands (multiple of 32)
 int split_weight_tf32(const float* W, int K, int N, float* Wt_hi, float* Wt_lo, cudaStream_t stream);
@@ -37,7 +37,7 @@ int split_tf32(const float* x, float* hi, float* lo, long long n, cudaStream_t s
 int gemm_tc_presplit(const float* A_hi, const float* A_lo, int M, const float* B_hi, const float* B_lo, int N, int Kpad,
                      const float* bias, float* C, int ldc, int splits, long long split_stride, cudaStream_t stream);
 int gemm_tc_splits_launched(int Kpad, int splits);   // how many partial outputs gemm_tc_presplit writes
-// fp16 head/tail variant (kind::f16): half the operand bytes and tensor time of the tf32 split; inputs of bounded range only
+// fp16 head/tail variant (fp16 wgmma): half the operand bytes and tensor time of the tf32 split; inputs of bounded range only
 bool gemm_tc_h16_supported(int M, int N, int K);
 int gemm_tc_kpad_h16(int K);             // contraction dimension as stored in the fp16 operands (multiple of 64)
 int split_weight_h16(const float* W, int K, int N, void* head, void* tail, float* scale2, cudaStream_t stream);

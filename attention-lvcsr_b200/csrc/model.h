@@ -117,7 +117,7 @@ struct lvsr_model {
   float* Wff_cat = nullptr;         // [Cfb, 3C] = [fork gate_inputs | fork inputs]
   float* bff_cat = nullptr;         // [3C]
   float* FF = nullptr;              // [(V+1), 3C] = lookup . Wff_cat + bff_cat
-  // K-major tf32 hi/lo splits of the dense-projection weights (tcgen05 path); null = SIMT path
+  // K-major tf32 hi/lo splits of the dense-projection weights (wgmma path); null = SIMT path
   std::vector<float*> Wcat_hi, Wcat_lo;
   float *Wp_hi = nullptr, *Wp_lo = nullptr;
   bool use_tc = true;

@@ -7,7 +7,7 @@
 // -> BurnIn and the in-place update.  The gradient buffer uses the flat parameter layout, so a data-parallel
 // caller all-reduces ONE buffer between lvsr_train_cost_and_grads and lvsr_train_apply_updates (SURVEY.md 8e).
 //
-// Structure of the backward pass (B200 view):
+// Structure of the backward pass:
 //   * everything that does not depend on the recurrence is a LARGE GEMM over all steps at once
 //     (weight gradients X^T dY as split-R TN products, input gradients dY W^T, the decoder's gate values
 //     re-computed for all L steps from the saved states and glimpses);
@@ -101,7 +101,7 @@ int copy2d(float* dst, int ld_dst, const float* src, int ld_src, int rows, int c
   return 0;
 }
 
-// K-major (contraction-major) tf32 hi/lo operand of the tcgen05 GEMM: [rows, Kpad] built from a [K, rows] matrix
+// K-major (contraction-major) tf32 hi/lo operand of the tensor-core GEMM: [rows, Kpad] built from a [K, rows] matrix
 struct TcOperand { float* hi = nullptr; float* lo = nullptr; int rows = 0, Kpad = 0; };
 
 // src [R, cols] (leading dimension ld) -> transposed hi/lo pair [cols, kpad(R)]
@@ -494,7 +494,7 @@ int lvsr_train_cost_and_grads(lvsr_model* m, const float* x, const float* mask, 
       float* dbcat = ws.f32((size_t)6 * D);
       LVSR_CHECK(dWcat && dbcat, "out of device memory (fork gradients)");
       // tensor-core path: every operand transposed once into K-major tf32 hi/lo pairs (the contraction runs over the
-      // T*B rows), then five split-K tcgen05 products share them; FFMA tiles for small problems / LVSR_NO_TC_GEMM
+      // T*B rows), then five split-K tensor-core products share them; FFMA tiles for small problems / LVSR_NO_TC_GEMM
       const bool tc = m->use_tc && rows >= 2048 && D % 128 == 0;
       TcOperand dPreT, XT, hrT, hpT[2];
       if (tc) {

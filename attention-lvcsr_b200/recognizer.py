@@ -67,7 +67,7 @@ class SpeechRecognizer(object):
                  max_decoded_length_scale=1, name="recognizer", device=None, **kwargs):
         # ---- what the CUDA path implements; everything else fails loudly ----------
         def unsupported(what):
-            raise NotImplementedError("attention-lvcsr_b200: %s is outside the B200 hot path "
+            raise NotImplementedError("attention-lvcsr_b200: %s is outside the GPU hot path "
                                       "(SURVEY.md section 8)" % what)
         if attention_type != "content_and_conv":
             unsupported("attention_type=%r" % attention_type)

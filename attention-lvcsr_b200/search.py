@@ -49,7 +49,7 @@ class BeamSearch(object):
     _smallest = staticmethod(_smallest)
 
     def compile(self):
-        """Nothing to compile: the kernels are ahead-of-time sm_100a code."""
+        """Nothing to compile: the kernels are ahead-of-time sm_90a code."""
         self.recognizer._require_ready()
         self.compiled = True
 

@@ -2,7 +2,7 @@
 """bench.py -- frames/sec of the attention-lvcsr hot path (encoder + teacher-forced
 attention decoder) at the BASELINE.json metric configuration.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 One "step" = one pass of the hot path over one synthetic batch per GPU:
@@ -11,11 +11,16 @@ B=64 utterances x T=1000 frames x F=40 filterbanks, 4x pyramidal BiGRU(256)
 GRU(256) decoder, L=125 teacher-forced steps, Maxout(2) readout over V=32 symbols.
 Multi-GPU: utterance batches shard across ranks (weak scaling, no data-path collective).
 
-Prints ONE JSON line on rank 0 (see the task contract): `value` = frames/s with inputs
+Prints ONE JSON line on rank 0: `value` = frames/s with inputs
 resident in HBM; `e2e` = same metric through the host-buffer C-ABI call
 (lvsr_recognizer_cost_host: pinned host inputs, H2D + D2H inside the timed region);
 `roofline` = attention-step kernel, algorithmic bytes / CUDA-event time vs the measured
-HBM peak; `cpu_baseline` = float32 twin of the oracle on a bounded sample of the workload.
+HBM peak; `cpu_baseline` = float32 twin of the oracle on a bounded sample of the workload;
+`gpu` = the card's name and power limit, which every absolute number above depends on.
+
+--dump-outputs DIR (metric mode): after the timed steps, the arrays the last timed step returned
+(encoder output, its mask, the [L, B] costs) go to DIR/<name>.npy as float32.  Inputs and weights come
+from fixed seeds, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -83,7 +88,7 @@ def init_values(shapes, seed=1, scale=10.0):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks + throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks + throttle reasons during the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -135,14 +140,28 @@ def measured_peaks():
     if os.path.exists(path):
         with open(path) as f:
             return json.load(f), "measured (MEASURED_PEAKS.json)"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0}, "fallback (B200_PROFILING.md)"
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "data sheet (H100 SXM, 700 W; not reached)"
 
 
-# DRAM traffic of ONE dec_scan_kernel launch at the metric configuration (dram__bytes_read.sum +
-# dram__bytes_write.sum of the `ncu --set full` capture summarised in profiles/r2a_summary.md /
-# profiles/r2a_dec_scan_metrics.csv), and the L2->SM bytes of the same capture.
-NCU_DEC_SCAN = {"config": (64, 1000, 125), "dram_bytes": 2.672282e9 + 1.510394e9, "l2_to_sm_bytes": 13.303018e9,
-                "l2_hit_pct": 70.18, "source": "profiles/r2a_dec_scan_metrics.csv"}
+def gpu_identity(index):
+    """Name, power limit and maximum SM clock of the card the numbers were measured on."""
+    out = {"name": None, "power_limit_w": None, "sm_max_mhz": None}
+    try:
+        r = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=name,power.limit,clocks.max.sm",
+                            "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=10)
+        if r.returncode == 0 and r.stdout.strip():
+            name, power, clock = [c.strip() for c in r.stdout.strip().splitlines()[0].split(",")]
+            out = {"name": name, "power_limit_w": float(power), "sm_max_mhz": float(clock)}
+    except Exception:
+        pass
+    return out
+
+
+def dump_outputs(directory, arrays):
+    """Write each array as DIR/<name>.npy (float32)."""
+    os.makedirs(directory, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(directory, name + ".npy"), a.detach().float().cpu().numpy())
 
 
 def attention_step_bytes(B, Tw, M, E):
@@ -458,7 +477,13 @@ def main():
     ap.add_argument("--no-train", action="store_true", help="metric mode: skip the training-step block")
     ap.add_argument("--batch", type=int, default=WORKLOAD["B"],
                     help="diagnostic only: utterances per GPU (the metric is quoted on the default)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="metric mode: write the arrays of the last timed step to DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and (args.impl != "ours" or args.mode != "metric"):
+        ap.error("--dump-outputs needs --impl ours --mode metric")
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
 
     rank = int(os.environ.get("RANK", "0"))
@@ -513,7 +538,7 @@ def main():
 
     def step_device():
         att, attm = rec.encode(xd, md)
-        return rec.cost_matrix(yd, ymd, att, attm)
+        return {"attended": att, "attended_mask": attm, "costs": rec.cost_matrix(yd, ymd, att, attm)}
 
     def step_host():
         return rec.cost(xh.numpy(), mh.numpy(), yh.numpy(), ymh.numpy())
@@ -526,17 +551,17 @@ def main():
         torch.cuda.synchronize(dev)
 
     def timed(fn, steps):
-        total_ms = 0.0
+        total_ms, last = 0.0, None
         for _ in range(steps):
             flush.fill_(1)                       # evict L2 between timed iterations
             torch.cuda.synchronize(dev)
             a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             a.record()
-            fn()
+            last = fn()
             b.record()
             torch.cuda.synchronize(dev)
             total_ms += a.elapsed_time(b)
-        return total_ms
+        return total_ms, last
 
     dist_mod = None
     if world > 1:
@@ -546,11 +571,11 @@ def main():
         sampler = ClockSampler(local_rank)
         sampler.start()
         if args.mode == "search":
-            sr = search_bench(pkg, torch, dev, rank, world, max(1, min(args.steps, 3)), 1, dist_mod, barrier,
+            sr = search_bench(pkg, torch, dev, rank, world, args.steps, 1, dist_mod, barrier,
                               cpu_baseline=not args.no_cpu_baseline)
             main_case = sr["config3_beam10"]
             line = {"metric": SEARCH_METRIC, "value": main_case["utterances_per_s"], "unit": "utterances/s", "n_gpus": world,
-                    "steps": max(1, min(args.steps, 3)), "warmup": 1, "ms_per_step": main_case["ms_per_batch"],
+                    "steps": args.steps, "warmup": 1, "ms_per_step": main_case["ms_per_batch"],
                     "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
                     "config": {"workload": "configs[2]: 32 utterances x <=800 frames per GPU, beam_size 10; configs[0] in `search`",
                                "parallelism": "dp%d (utterances sharded, no cross-device traffic)" % world},
@@ -565,6 +590,7 @@ def main():
         sampler.join(timeout=2)
         if rank == 0:
             line["clocks"] = sampler.summary()
+            line["gpu"] = gpu_identity(local_rank)
             print(json.dumps(line))
         if world > 1:
             dist_mod.destroy_process_group()
@@ -578,7 +604,8 @@ def main():
         sampler.join(timeout=2)
         if rank == 0:
             tr.update({"warmup": args.warmup, "higher_is_better": True, "vs_baseline": None, "data": "synthetic",
-                       "gpu_launches": tr["gpu_launches_per_step"] * args.steps, "clocks": sampler.summary()})
+                       "gpu_launches": tr["gpu_launches_per_step"] * args.steps, "clocks": sampler.summary(),
+                       "gpu": gpu_identity(local_rank)})
             print(json.dumps(tr))
         if world > 1:
             dist_mod.destroy_process_group()
@@ -593,8 +620,10 @@ def main():
     sampler.start()
     lib.lvsr_launch_count(1)
     barrier()
-    ms_dev = timed(step_device, args.steps)
+    ms_dev, last_outputs = timed(step_device, args.steps)
     barrier()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_outputs)
     launches = int(lib.lvsr_launch_count(1))
     ms_dev = max_over_ranks(ms_dev, world, dev, dist_mod)
 
@@ -624,7 +653,7 @@ def main():
     train_block = None
     if not args.no_train and args.batch == WORKLOAD["B"]:
         try:
-            train_block = train_bench(pkg, torch, dev, rank, world, max(2, min(args.steps, 5)), 2, dist_mod, flush, barrier)
+            train_block = train_bench(pkg, torch, dev, rank, world, args.steps, 2, dist_mod, flush, barrier)
         except Exception as e:          # the headline must survive a failure of the secondary measurement
             train_block = {"error": "%s: %s" % (type(e).__name__, e)}
 
@@ -654,20 +683,19 @@ def main():
         dec_us = (prof["attention"]["ms"] + prof["window"]["ms"] + prof["dense"]["ms"]) * 1e3 / max(1, att["launches"])
     achieved = launch_bytes / (k_us * 1e-6) / 1e9 if k_us > 0 else 0.0
     # the encoder recurrence has no bandwidth or tensor roofline (SURVEY.md 8d): report time per
-    # sequential step next to the fp32 FMA time of its two dependent products
+    # sequential step next to the fp32 FMA time of its two dependent products on all SMs at the maximum SM clock
     enc_steps, t_l = 0, W["T"]
     for k in NET["subsample"]:
         enc_steps += t_l
         t_l = -(-t_l // k)
     D = NET["dims_bidir"][0]
     fma_per_step = 2 * W["B"] * 3 * D * D
-    # D = 256: bigru_mma_kernel -- mma.sync m16n8k16 on fp16 head/tail splits (fp32-equivalent, DESIGN.md section 2);
-    # per CTA and step 12 weight tiles x 16 k-steps x 2 MMAs at the measured 2.0 cycles per MMA and SM
-    # (tools/micro/mma_rate.cu) = 768 cycles of tensor pipe
+    gpu = gpu_identity(local_rank)
+    sms = torch.cuda.get_device_properties(dev).multi_processor_count
     recurrence = {"kernel": "bigru_mma_kernel" if D == 256 else "bigru_kernel", "sequential_steps": enc_steps,
                   "us_per_step": prof["bigru"]["ms"] * 1e3 / enc_steps if enc_steps else None,
-                  "fp32_fma_floor_us": fma_per_step / (148 * 128 * 1.965e9) * 1e6,
-                  "mma_sync_floor_us": (12 * (D // 16) * 2 * 2.0) / 1.965e9 * 1e6 if D == 256 else None}
+                  "fp32_fma_floor_us": (fma_per_step / (sms * 128 * gpu["sm_max_mhz"] * 1e6) * 1e6
+                                        if gpu["sm_max_mhz"] else None)}
     out = {
         "metric": METRIC, "value": value, "unit": "frames/s", "n_gpus": world, "steps": args.steps,
         "warmup": args.warmup, "ms_per_step": ms_step, "higher_is_better": True, "scaling": "weak",
@@ -677,17 +705,10 @@ def main():
                 "d2h_bytes_per_step": int(W["L"] * W["B"] * 4)},
         "gpu_launches": launches,
         "clocks": sampler.summary(),
+        "gpu": gpu,
         "roofline": {"bound": "hbm", "kernel": kern,
                      "achieved": achieved, "peak": peaks["hbm_gbs"], "unit": "GB/s",
                      "frac": achieved / peaks["hbm_gbs"],
-                     "traffic": (NCU_DEC_SCAN["dram_bytes"] if (prof["dec_scan"]["launches"] > 0 and
-                                 (W["B"], W["T"], W["L"]) == NCU_DEC_SCAN["config"]) else None),
-                     "traffic_source": NCU_DEC_SCAN["source"],
-                     "l2_to_sm_GBps": (NCU_DEC_SCAN["l2_to_sm_bytes"] / (k_us * 1e-6) / 1e9
-                                       if (prof["dec_scan"]["launches"] > 0 and k_us > 0 and
-                                           (W["B"], W["T"], W["L"]) == NCU_DEC_SCAN["config"]) else None),
-                     "binds": "latency (dependent phases at 25 % occupancy); P and H are L2-resident (hit rate 70 %), "
-                              "HBM moves about half the algorithmic bytes",
                      "peak_source": peak_src,
                      "algorithmic_bytes_per_launch": launch_bytes, "us_per_launch": k_us,
                      "decoder_step_us": dec_us,

@@ -1,1 +1,1 @@
-"""The reference's package name over the B200 engine; see compat/README.md."""
+"""The reference's package name over the GPU engine; see compat/README.md."""

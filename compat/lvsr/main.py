@@ -1,4 +1,4 @@
-"""lvsr.main of the reference over the B200 engine: the entry points bin/run.py dispatches to
+"""lvsr.main of the reference over the GPU engine: the entry points bin/run.py dispatches to
 (bin/run.py:140-154 -> lvsr/main.py:522-703 train / train_multistage, :705-865 search, :868-884 sample).
 
 Same function names, arguments and printed report lines; the Blocks main loop, extensions, Bokeh plotting and
@@ -192,7 +192,7 @@ def sample(config, params, load_path, part):
 
 def _out_of_scope(name):
     def fn(*args, **kwargs):
-        raise NotImplementedError("lvsr.main.%s is outside the B200 hot path (SURVEY.md section 8); "
+        raise NotImplementedError("lvsr.main.%s is outside the GPU hot path (SURVEY.md section 8); "
                                   "available: train_multistage, search, sample" % name)
     fn.__name__ = name
     return fn

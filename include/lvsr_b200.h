@@ -1,5 +1,5 @@
 /*
- * lvsr_b200.h -- C ABI of the B200-native attention-lvcsr hot path.
+ * lvsr_b200.h -- C ABI of the H100-native attention-lvcsr hot path.
  *
  * The reference (rizar/attention-lvcsr) has no FFI of its own on this path: Theano
  * generates and compiles C at run time and the "operator ABI" is the set of compiled

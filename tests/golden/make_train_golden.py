@@ -1,5 +1,5 @@
 """Generate tests/golden/train_golden.npz: float64 gradient oracle (oracle/lvsr_oracle_grad.py) for a WSJ-architecture
-training batch big enough to run the production code paths (island-mode persistent decoder: B = 16; tcgen05 backward
+training batch big enough to run the production code paths (island-mode persistent decoder: B = 16; tensor-core backward
 GEMMs: T*B = 5120 rows), reduced to a few numbers per parameter:
 
     cost; for every parameter: sum(g), sum(|g|), max|g|, g . r  (r ~ N(0,1) from RandomState(7), drawn in parameter order)

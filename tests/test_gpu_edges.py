@@ -1,4 +1,4 @@
-"""Edge cases of the hot path on the B200: ragged / degenerate shapes, every readout variant, and
+"""Edge cases of the hot path on the GPU: ragged / degenerate shapes, every readout variant, and
 the error behaviour of the C ABI.  Same bar as test_gpu_parity.py (1e-4 relative against the
 float64 oracle, everything through ctypes -> liblvsr_b200.so)."""
 import numpy as np
@@ -244,7 +244,7 @@ def test_recurrent_weights_beyond_the_fp16_range():
 
 
 def test_fp16_split_projection_gemm_opt_in(monkeypatch):
-    """LVSR_F16_GEMM=1: the fork GEMMs of layers >= 1 and attention.preprocess on tcgen05 kind::f16 with fp16 head/tail
+    """LVSR_F16_GEMM=1: the fork GEMMs of layers >= 1 and attention.preprocess on fp16 wgmma with fp16 head/tail
     operands (gemm_tc.cu) -- the oracle bar of every other path, and agreement with the default 3xTF32 kernel."""
     torch = _torch()
     cfg = O.make_config(**WSJ_ENC)

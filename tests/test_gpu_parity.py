@@ -1,4 +1,4 @@
-"""CUDA path vs the float64 oracle on the same seeded inputs (run on the B200 box).
+"""CUDA path vs the float64 oracle on the same seeded inputs (run on an H100).
 
 Bar (BASELINE.json north_star): forward activations within 1e-4 relative of the
 reference math, identical argmax / beam token sequences.  Everything goes through the
