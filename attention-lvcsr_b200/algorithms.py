@@ -106,6 +106,9 @@ def step_rule_from_config(train_conf, reg_conf=None):
     if "adadelta" in names:
         rules.append(AdaDelta(train_conf["decay_rate"], train_conf["epsilon"]))
     if reg_conf.get("max_norm", False) > 0:
+        if reg_conf.get("max_norm_exclude_lookup", False):
+            raise NotImplementedError("max_norm_exclude_lookup (lvsr/main.py:494-496): the CUDA step clips every "
+                                      "WEIGHT parameter, the lookup table included")
         rules.append(Restrict(VariableClipping(reg_conf["max_norm"], axis=0), "WEIGHT"))
     rules.append(RemoveNotFinite(0.0))
     if train_conf.get("burn_in_steps", 0):
@@ -175,7 +178,12 @@ class GradientDescent(object):
     place of the symbolic cost (there is no graph to differentiate: the backward pass is part of the library).
 
     recognizer: attention_lvcsr_b200.SpeechRecognizer;  step_rule: CompositeRule as built by lvsr/main.py;
-    decay: config['regularization']['decay'] (lvsr/main.py:419-421)."""
+    decay: config['regularization']['decay'] (lvsr/main.py:419-421).
+
+    ``last_cost`` after ``process_batch`` is the reference's ``sequence_total_cost``, sum(cost_matrix) / batch size
+    (lvsr/main.py:340-344), WITHOUT the decay term: the gradient includes decay * ||WEIGHT parameters||^2, the reported
+    cost does not (it is ``train_cost`` minus that penalty), so costs stay comparable across decay settings and
+    no extra reduction over the parameters runs per step."""
 
     def __init__(self, recognizer=None, step_rule=None, decay=0.0, cost=None, parameters=None, gradients=None,
                  on_unused_sources="warn", **kwargs):

@@ -47,6 +47,8 @@ int gemm_tn(Arena& ws, const float* A, int lda, const float* B, int ldb, int R, 
   LVSR_CHECK(part, "out of device memory (TN partials)");
   TnArgs g;
   g.A = A; g.lda = lda; g.B = B; g.ldb = ldb; g.R = R; g.Mo = Mo; g.N = N; g.part = part; g.rows_per_split = rps;
+  g.vec_a = lda % 4 == 0 && reinterpret_cast<uintptr_t>(A) % 16 == 0;
+  g.vec_b = ldb % 4 == 0 && reinterpret_cast<uintptr_t>(B) % 16 == 0;
   dim3 grid(ceil_div(N, TN_BN), ceil_div(Mo, TN_BM), splits);
   gemm_tn_kernel<<<grid, 256, 0, st>>>(g);
   LVSR_LAUNCH_CHECK();
@@ -164,6 +166,14 @@ int lvsr_train_cost_and_grads(lvsr_model* m, const float* x, const float* mask, 
   const int V = c.num_phonemes, Cfb = c.dim_feedback, Cpm = c.post_merge_dim, Hd = Cpm / c.maxout_pieces;
   const int Tp = lvsr_encoded_length(m, T);
   const int R = L * B;
+  // shapes the backward kernels cannot take are refused before any work is enqueued
+  const size_t ro_smem = (size_t)8 * (Hd + 128) * sizeof(float);
+  LVSR_CHECK(ro_smem <= 48 * 1024 && V <= 128, "readout backward: post_merge_dim / num_phonemes too large");
+  const int tc_cap = ceil_div(Tp, AB_CS);
+  const size_t ab_smem = att_bwd_smem_floats(M, E, K, n, tc_cap) * sizeof(float);
+  LVSR_CHECK(ab_smem <= 227 * 1024 && M <= AB_NT && M % 128 == 0 && K <= 16 && E % 4 == 0,
+             "attention backward: shape unsupported (Tp=%d M=%d)", Tp, M);
+  LVSR_CHECK(E <= 1024, "encoded dim %d > 1024 unsupported in training", E);
   const long long* lab = reinterpret_cast<const long long*>(labels);
   Arena& ws = m->tws;
   // size the tape arena once per shape
@@ -284,9 +294,7 @@ int lvsr_train_cost_and_grads(lvsr_model* m, const float* x, const float* mask, 
     rb.bo = m->P(g + "/readout/post_merge/mlp/linear_0.b");
     rb.R = R; rb.Cpm = Cpm; rb.pieces = c.maxout_pieces; rb.V = V; rb.act = c.post_merge_activation;
     rb.labels = lab; rb.lmask = lmask; rb.gscale = gscale; rb.hid = hid; rb.dlogits = dlogits; rb.dmerged = dmerged;
-    const size_t smem = (size_t)8 * (Hd + 128) * sizeof(float);
-    LVSR_CHECK(smem <= 48 * 1024 && V <= 128, "readout backward: post_merge_dim / num_phonemes too large");
-    readout_bwd_kernel<<<ceil_div(R, 8), 256, smem, st>>>(rb);
+    readout_bwd_kernel<<<ceil_div(R, 8), 256, ro_smem, st>>>(rb);
     LVSR_LAUNCH_CHECK();
     if (int rc = gemm_tn(ws, hid, Hd, dlogits, V, R, Hd, V, grad_of(m, grads, g + "/readout/post_merge/mlp/linear_0.W"), V, false, st)) return rc;
     if (int rc = colsum(dlogits, R, V, V, grad_of(m, grads, g + "/readout/post_merge/mlp/linear_0.b"), false, st)) return rc;
@@ -350,10 +358,6 @@ int lvsr_train_cost_and_grads(lvsr_model* m, const float* x, const float* mask, 
   LVSR_CUDA_OK(cudaMemsetAsync(dsbuf[0], 0, (size_t)B * C * sizeof(float), st));
   if (int rc = onehot_rows(w0, B, Tp, st)) return rc;
   {
-    const int tc_cap = ceil_div(Tp, AB_CS);
-    const size_t ab_smem = att_bwd_smem_floats(M, E, K, n, tc_cap) * sizeof(float);
-    LVSR_CHECK(ab_smem <= 227 * 1024 && M <= AB_NT && M % 128 == 0 && K <= 16 && E % 4 == 0,
-               "attention backward: shape unsupported (Tp=%d M=%d)", Tp, M);
     const bool kp12 = att_bwd_kp(K) == 12;
     LVSR_CUDA_OK(cudaFuncSetAttribute(att_bwd_kernel<12>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ab_smem));
     LVSR_CUDA_OK(cudaFuncSetAttribute(att_bwd_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ab_smem));
@@ -464,7 +468,6 @@ int lvsr_train_cost_and_grads(lvsr_model* m, const float* x, const float* mask, 
   LVSR_CHECK(dH, "out of device memory (dH)");
   {
     dim3 grid(ceil_div(Tp, 8), B);
-    LVSR_CHECK(E <= 1024, "encoded dim %d > 1024 unsupported in training", E);
     dh_from_ctx_kernel<<<grid, 256, 0, st>>>(W_all, dCTX, L, B, Tp, E, dH, 0);
     LVSR_LAUNCH_CHECK();
     if (int rc = gemm_nn(dP, Tp * B, M, M, WpT, E, E, nullptr, dH, E, true, st)) return rc;
@@ -559,9 +562,11 @@ int lvsr_train_cost_and_grads(lvsr_model* m, const float* x, const float* mask, 
 }
 
 
+// Parameters with the WEIGHT role, the subjects of weight decay and max-norm (lvsr/main.py:418-420,493): Linear and
+// LookupTable W and the recurrent matrices.  The conv filters carry no role of their own (lvsr/bricks/attention.py:31-33).
 static bool is_weight_name(const std::string& name) {
   const std::string leaf = name.substr(name.rfind('.') + 1);
-  return leaf == "W" || leaf == "state_to_state" || leaf == "state_to_gates" || leaf == "filters";
+  return leaf == "W" || leaf == "state_to_state" || leaf == "state_to_gates";
 }
 
 int lvsr_train_apply_updates(lvsr_model* m, float* grads, float gscale, const lvsr_train_config* tc, void* stream) {

@@ -26,6 +26,7 @@ struct TnArgs {
   int R, Mo, N;
   float* part;            // [splits][Mo][N]
   int rows_per_split;
+  int vec_a, vec_b;       // rows of A / B start on 16-byte boundaries (aligned base, leading dimension % 4 == 0)
 };
 
 __global__ void __launch_bounds__(256) gemm_tn_kernel(TnArgs g) {
@@ -34,7 +35,8 @@ __global__ void __launch_bounds__(256) gemm_tn_kernel(TnArgs g) {
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
   const int n0 = blockIdx.x * TN_BN, m0 = blockIdx.y * TN_BM;
   const int r_lo = blockIdx.z * g.rows_per_split, r_hi = min(g.R, r_lo + g.rows_per_split);
-  // loaders: one float4 of one row per thread for each operand (16 rows x 64 columns per tile)
+  // loaders: four consecutive columns of one row per thread for each operand (16 rows x 64 columns per tile), one
+  // float4 where the row is 16-byte aligned, scalar loads otherwise (e.g. ldb = V = 63, lda = 123 features)
   const int lr = tid >> 4, lc = (tid & 15) * 4;
   float acc[4][4];
 #pragma unroll
@@ -49,17 +51,19 @@ __global__ void __launch_bounds__(256) gemm_tn_kernel(TnArgs g) {
     if (r < r_hi) {
       const float* ap = g.A + (long long)r * g.lda + m0 + lc;
       const float* bp = g.B + (long long)r * g.ldb + n0 + lc;
-      if (m0 + lc + 3 < g.Mo) ra = *reinterpret_cast<const float4*>(ap);
+      if (g.vec_a && m0 + lc + 3 < g.Mo) ra = *reinterpret_cast<const float4*>(ap);
       else {
         if (m0 + lc + 0 < g.Mo) ra.x = ap[0];
         if (m0 + lc + 1 < g.Mo) ra.y = ap[1];
         if (m0 + lc + 2 < g.Mo) ra.z = ap[2];
+        if (m0 + lc + 3 < g.Mo) ra.w = ap[3];
       }
-      if (n0 + lc + 3 < g.N) rb = *reinterpret_cast<const float4*>(bp);
+      if (g.vec_b && n0 + lc + 3 < g.N) rb = *reinterpret_cast<const float4*>(bp);
       else {
         if (n0 + lc + 0 < g.N) rb.x = bp[0];
         if (n0 + lc + 1 < g.N) rb.y = bp[1];
         if (n0 + lc + 2 < g.N) rb.z = bp[2];
+        if (n0 + lc + 3 < g.N) rb.w = bp[3];
       }
     }
   };

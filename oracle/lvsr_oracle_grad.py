@@ -169,13 +169,15 @@ def _cost_matrix(cfg, p, attended, attended_mask, labels, labels_mask):
     return costs
 
 
-WEIGHT_LEAVES = ("W", "state_to_state", "state_to_gates", "filters")
+WEIGHT_LEAVES = ("W", "state_to_state", "state_to_gates")
 
 
 def is_weight(name):
-    """Parameters carrying the WEIGHT role (or FILTER, a WeightRole): every Linear / LookupTable W, the
-    recurrent matrices (B/bricks/recurrent.py:571-572 add_role WEIGHT) and the conv filters
-    (lvsr/bricks/attention.py Conv1D -> FILTER); not biases, not initial states."""
+    """Parameters carrying the WEIGHT role, the ones VariableFilter(roles=[WEIGHT]) selects for the decay term and
+    the max-norm subjects (lvsr/main.py:418-420,493): every Linear / LookupTable W (B/bricks/simple.py:49,
+    B/bricks/lookup.py:42) and the recurrent matrices (B/bricks/recurrent.py:556,560).  Not biases, not initial
+    states, and not the conv filters: Conv1D._allocate (lvsr/bricks/attention.py:31-33) adds no role, so they carry
+    only the PARAMETER role every brick parameter gets (B/bricks/base.py:36-44)."""
     return name.rsplit(".", 1)[1] in WEIGHT_LEAVES
 
 

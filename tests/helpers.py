@@ -18,8 +18,8 @@ def package():
 
 def make_recognizer(cfg, params=None):
     pkg = package()
-    act = {"maxout": pkg.Maxout(cfg["maxout_pieces"]), "relu": pkg.Rectifier(), "tanh": pkg.Tanh()}[
-        cfg["post_merge_activation"]]
+    act = {"maxout": pkg.Maxout(cfg["maxout_pieces"]), "relu": pkg.Rectifier(), "tanh": pkg.Tanh(),
+           "identity": pkg.Identity()}[cfg["post_merge_activation"]]
     rec = pkg.SpeechRecognizer(
         input_dims={"recordings": cfg["num_features"]}, input_num_chars={}, eos_label=cfg["eos_label"],
         num_phonemes=cfg["num_phonemes"], dim_dec=cfg["dim_dec"], dims_bidir=cfg["dims_bidir"],
@@ -33,6 +33,82 @@ def make_recognizer(cfg, params=None):
     if params is not None:
         rec.set_parameter_values(params)
     return rec
+
+
+KINK_EPS = 2e-5      # > the float32 error of a readout pre-activation on the GPU (measured <= 5e-6 at T*B = 2048)
+_RO = "/recognizer/generator/readout"
+
+
+def relu_readout_kinks(cfg, params, batch, eps=KINK_EPS):
+    """(step, utterance, unit) of every label-unmasked row whose Rectifier readout pre-activation lies within eps of 0,
+    from the float64 oracle, and the pre-activations [L, B, post_merge_dim].  [] for the other activations."""
+    if cfg["post_merge_activation"] != "relu":
+        return [], None
+    x, m, labels, lm = batch
+    out = O.recognizer_cost(cfg, params, x, m, labels, lm, return_all=True)
+    pre = out["weighted_averages"] @ params[_RO + "/merge/transform_weighted_averages.W"] + params[_RO + "/post_merge/bias.b"]
+    if cfg["use_states_for_readout"]:
+        pre = pre + out["states"] @ params[_RO + "/merge/transform_states.W"]     # "states" = s_{i-1}, what step i reads out
+    live = np.ones(labels.shape, bool) if lm is None else np.asarray(lm) > 0
+    return [tuple(int(v) for v in i) for i in np.argwhere((np.abs(pre) < eps) & live[:, :, None])], pre
+
+
+def _one_sided_oracle_params(cfg, params, batch):
+    """The Rectifier's derivative jumps at 0.  A pre-activation within float32 error of the kink may land on either
+    side of it on the GPU, so such a unit is compared with the oracle's derivative from each side: the unit's bias is
+    moved so that its pre-activation is -1e-7 or +1e-7 (a change of the cost of order 1e-7 * |dcost/dx|).  Returns
+    `params` first, then one parameter set per combination of sides of the units near their kink."""
+    import itertools
+    kinks, pre = relu_readout_kinks(cfg, params, batch)
+    if not kinks:
+        return [params]
+    units = sorted({j for _, _, j in kinks})
+    assert len(units) == len(kinks) <= 4, kinks                       # one kink per unit, few of them
+    lm = batch[3]
+    live = np.ones(pre.shape[:2], bool) if lm is None else np.asarray(lm) > 0
+    out = [params]
+    for sides in itertools.product((-1e-7, 1e-7), repeat=len(kinks)):
+        p = dict(params)
+        b = np.array(params[_RO + "/post_merge/bias.b"], dtype=np.float64)
+        for (i, u, j), s in zip(kinks, sides):
+            shift = s - pre[i, u, j]
+            others = np.abs(pre[:, :, j][live])
+            assert (np.sort(others)[1] > 2 * abs(shift)), (i, u, j)      # no other row of the unit crosses 0
+            b[j] += shift
+        p[_RO + "/post_merge/bias.b"] = b
+        out.append(p)
+    return out
+
+
+def check_grads(cfg, params, batch, tol=1e-4, atol_frac=1e-6):
+    """One lvsr_train_cost_and_grads call against the float64 gradient oracle: the cost to 1e-4, each parameter's
+    gradient to `tol` of its own largest entry plus a floor of `atol_frac` of the model's largest gradient entry.  A
+    Rectifier readout unit on its kink (_one_sided_oracle_params) must match the oracle from one of the two sides."""
+    from oracle import lvsr_oracle_grad as G
+    pkg = package()
+    rec = make_recognizer(cfg, params)
+    algo = pkg.GradientDescent(recognizer=rec, step_rule=pkg.CompositeRule([pkg.RemoveNotFinite(0.0)]))
+    cost, grads = algo.cost_and_gradients(dict(zip(algo.SOURCES, batch)))
+    failures = []
+    for oracle_params in _one_sided_oracle_params(cfg, params, batch):
+        want_cost, want = G.cost_and_grads(cfg, oracle_params, *batch)
+        gmax = max(np.abs(w).max() for w in want.values())
+        errs = {}
+        for k, w in want.items():
+            errs[k] = float(np.abs(grads[k].astype(np.float64) - w).max() / max(np.abs(w).max(), 1e-30))
+        bad = {}
+        for k, e in errs.items():
+            # relative to the parameter's own largest gradient entry, with a floor relative to the model's largest
+            floor = atol_frac * gmax / max(np.abs(want[k]).max(), 1e-30)
+            if e > tol + floor:
+                bad[k] = (e, float(np.abs(want[k]).max()))
+        if abs(cost - want_cost) > 1e-4 * abs(want_cost):
+            bad["cost"] = (cost, want_cost)
+        print("cost", cost, "worst rel grad err %.2e" % max(errs.values()), "of", len(errs), "parameters")
+        if not bad:
+            return algo, rec
+        failures.append(bad)
+    raise AssertionError(failures)
 
 
 def rel_err(got, want):

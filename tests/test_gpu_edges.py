@@ -83,6 +83,17 @@ def test_readout_variants(activation, use_states):
     _compare_cost(cfg, params, x, m, labels, lm)
 
 
+@pytest.mark.parametrize("B,T", [(5, 40), (16, 160)])
+def test_feature_width_not_a_multiple_of_4(B, T):
+    """123 features (WSJ fbank + deltas + double deltas): the tensor-core GEMM needs a contraction that is a multiple of
+    4, so the first layer's fork GEMM runs on FFMA tiles; at a small batch and at 2560 rows."""
+    _torch()
+    cfg = O.make_config(**dict(PYRAMID, num_features=123))
+    params = O.init_params(cfg, seed=11, scale=10.0)
+    x, m, labels, lm = O.synthetic_batch(cfg, B=B, T=T, seed=B + T)
+    _compare_cost(cfg, params, x, m, labels, lm)
+
+
 def test_label_mask_freezes_states_after_the_end():
     """Rows whose labels have ended keep their last state and contribute zero cost
     (B/bricks/sequence_generators.py:311-319)."""

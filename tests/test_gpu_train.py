@@ -7,9 +7,12 @@ import numpy as np
 import pytest
 
 from helpers import O, PYRAMID, WSJ, make_recognizer, package
+from helpers import check_grads as _check_grads
 from oracle import lvsr_oracle_grad as G
 
 pytestmark = pytest.mark.gpu
+
+FILTERS = "/recognizer/generator/att_trans/conv_att/conv1d.filters"
 
 
 def _torch():
@@ -17,35 +20,6 @@ def _torch():
     if not torch.cuda.is_available():
         pytest.skip("no CUDA device")
     return torch
-
-
-def _grad_errors(got, want):
-    errs = {}
-    for k, w in want.items():
-        scale = max(np.abs(w).max(), 1e-30)
-        errs[k] = float(np.abs(got[k].astype(np.float64) - w).max() / scale)
-    return errs
-
-
-def _check_grads(cfg, params, batch, tol=1e-4, atol_frac=1e-6):
-    pkg = package()
-    rec = make_recognizer(cfg, params)
-    algo = pkg.GradientDescent(recognizer=rec, step_rule=pkg.CompositeRule([pkg.RemoveNotFinite(0.0)]))
-    cost, grads = algo.cost_and_gradients(dict(zip(algo.SOURCES, batch)))
-    want_cost, want = G.cost_and_grads(cfg, params, *batch)
-    assert abs(cost - want_cost) <= 1e-4 * abs(want_cost), (cost, want_cost)
-    gmax = max(np.abs(w).max() for w in want.values())
-    errs = _grad_errors(grads, want)
-    bad = {}
-    for k, e in errs.items():
-        # relative to the parameter's own largest gradient entry, with a floor relative to the model's largest
-        floor = atol_frac * gmax / max(np.abs(want[k]).max(), 1e-30)
-        if e > tol + floor:
-            bad[k] = (e, float(np.abs(want[k]).max()))
-    worst = max(errs.values())
-    print("cost", cost, "worst rel grad err %.2e" % worst, "of", len(errs), "parameters")
-    assert not bad, bad
-    return algo, rec
 
 
 PRIORS = [None, dict(type="window_around_median", before=5, after=7),
@@ -78,39 +52,98 @@ def test_gradients_island_batch_no_masks():
     _check_grads(cfg, params, (x, None, labels, None))
 
 
-@pytest.mark.parametrize("rules,max_norm", [(("momentum", "adadelta"), 1.0), (("momentum",), 0.0), (("adadelta",), 0.5)])
-def test_training_steps_match_oracle(rules, max_norm):
-    """Two process_batch calls == two oracle train_steps (float64) on the same batches."""
-    _torch()
+def _train_like_the_oracle(cfg, params, tc, steps=2, B=4, T=40):
+    """`steps` process_batch calls == as many oracle train_steps (float64) on the same batches: after every step the
+    cost, the gradient norm and every parameter agree.  Returns (recognizer, oracle parameters, oracle gradient norms)."""
     pkg = package()
-    cfg = O.make_config(**PYRAMID)
-    params = O.init_params(cfg, seed=5, scale=10.0)
-    tc = G.make_train_config(gradient_threshold=2.0, rules=rules, scale=0.05, momentum=0.5, decay_rate=0.95,
-                             epsilon=1e-6, max_norm=max_norm)
+    reg = dict(max_norm=tc["max_norm"])
     rec = make_recognizer(cfg, params)
-    algo = pkg.GradientDescent(recognizer=rec, step_rule=pkg.step_rule_from_config(tc, dict(max_norm=max_norm)))
+    algo = pkg.GradientDescent(recognizer=rec, step_rule=pkg.step_rule_from_config(tc, reg), decay=tc["decay"])
     algo.initialize()
     ref = OrderedDict((k, v.copy()) for k, v in params.items())
-    state = {}
-    for step in range(2):
-        batch = O.synthetic_batch(cfg, B=4, T=40, seed=100 + step)
+    state, norms = {}, []
+    for step in range(steps):
+        batch = O.synthetic_batch(cfg, B=B, T=T, seed=100 + step)
+        # last_cost is sequence_total_cost, the cost without the decay term (GradientDescent's docstring)
+        penalty = tc["decay"] * sum(float((v ** 2).sum()) for k, v in ref.items() if G.is_weight(k))
         ref, ref_cost, ref_grads = G.train_step(cfg, ref, state, batch, tc)
+        want_cost = ref_cost - penalty
         algo.process_batch(dict(zip(algo.SOURCES, batch)))
-        assert abs(float(algo.last_cost.item()) - ref_cost) <= 1e-4 * abs(ref_cost)
-        assert abs(algo.total_gradient_norm() - G.l2_norm(ref_grads.values())) <= 1e-4 * G.l2_norm(ref_grads.values())
+        assert abs(float(algo.last_cost.item()) - want_cost) <= 1e-4 * abs(want_cost), (step, algo.last_cost.item(), want_cost)
+        norms.append(G.l2_norm(ref_grads.values()))
+        assert abs(algo.total_gradient_norm() - norms[-1]) <= 1e-4 * norms[-1]
         got = rec.get_parameter_values()
         for k, v in ref.items():
             # compare the UPDATE (new - old would cancel; the parameters themselves are O(0.1..1))
             assert np.abs(got[k] - v).max() <= 2e-5 * max(1.0, np.abs(v).max()) + 1e-6, (step, k, np.abs(got[k] - v).max())
-    if max_norm > 0:
+    if tc["max_norm"] > 0:
         for k, v in rec.get_parameter_values().items():
             if G.is_weight(k):
-                assert (np.sqrt((v.astype(np.float64) ** 2).sum(axis=0)) <= max_norm * (1 + 1e-5)).all(), k
+                assert (np.sqrt((v.astype(np.float64) ** 2).sum(axis=0)) <= tc["max_norm"] * (1 + 1e-5)).all(), k
+    return rec, ref, norms
+
+
+def _params_with_long_filter_columns(cfg, max_norm):
+    """Trained-like parameters whose conv filters have columns (axis 0) both longer and shorter than max_norm."""
+    params = O.init_params(cfg, seed=5, scale=10.0)
+    f = params[FILTERS].copy()
+    f[:, ::2] *= 3.0 * max_norm / np.sqrt((f[:, ::2] ** 2).sum(axis=0)).min()
+    params[FILTERS] = f
+    cols = np.sqrt((f ** 2).sum(axis=0))
+    assert (cols[::2] > 2.9 * max_norm).all() and (cols[1::2] < max_norm).all()
+    return params
+
+
+@pytest.mark.parametrize("rules,max_norm", [(("momentum", "adadelta"), 1.0), (("momentum",), 0.0), (("adadelta",), 0.5)])
+def test_training_steps_match_oracle(rules, max_norm):
+    """Two process_batch calls == two oracle train_steps (float64) on the same batches."""
+    _torch()
+    cfg = O.make_config(**PYRAMID)
+    params = O.init_params(cfg, seed=5, scale=10.0)
+    tc = G.make_train_config(gradient_threshold=2.0, rules=rules, scale=0.05, momentum=0.5, decay_rate=0.95,
+                             epsilon=1e-6, max_norm=max_norm)
+    rec, ref, _ = _train_like_the_oracle(cfg, params, tc)
     # the forward pass uses the updated (re-packed) weights
     x, m, labels, lm = O.synthetic_batch(cfg, B=3, T=32, seed=5)
     want = O.recognizer_cost(cfg, ref, x, m, labels, lm)
     got = rec.cost(x, m, labels, lm)
     assert np.abs(got - want).max() <= 1e-3 * np.abs(want).max()
+
+
+def test_max_norm_clips_weights_but_not_the_conv_filters():
+    """Restrict(VariableClipping(max_norm, axis=0), WEIGHT) (lvsr/main.py:490-505): the conv filters have no WEIGHT role
+    (lvsr/bricks/attention.py:31-33), so filter columns far longer than max_norm move exactly as the oracle's, unclipped."""
+    _torch()
+    cfg = O.make_config(**PYRAMID)
+    params = _params_with_long_filter_columns(cfg, 1.0)
+    tc = G.make_train_config(gradient_threshold=2.0, rules=("momentum", "adadelta"), scale=0.05, momentum=0.5,
+                             decay_rate=0.95, epsilon=1e-6, max_norm=1.0)
+    rec, ref, _ = _train_like_the_oracle(cfg, params, tc)
+    got = rec.get_parameter_values()[FILTERS].astype(np.float64)
+    assert (np.sqrt((got[:, ::2] ** 2).sum(axis=0)) > 2.5).all()           # still far above max_norm
+
+
+def test_weight_decay_with_momentum_adadelta_and_max_norm():
+    """decay > 0 (lvsr/main.py:418-420) on the full WSJ chain: 2 decay W joins the gradient of every WEIGHT parameter
+    before the clipping norm; biases, initial states and the conv filters are not decayed."""
+    _torch()
+    cfg = O.make_config(**PYRAMID)
+    params = _params_with_long_filter_columns(cfg, 1.0)
+    tc = G.make_train_config(gradient_threshold=2.0, rules=("momentum", "adadelta"), scale=0.05, momentum=0.5,
+                             decay_rate=0.95, epsilon=1e-6, max_norm=1.0, decay=0.01)
+    _train_like_the_oracle(cfg, params, tc)
+
+
+@pytest.mark.parametrize("threshold,active", [(1e-3, True), (1e6, False)], ids=["always_clipped", "never_clipped"])
+def test_step_clipping_active_and_inactive(threshold, active):
+    """StepClipping (B/algorithms/__init__.py:634-643) with a threshold far below the gradient norm (every step is
+    rescaled to norm = threshold) and far above it (the step is the plain gradient)."""
+    _torch()
+    cfg = O.make_config(**PYRAMID)
+    params = O.init_params(cfg, seed=5, scale=10.0)
+    tc = G.make_train_config(gradient_threshold=threshold, rules=("momentum",), scale=0.05, momentum=0.5, max_norm=0.0)
+    _, _, norms = _train_like_the_oracle(cfg, params, tc)
+    assert all((n > 100 * threshold) if active else (n < threshold / 100) for n in norms), norms
 
 
 def test_non_finite_gradient_zeroes_the_parameter_and_burn_in_delays_updates():

@@ -153,6 +153,9 @@ def test_step_rule_chains_map_onto_the_train_config():
         A._to_train_config(A.CompositeRule([A.Momentum(0.1, 0.0), A.RemoveNotFinite(1)]))
     with pytest.raises(NotImplementedError):                # max-norm over another axis
         A._to_train_config(A.CompositeRule([A.Restrict(A.VariableClipping(1.0, axis=1), "WEIGHT"), A.RemoveNotFinite(0.0)]))
+    with pytest.raises(NotImplementedError):                # max-norm subjects without the lookup table (lvsr/main.py:494-496)
+        A.step_rule_from_config(wsj, dict(max_norm=1.0, max_norm_exclude_lookup=True))
+    assert len(A.step_rule_from_config(wsj, dict(max_norm=0.0, max_norm_exclude_lookup=True)).components) == 5
     with pytest.raises(ValueError):
         A.AdaDelta(decay_rate=2.0)                           # B/algorithms/__init__.py:481-482
     with pytest.raises(ValueError):

@@ -70,6 +70,69 @@ def test_weight_decay_term():
         assert_allclose(g1[k] - g0[k], 0.02 * params[k] if G.is_weight(k) else 0 * params[k], atol=1e-12)
 
 
+# ---- Blocks roles: which parameters decay and max-norm apply to ------------------------------
+
+def _blocks_roles(cfg):
+    """The role each recognizer parameter carries in the reference, brick by brick.  VariableFilter(roles=[WEIGHT])
+    selects the decay term's and the max-norm's subjects (lvsr/main.py:418-420,493).  Every brick parameter also
+    gets the PARAMETER role (B/bricks/base.py:36-44); listed here is the role the brick adds on top, or PARAMETER
+    when it adds none."""
+    roles = {}
+    # GatedRecurrent._allocate: state_to_state WEIGHT (B/bricks/recurrent.py:556), state_to_gates WEIGHT (:560),
+    # initial_state INITIAL_STATE (:564)
+    # Fork -> Linear: W WEIGHT (B/bricks/simple.py:49), b BIAS (B/bricks/simple.py:54)
+    for l in range(len(cfg["dims_bidir"])):
+        for d in ("forward", "backward"):
+            base = "/recognizer/encoder/bidir%d/%s" % (l, d)
+            roles[base + "/gatedrecurrent.state_to_state"] = "WEIGHT"
+            roles[base + "/gatedrecurrent.state_to_gates"] = "WEIGHT"
+            roles[base + "/gatedrecurrent.initial_state"] = "INITIAL_STATE"
+            roles[base + "/fork/fork_inputs.W"] = "WEIGHT"
+            roles[base + "/fork/fork_inputs.b"] = "BIAS"
+            roles[base + "/fork/fork_gate_inputs.W"] = "WEIGHT"
+            roles[base + "/fork/fork_gate_inputs.b"] = "BIAS"
+    g, a = "/recognizer/generator", "/recognizer/generator/att_trans"
+    if cfg["embed_outputs"]:
+        roles[g + "/readout/lookupfeedback/lookuptable.W"] = "WEIGHT"          # LookupTable, B/bricks/lookup.py:42
+    if cfg["use_states_for_readout"]:
+        roles[g + "/readout/merge/transform_states.W"] = "WEIGHT"              # Merge -> Linear(use_bias=False), simple.py:49
+    roles[g + "/readout/merge/transform_weighted_averages.W"] = "WEIGHT"       # simple.py:49
+    roles[g + "/readout/post_merge/bias.b"] = "BIAS"                           # Bias, B/bricks/simple.py:95
+    roles[g + "/readout/post_merge/mlp/linear_0.W"] = "WEIGHT"                 # simple.py:49
+    roles[g + "/readout/post_merge/mlp/linear_0.b"] = "BIAS"                   # simple.py:54
+    roles[g + "/fork/fork_inputs.W"] = "WEIGHT"                                # Fork -> Linear, simple.py:49 / :54
+    roles[g + "/fork/fork_inputs.b"] = "BIAS"
+    roles[g + "/fork/fork_gate_inputs.W"] = "WEIGHT"
+    roles[g + "/fork/fork_gate_inputs.b"] = "BIAS"
+    roles[a + "/transition.state_to_state"] = "WEIGHT"                         # GatedRecurrent, recurrent.py:556
+    roles[a + "/transition.state_to_gates"] = "WEIGHT"                         # recurrent.py:560
+    roles[a + "/transition.initial_state"] = "INITIAL_STATE"                   # recurrent.py:564
+    roles[a + "/conv_att/state_trans/transform_states.W"] = "WEIGHT"           # Linear(use_bias=False), simple.py:49
+    roles[a + "/conv_att/preprocess.W"] = "WEIGHT"                             # Linear, simple.py:49 / :54
+    roles[a + "/conv_att/preprocess.b"] = "BIAS"
+    roles[a + "/conv_att/energy_comp/linear.W"] = "WEIGHT"                     # MLP -> Linear, simple.py:49
+    roles[a + "/conv_att/handler.W"] = "WEIGHT"                                # Linear(use_bias=False), simple.py:49
+    roles[a + "/conv_att/conv1d.filters"] = "PARAMETER"                        # Conv1D._allocate adds no role (lvsr/bricks/attention.py:31-33)
+    roles[a + "/distribute/fork_inputs.W"] = "WEIGHT"                          # Distribute -> Fork -> Linear(use_bias=False)
+    roles[a + "/distribute/fork_gate_inputs.W"] = "WEIGHT"
+    return roles
+
+
+@pytest.mark.parametrize("variant", [{}, dict(embed_outputs=False), dict(use_states_for_readout=False)],
+                         ids=["wsj", "one_of_n_feedback", "no_states_for_readout"])
+def test_weight_role_table_of_the_wsj_model(variant):
+    """G.is_weight is True exactly for the WEIGHT-role parameters of the WSJ model: the conv filters are not among them,
+    so neither decay nor max-norm touches them."""
+    cfg = O.make_config(num_features=40, dims_bidir=[256] * 4, subsample=[1, 1, 2, 2], dim_dec=256, dim_matcher=512,
+                        conv_n=100, conv_num_filters=10, num_phonemes=32, post_merge_dims=[256], maxout_pieces=2,
+                        **variant)
+    roles = _blocks_roles(cfg)
+    names = list(O.param_shapes(cfg))
+    assert sorted(names) == sorted(roles)
+    wrong = {k: roles[k] for k in names if G.is_weight(k) != (roles[k] == "WEIGHT")}
+    assert not wrong, wrong
+
+
 # ---- step rules: the reference's literals ---------------------------------------------------
 
 def _grad_a(a):
