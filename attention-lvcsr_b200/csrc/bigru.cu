@@ -7,7 +7,9 @@
 //
 // Mapping (two DEPENDENT [rows,D]x[D,*] products per step, T sequential steps):
 //   * batch rows are independent -> a thread-block CLUSTER of CS CTAs owns RB = 4 rows of one
-//     direction; clusters never talk to each other (no grid-wide barrier).
+//     direction; clusters never talk to each other (no grid-wide barrier).  The tensor-core kernel also comes with
+//     RB = 8 rows per cluster, chosen when it needs fewer waves of clusters than RB = 4 (a cluster's CTAs must share one
+//     GPC, so an H100 holds fewer 4-CTA clusters than SMs / 4; see bigru_layer).
 //   * inside a cluster the hidden units are split: CTA `rank` owns UC = D/CS units, each of its
 //     warps 4 of them; the state_to_gates slice stays IN REGISTERS for the whole sequence, the
 //     state_to_state slice in shared memory -- weights are read from HBM once per layer.
@@ -425,7 +427,8 @@ int launch_bigru_t(const BiGruArgs& a, cudaStream_t stream) {
 // =====================================================================================================
 // Tensor-core variant of the same scan (D = 256 at the metric batch): the two recurrent products run on
 // mma.sync m16n8k16 (fp16 operands, fp32 accumulate) with the WEIGHT COLUMNS as the M dimension and the
-// cluster's RB = 4 batch rows in the N = 8 slot: a CTA's 192 columns are 12 M tiles.
+// cluster's batch rows in the N = 8 slot: a CTA's 192 columns are 12 M tiles.  Up to the RB = 8 paragraph below this
+// describes RB = 4.
 //
 // fp32 accuracy from fp16 operands: every operand is split into an fp16 head and an fp16 tail scaled by
 // 2^11 (x = head + tail / 2048; both exact to ~2^-22 of x) and
@@ -449,6 +452,14 @@ int launch_bigru_t(const BiGruArgs& a, cudaStream_t stream) {
 //                ship the tails and compute the update gate off the critical path.
 // The exchange protocol is the FFMA kernel's (st.async + complete_tx on the receiver's mbarrier, no cluster barrier
 // in the loop).
+//
+// RB = 8 rows per cluster (template parameter; halves the clusters of a batch, so a batch that would need two waves of
+// 4-row clusters runs in one): the N = 8 slot carries the HEADS of the 8 rows and a second B fragment their TAILS, so a
+// k-step issues three MMAs -- head_w * H_head, head_w * H_tail, tail_w * H_head -- into three accumulators of the same
+// lane layout (tail * tail stays dropped, as for RB = 4).  A plane row interleaves each 4-unit group as
+// [head01 head23 tail01 tail23]: one 16-byte load yields both B fragments of a k-step and one 16-byte st.async per peer
+// ships heads and tails of a (row, 4 units) role.  The 128 elementwise threads own the 128 roles one each (r, z, the
+// candidate and the sends of a role all run on its thread).
 __device__ __forceinline__ void mma_f16(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
   asm volatile(
       "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
@@ -467,6 +478,12 @@ __device__ __forceinline__ void split_pair(float x, float y, uint32_t& head, uin
 __device__ __forceinline__ void st_async_v2_b32(uint32_t remote_addr, uint32_t x, uint32_t y, uint32_t remote_bar) {
   asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.v2.b32 [%0], {%1, %2}, [%3];\n" ::"r"(remote_addr),
                "r"(x), "r"(y), "r"(remote_bar)
+               : "memory");
+}
+__device__ __forceinline__ void st_async_v4_b32(uint32_t remote_addr, uint4 v, uint32_t remote_bar) {
+  asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.v4.b32 [%0], {%1, %2, %3, %4}, [%5];\n" ::"r"(
+                   remote_addr),
+               "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w), "r"(remote_bar)
                : "memory");
 }
 __device__ __forceinline__ void named_bar_sync(int id, int count) {
@@ -495,7 +512,7 @@ __device__ __forceinline__ float range_scale(float warp_max_abs, float& inverse)
   return scale;
 }
 
-template <int D, bool TAPE>
+template <int D, bool TAPE, int RB>
 __global__ void __launch_bounds__(MMA_THREADS, 1)
 bigru_mma_kernel(BiGruArgs a) {
   constexpr int CS = MMA_CS;
@@ -510,16 +527,19 @@ bigru_mma_kernel(BiGruArgs a) {
   constexpr int NROLE = RB * UG;        // (row, unit group) roles
   static_assert(MT1 * KS1 == MMA_WARPS && MT2 * KS2 == MMA_WARPS && NK1 * KS1 == NK && NK2 * KS2 == NK, "tile split");
   static_assert(NK1 % 2 == 0 && NK2 % 2 == 0, "two k-steps per round of the MMA loops");
-  static_assert(2 * NROLE <= EW_WARPS * 32, "elementwise roles");
-  static_assert(RB == 4, "N columns: 4 rows of heads + 4 rows of tails");
-  // a plane row: 2 words per 4-unit group = packed (u, u+1), (u+2, u+3); + 8 words: the 16 lanes of a load phase
-  // (4 rows x 4 groups) then cover all 32 banks once
-  constexpr int RSH = D / 2 + 8;
+  static_assert(RB == 4 || RB == 8, "N columns: 4 rows of heads + 4 rows of tails, or 8 rows of heads (and of tails)");
+  static_assert((RB == 4 ? 2 : 1) * NROLE <= EW_WARPS * 32, "elementwise roles");
+  // RB = 4: two planes [heads | tails], a plane row holds 2 words per 4-unit group = packed (u, u+1), (u+2, u+3); + 8
+  // words: the 16 lanes of an 8-byte load phase (4 rows x 4 groups) then cover all 32 banks once.
+  // RB = 8: one plane, a row holds 4 words per group = [head01 head23 tail01 tail23]; + 16 words: the 8 lanes of a
+  // 16-byte load phase (2 rows x 4 groups) then cover all 32 banks once.
+  constexpr int PLANES = RB == 4 ? 2 : 1;
+  constexpr int RSH = RB == 4 ? D / 2 + 8 : D + 16;
   constexpr int RS1 = 2 * UC + 4, RS2 = UC + 4;   // 2 * RS mod 32 = 8: the row pairs of a C fragment spread over the banks
   constexpr uint32_t FULL_BYTES = RB * D * sizeof(uint32_t);
 
-  __shared__ __align__(128) uint32_t hbuf[2][RB][RSH];    // [heads | tails] of h
-  __shared__ __align__(128) uint32_t hrbuf[2][RB][RSH];   // ... of h * r
+  __shared__ __align__(128) uint32_t hbuf[PLANES][RB][RSH];    // heads and tails of h
+  __shared__ __align__(128) uint32_t hrbuf[PLANES][RB][RSH];   // ... of h * r
   __shared__ __align__(16) float red1[KS1][RB][RS1];
   __shared__ __align__(16) float red2[KS2][RB][RS2];
   __shared__ __align__(16) float zbuf[RB][UC];
@@ -539,7 +559,10 @@ bigru_mma_kernel(BiGruArgs a) {
 
   for (int i = tid; i < RB * D / 2; i += MMA_THREADS) {
     const int r = i / (D / 2), j = i % (D / 2);
-    split_pair(h0[2 * j], h0[2 * j + 1], hbuf[0][r][j], hbuf[1][r][j]);
+    if constexpr (RB == 4)
+      split_pair(h0[2 * j], h0[2 * j + 1], hbuf[0][r][j], hbuf[PLANES - 1][r][j]);
+    else
+      split_pair(h0[2 * j], h0[2 * j + 1], hbuf[0][r][4 * (j / 2) + j % 2], hbuf[0][r][4 * (j / 2) + 2 + j % 2]);
   }
   if (tid == 0) {
     mbar_init(bar_h, 1);
@@ -619,11 +642,18 @@ bigru_mma_kernel(BiGruArgs a) {
         }
       }
     }
-    // B fragments: N column g < 4 = heads of batch row g, N column g >= 4 = tails of batch row g - 4
-    const uint2* hb2 = reinterpret_cast<const uint2*>(&hbuf[g / RB][g % RB][kh * NK1 * 8 + 2 * tq]);
-    const uint2* hrb2 = reinterpret_cast<const uint2*>(&hrbuf[g / RB][g % RB][kq * NK2 * 8 + 2 * tq]);
-    float* const out1 = &red1[kh][2 * (tq & 1)][mt1 * 16 + g];
-    float* const out2 = &red2[kq][2 * (tq & 1)][mt2 * 16 + g];
+    // B fragments.  RB = 4: N column g < 4 = heads of batch row g, N column g >= 4 = tails of batch row g - 4 (one 8-byte
+    // load per k-step).  RB = 8: N column g = batch row g, heads and tails of a k-step in one 16-byte load.
+    const uint32_t* const hb = RB == 4 ? &hbuf[g / 4][g % 4][kh * NK1 * 8 + 2 * tq] : &hbuf[0][g][kh * NK1 * 16 + 4 * tq];
+    const uint32_t* const hrb =
+        RB == 4 ? &hrbuf[g / 4][g % 4][kq * NK2 * 8 + 2 * tq] : &hrbuf[0][g][kq * NK2 * 16 + 4 * tq];
+    const uint2* hb2 = reinterpret_cast<const uint2*>(hb);
+    const uint2* hrb2 = reinterpret_cast<const uint2*>(hrb);
+    const uint4* hb4 = reinterpret_cast<const uint4*>(hb);
+    const uint4* hrb4 = reinterpret_cast<const uint4*>(hrb);
+    // C fragment rows: RB = 4 -> batch rows 2 (tq & 1) + {0, 1} (lanes tq < 2 store), RB = 8 -> 2 tq + {0, 1}
+    float* const out1 = &red1[kh][RB == 4 ? 2 * (tq & 1) : 2 * tq][mt1 * 16 + g];
+    float* const out2 = &red2[kq][RB == 4 ? 2 * (tq & 1) : 2 * tq][mt2 * 16 + g];
     const bool tracer = tracing && tid == EW_WARPS * 32;
 #define BG_STAMP(j)                              \
   do {                                           \
@@ -641,7 +671,23 @@ bigru_mma_kernel(BiGruArgs a) {
         mbar_arm(bar_hr, FULL_BYTES);   // arrivals of (h*r)(s)
       }
       BG_STAMP(0);
-      {
+      if constexpr (RB == 8) {
+        // three accumulation chains, one per product term; all three hold (weight column, batch row) in the same lanes.
+        // (Splitting each into even / odd k-steps, as RB = 4 does, would reproduce its sums bit for bit but needs 12 more
+        // registers than the MMA warps have.)
+        float hh[4] = {0.f, 0.f, 0.f, 0.f}, ht[4] = {0.f, 0.f, 0.f, 0.f}, th[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+        for (int j = 0; j < NK1; ++j) {
+          const uint4 v = hb4[j * 4];
+          mma_f16(hh, wg_head[j], v.x, v.y);
+          mma_f16(ht, wg_head[j], v.z, v.w);
+          mma_f16(th, wg_tail[j], v.x, v.y);
+        }
+        out1[0] = (hh[0] + (ht[0] + th[0]) * kTailUnscale) * inv_g;
+        out1[RS1] = (hh[1] + (ht[1] + th[1]) * kTailUnscale) * inv_g;
+        out1[8] = (hh[2] + (ht[2] + th[2]) * kTailUnscale) * inv_g;
+        out1[RS1 + 8] = (hh[3] + (ht[3] + th[3]) * kTailUnscale) * inv_g;
+      } else {
         // four accumulation chains per warp (even / odd k-steps x head / tail weights): with two warps per scheduler a
         // chain of dependent MMAs would otherwise leave the tensor pipe waiting for its own results
         float c1[4] = {0.f, 0.f, 0.f, 0.f}, c2[4] = {0.f, 0.f, 0.f, 0.f};
@@ -674,7 +720,20 @@ bigru_mma_kernel(BiGruArgs a) {
       BG_STAMP(1);
       mbar_wait(bar_hr, (uint32_t)(s & 1));
       BG_STAMP(2);
-      {
+      if constexpr (RB == 8) {
+        float hh[4] = {0.f, 0.f, 0.f, 0.f}, ht[4] = {0.f, 0.f, 0.f, 0.f}, th[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+        for (int j = 0; j < NK2; ++j) {
+          const uint4 v = hrb4[j * 4];
+          mma_f16(hh, ws_head[j], v.x, v.y);
+          mma_f16(ht, ws_head[j], v.z, v.w);
+          mma_f16(th, ws_tail[j], v.x, v.y);
+        }
+        out2[0] = (hh[0] + (ht[0] + th[0]) * kTailUnscale) * inv_s;
+        out2[RS2] = (hh[1] + (ht[1] + th[1]) * kTailUnscale) * inv_s;
+        out2[8] = (hh[2] + (ht[2] + th[2]) * kTailUnscale) * inv_s;
+        out2[RS2 + 8] = (hh[3] + (ht[3] + th[3]) * kTailUnscale) * inv_s;
+      } else {
         float c1[4] = {0.f, 0.f, 0.f, 0.f}, c2[4] = {0.f, 0.f, 0.f, 0.f};
         float d1[4] = {0.f, 0.f, 0.f, 0.f}, d2[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
@@ -712,15 +771,19 @@ bigru_mma_kernel(BiGruArgs a) {
   } else {
     // =================================== elementwise warps ===========================================
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(EW_REGS));
-    const bool active = tid < 2 * NROLE;
-    const bool lead = tid < NROLE;            // ships the heads, writes the outputs; the others ship the tails and own z
+    const bool active = tid < PLANES * NROLE;
+    // RB = 4: the lead ships the heads and writes the outputs, its twin ships the tails and owns z.  RB = 8: one thread
+    // per role does all of it
+    const bool lead = tid < NROLE;
+    const bool owns_z = RB == 8 || !lead;
     const int rid = tid % NROLE;
     const int ug = rid % UG, erow = active ? rid / UG : 0;
     const int u_loc = 4 * ug, u_glob = rank * UC + u_loc;
     const bool row_ok = active && row0 + erow < B;
     const bool writer = row_ok && lead;
-    const int plane = lead ? 0 : 1;
-    const uint32_t loc_h = smem_u32(&hbuf[plane][erow][u_glob / 2]), loc_hr = smem_u32(&hrbuf[plane][erow][u_glob / 2]);
+    const int plane = RB == 4 && !lead ? 1 : 0;
+    const int word = RB == 4 ? u_glob / 2 : u_glob;   // first word of this role's group in a plane row
+    const uint32_t loc_h = smem_u32(&hbuf[plane][erow][word]), loc_hr = smem_u32(&hrbuf[plane][erow][word]);
     float h_own[4];
 #pragma unroll
     for (int i = 0; i < 4; ++i) h_own[i] = h0[u_glob + i];
@@ -744,7 +807,7 @@ bigru_mma_kernel(BiGruArgs a) {
     float pm = 1.f;
     if (row_ok) {
       pa = __ldg(reinterpret_cast<const float4*>(pre_ptr));
-      if (!lead) pz = __ldg(reinterpret_cast<const float4*>(pre_ptr + D));
+      if (owns_z) pz = __ldg(reinterpret_cast<const float4*>(pre_ptr + D));
       pr = __ldg(reinterpret_cast<const float4*>(pre_ptr + 2 * D));
       if (pm_ptr) pm = __ldg(pm_ptr);
     }
@@ -776,14 +839,19 @@ bigru_mma_kernel(BiGruArgs a) {
         uint32_t w0, w1, w2, w3;
         split_pair(h_own[0] * sr[0], h_own[1] * sr[1], w0, w1);
         split_pair(h_own[2] * sr[2], h_own[3] * sr[3], w2, w3);
-        const uint32_t x0 = lead ? w0 : w1, x1 = lead ? w2 : w3;
+        if constexpr (RB == 4) {
+          const uint32_t x0 = lead ? w0 : w1, x1 = lead ? w2 : w3;
 #pragma unroll
-        for (int p = 0; p < CS; ++p) st_async_v2_b32(map_to_rank(loc_hr, p), x0, x1, map_to_rank(bar_hr, p));
+          for (int p = 0; p < CS; ++p) st_async_v2_b32(map_to_rank(loc_hr, p), x0, x1, map_to_rank(bar_hr, p));
+        } else {
+#pragma unroll
+          for (int p = 0; p < CS; ++p) st_async_v4_b32(map_to_rank(loc_hr, p), make_uint4(w0, w2, w1, w3), map_to_rank(bar_hr, p));
+        }
         if constexpr (TAPE) {
           if (writer) *reinterpret_cast<float4*>(tape_ptr + 2 * D) = make_float4(sr[0], sr[1], sr[2], sr[3]);
         }
         if (more && row_ok) pr = __ldg(reinterpret_cast<const float4*>(pre_ptr + pre_step + 2 * D));
-        if (!lead) {
+        if (owns_z) {
           float sz[4] = {pz.x, pz.y, pz.z, pz.w};
 #pragma unroll
           for (int k = 0; k < KS1; ++k) {
@@ -821,9 +889,14 @@ bigru_mma_kernel(BiGruArgs a) {
         uint32_t w0, w1, w2, w3;
         split_pair(h_own[0], h_own[1], w0, w1);
         split_pair(h_own[2], h_own[3], w2, w3);
-        const uint32_t x0 = lead ? w0 : w1, x1 = lead ? w2 : w3;
+        if constexpr (RB == 4) {
+          const uint32_t x0 = lead ? w0 : w1, x1 = lead ? w2 : w3;
 #pragma unroll
-        for (int p = 0; p < CS; ++p) st_async_v2_b32(map_to_rank(loc_h, p), x0, x1, map_to_rank(bar_h, p));
+          for (int p = 0; p < CS; ++p) st_async_v2_b32(map_to_rank(loc_h, p), x0, x1, map_to_rank(bar_h, p));
+        } else {
+#pragma unroll
+          for (int p = 0; p < CS; ++p) st_async_v4_b32(map_to_rank(loc_h, p), make_uint4(w0, w2, w1, w3), map_to_rank(bar_h, p));
+        }
         if (writer) {
           const float4 hv = make_float4(h_own[0], h_own[1], h_own[2], h_own[3]);
           if (sub_phase == 0)
@@ -884,23 +957,55 @@ int mma_launch_config(cudaLaunchConfig_t& cfg, cudaLaunchAttribute* attr, int cl
   return 0;
 }
 
-template <int D, bool TAPE>
+// how many clusters of the tensor-core kernel the device holds at once (one CTA per SM, 4 SMs of one GPC per cluster)
+template <int D, int RB>
+int mma_clusters_resident() {
+  static int per_dev[LVSR_MAX_DEVICES];
+  static bool known[LVSR_MAX_DEVICES] = {false};
+  const int dev = current_device();
+  if (!known[dev]) {
+    known[dev] = true;
+    cudaLaunchConfig_t cfg;
+    cudaLaunchAttribute attr[1];
+    int k = 0;
+    if (mma_launch_config<D, false>(cfg, attr, 64, nullptr) != 0 ||
+        cudaOccupancyMaxActiveClusters(&k, bigru_mma_kernel<D, false, RB>, &cfg) != cudaSuccess) {
+      cudaGetLastError();
+      k = 0;
+    }
+    per_dev[dev] = k;
+  }
+  return per_dev[dev];
+}
+
+// waves of a launch of B rows: clusters never talk to each other, so a launch with more clusters than the device holds
+// at once runs them in turns, and every wave costs a whole sequence of steps (0: the kernel cannot be resident at all)
+template <int D, int RB>
+int mma_waves(int B) {
+  const int resident = mma_clusters_resident<D, RB>();
+  return resident > 0 ? ceil_div(2 * ceil_div(B, RB), resident) : 0;
+}
+
+template <int D, bool TAPE, int RB>
 int launch_bigru_mma_t(const BiGruArgs& a, cudaStream_t stream) {
   cudaLaunchConfig_t cfg;
   cudaLaunchAttribute attr[1];
-  if (int rc = mma_launch_config<D, TAPE>(cfg, attr, ceil_div(a.B, RB) * 2, stream)) return rc;
+  const int clusters = ceil_div(a.B, RB) * 2;
+  if (int rc = mma_launch_config<D, TAPE>(cfg, attr, clusters, stream)) return rc;
   static const bool trace = getenv("LVSR_BIGRU_TRACE") != nullptr;
   if (trace) {
     const int on = 1;
     LVSR_CUDA_OK(cudaMemcpyToSymbolAsync(g_bigru_trace_on, &on, sizeof(on), 0, cudaMemcpyHostToDevice, stream));
   }
-  LVSR_CUDA_OK(cudaLaunchKernelEx(&cfg, bigru_mma_kernel<D, TAPE>, a));
+  LVSR_CUDA_OK(cudaLaunchKernelEx(&cfg, bigru_mma_kernel<D, TAPE, RB>, a));
   g_launch_count++;
   if (trace) {
     unsigned long long h[12] = {0};
     LVSR_CUDA_OK(cudaMemcpyFromSymbolAsync(h, g_bigru_trace, sizeof(h), 0, cudaMemcpyDeviceToHost, stream));
     LVSR_CUDA_OK(cudaStreamSynchronize(stream));
     const double n = h[8] ? (double)h[8] : 1.0;
+    fprintf(stderr, "[bigru trace] mma<%d> RB=%d B=%d clusters=%d resident=%d waves=%d\n", D, RB, a.B, clusters,
+            mma_clusters_resident<D, RB>(), mma_waves<D, RB>(a.B));
     fprintf(stderr,
             "[bigru trace] mma<%d> T=%llu cycles/step  MMA warp: wait_h=%.0f gates=%.0f wait_hr=%.0f cand=%.0f | elementwise: "
             "wait_gates=%.0f r+send(+z)=%.0f wait_cand=%.0f cand+send+stores=%.0f\n",
@@ -924,31 +1029,10 @@ int launch_bigru_mma_t(const BiGruArgs& a, cudaStream_t stream) {
   return 0;
 }
 
-template <int D>
+template <int D, int RB>
 int launch_bigru_mma(const BiGruArgs& a, cudaStream_t stream) {
   LVSR_CHECK((a.tape == nullptr) == (a.hext == nullptr), "bigru: tape and hext go together");
-  return a.tape ? launch_bigru_mma_t<D, true>(a, stream) : launch_bigru_mma_t<D, false>(a, stream);
-}
-
-// how many clusters of the tensor-core kernel the device holds at once (one CTA per SM, 4 SMs of one GPC per cluster)
-template <int D>
-int mma_clusters_resident() {
-  static int per_dev[LVSR_MAX_DEVICES];
-  static bool known[LVSR_MAX_DEVICES] = {false};
-  const int dev = current_device();
-  if (!known[dev]) {
-    known[dev] = true;
-    cudaLaunchConfig_t cfg;
-    cudaLaunchAttribute attr[1];
-    int k = 0;
-    if (mma_launch_config<D, false>(cfg, attr, 64, nullptr) != 0 ||
-        cudaOccupancyMaxActiveClusters(&k, bigru_mma_kernel<D, false>, &cfg) != cudaSuccess) {
-      cudaGetLastError();
-      k = 0;
-    }
-    per_dev[dev] = k;
-  }
-  return per_dev[dev];
+  return a.tape ? launch_bigru_mma_t<D, true, RB>(a, stream) : launch_bigru_mma_t<D, false, RB>(a, stream);
 }
 
 int bigru_sm_count() { return device_sm_count(); }
@@ -1002,9 +1086,20 @@ int bigru_layer(const BiGruArgs& a, cudaStream_t stream) {
   // hidden size 256: tensor-core products.  Clusters never talk to each other, so a batch with more clusters than the
   // device holds at once (mma_clusters_resident, from the occupancy query) simply runs in waves -- still
   // ahead of the FFMA kernels, which would have to put two or more CTAs on every SM for such a batch.
-  bool mma = a.D == 256 && mma_clusters_resident<256>() > 0;
+  bool mma = a.D == 256 && mma_clusters_resident<256, 4>() > 0;
   if (const char* e = getenv("LVSR_BIGRU_MMA")) mma = a.D == 256 && atoi(e) != 0;
-  if (mma) return launch_bigru_mma<256>(a, stream);
+  if (mma) {
+    // 8-row clusters cost a third MMA per k-step and twice the elementwise work of a step, but halve the clusters:
+    // worth it only where that saves a wave
+    int rb = 4;
+    const int w8 = mma_waves<256, 8>(a.B);
+    if (w8 > 0 && w8 < mma_waves<256, 4>(a.B)) rb = 8;
+    if (const char* e = getenv("LVSR_BIGRU_RB")) {
+      rb = atoi(e);
+      if (rb != 4 && rb != 8) return set_error("bigru: LVSR_BIGRU_RB=%s (expected 4 or 8)", e);
+    }
+    return rb == 8 ? launch_bigru_mma<256, 8>(a, stream) : launch_bigru_mma<256, 4>(a, stream);
+  }
   switch (a.D) {
     case 128: return launch_bigru<128, 4, 8>(a, stream);
     case 256: return wide ? launch_bigru<256, 4, 16>(a, stream) : launch_bigru<256, 8, 8>(a, stream);
