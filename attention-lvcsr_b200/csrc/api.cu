@@ -324,12 +324,6 @@ int lvsr_model_destroy(lvsr_model* m) {
   for (float* p : m->bcat) if (p) cudaFree(p);
   for (float* p : m->Wcat_hi) if (p) cudaFree(p);
   for (float* p : m->Wcat_lo) if (p) cudaFree(p);
-  for (void* p : m->Wcat_h16_head) if (p) cudaFree(p);
-  for (void* p : m->Wcat_h16_tail) if (p) cudaFree(p);
-  for (float* p : m->Wcat_h16_scale) if (p) cudaFree(p);
-  if (m->Wp_h16_head) cudaFree(m->Wp_h16_head);
-  if (m->Wp_h16_tail) cudaFree(m->Wp_h16_tail);
-  if (m->Wp_h16_scale) cudaFree(m->Wp_h16_scale);
   if (m->Wp_hi) cudaFree(m->Wp_hi);
   if (m->Wp_lo) cudaFree(m->Wp_lo);
   if (m->Wd_cat) cudaFree(m->Wd_cat);
@@ -410,53 +404,6 @@ int lvsr_model_finalize(lvsr_model* m) {
 }  // extern "C"
 
 namespace lvsr {
-// fp16 head/tail operands for the projections that read BiGRU outputs (|h| <= 1): layers >= 1 and preprocess.
-// Allocated and split at their first use after a parameter change, i.e. AFTER the caller has reserved the workspace arena:
-// the arena keeps the device pages it gets without these buffers (the persistent decoder's step time can move with the
-// physical placement of its buffers).
-int ensure_h16(lvsr_model* m, cudaStream_t st) {
-  if (!m->use_tc || !m->use_h16 || !m->h16_stale) return 0;
-  const lvsr_config& c = m->cfg;
-  if (m->Wcat_h16_head.empty()) {
-    int dk2 = c.num_features;
-    for (int l = 0; l < c.num_layers; ++l) {
-      const int D = c.dims_bidir[l];
-      void *h = nullptr, *t = nullptr;
-      float* sc = nullptr;
-      if (l >= 1 && gemm_tc_h16_supported(128, 6 * D, dk2)) {
-        const size_t bytes = (size_t)gemm_tc_kpad_h16(dk2) * 6 * D * 2;
-        LVSR_CUDA_OK(cudaMalloc(&h, bytes));
-        LVSR_CUDA_OK(cudaMalloc(&t, bytes));
-        LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&sc), 2 * sizeof(float)));
-      }
-      m->Wcat_h16_head.push_back(h);
-      m->Wcat_h16_tail.push_back(t);
-      m->Wcat_h16_scale.push_back(sc);
-      dk2 = 2 * D;
-    }
-    if (gemm_tc_h16_supported(128, c.dim_matcher, m->E)) {
-      const size_t bytes = (size_t)gemm_tc_kpad_h16(m->E) * c.dim_matcher * 2;
-      LVSR_CUDA_OK(cudaMalloc(&m->Wp_h16_head, bytes));
-      LVSR_CUDA_OK(cudaMalloc(&m->Wp_h16_tail, bytes));
-      LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->Wp_h16_scale), 2 * sizeof(float)));
-    }
-  }
-  int dk2 = c.num_features;
-  for (int l = 0; l < c.num_layers; ++l) {
-    const int D = c.dims_bidir[l];
-    if (m->Wcat_h16_head[l])
-      if (int rc = split_weight_h16(m->Wcat[l], dk2, 6 * D, m->Wcat_h16_head[l], m->Wcat_h16_tail[l], m->Wcat_h16_scale[l], st))
-        return rc;
-    dk2 = 2 * D;
-  }
-  if (m->Wp_h16_head)
-    if (int rc = split_weight_h16(m->P(std::string(ATT) + "/preprocess.W"), m->E, c.dim_matcher, m->Wp_h16_head, m->Wp_h16_tail,
-                                  m->Wp_h16_scale, st))
-      return rc;
-  m->h16_stale = false;
-  return 0;
-}
-
 int finalize_on_stream(lvsr_model* m, cudaStream_t st, bool synchronise) {
   const lvsr_config& c = m->cfg;
   if (m->Wcat.empty()) {
@@ -533,11 +480,6 @@ int finalize_on_stream(lvsr_model* m, cudaStream_t st, bool synchronise) {
     if (m->Wp_hi)
       if (int rc = split_weight_tf32(m->P(std::string(ATT) + "/preprocess.W"), m->E, c.dim_matcher, m->Wp_hi, m->Wp_lo, st))
         return rc;
-    // fp16 head/tail operands of the same weights: re-split lazily at their next use (ensure_h16).  Opt-in
-    // (LVSR_F16_GEMM=1): half the operand bytes of the GEMMs, but extra device allocations that move the workspace to other
-    // physical pages, which the persistent decoder's step time is sensitive to.
-    m->use_h16 = getenv("LVSR_F16_GEMM") != nullptr && atoi(getenv("LVSR_F16_GEMM")) != 0;
-    m->h16_stale = true;
   }
   // fork(feedback(y)) for every symbol y, once: [(V+1), 3C]
   if (c.one_of_n_feedback) {
@@ -554,6 +496,63 @@ int finalize_on_stream(lvsr_model* m, cudaStream_t st, bool synchronise) {
                             cudaMemcpyDeviceToHost));
   if (synchronise) LVSR_CUDA_OK(cudaStreamSynchronize(st));
   m->finalized = true;
+  return 0;
+}
+
+// out[M, N] = A[M, K] . W + bias: the 3xTF32 wgmma GEMM when W has its K-major hi/lo split (W_hi, W_lo) and the shape suits
+// it, else the FFMA tile GEMM.  The split of A is scratch taken from `ws` and left there: it is dead once the GEMM is
+// enqueued, and the caller decides when to rewind it (lvsr_cost_matrix allocates the persistent decoder's buffers behind
+// it, and their place in the workspace is part of the decoder's measured step time).
+int projection_gemm(Arena& ws, const float* A, int M, int K, const float* W, const float* W_hi, const float* W_lo, int N,
+                    const float* bias, float* out, cudaStream_t st) {
+  if (W_hi && gemm_tc_supported(M, N, K)) {
+    float* a_hi = ws.f32((size_t)M * gemm_tc_kpad(K));
+    float* a_lo = ws.f32((size_t)M * gemm_tc_kpad(K));
+    LVSR_CHECK(a_hi && a_lo, "out of device memory (tf32 split scratch)");
+    return gemm_tc(A, a_hi, a_lo, M, K, W_hi, W_lo, N, bias, out, N, st);
+  }
+  return gemm_bias(make_gemm(A, M, K, W, N, bias, out), st);
+}
+
+int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int T, int B, float* attended,
+                float* attended_mask, LayerTape* tape, cudaStream_t st) {
+  const lvsr_config& c = m->cfg;
+  const float* cur = x;
+  int Tl = T, din = c.num_features;
+  long long mstride = B;
+  int kcum = 1;
+  for (int l = 0; l < c.num_layers; ++l) {
+    const int D = c.dims_bidir[l], k = c.subsample[l];
+    const int rows = Tl * B, Tout = ceil_div(Tl, k);
+    float* pre = ws.f32((size_t)rows * 6 * D);
+    float* hext = tape ? ws.f32((size_t)(Tl + 2) * B * 2 * D) : nullptr;
+    LVSR_CHECK(pre && (hext || !tape), "out of device memory (encoder pre-activations)");
+    // finalize splits the fork weights only while the tensor-core GEMM is on (null entry: a shape it refuses)
+    const size_t mark = ws.off;
+    if (int rc = projection_gemm(ws, cur, rows, din, m->Wcat[l], m->use_tc ? m->Wcat_hi[l] : nullptr,
+                                 m->use_tc ? m->Wcat_lo[l] : nullptr, 6 * D, m->bcat[l], pre, st))
+      return rc;
+    if (ws.off <= ws.cap) ws.off = mark;     // the split scratch is dead once the GEMM is enqueued (stream order)
+    float* out = (l == c.num_layers - 1) ? attended : ws.f32((size_t)Tout * B * 2 * D);
+    LVSR_CHECK(out, "out of device memory (encoder layer output)");
+    BiGruArgs a = {};
+    a.pre = pre; a.mask = mask; a.mask_tstride = mstride;
+    const std::string bf = enc_base(l, 0) + "/gatedrecurrent", bb = enc_base(l, 1) + "/gatedrecurrent";
+    a.Wg_f = m->P(bf + ".state_to_gates"); a.Ws_f = m->P(bf + ".state_to_state"); a.h0_f = m->P(bf + ".initial_state");
+    a.Wg_b = m->P(bb + ".state_to_gates"); a.Ws_b = m->P(bb + ".state_to_state"); a.h0_b = m->P(bb + ".initial_state");
+    a.out = out; a.T = Tl; a.B = B; a.D = D; a.subsample = k;
+    if (tape) {
+      a.tape = pre; a.hext = hext;
+      tape[l] = {cur, pre, hext, out, Tl, Tout, din, D, k, mstride};
+    }
+    if (int rc = bigru_layer(a, st)) return rc;
+    cur = out; Tl = Tout; din = 2 * D; mstride *= k; kcum *= k;
+  }
+  if (mask) {
+    if (int rc = gather_time_subsample(attended_mask, mask, Tl, kcum, B, st)) return rc;
+  } else {
+    if (int rc = fill_f32(attended_mask, (long long)Tl * B, 1.f, st)) return rc;   // lvsr/bricks/__init__.py:78
+  }
   return 0;
 }
 }  // namespace lvsr
@@ -576,59 +575,7 @@ int lvsr_encoder_forward(lvsr_model* m, const float* x, const float* mask, int32
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   m->ws.reserve(encoder_ws_bytes(m, T, B), st);
   ArenaScope scope(m, st);
-  const lvsr_config& c = m->cfg;
-  const float* cur = x;
-  int Tl = T, din = c.num_features;
-  long long mstride = B;
-  int kcum = 1;
-  for (int l = 0; l < c.num_layers; ++l) {
-    const int D = c.dims_bidir[l], k = c.subsample[l];
-    const int rows = Tl * B;
-    float* pre = m->ws.f32((size_t)rows * 6 * D);
-    LVSR_CHECK(pre, "out of device memory (encoder pre-activations)");
-    static const int h16_mask_e = getenv("LVSR_F16_GEMM_MASK") ? atoi(getenv("LVSR_F16_GEMM_MASK")) : 3;
-    if (l == 1 && (h16_mask_e & 1))
-      if (int rc = ensure_h16(m, st)) return rc;
-    if ((h16_mask_e & 1) && m->use_tc && m->use_h16 && l < (int)m->Wcat_h16_head.size() && m->Wcat_h16_head[l] && gemm_tc_h16_supported(rows, 6 * D, din)) {
-      // input = the previous layer's BiGRU output: fp16 head/tail operands (gemm_tc.cu)
-      const size_t mark = m->ws.off;
-      const size_t halfs = (size_t)rows * gemm_tc_kpad_h16(din);
-      float* a_h = m->ws.f32((halfs + 1) / 2);
-      float* a_t = m->ws.f32((halfs + 1) / 2);
-      LVSR_CHECK(a_h && a_t, "out of device memory (fp16 split scratch)");
-      if (int rc = gemm_tc_h16(cur, a_h, a_t, rows, din, m->Wcat_h16_head[l], m->Wcat_h16_tail[l], m->Wcat_h16_scale[l], 6 * D,
-                               m->bcat[l], pre, 6 * D, st))
-        return rc;
-      if (m->ws.off <= m->ws.cap) m->ws.off = mark;
-    } else if (m->use_tc && l < (int)m->Wcat_hi.size() && m->Wcat_hi[l] && gemm_tc_supported(rows, 6 * D, din)) {
-      const size_t mark = m->ws.off;
-      float* a_hi = m->ws.f32((size_t)rows * gemm_tc_kpad(din));
-      float* a_lo = m->ws.f32((size_t)rows * gemm_tc_kpad(din));
-      LVSR_CHECK(a_hi && a_lo, "out of device memory (tf32 split scratch)");
-      if (int rc = gemm_tc(cur, a_hi, a_lo, rows, din, m->Wcat_hi[l], m->Wcat_lo[l], 6 * D, m->bcat[l], pre, 6 * D, st)) return rc;
-      if (m->ws.off <= m->ws.cap) m->ws.off = mark;     // scratch is dead once the GEMM is enqueued (stream order)
-    } else {
-      GemmArgs g = make_gemm(cur, rows, din, m->Wcat[l], 6 * D, m->bcat[l], pre);
-      if (int rc = gemm_bias(g, st)) return rc;
-    }
-    const int Tout = ceil_div(Tl, k);
-    float* out = (l == c.num_layers - 1) ? attended : m->ws.f32((size_t)Tout * B * 2 * D);
-    LVSR_CHECK(out, "out of device memory (encoder layer output)");
-    BiGruArgs a = {};
-    a.pre = pre; a.mask = mask; a.mask_tstride = mstride;
-    const std::string bf = enc_base(l, 0) + "/gatedrecurrent", bb = enc_base(l, 1) + "/gatedrecurrent";
-    a.Wg_f = m->P(bf + ".state_to_gates"); a.Ws_f = m->P(bf + ".state_to_state"); a.h0_f = m->P(bf + ".initial_state");
-    a.Wg_b = m->P(bb + ".state_to_gates"); a.Ws_b = m->P(bb + ".state_to_state"); a.h0_b = m->P(bb + ".initial_state");
-    a.out = out; a.T = Tl; a.B = B; a.D = D; a.subsample = k;
-    if (int rc = bigru_layer(a, st)) return rc;
-    cur = out; Tl = Tout; din = 2 * D; mstride *= k; kcum *= k;
-  }
-  if (mask) {
-    if (int rc = gather_time_subsample(attended_mask, mask, Tl, kcum, B, st)) return rc;
-  } else {
-    if (int rc = fill_f32(attended_mask, (long long)Tl * B, 1.f, st)) return rc;   // lvsr/bricks/__init__.py:78
-  }
-  return 0;
+  return run_encoder(m, m->ws, x, mask, T, B, attended, attended_mask, nullptr, st);
 }
 
 int lvsr_preprocess(lvsr_model* m, const float* attended, int32_t Tp, int32_t U, float* out, void* stream) {
@@ -636,29 +583,9 @@ int lvsr_preprocess(lvsr_model* m, const float* attended, int32_t Tp, int32_t U,
   if (int rc = check_ready(m)) return rc;
   LVSR_CHECK(attended && out && Tp > 0 && U > 0, "preprocess: bad arguments");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  static const int h16_mask_p = getenv("LVSR_F16_GEMM_MASK") ? atoi(getenv("LVSR_F16_GEMM_MASK")) : 3;
-  if (h16_mask_p & 2)
-    if (int rc = ensure_h16(m, st)) return rc;
-  if ((h16_mask_p & 2) && m->use_tc && m->use_h16 && m->Wp_h16_head && gemm_tc_h16_supported(Tp * U, m->cfg.dim_matcher, m->E)) {
-    ArenaScope scope(m, st);
-    const size_t halfs = (size_t)Tp * U * gemm_tc_kpad_h16(m->E);
-    float* a_h = m->ws.f32((halfs + 1) / 2);
-    float* a_t = m->ws.f32((halfs + 1) / 2);
-    LVSR_CHECK(a_h && a_t, "out of device memory (fp16 split scratch)");
-    return gemm_tc_h16(attended, a_h, a_t, Tp * U, m->E, m->Wp_h16_head, m->Wp_h16_tail, m->Wp_h16_scale, m->cfg.dim_matcher,
-                       m->P(std::string(ATT) + "/preprocess.b"), out, m->cfg.dim_matcher, st);
-  }
-  if (m->use_tc && m->Wp_hi && gemm_tc_supported(Tp * U, m->cfg.dim_matcher, m->E)) {
-    ArenaScope scope(m, st);
-    float* a_hi = m->ws.f32((size_t)Tp * U * gemm_tc_kpad(m->E));
-    float* a_lo = m->ws.f32((size_t)Tp * U * gemm_tc_kpad(m->E));
-    LVSR_CHECK(a_hi && a_lo, "out of device memory (tf32 split scratch)");
-    return gemm_tc(attended, a_hi, a_lo, Tp * U, m->E, m->Wp_hi, m->Wp_lo, m->cfg.dim_matcher,
-                   m->P(std::string(ATT) + "/preprocess.b"), out, m->cfg.dim_matcher, st);
-  }
-  GemmArgs g = make_gemm(attended, Tp * U, m->E, m->P(std::string(ATT) + "/preprocess.W"), m->cfg.dim_matcher,
-                         m->P(std::string(ATT) + "/preprocess.b"), out);
-  return gemm_bias(g, st);
+  ArenaScope scope(m, st);
+  return projection_gemm(m->ws, attended, Tp * U, m->E, m->P(std::string(ATT) + "/preprocess.W"), m->use_tc ? m->Wp_hi : nullptr,
+                         m->Wp_lo, m->cfg.dim_matcher, m->P(std::string(ATT) + "/preprocess.b"), out, st);
 }
 
 int lvsr_cost_matrix(lvsr_model* m, const float* attended, const float* attended_mask, int32_t Tp, int32_t B,

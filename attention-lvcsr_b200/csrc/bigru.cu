@@ -100,13 +100,10 @@ __device__ __forceinline__ void st_async_v4(uint32_t remote_addr, float x, float
 // 72 loads per warp and step; k over 32 lanes: 24 loads but 46 exchanges and ~1000 instructions
 // per warp and step (issue-bound); 16 lanes sits between.
 //
-// Two shapes: <D, 8 or 4 CTAs, 8 warps> = 256 threads, two CTAs (two different clusters) per SM,
-// and <256, 4 CTAs, 16 warps> = 512 threads, one CTA per SM.  At the metric batch the second wins:
-// with two clusters sharing every SM any stall of one CTA delays its whole 8-CTA cluster twice per
-// step.
+// Shapes: <256, 8 CTAs, 8 warps> and <128, 4 CTAs, 8 warps> = 256 threads, two CTAs (two different clusters) per SM.
 // TAPE: training forward (stores c / z / r over the pre-activations and every frame of h); compiled out for inference
 template <int D, int CS, int NWARP, bool TAPE>
-__global__ void __launch_bounds__(NWARP * 32, NWARP == 8 ? 2 : 1)
+__global__ void __launch_bounds__(NWARP * 32, 2)
 bigru_kernel(BiGruArgs a) {
   constexpr int UC = D / CS;          // units owned by this CTA
   constexpr int KL = 16;              // lanes that split k
@@ -1035,54 +1032,13 @@ int launch_bigru_mma(const BiGruArgs& a, cudaStream_t stream) {
   return a.tape ? launch_bigru_mma_t<D, true, RB>(a, stream) : launch_bigru_mma_t<D, false, RB>(a, stream);
 }
 
-int bigru_sm_count() { return device_sm_count(); }
-
-// how many <256, 4, 16> clusters the device holds at once (a GPC takes floor(SMs / 4) of them; the
-// count differs between parts with different floor-sweeping, so ask the driver)
-int wide_clusters_resident() {
-  static int per_dev[LVSR_MAX_DEVICES];
-  static bool known[LVSR_MAX_DEVICES] = {false};
-  const int dev = current_device();
-  int& n = per_dev[dev];
-  if (!known[dev]) {
-    known[dev] = true;
-    constexpr size_t W2S_BYTES = (size_t)16 * (256 / 16 / 4) * 2 * 32 * 4 * sizeof(float);
-    cudaFuncSetAttribute(bigru_kernel<256, 4, 16, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)W2S_BYTES);
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(4 * 64);
-    cfg.blockDim = dim3(16 * 32);
-    cfg.dynamicSmemBytes = W2S_BYTES;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 4;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    int k = 0;
-    if (cudaOccupancyMaxActiveClusters(&k, bigru_kernel<256, 4, 16, false>, &cfg) != cudaSuccess) {
-      cudaGetLastError();
-      k = 0;
-    }
-    n = k;
-  }
-  return n;
-}
-
 }  // namespace
 
 bool bigru_supported(int D) { return D == 128 || D == 256; }
 
-
-
 int bigru_layer(const BiGruArgs& a, cudaStream_t stream) {
   ProfScope prof("bigru", stream);
   if (a.T <= 0 || a.B <= 0) return 0;
-  // D = 256: 4 CTAs x 16 warps (one CTA per SM) as soon as the 8 x 8 shape would have to put two
-  // CTAs on an SM, as long as every such cluster still gets SMs of its own
-  const int groups = ceil_div(a.B, RB);
-  bool wide = a.D == 256 && 8 * groups * 2 > bigru_sm_count() && groups * 2 <= wide_clusters_resident();
-  if (const char* e = getenv("LVSR_BIGRU_WIDE")) wide = a.D == 256 && atoi(e) != 0;
   // hidden size 256: tensor-core products.  Clusters never talk to each other, so a batch with more clusters than the
   // device holds at once (mma_clusters_resident, from the occupancy query) simply runs in waves -- still
   // ahead of the FFMA kernels, which would have to put two or more CTAs on every SM for such a batch.
@@ -1102,7 +1058,7 @@ int bigru_layer(const BiGruArgs& a, cudaStream_t stream) {
   }
   switch (a.D) {
     case 128: return launch_bigru<128, 4, 8>(a, stream);
-    case 256: return wide ? launch_bigru<256, 4, 16>(a, stream) : launch_bigru<256, 8, 8>(a, stream);
+    case 256: return launch_bigru<256, 8, 8>(a, stream);
     default:
       return set_error("bigru: unsupported hidden size %d (supported: 128, 256)", a.D);
   }

@@ -21,7 +21,6 @@
 // On an H100 a 128 x 256 tile (2 stages, 128 accumulators per thread) measured 7 % slower for the
 // projections of the metric configuration than this shape.
 #include <cuda.h>
-#include <cuda_fp16.h>
 
 #include "kernels.h"
 
@@ -35,7 +34,6 @@ constexpr int TC_STAGES = 3;
 constexpr uint32_t TC_TILE_BYTES = TC_BM * TC_BK * sizeof(float);          // 16 KB: one 128-row operand tile
 constexpr uint32_t TC_STAGE_BYTES = 4 * TC_TILE_BYTES;                     // A_hi, A_lo, B_hi, B_lo
 constexpr size_t TC_SMEM = (size_t)TC_STAGES * TC_STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
-constexpr int TC_BK_H16 = 64;      // fp16 operands: one 128-byte swizzle row holds 64 k values
 
 __device__ __forceinline__ uint32_t smem_addr(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
 
@@ -73,7 +71,7 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
 // ---- wgmma ---------------------------------------------------------------------------------------------------------
 // K-major, SWIZZLE_128B canonical layout: rows are 128 B, 8-row groups are 1024 B apart (sm_90 shared-memory matrix
 // descriptor: start address, leading byte offset (unused for swizzled K-major), stride byte offset, layout type 1 =
-// 128-byte swizzle).  One k-step (8 tf32 or 16 fp16 values = 32 bytes) further along a row is start address + 2.
+// 128-byte swizzle).  One k-step (8 tf32 values = 32 bytes) further along a row is start address + 2.
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);          // start address, 16 B units
@@ -109,20 +107,6 @@ __device__ __forceinline__ void wgmma_tf32_n128(float (&d)[64], uint64_t desc_a,
         LVSR_ACC8(d, 32), LVSR_ACC8(d, 40), LVSR_ACC8(d, 48), LVSR_ACC8(d, 56)
       : "l"(desc_a), "l"(desc_b), "r"(scale_d));
 }
-__device__ __forceinline__ void wgmma_f16_n128(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %66, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {"
-      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
-      "}, %64, %65, p, 1, 1, 0, 0;\n\t}\n"
-      : LVSR_ACC8(d, 0), LVSR_ACC8(d, 8), LVSR_ACC8(d, 16), LVSR_ACC8(d, 24),
-        LVSR_ACC8(d, 32), LVSR_ACC8(d, 40), LVSR_ACC8(d, 48), LVSR_ACC8(d, 56)
-      : "l"(desc_a), "l"(desc_b), "r"(scale_d));
-}
 #undef LVSR_ACC8
 
 struct TcGemmParams {
@@ -131,14 +115,8 @@ struct TcGemmParams {
   int M, N, K, ldc;
   int kb_per_split;            // K blocks handled by one blockIdx.z (split-K: partial products, summed by the caller)
   long long c_split_stride;    // elements between the partial outputs of consecutive splits
-  const float* out_scale;      // H16: device pointer to the factor that undoes the power-of-two weight scaling (or null)
 };
 
-// H16: operands are fp16 heads and fp16 tails scaled by 2^11 (x = head + tail / 2048); head.head goes to one set of
-// accumulators, tail.head + head.tail to a second one, the epilogue adds main + cross / 2048.  Same 2^-22 error class as
-// the 3xTF32 split at half the operand bytes and half the tensor time (an fp16 wgmma does twice the MACs of a tf32 one)
-// -- for operands of known range only (the BiGRU outputs, |h| <= 1, against weights scaled below 2^14).
-template <bool H16>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
                const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo,
@@ -146,7 +124,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B needs 1024-byte aligned tiles
   uint8_t* tiles = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  constexpr int BKE = H16 ? TC_BK_H16 : TC_BK;          // k values per 128-byte row
   constexpr int NACC = TC_BN / 2;                       // accumulators per consumer thread (m64 x 128 over 128 threads)
   unsigned long long* bars = reinterpret_cast<unsigned long long*>(tiles + (size_t)TC_STAGES * TC_STAGE_BYTES);
   // bars[0..S): full (TMA bytes landed), bars[S..2S): empty (both consumer warpgroups are done with the slot)
@@ -154,7 +131,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
   const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
   const int n0 = blockIdx.x * TC_BN, m0 = blockIdx.y * TC_BM;
   const int kb0 = blockIdx.z * p.kb_per_split;
-  const int nkb = min(p.kb_per_split, p.K / BKE - kb0);
+  const int nkb = min(p.kb_per_split, p.K / TC_BK - kb0);
   p.C += (long long)blockIdx.z * p.c_split_stride;
 
   if (threadIdx.x == 0) {
@@ -176,10 +153,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
         const uint32_t full = smem_addr(&bars[s]);
         bar_expect_tx(full, TC_STAGE_BYTES);
         const uint32_t base = smem_addr(tiles + (size_t)s * TC_STAGE_BYTES);
-        tma_load_2d(base + 0 * TC_TILE_BYTES, &map_a_hi, (kb0 + kb) * BKE, m0, full);
-        tma_load_2d(base + 1 * TC_TILE_BYTES, &map_a_lo, (kb0 + kb) * BKE, m0, full);
-        tma_load_2d(base + 2 * TC_TILE_BYTES, &map_b_hi, (kb0 + kb) * BKE, n0, full);
-        tma_load_2d(base + 3 * TC_TILE_BYTES, &map_b_lo, (kb0 + kb) * BKE, n0, full);
+        tma_load_2d(base + 0 * TC_TILE_BYTES, &map_a_hi, (kb0 + kb) * TC_BK, m0, full);
+        tma_load_2d(base + 1 * TC_TILE_BYTES, &map_a_lo, (kb0 + kb) * TC_BK, m0, full);
+        tma_load_2d(base + 2 * TC_TILE_BYTES, &map_b_hi, (kb0 + kb) * TC_BK, n0, full);
+        tma_load_2d(base + 3 * TC_TILE_BYTES, &map_b_lo, (kb0 + kb) * TC_BK, n0, full);
       }
     }
     return;
@@ -187,11 +164,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
 
   // ===== consumers: warpgroup wg - 1 owns rows [64 (wg - 1), +64) of the tile =====
   const uint32_t a_off = (uint32_t)(wg - 1) * 64 * 128;          // 64 rows of 128 bytes into each A tile
-  float acc[NACC], accx[H16 ? NACC : 1];
+  float acc[NACC];
 #pragma unroll
   for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
-#pragma unroll
-  for (int i = 0; i < (H16 ? NACC : 1); ++i) accx[i] = 0.f;
   for (int kb = 0; kb < nkb; ++kb) {
     const int s = kb % TC_STAGES;
     bar_wait(smem_addr(&bars[s]), (uint32_t)((kb / TC_STAGES) & 1));
@@ -202,34 +177,24 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
 #pragma unroll
     for (int k = 0; k < 4; ++k) {                      // 4 k-steps of 32 bytes per 128-byte row
       const uint64_t adv = (uint64_t)(k * 2);
-      if constexpr (H16) {
-        wgmma_f16_n128(accx, da_lo + adv, db_hi + adv, 1u);     // cross terms
-        wgmma_f16_n128(accx, da_hi + adv, db_lo + adv, 1u);
-        wgmma_f16_n128(acc, da_hi + adv, db_hi + adv, 1u);
-      } else {
-        wgmma_tf32_n128(acc, da_lo + adv, db_hi + adv, 1u);     // small terms first
-        wgmma_tf32_n128(acc, da_hi + adv, db_lo + adv, 1u);
-        wgmma_tf32_n128(acc, da_hi + adv, db_hi + adv, 1u);
-      }
+      wgmma_tf32_n128(acc, da_lo + adv, db_hi + adv, 1u);     // small terms first
+      wgmma_tf32_n128(acc, da_hi + adv, db_lo + adv, 1u);
+      wgmma_tf32_n128(acc, da_hi + adv, db_hi + adv, 1u);
     }
     wgmma_commit();
     // the products of stage kb - 1 have retired: its slot goes back to the producer
     wgmma_wait<1>();
     acc_fence(acc);
-    if constexpr (H16) acc_fence(accx);
     if (kb > 0 && t == 0) bar_arrive(smem_addr(&bars[TC_STAGES + (kb - 1) % TC_STAGES]));
   }
   wgmma_wait<0>();
   acc_fence(acc);
-  if constexpr (H16) acc_fence(accx);
 
   // ===== epilogue: accumulator fragment -> global (+bias).  Register 4j + {0,1}: row 16 warp + lane / 4, columns
   // 8j + 2 (lane % 4) + {0,1}; register 4j + {2,3}: the same columns 8 rows further down. =====
   const int warp = t >> 5, lane = t & 31;
   const int r0 = m0 + (wg - 1) * 64 + warp * 16 + (lane >> 2);
   const int cbase = n0 + 2 * (lane & 3);
-  float os = 1.f;
-  if constexpr (H16) os = p.out_scale ? __ldg(p.out_scale) : 1.f;
 #pragma unroll
   for (int j = 0; j < TC_BN / 8; ++j) {
     const int col = cbase + 8 * j;
@@ -238,11 +203,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int row = r0 + 8 * h;
-      float x = acc[4 * j + 2 * h], y = acc[4 * j + 2 * h + 1];
-      if constexpr (H16) {
-        x = fmaf(accx[4 * j + 2 * h], 1.f / 2048.f, x) * os;
-        y = fmaf(accx[4 * j + 2 * h + 1], 1.f / 2048.f, y) * os;
-      }
+      const float x = acc[4 * j + 2 * h], y = acc[4 * j + 2 * h + 1];
       if (row < p.M) *reinterpret_cast<float2*>(p.C + (long long)row * p.ldc + col) = make_float2(x + b.x, y + b.y);
     }
   }
@@ -392,7 +353,7 @@ int gemm_tc_presplit(const float* A_hi, const float* A_lo, int M, const float* B
   static bool configured[LVSR_MAX_DEVICES] = {false};
   const int dev = current_device();
   if (!configured[dev]) {
-    LVSR_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM));
+    LVSR_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM));
     configured[dev] = true;
   }
   const int total_kb = Kpad / TC_BK;
@@ -401,9 +362,8 @@ int gemm_tc_presplit(const float* A_hi, const float* A_lo, int M, const float* B
   p.C = C; p.bias = bias; p.M = M; p.N = N; p.K = Kpad; p.ldc = ldc;
   p.kb_per_split = ceil_div(total_kb, splits);
   p.c_split_stride = split_stride;
-  p.out_scale = nullptr;
   dim3 grid(N / TC_BN, ceil_div(M, TC_BM), ceil_div(total_kb, p.kb_per_split));
-  gemm_tc_kernel<false><<<grid, TC_THREADS, TC_SMEM, stream>>>(ma_hi, ma_lo, mb_hi, mb_lo, p);
+  gemm_tc_kernel<<<grid, TC_THREADS, TC_SMEM, stream>>>(ma_hi, ma_lo, mb_hi, mb_lo, p);
   LVSR_LAUNCH_CHECK();
   return 0;
 }
@@ -425,149 +385,6 @@ int gemm_tc(const float* A, float* A_hi, float* A_lo, int M, int K, const float*
   }
   LVSR_LAUNCH_CHECK();
   return gemm_tc_presplit(A_hi, A_lo, M, Wt_hi, Wt_lo, N, Kpad, bias, C, ldc, 1, 0, stream);
-}
-
-
-// ---- fp16 head/tail variant (inference projections whose input is a BiGRU output) ------------------------------------
-namespace {
-
-__device__ __forceinline__ void split_h16(float x, float y, __half2& head, __half2& tail) {
-  head = __floats2half2_rn(x, y);
-  const float2 hf = __half22float2(head);
-  tail = __floats2half2_rn((x - hf.x) * 2048.f, (y - hf.y) * 2048.f);
-}
-
-// x [M, K] fp32 -> heads / scaled tails [M, Kpad] fp16 (zero padding of the contraction dimension)
-__global__ void split_h16_kernel(const float* __restrict__ x, __half2* __restrict__ head, __half2* __restrict__ tail, long long M,
-                                 int K, int Kpad) {
-  const long long total = M * (Kpad / 2);
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    const long long r = i / (Kpad / 2);
-    const int k = (int)(i % (Kpad / 2)) * 2;
-    float a = 0.f, b = 0.f;
-    if (k + 1 < K) {
-      const float2 v = *reinterpret_cast<const float2*>(x + r * K + k);      // K % 2 == 0, rows 8-byte aligned
-      a = v.x; b = v.y;
-    } else if (k < K) {
-      a = x[r * K + k];
-    }
-    __half2 h, t;
-    split_h16(a, b, h, t);
-    head[i] = h;
-    tail[i] = t;
-  }
-}
-
-// scale2[0] = power of two that brings max|W| below 2^14 (1 for every sane model), scale2[1] = its inverse
-__global__ void weight_scale_kernel(const float* __restrict__ W, long long n, float* __restrict__ scale2) {
-  __shared__ float red[32];
-  float mx = 0.f;
-  for (long long i = threadIdx.x; i < n; i += blockDim.x) mx = fmaxf(mx, fabsf(W[i]));
-  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = mx;
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    mx = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.f;
-    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-    if (threadIdx.x == 0) {
-      float sc = 1.f, inv = 1.f;
-      if (mx > 16384.f && mx < 3.0e38f) {
-        const int e = ((__float_as_int(mx) >> 23) & 0xff) - 127;
-        sc = __int_as_float((127 - (e - 13)) << 23);
-        inv = __int_as_float((127 + (e - 13)) << 23);
-      }
-      scale2[0] = sc;
-      scale2[1] = inv;
-    }
-  }
-}
-
-// [K, N] row-major -> K-major [N, Kpad] heads / scaled tails of W * scale2[0]
-__global__ void transpose_split_h16_kernel(const float* __restrict__ W, __half* __restrict__ head, __half* __restrict__ tail,
-                                           int K, int N, int Kpad, int ldw, const float* __restrict__ scale2) {
-  __shared__ float tile[32][33];
-  const float sc = scale2[0];
-  const int k0 = blockIdx.y * 32, n0 = blockIdx.x * 32;
-  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-    const int k = k0 + i, n = n0 + threadIdx.x;
-    tile[i][threadIdx.x] = (k < K && n < N) ? W[(long long)k * ldw + n] * sc : 0.f;
-  }
-  __syncthreads();
-  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-    const int n = n0 + i, k = k0 + threadIdx.x;
-    if (n < N && k < Kpad) {
-      const float a = tile[threadIdx.x][i];
-      const __half h = __float2half_rn(a);
-      head[(long long)n * Kpad + k] = h;
-      tail[(long long)n * Kpad + k] = __float2half_rn((a - __half2float(h)) * 2048.f);
-    }
-  }
-}
-
-// 2-D fp16 tensor [rows, Kpad] (K contiguous), box = [box_rows, 64 halfs], 128-byte swizzle
-int make_map_h16(CUtensorMap* map, const void* ptr, long long rows, int Kpad, int box_rows) {
-  cuuint64_t dims[2] = {(cuuint64_t)Kpad, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)Kpad * sizeof(__half)};
-  cuuint32_t box[2] = {(cuuint32_t)TC_BK_H16, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = g_encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  LVSR_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled (fp16) failed (%d)", (int)r);
-  return 0;
-}
-
-}  // namespace
-
-int gemm_tc_kpad_h16(int K) { return ceil_div(K, TC_BK_H16) * TC_BK_H16; }
-bool gemm_tc_h16_supported(int M, int N, int K) { return M >= 1 && N % TC_BN == 0 && K >= 2 && K % 2 == 0; }
-
-// head / tail: [N, gemm_tc_kpad_h16(K)] halfs; scale2: 2 floats on the device
-int split_weight_h16(const float* W, int K, int N, void* head, void* tail, float* scale2, cudaStream_t stream) {
-  const int Kpad = gemm_tc_kpad_h16(K);
-  weight_scale_kernel<<<1, 1024, 0, stream>>>(W, (long long)K * N, scale2);
-  LVSR_LAUNCH_CHECK();
-  dim3 grid(ceil_div(N, 32), ceil_div(Kpad, 32)), block(32, 8);
-  transpose_split_h16_kernel<<<grid, block, 0, stream>>>(W, static_cast<__half*>(head), static_cast<__half*>(tail), K, N, Kpad, N,
-                                                          scale2);
-  LVSR_LAUNCH_CHECK();
-  return 0;
-}
-
-// C[M,N] = A[M,K] . W + bias with W given as the K-major head/tail pair of split_weight_h16.  |A| must stay inside the
-// fp16 range (the callers pass BiGRU outputs).  A_head / A_tail: scratch of M * gemm_tc_kpad_h16(K) halfs each.
-int gemm_tc_h16(const float* A, void* A_head, void* A_tail, int M, int K, const void* Wt_head, const void* Wt_tail,
-                const float* scale2, int N, const float* bias, float* C, int ldc, cudaStream_t stream) {
-  ProfScope prof("gemm", stream);
-  LVSR_CHECK(gemm_tc_h16_supported(M, N, K), "gemm_tc_h16: unsupported shape M=%d N=%d K=%d", M, N, K);
-  if (int rc = get_encode()) return rc;
-  const int Kpad = gemm_tc_kpad_h16(K);
-  {
-    const long long n = (long long)M * (Kpad / 2);
-    split_h16_kernel<<<(int)std::min<long long>(4096, (n + 255) / 256), 256, 0, stream>>>(
-        A, static_cast<__half2*>(A_head), static_cast<__half2*>(A_tail), M, K, Kpad);
-    LVSR_LAUNCH_CHECK();
-  }
-  CUtensorMap ma_h, ma_t, mb_h, mb_t;
-  if (int rc = make_map_h16(&ma_h, A_head, M, Kpad, TC_BM)) return rc;
-  if (int rc = make_map_h16(&ma_t, A_tail, M, Kpad, TC_BM)) return rc;
-  if (int rc = make_map_h16(&mb_h, Wt_head, N, Kpad, TC_BN)) return rc;
-  if (int rc = make_map_h16(&mb_t, Wt_tail, N, Kpad, TC_BN)) return rc;
-  static bool configured[LVSR_MAX_DEVICES] = {false};
-  const int dev = current_device();
-  if (!configured[dev]) {
-    LVSR_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM));
-    configured[dev] = true;
-  }
-  TcGemmParams p;
-  p.C = C; p.bias = bias; p.M = M; p.N = N; p.K = Kpad; p.ldc = ldc;
-  p.kb_per_split = Kpad / TC_BK_H16;
-  p.c_split_stride = 0;
-  p.out_scale = scale2 ? scale2 + 1 : nullptr;
-  dim3 grid(N / TC_BN, ceil_div(M, TC_BM), 1);
-  gemm_tc_kernel<true><<<grid, TC_THREADS, TC_SMEM, stream>>>(ma_h, ma_t, mb_h, mb_t, p);
-  LVSR_LAUNCH_CHECK();
-  return 0;
 }
 
 }  // namespace lvsr

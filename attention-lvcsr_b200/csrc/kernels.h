@@ -37,12 +37,6 @@ int split_tf32(const float* x, float* hi, float* lo, long long n, cudaStream_t s
 int gemm_tc_presplit(const float* A_hi, const float* A_lo, int M, const float* B_hi, const float* B_lo, int N, int Kpad,
                      const float* bias, float* C, int ldc, int splits, long long split_stride, cudaStream_t stream);
 int gemm_tc_splits_launched(int Kpad, int splits);   // how many partial outputs gemm_tc_presplit writes
-// fp16 head/tail variant (fp16 wgmma): half the operand bytes and tensor time of the tf32 split; inputs of bounded range only
-bool gemm_tc_h16_supported(int M, int N, int K);
-int gemm_tc_kpad_h16(int K);             // contraction dimension as stored in the fp16 operands (multiple of 64)
-int split_weight_h16(const float* W, int K, int N, void* head, void* tail, float* scale2, cudaStream_t stream);
-int gemm_tc_h16(const float* A, void* A_head, void* A_tail, int M, int K, const void* Wt_head, const void* Wt_tail,
-                const float* scale2, int N, const float* bias, float* C, int ldc, cudaStream_t stream);
 int gemm_tc(const float* A, float* A_hi, float* A_lo, int M, int K, const float* Wt_hi, const float* Wt_lo, int N,
             const float* bias, float* C, int ldc, cudaStream_t stream);
 

@@ -121,14 +121,6 @@ struct lvsr_model {
   std::vector<float*> Wcat_hi, Wcat_lo;
   float *Wp_hi = nullptr, *Wp_lo = nullptr;
   bool use_tc = true;
-  // fp16 head/tail splits of the same weights for the inference projections whose input is a BiGRU output (layers >= 1,
-  // preprocess): K-major [N, Kpad64] halfs + {scale, 1/scale} on the device; null = tf32 path
-  std::vector<void*> Wcat_h16_head, Wcat_h16_tail;
-  std::vector<float*> Wcat_h16_scale;
-  void *Wp_h16_head = nullptr, *Wp_h16_tail = nullptr;
-  float* Wp_h16_scale = nullptr;
-  bool use_h16 = true;
-  bool h16_stale = true;            // the fp16 operands do not match the parameters (re-split at the next use)
   float v_bias = 0.f;               // host copy of energy_comp/linear.b
   unsigned* status = nullptr;       // device word: launch status of the data-flow decoder (common.cuh LVSR_FLOW_*)
   bool force_stepwise = false;      // set while a failed persistent launch is re-run on the step-wise kernels
@@ -202,8 +194,23 @@ static inline int check_ready(lvsr_model* m) {
   return 0;
 }
 
+// One encoder layer as the training step's backward pass reads it.
+struct LayerTape {
+  const float* X;      // input of the layer [T*B, Din]
+  float* pre;          // [T*B, 6D] forward tape, then dPre
+  float* hext;         // [(T+2), B, 2D]
+  float* out;          // [Tout, B, 2D]
+  int T, Tout, Din, D, k;
+  long long mstride;
+};
+
 // shared orchestration pieces (api.cu)
 int finalize_on_stream(lvsr_model* m, cudaStream_t st, bool synchronise);
+// Every encoder layer (fork projection + BiGRU scan) and the mask of the encoded frames: attended [Tp, B, E] (the last
+// layer writes it), attended_mask [Tp, B].  Buffers come from `ws`.  Without a tape (inference) the BiGRU runs without
+// the training stores; with one, tape[l] records layer l's buffers (and allocates hext) for the backward pass.
+int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int T, int B, float* attended,
+                float* attended_mask, LayerTape* tape, cudaStream_t st);
 int readout_merged(lvsr_model* m, int R, const float* states, const float* ctx, float* merged, cudaStream_t st);
 ReadoutArgs readout_args(lvsr_model* m, int R, const float* merged);
 size_t encoder_ws_bytes(const lvsr_model* m, int T, int B);

@@ -135,15 +135,6 @@ int gemm_tn_tc(Arena& ws, const TcOperand& A, int a0, int Mo, const TcOperand& B
   return 0;
 }
 
-struct LayerTape {
-  const float* X;      // input of the layer [T*B, Din]
-  float* pre;          // [T*B, 6D] forward tape, then dPre
-  float* hext;         // [(T+2), B, 2D]
-  float* out;          // [Tout, B, 2D]
-  int T, Tout, Din, D, k;
-  long long mstride;
-};
-
 float* grad_of(lvsr_model* m, float* grads, const std::string& name) {
   auto it = m->index.find(name);
   return it == m->index.end() ? nullptr : grads + m->params[it->second].offset;
@@ -195,50 +186,11 @@ int lvsr_train_cost_and_grads(lvsr_model* m, const float* x, const float* mask, 
   LVSR_CUDA_OK(cudaMemsetAsync(grads, 0, (size_t)m->flat_count * sizeof(float), st));
 
   // =========================== forward, keeping the tape ===========================
-  std::vector<LayerTape> tape(c.num_layers);
-  {
-    const float* cur = x;
-    int Tl = T, din = c.num_features;
-    long long mstride = B;
-    for (int l = 0; l < c.num_layers; ++l) {
-      const int D = c.dims_bidir[l], k = c.subsample[l], rows = Tl * B, Tout = ceil_div(Tl, k);
-      LayerTape& tp = tape[l];
-      tp.X = cur; tp.T = Tl; tp.Tout = Tout; tp.Din = din; tp.D = D; tp.k = k; tp.mstride = mstride;
-      tp.pre = ws.f32((size_t)rows * 6 * D);
-      tp.hext = ws.f32((size_t)(Tl + 2) * B * 2 * D);
-      tp.out = ws.f32((size_t)Tout * B * 2 * D);
-      LVSR_CHECK(tp.pre && tp.hext && tp.out, "out of device memory (encoder tape)");
-      if (m->use_tc && l < (int)m->Wcat_hi.size() && m->Wcat_hi[l] && gemm_tc_supported(rows, 6 * D, din)) {
-        const size_t mark = ws.off;
-        float* a_hi = ws.f32((size_t)rows * gemm_tc_kpad(din));
-        float* a_lo = ws.f32((size_t)rows * gemm_tc_kpad(din));
-        LVSR_CHECK(a_hi && a_lo, "out of device memory (tf32 split scratch)");
-        if (int rc = gemm_tc(cur, a_hi, a_lo, rows, din, m->Wcat_hi[l], m->Wcat_lo[l], 6 * D, m->bcat[l], tp.pre, 6 * D, st)) return rc;
-        if (ws.off <= ws.cap) ws.off = mark;
-      } else {
-        if (int rc = gemm_nn(cur, rows, din, din, m->Wcat[l], 6 * D, 6 * D, m->bcat[l], tp.pre, 6 * D, false, st)) return rc;
-      }
-      BiGruArgs a = {};
-      a.pre = tp.pre; a.mask = mask; a.mask_tstride = mstride;
-      const std::string bf = enc_base(l, 0) + "/gatedrecurrent", bb = enc_base(l, 1) + "/gatedrecurrent";
-      a.Wg_f = m->P(bf + ".state_to_gates"); a.Ws_f = m->P(bf + ".state_to_state"); a.h0_f = m->P(bf + ".initial_state");
-      a.Wg_b = m->P(bb + ".state_to_gates"); a.Ws_b = m->P(bb + ".state_to_state"); a.h0_b = m->P(bb + ".initial_state");
-      a.out = tp.out; a.T = Tl; a.B = B; a.D = D; a.subsample = k;
-      a.tape = tp.pre; a.hext = tp.hext;
-      if (int rc = bigru_layer(a, st)) return rc;
-      cur = tp.out; Tl = Tout; din = 2 * D; mstride *= k;
-    }
-  }
-  const float* Hatt = tape.back().out;                       // attended [Tp, B, E]
+  float* Hatt = ws.f32((size_t)Tp * B * E);                  // attended [Tp, B, E]
   float* attm = ws.f32((size_t)Tp * B);
-  LVSR_CHECK(attm, "out of device memory");
-  if (mask) {
-    int kcum = 1;
-    for (int l = 0; l < c.num_layers; ++l) kcum *= c.subsample[l];
-    if (int rc = gather_time_subsample(attm, mask, Tp, kcum, B, st)) return rc;
-  } else {
-    if (int rc = fill_f32(attm, (long long)Tp * B, 1.f, st)) return rc;
-  }
+  LVSR_CHECK(Hatt && attm, "out of device memory (encoder output)");
+  std::vector<LayerTape> tape(c.num_layers);
+  if (int rc = run_encoder(m, ws, x, mask, T, B, Hatt, attm, tape.data(), st)) return rc;
   float* costs = ws.f32((size_t)R);
   float* W_all = ws.f32((size_t)R * Tp);        // alignments alpha_i
   float* S_prev = ws.f32((size_t)R * C);        // s_{i-1}

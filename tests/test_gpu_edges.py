@@ -253,22 +253,3 @@ def test_recurrent_weights_beyond_the_fp16_range():
     x, m, labels, lm = O.synthetic_batch(cfg, B=4, T=24, seed=21)
     _compare_cost(cfg, params, x, m, labels, lm)
 
-
-def test_fp16_split_projection_gemm_opt_in(monkeypatch):
-    """LVSR_F16_GEMM=1: the fork GEMMs of layers >= 1 and attention.preprocess on fp16 wgmma with fp16 head/tail
-    operands (gemm_tc.cu) -- the oracle bar of every other path, and agreement with the default 3xTF32 kernel."""
-    torch = _torch()
-    cfg = O.make_config(**WSJ_ENC)
-    params = O.init_params(cfg, seed=3, scale=10.0)
-    x, m, labels, lm = O.synthetic_batch(cfg, B=6, T=64, seed=31)
-    ref_rec = make_recognizer(cfg, params)                      # parameters are finalised at the first call
-    ref_att = ref_rec.encode(x, m)[0].clone()
-    ref_pre = ref_rec.cost_matrix(labels, lm, ref_att, ref_rec.encode(x, m)[1], return_all=True)["costs"].clone()
-    monkeypatch.setenv("LVSR_F16_GEMM", "1")
-    errs = _compare_cost(cfg, params, x, m, labels, lm)         # a fresh recognizer: finalize reads the switch
-    rec = make_recognizer(cfg, params)
-    att, attm = rec.encode(x, m)
-    d_att = float((att - ref_att).abs().max() / ref_att.abs().max())
-    d_cost = float((rec.cost_matrix(labels, lm, att, attm, return_all=True)["costs"] - ref_pre).abs().max() / ref_pre.abs().max())
-    print("fp16-split GEMM vs oracle", errs, "vs 3xTF32", d_att, d_cost)
-    assert d_att < 2e-5 and d_cost < TOL, (d_att, d_cost)

@@ -1,5 +1,5 @@
-"""Numerics of the fp16 head/tail split the tensor-core BiGRU (csrc/bigru.cu: bigru_mma_kernel) and the opt-in fp16 GEMM
-(csrc/gemm_tc.cu) feed to the tensor cores, restated in numpy: x = head + tail / 2^11 with fp16 head and fp16 tail, product
+"""Numerics of the fp16 head/tail split the tensor-core BiGRU (csrc/bigru.cu: bigru_mma_kernel) feeds to the tensor cores,
+restated in numpy: x = head + tail / 2^11 with fp16 head and fp16 tail, product
 head_w*head_h + (head_w*tail_h + tail_w*head_h) / 2^11.  The claim in DESIGN.md section 2 is an error of 2^-21 of sum |w h|
 (the dropped tail*tail term), i.e. the class of the 3xTF32 split; the power-of-two range scaling must be exact."""
 import numpy as np
@@ -26,7 +26,7 @@ def split_dot(w, h):
 
 
 def range_scale(max_abs):
-    """mirror of range_scale() in bigru.cu / weight_scale_kernel in gemm_tc.cu"""
+    """mirror of range_scale() in bigru.cu"""
     if not (16384.0 < max_abs < 3.0e38):
         return 1.0, 1.0
     e = int(np.floor(np.log2(max_abs)))
