@@ -56,6 +56,8 @@ class LvsrTrainConfig(C.Structure):
 # name -> (restype, argtypes); every symbol include/lvsr_b200.h declares
 _P = C.c_void_p
 _I = C.c_int32
+# lvsr_validate_fn(validate_user, utt, tokens, length); VALIDATE_FN() is the NULL callback
+VALIDATE_FN = C.CFUNCTYPE(C.c_int32, _P, C.c_int32, C.POINTER(C.c_int64), C.c_int32)
 SIGNATURES = {
     "lvsr_last_error": (C.c_char_p, []),
     "lvsr_version": (C.c_int, []),
@@ -79,10 +81,8 @@ SIGNATURES = {
     "lvsr_initial_states": (C.c_int, [_P, _I, _I, _P, _P, _P, _P, _P, _P, _P]),
     "lvsr_logprobs": (C.c_int, [_P, _P, _P, _P, _I, _I, _P, _I, _P, _P, _P, _P, _P]),
     "lvsr_next_states": (C.c_int, [_P, _P, _P, _P, _I, _I, _P, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
-    "lvsr_search_expand": (C.c_int, [_P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _I, _P, _P, _P, _P, _P, _P, _P, _P]),
-    "lvsr_search_advance": (C.c_int, [_P, _P, _P, _P, _I, _I, _P, _I, _P, _P, _P, _P, _P, _I, _P, _P, _P, _P, _P, _P, _I,
-                                      _P, _P, _P, _P, _P, _P]),
-    "lvsr_beam_search_many": (C.c_int, [_P, _P, _P, _P, _I, _I, _P, _P, _I, _I, _I, C.c_double, C.c_double, _I, C.POINTER(_P), _P]),
+    "lvsr_beam_search_many": (C.c_int, [_P, _P, _P, _P, _I, _I, _P, _P, _I, _I, _I, C.c_double, C.c_double, _I, VALIDATE_FN,
+                                        _P, C.POINTER(_P), _P]),
     "lvsr_search_result_count": (C.c_int, [_P, _I]),
     "lvsr_search_result_length": (C.c_int, [_P, _I, _I]),
     "lvsr_search_result_get": (C.c_int, [_P, _I, _I, _P, _P]),

@@ -229,7 +229,7 @@ size_t cost_ws_bytes(const lvsr_model* m, int Tp, int B, int L) {
 extern "C" {
 
 const char* lvsr_last_error(void) { return g_last_error.c_str(); }
-int lvsr_version(void) { return 100; }
+int lvsr_version(void) { return 101; }
 int64_t lvsr_launch_count(int reset) {
   const int64_t v = g_launch_count;
   if (reset) g_launch_count = 0;
@@ -844,19 +844,15 @@ int lvsr_next_states(lvsr_model* m, const float* attended, const float* preproce
   return add_i64(reinterpret_cast<long long*>(next_step), reinterpret_cast<const long long*>(step), R, 1, st);
 }
 
-int lvsr_search_expand(lvsr_model* m, const float* attended, const float* preprocessed, const float* attended_mask,
-                       int32_t Tp, int32_t U, const int32_t* utt_len, const int32_t* row_utt, const int32_t* row_seg,
-                       const int32_t* seg_start, int32_t nseg, int32_t R, const float* states, const float* weights,
-                       const int64_t* step, const float* cost_so_far, int32_t k, float* wavg, float* new_weights,
-                       float* new_energies, int32_t* top_parent, int32_t* top_symbol, float* top_cost, int32_t* top_count,
-                       void* stream) {
-  DeviceGuard device_guard(m);
-  if (int rc = check_ready(m)) return rc;
-  LVSR_CHECK(attended && preprocessed && attended_mask && row_utt && row_seg && seg_start && states && weights && step &&
-                 cost_so_far && wavg && new_weights && new_energies && top_parent && top_symbol && top_cost && top_count &&
-                 Tp > 0 && U > 0 && nseg > 0 && R > 0 && k > 0,
-             "search_expand: bad arguments");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
+}  // extern "C"
+
+namespace lvsr {
+
+int search_expand(lvsr_model* m, const float* attended, const float* preprocessed, const float* attended_mask, int Tp,
+                  int U, const int* utt_len, const int* row_utt, const int* row_seg, const int* seg_start, int nseg,
+                  int R, const float* states, const float* weights, const long long* step, const float* cost_so_far,
+                  int k, float* wavg, float* new_weights, float* new_energies, int* top_parent, int* top_symbol,
+                  float* top_cost, int* top_count, cudaStream_t st) {
   ArenaScope scope(m, st);
   const lvsr_config& c = m->cfg;
   Arena& ws = m->ws;
@@ -867,8 +863,8 @@ int lvsr_search_expand(lvsr_model* m, const float* attended, const float* prepro
   sg.seg_start = seg_start; sg.nseg = nseg; sg.seg_len = utt_len; sg.row_seg = row_seg;
   // take_glimpses ONCE per hypothesis: the same glimpse feeds the readout (logprobs_computer) and, for the
   // surviving parents, the state update (next_state_computer) -- B/search.py:109-142 computes it twice
-  if (int rc = glimpses(m, attended, preprocessed, attended_mask, Tp, U, row_utt, R, states, weights,
-                        reinterpret_cast<const long long*>(step), 0, new_weights, new_energies, wavg, st, sg)) return rc;
+  if (int rc = glimpses(m, attended, preprocessed, attended_mask, Tp, U, row_utt, R, states, weights, step, 0,
+                        new_weights, new_energies, wavg, st, sg)) return rc;
   if (int rc = readout_merged(m, R, states, wavg, merged, st)) return rc;
   ReadoutArgs r = readout_args(m, R, merged);
   r.costs_all = neglogp;
@@ -876,17 +872,12 @@ int lvsr_search_expand(lvsr_model* m, const float* attended, const float* prepro
   return segment_topk(neglogp, cost_so_far, seg_start, nseg, c.num_phonemes, k, top_parent, top_symbol, top_cost, top_count, st);
 }
 
-int lvsr_search_advance(lvsr_model* m, const float* attended, const float* preprocessed, const float* attended_mask,
-                        int32_t Tp, int32_t U, const int32_t* utt_len, int32_t Rn, const int32_t* parent,
-                        const int64_t* symbols, const int32_t* row_utt, const int32_t* row_seg, const int32_t* seg_start,
-                        int32_t nseg, const float* states, const float* weights, const int64_t* step, const float* wavg,
-                        const float* new_weights, const float* new_energies, int32_t reuse_glimpses, float* n_states,
-                        float* n_wavg, float* n_weights, float* n_energies, int64_t* n_step, void* stream) {
-  DeviceGuard device_guard(m);
-  if (int rc = check_ready(m)) return rc;
-  LVSR_CHECK(parent && symbols && states && step && n_states && n_wavg && n_weights && n_energies && n_step && Rn > 0 && Tp > 0,
-             "search_advance: bad arguments");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
+int search_advance(lvsr_model* m, const float* attended, const float* preprocessed, const float* attended_mask, int Tp,
+                   int U, const int* utt_len, int Rn, const int* parent, const long long* symbols, const int* row_utt,
+                   const int* row_seg, const int* seg_start, int nseg, const float* states, const float* weights,
+                   const long long* step, const float* wavg, const float* new_weights, const float* new_energies,
+                   float* n_states, float* n_wavg, float* n_weights, float* n_energies, long long* n_step,
+                   cudaStream_t st) {
   ArenaScope scope(m, st);
   const lvsr_config& c = m->cfg;
   Arena& ws = m->ws;
@@ -894,29 +885,30 @@ int lvsr_search_advance(lvsr_model* m, const float* attended, const float* prepr
   float* s_sel = ws.f32((size_t)Rn * C);
   LVSR_CHECK(s_sel, "out of device memory (search workspace)");
   if (int rc = gather_rows(s_sel, states, parent, Rn, C, st)) return rc;
-  if (reuse_glimpses) {
-    LVSR_CHECK(wavg && new_weights && new_energies, "search_advance: glimpses of the parents are missing");
+  if (c.prior_type == LVSR_PRIOR_EXPANDING) {
     if (int rc = gather_rows(n_wavg, wavg, parent, Rn, E, st)) return rc;
     if (int rc = gather_rows(n_weights, new_weights, parent, Rn, Tp, st)) return rc;
     if (int rc = gather_rows(n_energies, new_energies, parent, Rn, Tp, st)) return rc;
   } else {
     // window priors: the reference recomputes the glimpses over the SELECTED parents, whose batch-global cut
     // (lvsr/bricks/attention.py:151-152) can differ from the cut over the whole beam
-    LVSR_CHECK(attended && preprocessed && attended_mask && row_utt && row_seg && seg_start && weights && nseg > 0,
-               "search_advance: contexts are required to recompute the glimpses");
     float* w_sel = ws.f32((size_t)Rn * Tp);
     long long* st_sel = ws.i64((size_t)Rn);
     LVSR_CHECK(w_sel && st_sel, "out of device memory (search workspace)");
     if (int rc = gather_rows(w_sel, weights, parent, Rn, Tp, st)) return rc;
-    if (int rc = gather_i64(st_sel, reinterpret_cast<const long long*>(step), parent, Rn, 0, st)) return rc;
+    if (int rc = gather_i64(st_sel, step, parent, Rn, 0, st)) return rc;
     Segments sg;
     sg.seg_start = seg_start; sg.nseg = nseg; sg.seg_len = utt_len; sg.row_seg = row_seg;
     if (int rc = glimpses(m, attended, preprocessed, attended_mask, Tp, U, row_utt, Rn, s_sel, w_sel, st_sel, 0, n_weights,
                           n_energies, n_wavg, st, sg)) return rc;
   }
-  if (int rc = transition(m, Rn, s_sel, n_wavg, reinterpret_cast<const long long*>(symbols), nullptr, n_states, st)) return rc;
-  return gather_i64(reinterpret_cast<long long*>(n_step), reinterpret_cast<const long long*>(step), parent, Rn, 1, st);
+  if (int rc = transition(m, Rn, s_sel, n_wavg, symbols, nullptr, n_states, st)) return rc;
+  return gather_i64(n_step, step, parent, Rn, 1, st);
 }
+
+}  // namespace lvsr
+
+extern "C" {
 
 int lvsr_recognizer_cost_host(lvsr_model* m, const float* x_h, const float* mask_h, const int64_t* labels_h,
                               const float* lmask_h, int32_t T, int32_t B, int32_t L, float* costs_h, void* stream) {

@@ -216,4 +216,30 @@ ReadoutArgs readout_args(lvsr_model* m, int R, const float* merged);
 size_t encoder_ws_bytes(const lvsr_model* m, int T, int B);
 size_t cost_ws_bytes(const lvsr_model* m, int Tp, int B, int L);
 
+// The two device steps of lvsr_beam_search_many (search.cu), which holds the device guard and has finalized the
+// model.  The hypotheses (rows) of utterance s are the contiguous rows [seg_start[s], seg_start[s+1]) -- one segment
+// is what the reference calls the batch inside BeamSearch.search, so the batch-global window cut of take_glimpses
+// is taken per segment.  row_utt[r] = column of the row's utterance in attended / preprocessed / attended_mask
+// [T',U,.]; row_seg[r] = its segment; utt_len[s] = valid encoded frames of the segment's utterance.
+//
+// search_expand = logprobs_computer + BeamSearch._smallest (B/search.py:109-117,220-242,341-344): take_glimpses once
+// per row (kept in wavg / new_weights / new_energies for search_advance), readout, -log softmax, and per segment the
+// k smallest cost_so_far + (-logp) in increasing order: top_parent (row index), top_symbol, top_cost [nseg * k],
+// top_count [nseg] (= min(k, width * V); -1 if a log-probability was not finite).
+int search_expand(lvsr_model* m, const float* attended, const float* preprocessed, const float* attended_mask, int Tp,
+                  int U, const int* utt_len, const int* row_utt, const int* row_seg, const int* seg_start, int nseg,
+                  int R, const float* states, const float* weights, const long long* step, const float* cost_so_far,
+                  int k, float* wavg, float* new_weights, float* new_energies, int* top_parent, int* top_symbol,
+                  float* top_cost, int* top_count, cudaStream_t st);
+// search_advance = next_state_computer (B/search.py:119-142) for the Rn selected children (parent rows + symbols):
+// gathers the parents' state and, under the expanding prior, their glimpses from search_expand (exact there because
+// the window does not depend on which rows are in the batch); under the window_around_* priors it recomputes
+// take_glimpses over the selected rows as the reference does.  Then Distribute + GRU step; step + 1.
+int search_advance(lvsr_model* m, const float* attended, const float* preprocessed, const float* attended_mask, int Tp,
+                   int U, const int* utt_len, int Rn, const int* parent, const long long* symbols, const int* row_utt,
+                   const int* row_seg, const int* seg_start, int nseg, const float* states, const float* weights,
+                   const long long* step, const float* wavg, const float* new_weights, const float* new_energies,
+                   float* n_states, float* n_wavg, float* n_weights, float* n_energies, long long* n_step,
+                   cudaStream_t st);
+
 }  // namespace lvsr

@@ -1,11 +1,11 @@
 // BeamSearch.search for MANY utterances, the whole loop native (libs/blocks/blocks/search.py:244-399 as modified by
 // lvsr: char_discount, round_to_inf, stop_on, ignore_first_eol; driven by lvsr/bricks/recognizer.py:513-533).
 //
-// The per-step device work is lvsr_search_expand / lvsr_search_advance (api.cu): one glimpse per hypothesis, readout,
+// The per-step device work is search_expand / search_advance (api.cu): one glimpse per hypothesis, readout,
 // per-utterance k-best on the GPU, gather + transition.  This file is the reference's host bookkeeping -- histories,
 // the `done` list, the two stopping criteria, the final ranking -- in C++, so a step costs one small H2D, one small
-// D2H and one stream synchronisation for ALL utterances instead of a Python loop per utterance.  The Python mirror
-// (attention-lvcsr_b200/search.py) keeps an equivalent loop for searches with a validate_solution_function callback.
+// D2H and one stream synchronisation for ALL utterances instead of a Python loop per utterance.  It is the only
+// search loop: a validate_solution_function reaches it as the `validate` callback.
 //
 // Arithmetic that decides orderings is done the way numpy / Python do it there: cumulative costs are float32
 // (numpy.take / vstack of float32 arrays), the ranking key `cost - char_discount * len` is float64, sorting is stable.
@@ -60,7 +60,8 @@ extern "C" {
 int lvsr_beam_search_many(lvsr_model* m, const float* attended, const float* preprocessed, const float* attended_mask,
                           int32_t Tp, int32_t U, const int32_t* utt_len_host, const int32_t* max_length_host,
                           int32_t beam_size, int32_t eol_symbol, int32_t ignore_first_eol, double char_discount,
-                          double round_to_inf, int32_t stop_on_optimistic, lvsr_search_result** result, void* stream) {
+                          double round_to_inf, int32_t stop_on_optimistic, lvsr_validate_fn validate, void* validate_user,
+                          lvsr_search_result** result, void* stream) {
   DeviceGuard device_guard(m);
   if (int rc = check_ready(m)) return rc;
   LVSR_CHECK(attended && preprocessed && attended_mask && utt_len_host && max_length_host && result && Tp > 0 && U > 0 && beam_size > 0,
@@ -69,7 +70,6 @@ int lvsr_beam_search_many(lvsr_model* m, const float* attended, const float* pre
   const lvsr_config& c = m->cfg;
   const int C = c.dim_dec, E = m->E, V = c.num_phonemes, k = beam_size;
   const int Rmax = U * k;
-  const int reuse = c.prior_type == LVSR_PRIOR_EXPANDING ? 1 : 0;
 
   // ---- device state: two sets of (states, weights, step) + the per-step outputs, one allocation -----------------
   auto rnd = [](size_t b) { return (b + 255) & ~(size_t)255; };
@@ -201,9 +201,9 @@ int lvsr_beam_search_many(lvsr_model* m, const float* attended, const float* pre
     LVSR_CUDA_OK(cudaMemcpyAsync(d_cost, h_cost, (size_t)R * sizeof(float), cudaMemcpyHostToDevice, st));
     int* d_seg = d_meta; int* d_rseg = d_seg + nseg + 1; int* d_rutt = d_rseg + R; int* d_len = d_rutt + R;
     int* tp = d_top; int* ts = tp + nseg * k; float* tc = reinterpret_cast<float*>(ts + nseg * k); int* tn = ts + 2 * nseg * k;
-    if (int rc = lvsr_search_expand(m, attended, preprocessed, attended_mask, Tp, U, d_len, d_rutt, d_rseg, d_seg, nseg, R,
-                                    states[curset], weights[curset], reinterpret_cast<int64_t*>(step[curset]), d_cost, k, wavg,
-                                    new_w, new_e, tp, ts, tc, tn, stream)) return rc;
+    if (int rc = search_expand(m, attended, preprocessed, attended_mask, Tp, U, d_len, d_rutt, d_rseg, d_seg, nseg, R,
+                               states[curset], weights[curset], step[curset], d_cost, k, wavg, new_w, new_e, tp, ts, tc, tn,
+                               st)) return rc;
     LVSR_CUDA_OK(cudaMemcpyAsync(h_top, d_top, ((size_t)3 * nseg * k + nseg) * sizeof(int), cudaMemcpyDeviceToHost, st));
     LVSR_CUDA_OK(cudaStreamSynchronize(st));                 // the step's only synchronisation
     const int* hp = h_top; const int* hs = hp + nseg * k;
@@ -236,8 +236,13 @@ int lvsr_beam_search_many(lvsr_model* m, const float* attended, const float* pre
         const size_t n = costs2[j].size();
         // finished: last symbol is eol and the step's own cost stays below round_to_inf (float32 difference, :365-367)
         if (is_eol && (double)(float)(costs2[j][n - 1] - costs2[j][n - 2]) < round_to_inf) {
-          lvsr_search_result::Hyp h; h.tokens = outs2[j]; h.costs = costs2[j];
-          ut.done.push_back(std::move(h));
+          // validate_solution_function (:368-370); the step has synchronised, so nothing is in flight on an abort
+          const int32_t valid = validate ? validate(validate_user, order[s], outs2[j].data(), (int32_t)n) : 1;
+          LVSR_CHECK(valid >= 0, "beam_search_many: the validate callback failed for utterance %d", order[s]);
+          if (valid) {
+            lvsr_search_result::Hyp h; h.tokens = outs2[j]; h.costs = costs2[j];
+            ut.done.push_back(std::move(h));
+          }
         }
         const bool alive = !is_eol || (ignore_first_eol && i == 0);
         if (alive) { keep_after.push_back(base + j); outs3.push_back(std::move(outs2[j])); costs3.push_back(std::move(costs2[j])); }
@@ -269,11 +274,9 @@ int lvsr_beam_search_many(lvsr_model* m, const float* attended, const float* pre
     // advance writes into the other set (or, when rows are dropped afterwards, into scratch that is then compacted)
     float* a_states = all_kept ? states[o] : tmp_s;
     float* a_weights = all_kept ? weights[o] : tmp_w;
-    if (int rc = lvsr_search_advance(m, attended, preprocessed, attended_mask, Tp, U, d_len2, Rs, d_par,
-                                     reinterpret_cast<const int64_t*>(d_sym), d_rutt2, d_rseg2, d_seg2, nseg, states[curset],
-                                     weights[curset], reinterpret_cast<const int64_t*>(step[curset]), wavg, new_w, new_e, reuse,
-                                     a_states, n_wavg, a_weights, n_e,
-                                     reinterpret_cast<int64_t*>(all_kept ? step[o] : tmp_step), stream)) return rc;
+    if (int rc = search_advance(m, attended, preprocessed, attended_mask, Tp, U, d_len2, Rs, d_par, d_sym, d_rutt2, d_rseg2,
+                                d_seg2, nseg, states[curset], weights[curset], step[curset], wavg, new_w, new_e, a_states,
+                                n_wavg, a_weights, n_e, all_kept ? step[o] : tmp_step, st)) return rc;
     if (!all_kept && nkeep > 0) {
       if (int rc = gather_rows(states[o], a_states, d_keep, nkeep, C, st)) return rc;
       if (int rc = gather_rows(weights[o], a_weights, d_keep, nkeep, Tp, st)) return rc;

@@ -139,52 +139,28 @@ int lvsr_next_states(lvsr_model* m, const float* attended_dev, const float* prep
                      float* next_weights_dev, float* next_energies_dev, int64_t* next_step_dev,
                      void* stream);
 
-/* ---- batched beam search: one step for MANY utterances --------------------------------------------
- * The hypotheses (rows) of utterance s are the contiguous rows [seg_start[s], seg_start[s+1]) -- one segment is
- * what the reference calls the batch inside BeamSearch.search (libs/blocks/blocks/search.py:244-399), so the
- * batch-global window cut of take_glimpses is taken per segment.  row_utt[r] = column of the row's utterance in
- * attended / preprocessed / attended_mask [T',U,.]; row_seg[r] = its segment; utt_len[s] = valid encoded frames of
- * the segment's utterance (NULL: T').  All hypothesis state stays on the device:
- *
- *   lvsr_search_expand  = logprobs_computer + BeamSearch._smallest (:109-117,220-242,341-344): take_glimpses once per
- *     row (kept in wavg / new_weights / new_energies for lvsr_search_advance), readout, -log softmax, and per
- *     segment the k smallest cost_so_far + (-logp) in increasing order: top_parent (row index), top_symbol,
- *     top_cost [nseg * k], top_count [nseg] (= min(k, width * V); -1 if a log-probability was not finite).
- *     Only these k triples per utterance have to reach the host.
- *   lvsr_search_advance = next_state_computer (:119-142) for the Rn selected children (parent rows + symbols):
- *     gathers the parents' state and -- reuse_glimpses != 0 -- their glimpses (exact when the window does not
- *     depend on which rows are in the batch: the expanding prior), else recomputes take_glimpses over the selected
- *     rows as the reference does (window_around_* priors); then Distribute + GRU step; step + 1. */
-int lvsr_search_expand(lvsr_model* m, const float* attended_dev, const float* preprocessed_dev,
-                       const float* attended_mask_dev, int32_t Tp, int32_t U, const int32_t* utt_len_dev,
-                       const int32_t* row_utt_dev, const int32_t* row_seg_dev, const int32_t* seg_start_dev,
-                       int32_t nseg, int32_t R, const float* states_dev, const float* weights_dev,
-                       const int64_t* step_dev, const float* cost_so_far_dev, int32_t k, float* wavg_dev,
-                       float* new_weights_dev, float* new_energies_dev, int32_t* top_parent_dev,
-                       int32_t* top_symbol_dev, float* top_cost_dev, int32_t* top_count_dev, void* stream);
-int lvsr_search_advance(lvsr_model* m, const float* attended_dev, const float* preprocessed_dev,
-                        const float* attended_mask_dev, int32_t Tp, int32_t U, const int32_t* utt_len_dev, int32_t Rn,
-                        const int32_t* parent_dev, const int64_t* symbols_dev, const int32_t* row_utt_dev,
-                        const int32_t* row_seg_dev, const int32_t* seg_start_dev, int32_t nseg, const float* states_dev,
-                        const float* weights_dev, const int64_t* step_dev, const float* wavg_dev,
-                        const float* new_weights_dev, const float* new_energies_dev, int32_t reuse_glimpses,
-                        float* next_states_dev, float* next_wavg_dev, float* next_weights_dev,
-                        float* next_energies_dev, int64_t* next_step_dev, void* stream);
-
-/* The whole search loop of BeamSearch.search (libs/blocks/blocks/search.py:244-399) for U utterances decoded in
- * lock-step: the reference's bookkeeping (histories, `done`, both stopping criteria, final ranking) in C++ around
- * lvsr_search_expand / lvsr_search_advance; per step one small H2D, one small D2H, one synchronisation for ALL
- * utterances.  utt_len_host[u] = valid encoded frames, max_length_host[u] = int(T_u / max_decoded_length_scale)
+/* ---- beam search: the whole loop of BeamSearch.search for MANY utterances -------------------------
+ * (libs/blocks/blocks/search.py:244-399) for U utterances decoded in lock-step: all hypothesis state and the k-best
+ * selection stay on the device, and the reference's bookkeeping (histories, `done`, both stopping criteria, final
+ * ranking) runs in C++; per step one small H2D, one small D2H, one synchronisation for ALL utterances.
+ * utt_len_host[u] = valid encoded frames, max_length_host[u] = int(T_u / max_decoded_length_scale)
  * (lvsr/bricks/recognizer.py:519-520).  stop_on_optimistic: 0 = 'patience', 1 = 'optimistic_future_cost'.
  * Result: per utterance the finished hypotheses ranked by cost - char_discount * length, each as its full token
- * and cumulative-cost history INCLUDING the initial symbol (what BeamSearch keeps in `done`).  A
- * validate_solution_function callback is not available here (the Python mirror runs its own loop for that). */
+ * and cumulative-cost history INCLUDING the initial symbol (what BeamSearch keeps in `done`).
+ *
+ * validate (may be NULL: every finished hypothesis is kept) is the reference's validate_solution_function
+ * (:365-371): called once for every hypothesis that has just ended in eol_symbol, with the utterance index and
+ * the full token history including the initial symbol, in utterance order and then in increasing candidate
+ * order.  It returns 1 to add the hypothesis to `done`, 0 to drop it, and a negative value to abort the search:
+ * lvsr_beam_search_many then returns non-zero without a result.  `validate_user` is passed through unchanged. */
+typedef int32_t (*lvsr_validate_fn)(void* validate_user, int32_t utt, const int64_t* tokens, int32_t length);
 typedef struct lvsr_search_result lvsr_search_result;
 int lvsr_beam_search_many(lvsr_model* m, const float* attended_dev, const float* preprocessed_dev,
                           const float* attended_mask_dev, int32_t Tp, int32_t U, const int32_t* utt_len_host,
                           const int32_t* max_length_host, int32_t beam_size, int32_t eol_symbol,
                           int32_t ignore_first_eol, double char_discount, double round_to_inf,
-                          int32_t stop_on_optimistic, lvsr_search_result** result, void* stream);
+                          int32_t stop_on_optimistic, lvsr_validate_fn validate, void* validate_user,
+                          lvsr_search_result** result, void* stream);
 int lvsr_search_result_count(const lvsr_search_result* r, int32_t utt);                     /* finished hypotheses */
 int lvsr_search_result_length(const lvsr_search_result* r, int32_t utt, int32_t j);         /* history length     */
 int lvsr_search_result_get(const lvsr_search_result* r, int32_t utt, int32_t j, int64_t* tokens, float* costs);

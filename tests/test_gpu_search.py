@@ -1,5 +1,6 @@
-"""Batched, device-resident beam search (lvsr_search_expand / lvsr_search_advance, BeamSearch.search_many)
-against the float64 oracle's line-for-line BeamSearch.search run per utterance: identical token lists."""
+"""Batched, device-resident beam search (lvsr_beam_search_many, BeamSearch.search_many) against the float64
+oracle's line-for-line BeamSearch.search run per utterance: identical token lists, also when a
+validate_solution_function filters the finished hypotheses."""
 import numpy as np
 import pytest
 
@@ -22,7 +23,7 @@ def _peaky(cfg, seed, gain=10.0, eos_bias=1.0):
     return params
 
 
-PRIORS = [None, dict(type="window_around_median", before=6, after=8),
+PRIORS = [None, dict(type="window_around_median", before=6, after=8), dict(type="window_around_mean", before=7, after=7),
           dict(type="expanding", initial_begin=0, initial_end=6, min_speed=0.8, max_speed=2.5)]
 
 
@@ -85,37 +86,84 @@ def test_search_launch_count_is_shared_by_all_utterances():
     assert many <= 1.5 * one                              # not 12x
 
 
-@pytest.mark.parametrize("stop_on,char_discount", [("patience", 0.0), ("optimistic_future_cost", 0.2)])
-def test_native_loop_equals_python_loop(stop_on, char_discount):
-    """lvsr_beam_search_many (the loop in C++) returns exactly what the Python mirror of BeamSearch.search returns:
-    every finished hypothesis, its per-step costs and the ranking."""
-    _torch()
+def _validated_case():
     cfg = O.make_config(prior=dict(type="window_around_mean", before=7, after=7), max_decoded_length_scale=2.5, **PYRAMID)
-    params = _peaky(cfg, 4)
+    params = _peaky(cfg, 11, eos_bias=2.0)           # about 50 finished hypotheses, about half of them kept
     rng = np.random.RandomState(8)
     utts = [rng.normal(size=(T, cfg["num_features"])).astype(np.float32) for T in (60, 33, 48, 25, 57)]
     rec = make_recognizer(cfg, params)
     rec.init_beam_search(6)
-    bs = rec._beam_search
-    maxl = [int(u.shape[0] / 2.5) for u in utts]
-    native = bs.search_many(utts, cfg["eos_label"], maxl, stop_on=stop_on, char_discount=char_discount,
-                            raise_on_failure=False, as_arrays=True)
-    bs.force_python_loop = True
-    python = bs.search_many(utts, cfg["eos_label"], maxl, stop_on=stop_on, char_discount=char_discount,
-                            raise_on_failure=False, as_arrays=True)
-    bs.force_python_loop = False
-    assert len(native) == len(python) == 5
-    compared = 0
-    for a, b in zip(native, python):
-        assert (a is None) == (b is None)
-        if a is None:
+    return cfg, params, utts, rec, [int(u.shape[0] / 2.5) for u in utts]
+
+
+def _keep(T, seq):
+    """Keeps a finished hypothesis by the parity of its length plus its utterance's frame count, so that a
+    validator handed another utterance's inputs decides differently."""
+    return (len(seq) + T) % 2 == 0
+
+
+@pytest.mark.parametrize("stop_on,char_discount", [("patience", 0.0), ("optimistic_future_cost", 0.2)])
+def test_validate_solution_function_matches_oracle(stop_on, char_discount):
+    """The C++ loop calls validate_solution_function where BeamSearch.search does (B/search.py:365-371): with
+    one that rejects some finished hypotheses, every utterance gives the oracle's tokens and costs."""
+    _torch()
+    cfg, params, utts, rec, maxl = _validated_case()
+    ivs = [{"recordings": u[:, None, :]} for u in utts]
+    calls = []
+
+    def validate(inputs, seq):
+        calls.append((inputs, seq))
+        return _keep(inputs["recordings"].shape[0], seq)
+
+    got = rec._beam_search.search_many(utts, cfg["eos_label"], maxl, stop_on=stop_on, char_discount=char_discount,
+                                       raise_on_failure=False, validate_solution_function=validate, input_values=ivs)
+    n_found = 0
+    for u, g in zip(utts, got):
+        try:
+            want = O.beam_search(cfg, params, u, 6, stop_on=stop_on, char_discount=char_discount,
+                                 validate_solution_function=lambda recordings, seq: _keep(recordings.shape[0], seq))
+        except O.CandidateNotFoundError:
+            assert g is None
             continue
-        for x, y in zip(a, b):
-            assert x.shape == y.shape and np.array_equal(x, y)
-        compared += a[0].shape[1]
-    assert compared >= 1
-    # a validate_solution_function routes through the Python loop and filters hypotheses
-    only_short = bs.search_many(utts[:1], cfg["eos_label"], maxl[:1], stop_on=stop_on, char_discount=char_discount,
-                                raise_on_failure=False, validate_solution_function=lambda inputs, seq: len(seq) <= 3)
-    if only_short[0] is not None:
-        assert all(len(o) <= 2 for o in only_short[0][0])
+        assert g is not None
+        n_found += 1
+        assert g[0] == want[0]
+        assert np.allclose(g[1], want[1], rtol=1e-3, atol=5e-3)
+    kept = [_keep(iv["recordings"].shape[0], seq) for iv, seq in calls]
+    print("utterances with a result:", n_found, "validator calls:", len(calls), "kept:", sum(kept))
+    assert n_found >= 1 and any(kept) and not all(kept)
+    for inputs, seq in calls:
+        assert any(inputs is iv for iv in ivs)
+        assert seq.dtype == np.int64 and seq[0] == cfg["num_phonemes"] and seq[-1] == cfg["eos_label"]
+    # BeamSearch.search hands the validator the caller's own input dict
+    u = next(u for u, g in enumerate(got) if g is not None)
+    seen = []
+    iv = {"recordings": utts[u][:, None, :]}
+    rec._beam_search.search(iv, cfg["eos_label"], maxl[u], stop_on=stop_on, char_discount=char_discount,
+                            validate_solution_function=lambda inputs, seq: seen.append(inputs) or True)
+    assert seen and all(inputs is iv for inputs in seen)
+
+
+def test_validate_solution_function_rejecting_or_raising():
+    """A validator that rejects everything leaves no candidate; an exception it raises reaches the caller as
+    itself, and the recognizer searches as before afterwards."""
+    _torch()
+    cfg, params, utts, rec, maxl = _validated_case()
+    bs = rec._beam_search
+    before = bs.search_many(utts, cfg["eos_label"], maxl, raise_on_failure=False, as_arrays=True)
+    assert any(r is not None for r in before)
+    assert bs.search_many(utts, cfg["eos_label"], maxl, raise_on_failure=False,
+                          validate_solution_function=lambda inputs, seq: False) == [None] * len(utts)
+    with pytest.raises(package().CandidateNotFoundError):
+        bs.search_many(utts, cfg["eos_label"], maxl, validate_solution_function=lambda inputs, seq: False)
+
+    def broken(inputs, seq):
+        raise ValueError("validator failed on %d tokens" % len(seq))
+
+    with pytest.raises(ValueError, match="validator failed on"):
+        bs.search_many(utts, cfg["eos_label"], maxl, validate_solution_function=broken)
+    after = bs.search_many(utts, cfg["eos_label"], maxl, raise_on_failure=False, as_arrays=True)
+    for a, b in zip(before, after):
+        assert (a is None) == (b is None)
+        if a is not None:
+            assert all(np.array_equal(x, y) for x, y in zip(a, b))
