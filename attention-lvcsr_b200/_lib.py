@@ -14,6 +14,7 @@ LVSR_MAX_LAYERS = 8
 NORMALIZERS = {"softmax": 0, "logistic": 1, "relu": 2}
 ACTIVATIONS = {"maxout": 0, "relu": 1, "tanh": 2, "identity": 3}
 PRIORS = {"expanding": 0, "window_around_mean": 1, "window_around_median": 2}
+ATTENTION_TYPES = {"content_and_conv": 0, "content": 1}
 
 
 class LvsrConfig(C.Structure):
@@ -42,7 +43,7 @@ class LvsrConfig(C.Structure):
         ("prior_before", C.c_double),
         ("prior_after", C.c_double),
         ("one_of_n_feedback", C.c_int32),
-        ("reserved", C.c_int32),
+        ("attention_type", C.c_int32),
     ]
 
 

@@ -87,7 +87,7 @@ void build_param_table(lvsr_model* m) {
   }
   const int E = m->E, C = c.dim_dec, M = c.dim_matcher, K = c.conv_num_filters, w = 2 * c.conv_n + 1;
   const int V = c.num_phonemes, Cfb = c.dim_feedback, Cpm = c.post_merge_dim;
-  const std::string g = GEN, t = TR, a = ATT;
+  const std::string g = GEN, t = TR, a = att_base(m);
   if (!c.one_of_n_feedback) add_param(m, g + "/readout/lookupfeedback/lookuptable.W", V + 1, Cfb);
   if (c.use_states_for_readout) add_param(m, g + "/readout/merge/transform_states.W", C, Cpm);
   add_param(m, g + "/readout/merge/transform_weighted_averages.W", E, Cpm);
@@ -106,8 +106,10 @@ void build_param_table(lvsr_model* m) {
   add_param(m, a + "/preprocess.W", E, M);
   if (c.energy_normalizer != LVSR_NORM_SOFTMAX) add_param(m, a + "/energy_comp/linear.b", 1);
   add_param(m, a + "/energy_comp/linear.W", M, 1);
-  add_param(m, a + "/handler.W", K, M);
-  add_param(m, a + "/conv1d.filters", K, w);
+  if (!content_attention(m)) {            // SequenceContentAttention has no location term (B/bricks/attention.py:259-414)
+    add_param(m, a + "/handler.W", K, M);
+    add_param(m, a + "/conv1d.filters", K, w);
+  }
   add_param(m, t + "/distribute/fork_inputs.W", E, C);
   add_param(m, t + "/distribute/fork_gate_inputs.W", E, 2 * C);
 }
@@ -134,7 +136,7 @@ int glimpses(lvsr_model* m, const float* H, const float* P, const float* maskH, 
   float* lohi = ws.f32((size_t)2 * R);
   LVSR_CHECK(q && win && lohi, "out of device memory (workspace)");
   DenseArgs d = {};
-  d.X1 = states; d.K1 = c.dim_dec; d.W1 = m->P(std::string(ATT) + "/state_trans/transform_states.W");
+  d.X1 = states; d.K1 = c.dim_dec; d.W1 = m->P(att_base(m) + "/state_trans/transform_states.W");
   d.R = R; d.N = c.dim_matcher; d.mode = DENSE_PLAIN; d.out = q;
   if (int rc = dense_step(d, st)) return rc;
   WindowArgs wa = {};
@@ -145,14 +147,14 @@ int glimpses(lvsr_model* m, const float* H, const float* P, const float* maskH, 
   AttStepArgs a = {};
   a.P = P; a.H = H; a.maskH = maskH; a.row_utt = row_utt; a.q = q; a.w_prev = w_prev; a.win = win; a.lohi = lohi;
   a.row_seg = sg.seg_start ? sg.row_seg : nullptr;
-  a.filt = m->P(std::string(ATT) + "/conv1d.filters");
-  a.Wh = m->P(std::string(ATT) + "/handler.W");
-  a.v = m->P(std::string(ATT) + "/energy_comp/linear.W");
+  a.filt = m->P(att_base(m) + "/conv1d.filters");     // null for content attention
+  a.Wh = m->P(att_base(m) + "/handler.W");
+  a.v = m->P(att_base(m) + "/energy_comp/linear.W");
   a.v_bias = m->v_bias;   // energy bias exists only when the normaliser is not softmax
   a.w_out = w_out; a.e_out = e_out; a.ctx = ctx;
   a.R = R; a.U = U; a.Tp = Tp; a.M = c.dim_matcher; a.E = m->E; a.K = c.conv_num_filters; a.n = c.conv_n;
   a.normalizer = c.energy_normalizer;
-  return attention_step(a, st);
+  return attention_step(a, !content_attention(m), st);
 }
 
 // compute_states for R rows: distribute + fork(feedback) + GRU step.
@@ -229,7 +231,7 @@ size_t cost_ws_bytes(const lvsr_model* m, int Tp, int B, int L) {
 extern "C" {
 
 const char* lvsr_last_error(void) { return g_last_error.c_str(); }
-int lvsr_version(void) { return 101; }
+int lvsr_version(void) { return 102; }
 int64_t lvsr_launch_count(int reset) {
   const int64_t v = g_launch_count;
   if (reset) g_launch_count = 0;
@@ -279,15 +281,31 @@ int lvsr_model_create(const lvsr_config* cfg, lvsr_model** out) {
              "bad post_merge_activation");
   LVSR_CHECK(cfg->post_merge_activation == LVSR_ACT_MAXOUT || cfg->maxout_pieces == 1,
              "maxout_pieces must be 1 unless the activation is Maxout");
-  LVSR_CHECK(cfg->conv_num_filters >= 1 && cfg->conv_num_filters <= 16, "conv_num_filters %d not in [1,16]", cfg->conv_num_filters);
+  LVSR_CHECK(cfg->attention_type == LVSR_ATT_CONTENT_AND_CONV || cfg->attention_type == LVSR_ATT_CONTENT,
+             "attention_type %d unsupported (0: content_and_conv, 1: content)", cfg->attention_type);
+  const bool content = cfg->attention_type == LVSR_ATT_CONTENT;
+  LVSR_CHECK(content || (cfg->conv_num_filters >= 1 && cfg->conv_num_filters <= 16), "conv_num_filters %d not in [1,16]",
+             cfg->conv_num_filters);
   // the centre crop [:, :, n:-n] of the reference is EMPTY for n = 0 (lvsr/bricks/attention.py:109-110)
-  LVSR_CHECK(cfg->conv_n >= 1, "conv_n must be >= 1 (got %d)", cfg->conv_n);
+  LVSR_CHECK(content || cfg->conv_n >= 1, "conv_n must be >= 1 (got %d)", cfg->conv_n);
   LVSR_CHECK(cfg->num_phonemes >= 1 && cfg->num_phonemes <= 128, "num_phonemes out of range");
   int dev_count = 0;
   LVSR_CUDA_OK(cudaGetDeviceCount(&dev_count));
   LVSR_CHECK(dev_count > 0, "no CUDA device: the GPU path has no CPU fallback");
   lvsr_model* m = new lvsr_model();
   m->cfg = *cfg;
+  if (content) {
+    // SequenceContentAttention takes none of these (lvsr/bricks/recognizer.py:261-265): softmax weights over every
+    // frame, which is the expanding window [0, length) that never moves
+    lvsr_config& c = m->cfg;
+    c.conv_n = c.conv_num_filters = 0;
+    c.energy_normalizer = LVSR_NORM_SOFTMAX;
+    c.prior_type = LVSR_PRIOR_EXPANDING;
+    c.prior_initial_begin = 0.0;
+    c.prior_initial_end = 1e30;
+    c.prior_min_speed = c.prior_max_speed = 0.0;
+    c.prior_before = c.prior_after = 0.0;
+  }
   LVSR_CUDA_OK(cudaGetDevice(&m->device));
   m->E = 2 * cfg->dims_bidir[cfg->num_layers - 1];
   build_param_table(m);
@@ -478,7 +496,7 @@ int finalize_on_stream(lvsr_model* m, cudaStream_t st, bool synchronise) {
       dk = 2 * D;
     }
     if (m->Wp_hi)
-      if (int rc = split_weight_tf32(m->P(std::string(ATT) + "/preprocess.W"), m->E, c.dim_matcher, m->Wp_hi, m->Wp_lo, st))
+      if (int rc = split_weight_tf32(m->P(att_base(m) + "/preprocess.W"), m->E, c.dim_matcher, m->Wp_hi, m->Wp_lo, st))
         return rc;
   }
   // fork(feedback(y)) for every symbol y, once: [(V+1), 3C]
@@ -492,7 +510,7 @@ int finalize_on_stream(lvsr_model* m, cudaStream_t st, bool synchronise) {
   }
   m->v_bias = 0.f;
   if (c.energy_normalizer != LVSR_NORM_SOFTMAX)
-    LVSR_CUDA_OK(cudaMemcpy(&m->v_bias, m->P(std::string(ATT) + "/energy_comp/linear.b"), sizeof(float),
+    LVSR_CUDA_OK(cudaMemcpy(&m->v_bias, m->P(att_base(m) + "/energy_comp/linear.b"), sizeof(float),
                             cudaMemcpyDeviceToHost));
   if (synchronise) LVSR_CUDA_OK(cudaStreamSynchronize(st));
   m->finalized = true;
@@ -584,8 +602,8 @@ int lvsr_preprocess(lvsr_model* m, const float* attended, int32_t Tp, int32_t U,
   LVSR_CHECK(attended && out && Tp > 0 && U > 0, "preprocess: bad arguments");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   ArenaScope scope(m, st);
-  return projection_gemm(m->ws, attended, Tp * U, m->E, m->P(std::string(ATT) + "/preprocess.W"), m->use_tc ? m->Wp_hi : nullptr,
-                         m->Wp_lo, m->cfg.dim_matcher, m->P(std::string(ATT) + "/preprocess.b"), out, st);
+  return projection_gemm(m->ws, attended, Tp * U, m->E, m->P(att_base(m) + "/preprocess.W"), m->use_tc ? m->Wp_hi : nullptr,
+                         m->Wp_lo, m->cfg.dim_matcher, m->P(att_base(m) + "/preprocess.b"), out, st);
 }
 
 int lvsr_cost_matrix(lvsr_model* m, const float* attended, const float* attended_mask, int32_t Tp, int32_t B,
@@ -622,14 +640,14 @@ int lvsr_cost_matrix(lvsr_model* m, const float* attended, const float* attended
   if (getenv("LVSR_NO_DEC_SCAN") == nullptr && !m->force_stepwise) {
     DecScanArgs d = {};
     d.P = P; d.H = attended; d.maskH = attended_mask;
-    d.filt = m->P(std::string(ATT) + "/conv1d.filters");
-    d.Wh = m->P(std::string(ATT) + "/handler.W");
-    d.v = m->P(std::string(ATT) + "/energy_comp/linear.W");
+    d.filt = m->P(att_base(m) + "/conv1d.filters");     // null for content attention
+    d.Wh = m->P(att_base(m) + "/handler.W");
+    d.v = m->P(att_base(m) + "/energy_comp/linear.W");
     d.v_bias = m->v_bias;
     d.prior = prior_of(c);
     d.Wb1 = m->Wb1;
     d.Wstate = m->P(std::string(TR) + "/transition.state_to_state");
-    d.Ws = m->P(std::string(ATT) + "/state_trans/transform_states.W");
+    d.Ws = m->P(att_base(m) + "/state_trans/transform_states.W");
     d.FF = m->FF;
     d.labels = lab; d.lmask = labels_mask;
     d.s_all = s_all; d.ctx_all = ctx_all; d.w0 = w0;
@@ -659,7 +677,7 @@ int lvsr_cost_matrix(lvsr_model* m, const float* attended, const float* attended
       LVSR_CUDA_OK(cudaMemsetAsync(d.trace, 0, ((size_t)2 * L * 9 + (size_t)L * 12 + (size_t)L * B) * 8, st));
     }
     int supported = 0;
-    if (int rc = dec_scan_try(d, &supported, st)) return rc;
+    if (int rc = dec_scan_try(d, !content_attention(m), &supported, st)) return rc;
     scanned = supported != 0;
     if (scanned && getenv("LVSR_DEC_CHECK") != nullptr) {
       // debug post-condition: the launch reported success and every hand-over word was written
@@ -780,8 +798,13 @@ int lvsr_initial_states(lvsr_model* m, int32_t Tp, int32_t R, float* states, int
   if (int rc = broadcast_rows(states, m->P(std::string(TR) + "/transition.initial_state"), R, c.dim_dec, st)) return rc;
   if (int rc = fill_i64(reinterpret_cast<long long*>(outputs), R, c.num_phonemes, st)) return rc;   // recognizer.py:286
   if (int rc = fill_f32(wavg, (long long)R * m->E, 0.f, st)) return rc;
-  if (int rc = onehot_rows(weights, R, Tp, st)) return rc;
-  if (int rc = onehot_rows(energies, R, Tp, st)) return rc;
+  if (content_attention(m)) {             // B/bricks/attention.py:392-395: zero weights; no energies state
+    if (int rc = fill_f32(weights, (long long)R * Tp, 0.f, st)) return rc;
+    if (int rc = fill_f32(energies, (long long)R * Tp, 0.f, st)) return rc;
+  } else {
+    if (int rc = onehot_rows(weights, R, Tp, st)) return rc;
+    if (int rc = onehot_rows(energies, R, Tp, st)) return rc;
+  }
   return fill_i64(reinterpret_cast<long long*>(step), R, 0, st);
 }
 

@@ -102,7 +102,8 @@ __global__ void __launch_bounds__(256) window_kernel(WindowArgs a) {
 // ---------------------------------------------------------------------------------
 // attention step kernel: one cluster of `cs` CTAs per decoder row
 // ---------------------------------------------------------------------------------
-__global__ void __launch_bounds__(ATT_THREADS, 1) att_step_kernel(AttStepArgs a, int tc_cap) {
+template <bool LOC>
+__device__ __forceinline__ void att_step_row(const AttStepArgs& a, int tc_cap) {
   extern __shared__ __align__(16) float smem[];
   cg::cluster_group cluster = cg::this_cluster();
   const int cs = (int)cluster.num_blocks();
@@ -124,20 +125,29 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) att_step_kernel(AttStepArgs a,
   const int sg = a.row_seg ? a.row_seg[row] : 0;
   io.b0 = a.win[2 * sg]; io.b1 = a.win[2 * sg + 1];
   io.lo = a.lohi[2 * row]; io.hi = a.lohi[2 * row + 1];
-  attention_row(io, smem, tc_cap, rank, cs, false, false, true);
+  attention_row<false, LOC>(io, smem, tc_cap, rank, cs, false, false, true);
+}
+
+__global__ void __launch_bounds__(ATT_THREADS, 1) att_step_kernel(AttStepArgs a, int tc_cap) { att_step_row<true>(a, tc_cap); }
+
+// content-only attention (SequenceContentAttention.take_glimpses, B/bricks/attention.py:370-388)
+__global__ void __launch_bounds__(ATT_THREADS, 1) att_content_step_kernel(AttStepArgs a, int tc_cap) {
+  att_step_row<false>(a, tc_cap);
 }
 
 int num_sms() { return device_sm_count(); }
 
-int launch_att(const AttStepArgs& a, int cs, cudaStream_t stream) {
+int launch_att(const AttStepArgs& a, bool loc, int cs, cudaStream_t stream) {
   const int tc_cap = ceil_div(a.Tp, cs);
-  const size_t smem = att_smem_floats(a.M, a.E, a.K, a.n, tc_cap, cs) * sizeof(float);
+  const size_t smem = (loc ? att_smem_floats(a.M, a.E, a.K, a.n, tc_cap, cs) : att_smem_floats<false>(a.M, a.E, 0, 0, tc_cap, cs)) *
+                      sizeof(float);
   LVSR_CHECK(smem <= 227 * 1024, "attention_step: shared memory %zu B exceeds 227 KB (Tp=%d, cs=%d)", smem, a.Tp, cs);
-  static size_t configured[LVSR_MAX_DEVICES] = {0};
+  static size_t configured[2][LVSR_MAX_DEVICES] = {{0}};
   const int dev = current_device();
-  if (smem > configured[dev]) {
-    LVSR_CUDA_OK(cudaFuncSetAttribute(att_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    configured[dev] = smem;
+  void (*kernel)(AttStepArgs, int) = loc ? att_step_kernel : att_content_step_kernel;
+  if (smem > configured[loc][dev]) {
+    LVSR_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    configured[loc][dev] = smem;
   }
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(a.R * cs);
@@ -151,7 +161,7 @@ int launch_att(const AttStepArgs& a, int cs, cudaStream_t stream) {
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  LVSR_CUDA_OK(cudaLaunchKernelEx(&cfg, att_step_kernel, a, tc_cap));
+  LVSR_CUDA_OK(cudaLaunchKernelEx(&cfg, kernel, a, tc_cap));
   g_launch_count++;
   return 0;
 }
@@ -165,18 +175,18 @@ int attention_window(const WindowArgs& a, cudaStream_t stream) {
   return 0;
 }
 
-int attention_step(const AttStepArgs& a, cudaStream_t stream) {
+int attention_step(const AttStepArgs& a, bool location, cudaStream_t stream) {
   ProfScope prof("attention", stream);
   LVSR_CHECK(a.M == 128 || a.M == 256 || a.M == 512, "attention_step: dim_matcher %d unsupported (128, 256 or 512)", a.M);
   LVSR_CHECK(a.E % 4 == 0 && a.E <= 4 * ATT_NT, "attention_step: encoded dim must be a multiple of 4 and <= %d", 4 * ATT_NT);
   LVSR_CHECK(a.E / 4 <= ATT_THREADS, "attention_step: encoded dim %d > 1024 unsupported", a.E);
-  LVSR_CHECK(a.K >= 1 && a.K <= 16, "attention_step: conv_num_filters %d not in [1,16]", a.K);
+  LVSR_CHECK(!location || (a.K >= 1 && a.K <= 16), "attention_step: conv_num_filters %d not in [1,16]", a.K);
   if (a.R <= 0) return 0;
   // cluster size: split a row's window over as many CTAs as keeps R*cs within one wave
   int cs = 1;
   const int sms = num_sms();
   while (cs < 8 && a.R * cs * 2 <= sms && ceil_div(a.Tp, cs * 2) >= 16) cs *= 2;
-  return launch_att(a, cs, stream);
+  return launch_att(a, location, cs, stream);
 }
 
 }  // namespace lvsr

@@ -39,14 +39,19 @@ __host__ __device__ inline size_t att_red_floats(int E, int tc_cap) {
 // Shared-memory footprint (floats) of attention_row for a chunk capacity of tc_cap positions.
 // wh_rows: rows of the handler copy in shared memory: 16 (zero-padded to the MMA depth, unpredicated fragment loads: the
 // fast default) or K (compact; the planner falls back to it when the padded copy does not fit, e.g. 16 rows x T' = 2000)
+// LOC = false (content-only attention): no handler, filters, previous alignment or location features; K, n and wh_rows
+// are ignored.
+template <bool LOC = true>
 __host__ __device__ inline size_t att_smem_floats(int M, int E, int K, int n, int tc_cap, int cs, int wh_rows = 16) {
   size_t f = 0;
   f += M;                                         // sq
   f += M;                                         // sv
-  f += (size_t)wh_rows * M;                       // sWh (rows >= K are zero, or supplied by predicates in the compact layout)
-  f += (size_t)(2 * n + 1) * att_filter_row(K);   // sfiltT [tap][filter]
-  f += tc_cap + 2 * n + 8;                        // salpha
-  f += (size_t)(tc_cap + 16) * 16;                // sF: packed bf16 pairs, 8 hi + 8 lo words per position
+  if (LOC) {
+    f += (size_t)wh_rows * M;                     // sWh (rows >= K are zero, or supplied by predicates in the compact layout)
+    f += (size_t)(2 * n + 1) * att_filter_row(K); // sfiltT [tap][filter]
+    f += tc_cap + 2 * n + 8;                      // salpha
+    f += (size_t)(tc_cap + 16) * 16;              // sF: packed bf16 pairs, 8 hi + 8 lo words per position
+  }
   f += tc_cap + 16;                               // se
   f += tc_cap + 16;                               // su
   f += 96;                                        // block reduction scratch
@@ -112,17 +117,23 @@ struct AttSmem {
   uint32_t* sF;          // [(tc_cap+16)][16]: words 0..7 = hi pairs, 8..15 = lo pairs
 };
 
+template <bool LOC = true>
 __device__ __forceinline__ AttSmem att_carve(float* smem, int M, int E, int K, int n, int tc_cap, int cs, int wh_rows = 16) {
   AttSmem s;
   float* p = smem;
   s.sq = p; p += M;
   s.sv = p; p += M;
-  s.sWh = p; p += (size_t)wh_rows * M;
-  s.sfiltT = p; p += (size_t)(2 * n + 1) * att_filter_row(K);
-  p += (4 - ((p - smem) & 3)) & 3;
-  s.salpha = p; p += tc_cap + 2 * n + 8;
-  p += (4 - ((p - smem) & 3)) & 3;
-  s.sF = reinterpret_cast<uint32_t*>(p); p += (size_t)(tc_cap + 16) * 16;
+  if constexpr (LOC) {
+    s.sWh = p; p += (size_t)wh_rows * M;
+    s.sfiltT = p; p += (size_t)(2 * n + 1) * att_filter_row(K);
+    p += (4 - ((p - smem) & 3)) & 3;
+    s.salpha = p; p += tc_cap + 2 * n + 8;
+    p += (4 - ((p - smem) & 3)) & 3;
+    s.sF = reinterpret_cast<uint32_t*>(p); p += (size_t)(tc_cap + 16) * 16;
+  } else {
+    s.sWh = s.sfiltT = s.salpha = nullptr;
+    s.sF = nullptr;
+  }
   s.se = p; p += tc_cap + 16;
   s.su = p; p += tc_cap + 16;
   s.sblk = p; p += 96;
@@ -134,11 +145,13 @@ __device__ __forceinline__ AttSmem att_carve(float* smem, int M, int E, int K, i
 }
 
 // Constants that never change during a sequence: energy vector, handler (zero-padded to 16
-// rows), transposed + zero-padded filter bank.  Persistent callers stage them once.
+// rows), transposed + zero-padded filter bank (LOC = false: the energy vector only).  Persistent callers stage them once.
+template <bool LOC = true>
 __device__ __forceinline__ void att_stage_constants(const AttSmem& s, const float* v, const float* Wh,
                                                     const float* filt, int M, int K, int n, int wh_rows = 16) {
   const int tid = threadIdx.x, w = 2 * n + 1, fw = att_filter_row(K);
   for (int i = tid; i < M; i += ATT_NT) s.sv[i] = v[i];
+  if constexpr (!LOC) return;
   for (int i = tid; i < wh_rows * M; i += ATT_NT) s.sWh[i] = (i / M < K) ? Wh[i] : 0.f;
   for (int i = tid; i < w * fw; i += ATT_NT) {
     const int j = i / fw, k = i % fw;
@@ -159,8 +172,9 @@ __device__ __forceinline__ void mma_bf16_16816(float (&d)[4], const uint32_t (&a
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
-// NTW: 8-column tiles of the matcher dimension per warp (M = 128 * NTW).
-template <int NTW, bool COMPACT>
+// NTW: 8-column tiles of the matcher dimension per warp (M = 128 * NTW).  LOC = false (content-only attention):
+// e[t] = v . tanh(P[t] + q) on the FP32 pipes, same accumulator layout without the handler product.
+template <int NTW, bool COMPACT, bool LOC = true>
 __device__ __forceinline__ void att_energies(const AttRowIO& a, const AttSmem& s, int nt, int t0, int tc_cap) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int g = lane >> 2, tig = lane & 3;
@@ -172,6 +186,7 @@ __device__ __forceinline__ void att_energies(const AttRowIO& a, const AttSmem& s
   for (int j = 0; j < NTW; ++j) {
     const int n0 = (warp * NTW + j) * 8;
     const int colb = n0 + g;                       // B fragment column
+    if constexpr (LOC) {
     // B fragment rows 2tig, 2tig+1, 2tig+8, 2tig+9 of the 16-deep product; only K rows exist (K <= 16)
     auto wh = [&](int row) -> float { return (!COMPACT || row < a.K) ? s.sWh[(size_t)row * M + colb] : 0.f; };
     const float w00 = wh(2 * tig), w01 = wh(2 * tig + 1), w10 = wh(2 * tig + 8), w11 = wh(2 * tig + 9);
@@ -180,6 +195,7 @@ __device__ __forceinline__ void att_energies(const AttRowIO& a, const AttSmem& s
     bh[j][1] = pack_bf16(h10, h11);
     bl[j][0] = pack_bf16(w00 - h00, w01 - h01);
     bl[j][1] = pack_bf16(w10 - h10, w11 - h11);
+    }
     const int colc = n0 + 2 * tig;                 // accumulator columns
     vv[j][0] = s.sv[colc]; vv[j][1] = s.sv[colc + 1];
     qq[j][0] = s.sq[colc]; qq[j][1] = s.sq[colc + 1];
@@ -202,10 +218,12 @@ __device__ __forceinline__ void att_energies(const AttRowIO& a, const AttSmem& s
     if (tile + 1 < ntile) load_p(pn, tile + 1);
     const int ta = tile * 16 + g, tb = ta + 8;
     uint32_t ah[4], al[4];
+    if constexpr (LOC) {
     ah[0] = s.sF[(size_t)ta * 16 + tig];     ah[1] = s.sF[(size_t)tb * 16 + tig];
     ah[2] = s.sF[(size_t)ta * 16 + tig + 4]; ah[3] = s.sF[(size_t)tb * 16 + tig + 4];
     al[0] = s.sF[(size_t)ta * 16 + 8 + tig];     al[1] = s.sF[(size_t)tb * 16 + 8 + tig];
     al[2] = s.sF[(size_t)ta * 16 + 8 + tig + 4]; al[3] = s.sF[(size_t)tb * 16 + 8 + tig + 4];
+    }
     float ea = 0.f, eb = 0.f;
 #pragma unroll
     for (int j = 0; j < NTW; ++j) {
@@ -214,9 +232,11 @@ __device__ __forceinline__ void att_energies(const AttRowIO& a, const AttSmem& s
       d[2] = pc[j][1].x + qq[j][0]; d[3] = pc[j][1].y + qq[j][1];
       DBG_NAN(4, pc[j][0].x + pc[j][0].y + pc[j][1].x + pc[j][1].y, tile * 16 + g);
       DBG_NAN(5, qq[j][0] + qq[j][1], j);
-      mma_bf16_16816(d, al, bh[j][0], bh[j][1]);     // small terms first
-      mma_bf16_16816(d, ah, bl[j][0], bl[j][1]);
-      mma_bf16_16816(d, ah, bh[j][0], bh[j][1]);
+      if constexpr (LOC) {
+        mma_bf16_16816(d, al, bh[j][0], bh[j][1]);   // small terms first
+        mma_bf16_16816(d, ah, bl[j][0], bl[j][1]);
+        mma_bf16_16816(d, ah, bh[j][0], bh[j][1]);
+      }
       DBG_NAN(6, d[0] + d[1] + d[2] + d[3], tile * 16 + g);
       ea = fmaf(vv[j][0], fast_tanh(d[0]), ea);
       ea = fmaf(vv[j][1], fast_tanh(d[1]), ea);
@@ -246,7 +266,9 @@ __device__ __forceinline__ float gmax_of(const float* xs, int cs) {
 // sentinel-initialised buffers (common.cuh, "the data is the flag"): they are read with polling
 // loads and the outputs other CTAs consume are written with gpu-scope stores.
 // `entry_wait_pending`: the caller issued barrier.cluster.arrive at kernel entry.
-template <bool COMPACT = false>
+// LOC = false: content-only attention (B/bricks/attention.py:259-414): no previous alignment, conv or handler, so in
+// flow mode only the query is waited for; e_out receives zeros (the reference keeps no energies for it).
+template <bool COMPACT = false, bool LOC = true>
 __device__ __forceinline__ void attention_row(const AttRowIO& a, float* smem, int tc_cap, int rank, int cs,
                                               bool constants_staged, bool flow,
                                               bool entry_wait_pending) {
@@ -254,7 +276,7 @@ __device__ __forceinline__ void attention_row(const AttRowIO& a, float* smem, in
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   constexpr int NT = ATT_NT, NW = ATT_NW;
   const int M = a.M, E = a.E, K = a.K, n = a.n, w = 2 * n + 1, Tp = a.Tp, U = a.U, u = a.u;
-  const AttSmem s = att_carve(smem, M, E, K, n, tc_cap, cs, a.wh_rows);
+  const AttSmem s = att_carve<LOC>(smem, M, E, K, n, tc_cap, cs, a.wh_rows);
 
   const int b0 = a.b0;
   const int Tw = max(0, a.b1 - a.b0);
@@ -264,8 +286,8 @@ __device__ __forceinline__ void attention_row(const AttRowIO& a, float* smem, in
 
   ATT_STAMP(0);
   // ---- stage the row's query, the slice of the previous alignment, zero the energies ----
-  if (!constants_staged) att_stage_constants(s, a.v, a.Wh, a.filt, M, K, n, a.wh_rows);
-  {
+  if (!constants_staged) att_stage_constants<LOC>(s, a.v, a.Wh, a.filt, M, K, n, a.wh_rows);
+  if constexpr (LOC) {
     const int len = nt + 2 * n + 8;
     for (int i = tid; i < len; i += NT) {
       const int prel = t0 - n + i;            // window-relative position; zero padding is
@@ -287,7 +309,7 @@ __device__ __forceinline__ void attention_row(const AttRowIO& a, float* smem, in
 
   // ---- location features F[t][k] = sum_j alpha_cut[t + 2n - j] * filt[k][j], written as the
   //      bf16 hi/lo A-fragments of the handler product ----------------------------------
-  {
+  if constexpr (LOC) {
     const int fw = att_filter_row(K);
     const int qtr = lane >> 3;                         // tap quarter 0..3
     const int seg = (w + 3) / 4;
@@ -353,9 +375,9 @@ __device__ __forceinline__ void attention_row(const AttRowIO& a, float* smem, in
   ATT_STAMP(2);
 
   // ---- energies: e[t] = v . tanh(P[t] + q + F[t] . Wh) on the tensor cores -------------
-  if (M == 512) att_energies<4, COMPACT>(a, s, nt, t0, tc_cap);
-  else if (M == 256) att_energies<2, COMPACT>(a, s, nt, t0, tc_cap);
-  else att_energies<1, COMPACT>(a, s, nt, t0, tc_cap);
+  if (M == 512) att_energies<4, COMPACT, LOC>(a, s, nt, t0, tc_cap);
+  else if (M == 256) att_energies<2, COMPACT, LOC>(a, s, nt, t0, tc_cap);
+  else att_energies<1, COMPACT, LOC>(a, s, nt, t0, tc_cap);
   __syncthreads();
   {
     // e[t] = the 16 warps' partial sums, added in a fixed order
@@ -543,7 +565,7 @@ __device__ __forceinline__ void attention_row(const AttRowIO& a, float* smem, in
   for (int t = tid; t < nt; t += NT) {
     const float wv = s.su[t] * myscale * inv;
     if (flow) st_flow_f32(a.w_out + b0 + t0 + t, wv); else a.w_out[b0 + t0 + t] = wv;
-    a.e_out[b0 + t0 + t] = s.se[t];
+    a.e_out[b0 + t0 + t] = LOC ? s.se[t] : 0.f;
   }
   // zero outside the window (paste into zeros, attention.py:177-181); ranks interleave the work
   for (int pidx = rank * NT + tid; pidx < Tp; pidx += cs * NT) {

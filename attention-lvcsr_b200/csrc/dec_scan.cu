@@ -204,9 +204,10 @@ __device__ __forceinline__ void dense_dispatch(int nq, const DenseIO& d, const f
 }
 
 // COMPACT: the handler copy in shared memory holds only its K rows (a.wh_rows == K); a separate instantiation so that
-// the default kernel's energy loop stays exactly the unpredicated code (it is sensitive to every extra register)
-template <bool COMPACT>
-__global__ void __launch_bounds__(DS_THREADS, 1) dec_scan_kernel(DecScanArgs a) {
+// the default kernel's energy loop stays exactly the unpredicated code (it is sensitive to every extra register).
+// LOC = false: content-only attention (no previous alignment, conv or handler; see attention_row).
+template <bool COMPACT, bool LOC>
+__device__ __forceinline__ void dec_scan_body(const DecScanArgs& a) {
   extern __shared__ __align__(16) float smem[];
   cg::cluster_group cluster = cg::this_cluster();
   const int cs = (int)cluster.num_blocks();
@@ -253,7 +254,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) dec_scan_kernel(DecScanArgs a) 
 
   // ---- shared memory: [attention region][w1][w2][w3][red] -----------------------------
   float* att = smem;
-  size_t off = att_smem_floats(M, E, a.K, a.n, a.tc_cap, cs, a.wh_rows);
+  size_t off = att_smem_floats<LOC>(M, E, a.K, a.n, a.tc_cap, cs, a.wh_rows);
   off = (off + 3) & ~(size_t)3;
   const int ws1 = a.nc1 + 4, ws2 = a.nc2 + 4, ws3 = a.nc3 + 4;
   float* w1s = smem + off; off += (size_t)(E + C) * ws1;
@@ -263,7 +264,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) dec_scan_kernel(DecScanArgs a) 
   off = (off + 3) & ~(size_t)3;
   // the cross-warp scratch of the dense tiles may live in the attention phase's reduction scratch: a CTA runs its
   // phases one after the other (CTA barriers in between), so the two never hold live data at the same time
-  float* red = a.red_alias ? att_carve(att, M, E, a.K, a.n, a.tc_cap, cs, a.wh_rows).sred : smem + off;
+  float* red = a.red_alias ? att_carve<LOC>(att, M, E, a.K, a.n, a.tc_cap, cs, a.wh_rows).sred : smem + off;
 
   // ---- one-time staging: weight slices + attention constants -----------------------------
   for (int i = tid; i < (E + C) * a.nc1; i += DS_THREADS) {
@@ -282,7 +283,8 @@ __global__ void __launch_bounds__(DS_THREADS, 1) dec_scan_kernel(DecScanArgs a) 
     const int k = i / a.nc3, c = i % a.nc3, col = cgi * a.nc3 + c;
     w3s[(size_t)k * ws3 + c] = (in3 && col < M) ? a.Ws[(long long)k * M + col] : 0.f;
   }
-  att_stage_constants(att_carve(att, M, E, a.K, a.n, a.tc_cap, cs, a.wh_rows), a.v, a.Wh, a.filt, M, a.K, a.n, a.wh_rows);
+  att_stage_constants<LOC>(att_carve<LOC>(att, M, E, a.K, a.n, a.tc_cap, cs, a.wh_rows), a.v, a.Wh, a.filt, M, a.K, a.n,
+                           a.wh_rows);
   __syncthreads();
 
   // query of the first step: q = s_0 . W_state
@@ -334,7 +336,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) dec_scan_kernel(DecScanArgs a) 
         b1 = (int)ceil(ee);
       } else {
         // the batch-global cut needs the position statistic of EVERY row of the previous step
-        float* wsh = att + att_smem_floats(M, E, a.K, a.n, a.tc_cap, cs, a.wh_rows) - 8;   // spare floats at the tail
+        float* wsh = att + att_smem_floats<LOC>(M, E, a.K, a.n, a.tc_cap, cs, a.wh_rows) - 8;   // spare floats at the tail
         if (warp == 0) {
           float mn = 1e30f, mx = -1e30f;
           for (int r = lane; r < R; r += 32) {
@@ -372,7 +374,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) dec_scan_kernel(DecScanArgs a) 
       io.rowpos_out = (a.prior.type == LVSR_PRIOR_EXPANDING) ? nullptr : (rowpos_wr + row);
       io.rowpos_mode = a.prior.type;
       io.trace = (a.trace && bid == 0) ? a.trace + (size_t)2 * a.L * 9 + (size_t)i * 8 : nullptr;
-      attention_row<COMPACT>(io, att, a.tc_cap, rank, cs, true, true, false);
+      attention_row<COMPACT, LOC>(io, att, a.tc_cap, rank, cs, true, true, false);
     }
     DS_STAMP(1);
     if (a.trace && rank == 0 && tid == 0 && cluster_id < R)
@@ -417,6 +419,14 @@ __global__ void __launch_bounds__(DS_THREADS, 1) dec_scan_kernel(DecScanArgs a) 
   cluster.sync();   // no CTA exits while a peer may still address its shared memory
 }
 
+template <bool COMPACT>
+__global__ void __launch_bounds__(DS_THREADS, 1) dec_scan_kernel(DecScanArgs a) { dec_scan_body<COMPACT, true>(a); }
+
+// content-only attention: the persistent decoder hands over only the query between the dense phases and the attention
+__global__ void __launch_bounds__(DS_THREADS, 1) dec_content_kernel(DecScanArgs a) { dec_scan_body<false, false>(a); }
+
+using DecKernel = void (*)(DecScanArgs);
+
 int sm_count() { return device_sm_count(); }
 
 int round_up8(int x) { return (x + 7) & ~7; }
@@ -427,7 +437,7 @@ bool kper_ok(int ktot) {
 
 // Fill the derived fields for a grid of G CTAs; returns the dynamic shared memory in bytes (0 = unsupported).
 // want_islands: cut the batch into independent islands of <= 16 rows (grid = R*cs exactly).
-size_t derive(DecScanArgs& a, int cs, int G, bool want_islands) {
+size_t derive(DecScanArgs& a, int cs, int G, bool want_islands, bool loc) {
   const int R = a.B, C = a.C, E = a.E, M = a.M;
   a.cs = cs;
   a.tc_cap = ceil_div(a.Tp, cs);
@@ -450,7 +460,7 @@ size_t derive(DecScanArgs& a, int cs, int G, bool want_islands) {
   // handler copy: zero-padded to 16 rows (fast path) if it fits, else only its K rows (long utterances)
   for (int rows : {16, a.K}) {
     a.wh_rows = rows;
-    size_t f = att_smem_floats(M, E, a.K, a.n, a.tc_cap, cs, a.wh_rows);
+    size_t f = loc ? att_smem_floats(M, E, a.K, a.n, a.tc_cap, cs, a.wh_rows) : att_smem_floats<false>(M, E, 0, 0, a.tc_cap, cs);
     f = (f + 3) & ~(size_t)3;
     f += (size_t)(E + C) * (a.nc1 + 4) + (size_t)C * (a.nc2 + 4) + (size_t)C * (a.nc3 + 4);
     f = (f + 3) & ~(size_t)3;
@@ -462,25 +472,26 @@ size_t derive(DecScanArgs& a, int cs, int G, bool want_islands) {
   return 0;
 }
 
-int plan_and_launch(DecScanArgs& a, int* supported, cudaStream_t stream) {
+int plan_and_launch(DecScanArgs& a, bool loc, int* supported, cudaStream_t stream) {
   *supported = 0;
   const int sms = sm_count();
   const int R = a.B, C = a.C, E = a.E, M = a.M;
   if (!kper_ok(E + C) || !kper_ok(C) || !(M == 128 || M == 256 || M == 512) || E % 4 != 0 || E / 4 > DS_THREADS) return 0;
-  if (a.K < 1 || a.K > 16 || R < 1) return 0;
+  if ((loc && (a.K < 1 || a.K > 16)) || R < 1) return 0;
   int cs = 1;
   while (cs < 8 && R * cs * 2 <= sms && ceil_div(a.Tp, cs * 2) >= 16) cs *= 2;
   LVSR_CUDA_OK(cudaFuncSetAttribute(dec_scan_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
   LVSR_CUDA_OK(cudaFuncSetAttribute(dec_scan_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+  if (!loc) LVSR_CUDA_OK(cudaFuncSetAttribute(dec_content_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
   for (; cs >= 1; cs >>= 1) {
     // prefer islands (grid = one cluster per row); fall back to one global island on all SMs
     bool islands = R >= DS_ROWS;
     int G = islands ? R * cs : (sms / cs) * cs;
-    size_t smem = derive(a, cs, G, islands);
+    size_t smem = derive(a, cs, G, islands, loc);
     if (smem == 0 && islands) {
       islands = false;
       G = (sms / cs) * cs;
-      smem = derive(a, cs, G, false);
+      smem = derive(a, cs, G, false, loc);
     }
     if (smem == 0) continue;
     // every cluster must be co-resident (consumers poll producers): ask the driver how many fit.  GPCs of
@@ -501,9 +512,8 @@ int plan_and_launch(DecScanArgs& a, int* supported, cudaStream_t stream) {
     cfg.attrs = attr;
     cfg.numAttrs = 1;
     int max_clusters = 0;
-    const bool compact = a.wh_rows != 16;
-    if ((compact ? cudaOccupancyMaxActiveClusters(&max_clusters, dec_scan_kernel<true>, &cfg)
-                 : cudaOccupancyMaxActiveClusters(&max_clusters, dec_scan_kernel<false>, &cfg)) != cudaSuccess) {
+    const DecKernel kernel = !loc ? dec_content_kernel : a.wh_rows != 16 ? dec_scan_kernel<true> : dec_scan_kernel<false>;
+    if (cudaOccupancyMaxActiveClusters(&max_clusters, kernel, &cfg) != cudaSuccess) {
       cudaGetLastError();
       continue;
     }
@@ -511,7 +521,7 @@ int plan_and_launch(DecScanArgs& a, int* supported, cudaStream_t stream) {
       if (islands) continue;          // islands need exactly one cluster per row
       G = max_clusters * cs;
       if (G < cs) continue;
-      smem = derive(a, cs, G, false);
+      smem = derive(a, cs, G, false, loc);
       if (smem == 0) continue;
       cfg.gridDim = dim3(G);
       cfg.dynamicSmemBytes = smem;
@@ -524,8 +534,7 @@ int plan_and_launch(DecScanArgs& a, int* supported, cudaStream_t stream) {
       LVSR_CUDA_OK(cudaMemcpyToSymbolAsync(g_flow_spin_limit, &lim, sizeof(lim), 0, cudaMemcpyHostToDevice, stream));
       LVSR_CUDA_OK(cudaMemcpyToSymbolAsync(g_flow_status, &a.status, sizeof(a.status), 0, cudaMemcpyHostToDevice, stream));
     }
-    cudaError_t e = (a.wh_rows != 16) ? cudaLaunchKernelEx(&cfg, dec_scan_kernel<true>, a)
-                                      : cudaLaunchKernelEx(&cfg, dec_scan_kernel<false>, a);
+    cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, a);
     if (e != cudaSuccess) {
       cudaGetLastError();
       continue;
@@ -555,9 +564,9 @@ int plan_and_launch(DecScanArgs& a, int* supported, cudaStream_t stream) {
 
 // Runs the persistent decoder if the shapes fit (*supported = 1); otherwise leaves everything
 // untouched (*supported = 0) and the caller falls back to the per-step kernels.
-int dec_scan_try(DecScanArgs& a, int* supported, cudaStream_t stream) {
+int dec_scan_try(DecScanArgs& a, bool location, int* supported, cudaStream_t stream) {
   ProfScope prof("dec_scan", stream);
-  return plan_and_launch(a, supported, stream);
+  return plan_and_launch(a, location, supported, stream);
 }
 
 }  // namespace lvsr

@@ -146,6 +146,11 @@ namespace lvsr {
 static const char* const GEN = "/recognizer/generator";
 static const char* const TR = "/recognizer/generator/att_trans";
 static const char* const ATT = "/recognizer/generator/att_trans/conv_att";
+static const char* const CONT = "/recognizer/generator/att_trans/cont_att";
+
+static inline bool content_attention(const lvsr_model* m) { return m->cfg.attention_type == LVSR_ATT_CONTENT; }
+// brick path of the attention's parameters
+static inline std::string att_base(const lvsr_model* m) { return content_attention(m) ? CONT : ATT; }
 
 static inline std::string enc_base(int l, int dir) {
   char buf[128];
@@ -232,8 +237,9 @@ int search_expand(lvsr_model* m, const float* attended, const float* preprocesse
                   int k, float* wavg, float* new_weights, float* new_energies, int* top_parent, int* top_symbol,
                   float* top_cost, int* top_count, cudaStream_t st);
 // search_advance = next_state_computer (B/search.py:119-142) for the Rn selected children (parent rows + symbols):
-// gathers the parents' state and, under the expanding prior, their glimpses from search_expand (exact there because
-// the window does not depend on which rows are in the batch); under the window_around_* priors it recomputes
+// gathers the parents' state and, under the expanding prior and for content attention, their glimpses from
+// search_expand (exact there because the window does not depend on which rows are in the batch); under the
+// window_around_* priors it recomputes
 // take_glimpses over the selected rows as the reference does.  Then Distribute + GRU step; step + 1.
 int search_advance(lvsr_model* m, const float* attended, const float* preprocessed, const float* attended_mask, int Tp,
                    int U, const int* utt_len, int Rn, const int* parent, const long long* symbols, const int* row_utt,

@@ -160,8 +160,9 @@ int lvsr_train_cost_and_grads(lvsr_model* m, const float* x, const float* mask, 
   // shapes the backward kernels cannot take are refused before any work is enqueued
   const size_t ro_smem = (size_t)8 * (Hd + 128) * sizeof(float);
   LVSR_CHECK(ro_smem <= 48 * 1024 && V <= 128, "readout backward: post_merge_dim / num_phonemes too large");
+  const bool content = content_attention(m);
   const int tc_cap = ceil_div(Tp, AB_CS);
-  const size_t ab_smem = att_bwd_smem_floats(M, E, K, n, tc_cap) * sizeof(float);
+  const size_t ab_smem = (content ? att_bwd_content_smem_floats(E, tc_cap) : att_bwd_smem_floats(M, E, K, n, tc_cap)) * sizeof(float);
   LVSR_CHECK(ab_smem <= 227 * 1024 && M <= AB_NT && M % 128 == 0 && K <= 16 && E % 4 == 0,
              "attention backward: shape unsupported (Tp=%d M=%d)", Tp, M);
   LVSR_CHECK(E <= 1024, "encoded dim %d > 1024 unsupported in training", E);
@@ -201,7 +202,7 @@ int lvsr_train_cost_and_grads(lvsr_model* m, const float* x, const float* mask, 
   LVSR_LAUNCH_CHECK();
 
   // =========================== backward ===========================
-  const std::string g = GEN, t = TR, at = ATT;
+  const std::string g = GEN, t = TR, at = att_base(m);
   // ---- transposed weights used as right-hand sides of dY . W^T -------------------------------
   float* WoT_unused = nullptr; (void)WoT_unused;
   float* WmsT = c.use_states_for_readout ? ws.f32((size_t)Cpm * C) : nullptr;     // [Cpm, C]
@@ -286,7 +287,7 @@ int lvsr_train_cost_and_grads(lvsr_model* m, const float* x, const float* mask, 
   int* win = ws.i32(2);
   float* lohi = ws.f32((size_t)2 * B);
   LVSR_CHECK(G && Z && Rg && HR && Cc && Q && P && dP && dG && dCTX && dQp && dsbuf[0] && dsbuf[1] && keep && dHR && dspart &&
-                 dAbuf[0] && dAbuf[1] && w0 && acc_v && acc_Wh && acc_filt && win && lohi,
+                 dAbuf[0] && dAbuf[1] && w0 && acc_v && (content || (acc_Wh && acc_filt)) && win && lohi,
              "out of device memory (decoder backward)");
   if (int rc = lvsr_preprocess(m, Hatt, Tp, B, P, stream)) return rc;
   if (int rc = gemm_nn(CTX, R, E, E, m->Wd_cat, 3 * C, 3 * C, nullptr, G, 3 * C, false, st)) return rc;
@@ -305,14 +306,17 @@ int lvsr_train_cost_and_grads(lvsr_model* m, const float* x, const float* mask, 
   if (int rc = gemm_nn(S_prev, R, C, C, m->P(at + "/state_trans/transform_states.W"), M, M, nullptr, Q, M, false, st)) return rc;
   LVSR_CUDA_OK(cudaMemsetAsync(dP, 0, (size_t)Tp * B * M * sizeof(float), st));
   LVSR_CUDA_OK(cudaMemsetAsync(acc_v, 0, (size_t)nct * M * sizeof(float), st));
-  LVSR_CUDA_OK(cudaMemsetAsync(acc_Wh, 0, (size_t)nct * K * M * sizeof(float), st));
-  LVSR_CUDA_OK(cudaMemsetAsync(acc_filt, 0, (size_t)nct * K * w * sizeof(float), st));
+  if (!content) {
+    LVSR_CUDA_OK(cudaMemsetAsync(acc_Wh, 0, (size_t)nct * K * M * sizeof(float), st));
+    LVSR_CUDA_OK(cudaMemsetAsync(acc_filt, 0, (size_t)nct * K * w * sizeof(float), st));
+  }
   LVSR_CUDA_OK(cudaMemsetAsync(dsbuf[0], 0, (size_t)B * C * sizeof(float), st));
   if (int rc = onehot_rows(w0, B, Tp, st)) return rc;
   {
     const bool kp12 = att_bwd_kp(K) == 12;
     LVSR_CUDA_OK(cudaFuncSetAttribute(att_bwd_kernel<12>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ab_smem));
     LVSR_CUDA_OK(cudaFuncSetAttribute(att_bwd_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ab_smem));
+    LVSR_CUDA_OK(cudaFuncSetAttribute(att_bwd_content_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ab_smem));
     const int ew = ceil_div(B * C, 256);
     for (int i = L - 1; i >= 0; --i) {
       ProfScope prof("dec_bwd_step", st);
@@ -332,9 +336,11 @@ int lvsr_train_cost_and_grads(lvsr_model* m, const float* x, const float* mask, 
                           C, dctx_i, E)) return rc;
       // attention backward
       const float* w_prev = i == 0 ? w0 : W_all + (size_t)(i - 1) * B * Tp;
-      WindowArgs wa = {};
-      wa.weights = w_prev; wa.step = nullptr; wa.step_offset = i; wa.R = B; wa.Tp = Tp; wa.prior = prior_of(c); wa.win = win; wa.lohi = lohi;
-      if (int rc = attention_window(wa, st)) return rc;
+      if (!content) {                     // content attention attends every frame: no window
+        WindowArgs wa = {};
+        wa.weights = w_prev; wa.step = nullptr; wa.step_offset = i; wa.R = B; wa.Tp = Tp; wa.prior = prior_of(c); wa.win = win; wa.lohi = lohi;
+        if (int rc = attention_window(wa, st)) return rc;
+      }
       AttBwdArgs ab = {};
       ab.P = P; ab.H = Hatt; ab.maskH = attm; ab.q = Q + (size_t)i * B * M; ab.w_prev = w_prev; ab.w_cur = W_all + (size_t)i * B * Tp;
       ab.ctx = CTX + (size_t)i * B * E; ab.dctx = dctx_i;
@@ -346,7 +352,8 @@ int lvsr_train_cost_and_grads(lvsr_model* m, const float* x, const float* mask, 
       ab.B = B; ab.Tp = Tp; ab.M = M; ab.E = E; ab.K = K; ab.n = n;
       {
         ProfScope prof_ab("att_bwd", st);
-        if (kp12) att_bwd_kernel<12><<<nct, AB_NT, ab_smem, st>>>(ab, tc_cap);
+        if (content) att_bwd_content_kernel<<<nct, AB_NT, ab_smem, st>>>(ab, tc_cap);
+        else if (kp12) att_bwd_kernel<12><<<nct, AB_NT, ab_smem, st>>>(ab, tc_cap);
         else att_bwd_kernel<16><<<nct, AB_NT, ab_smem, st>>>(ab, tc_cap);
         LVSR_LAUNCH_CHECK();
       }
@@ -410,10 +417,12 @@ int lvsr_train_cost_and_grads(lvsr_model* m, const float* x, const float* mask, 
     // attention constants: sums of the per-CTA partials
     reduce_partials_kernel<<<grid1d(M), 256, 0, st>>>(acc_v, nct, M, grad_of(m, grads, at + "/energy_comp/linear.W"));
     LVSR_LAUNCH_CHECK();
-    reduce_partials_kernel<<<grid1d((long long)K * M), 256, 0, st>>>(acc_Wh, nct, (long long)K * M, grad_of(m, grads, at + "/handler.W"));
-    LVSR_LAUNCH_CHECK();
-    reduce_partials_kernel<<<grid1d((long long)K * w), 256, 0, st>>>(acc_filt, nct, (long long)K * w, grad_of(m, grads, at + "/conv1d.filters"));
-    LVSR_LAUNCH_CHECK();
+    if (!content) {
+      reduce_partials_kernel<<<grid1d((long long)K * M), 256, 0, st>>>(acc_Wh, nct, (long long)K * M, grad_of(m, grads, at + "/handler.W"));
+      LVSR_LAUNCH_CHECK();
+      reduce_partials_kernel<<<grid1d((long long)K * w), 256, 0, st>>>(acc_filt, nct, (long long)K * w, grad_of(m, grads, at + "/conv1d.filters"));
+      LVSR_LAUNCH_CHECK();
+    }
   }
   // ---- gradient of the attended sequence: glimpses + preprocess --------------------------------
   float* dH = ws.f32((size_t)Tp * B * E);

@@ -718,6 +718,78 @@ __global__ void __launch_bounds__(AB_NT, 1) att_bwd_kernel(AttBwdArgs a, int tc_
   }
 }
 
+// Content-only attention (SequenceContentAttention, B/bricks/attention.py:259-414): the same step backward without the
+// location term -- no conv recompute, no dF, no handler / filter partials and no gradient into alpha_{i-1} (the weights
+// of step i depend on s_{i-1} and the attended sequence only).  Every frame is attended: the window is [0, Tp).
+__host__ __device__ inline size_t att_bwd_content_smem_floats(int E, int tc_cap) {
+  return (size_t)((tc_cap + 3) & ~3) + E + 64 + 16;     // sde | sdctx | block reductions
+}
+
+__global__ void __launch_bounds__(AB_NT, 1) att_bwd_content_kernel(AttBwdArgs a, int tc_cap) {
+  extern __shared__ __align__(16) float smem[];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int b = blockIdx.x / AB_CS, rank = blockIdx.x % AB_CS;
+  const int M = a.M, E = a.E, Tp = a.Tp, B = a.B;
+  float* sde = smem;
+  float* sdctx = sde + ((tc_cap + 3) & ~3);
+  float* sred = sdctx + E;
+  const int tc = (Tp + AB_CS - 1) / AB_CS;
+  const int t0 = min(Tp, rank * tc), t1 = min(Tp, t0 + tc);
+  const int nt = t1 - t0;
+
+  for (int i = tid; i < E; i += AB_NT) sdctx[i] = a.dctx[(long long)b * E + i];
+  // S = sum_t alpha_i[t] dalpha_i[t] = dctx . ctx_i
+  float part = 0.f;
+  for (int i = tid; i < E; i += AB_NT) part += a.dctx[(long long)b * E + i] * a.ctx[(long long)b * E + i];
+  const float S = block_sum_512(part, sred);      // (contains the __syncthreads that publish the staging)
+
+  // ---- de[t] = alpha_i[t] (dctx . H[t] - S) for the owned positions: one warp per position ----
+  for (int t = warp; t < nt; t += AB_NT / 32) {
+    const long long pos = t0 + t;
+    const float* hrow = a.H + (pos * B + b) * E;
+    float d = 0.f;
+    for (int e = lane * 4; e < E; e += 128) {
+      const float4 h4 = __ldg(reinterpret_cast<const float4*>(hrow + e));
+      const float4 c4 = *reinterpret_cast<const float4*>(sdctx + e);
+      d = fmaf(h4.x, c4.x, d); d = fmaf(h4.y, c4.y, d); d = fmaf(h4.z, c4.z, d); d = fmaf(h4.w, c4.w, d);
+    }
+    d = warp_sum(d);
+    if (lane == 0) sde[t] = a.w_cur[(long long)b * Tp + pos] * (d - S);
+  }
+  __syncthreads();
+
+  // ---- one thread per matcher column, 16 positions of P and dP in flight ----
+  if (tid >= M) return;
+  const int m = tid;
+  const float qm = a.q[(long long)b * M + m], vm = a.v[m];
+  float dq = 0.f, dv = 0.f;
+  for (int tb = 0; tb < nt; tb += AB_TILE) {
+    const int tn = min(AB_TILE, nt - tb);
+    float pv[AB_TILE], dpv[AB_TILE];
+#pragma unroll
+    for (int tl = 0; tl < AB_TILE; ++tl) {
+      if (tl < tn) {
+        const long long o = ((long long)(t0 + tb + tl) * B + b) * M + m;
+        pv[tl] = __ldg(a.P + o);
+        dpv[tl] = a.dP[o];
+      }
+    }
+#pragma unroll
+    for (int tl = 0; tl < AB_TILE; ++tl) {
+      if (tl < tn) {
+        const float th = tanhf_acc(pv[tl] + qm);
+        const float de = sde[tb + tl];
+        const float dm = de * vm * (1.f - th * th);
+        a.dP[((long long)(t0 + tb + tl) * B + b) * M + m] = dpv[tl] + dm;
+        dq += dm;
+        dv = fmaf(de, th, dv);
+      }
+    }
+  }
+  a.dq_part[((long long)rank * B + b) * M + m] = dq;
+  a.acc_v[(long long)blockIdx.x * M + m] += dv;
+}
+
 // out[i] = sum over the CTAs' partials (fixed order)
 __global__ void reduce_partials_kernel(const float* part, int nparts, long long n, float* out) {
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {

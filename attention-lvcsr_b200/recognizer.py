@@ -69,7 +69,7 @@ class SpeechRecognizer(object):
         def unsupported(what):
             raise NotImplementedError("attention-lvcsr_b200: %s is outside the GPU hot path "
                                       "(SURVEY.md section 8)" % what)
-        if attention_type != "content_and_conv":
+        if attention_type not in _lib.ATTENTION_TYPES:
             unsupported("attention_type=%r" % attention_type)
         if lm:
             unsupported("language-model shallow fusion")
@@ -103,11 +103,16 @@ class SpeechRecognizer(object):
         act = post_merge_activation if post_merge_activation is not None else _bricks.Tanh()
         if dim_matcher is None:
             dim_matcher = dim_dec                                  # recognizer.py:225-226
-        if conv_n is None:
+        content = attention_type == "content"
+        if conv_n is None and not content:
             raise ValueError("conv_n is required for content_and_conv attention")
         subsample = list(subsample) if subsample else [1] * len(dims_bidir)
         prior = dict(prior) if prior else dict(type="expanding", initial_begin=0, initial_end=10000,
                                                min_speed=0, max_speed=0)    # lvsr/bricks/attention.py:72-74
+        if content:
+            # SequenceContentAttention takes no conv, normaliser or prior (lvsr/bricks/recognizer.py:261-265): the
+            # reference ignores these keys, and so does the library
+            conv_n, conv_num_filters, energy_normalizer, prior = 0, 0, None, None
         self.net = dict(
             num_features=int(input_dims["recordings"]), dims_bidir=[int(d) for d in dims_bidir],
             subsample=[int(k) for k in subsample], dim_dec=int(dim_dec), dim_matcher=int(dim_matcher),
@@ -119,14 +124,17 @@ class SpeechRecognizer(object):
             post_merge_dim=int(post_merge_dims[0]) if post_merge_dims else int(num_phonemes),
             post_merge_activation=act.kind, maxout_pieces=int(getattr(act, "num_pieces", 1)),
             use_states_for_readout=bool(use_states_for_readout),
-            energy_normalizer=energy_normalizer or "softmax", prior=prior)
+            energy_normalizer=energy_normalizer or "softmax", prior=prior, attention_type=attention_type)
         if not post_merge_dims:
             # Readout's default post_merge is a bare Bias on readout_dim (sequence_generators.py:596-599)
             self.net["post_merge_activation"] = "identity"
             unsupported("readout without post_merge_dims")
 
         # brick-tree handles
-        attention = _Child("conv_att", prior=prior, energy_normalizer=self.net["energy_normalizer"])
+        if content:
+            attention = _Child("cont_att")
+        else:
+            attention = _Child("conv_att", prior=prior, energy_normalizer=self.net["energy_normalizer"])
         transition = _Child("att_trans", attention=attention)
         readout = _Child("readout", emitter=_Child("emitter"), readout=None)
         self.generator = _Child("generator", transition=transition, readout=readout)
@@ -186,7 +194,8 @@ class SpeechRecognizer(object):
         cfg.post_merge_activation = _lib.ACTIVATIONS[n["post_merge_activation"]]
         cfg.use_states_for_readout = int(n["use_states_for_readout"])
         cfg.energy_normalizer = _lib.NORMALIZERS[n["energy_normalizer"]]
-        p = n["prior"]
+        cfg.attention_type = _lib.ATTENTION_TYPES[n.get("attention_type", "content_and_conv")]
+        p = n["prior"] or {}
         cfg.prior_type = _lib.PRIORS[p.get("type", "expanding")]
         cfg.prior_initial_begin = float(p.get("initial_begin", 0))
         cfg.prior_initial_end = float(p.get("initial_end", 10000))

@@ -35,6 +35,11 @@ enum { LVSR_MAX_LAYERS = 8 };
 enum { LVSR_NORM_SOFTMAX = 0, LVSR_NORM_LOGISTIC = 1, LVSR_NORM_RELU = 2 };
 enum { LVSR_ACT_MAXOUT = 0, LVSR_ACT_RELU = 1, LVSR_ACT_TANH = 2, LVSR_ACT_IDENTITY = 3 };
 enum { LVSR_PRIOR_EXPANDING = 0, LVSR_PRIOR_WINDOW_MEAN = 1, LVSR_PRIOR_WINDOW_MEDIAN = 2 };
+/* attention_type (lvsr/bricks/recognizer.py:261-277): SequenceContentAndConvAttention ("conv_att") or
+ * SequenceContentAttention ("cont_att", libs/blocks/blocks/bricks/attention.py:259-414).  Content attention has no
+ * conv, handler, window or energy bias: conv_n, conv_num_filters, energy_normalizer and the prior are ignored, as the
+ * reference does not pass them to that brick; every encoded frame of an utterance is attended. */
+enum { LVSR_ATT_CONTENT_AND_CONV = 0, LVSR_ATT_CONTENT = 1 };
 
 /* The subset of config['net'] the path depends on
  * (SpeechRecognizer.__init__, lvsr/bricks/recognizer.py:176-204). */
@@ -60,7 +65,7 @@ typedef struct {
   int32_t one_of_n_feedback;       /* 0: LookupFeedback(V+1, dim_feedback) (embed_outputs=True, the default);
                                       1: OneOfNFeedback(V+1) (embed_outputs=False, lvsr/bricks/__init__.py:86-109;
                                       exp/wsj/configs/wsj_jan_new.yaml:46): feedback = one-hot, dim_feedback = V+1  */
-  int32_t reserved;
+  int32_t attention_type;          /* LVSR_ATT_* (0, the zeroed default: content_and_conv)                      */
 } lvsr_config;
 
 const char* lvsr_last_error(void);
@@ -124,7 +129,9 @@ int lvsr_cost_matrix(lvsr_model* m, const float* attended_dev, const float* atte
 /* ---- the BeamSearch state functions (libs/blocks/blocks/search.py:101-142) ---------
  * R rows (beam hypotheses); row r attends utterance row_utt[r] of `attended` [T',U,E]
  * (row_utt NULL = identity, U == R: the reference's replicated-context call).
- * `preprocessed` may be NULL: it is then recomputed, as the reference does on every call. */
+ * `preprocessed` may be NULL: it is then recomputed, as the reference does on every call.
+ * Content attention: the initial weights and energies are zeros (libs/blocks/blocks/bricks/attention.py:392-395), and
+ * every energies output (here and in lvsr_cost_matrix) is zeros (lvsr/bricks/recognizer.py:475-478). */
 int lvsr_initial_states(lvsr_model* m, int32_t Tp, int32_t R, float* states_dev, int64_t* outputs_dev,
                         float* weighted_averages_dev, float* weights_dev, float* energies_dev,
                         int64_t* step_dev, void* stream);
