@@ -14,7 +14,12 @@
 //     the location term only).  wgmma does not apply: K = 10, the accumulator is consumed
 //     immediately by tanh in registers, and each warp owns a private 16x32 strip;
 //   * tanh = 1 - 2/(1+2^(2x log2e)): 2 MUFU + 3 FP32 instructions, |err| ~ 2e-7;
-//   * context: 8 independent 16-byte loads in flight per thread, 512 threads.
+//   * P: every line of the CTA's P rows is requested into L2 (prefetch.global.L2) when the energies
+//     start, and each 16-position tile is loaded when its turn comes.  A register double buffer of
+//     the next tile does not fit: at 512 threads the kernels run at the 128-register cap, the buffer
+//     was spilled right after its loads were issued (the spill store waits for the data, so nothing
+//     overlapped), and local memory lives in L2 because shared memory takes nearly all of L1;
+//   * context: 8 independent 16-byte loads in flight per thread up to the last position, 512 threads.
 #pragma once
 #include <cuda_bf16.h>
 
@@ -204,7 +209,7 @@ __device__ __forceinline__ void att_energies(const AttRowIO& a, const AttSmem& s
   const int ntile = (nt + 15) / 16;
   const float* pbase = a.P + ((long long)(a.b0 + t0) * a.U + a.u) * M + warp * NTW * 8 + 2 * tig;
   const long long prow = (long long)a.U * M;
-  float2 pc[NTW][2], pn[NTW][2];
+  float2 pc[NTW][2];
   auto load_p = [&](float2 (&dst)[NTW][2], int tile) {
     const int r0 = min(tile * 16 + g, nt - 1), r1 = min(tile * 16 + g + 8, nt - 1);   // clamp: tail rows are discarded
 #pragma unroll
@@ -213,9 +218,8 @@ __device__ __forceinline__ void att_energies(const AttRowIO& a, const AttSmem& s
       dst[j][1] = __ldg(reinterpret_cast<const float2*>(pbase + r1 * prow + j * 8));
     }
   };
-  if (ntile > 0) load_p(pc, 0);
   for (int tile = 0; tile < ntile; ++tile) {
-    if (tile + 1 < ntile) load_p(pn, tile + 1);
+    load_p(pc, tile);      // from L2: attention_row requested every line of the slice when the energies started
     const int ta = tile * 16 + g, tb = ta + 8;
     uint32_t ah[4], al[4];
     if constexpr (LOC) {
@@ -250,8 +254,6 @@ __device__ __forceinline__ void att_energies(const AttRowIO& a, const AttSmem& s
       part[ta] = ea;       // this warp's private partial sums; rows >= nt land in the 16-row padding
       part[tb] = eb;
     }
-#pragma unroll
-    for (int j = 0; j < NTW; ++j) { pc[j][0] = pn[j][0]; pc[j][1] = pn[j][1]; }
   }
 }
 
@@ -375,6 +377,14 @@ __device__ __forceinline__ void attention_row(const AttRowIO& a, float* smem, in
   ATT_STAMP(2);
 
   // ---- energies: e[t] = v . tanh(P[t] + q + F[t] . Wh) on the tensor cores -------------
+  {
+    // every 128-byte line of this CTA's P rows is requested into L2 at once, so the tile loads of the
+    // energy loop wait for L2 instead of one HBM round trip per tile
+    const int lines = M / 32;
+    const float* pb = a.P + ((long long)(b0 + t0) * U + u) * M;
+    for (int l = tid; l < nt * lines; l += NT)
+      asm volatile("prefetch.global.L2 [%0];\n" ::"l"(pb + (long long)(l / lines) * U * M + (l % lines) * 32));
+  }
   if (M == 512) att_energies<4, COMPACT, LOC>(a, s, nt, t0, tc_cap);
   else if (M == 256) att_energies<2, COMPACT, LOC>(a, s, nt, t0, tc_cap);
   else att_energies<1, COMPACT, LOC>(a, s, nt, t0, tc_cap);
@@ -444,22 +454,21 @@ __device__ __forceinline__ void attention_row(const AttRowIO& a, float* smem, in
       float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
       const float* hbase = a.H + ((long long)(b0 + t0) * U + u) * E + c4 * 4;
       const long long hstride = (long long)U * E;
-      int t = g;
-      for (; t + 7 * ng < nt; t += 8 * ng) {
+      // the last batch re-reads position nt - 1 for its missing slots and leaves them out of the sum: 8 loads stay in
+      // flight up to the last position, and the positions are added in the same order as one at a time
+      for (int t = g; t < nt; t += 8 * ng) {
         float4 h[8];
 #pragma unroll
-        for (int q = 0; q < 8; ++q) h[q] = __ldg(reinterpret_cast<const float4*>(hbase + (long long)(t + q * ng) * hstride));
+        for (int q = 0; q < 8; ++q)
+          h[q] = __ldg(reinterpret_cast<const float4*>(hbase + (long long)min(t + q * ng, nt - 1) * hstride));
 #pragma unroll
         for (int q = 0; q < 8; ++q) {
-          const float wq = s.su[t + q * ng];
-          acc.x = fmaf(wq, h[q].x, acc.x); acc.y = fmaf(wq, h[q].y, acc.y);
-          acc.z = fmaf(wq, h[q].z, acc.z); acc.w = fmaf(wq, h[q].w, acc.w);
+          if (t + q * ng < nt) {
+            const float wq = s.su[t + q * ng];
+            acc.x = fmaf(wq, h[q].x, acc.x); acc.y = fmaf(wq, h[q].y, acc.y);
+            acc.z = fmaf(wq, h[q].z, acc.z); acc.w = fmaf(wq, h[q].w, acc.w);
+          }
         }
-      }
-      for (; t < nt; t += ng) {
-        const float4 h0 = __ldg(reinterpret_cast<const float4*>(hbase + (long long)t * hstride));
-        const float w0 = s.su[t];
-        acc.x = fmaf(w0, h0.x, acc.x); acc.y = fmaf(w0, h0.y, acc.y); acc.z = fmaf(w0, h0.z, acc.z); acc.w = fmaf(w0, h0.w, acc.w);
       }
       *reinterpret_cast<float4*>(s.sred + (size_t)g * E + c4 * 4) = acc;
     }
