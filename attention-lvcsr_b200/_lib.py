@@ -15,6 +15,10 @@ NORMALIZERS = {"softmax": 0, "logistic": 1, "relu": 2}
 ACTIVATIONS = {"maxout": 0, "relu": 1, "tanh": 2, "identity": 3}
 PRIORS = {"expanding": 0, "window_around_mean": 1, "window_around_median": 2}
 ATTENTION_TYPES = {"content_and_conv": 0, "content": 1}
+# slots of lvsr_model_decoder_plan's report (LVSR_PLAN_*) and the kernel names of its `kernel` slot (LVSR_PLAN_DEC_*)
+PLAN_SLOTS = ("ran", "kernel", "cs", "grid", "nisl", "nrg", "ncg", "nc1", "nc2", "nc3", "tc_cap", "wh_rows", "red_alias",
+              "att_cs", "max_clusters")
+PLAN_KERNELS = ("stepwise", "dec_scan", "dec_scan<COMPACT>", "dec_content")
 
 
 class LvsrConfig(C.Structure):
@@ -74,6 +78,7 @@ SIGNATURES = {
     "lvsr_model_flat_params": (C.c_void_p, [_P]),
     "lvsr_model_finalize": (C.c_int, [_P]),
     "lvsr_model_status": (C.c_int, [_P, C.POINTER(C.c_int32), C.POINTER(C.c_int64)]),
+    "lvsr_model_decoder_plan": (C.c_int, [_P, C.POINTER(C.c_int32)]),
     "lvsr_encoded_length": (C.c_int, [_P, _I]),
     "lvsr_encoded_dim": (C.c_int, [_P]),
     "lvsr_encoder_forward": (C.c_int, [_P, _P, _P, _I, _I, _P, _P, _P]),

@@ -154,7 +154,7 @@ int glimpses(lvsr_model* m, const float* H, const float* P, const float* maskH, 
   a.w_out = w_out; a.e_out = e_out; a.ctx = ctx;
   a.R = R; a.U = U; a.Tp = Tp; a.M = c.dim_matcher; a.E = m->E; a.K = c.conv_num_filters; a.n = c.conv_n;
   a.normalizer = c.energy_normalizer;
-  return attention_step(a, !content_attention(m), st);
+  return attention_step(a, !content_attention(m), &m->att_cs, st);
 }
 
 // compute_states for R rows: distribute + fork(feedback) + GRU step.
@@ -231,7 +231,7 @@ size_t cost_ws_bytes(const lvsr_model* m, int Tp, int B, int L) {
 extern "C" {
 
 const char* lvsr_last_error(void) { return g_last_error.c_str(); }
-int lvsr_version(void) { return 102; }
+int lvsr_version(void) { return 103; }
 int64_t lvsr_launch_count(int reset) {
   const int64_t v = g_launch_count;
   if (reset) g_launch_count = 0;
@@ -368,6 +368,13 @@ int lvsr_model_status(lvsr_model* m, int32_t* launch_status, int64_t* stepwise_f
   LVSR_CUDA_OK(cudaMemcpy(&hst, m->status, sizeof(hst), cudaMemcpyDeviceToHost));   // synchronises with the device
   *launch_status = (int32_t)hst;
   if (stepwise_fallbacks) *stepwise_fallbacks = m->dec_fallbacks;
+  return 0;
+}
+
+int lvsr_model_decoder_plan(const lvsr_model* m, int32_t out[16]) {
+  LVSR_CHECK(m && out, "null argument");
+  for (int i = 0; i < 16; ++i) out[i] = m->dec_plan[i];
+  out[LVSR_PLAN_ATT_CS] = m->att_cs;
   return 0;
 }
 
@@ -636,6 +643,7 @@ int lvsr_cost_matrix(lvsr_model* m, const float* attended, const float* attended
   if (int rc = fill_f32(costs, (long long)L * B, 0.f, st)) return rc;
 
   bool scanned = false;
+  for (int32_t& v : m->dec_plan) v = 0;
   LVSR_CUDA_OK(cudaMemsetAsync(m->status, 0, sizeof(unsigned), st));
   if (getenv("LVSR_NO_DEC_SCAN") == nullptr && !m->force_stepwise) {
     DecScanArgs d = {};
@@ -676,9 +684,19 @@ int lvsr_cost_matrix(lvsr_model* m, const float* attended, const float* attended
       d.trace = reinterpret_cast<unsigned long long*>(ws.i64((size_t)2 * L * 9 + (size_t)L * 12 + (size_t)L * B));
       LVSR_CUDA_OK(cudaMemsetAsync(d.trace, 0, ((size_t)2 * L * 9 + (size_t)L * 12 + (size_t)L * B) * 8, st));
     }
-    int supported = 0;
-    if (int rc = dec_scan_try(d, !content_attention(m), &supported, st)) return rc;
+    int supported = 0, grid = 0, max_clusters = 0;
+    if (int rc = dec_scan_try(d, !content_attention(m), &supported, &grid, &max_clusters, st)) return rc;
     scanned = supported != 0;
+    int32_t* p = m->dec_plan;
+    p[LVSR_PLAN_MAX_CLUSTERS] = max_clusters;
+    if (scanned) {
+      p[LVSR_PLAN_RAN] = 1;
+      p[LVSR_PLAN_KERNEL] = content_attention(m) ? LVSR_PLAN_DEC_CONTENT : d.wh_rows != 16 ? LVSR_PLAN_DEC_SCAN_COMPACT
+                                                                                            : LVSR_PLAN_DEC_SCAN;
+      p[LVSR_PLAN_CS] = d.cs; p[LVSR_PLAN_GRID] = grid; p[LVSR_PLAN_NISL] = d.nisl; p[LVSR_PLAN_NRG] = d.nrg;
+      p[LVSR_PLAN_NCG] = d.ncg; p[LVSR_PLAN_NC1] = d.nc1; p[LVSR_PLAN_NC2] = d.nc2; p[LVSR_PLAN_NC3] = d.nc3;
+      p[LVSR_PLAN_TC_CAP] = d.tc_cap; p[LVSR_PLAN_WH_ROWS] = d.wh_rows; p[LVSR_PLAN_RED_ALIAS] = d.red_alias;
+    }
     if (scanned && getenv("LVSR_DEC_CHECK") != nullptr) {
       // debug post-condition: the launch reported success and every hand-over word was written
       LVSR_CUDA_OK(cudaStreamSynchronize(st));

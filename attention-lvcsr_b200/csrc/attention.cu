@@ -175,7 +175,7 @@ int attention_window(const WindowArgs& a, cudaStream_t stream) {
   return 0;
 }
 
-int attention_step(const AttStepArgs& a, bool location, cudaStream_t stream) {
+int attention_step(const AttStepArgs& a, bool location, int* cs_out, cudaStream_t stream) {
   ProfScope prof("attention", stream);
   LVSR_CHECK(a.M == 128 || a.M == 256 || a.M == 512, "attention_step: dim_matcher %d unsupported (128, 256 or 512)", a.M);
   LVSR_CHECK(a.E % 4 == 0 && a.E <= 4 * ATT_NT, "attention_step: encoded dim must be a multiple of 4 and <= %d", 4 * ATT_NT);
@@ -186,6 +186,18 @@ int attention_step(const AttStepArgs& a, bool location, cudaStream_t stream) {
   int cs = 1;
   const int sms = num_sms();
   while (cs < 8 && a.R * cs * 2 <= sms && ceil_div(a.Tp, cs * 2) >= 16) cs *= 2;
+  // LVSR_ATT_CS=1|2|4|8 (DESIGN §7, read on every call) replaces the one-wave choice above when the forced size keeps
+  // ceil(T'/cs) >= 16 and its shared memory fits; otherwise it is declined.  Clusters of one step never wait for each
+  // other, so the grid need not be co-resident.
+  if (const char* s = getenv("LVSR_ATT_CS")) {
+    const int f = atoi(s);
+    LVSR_CHECK(f == 1 || f == 2 || f == 4 || f == 8, "LVSR_ATT_CS=%s: expected 1, 2, 4 or 8", s);
+    const int cap = ceil_div(a.Tp, f);
+    const size_t smem = (location ? att_smem_floats(a.M, a.E, a.K, a.n, cap, f) : att_smem_floats<false>(a.M, a.E, 0, 0, cap, f)) *
+                        sizeof(float);
+    if ((f == 1 || cap >= 16) && smem <= 227 * 1024) cs = f;
+  }
+  *cs_out = cs;
   return launch_att(a, location, cs, stream);
 }
 

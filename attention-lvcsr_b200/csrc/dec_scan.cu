@@ -20,6 +20,8 @@
 //     the sentinel (common.cuh: ld_flow / st_flow).  One store + one load per hand-over.
 //   * the window statistics of the next step (mean / median position) ride on the attention
 //     exchange, so the windowing priors need no extra pass and no host round trip.
+#include <string.h>
+
 #include "attention_row.cuh"
 
 namespace lvsr {
@@ -437,7 +439,8 @@ bool kper_ok(int ktot) {
 
 // Fill the derived fields for a grid of G CTAs; returns the dynamic shared memory in bytes (0 = unsupported).
 // want_islands: cut the batch into independent islands of <= 16 rows (grid = R*cs exactly).
-size_t derive(DecScanArgs& a, int cs, int G, bool want_islands, bool loc) {
+// compact_only: skip the zero-padded handler copy (LVSR_DEC_HANDLER=compact).
+size_t derive(DecScanArgs& a, int cs, int G, bool want_islands, bool loc, bool compact_only) {
   const int R = a.B, C = a.C, E = a.E, M = a.M;
   a.cs = cs;
   a.tc_cap = ceil_div(a.Tp, cs);
@@ -459,6 +462,7 @@ size_t derive(DecScanArgs& a, int cs, int G, bool want_islands, bool loc) {
   a.red_alias = att_red_floats(E, a.tc_cap) >= red_f ? 1 : 0;
   // handler copy: zero-padded to 16 rows (fast path) if it fits, else only its K rows (long utterances)
   for (int rows : {16, a.K}) {
+    if (compact_only && rows == 16) continue;
     a.wh_rows = rows;
     size_t f = loc ? att_smem_floats(M, E, a.K, a.n, a.tc_cap, cs, a.wh_rows) : att_smem_floats<false>(M, E, 0, 0, a.tc_cap, cs);
     f = (f + 3) & ~(size_t)3;
@@ -472,26 +476,63 @@ size_t derive(DecScanArgs& a, int cs, int G, bool want_islands, bool loc) {
   return 0;
 }
 
-int plan_and_launch(DecScanArgs& a, bool loc, int* supported, cudaStream_t stream) {
+// Plan-forcing switches (DESIGN §7), read on every call.  They only remove candidates from the search below: the
+// shared-memory fit, the occupancy query, one cluster per row and ceil(T'/cs) >= 16 for cs > 1 stay in force, so a
+// forced plan that does not fit is declined (the caller runs the step-wise kernels) and never launched.
+struct DecForce {
+  int cs = 0;            // LVSR_DEC_CS=1|2|4|8 (0: any); replaces the one-wave start R*cs*2 <= SMs
+  int layout = -1;       // LVSR_DEC_LAYOUT=islands (1) | global (0); -1: islands when they fit, else global
+  bool compact = false;  // LVSR_DEC_HANDLER=compact: only the compact handler copy (dec_scan_kernel<true>)
+};
+
+int read_dec_force(DecForce* f) {
+  *f = DecForce();
+  if (const char* s = getenv("LVSR_DEC_CS")) {
+    f->cs = atoi(s);
+    LVSR_CHECK(f->cs == 1 || f->cs == 2 || f->cs == 4 || f->cs == 8, "LVSR_DEC_CS=%s: expected 1, 2, 4 or 8", s);
+  }
+  if (const char* s = getenv("LVSR_DEC_LAYOUT")) {
+    LVSR_CHECK(!strcmp(s, "islands") || !strcmp(s, "global"), "LVSR_DEC_LAYOUT=%s: expected islands or global", s);
+    f->layout = !strcmp(s, "islands") ? 1 : 0;
+  }
+  if (const char* s = getenv("LVSR_DEC_HANDLER")) {
+    LVSR_CHECK(!strcmp(s, "compact"), "LVSR_DEC_HANDLER=%s: expected compact", s);
+    f->compact = true;
+  }
+  return 0;
+}
+
+int plan_and_launch(DecScanArgs& a, bool loc, int* supported, int* grid, int* max_clusters_seen, cudaStream_t stream) {
   *supported = 0;
+  *grid = 0;
+  *max_clusters_seen = 0;
+  DecForce force;
+  if (int rc = read_dec_force(&force)) return rc;
   const int sms = sm_count();
   const int R = a.B, C = a.C, E = a.E, M = a.M;
   if (!kper_ok(E + C) || !kper_ok(C) || !(M == 128 || M == 256 || M == 512) || E % 4 != 0 || E / 4 > DS_THREADS) return 0;
   if ((loc && (a.K < 1 || a.K > 16)) || R < 1) return 0;
+  if (force.compact && !loc) return 0;     // content attention has no handler
   int cs = 1;
   while (cs < 8 && R * cs * 2 <= sms && ceil_div(a.Tp, cs * 2) >= 16) cs *= 2;
+  if (force.cs) {
+    if (force.cs > 1 && ceil_div(a.Tp, force.cs) < 16) return 0;
+    cs = force.cs;
+  }
   LVSR_CUDA_OK(cudaFuncSetAttribute(dec_scan_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
   LVSR_CUDA_OK(cudaFuncSetAttribute(dec_scan_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
   if (!loc) LVSR_CUDA_OK(cudaFuncSetAttribute(dec_content_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
   for (; cs >= 1; cs >>= 1) {
+    if (force.cs && cs != force.cs) break;
     // prefer islands (grid = one cluster per row); fall back to one global island on all SMs
-    bool islands = R >= DS_ROWS;
+    bool islands = R >= DS_ROWS && force.layout != 0;
+    if (force.layout == 1 && !islands) break;
     int G = islands ? R * cs : (sms / cs) * cs;
-    size_t smem = derive(a, cs, G, islands, loc);
-    if (smem == 0 && islands) {
+    size_t smem = derive(a, cs, G, islands, loc, force.compact);
+    if (smem == 0 && islands && force.layout != 1) {
       islands = false;
       G = (sms / cs) * cs;
-      smem = derive(a, cs, G, false, loc);
+      smem = derive(a, cs, G, false, loc, force.compact);
     }
     if (smem == 0) continue;
     // every cluster must be co-resident (consumers poll producers): ask the driver how many fit.  GPCs of
@@ -517,12 +558,14 @@ int plan_and_launch(DecScanArgs& a, bool loc, int* supported, cudaStream_t strea
       cudaGetLastError();
       continue;
     }
+    *max_clusters_seen = max_clusters;
     if (max_clusters * cs < G) {
       if (islands) continue;          // islands need exactly one cluster per row
       G = max_clusters * cs;
       if (G < cs) continue;
-      smem = derive(a, cs, G, false, loc);
-      if (smem == 0) continue;
+      const int wh_rows = a.wh_rows;
+      smem = derive(a, cs, G, false, loc, force.compact);
+      if (smem == 0 || a.wh_rows != wh_rows) continue;     // `kernel` was chosen for the first handler layout
       cfg.gridDim = dim3(G);
       cfg.dynamicSmemBytes = smem;
     }
@@ -541,6 +584,7 @@ int plan_and_launch(DecScanArgs& a, bool loc, int* supported, cudaStream_t strea
     }
     g_launch_count++;
     *supported = 1;
+    *grid = G;
 #ifdef LVSR_DEC_DEBUG
     {
       LVSR_CUDA_OK(cudaStreamSynchronize(stream));
@@ -562,11 +606,12 @@ int plan_and_launch(DecScanArgs& a, bool loc, int* supported, cudaStream_t strea
 
 }  // namespace
 
-// Runs the persistent decoder if the shapes fit (*supported = 1); otherwise leaves everything
-// untouched (*supported = 0) and the caller falls back to the per-step kernels.
-int dec_scan_try(DecScanArgs& a, bool location, int* supported, cudaStream_t stream) {
+// Runs the persistent decoder if the shapes fit (*supported = 1, the derived fields of `a` and *grid describe the
+// launched plan); otherwise leaves the buffers untouched (*supported = 0) and the caller falls back to the per-step
+// kernels.  *max_clusters = the answer of the last occupancy query (0 if none was made).
+int dec_scan_try(DecScanArgs& a, bool location, int* supported, int* grid, int* max_clusters, cudaStream_t stream) {
   ProfScope prof("dec_scan", stream);
-  return plan_and_launch(a, location, supported, stream);
+  return plan_and_launch(a, location, supported, grid, max_clusters, stream);
 }
 
 }  // namespace lvsr

@@ -115,8 +115,8 @@ struct AttStepArgs {
   int R, U, Tp, M, E, K, n, normalizer;
 };
 // location = false: content-only attention (no previous alignment, conv or handler; filt / Wh / K / n unused, e_out
-// receives zeros)
-int attention_step(const AttStepArgs& a, bool location, cudaStream_t stream);
+// receives zeros).  *cs_out = the cluster size launched.
+int attention_step(const AttStepArgs& a, bool location, int* cs_out, cudaStream_t stream);
 int attention_max_cluster();
 
 // ---- decoder.cu ---------------------------------------------------------------------
@@ -189,7 +189,7 @@ struct DecScanArgs {
   int wh_rows;                         // handler rows in shared memory: 16 (fast) or K (compact, long utterances)
   int red_alias;                       // dense-tile scratch shares the attention reduction scratch (long utterances)
 };
-int dec_scan_try(DecScanArgs& a, bool location, int* supported, cudaStream_t stream);
+int dec_scan_try(DecScanArgs& a, bool location, int* supported, int* grid, int* max_clusters, cudaStream_t stream);
 
 // small utility kernels
 int fill_f32(float* p, long long n, float v, cudaStream_t stream);

@@ -125,6 +125,8 @@ struct lvsr_model {
   unsigned* status = nullptr;       // device word: launch status of the data-flow decoder (common.cuh LVSR_FLOW_*)
   bool force_stepwise = false;      // set while a failed persistent launch is re-run on the step-wise kernels
   long long dec_fallbacks = 0;      // how often that happened
+  int32_t dec_plan[16] = {0};       // plan of the last lvsr_cost_matrix (lvsr_model_decoder_plan, LVSR_PLAN_* slots)
+  int att_cs = 0;                   // cluster size of the last attention_step launch
   bool finalized = false;
   Arena ws;
   // ---- training (train.cu) ----

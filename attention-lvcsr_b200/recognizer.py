@@ -370,6 +370,20 @@ class SpeechRecognizer(object):
         _lib.check(lib.lvsr_model_status(h, C.byref(st), C.byref(fb)))
         return int(st.value), int(fb.value)
 
+    def decoder_plan(self):
+        """Plan of the last cost_matrix (lvsr_model_decoder_plan) as a dict: ran (the persistent decoder ran),
+        kernel ("dec_scan", "dec_scan<COMPACT>", "dec_content" or "stepwise"), cs, grid, nisl, nrg, ncg, nc1, nc2,
+        nc3, tc_cap, wh_rows, red_alias, max_clusters (the planner's last occupancy answer) and att_cs (cluster
+        size of the last attention step)."""
+        import ctypes as C
+        lib, h = _lib.load(), self._require_ready()
+        out = (C.c_int32 * 16)()
+        _lib.check(lib.lvsr_model_decoder_plan(h, out))
+        plan = {k: int(out[i]) for i, k in enumerate(_lib.PLAN_SLOTS)}
+        plan["ran"] = bool(plan["ran"])
+        plan["kernel"] = _lib.PLAN_KERNELS[plan["kernel"]]
+        return plan
+
     def encoded_length(self, T):
         return int(_lib.load().lvsr_encoded_length(self._require_ready(), int(T)))
 

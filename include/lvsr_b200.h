@@ -100,6 +100,30 @@ int lvsr_model_finalize(lvsr_model* m);
  * kernels by itself and counts it in *stepwise_fallbacks (may be NULL).  No reference counterpart:
  * Theano raises from inside the compiled function instead. */
 int lvsr_model_status(lvsr_model* m, int32_t* launch_status, int64_t* stepwise_fallbacks);
+/* Plan of the decoder (host state, no synchronisation): out[LVSR_PLAN_*] describes the LAST lvsr_cost_matrix on this
+ * handle (training forwards included), all zero except MAX_CLUSTERS when it ran on the step-wise kernels, and
+ * out[LVSR_PLAN_ATT_CS] the cluster size of the last attention step (state functions, beam search and the step-wise
+ * fallback; 0 before the first).  The plan-forcing switches LVSR_DEC_CS, LVSR_DEC_LAYOUT, LVSR_DEC_HANDLER and
+ * LVSR_ATT_CS (DESIGN §7) narrow what the planners may choose; this report says what they did choose. */
+enum {
+  LVSR_PLAN_RAN = 0,          /* 1: the persistent decoder ran                                                 */
+  LVSR_PLAN_KERNEL = 1,       /* LVSR_PLAN_DEC_*                                                               */
+  LVSR_PLAN_CS = 2,           /* CTAs per row cluster                                                          */
+  LVSR_PLAN_GRID = 3,         /* CTAs launched                                                                 */
+  LVSR_PLAN_NISL = 4,         /* islands (0: global layout)                                                    */
+  LVSR_PLAN_NRG = 5,          /* 16-row groups of the global layout (1 in islands)                             */
+  LVSR_PLAN_NCG = 6,          /* column groups of the dense tiles                                              */
+  LVSR_PLAN_NC1 = 7,          /* columns per CTA: gate tile, candidate tile, query tile                        */
+  LVSR_PLAN_NC2 = 8,
+  LVSR_PLAN_NC3 = 9,
+  LVSR_PLAN_TC_CAP = 10,      /* positions per rank (ceil(T'/cs))                                              */
+  LVSR_PLAN_WH_ROWS = 11,     /* handler rows in shared memory: 16 (padded) or K (compact)                     */
+  LVSR_PLAN_RED_ALIAS = 12,   /* 1: the dense tiles' scratch shares the attention reduction scratch            */
+  LVSR_PLAN_ATT_CS = 13,      /* cluster size of the last attention step launch                                */
+  LVSR_PLAN_MAX_CLUSTERS = 14 /* answer of the planner's last occupancy query (0: none made)                   */
+};
+enum { LVSR_PLAN_STEPWISE = 0, LVSR_PLAN_DEC_SCAN = 1, LVSR_PLAN_DEC_SCAN_COMPACT = 2, LVSR_PLAN_DEC_CONTENT = 3 };
+int lvsr_model_decoder_plan(const lvsr_model* m, int32_t out[16]);
 
 /* ---- encoder: BeamSearch.context_computer / Encoder.apply -------------------------
  * (libs/blocks/blocks/search.py:97-99; lvsr/bricks/__init__.py:71-78).

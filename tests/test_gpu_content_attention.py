@@ -64,13 +64,13 @@ def _forward(rec, x, m, labels, lm):
     return att.cpu().numpy(), {k: v.cpu().numpy() for k, v in r.items()}
 
 
-def test_content_model_has_the_cont_att_parameter_table():
+def test_content_model_has_the_cont_att_parameter_table_at_abi_103():
     _torch()
     cfg = _cfg(SMALL)
     rec = _make(cfg)
     assert list(rec.parameter_shapes().items()) == list(CO.param_shapes(cfg).items())
     assert rec.generator.transition.attention.name == "cont_att"
-    assert package()._lib.load().lvsr_version() == 102
+    assert package()._lib.load().lvsr_version() == 103
 
 
 @pytest.mark.parametrize("arch,B,T", [("SMALL", 16, 60), ("PYRAMID", 37, 80), ("WSJ", 64, 48)])
@@ -83,6 +83,7 @@ def test_content_forward_matches_oracle(arch, B, T):
     with _env(LVSR_DEC_CHECK="1"):
         att, got = _forward(rec, x, m, labels, lm)
     assert rec.launch_status() == (0, 0)
+    assert rec.decoder_plan()["kernel"] == "dec_content"
     want_att, want_attm = O.encoder(cfg, params, x, m)
     want = CO.cost_matrix(cfg, params, want_att, want_attm, labels, lm, return_all=True)
     assert rel_err(att, want_att) < 1e-4
@@ -108,6 +109,7 @@ def test_content_forward_at_a_long_timit_like_length():
     rec = _make(cfg, params)
     with _env(LVSR_DEC_CHECK="1"):
         att, got = _forward(rec, x, m, labels, lm)
+    assert rec.decoder_plan()["kernel"] == "dec_content"
     want_att, want_attm = O.encoder(cfg, params, x, m)
     want = CO.cost_matrix(cfg, params, want_att, want_attm, labels, lm, return_all=True)
     for k in ("costs", "weights", "states", "weighted_averages"):

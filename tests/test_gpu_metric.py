@@ -42,6 +42,8 @@ def test_benchmarked_shapes_match_float64_oracle(name, B, T, L, monkeypatch):
     r = rec.cost_matrix(labels, lm, att, attm, return_all=True)
     status, fallbacks = rec.launch_status()
     assert status == 0 and fallbacks == 0
+    plan = rec.decoder_plan()
+    assert plan["ran"] and plan["nisl"] == B // 16, plan
     g = {k: v.double().cpu().numpy() for k, v in r.items()}
     errs["costs"] = rel_err(g["costs"], gold["costs"])
     errs["states"] = rel_err(g["states"].dot(proj["pC"]), gold["states_p"])
@@ -73,18 +75,21 @@ PRIORS = [
 @pytest.mark.parametrize("prior", PRIORS, ids=lambda p: p["type"] + str(p.get("initial_end", p.get("before"))))
 @pytest.mark.parametrize("B", [16, 37, 64])
 def test_island_mode_matches_oracle(prior, B, monkeypatch):
-    """B >= 16 runs the persistent decoder in island mode (dec_scan.cu): 1, 3 and 4 islands,
-    ragged island sizes (37 = 13+12+12), every window prior."""
+    """B >= 16 runs the persistent decoder in island mode (dec_scan.cu): 1, 3 and 4 islands, ragged island sizes
+    (37 = 13+12+12), every window prior.  T' = 32 lets the planner choose 2-CTA clusters; at cs 1 the 12-row islands
+    of B = 37 have too few CTAs for the dense tiles and the planner would take the global layout instead."""
     _torch()
     monkeypatch.setenv("LVSR_DEC_CHECK", "1")
     cfg = O.make_config(prior=prior, **PYRAMID)
     params = O.init_params(cfg, seed=8, scale=10.0)
-    x, m, labels, lm = O.synthetic_batch(cfg, B=B, T=96, seed=31 + B)
+    x, m, labels, lm = O.synthetic_batch(cfg, B=B, T=128, seed=31 + B)
     att, attm = O.encoder(cfg, params, x, m)
     want = O.cost_matrix(cfg, params, att, attm, labels, lm, return_all=True)
     rec = make_recognizer(cfg, params)
     got = rec.cost_matrix(labels, lm, att.astype(np.float32), attm.astype(np.float32), return_all=True)
     assert rec.launch_status() == (0, 0)
+    plan = rec.decoder_plan()
+    assert plan["ran"] and plan["cs"] == 2 and plan["nisl"] == -(-B // 16) and plan["grid"] == 2 * B, plan
     errs = {k: rel_err(got[k].cpu().numpy(), want[k]) for k in
             ("costs", "weights", "energies", "states", "weighted_averages")}
     print(prior["type"], B, errs)
@@ -123,5 +128,7 @@ def test_long_utterance_persistent_decoder_matches_oracle(monkeypatch):
     lib.lvsr_profile_enable(0)
     assert cnt.value == 0, "the step-wise fallback ran instead of the persistent decoder"
     assert rec.launch_status() == (0, 0)
+    plan = rec.decoder_plan()
+    assert plan["ran"] and plan["cs"] == 4 and plan["nisl"] == 1 and plan["red_alias"] == 1, plan
     for k in ("costs", "weights", "energies", "states", "weighted_averages"):
         assert rel_err(got[k].cpu().numpy(), want[k]) < TOL, k

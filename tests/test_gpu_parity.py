@@ -266,6 +266,8 @@ def test_config5_timit_long_utterance_properties():
     att, attm = rec.encode(x, m)
     assert tuple(att.shape) == (2000, 16, 512)
     r = rec.cost_matrix(labels, lm, att, attm, return_all=True)
+    plan = rec.decoder_plan()
+    assert plan["ran"] and plan["kernel"] == "dec_scan<COMPACT>", plan      # the padded handler copy does not fit
     w = r["weights"]
     assert bool(torch.isfinite(r["costs"]).all())
     assert torch.allclose(w.sum(dim=2), torch.ones_like(w.sum(dim=2)), atol=1e-4)
@@ -285,8 +287,10 @@ def test_persistent_decoder_equals_stepwise_kernels(monkeypatch):
     rec = make_recognizer(cfg, params)
     att, attm = rec.encode(x, m)
     a = rec.cost_matrix(labels, lm, att, attm, return_all=True)
+    assert rec.decoder_plan()["ran"]
     monkeypatch.setenv("LVSR_NO_DEC_SCAN", "1")
     b = rec.cost_matrix(labels, lm, att, attm, return_all=True)
+    assert not rec.decoder_plan()["ran"]
     for k in ("costs", "weights", "energies", "states", "weighted_averages"):
         assert rel_err(a[k].cpu().numpy(), b[k].cpu().numpy()) < 2e-5, k
 

@@ -45,11 +45,14 @@ def test_gradients_match_oracle_wsj_architecture():
 
 
 def test_gradients_island_batch_no_masks():
+    """Two 16-row islands of the persistent decoder (cs 1: T' = 10 is too short for larger clusters)."""
     _torch()
     cfg = O.make_config(**PYRAMID)
     params = O.init_params(cfg, seed=7, scale=10.0)
-    x, m, labels, lm = O.synthetic_batch(cfg, B=18, T=40, seed=12)
-    _check_grads(cfg, params, (x, None, labels, None))
+    x, m, labels, lm = O.synthetic_batch(cfg, B=32, T=40, seed=12)
+    _, rec = _check_grads(cfg, params, (x, None, labels, None))
+    plan = rec.decoder_plan()
+    assert plan["ran"] and plan["nisl"] == 2 and plan["cs"] == 1, plan
 
 
 def _train_like_the_oracle(cfg, params, tc, steps=2, B=4, T=40):
