@@ -58,6 +58,16 @@ class LvsrTrainConfig(C.Structure):
                 ("epsilon", C.c_float), ("max_norm", C.c_float), ("burn_in_steps", C.c_int32), ("decay", C.c_float)]
 
 
+LM_MAX_STATES = 7
+
+
+class LvsrLmFusion(C.Structure):
+    """Mirror of ``lvsr_lm_fusion`` (include/lvsr_b200.h)."""
+    _fields_ = [("weight", C.c_double), ("am_beta", C.c_double), ("no_transition_cost", C.c_double),
+                ("normalize_am_weights", C.c_int32), ("normalize_lm_weights", C.c_int32),
+                ("normalize_tot_weights", C.c_int32)]
+
+
 # name -> (restype, argtypes); every symbol include/lvsr_b200.h declares
 _P = C.c_void_p
 _I = C.c_int32
@@ -93,6 +103,10 @@ SIGNATURES = {
     "lvsr_search_result_length": (C.c_int, [_P, _I, _I]),
     "lvsr_search_result_get": (C.c_int, [_P, _I, _I, _P, _P]),
     "lvsr_search_result_destroy": (C.c_int, [_P]),
+    "lvsr_model_set_lm": (C.c_int, [_P, _I, _I, _P, C.c_int64, _P, _P, _P, C.POINTER(LvsrLmFusion)]),
+    "lvsr_model_clear_lm": (C.c_int, [_P]),
+    "lvsr_lm_initial_states": (C.c_int, [_P, _I, _P, _P, _P, _P]),
+    "lvsr_lm_next_states": (C.c_int, [_P, _I, _P, _P, _P, _P, _P, _P, _P]),
     "lvsr_recognizer_cost_host": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _P, _P]),
     "lvsr_train_cost_and_grads": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _I, C.c_float, _P, _P, _P]),
     "lvsr_train_apply_updates": (C.c_int, [_P, _P, C.c_float, C.POINTER(LvsrTrainConfig), _P]),

@@ -189,6 +189,10 @@ class GradientDescent(object):
                  on_unused_sources="warn", **kwargs):
         if recognizer is None:
             raise ValueError("GradientDescent needs the recognizer (no symbolic cost exists in the CUDA path)")
+        if getattr(recognizer, "lm", None):
+            # with an LM the reference's emitter is LMEmitter, whose costs are the fused readout's: inference only
+            raise NotImplementedError("attention-lvcsr_b200: training with a language model (shallow fusion is "
+                                      "inference only)")
         self.recognizer = recognizer
         self.step_rule = step_rule if step_rule is not None else CompositeRule([Scale(), RemoveNotFinite(0.0)])
         self._tc = _to_train_config(self.step_rule, decay)

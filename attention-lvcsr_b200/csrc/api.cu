@@ -203,6 +203,41 @@ ReadoutArgs readout_args(lvsr_model* m, int R, const float* merged) {
   return r;
 }
 
+LmFst lm_fst(lvsr_model* m) {
+  LmFst f = {};
+  f.off = m->lm_off; f.label = m->lm_label; f.next = m->lm_next; f.weight = m->lm_weight;
+  f.start = m->lm_start; f.V = m->cfg.num_phonemes;
+  f.no_transition_cost = (float)m->lm_fusion.no_transition_cost;
+  f.status = m->lm_status;
+  return f;
+}
+
+void lm_fuse(const lvsr_model* m, ReadoutArgs& r, const float* lm_add) {
+  const lvsr_lm_fusion& u = m->lm_fusion;
+  r.lm_add = lm_add;
+  r.lm_weight = (float)u.weight; r.am_beta = (float)u.am_beta;
+  r.norm_am = u.normalize_am_weights != 0; r.norm_lm = u.normalize_lm_weights != 0;
+  r.norm_tot = u.normalize_tot_weights != 0;
+}
+
+int lm_report(unsigned status) {
+  LVSR_CHECK(status != LVSR_LM_TOO_MANY_STATES, "language model: a hypothesis reached more than %d FST states",
+             (int)LVSR_LM_MAX_STATES);
+  LVSR_CHECK(status != LVSR_LM_CLOSURE_CAP, "language model: an epsilon closure exceeded 32 FST states");
+  LVSR_CHECK(status != LVSR_LM_CYCLE, "language model: the FST has an epsilon cycle");
+  LVSR_CHECK(status == 0, "language model: status %u", status);
+  return 0;
+}
+
+// Synchronises st and turns the LM status word into an error return (clearing it).
+static int lm_sync_status(lvsr_model* m, cudaStream_t st) {
+  unsigned h = 0;
+  LVSR_CUDA_OK(cudaMemcpyAsync(&h, m->lm_status, sizeof(h), cudaMemcpyDeviceToHost, st));
+  LVSR_CUDA_OK(cudaStreamSynchronize(st));
+  if (h) LVSR_CUDA_OK(cudaMemset(m->lm_status, 0, sizeof(unsigned)));
+  return lm_report(h);
+}
+
 size_t encoder_ws_bytes(const lvsr_model* m, int T, int B) {
   size_t total = 0;
   int Tl = T;
@@ -355,6 +390,7 @@ int lvsr_model_destroy(lvsr_model* m) {
   if (m->opt_ms_dx) cudaFree(m->opt_ms_dx);
   if (m->opt_scratch) cudaFree(m->opt_scratch);
   if (m->opt_desc) cudaFree(m->opt_desc);
+  lvsr_model_clear_lm(m);
   m->tws.destroy();
   m->ws.destroy();
   delete m;
@@ -424,6 +460,75 @@ int lvsr_model_finalize(lvsr_model* m) {
   DeviceGuard device_guard(m);
   LVSR_CHECK(m, "null model");
   return finalize_on_stream(m, 0, true);
+}
+
+int lvsr_model_clear_lm(lvsr_model* m) {
+  DeviceGuard device_guard(m);
+  LVSR_CHECK(m, "null model");
+  if (m->lm_off) {
+    LVSR_CUDA_OK(cudaDeviceSynchronize());       // a search or cost call may still read the tables
+    cudaFree(m->lm_off); cudaFree(m->lm_label); cudaFree(m->lm_next); cudaFree(m->lm_weight);
+  }
+  if (m->lm_status) cudaFree(m->lm_status);
+  m->lm_off = nullptr; m->lm_label = m->lm_next = nullptr; m->lm_weight = nullptr; m->lm_status = nullptr;
+  return 0;
+}
+
+int lvsr_model_set_lm(lvsr_model* m, int32_t num_states, int32_t start, const int64_t* off, int64_t num_arcs,
+                      const int32_t* label, const int32_t* next, const float* weight, const lvsr_lm_fusion* fusion) {
+  DeviceGuard device_guard(m);
+  LVSR_CHECK(m && off && fusion && num_states > 0 && num_arcs >= 0 && (num_arcs == 0 || (label && next && weight)),
+             "set_lm: bad arguments");
+  LVSR_CHECK(start >= 0 && start < num_states, "set_lm: start state %d outside [0, %d)", start, num_states);
+  LVSR_CHECK(off[0] == 0 && off[num_states] == num_arcs, "set_lm: arc offsets must run from 0 to num_arcs");
+  const int V = m->cfg.num_phonemes;
+  for (int32_t s = 0; s < num_states; ++s) {
+    LVSR_CHECK(off[s] <= off[s + 1], "set_lm: arc offsets decrease at state %d", s);
+    for (int64_t j = off[s]; j < off[s + 1]; ++j) {
+      LVSR_CHECK(label[j] >= 0 && label[j] <= V && next[j] >= 0 && next[j] < num_states,
+                 "set_lm: arc %lld of state %d has label %d / next state %d out of range", (long long)j, s, label[j], next[j]);
+      LVSR_CHECK(j == off[s] || label[j - 1] < label[j] || (label[j - 1] == label[j] && next[j - 1] <= next[j]),
+                 "set_lm: the arcs of state %d are not sorted by (label, next state)", s);
+    }
+  }
+  if (int rc = lvsr_model_clear_lm(m)) return rc;
+  const size_t na = (size_t)std::max<int64_t>(num_arcs, 1);
+  LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->lm_status), sizeof(unsigned)));
+  LVSR_CUDA_OK(cudaMemset(m->lm_status, 0, sizeof(unsigned)));
+  LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->lm_off), (size_t)(num_states + 1) * sizeof(long long)));
+  LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->lm_label), na * sizeof(int)));
+  LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->lm_next), na * sizeof(int)));
+  LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->lm_weight), na * sizeof(float)));
+  LVSR_CUDA_OK(cudaMemcpy(m->lm_off, off, (size_t)(num_states + 1) * sizeof(long long), cudaMemcpyHostToDevice));
+  if (num_arcs > 0) {
+    LVSR_CUDA_OK(cudaMemcpy(m->lm_label, label, (size_t)num_arcs * sizeof(int), cudaMemcpyHostToDevice));
+    LVSR_CUDA_OK(cudaMemcpy(m->lm_next, next, (size_t)num_arcs * sizeof(int), cudaMemcpyHostToDevice));
+    LVSR_CUDA_OK(cudaMemcpy(m->lm_weight, weight, (size_t)num_arcs * sizeof(float), cudaMemcpyHostToDevice));
+  }
+  m->lm_start = start;
+  m->lm_fusion = *fusion;
+  return 0;
+}
+
+int lvsr_lm_initial_states(lvsr_model* m, int32_t R, int32_t* states, double* weights, float* add, void* stream) {
+  DeviceGuard device_guard(m);
+  LVSR_CHECK(m && lm_attached(m), "lm_initial_states: no language model attached");
+  LVSR_CHECK(states && weights && add && R > 0, "lm_initial_states: bad arguments");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (int rc = lm_step(lm_fst(m), R, nullptr, nullptr, nullptr, nullptr, states, weights, add, st)) return rc;
+  return lm_sync_status(m, st);
+}
+
+int lvsr_lm_next_states(lvsr_model* m, int32_t R, const int32_t* states, const double* weights, const int64_t* outputs,
+                        int32_t* next_states, double* next_weights, float* next_add, void* stream) {
+  DeviceGuard device_guard(m);
+  LVSR_CHECK(m && lm_attached(m), "lm_next_states: no language model attached");
+  LVSR_CHECK(states && weights && outputs && next_states && next_weights && next_add && R > 0,
+             "lm_next_states: bad arguments");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (int rc = lm_step(lm_fst(m), R, states, weights, nullptr, reinterpret_cast<const long long*>(outputs), next_states,
+                       next_weights, next_add, st)) return rc;
+  return lm_sync_status(m, st);
 }
 
 }  // extern "C"
@@ -620,7 +725,7 @@ int lvsr_cost_matrix(lvsr_model* m, const float* attended, const float* attended
   if (int rc = check_ready(m)) return rc;
   LVSR_CHECK(attended && attended_mask && labels && costs && Tp > 0 && B > 0 && L > 0, "cost_matrix: bad arguments");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  m->ws.reserve(cost_ws_bytes(m, Tp, B, L), st);
+  m->ws.reserve(cost_ws_bytes(m, Tp, B, L) + (lm_attached(m) ? (size_t)L * B * m->cfg.num_phonemes * sizeof(float) : 0), st);
   ArenaScope scope(m, st);
   const lvsr_config& c = m->cfg;
   Arena& ws = m->ws;
@@ -783,6 +888,14 @@ int lvsr_cost_matrix(lvsr_model* m, const float* attended, const float* attended
     if (ws.off <= ws.cap) ws.off = mark;   // per-step scratch is reusable (stream order)
     w_prev = w_i;
   }
+  // the language model's cost rows in force before each label (sequence_generators.py:284-289), then fused below
+  float* lm_add = nullptr;
+  if (lm_attached(m)) {
+    lm_add = ws.f32((size_t)L * B * c.num_phonemes);
+    LVSR_CHECK(lm_add, "out of device memory (language model costs)");
+    if (int rc = lm_path(lm_fst(m), L, B, lab, labels_mask, lm_add, st)) return rc;
+    if (int rc = lm_sync_status(m, st)) return rc;
+  }
   // readout(states[:-1], glimpses[1:]) for all steps at once, then the emitter cost
   {
     const int R = L * B;
@@ -799,6 +912,7 @@ int lvsr_cost_matrix(lvsr_model* m, const float* attended, const float* attended
     ReadoutArgs r = readout_args(m, R, merged);
     r.labels = lab; r.lmask = labels_mask; r.costs_picked = costs;
     r.poison = scanned ? m->status : nullptr;
+    if (lm_add) lm_fuse(m, r, lm_add);
     if (int rc = readout_costs(r, st)) return rc;
   }
   if (states_out)
@@ -892,8 +1006,8 @@ namespace lvsr {
 int search_expand(lvsr_model* m, const float* attended, const float* preprocessed, const float* attended_mask, int Tp,
                   int U, const int* utt_len, const int* row_utt, const int* row_seg, const int* seg_start, int nseg,
                   int R, const float* states, const float* weights, const long long* step, const float* cost_so_far,
-                  int k, float* wavg, float* new_weights, float* new_energies, int* top_parent, int* top_symbol,
-                  float* top_cost, int* top_count, cudaStream_t st) {
+                  const float* lm_add, int k, float* wavg, float* new_weights, float* new_energies, int* top_parent,
+                  int* top_symbol, float* top_cost, int* top_count, cudaStream_t st) {
   ArenaScope scope(m, st);
   const lvsr_config& c = m->cfg;
   Arena& ws = m->ws;
@@ -909,6 +1023,7 @@ int search_expand(lvsr_model* m, const float* attended, const float* preprocesse
   if (int rc = readout_merged(m, R, states, wavg, merged, st)) return rc;
   ReadoutArgs r = readout_args(m, R, merged);
   r.costs_all = neglogp;
+  if (lm_add) lm_fuse(m, r, lm_add);
   if (int rc = readout_costs(r, st)) return rc;
   return segment_topk(neglogp, cost_so_far, seg_start, nseg, c.num_phonemes, k, top_parent, top_symbol, top_cost, top_count, st);
 }

@@ -114,6 +114,48 @@ __global__ void __launch_bounds__(256) dense_kernel(DenseArgs a) {
   }
 }
 
+// log_softmax over the row's V entries, 4 per lane (entries >= V are -inf and stay so)
+__device__ __forceinline__ void warp_log_softmax(float (&x)[4], int lane, int V) {
+  float mx = -INFINITY;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) mx = fmaxf(mx, x[q]);
+  mx = warp_max(mx);
+  float se = 0.f;
+#pragma unroll
+  for (int q = 0; q < 4; ++q)
+    if (lane + q * 32 < V) se += expf(x[q] - mx);
+  const float lse = logf(warp_sum(se));
+#pragma unroll
+  for (int q = 0; q < 4; ++q) x[q] = (x[q] - mx) - lse;
+}
+
+// ShallowFusionReadout.readout + LMEmitter.costs / cost (lvsr/bricks/language_models.py), in float32 like the reference
+__device__ __forceinline__ void readout_fused(const ReadoutArgs& a, int r, int lane, const float (&logit)[4]) {
+  float x[4], l[4];
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const int v = lane + q * 32;
+    x[q] = v < a.V ? a.am_beta * logit[q] : -INFINITY;
+    l[q] = v < a.V ? -a.lm_add[(long long)r * a.V + v] : -INFINITY;
+  }
+  if (a.norm_am) warp_log_softmax(x, lane, a.V);
+  if (a.norm_lm) warp_log_softmax(l, lane, a.V);
+#pragma unroll
+  for (int q = 0; q < 4; ++q) x[q] = lane + q * 32 < a.V ? x[q] + a.lm_weight * l[q] : -INFINITY;
+  if (a.norm_tot) warp_log_softmax(x, lane, a.V);
+  const long long lab = a.labels ? a.labels[r] : -1;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const int v = lane + q * 32;
+    if (v < a.V) {
+      float cost = -x[q];
+      if (a.poison && *a.poison != 0u) cost = __int_as_float(0x7fc00000);
+      if (a.costs_all) a.costs_all[(long long)r * a.V + v] = cost;
+      if (a.costs_picked && v == lab) a.costs_picked[r] = cost * (a.lmask ? a.lmask[r] : 1.f);
+    }
+  }
+}
+
 // One warp per row.
 __global__ void __launch_bounds__(256) readout_kernel(ReadoutArgs a) {
   extern __shared__ float sh[];
@@ -153,6 +195,10 @@ __global__ void __launch_bounds__(256) readout_kernel(ReadoutArgs a) {
     vmax = fmaxf(vmax, s);
   }
   vmax = warp_max(vmax);
+  if (a.lm_add) {
+    readout_fused(a, r, lane, logit);
+    return;
+  }
   float se = 0.f;
 #pragma unroll
   for (int q = 0; q < 4; ++q)

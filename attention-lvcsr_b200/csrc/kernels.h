@@ -153,8 +153,35 @@ struct ReadoutArgs {
   float* costs_all;        // [R, V] or nullptr
   float* costs_picked;     // [R] or nullptr
   const unsigned* poison;  // optional launch-status word of the producer: non-zero -> every cost is NaN
+  // shallow fusion (ShallowFusionReadout + LMEmitter, lvsr/bricks/language_models.py): with lm_add the cost is -x,
+  // x = am_beta * logits (log-softmaxed if norm_am) + lm_weight * (-lm_add, log-softmaxed if norm_lm), log-softmaxed
+  // again if norm_tot.  lm_add == nullptr: the plain SoftmaxEmitter cost.
+  const float* lm_add;     // [R, V] or nullptr
+  float lm_weight, am_beta;
+  int norm_am, norm_lm, norm_tot;
 };
 int readout_costs(const ReadoutArgs& a, cudaStream_t stream);
+
+// ---- lm.cu: FST language model states (float64 weights, at most LVSR_LM_MAX_STATES per hypothesis) --------------
+enum { LVSR_LM_TOO_MANY_STATES = 1, LVSR_LM_CLOSURE_CAP = 2, LVSR_LM_CYCLE = 3 };   // status word codes
+struct LmFst {
+  const long long* off;    // [num_states + 1] arc offsets
+  const int* label;        // [num_arcs] NN label + 1, 0 = epsilon; sorted by (label, next) within a state
+  const int* next;         // [num_arcs]
+  const float* weight;     // [num_arcs]
+  int start, V;
+  float no_transition_cost;
+  unsigned* status;        // first error of a launch (LVSR_LM_*), zeroed by the caller
+};
+// One warp per row: the set of row parent[r] (identity if null) advanced by symbols[r], or, with symbols == nullptr,
+// expand({start}); writes the set (padded with -1 / 0) and its cost row add_out [R, V].
+int lm_step(const LmFst& f, int R, const int* src_states, const double* src_weights, const int* parent,
+            const long long* symbols, int* states_out, double* weights_out, float* add_out, cudaStream_t stream);
+// Teacher forcing: add [L, B, V], row (i, b) = the cost row in force before labels[i, b]; masked labels are skipped.
+int lm_path(const LmFst& f, int L, int B, const long long* labels, const float* lmask, float* add, cudaStream_t stream);
+// dst row r = src row idx[r] of the (states, weights, add) triple
+int lm_gather(int* states, double* weights, float* add, const int* src_states, const double* src_weights,
+              const float* src_add, const int* idx, int Rn, int V, cudaStream_t stream);
 
 // ---- dec_scan.cu: persistent teacher-forced decoder -----------------------------------
 struct DecScanArgs {

@@ -128,6 +128,13 @@ struct lvsr_model {
   int32_t dec_plan[16] = {0};       // plan of the last lvsr_cost_matrix (lvsr_model_decoder_plan, LVSR_PLAN_* slots)
   int att_cs = 0;                   // cluster size of the last attention_step launch
   bool finalized = false;
+  // ---- FST language model (lvsr_model_set_lm); lm_off == nullptr: none attached ----
+  long long* lm_off = nullptr;
+  int *lm_label = nullptr, *lm_next = nullptr;
+  float* lm_weight = nullptr;
+  int lm_start = 0;
+  lvsr_lm_fusion lm_fusion = {};
+  unsigned* lm_status = nullptr;
   Arena ws;
   // ---- training (train.cu) ----
   Arena tws;                        // tape + backward workspace
@@ -220,6 +227,12 @@ int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int
                 float* attended_mask, LayerTape* tape, cudaStream_t st);
 int readout_merged(lvsr_model* m, int R, const float* states, const float* ctx, float* merged, cudaStream_t st);
 ReadoutArgs readout_args(lvsr_model* m, int R, const float* merged);
+// language model (api.cu): the device view of the attached FST, the fusion fields of a readout, and the LM status
+// word read back after a synchronisation of st (an error return when a kernel reported one; the word is cleared)
+static inline bool lm_attached(const lvsr_model* m) { return m->lm_off != nullptr; }
+LmFst lm_fst(lvsr_model* m);
+void lm_fuse(const lvsr_model* m, ReadoutArgs& r, const float* lm_add);
+int lm_report(unsigned status);
 size_t encoder_ws_bytes(const lvsr_model* m, int T, int B);
 size_t cost_ws_bytes(const lvsr_model* m, int Tp, int B, int L);
 
@@ -233,11 +246,12 @@ size_t cost_ws_bytes(const lvsr_model* m, int Tp, int B, int L);
 // per row (kept in wavg / new_weights / new_energies for search_advance), readout, -log softmax, and per segment the
 // k smallest cost_so_far + (-logp) in increasing order: top_parent (row index), top_symbol, top_cost [nseg * k],
 // top_count [nseg] (= min(k, width * V); -1 if a log-probability was not finite).
+// lm_add [R, V] (null without a language model) is fused into the readout.
 int search_expand(lvsr_model* m, const float* attended, const float* preprocessed, const float* attended_mask, int Tp,
                   int U, const int* utt_len, const int* row_utt, const int* row_seg, const int* seg_start, int nseg,
                   int R, const float* states, const float* weights, const long long* step, const float* cost_so_far,
-                  int k, float* wavg, float* new_weights, float* new_energies, int* top_parent, int* top_symbol,
-                  float* top_cost, int* top_count, cudaStream_t st);
+                  const float* lm_add, int k, float* wavg, float* new_weights, float* new_energies, int* top_parent,
+                  int* top_symbol, float* top_cost, int* top_count, cudaStream_t st);
 // search_advance = next_state_computer (B/search.py:119-142) for the Rn selected children (parent rows + symbols):
 // gathers the parents' state and, under the expanding prior and for content attention, their glimpses from
 // search_expand (exact there because the window does not depend on which rows are in the batch); under the

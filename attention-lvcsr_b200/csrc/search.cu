@@ -103,7 +103,7 @@ int lvsr_beam_search_many(lvsr_model* m, const float* attended, const float* pre
   int* d_top = reinterpret_cast<int*>(take(sz_top));
   LVSR_CHECK((size_t)(cur - dev) <= total, "beam_search_many: workspace accounting");
 
-  static thread_local Pinned pin_in, pin_out;
+  static thread_local Pinned pin_in, pin_out, pin_lm;
   if (int rc = pin_in.ensure(((size_t)8 * Rmax + 4 * U + 64) * sizeof(int) + (size_t)Rmax * (sizeof(long long) + sizeof(float)))) return rc;
   if (int rc = pin_out.ensure(((size_t)3 * U * k + U) * sizeof(int))) return rc;
   int* h_meta = static_cast<int*>(pin_in.p);
@@ -111,10 +111,45 @@ int lvsr_beam_search_many(lvsr_model* m, const float* attended, const float* pre
   float* h_cost = reinterpret_cast<float*>(h_sym + Rmax);
   int* h_top = static_cast<int*>(pin_out.p);
 
+  // language model state of every row (FSTTransition's states / weights / add), in both sets and the advance scratch
+  const bool lm = lm_attached(m);
+  int* lm_s[3] = {nullptr, nullptr, nullptr};
+  double* lm_w[3] = {nullptr, nullptr, nullptr};
+  float* lm_a[3] = {nullptr, nullptr, nullptr};
+  unsigned* h_lm = nullptr;
+  char* lm_dev = nullptr;
+  if (lm) {
+    const size_t sz_ls = rnd((size_t)Rmax * LVSR_LM_MAX_STATES * sizeof(int));
+    const size_t sz_lw = rnd((size_t)Rmax * LVSR_LM_MAX_STATES * sizeof(double)), sz_la = rnd((size_t)Rmax * V * sizeof(float));
+    LVSR_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&lm_dev), 3 * (sz_ls + sz_lw + sz_la), st));
+    char* p = lm_dev;
+    for (int i = 0; i < 3; ++i) {
+      lm_w[i] = reinterpret_cast<double*>(p); p += sz_lw;
+      lm_s[i] = reinterpret_cast<int*>(p); p += sz_ls;
+      lm_a[i] = reinterpret_cast<float*>(p); p += sz_la;
+    }
+    if (int rc = pin_lm.ensure(sizeof(unsigned))) return rc;
+    h_lm = static_cast<unsigned*>(pin_lm.p);
+  }
+  struct FreeLm { char* p; cudaStream_t s; ~FreeLm() { if (p) cudaFreeAsync(p, s); } } free_lm{lm_dev, st};
+  // the LM status word travels with the step's own copies and is checked after its synchronisations
+  auto lm_fetch = [&]() -> int {
+    if (lm) LVSR_CUDA_OK(cudaMemcpyAsync(h_lm, m->lm_status, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+    return 0;
+  };
+  auto lm_check = [&]() -> int {
+    if (!lm || *h_lm == 0) return 0;
+    const unsigned s = *h_lm;
+    LVSR_CUDA_OK(cudaMemset(m->lm_status, 0, sizeof(unsigned)));
+    return lm_report(s);
+  };
+
   // initial states: one row per utterance (B/search.py:103-104: initial_states(1))
   int curset = 0;
   if (int rc = lvsr_initial_states(m, Tp, U, states[0], reinterpret_cast<int64_t*>(tmp_step), wavg, weights[0], new_e,
                                    reinterpret_cast<int64_t*>(step[0]), stream)) return rc;
+  if (lm)
+    if (int rc = lm_step(lm_fst(m), U, nullptr, nullptr, nullptr, nullptr, lm_s[0], lm_w[0], lm_a[0], st)) return rc;
 
   std::vector<Utt> utts(U);
   int longest = 0;
@@ -172,6 +207,9 @@ int lvsr_beam_search_many(lvsr_model* m, const float* attended, const float* pre
       if (int rc = gather_rows(states[o], states[curset], d_meta, Rn, C, st)) return rc;
       if (int rc = gather_rows(weights[o], weights[curset], d_meta, Rn, Tp, st)) return rc;
       if (int rc = gather_i64(step[o], step[curset], d_meta, Rn, 0, st)) return rc;
+      if (lm)
+        if (int rc = lm_gather(lm_s[o], lm_w[o], lm_a[o], lm_s[curset], lm_w[curset], lm_a[curset], d_meta, Rn, V, st))
+          return rc;
       LVSR_CUDA_OK(cudaStreamSynchronize(st));           // h_meta is reused below
       curset = o;
     }
@@ -202,10 +240,12 @@ int lvsr_beam_search_many(lvsr_model* m, const float* attended, const float* pre
     int* d_seg = d_meta; int* d_rseg = d_seg + nseg + 1; int* d_rutt = d_rseg + R; int* d_len = d_rutt + R;
     int* tp = d_top; int* ts = tp + nseg * k; float* tc = reinterpret_cast<float*>(ts + nseg * k); int* tn = ts + 2 * nseg * k;
     if (int rc = search_expand(m, attended, preprocessed, attended_mask, Tp, U, d_len, d_rutt, d_rseg, d_seg, nseg, R,
-                               states[curset], weights[curset], step[curset], d_cost, k, wavg, new_w, new_e, tp, ts, tc, tn,
-                               st)) return rc;
+                               states[curset], weights[curset], step[curset], d_cost, lm ? lm_a[curset] : nullptr, k, wavg,
+                               new_w, new_e, tp, ts, tc, tn, st)) return rc;
     LVSR_CUDA_OK(cudaMemcpyAsync(h_top, d_top, ((size_t)3 * nseg * k + nseg) * sizeof(int), cudaMemcpyDeviceToHost, st));
+    if (int rc = lm_fetch()) return rc;
     LVSR_CUDA_OK(cudaStreamSynchronize(st));                 // the step's only synchronisation
+    if (int rc = lm_check()) return rc;
     const int* hp = h_top; const int* hs = hp + nseg * k;
     const float* hc = reinterpret_cast<const float*>(hs + nseg * k); const int* hn = hs + 2 * nseg * k;
 
@@ -277,12 +317,20 @@ int lvsr_beam_search_many(lvsr_model* m, const float* attended, const float* pre
     if (int rc = search_advance(m, attended, preprocessed, attended_mask, Tp, U, d_len2, Rs, d_par, d_sym, d_rutt2, d_rseg2,
                                 d_seg2, nseg, states[curset], weights[curset], step[curset], wavg, new_w, new_e, a_states,
                                 n_wavg, a_weights, n_e, all_kept ? step[o] : tmp_step, st)) return rc;
+    const int la = all_kept ? o : 2;                       // FSTTransition.apply of the selected children
+    if (lm)
+      if (int rc = lm_step(lm_fst(m), Rs, lm_s[curset], lm_w[curset], d_par, d_sym, lm_s[la], lm_w[la], lm_a[la], st))
+        return rc;
     if (!all_kept && nkeep > 0) {
       if (int rc = gather_rows(states[o], a_states, d_keep, nkeep, C, st)) return rc;
       if (int rc = gather_rows(weights[o], a_weights, d_keep, nkeep, Tp, st)) return rc;
       if (int rc = gather_i64(step[o], tmp_step, d_keep, nkeep, 0, st)) return rc;
+      if (lm)
+        if (int rc = lm_gather(lm_s[o], lm_w[o], lm_a[o], lm_s[2], lm_w[2], lm_a[2], d_keep, nkeep, V, st)) return rc;
     }
+    if (int rc = lm_fetch()) return rc;
     LVSR_CUDA_OK(cudaStreamSynchronize(st));               // pinned staging is rewritten by the next step
+    if (int rc = lm_check()) return rc;
     curset = o;
   }
 

@@ -149,6 +149,7 @@ int lvsr_train_cost_and_grads(lvsr_model* m, const float* x, const float* mask, 
   DeviceGuard device_guard(m);
   if (int rc = check_ready(m)) return rc;
   LVSR_CHECK(x && labels && cost_out && grads && T > 0 && B > 0 && L > 0, "train_cost_and_grads: bad arguments");
+  LVSR_CHECK(!lm_attached(m), "train_cost_and_grads: shallow fusion is inference only (detach the language model)");
   const lvsr_config& c = m->cfg;
   LVSR_CHECK(c.energy_normalizer == LVSR_NORM_SOFTMAX,
              "training supports the softmax energy normaliser only (logistic / relu: inference only)");

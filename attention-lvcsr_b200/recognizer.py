@@ -23,6 +23,7 @@ import numpy as np
 
 from . import _lib
 from . import bricks as _bricks
+from . import lm as _lm
 from .search import BeamSearch, CandidateNotFoundError  # noqa: F401
 
 
@@ -42,6 +43,24 @@ class _Variable(object):
 
 def _ptr(t):
     return None if t is None else t.data_ptr()
+
+
+# config['net']['lm'] keys and their defaults (lvsr/bricks/recognizer.py:324-331, LanguageModel's no_transition_cost)
+LM_DEFAULTS = OrderedDict(weight=0.0, normalize_am_weights=True, normalize_lm_weights=False,
+                          normalize_tot_weights=False, am_beta=1.0, no_transition_cost=1e12, type_="fst")
+
+
+def _lm_config(lm):
+    unknown = sorted(set(lm) - set(LM_DEFAULTS) - {"path"})
+    if unknown:
+        raise TypeError("unknown lm option(s) %s" % unknown)
+    out = OrderedDict(LM_DEFAULTS)
+    out.update(lm)
+    if out["type_"] != "fst":
+        raise ValueError("lm type_ %r: only 'fst' exists" % (out["type_"],))
+    if not (out["normalize_am_weights"] or out["normalize_lm_weights"] or out["normalize_tot_weights"]):
+        logger.warning("Beam search is prone to fail with no log-prob normalization")
+    return out
 
 
 class _Child(object):
@@ -71,8 +90,12 @@ class SpeechRecognizer(object):
                                       "(SURVEY.md section 8)" % what)
         if attention_type not in _lib.ATTENTION_TYPES:
             unsupported("attention_type=%r" % attention_type)
-        if lm:
-            unsupported("language-model shallow fusion")
+        if lm and not lm.get("path"):
+            # the reference then swaps in LMEmitter with the unfused readout: costs become raw logits
+            unsupported("lm without a path")
+        if lm and character_map is None:
+            unsupported("lm without a character_map")
+        lm = _lm_config(lm) if lm else None
         if not bidir:
             unsupported("unidirectional encoder")
         if dims_top:
@@ -93,6 +116,8 @@ class SpeechRecognizer(object):
         self.eos_label = eos_label
         self.data_prepend_eos = data_prepend_eos
         self.character_map = character_map
+        self.lm = lm
+        self._lm_tables = _lm.load(lm["path"], character_map, int(num_phonemes)) if lm else None
         self.criterion = criterion or dict(name="log_likelihood")
         self.max_decoded_length_scale = max_decoded_length_scale
         self.rec_weights_init = None
@@ -216,7 +241,27 @@ class SpeechRecognizer(object):
                 cfg = self._make_config()
                 _lib.check(lib.lvsr_model_create(C.byref(cfg), C.byref(h)))
             self._handle = h
+            if self.lm:
+                self._attach_lm(lib, h)
         return self._handle
+
+    def _attach_lm(self, lib, h):
+        """LanguageModel + ShallowFusionReadout (lvsr/bricks/recognizer.py:322-338) on the handle."""
+        import ctypes as C
+        t, o = self._lm_tables, self.lm
+        fusion = _lib.LvsrLmFusion(weight=float(o["weight"]), am_beta=float(o["am_beta"]),
+                                   no_transition_cost=float(o["no_transition_cost"]),
+                                   normalize_am_weights=int(bool(o["normalize_am_weights"])),
+                                   normalize_lm_weights=int(bool(o["normalize_lm_weights"])),
+                                   normalize_tot_weights=int(bool(o["normalize_tot_weights"])))
+        try:
+            _lib.check(lib.lvsr_model_set_lm(h, t["num_states"], t["start"], t["offsets"].ctypes.data, len(t["label"]),
+                                             t["label"].ctypes.data, t["next"].ctypes.data, t["weight"].ctypes.data,
+                                             C.byref(fusion)))
+        except Exception:
+            lib.lvsr_model_destroy(h)
+            self._handle = None
+            raise
 
     def __del__(self):
         try:
@@ -329,7 +374,7 @@ class SpeechRecognizer(object):
     # pickling: device handles do not travel (lvsr/bricks/recognizer.py:549-562 drops the compiled functions)
     def __getstate__(self):
         state = dict(self.__dict__)
-        for attr in ("_handle", "_beam_search", "_generator_state"):
+        for attr in ("_handle", "_beam_search", "_generator_state", "_lm_tables"):    # the FST reloads from lm['path']
             state.pop(attr, None)
         state["_device"] = None if self._device is None else str(self._device)
         state["_saved_parameters"] = None if self._handle is None else self.get_parameter_values()
@@ -340,6 +385,9 @@ class SpeechRecognizer(object):
         self.__dict__.update(state)
         self._handle = None
         self._beam_search = None
+        lm = self.__dict__.get("lm")
+        self.lm = lm
+        self._lm_tables = _lm.load(lm["path"], self.character_map, self.net["num_phonemes"]) if lm else None
         if saved is not None:
             try:
                 self.set_parameter_values(saved)
@@ -548,6 +596,9 @@ class SpeechRecognizer(object):
         (sequence_generators.py:772-778; a seeded Philox stream on the device instead of Theano's MRG stream, so
         draws differ from the reference while their distribution does not), ``sample=False`` emits the arg-max.
         Returns dict(outputs [n,B] int64, costs [n,B] = -log p(emitted), states [n,B,C], weights [n,B,T'])."""
+        if self.lm:
+            # LMEmitter.emit returns zeros in the reference: generating with an LM is not defined there
+            raise NotImplementedError("attention-lvcsr_b200: generate / sample with a language model")
         torch = self._torch()
         att, attm = self.encode(recordings, recordings_mask)
         B, Tp = att.shape[1], att.shape[0]
@@ -613,6 +664,29 @@ class SpeechRecognizer(object):
                                            _ptr(st["weighted_averages"]), _ptr(st["weights"]),
                                            _ptr(st["energies"]), _ptr(st["step"]), self._stream()))
         return st
+
+    # the language model's initial_state_computer / next_state_computer (FSTTransition, lvsr/bricks/language_models.py)
+    def _lm_initial_states(self, R):
+        torch = self._torch()
+        lib, h = _lib.load(), self._require_ready()
+        st = OrderedDict(lm_states=torch.empty((R, _lib.LM_MAX_STATES), dtype=torch.int32, device=self.device),
+                         lm_weights=torch.empty((R, _lib.LM_MAX_STATES), dtype=torch.float64, device=self.device),
+                         lm_add=torch.empty((R, self.net["num_phonemes"]), dtype=torch.float32, device=self.device))
+        _lib.check(lib.lvsr_lm_initial_states(h, R, _ptr(st["lm_states"]), _ptr(st["lm_weights"]), _ptr(st["lm_add"]),
+                                              self._stream()))
+        return st
+
+    def _lm_next_states(self, st, outputs):
+        torch = self._torch()
+        lib, h = _lib.load(), self._require_ready()
+        y = self._dev(outputs, torch.int64)
+        s, w = self._dev(st["lm_states"], torch.int32), self._dev(st["lm_weights"], torch.float64)
+        R = s.shape[0]
+        nxt = OrderedDict(lm_states=torch.empty_like(s), lm_weights=torch.empty_like(w),
+                          lm_add=torch.empty((R, self.net["num_phonemes"]), dtype=torch.float32, device=self.device))
+        _lib.check(lib.lvsr_lm_next_states(h, R, _ptr(s), _ptr(w), _ptr(y), _ptr(nxt["lm_states"]),
+                                           _ptr(nxt["lm_weights"]), _ptr(nxt["lm_add"]), self._stream()))
+        return nxt
 
     def _row_utt(self, contexts, R):
         torch = self._torch()

@@ -46,7 +46,8 @@ class Data(object):
         self.num_labels = self.info_dataset.num_labels
         self.num_features = self.info_dataset.num_features
         self.eos_label = self.num_labels - 1 if add_eos else None       # the npz reserves its last symbol for eos
-        self.character_map = None
+        chars = self.info_dataset.characters        # {character: label}, what the LM's symbol remap reads
+        self.character_map = None if chars is None else {c: i for i, c in enumerate(chars)}
 
     def get_dataset(self, part, add_sources=()):
         return NpzAudioDataset(self.path, self.name_mapping.get(part, part))

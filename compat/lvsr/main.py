@@ -123,6 +123,15 @@ def search(config, params, load_path, part, decode_only, report, decoded_save, n
         os.makedirs(report, exist_ok=True)
         print_to = open(os.path.join(report, "report.txt"), "w")
     num_examples = total_nll = total_errors = total_length = 0.0
+    total_wer_errors = total_word_length = 0.0
+    to_words = None
+    if config.get("vocabulary"):
+        # word error rate over the vocabulary's word ids (lvsr/main.py:757-765)
+        with open(os.path.expandvars(config["vocabulary"])) as f:
+            vocabulary = dict(line.split() for line in f.readlines())
+
+        def to_words(chars):
+            return [vocabulary[w] if w in vocabulary else vocabulary["<UNK>"] for w in chars.split()]
     for number, example in enumerate(data.examples(part, shuffle=part == "train", seed=seed,
                                                    num_examples=500 if part == "train" else None)):
         if decode_only and number not in decode_only:
@@ -164,6 +173,10 @@ def search(config, params, load_path, part, decode_only, report, decoded_save, n
             error = 1
         total_errors += len(groundtruth) * error
         total_length += len(groundtruth)
+        if to_words:
+            wer_error = min(1, wer(to_words(groundtruth_text), to_words(recognized_text)))
+            total_wer_errors += len(groundtruth) * wer_error
+            total_word_length += len(groundtruth)
         if decoded_file is not None:
             print("{} {}".format(uttids, " ".join(recognized)), file=decoded_file)
         print("Decoding took:", took, file=print_to)
@@ -173,6 +186,9 @@ def search(config, params, load_path, part, decode_only, report, decoded_save, n
             print("Recognized cost:", costs_recognized.sum(), file=print_to)
         print("CER:", error, file=print_to)
         print("Average CER:", total_errors / total_length, file=print_to)
+        if to_words:
+            print("WER:", wer_error, file=print_to)
+            print("Average WER:", total_wer_errors / total_word_length, file=print_to)
         print_to.flush()
     if decoded_file is not None:
         decoded_file.close()

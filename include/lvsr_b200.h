@@ -197,6 +197,39 @@ int lvsr_search_result_length(const lvsr_search_result* r, int32_t utt, int32_t 
 int lvsr_search_result_get(const lvsr_search_result* r, int32_t utt, int32_t j, int64_t* tokens, float* costs);
 int lvsr_search_result_destroy(lvsr_search_result* r);
 
+/* ---- FST language model, shallow fusion (lvsr/bricks/language_models.py, lvsr/ops.py:22-233) ----------------
+ * lvsr_model_set_lm attaches an FST given as host arrays in NN label space: arcs of state s are
+ * [arc_offsets[s], arc_offsets[s+1]) (arc_offsets has num_states + 1 entries), arc_label = NN symbol + 1 with
+ * 0 = epsilon, each state's arcs sorted by (label, next state); arc weights are costs (negative log).  While it is
+ * attached, lvsr_cost_matrix (and so lvsr_recognizer_cost_host) and lvsr_beam_search_many return the costs of
+ * ShallowFusionReadout + LMEmitter instead of -log softmax, and lvsr_train_cost_and_grads refuses to run.
+ * lvsr_cost_matrix then synchronises its stream once, to report an LM error.  lvsr_model_clear_lm detaches it.
+ *
+ * The LM state of a row is a set of at most LVSR_LM_MAX_STATES (fst state int32, weight float64) pairs padded with
+ * state -1 / weight 0, and its cost row add [V] (float32; no_transition_cost where a symbol leads nowhere, and
+ * everywhere once the set is empty).  lvsr_lm_initial_states writes expand({start: 0}) for R rows;
+ * lvsr_lm_next_states advances row r by outputs[r] (int64).  Both synchronise the stream and return an error when a
+ * set exceeds LVSR_LM_MAX_STATES, an epsilon closure exceeds 32 states or an epsilon cycle is met; the handle stays
+ * usable. */
+enum { LVSR_LM_MAX_STATES = 7 };
+typedef struct {
+  double weight;                   /* lm weight (reference default 0.0)                          */
+  double am_beta;                  /* scale of the acoustic logits (1.0)                         */
+  double no_transition_cost;       /* cost of a symbol without an arc (1e12)                     */
+  int32_t normalize_am_weights;    /* log_softmax of the scaled logits (reference default 1)     */
+  int32_t normalize_lm_weights;    /* log_softmax of -add (0)                                    */
+  int32_t normalize_tot_weights;   /* log_softmax of the sum (0)                                 */
+} lvsr_lm_fusion;
+int lvsr_model_set_lm(lvsr_model* m, int32_t num_states, int32_t start, const int64_t* arc_offsets_host, int64_t num_arcs,
+                      const int32_t* arc_label_host, const int32_t* arc_next_host, const float* arc_weight_host,
+                      const lvsr_lm_fusion* fusion);
+int lvsr_model_clear_lm(lvsr_model* m);
+int lvsr_lm_initial_states(lvsr_model* m, int32_t R, int32_t* states_dev, double* weights_dev, float* add_dev,
+                           void* stream);
+int lvsr_lm_next_states(lvsr_model* m, int32_t R, const int32_t* states_dev, const double* weights_dev,
+                        const int64_t* outputs_dev, int32_t* next_states_dev, double* next_weights_dev,
+                        float* next_add_dev, void* stream);
+
 /* ---- host-buffer entry points (the call a user of the reference makes) -------------
  * SpeechRecognizer.cost on a batch (lvsr/bricks/recognizer.py:375-390): H2D copies,
  * encoder, cost_matrix, D2H of costs [L,B]; synchronises.  Buffers should be pinned. */
@@ -242,7 +275,7 @@ int64_t lvsr_launch_count(int reset);
 /* Per-kernel-class device timing (CUDA events recorded on the launching stream around every
  * launch of that class) -- the analogue of the reference's Theano ProfileStats
  * (libs/Theano/theano/compile/profiling.py:97).  Classes: "gemm", "bigru", "attention",
- * "window", "dense", "readout".  lvsr_profile_read synchronises the device, returns the
+ * "window", "dense", "readout", "lm".  lvsr_profile_read synchronises the device, returns the
  * summed milliseconds and launch count recorded since the last read of that class. */
 int lvsr_profile_enable(int on);
 int lvsr_profile_read(const char* kernel_class, double* total_ms, int64_t* count);
