@@ -29,10 +29,51 @@ def make_recognizer(cfg, params=None):
         embed_outputs=cfg.get("embed_outputs", True), prior=cfg["prior"], energy_normalizer=cfg["energy_normalizer"],
         use_states_for_readout=cfg["use_states_for_readout"],
         max_decoded_length_scale=cfg["max_decoded_length_scale"],
+        attention_type=cfg.get("attention_type", "content_and_conv"),
         enc_transition=pkg.GatedRecurrent, dec_transition=pkg.GatedRecurrent, data_prepend_eos=False)
     if params is not None:
         rec.set_parameter_values(params)
     return rec
+
+
+# ---- element-by-element comparison with the float64 oracle -------------------------------------------------------
+
+def f32(a):
+    """The float32 rounding of `a`, in float64: what the oracle is given so that the errors measured are the kernels'."""
+    return np.asarray(a, dtype=np.float32).astype(np.float64)
+
+
+def elementwise_err(got, want, floor=0.1):
+    """max |got - want| / (|want| + floor * max|want|): a wrong small element counts, a float32 absolute error of an
+    element near 0 does not."""
+    got, want = np.asarray(got, np.float64), np.asarray(want, np.float64)
+    scale = np.abs(want).max()
+    return float((np.abs(got - want) / (np.abs(want) + floor * max(scale, 1e-30))).max())
+
+
+def check_weights(w, ww, errs, key="weights"):
+    """Attention weights: exactly 0 where the oracle's are 0 (outside the window, masked positions, rows without a
+    valid position), < 1e-29 where the oracle's are below 1e-30; errs[key] = the worst relative error per element
+    elsewhere, errs[key + "_sum"] = the worst distance of a row sum from 1 over the rows with a valid position."""
+    w, ww = np.asarray(w, np.float64), np.asarray(ww, np.float64)
+    zero = ww == 0
+    assert not np.any(w[zero]), "%s: %d non-zero weights where the oracle's are 0 (outside the window or masked)" % (
+        key, int(np.count_nonzero(w[zero])))
+    tiny = (ww > 0) & (ww < 1e-30)
+    assert np.all(np.abs(w[tiny]) < 1e-29), key
+    big = ww >= 1e-30
+    errs[key] = float((np.abs(w[big] - ww[big]) / ww[big]).max()) if big.any() else 0.0
+    s, sw = w.sum(-1), ww.sum(-1)
+    valid = sw > 0.5                                # rows with a valid position sum to 1 in the oracle, others to 0
+    assert np.all(s[~valid] == 0), key
+    errs[key + "_sum"] = float(np.abs(s[valid] - 1).max()) if valid.any() else 0.0
+
+
+def check_energies(e, we, errs):
+    """Energies: exactly 0 outside the window; errs["energies"] = the worst absolute error over the largest magnitude."""
+    e, we = np.asarray(e, np.float64), np.asarray(we, np.float64)
+    assert not np.any(e[we == 0]), "non-zero energies outside the window"
+    errs["energies"] = float(np.abs(e - we).max() / max(np.abs(we).max(), 1e-30))
 
 
 KINK_EPS = 2e-5      # > the float32 error of a readout pre-activation on the GPU (measured <= 5e-6 at T*B = 2048)
@@ -109,6 +150,39 @@ def check_grads(cfg, params, batch, tol=1e-4, atol_frac=1e-6):
             return algo, rec
         failures.append(bad)
     raise AssertionError(failures)
+
+
+def train_like_the_oracle(cfg, params, tc, steps=2, B=4, T=40):
+    """`steps` process_batch calls == as many oracle train_steps (float64) on the same batches: after every step the
+    cost, the gradient norm and every parameter agree.  Returns (recognizer, oracle parameters, oracle gradient norms)."""
+    from collections import OrderedDict
+    from oracle import lvsr_oracle_grad as G
+    pkg = package()
+    reg = dict(max_norm=tc["max_norm"])
+    rec = make_recognizer(cfg, params)
+    algo = pkg.GradientDescent(recognizer=rec, step_rule=pkg.step_rule_from_config(tc, reg), decay=tc["decay"])
+    algo.initialize()
+    ref = OrderedDict((k, v.copy()) for k, v in params.items())
+    state, norms = {}, []
+    for step in range(steps):
+        batch = O.synthetic_batch(cfg, B=B, T=T, seed=100 + step)
+        # last_cost is sequence_total_cost, the cost without the decay term (GradientDescent's docstring)
+        penalty = tc["decay"] * sum(float((v ** 2).sum()) for k, v in ref.items() if G.is_weight(k))
+        ref, ref_cost, ref_grads = G.train_step(cfg, ref, state, batch, tc)
+        want_cost = ref_cost - penalty
+        algo.process_batch(dict(zip(algo.SOURCES, batch)))
+        assert abs(float(algo.last_cost.item()) - want_cost) <= 1e-4 * abs(want_cost), (step, algo.last_cost.item(), want_cost)
+        norms.append(G.l2_norm(ref_grads.values()))
+        assert abs(algo.total_gradient_norm() - norms[-1]) <= 1e-4 * norms[-1]
+        got = rec.get_parameter_values()
+        for k, v in ref.items():
+            # compare the UPDATE (new - old would cancel; the parameters themselves are O(0.1..1))
+            assert np.abs(got[k] - v).max() <= 2e-5 * max(1.0, np.abs(v).max()) + 1e-6, (step, k, np.abs(got[k] - v).max())
+    if tc["max_norm"] > 0:
+        for k, v in rec.get_parameter_values().items():
+            if G.is_weight(k):
+                assert (np.sqrt((v.astype(np.float64) ** 2).sum(axis=0)) <= tc["max_norm"] * (1 + 1e-5)).all(), k
+    return rec, ref, norms
 
 
 def rel_err(got, want):

@@ -30,6 +30,8 @@ import pytest
 
 import content_oracle as CO
 from helpers import O, check_grads, make_recognizer, package
+from helpers import check_energies as _check_energies, check_weights as _check_weights
+from helpers import elementwise_err as _elementwise, f32 as _f32
 
 pytestmark = pytest.mark.gpu
 
@@ -66,10 +68,6 @@ def _torch():
 def _tp(cs, extra=3):
     """Smallest T' with ceil(T'/cs) >= 16 (the planners' rule for cs > 1), plus `extra` so it is not a multiple of cs."""
     return max(16 * cs, 24) + extra
-
-
-def _f32(a):
-    return np.asarray(a, dtype=np.float32).astype(np.float64)
 
 
 def _params(cfg, seed, content=False, normalizer="softmax"):
@@ -139,33 +137,6 @@ def _assert_plan(plan, cs, layout, kernel, B, what):
         assert plan["nisl"] == -(-B // 16) and plan["grid"] == B * plan["cs"] and plan["nrg"] == 1, (what, plan)
     elif layout == "global":
         assert plan["nisl"] == 0 and plan["nrg"] == -(-B // 16) and plan["grid"] >= B * plan["cs"], (what, plan)
-
-
-def _elementwise(got, want, floor=FLOOR):
-    got, want = np.asarray(got, np.float64), np.asarray(want, np.float64)
-    scale = np.abs(want).max()
-    return float((np.abs(got - want) / (np.abs(want) + floor * max(scale, 1e-30))).max())
-
-
-def _check_weights(w, ww, errs, key="weights"):
-    w, ww = np.asarray(w, np.float64), np.asarray(ww, np.float64)
-    zero = ww == 0
-    assert not np.any(w[zero]), "%s: %d non-zero weights where the oracle's are 0 (outside the window or masked)" % (
-        key, int(np.count_nonzero(w[zero])))
-    tiny = (ww > 0) & (ww < 1e-30)
-    assert np.all(np.abs(w[tiny]) < 1e-29), key
-    big = ww >= 1e-30
-    errs[key] = float((np.abs(w[big] - ww[big]) / ww[big]).max()) if big.any() else 0.0
-    s, sw = w.sum(-1), ww.sum(-1)
-    valid = sw > 0.5                                # rows with a valid position sum to 1 in the oracle, others to 0
-    assert np.all(s[~valid] == 0), key
-    errs[key + "_sum"] = float(np.abs(s[valid] - 1).max()) if valid.any() else 0.0
-
-
-def _check_energies(e, we, errs):
-    e, we = np.asarray(e, np.float64), np.asarray(we, np.float64)
-    assert not np.any(e[we == 0]), "non-zero energies outside the window"
-    errs["energies"] = float(np.abs(e - we).max() / max(np.abs(we).max(), 1e-30))
 
 
 def _compare(got, want, content, what):

@@ -1,12 +1,10 @@
 """Training step on the GPU against the gradient / optimizer oracle (oracle/lvsr_oracle_grad.py):
 gradients of every parameter (1e-4 of the parameter's largest gradient entry + a small absolute floor),
 the cost, and parameters after updates with the step-rule chain of lvsr/main.py:480-519."""
-from collections import OrderedDict
-
 import numpy as np
 import pytest
 
-from helpers import O, PYRAMID, WSJ, make_recognizer, package
+from helpers import O, PYRAMID, WSJ, make_recognizer, package, train_like_the_oracle
 from helpers import check_grads as _check_grads
 from oracle import lvsr_oracle_grad as G
 
@@ -55,37 +53,6 @@ def test_gradients_island_batch_no_masks():
     assert plan["ran"] and plan["nisl"] == 2 and plan["cs"] == 1, plan
 
 
-def _train_like_the_oracle(cfg, params, tc, steps=2, B=4, T=40):
-    """`steps` process_batch calls == as many oracle train_steps (float64) on the same batches: after every step the
-    cost, the gradient norm and every parameter agree.  Returns (recognizer, oracle parameters, oracle gradient norms)."""
-    pkg = package()
-    reg = dict(max_norm=tc["max_norm"])
-    rec = make_recognizer(cfg, params)
-    algo = pkg.GradientDescent(recognizer=rec, step_rule=pkg.step_rule_from_config(tc, reg), decay=tc["decay"])
-    algo.initialize()
-    ref = OrderedDict((k, v.copy()) for k, v in params.items())
-    state, norms = {}, []
-    for step in range(steps):
-        batch = O.synthetic_batch(cfg, B=B, T=T, seed=100 + step)
-        # last_cost is sequence_total_cost, the cost without the decay term (GradientDescent's docstring)
-        penalty = tc["decay"] * sum(float((v ** 2).sum()) for k, v in ref.items() if G.is_weight(k))
-        ref, ref_cost, ref_grads = G.train_step(cfg, ref, state, batch, tc)
-        want_cost = ref_cost - penalty
-        algo.process_batch(dict(zip(algo.SOURCES, batch)))
-        assert abs(float(algo.last_cost.item()) - want_cost) <= 1e-4 * abs(want_cost), (step, algo.last_cost.item(), want_cost)
-        norms.append(G.l2_norm(ref_grads.values()))
-        assert abs(algo.total_gradient_norm() - norms[-1]) <= 1e-4 * norms[-1]
-        got = rec.get_parameter_values()
-        for k, v in ref.items():
-            # compare the UPDATE (new - old would cancel; the parameters themselves are O(0.1..1))
-            assert np.abs(got[k] - v).max() <= 2e-5 * max(1.0, np.abs(v).max()) + 1e-6, (step, k, np.abs(got[k] - v).max())
-    if tc["max_norm"] > 0:
-        for k, v in rec.get_parameter_values().items():
-            if G.is_weight(k):
-                assert (np.sqrt((v.astype(np.float64) ** 2).sum(axis=0)) <= tc["max_norm"] * (1 + 1e-5)).all(), k
-    return rec, ref, norms
-
-
 def _params_with_long_filter_columns(cfg, max_norm):
     """Trained-like parameters whose conv filters have columns (axis 0) both longer and shorter than max_norm."""
     params = O.init_params(cfg, seed=5, scale=10.0)
@@ -105,7 +72,7 @@ def test_training_steps_match_oracle(rules, max_norm):
     params = O.init_params(cfg, seed=5, scale=10.0)
     tc = G.make_train_config(gradient_threshold=2.0, rules=rules, scale=0.05, momentum=0.5, decay_rate=0.95,
                              epsilon=1e-6, max_norm=max_norm)
-    rec, ref, _ = _train_like_the_oracle(cfg, params, tc)
+    rec, ref, _ = train_like_the_oracle(cfg, params, tc)
     # the forward pass uses the updated (re-packed) weights
     x, m, labels, lm = O.synthetic_batch(cfg, B=3, T=32, seed=5)
     want = O.recognizer_cost(cfg, ref, x, m, labels, lm)
@@ -121,7 +88,7 @@ def test_max_norm_clips_weights_but_not_the_conv_filters():
     params = _params_with_long_filter_columns(cfg, 1.0)
     tc = G.make_train_config(gradient_threshold=2.0, rules=("momentum", "adadelta"), scale=0.05, momentum=0.5,
                              decay_rate=0.95, epsilon=1e-6, max_norm=1.0)
-    rec, ref, _ = _train_like_the_oracle(cfg, params, tc)
+    rec, ref, _ = train_like_the_oracle(cfg, params, tc)
     got = rec.get_parameter_values()[FILTERS].astype(np.float64)
     assert (np.sqrt((got[:, ::2] ** 2).sum(axis=0)) > 2.5).all()           # still far above max_norm
 
@@ -134,7 +101,7 @@ def test_weight_decay_with_momentum_adadelta_and_max_norm():
     params = _params_with_long_filter_columns(cfg, 1.0)
     tc = G.make_train_config(gradient_threshold=2.0, rules=("momentum", "adadelta"), scale=0.05, momentum=0.5,
                              decay_rate=0.95, epsilon=1e-6, max_norm=1.0, decay=0.01)
-    _train_like_the_oracle(cfg, params, tc)
+    train_like_the_oracle(cfg, params, tc)
 
 
 @pytest.mark.parametrize("threshold,active", [(1e-3, True), (1e6, False)], ids=["always_clipped", "never_clipped"])
@@ -145,7 +112,7 @@ def test_step_clipping_active_and_inactive(threshold, active):
     cfg = O.make_config(**PYRAMID)
     params = O.init_params(cfg, seed=5, scale=10.0)
     tc = G.make_train_config(gradient_threshold=threshold, rules=("momentum",), scale=0.05, momentum=0.5, max_norm=0.0)
-    _, _, norms = _train_like_the_oracle(cfg, params, tc)
+    _, _, norms = train_like_the_oracle(cfg, params, tc)
     assert all((n > 100 * threshold) if active else (n < threshold / 100) for n in norms), norms
 
 
