@@ -19,6 +19,12 @@ ATTENTION_TYPES = {"content_and_conv": 0, "content": 1}
 PLAN_SLOTS = ("ran", "kernel", "cs", "grid", "nisl", "nrg", "ncg", "nc1", "nc2", "nc3", "tc_cap", "wh_rows", "red_alias",
               "att_cs", "max_clusters")
 PLAN_KERNELS = ("stepwise", "dec_scan", "dec_scan<COMPACT>", "dec_content")
+# slots of lvsr_model_encoder_plan's report (LVSR_ENC_*), the GEMM paths (LVSR_ENC_PATH_*) and the scan kernels
+# (LVSR_ENC_BIGRU_*)
+ENC_PLAN_SLOTS = ("proj", "kpad", "bigru", "tape", "rb", "cs", "clusters", "resident", "waves", "T", "bwd_cs", "wgrad",
+                  "wgrad_splits", "wgrad_kpad", "dx")
+ENC_PATHS = (None, "tc", "ffma")
+ENC_BIGRU_KERNELS = (None, "ffma", "mma")
 
 
 class LvsrConfig(C.Structure):
@@ -89,6 +95,7 @@ SIGNATURES = {
     "lvsr_model_finalize": (C.c_int, [_P]),
     "lvsr_model_status": (C.c_int, [_P, C.POINTER(C.c_int32), C.POINTER(C.c_int64)]),
     "lvsr_model_decoder_plan": (C.c_int, [_P, C.POINTER(C.c_int32)]),
+    "lvsr_model_encoder_plan": (C.c_int, [_P, _I, C.POINTER(C.c_int32)]),
     "lvsr_encoded_length": (C.c_int, [_P, _I]),
     "lvsr_encoded_dim": (C.c_int, [_P]),
     "lvsr_encoder_forward": (C.c_int, [_P, _P, _P, _I, _I, _P, _P, _P]),

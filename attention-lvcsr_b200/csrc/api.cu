@@ -266,7 +266,7 @@ size_t cost_ws_bytes(const lvsr_model* m, int Tp, int B, int L) {
 extern "C" {
 
 const char* lvsr_last_error(void) { return g_last_error.c_str(); }
-int lvsr_version(void) { return 103; }
+int lvsr_version(void) { return 104; }
 int64_t lvsr_launch_count(int reset) {
   const int64_t v = g_launch_count;
   if (reset) g_launch_count = 0;
@@ -411,6 +411,17 @@ int lvsr_model_decoder_plan(const lvsr_model* m, int32_t out[16]) {
   LVSR_CHECK(m && out, "null argument");
   for (int i = 0; i < 16; ++i) out[i] = m->dec_plan[i];
   out[LVSR_PLAN_ATT_CS] = m->att_cs;
+  return 0;
+}
+
+int lvsr_model_encoder_plan(const lvsr_model* m, int32_t layer, int32_t out[16]) {
+  LVSR_CHECK(m && out, "null argument");
+  LVSR_CHECK(layer >= -1 && layer < m->cfg.num_layers, "encoder_plan: layer %d outside [-1, %d)", layer, m->cfg.num_layers);
+  for (int i = 0; i < 16; ++i) out[i] = layer >= 0 ? m->enc_plan[layer][i] : 0;
+  if (layer < 0) {
+    out[LVSR_ENC_PROJ] = m->pre_plan[0];
+    out[LVSR_ENC_KPAD] = m->pre_plan[1];
+  }
   return 0;
 }
 
@@ -634,13 +645,15 @@ int finalize_on_stream(lvsr_model* m, cudaStream_t st, bool synchronise) {
 // enqueued, and the caller decides when to rewind it (lvsr_cost_matrix allocates the persistent decoder's buffers behind
 // it, and their place in the workspace is part of the decoder's measured step time).
 int projection_gemm(Arena& ws, const float* A, int M, int K, const float* W, const float* W_hi, const float* W_lo, int N,
-                    const float* bias, float* out, cudaStream_t st) {
+                    const float* bias, float* out, cudaStream_t st, int* kpad) {
   if (W_hi && gemm_tc_supported(M, N, K)) {
     float* a_hi = ws.f32((size_t)M * gemm_tc_kpad(K));
     float* a_lo = ws.f32((size_t)M * gemm_tc_kpad(K));
     LVSR_CHECK(a_hi && a_lo, "out of device memory (tf32 split scratch)");
+    if (kpad) *kpad = gemm_tc_kpad(K);
     return gemm_tc(A, a_hi, a_lo, M, K, W_hi, W_lo, N, bias, out, N, st);
   }
+  if (kpad) *kpad = 0;
   return gemm_bias(make_gemm(A, M, K, W, N, bias, out), st);
 }
 
@@ -651,6 +664,8 @@ int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int
   int Tl = T, din = c.num_features;
   long long mstride = B;
   int kcum = 1;
+  for (int l = 0; l < c.num_layers; ++l)
+    for (int s = LVSR_ENC_PROJ; s <= LVSR_ENC_T; ++s) m->enc_plan[l][s] = 0;
   for (int l = 0; l < c.num_layers; ++l) {
     const int D = c.dims_bidir[l], k = c.subsample[l];
     const int rows = Tl * B, Tout = ceil_div(Tl, k);
@@ -659,9 +674,13 @@ int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int
     LVSR_CHECK(pre && (hext || !tape), "out of device memory (encoder pre-activations)");
     // finalize splits the fork weights only while the tensor-core GEMM is on (null entry: a shape it refuses)
     const size_t mark = ws.off;
+    int32_t* plan = m->enc_plan[l];
+    int kpad = 0;
     if (int rc = projection_gemm(ws, cur, rows, din, m->Wcat[l], m->use_tc ? m->Wcat_hi[l] : nullptr,
-                                 m->use_tc ? m->Wcat_lo[l] : nullptr, 6 * D, m->bcat[l], pre, st))
+                                 m->use_tc ? m->Wcat_lo[l] : nullptr, 6 * D, m->bcat[l], pre, st, &kpad))
       return rc;
+    plan[LVSR_ENC_PROJ] = kpad ? LVSR_ENC_PATH_TC : LVSR_ENC_PATH_FFMA;
+    plan[LVSR_ENC_KPAD] = kpad;
     if (ws.off <= ws.cap) ws.off = mark;     // the split scratch is dead once the GEMM is enqueued (stream order)
     float* out = (l == c.num_layers - 1) ? attended : ws.f32((size_t)Tout * B * 2 * D);
     LVSR_CHECK(out, "out of device memory (encoder layer output)");
@@ -675,7 +694,16 @@ int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int
       a.tape = pre; a.hext = hext;
       tape[l] = {cur, pre, hext, out, Tl, Tout, din, D, k, mstride};
     }
-    if (int rc = bigru_layer(a, st)) return rc;
+    BiGruPlan bp;
+    if (int rc = bigru_layer(a, st, &bp)) return rc;
+    plan[LVSR_ENC_BIGRU] = bp.kernel;
+    plan[LVSR_ENC_TAPE] = tape ? 1 : 0;
+    plan[LVSR_ENC_RB] = bp.rb;
+    plan[LVSR_ENC_CS] = bp.cs;
+    plan[LVSR_ENC_CLUSTERS] = bp.clusters;
+    plan[LVSR_ENC_RESIDENT] = bp.resident;
+    plan[LVSR_ENC_WAVES] = bp.waves;
+    plan[LVSR_ENC_T] = Tl;
     cur = out; Tl = Tout; din = 2 * D; mstride *= k; kcum *= k;
   }
   if (mask) {
@@ -714,8 +742,15 @@ int lvsr_preprocess(lvsr_model* m, const float* attended, int32_t Tp, int32_t U,
   LVSR_CHECK(attended && out && Tp > 0 && U > 0, "preprocess: bad arguments");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   ArenaScope scope(m, st);
-  return projection_gemm(m->ws, attended, Tp * U, m->E, m->P(att_base(m) + "/preprocess.W"), m->use_tc ? m->Wp_hi : nullptr,
-                         m->Wp_lo, m->cfg.dim_matcher, m->P(att_base(m) + "/preprocess.b"), out, st);
+  int kpad = 0;
+  m->pre_plan[0] = m->pre_plan[1] = 0;
+  if (int rc = projection_gemm(m->ws, attended, Tp * U, m->E, m->P(att_base(m) + "/preprocess.W"),
+                               m->use_tc ? m->Wp_hi : nullptr, m->Wp_lo, m->cfg.dim_matcher,
+                               m->P(att_base(m) + "/preprocess.b"), out, st, &kpad))
+    return rc;
+  m->pre_plan[0] = kpad ? LVSR_ENC_PATH_TC : LVSR_ENC_PATH_FFMA;
+  m->pre_plan[1] = kpad;
+  return 0;
 }
 
 int lvsr_cost_matrix(lvsr_model* m, const float* attended, const float* attended_mask, int32_t Tp, int32_t B,

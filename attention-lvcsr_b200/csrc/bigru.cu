@@ -29,6 +29,7 @@
 #include <cuda_fp16.h>
 
 #include "kernels.h"
+#include "lvsr_b200.h"
 
 namespace lvsr {
 
@@ -378,9 +379,43 @@ bigru_kernel(BiGruArgs a) {
   cluster_sync_all();
 }
 
+// dynamic shared memory of bigru_kernel<D, CS, NWARP, *>
+template <int D, int NWARP>
+constexpr size_t ffma_smem_bytes() { return (size_t)NWARP * (D / 16 / 4) * 2 * 32 * 4 * sizeof(float); }
+
+// how many clusters of the FFMA kernel the device holds at once (encoder plan report only: the FFMA kernel is never
+// chosen by it)
 template <int D, int CS, int NWARP, bool TAPE>
-int launch_bigru_t(const BiGruArgs& a, cudaStream_t stream) {
-  constexpr size_t W2S_BYTES = (size_t)NWARP * (D / 16 / 4) * 2 * 32 * 4 * sizeof(float);
+int ffma_clusters_resident() {
+  static int per_dev[LVSR_MAX_DEVICES];
+  static bool known[LVSR_MAX_DEVICES] = {false};
+  const int dev = current_device();
+  if (!known[dev]) {
+    known[dev] = true;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(CS * 64);
+    cfg.blockDim = dim3(NWARP * 32);
+    cfg.dynamicSmemBytes = ffma_smem_bytes<D, NWARP>();
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = CS;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    int k = 0;
+    if (cudaOccupancyMaxActiveClusters(&k, bigru_kernel<D, CS, NWARP, TAPE>, &cfg) != cudaSuccess) {
+      cudaGetLastError();
+      k = 0;
+    }
+    per_dev[dev] = k;
+  }
+  return per_dev[dev];
+}
+
+template <int D, int CS, int NWARP, bool TAPE>
+int launch_bigru_t(const BiGruArgs& a, cudaStream_t stream, BiGruPlan* plan) {
+  constexpr size_t W2S_BYTES = ffma_smem_bytes<D, NWARP>();
   static bool configured[LVSR_MAX_DEVICES] = {false};
   const int dev = current_device();
   if (!configured[dev]) {
@@ -408,6 +443,10 @@ int launch_bigru_t(const BiGruArgs& a, cudaStream_t stream) {
   }
   LVSR_CUDA_OK(cudaLaunchKernelEx(&cfg, bigru_kernel<D, CS, NWARP, TAPE>, a));
   g_launch_count++;
+  if (plan) {
+    const int resident = ffma_clusters_resident<D, CS, NWARP, TAPE>();
+    *plan = {LVSR_ENC_BIGRU_FFMA, RB, CS, 2 * groups, resident, resident > 0 ? ceil_div(2 * groups, resident) : 0};
+  }
   if (trace) {
     unsigned long long h[8] = {0};
     LVSR_CUDA_OK(cudaMemcpyFromSymbolAsync(h, g_bigru_trace, sizeof(h), 0, cudaMemcpyDeviceToHost, stream));
@@ -933,9 +972,9 @@ bigru_mma_kernel(BiGruArgs a) {
 }
 
 template <int D, int CS, int NWARP>
-int launch_bigru(const BiGruArgs& a, cudaStream_t stream) {
+int launch_bigru(const BiGruArgs& a, cudaStream_t stream, BiGruPlan* plan) {
   LVSR_CHECK((a.tape == nullptr) == (a.hext == nullptr), "bigru: tape and hext go together");
-  return a.tape ? launch_bigru_t<D, CS, NWARP, true>(a, stream) : launch_bigru_t<D, CS, NWARP, false>(a, stream);
+  return a.tape ? launch_bigru_t<D, CS, NWARP, true>(a, stream, plan) : launch_bigru_t<D, CS, NWARP, false>(a, stream, plan);
 }
 
 template <int D, bool TAPE>
@@ -1027,17 +1066,21 @@ int launch_bigru_mma_t(const BiGruArgs& a, cudaStream_t stream) {
 }
 
 template <int D, int RB>
-int launch_bigru_mma(const BiGruArgs& a, cudaStream_t stream) {
+int launch_bigru_mma(const BiGruArgs& a, cudaStream_t stream, BiGruPlan* plan) {
   LVSR_CHECK((a.tape == nullptr) == (a.hext == nullptr), "bigru: tape and hext go together");
-  return a.tape ? launch_bigru_mma_t<D, true, RB>(a, stream) : launch_bigru_mma_t<D, false, RB>(a, stream);
+  if (int rc = a.tape ? launch_bigru_mma_t<D, true, RB>(a, stream) : launch_bigru_mma_t<D, false, RB>(a, stream)) return rc;
+  if (plan)
+    *plan = {LVSR_ENC_BIGRU_MMA, RB, MMA_CS, ceil_div(a.B, RB) * 2, mma_clusters_resident<D, RB>(), mma_waves<D, RB>(a.B)};
+  return 0;
 }
 
 }  // namespace
 
 bool bigru_supported(int D) { return D == 128 || D == 256; }
 
-int bigru_layer(const BiGruArgs& a, cudaStream_t stream) {
+int bigru_layer(const BiGruArgs& a, cudaStream_t stream, BiGruPlan* plan) {
   ProfScope prof("bigru", stream);
+  if (plan) *plan = {};
   if (a.T <= 0 || a.B <= 0) return 0;
   // hidden size 256: tensor-core products.  Clusters never talk to each other, so a batch with more clusters than the
   // device holds at once (mma_clusters_resident, from the occupancy query) simply runs in waves -- still
@@ -1054,11 +1097,11 @@ int bigru_layer(const BiGruArgs& a, cudaStream_t stream) {
       rb = atoi(e);
       if (rb != 4 && rb != 8) return set_error("bigru: LVSR_BIGRU_RB=%s (expected 4 or 8)", e);
     }
-    return rb == 8 ? launch_bigru_mma<256, 8>(a, stream) : launch_bigru_mma<256, 4>(a, stream);
+    return rb == 8 ? launch_bigru_mma<256, 8>(a, stream, plan) : launch_bigru_mma<256, 4>(a, stream, plan);
   }
   switch (a.D) {
-    case 128: return launch_bigru<128, 4, 8>(a, stream);
-    case 256: return launch_bigru<256, 8, 8>(a, stream);
+    case 128: return launch_bigru<128, 4, 8>(a, stream, plan);
+    case 256: return launch_bigru<256, 8, 8>(a, stream, plan);
     default:
       return set_error("bigru: unsupported hidden size %d (supported: 128, 256)", a.D);
   }

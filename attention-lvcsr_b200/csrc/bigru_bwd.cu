@@ -281,9 +281,11 @@ int launch_bwd(const BiGruBwdArgs& a, cudaStream_t stream) {
 
 }  // namespace
 
-int bigru_layer_backward(const BiGruBwdArgs& a, cudaStream_t stream) {
+int bigru_layer_backward(const BiGruBwdArgs& a, cudaStream_t stream, int* cs_out) {
   ProfScope prof("bigru_bwd", stream);
+  if (cs_out) *cs_out = 0;
   if (a.T <= 0 || a.B <= 0) return 0;
+  if (cs_out && bigru_supported(a.D)) *cs_out = a.D / UC;
   switch (a.D) {
     case 128: return launch_bwd<128, 4>(a, stream);
     case 256: return launch_bwd<256, 8>(a, stream);

@@ -55,7 +55,10 @@ struct BiGruArgs {
                            // (backward half) = the broadcast initial states
 };
 bool bigru_supported(int D);
-int bigru_layer(const BiGruArgs& a, cudaStream_t stream);
+// what bigru_layer launched (lvsr_model_encoder_plan): kernel LVSR_ENC_BIGRU_*, rows and CTAs per cluster, clusters,
+// the clusters of that kernel the device holds at once (occupancy query) and the waves that makes
+struct BiGruPlan { int kernel, rb, cs, clusters, resident, waves; };
+int bigru_layer(const BiGruArgs& a, cudaStream_t stream, BiGruPlan* plan = nullptr);
 
 // ---- bigru_bwd.cu: reverse-time scan of one layer (training) ------------------------------
 struct BiGruBwdArgs {
@@ -69,7 +72,7 @@ struct BiGruBwdArgs {
   float* dh0;              // [2, B, D]: gradient of the broadcast initial state, per direction and row
   int T, B, D, subsample;
 };
-int bigru_layer_backward(const BiGruBwdArgs& a, cudaStream_t stream);
+int bigru_layer_backward(const BiGruBwdArgs& a, cudaStream_t stream, int* cs_out = nullptr);   // *cs_out: CTAs per cluster
 
 // ---- attention.cu -------------------------------------------------------------------
 struct PriorParams {

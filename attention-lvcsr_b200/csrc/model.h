@@ -127,6 +127,8 @@ struct lvsr_model {
   long long dec_fallbacks = 0;      // how often that happened
   int32_t dec_plan[16] = {0};       // plan of the last lvsr_cost_matrix (lvsr_model_decoder_plan, LVSR_PLAN_* slots)
   int att_cs = 0;                   // cluster size of the last attention_step launch
+  int32_t enc_plan[LVSR_MAX_LAYERS][16] = {};   // per layer: lvsr_model_encoder_plan's LVSR_ENC_* slots
+  int32_t pre_plan[2] = {0, 0};     // last lvsr_preprocess: path (LVSR_ENC_PATH_*), Kpad
   bool finalized = false;
   // ---- FST language model (lvsr_model_set_lm); lm_off == nullptr: none attached ----
   long long* lm_off = nullptr;
@@ -225,6 +227,10 @@ int finalize_on_stream(lvsr_model* m, cudaStream_t st, bool synchronise);
 // the training stores; with one, tape[l] records layer l's buffers (and allocates hext) for the backward pass.
 int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int T, int B, float* attended,
                 float* attended_mask, LayerTape* tape, cudaStream_t st);
+// out[M, N] = A[M, K] . W + bias on the tensor cores when W_hi / W_lo are given and the shape suits them, else on FFMA
+// tiles; *kpad (may be null) = the contraction as the tensor-core GEMM stored it, 0 on FFMA
+int projection_gemm(Arena& ws, const float* A, int M, int K, const float* W, const float* W_hi, const float* W_lo, int N,
+                    const float* bias, float* out, cudaStream_t st, int* kpad = nullptr);
 int readout_merged(lvsr_model* m, int R, const float* states, const float* ctx, float* merged, cudaStream_t st);
 ReadoutArgs readout_args(lvsr_model* m, int R, const float* merged);
 // language model (api.cu): the device view of the attached FST, the fusion fields of a readout, and the LM status

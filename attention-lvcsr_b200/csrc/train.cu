@@ -33,15 +33,17 @@ inline int grid1d(long long n, int block = 256, int cap = 2048) {
   return (int)std::min<long long>(cap, std::max<long long>(1, (n + block - 1) / block));
 }
 
-// C[Mo,N] (ldc) (+)= A[:, m-cols]^T . B over R rows
+// C[Mo,N] (ldc) (+)= A[:, m-cols]^T . B over R rows; *splits_out (may be null) = the partial products of the R rows
 int gemm_tn(Arena& ws, const float* A, int lda, const float* B, int ldb, int R, int Mo, int N, float* C, int ldc,
-            bool accumulate, cudaStream_t st) {
+            bool accumulate, cudaStream_t st, int* splits_out = nullptr) {
   ProfScope prof("gemm_tn", st);
+  if (splits_out) *splits_out = 0;
   if (R <= 0 || Mo <= 0 || N <= 0) return 0;
   const int tiles = ceil_div(Mo, TN_BM) * ceil_div(N, TN_BN);
   int splits = std::max(1, std::min(ceil_div(2 * device_sm_count(), tiles), ceil_div(R, 4 * TN_BK)));
   int rps = ceil_div(ceil_div(R, splits), TN_BK) * TN_BK;
   splits = ceil_div(R, rps);
+  if (splits_out) *splits_out = splits;
   const size_t mark = ws.off;
   float* part = ws.f32((size_t)splits * Mo * N);
   LVSR_CHECK(part, "out of device memory (TN partials)");
@@ -117,13 +119,15 @@ int make_tc_operand(Arena& ws, const float* src, int R, int cols, int ld, TcOper
 }
 
 // C[Mo, N] (ldc) (+)= A^T B on the tensor cores: A, B given as K-major operands (rows a0.. / b0..), split-K over the
-// contraction (R) so that every SM gets a tile; partials are summed in a fixed order.
+// contraction (R) so that every SM gets a tile; partials are summed in a fixed order.  *splits_out (may be null) = the
+// partial products launched.
 int gemm_tn_tc(Arena& ws, const TcOperand& A, int a0, int Mo, const TcOperand& B, int b0, int N, float* C, int ldc,
-               bool accumulate, cudaStream_t st) {
+               bool accumulate, cudaStream_t st, int* splits_out = nullptr) {
   ProfScope prof("gemm_tn", st);
   const int tiles = ceil_div(Mo, 128) * (N / (N % 256 == 0 ? 256 : 128));
   const int want = std::max(1, std::min(32, ceil_div(device_sm_count(), tiles)));
   const int splits = gemm_tc_splits_launched(A.Kpad, want);
+  if (splits_out) *splits_out = splits;
   const size_t mark = ws.off;
   float* part = ws.f32((size_t)splits * Mo * N);
   LVSR_CHECK(part, "out of device memory (TN partials)");
@@ -185,6 +189,8 @@ int lvsr_train_cost_and_grads(lvsr_model* m, const float* x, const float* mask, 
     ws.reserve(bytes, st);
   }
   ArenaScope scope(ws, st);
+  for (int l = 0; l < c.num_layers; ++l)
+    for (int s = LVSR_ENC_BWD_CS; s <= LVSR_ENC_DX; ++s) m->enc_plan[l][s] = 0;
   LVSR_CUDA_OK(cudaMemsetAsync(grads, 0, (size_t)m->flat_count * sizeof(float), st));
 
   // =========================== forward, keeping the tape ===========================
@@ -451,7 +457,10 @@ int lvsr_train_cost_and_grads(lvsr_model* m, const float* x, const float* mask, 
     a.Wg_f = m->P(bf + "/gatedrecurrent.state_to_gates"); a.Ws_f = m->P(bf + "/gatedrecurrent.state_to_state");
     a.Wg_b = m->P(bb + "/gatedrecurrent.state_to_gates"); a.Ws_b = m->P(bb + "/gatedrecurrent.state_to_state");
     a.hr_out = hr; a.dh0 = dh0; a.T = tp.T; a.B = B; a.D = D; a.subsample = tp.k;
-    if (int rc = bigru_layer_backward(a, st)) return rc;
+    int32_t* plan = m->enc_plan[l];
+    int bwd_cs = 0, wsplits = 0;
+    if (int rc = bigru_layer_backward(a, st, &bwd_cs)) return rc;
+    plan[LVSR_ENC_BWD_CS] = bwd_cs;
     // fork: dWcat = X^T dPre, dbcat = colsum(dPre); columns per direction [inputs D | gate_inputs 2D]
     {
       const size_t mark = ws.off;
@@ -470,10 +479,13 @@ int lvsr_train_cost_and_grads(lvsr_model* m, const float* x, const float* mask, 
           const float* hprev = tp.hext + (size_t)(dir ? 2 : 0) * B * 2 * D + dir * D;
           if (int rc = make_tc_operand(ws, hprev, rows, D, 2 * D, &hpT[dir], st)) return rc;
         }
-        if (int rc = gemm_tn_tc(ws, XT, 0, tp.Din, dPreT, 0, 6 * D, dWcat, 6 * D, false, st)) return rc;
+        if (int rc = gemm_tn_tc(ws, XT, 0, tp.Din, dPreT, 0, 6 * D, dWcat, 6 * D, false, st, &wsplits)) return rc;
       } else {
-        if (int rc = gemm_tn(ws, tp.X, tp.Din, tp.pre, 6 * D, rows, tp.Din, 6 * D, dWcat, 6 * D, false, st)) return rc;
+        if (int rc = gemm_tn(ws, tp.X, tp.Din, tp.pre, 6 * D, rows, tp.Din, 6 * D, dWcat, 6 * D, false, st, &wsplits)) return rc;
       }
+      plan[LVSR_ENC_WGRAD] = tc ? LVSR_ENC_PATH_TC : LVSR_ENC_PATH_FFMA;
+      plan[LVSR_ENC_WGRAD_SPLITS] = wsplits;
+      plan[LVSR_ENC_WGRAD_KPAD] = tc ? dPreT.Kpad : 0;
       if (int rc = colsum(tp.pre, rows, 6 * D, 6 * D, dbcat, false, st)) return rc;
       for (int dir = 0; dir < 2; ++dir) {
         const std::string b = enc_base(l, dir);
@@ -513,9 +525,11 @@ int lvsr_train_cost_and_grads(lvsr_model* m, const float* x, const float* mask, 
         if (int rc = split_tf32(m->Wcat[l], w_hi, w_lo, (long long)tp.Din * 6 * D, st)) return rc;
         if (int rc = gemm_tc(tp.pre, a_hi, a_lo, rows, 6 * D, w_hi, w_lo, tp.Din, nullptr, dX, tp.Din, st)) return rc;
         if (ws.off <= ws.cap) ws.off = mark;
+        plan[LVSR_ENC_DX] = LVSR_ENC_PATH_TC;
       } else {
         if (int rc = transpose(m->Wcat[l], WcatT, tp.Din, 6 * D, st)) return rc;
         if (int rc = gemm_nn(tp.pre, rows, 6 * D, 6 * D, WcatT, tp.Din, tp.Din, nullptr, dX, tp.Din, false, st)) return rc;
+        plan[LVSR_ENC_DX] = LVSR_ENC_PATH_FFMA;
       }
       dout = dX;
     }

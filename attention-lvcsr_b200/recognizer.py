@@ -432,6 +432,32 @@ class SpeechRecognizer(object):
         plan["kernel"] = _lib.PLAN_KERNELS[plan["kernel"]]
         return plan
 
+    def _encoder_plan_row(self, layer):
+        import ctypes as C
+        lib, h = _lib.load(), self._require_ready()
+        out = (C.c_int32 * 16)()
+        _lib.check(lib.lvsr_model_encoder_plan(h, int(layer), out))
+        plan = {k: int(out[i]) for i, k in enumerate(_lib.ENC_PLAN_SLOTS)}
+        for k in ("proj", "wgrad", "dx"):
+            plan[k] = _lib.ENC_PATHS[plan[k]]
+        plan["bigru"] = _lib.ENC_BIGRU_KERNELS[plan["bigru"]]
+        plan["tape"] = bool(plan["tape"])
+        return plan
+
+    def encoder_plan(self):
+        """What the encoder ran (lvsr_model_encoder_plan), one dict per layer.  Of the last encoder forward: proj (fork
+        projection GEMM: "tc" or "ffma"), kpad (its contraction as the tensor-core GEMM stores it, 0 on FFMA), bigru
+        ("mma" or "ffma"), tape (a training forward), rb and cs (rows and CTAs per cluster), clusters, resident (clusters
+        of that kernel the device holds at once), waves and T (frames scanned).  Of the last training step: bwd_cs
+        (CTAs per cluster of the reverse-time scan), wgrad ("tc" or "ffma"), wgrad_splits, wgrad_kpad (the padded
+        contraction over T*B rows, 0 on FFMA) and dx ("tc", "ffma", or None for layer 0).  None / 0: not run."""
+        return [self._encoder_plan_row(l) for l in range(len(self.net["dims_bidir"]))]
+
+    def preprocess_plan(self):
+        """Path of the last preprocess GEMM (lvsr_model_encoder_plan, layer -1): {"proj": "tc" | "ffma", "kpad": ...}."""
+        plan = self._encoder_plan_row(-1)
+        return {"proj": plan["proj"], "kpad": plan["kpad"]}
+
     def encoded_length(self, T):
         return int(_lib.load().lvsr_encoded_length(self._require_ready(), int(T)))
 

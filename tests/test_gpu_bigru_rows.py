@@ -33,12 +33,14 @@ def test_eight_row_clusters_agree_with_four_row_clusters(monkeypatch):
     rec = make_recognizer(cfg, params)
     monkeypatch.setenv("LVSR_BIGRU_MMA", "0")
     ffma = rec.encode(x, m)[0].clone()
+    assert [p["bigru"] for p in rec.encoder_plan()] == ["ffma"] * 4
     monkeypatch.setenv("LVSR_BIGRU_MMA", "1")
     got = {}
     for rb in (4, 8):
         monkeypatch.setenv("LVSR_BIGRU_RB", str(rb))
         got[rb] = rec.encode(x, m)[0].clone()
         assert bool(torch.isfinite(got[rb]).all()), rb
+        assert [(p["bigru"], p["rb"]) for p in rec.encoder_plan()] == [("mma", rb)] * 4
     scale = float(ffma.abs().max())
     d48 = float((got[8] - got[4]).abs().max()) / scale
     d4f, d8f = (float((got[rb] - ffma).abs().max()) / scale for rb in (4, 8))

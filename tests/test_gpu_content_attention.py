@@ -64,13 +64,13 @@ def _forward(rec, x, m, labels, lm):
     return att.cpu().numpy(), {k: v.cpu().numpy() for k, v in r.items()}
 
 
-def test_content_model_has_the_cont_att_parameter_table_at_abi_103():
+def test_content_model_has_the_cont_att_parameter_table_at_abi_104():
     _torch()
     cfg = _cfg(SMALL)
     rec = _make(cfg)
     assert list(rec.parameter_shapes().items()) == list(CO.param_shapes(cfg).items())
     assert rec.generator.transition.attention.name == "cont_att"
-    assert package()._lib.load().lvsr_version() == 103
+    assert package()._lib.load().lvsr_version() == 104
 
 
 @pytest.mark.parametrize("arch,B,T", [("SMALL", 16, 60), ("PYRAMID", 37, 80), ("WSJ", 64, 48)])

@@ -18,10 +18,13 @@ def _torch():
     return torch
 
 
-def _compare_cost(cfg, params, x, m, labels, lm):
+def _compare_cost(cfg, params, x, m, labels, lm, plan=None):
+    """plan (optional): called with the encoder plan report of the forward."""
     want = O.recognizer_cost(cfg, params, x, m, labels, lm, return_all=True)
     rec = make_recognizer(cfg, params)
     att, attm = rec.encode(x, m)
+    if plan is not None:
+        plan(rec.encoder_plan())
     o_att, o_mask = O.encoder(cfg, params, x, m)
     assert rel_err(att.cpu().numpy(), o_att) < TOL
     assert np.array_equal(attm.cpu().numpy(), o_mask.astype(np.float32))
@@ -91,7 +94,10 @@ def test_feature_width_not_a_multiple_of_4(B, T):
     cfg = O.make_config(**dict(PYRAMID, num_features=123))
     params = O.init_params(cfg, seed=11, scale=10.0)
     x, m, labels, lm = O.synthetic_batch(cfg, B=B, T=T, seed=B + T)
-    _compare_cost(cfg, params, x, m, labels, lm)
+
+    def both_paths(plan):
+        assert [p["proj"] for p in plan] == ["ffma", "tc", "tc"], plan
+    _compare_cost(cfg, params, x, m, labels, lm, plan=both_paths)
 
 
 def test_label_mask_freezes_states_after_the_end():
@@ -231,8 +237,10 @@ def test_tensor_core_bigru_agrees_with_the_fp32_kernel(monkeypatch):
     rec = make_recognizer(cfg, params)
     monkeypatch.setenv("LVSR_BIGRU_MMA", "0")
     ref = rec.encode(x, m)[0].clone()
+    assert [p["bigru"] for p in rec.encoder_plan()] == ["ffma"] * 4
     monkeypatch.setenv("LVSR_BIGRU_MMA", "1")
     got = rec.encode(x, m)[0]
+    assert [p["bigru"] for p in rec.encoder_plan()] == ["mma"] * 4
     err = float((got - ref).abs().max() / ref.abs().max())
     print("mma vs ffma bigru", err)
     assert bool(torch.isfinite(got).all()) and err < 1e-5

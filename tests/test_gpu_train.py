@@ -178,11 +178,14 @@ def test_gradients_with_tensor_core_backward_gemms(monkeypatch):
     batch = O.synthetic_batch(cfg, B=32, T=64, seed=77)
     algo, rec = _check_grads(cfg, params, batch)
     _, g_tc = algo.cost_and_gradients(dict(zip(algo.SOURCES, batch)))
+    # 2048 rows at layers 0 and 1, 1024 at layer 2
+    assert [(p["wgrad"], p["dx"]) for p in rec.encoder_plan()] == [("tc", None), ("tc", "tc"), ("ffma", "tc")]
     monkeypatch.setenv("LVSR_NO_TC_GEMM", "1")
     pkg = package()
     rec2 = make_recognizer(cfg, params)
     algo2 = pkg.GradientDescent(recognizer=rec2, step_rule=pkg.CompositeRule([pkg.RemoveNotFinite(0.0)]))
     _, g_ff = algo2.cost_and_gradients(dict(zip(algo2.SOURCES, batch)))
+    assert [(p["wgrad"], p["dx"]) for p in rec2.encoder_plan()] == [("ffma", None), ("ffma", "ffma"), ("ffma", "ffma")]
     for k in g_tc:
         scale = max(np.abs(g_ff[k]).max(), 1e-30)
         assert np.abs(g_tc[k] - g_ff[k]).max() / scale < 2e-4, k

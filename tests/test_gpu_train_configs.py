@@ -65,7 +65,8 @@ def test_encoder_stacks(dims, subsample):
 
 def test_feature_width_not_a_multiple_of_4():
     """123 features (WSJ fbank + deltas + double deltas): the first layer's fork GEMMs run on FFMA tiles."""
-    _check(num_features=123)
+    _, rec = _check(num_features=123)
+    assert [p["proj"] for p in rec.encoder_plan()] == ["ffma", "tc", "tc"]
 
 
 def test_odd_batch_with_a_one_frame_utterance():
