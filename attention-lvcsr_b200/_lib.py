@@ -19,11 +19,12 @@ ATTENTION_TYPES = {"content_and_conv": 0, "content": 1}
 PLAN_SLOTS = ("ran", "kernel", "cs", "grid", "nisl", "nrg", "ncg", "nc1", "nc2", "nc3", "tc_cap", "wh_rows", "red_alias",
               "att_cs", "max_clusters")
 PLAN_KERNELS = ("stepwise", "dec_scan", "dec_scan<COMPACT>", "dec_content")
-# slots of lvsr_model_encoder_plan's report (LVSR_ENC_*), the GEMM paths (LVSR_ENC_PATH_*) and the scan kernels
-# (LVSR_ENC_BIGRU_*)
+# slots of lvsr_model_encoder_plan's report (LVSR_ENC_*), the GEMM paths (LVSR_ENC_PATH_*), the operands of the
+# tensor-core projection (LVSR_ENC_OPS_*) and the scan kernels (LVSR_ENC_BIGRU_*)
 ENC_PLAN_SLOTS = ("proj", "kpad", "bigru", "tape", "rb", "cs", "clusters", "resident", "waves", "T", "bwd_cs", "wgrad",
-                  "wgrad_splits", "wgrad_kpad", "dx")
+                  "wgrad_splits", "wgrad_kpad", "dx", "operands")
 ENC_PATHS = (None, "tc", "ffma")
+ENC_OPERANDS = (None, "tf32x3", "f16x3")
 ENC_BIGRU_KERNELS = (None, "ffma", "mma")
 
 

@@ -375,10 +375,8 @@ int lvsr_model_destroy(lvsr_model* m) {
   if (m->flat) cudaFree(m->flat);
   for (float* p : m->Wcat) if (p) cudaFree(p);
   for (float* p : m->bcat) if (p) cudaFree(p);
-  for (float* p : m->Wcat_hi) if (p) cudaFree(p);
-  for (float* p : m->Wcat_lo) if (p) cudaFree(p);
-  if (m->Wp_hi) cudaFree(m->Wp_hi);
-  if (m->Wp_lo) cudaFree(m->Wp_lo);
+  for (TcWeights& t : m->Wcat_tc) if (t.mem) cudaFree(t.mem);
+  if (m->Wp_tc.mem) cudaFree(m->Wp_tc.mem);
   if (m->Wd_cat) cudaFree(m->Wd_cat);
   if (m->Wb1) cudaFree(m->Wb1);
   if (m->Wff_cat) cudaFree(m->Wff_cat);
@@ -421,6 +419,7 @@ int lvsr_model_encoder_plan(const lvsr_model* m, int32_t layer, int32_t out[16])
   if (layer < 0) {
     out[LVSR_ENC_PROJ] = m->pre_plan[0];
     out[LVSR_ENC_KPAD] = m->pre_plan[1];
+    out[LVSR_ENC_OPERANDS] = m->pre_plan[2];
   }
   return 0;
 }
@@ -545,6 +544,30 @@ int lvsr_lm_next_states(lvsr_model* m, int32_t R, const int32_t* states, const d
 }  // extern "C"
 
 namespace lvsr {
+// W [K, N] packed for the tensor-core GEMM into tw (allocated on first use): fp16 head/tail planes when K is a multiple
+// of 64 (the forward projections' operand kind, see projection_gemm), else tf32 hi/lo planes; shapes neither kernel
+// takes stay unpacked
+static int pack_tc_weights(TcWeights& tw, const float* W, int K, int N, cudaStream_t st) {
+  if (!tw.mem) {
+    if (gemm_f16_supported(128, N, K)) {
+      const size_t plane = (size_t)N * K * sizeof(__half);
+      LVSR_CUDA_OK(cudaMalloc(&tw.mem, 2 * plane + (size_t)N * sizeof(int)));
+      tw.head = static_cast<__half*>(tw.mem);
+      tw.tail = reinterpret_cast<__half*>(static_cast<char*>(tw.mem) + plane);
+      tw.ew = reinterpret_cast<int*>(static_cast<char*>(tw.mem) + 2 * plane);
+    } else if (gemm_tc_supported(128, N, K)) {
+      const size_t plane = (size_t)N * gemm_tc_kpad(K);
+      LVSR_CUDA_OK(cudaMalloc(&tw.mem, 2 * plane * sizeof(float)));
+      tw.hi = static_cast<float*>(tw.mem);
+      tw.lo = tw.hi + plane;
+    } else {
+      return 0;
+    }
+  }
+  if (tw.head) return split_weight_f16(W, K, N, tw.head, tw.tail, tw.ew, st);
+  return split_weight_tf32(W, K, N, tw.hi, tw.lo, st);
+}
+
 int finalize_on_stream(lvsr_model* m, cudaStream_t st, bool synchronise) {
   const lvsr_config& c = m->cfg;
   if (m->Wcat.empty()) {
@@ -590,37 +613,16 @@ int finalize_on_stream(lvsr_model* m, cudaStream_t st, bool synchronise) {
   if (int rc = copy_cols(m->Wff_cat, 3 * C, 2 * C, m->P(g + "/fork/fork_inputs.W"), Cfb, C, st)) return rc;
   if (int rc = copy_cols(m->bff_cat, 3 * C, 0, m->P(g + "/fork/fork_gate_inputs.b"), 1, 2 * C, st)) return rc;
   if (int rc = copy_cols(m->bff_cat, 3 * C, 2 * C, m->P(g + "/fork/fork_inputs.b"), 1, C, st)) return rc;
-  // tensor-core operands: K-major tf32 hi/lo pairs of the fork and preprocess weights
+  // tensor-core operands of the fork and preprocess weights (K-major fp16 head/tail planes or tf32 hi/lo pairs)
   m->use_tc = getenv("LVSR_NO_TC_GEMM") == nullptr;
   if (m->use_tc) {
-    if (m->Wcat_hi.empty()) {
-      int dk = c.num_features;
-      for (int l = 0; l < c.num_layers; ++l) {
-        const int D = c.dims_bidir[l];
-        float *h = nullptr, *lo = nullptr;
-        if (gemm_tc_supported(128, 6 * D, dk)) {
-          LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&h), (size_t)gemm_tc_kpad(dk) * 6 * D * sizeof(float)));
-          LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&lo), (size_t)gemm_tc_kpad(dk) * 6 * D * sizeof(float)));
-        }
-        m->Wcat_hi.push_back(h);
-        m->Wcat_lo.push_back(lo);
-        dk = 2 * D;
-      }
-      if (gemm_tc_supported(128, c.dim_matcher, m->E)) {
-        LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->Wp_hi), (size_t)gemm_tc_kpad(m->E) * c.dim_matcher * sizeof(float)));
-        LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->Wp_lo), (size_t)gemm_tc_kpad(m->E) * c.dim_matcher * sizeof(float)));
-      }
-    }
+    m->Wcat_tc.resize(c.num_layers);
     int dk = c.num_features;
     for (int l = 0; l < c.num_layers; ++l) {
-      const int D = c.dims_bidir[l];
-      if (m->Wcat_hi[l])
-        if (int rc = split_weight_tf32(m->Wcat[l], dk, 6 * D, m->Wcat_hi[l], m->Wcat_lo[l], st)) return rc;
-      dk = 2 * D;
+      if (int rc = pack_tc_weights(m->Wcat_tc[l], m->Wcat[l], dk, 6 * c.dims_bidir[l], st)) return rc;
+      dk = 2 * c.dims_bidir[l];
     }
-    if (m->Wp_hi)
-      if (int rc = split_weight_tf32(m->P(att_base(m) + "/preprocess.W"), m->E, c.dim_matcher, m->Wp_hi, m->Wp_lo, st))
-        return rc;
+    if (int rc = pack_tc_weights(m->Wp_tc, m->P(att_base(m) + "/preprocess.W"), m->E, c.dim_matcher, st)) return rc;
   }
   // fork(feedback(y)) for every symbol y, once: [(V+1), 3C]
   if (c.one_of_n_feedback) {
@@ -640,20 +642,33 @@ int finalize_on_stream(lvsr_model* m, cudaStream_t st, bool synchronise) {
   return 0;
 }
 
-// out[M, N] = A[M, K] . W + bias: the 3xTF32 wgmma GEMM when W has its K-major hi/lo split (W_hi, W_lo) and the shape suits
-// it, else the FFMA tile GEMM.  The split of A is scratch taken from `ws` and left there: it is dead once the GEMM is
-// enqueued, and the caller decides when to rewind it (lvsr_cost_matrix allocates the persistent decoder's buffers behind
-// it, and their place in the workspace is part of the decoder's measured step time).
-int projection_gemm(Arena& ws, const float* A, int M, int K, const float* W, const float* W_hi, const float* W_lo, int N,
-                    const float* bias, float* out, cudaStream_t st, int* kpad) {
-  if (W_hi && gemm_tc_supported(M, N, K)) {
+// out[M, N] = A[M, K] . W + bias: the wgmma GEMM when W has a tensor-core form (tw, packed by finalize) and the shape
+// suits it, else the FFMA tile GEMM.  The operand kind follows K: fp16 head/tail (f16x3) when K is a multiple of 64, so
+// every encoder layer from 1 on and the preprocess, 3xTF32 with K padded to a multiple of 32 otherwise (layer 0 at 40
+// features).  The split of A is scratch taken from `ws` and left there: it is dead once the GEMM is enqueued, and the
+// caller decides when to rewind it (lvsr_cost_matrix allocates the persistent decoder's buffers behind it, and their
+// place in the workspace is part of the decoder's measured step time).  Both kinds take the same 2 M kpad(K) floats,
+// so that place does not depend on the kind: the fp16 planes (M K halves each) fill the first half, the row exponents
+// sit at the start of the second.
+int projection_gemm(Arena& ws, const float* A, int M, int K, const float* W, const TcWeights* tw, int N,
+                    const float* bias, float* out, cudaStream_t st, int* kpad, int* operands) {
+  const bool f16 = tw && tw->head && gemm_f16_supported(M, N, K);
+  const bool tf32 = tw && tw->hi && gemm_tc_supported(M, N, K);
+  if (f16 || tf32) {
     float* a_hi = ws.f32((size_t)M * gemm_tc_kpad(K));
     float* a_lo = ws.f32((size_t)M * gemm_tc_kpad(K));
-    LVSR_CHECK(a_hi && a_lo, "out of device memory (tf32 split scratch)");
+    LVSR_CHECK(a_hi && a_lo, "out of device memory (tensor-core split scratch)");
     if (kpad) *kpad = gemm_tc_kpad(K);
-    return gemm_tc(A, a_hi, a_lo, M, K, W_hi, W_lo, N, bias, out, N, st);
+    if (operands) *operands = f16 ? LVSR_ENC_OPS_F16X3 : LVSR_ENC_OPS_TF32X3;
+    if (f16) {
+      __half* a_head = reinterpret_cast<__half*>(a_hi);
+      return gemm_f16(A, a_head, a_head + (size_t)M * K, reinterpret_cast<int*>(a_lo), M, K, tw->head, tw->tail, tw->ew,
+                      N, bias, out, N, st);
+    }
+    return gemm_tc(A, a_hi, a_lo, M, K, tw->hi, tw->lo, N, bias, out, N, st);
   }
   if (kpad) *kpad = 0;
+  if (operands) *operands = LVSR_ENC_OPS_NONE;
   return gemm_bias(make_gemm(A, M, K, W, N, bias, out), st);
 }
 
@@ -664,8 +679,10 @@ int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int
   int Tl = T, din = c.num_features;
   long long mstride = B;
   int kcum = 1;
-  for (int l = 0; l < c.num_layers; ++l)
+  for (int l = 0; l < c.num_layers; ++l) {
     for (int s = LVSR_ENC_PROJ; s <= LVSR_ENC_T; ++s) m->enc_plan[l][s] = 0;
+    m->enc_plan[l][LVSR_ENC_OPERANDS] = 0;
+  }
   for (int l = 0; l < c.num_layers; ++l) {
     const int D = c.dims_bidir[l], k = c.subsample[l];
     const int rows = Tl * B, Tout = ceil_div(Tl, k);
@@ -675,12 +692,13 @@ int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int
     // finalize splits the fork weights only while the tensor-core GEMM is on (null entry: a shape it refuses)
     const size_t mark = ws.off;
     int32_t* plan = m->enc_plan[l];
-    int kpad = 0;
-    if (int rc = projection_gemm(ws, cur, rows, din, m->Wcat[l], m->use_tc ? m->Wcat_hi[l] : nullptr,
-                                 m->use_tc ? m->Wcat_lo[l] : nullptr, 6 * D, m->bcat[l], pre, st, &kpad))
+    int kpad = 0, operands = 0;
+    if (int rc = projection_gemm(ws, cur, rows, din, m->Wcat[l], m->use_tc ? &m->Wcat_tc[l] : nullptr, 6 * D, m->bcat[l],
+                                 pre, st, &kpad, &operands))
       return rc;
     plan[LVSR_ENC_PROJ] = kpad ? LVSR_ENC_PATH_TC : LVSR_ENC_PATH_FFMA;
     plan[LVSR_ENC_KPAD] = kpad;
+    plan[LVSR_ENC_OPERANDS] = operands;
     if (ws.off <= ws.cap) ws.off = mark;     // the split scratch is dead once the GEMM is enqueued (stream order)
     float* out = (l == c.num_layers - 1) ? attended : ws.f32((size_t)Tout * B * 2 * D);
     LVSR_CHECK(out, "out of device memory (encoder layer output)");
@@ -742,14 +760,15 @@ int lvsr_preprocess(lvsr_model* m, const float* attended, int32_t Tp, int32_t U,
   LVSR_CHECK(attended && out && Tp > 0 && U > 0, "preprocess: bad arguments");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   ArenaScope scope(m, st);
-  int kpad = 0;
-  m->pre_plan[0] = m->pre_plan[1] = 0;
+  int kpad = 0, operands = 0;
+  m->pre_plan[0] = m->pre_plan[1] = m->pre_plan[2] = 0;
   if (int rc = projection_gemm(m->ws, attended, Tp * U, m->E, m->P(att_base(m) + "/preprocess.W"),
-                               m->use_tc ? m->Wp_hi : nullptr, m->Wp_lo, m->cfg.dim_matcher,
-                               m->P(att_base(m) + "/preprocess.b"), out, st, &kpad))
+                               m->use_tc ? &m->Wp_tc : nullptr, m->cfg.dim_matcher, m->P(att_base(m) + "/preprocess.b"),
+                               out, st, &kpad, &operands))
     return rc;
   m->pre_plan[0] = kpad ? LVSR_ENC_PATH_TC : LVSR_ENC_PATH_FFMA;
   m->pre_plan[1] = kpad;
+  m->pre_plan[2] = operands;
   return 0;
 }
 

@@ -1,26 +1,33 @@
 // Tensor-core path for the dense projections: C[M,N] = A[M,K] . W[K,N] + bias on the Hopper
-// warpgroup tensor cores (wgmma.mma_async kind tf32, fp32 accumulators in registers, operands staged
-// by TMA into 128B-swizzled shared memory).
+// warpgroup tensor cores (wgmma.mma_async, fp32 accumulators in registers, operands staged by TMA into 128B-swizzled
+// shared memory).
 //
 // Replaces the whole-sequence tensor.dot of Fork(Linear) in RecurrentWithFork
 // (lvsr/bricks/__init__.py:39-43) and attention.preprocess (lvsr/bricks/attention.py:228-230):
 // the only genuinely dense contractions of the path (SURVEY.md 8a-a2: 260 GFLOP per batch).
 //
-// Precision: the 1e-4 gate against the float64 oracle rules out single-pass tf32 (2^-11 per
-// product).  Every operand is split EXACTLY into two tf32 numbers, x = hi + lo
-// (hi = x with the low 13 mantissa bits cleared, lo = tf32(x - hi)), and three products
-// are accumulated in fp32:  lo.hi + hi.lo + hi.hi  (the dropped lo.lo term is 2^-22).
-// The split of A is one streaming pass (split_tf32_kernel); W is split once at
-// lvsr_model_finalize and kept K-major ([N,K]) so both operands use the K-major SWIZZLE_128B
-// canonical layout (wgmma reads tf32 operands from shared memory only in K-major form).
+// Precision: the 1e-4 gate against the float64 oracle rules out a single pass of tf32 or fp16 (2^-11 per product).
+// Every operand is split into two parts and three products are accumulated in fp32, small terms first
+// (lo.hi + hi.lo + hi.hi; the dropped lo.lo term is 2^-22).  One kernel template, two operand kinds:
+//  * tf32 (F16 = false): x = hi + lo EXACTLY, hi = x with the low 13 mantissa bits cleared, lo = tf32(x - hi).  Any K
+//    (zero-padded to a multiple of 32); the backward products and contractions that are not a multiple of 64.
+//  * fp16 (F16 = true): every row of A and every column of W is first scaled by a power of two 2^e that puts its
+//    largest magnitude into [2^13, 2^14), then x 2^e = head + tail with head = fp16(x 2^e), tail = fp16(x 2^e - head).
+//    The representation error is 2^-22 of |x 2^e|, or 2^-25 absolute once the tail falls into the fp16 subnormals (2^-38
+//    of the row's or column's largest value).  The epilogue unscales exactly: C = ldexp(acc, -(e_row + e_col)) + bias.
+//    Half the operand bytes and twice the tf32 rate: K a multiple of 64, the forward projections.
+// A is split by one streaming pass per GEMM (split_tf32_kernel / split_pad_tf32_kernel, split_rows_f16_kernel); W once
+// per lvsr_model_finalize, kept K-major ([N, K]) so both operands use the K-major SWIZZLE_128B canonical layout (wgmma
+// reads tf32 operands from shared memory only in K-major form).
 //
-// Kernel shape: one 128 x 128 output tile per CTA, BK = 32 floats (one 128-byte swizzle row),
-// 3-stage TMA -> wgmma mbarrier pipeline (4 operand tiles = 64 KB per stage), three warpgroups:
+// Kernel shape: 128 x 128 output tiles, one 128-byte swizzle row per k-block (32 tf32 or 64 fp16 values),
+// 3-stage TMA -> wgmma mbarrier pipeline (4 operand tiles = 64 KB per stage), one persistent CTA per SM, three warpgroups:
 // warpgroup 0 = TMA producer (one thread), warpgroups 1 and 2 = consumers, each owning 64 rows of the
-// tile (wgmma m64n128k8 into registers, then bias add and stores straight from the accumulators).
+// tile (wgmma m64n128k8 / m64n128k16 into registers, then bias add and stores straight from the accumulators).
 // On an H100 a 128 x 256 tile (2 stages, 128 accumulators per thread) measured 7 % slower for the
-// projections of the metric configuration than this shape.
+// projections of the metric configuration than this shape (tf32 operands).
 #include <cuda.h>
+#include <cuda_fp16.h>
 
 #include "kernels.h"
 
@@ -29,10 +36,11 @@ namespace lvsr {
 namespace {
 
 constexpr int TC_BM = 128, TC_BN = 128, TC_BK = 32;      // TC_BN: the granularity N must be a multiple of
+constexpr int TC_BK_F16 = 64;                            // fp16 values per 128-byte row: the k-block of the fp16 kind
 constexpr int TC_THREADS = 384;                          // producer warpgroup + two consumer warpgroups
 constexpr int TC_STAGES = 3;
-constexpr uint32_t TC_TILE_BYTES = TC_BM * TC_BK * sizeof(float);          // 16 KB: one 128-row operand tile
-constexpr uint32_t TC_STAGE_BYTES = 4 * TC_TILE_BYTES;                     // A_hi, A_lo, B_hi, B_lo
+constexpr uint32_t TC_TILE_BYTES = TC_BM * 128;                            // 16 KB: one 128-row operand tile
+constexpr uint32_t TC_STAGE_BYTES = 4 * TC_TILE_BYTES;                     // A_hi, A_lo, B_hi, B_lo (heads and tails)
 constexpr size_t TC_SMEM = (size_t)TC_STAGES * TC_STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
 
 __device__ __forceinline__ uint32_t smem_addr(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
@@ -71,7 +79,7 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
 // ---- wgmma ---------------------------------------------------------------------------------------------------------
 // K-major, SWIZZLE_128B canonical layout: rows are 128 B, 8-row groups are 1024 B apart (sm_90 shared-memory matrix
 // descriptor: start address, leading byte offset (unused for swizzled K-major), stride byte offset, layout type 1 =
-// 128-byte swizzle).  One k-step (8 tf32 values = 32 bytes) further along a row is start address + 2.
+// 128-byte swizzle).  One k-step (8 tf32 or 16 fp16 values = 32 bytes) further along a row is start address + 2.
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);          // start address, 16 B units
@@ -93,30 +101,58 @@ __device__ __forceinline__ void acc_fence(float (&d)[N]) {
 
 #define LVSR_ACC8(d, i) \
   "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
-__device__ __forceinline__ void wgmma_tf32_n128(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %66, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {"
-      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
-      "}, %64, %65, p, 1, 1;\n\t}\n"
-      : LVSR_ACC8(d, 0), LVSR_ACC8(d, 8), LVSR_ACC8(d, 16), LVSR_ACC8(d, 24),
-        LVSR_ACC8(d, 32), LVSR_ACC8(d, 40), LVSR_ACC8(d, 48), LVSR_ACC8(d, 56)
-      : "l"(desc_a), "l"(desc_b), "r"(scale_d));
+#define LVSR_ACC64 "{"                                                                        \
+  "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                    \
+  "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "          \
+  "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "          \
+  "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}"
+// d[64] (+)= A (64 x k, K-major) . B (128 x k, K-major)^T: k = 8 tf32 or 16 fp16 values, 32 bytes of each row
+template <bool F16>
+__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
+  if constexpr (F16) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 " LVSR_ACC64 ", %64, %65, p, 1, 1, 0, 0;\n\t}\n"
+        : LVSR_ACC8(d, 0), LVSR_ACC8(d, 8), LVSR_ACC8(d, 16), LVSR_ACC8(d, 24),
+          LVSR_ACC8(d, 32), LVSR_ACC8(d, 40), LVSR_ACC8(d, 48), LVSR_ACC8(d, 56)
+        : "l"(desc_a), "l"(desc_b), "r"(scale_d));
+  } else {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 " LVSR_ACC64 ", %64, %65, p, 1, 1;\n\t}\n"
+        : LVSR_ACC8(d, 0), LVSR_ACC8(d, 8), LVSR_ACC8(d, 16), LVSR_ACC8(d, 24),
+          LVSR_ACC8(d, 32), LVSR_ACC8(d, 40), LVSR_ACC8(d, 48), LVSR_ACC8(d, 56)
+        : "l"(desc_a), "l"(desc_b), "r"(scale_d));
+  }
 }
+#undef LVSR_ACC64
 #undef LVSR_ACC8
 
 struct TcGemmParams {
   float* C;
   const float* bias;
+  const int* ea;               // fp16 operands: exponent of every row of A [M] and column of B [N] (the scaling 2^e)
+  const int* eb;
   int M, N, K, ldc;
-  int kb_per_split;            // K blocks handled by one blockIdx.z (split-K: partial products, summed by the caller)
+  int tiles_n, tiles_m, tiles; // output tiles along N and M, and in all (times the splits)
+  int kb_per_split;            // K blocks of one split (split-K: partial products, summed by the caller)
   long long c_split_stride;    // elements between the partial outputs of consecutive splits
 };
 
+// x 2^-e, exactly unless the result leaves the normal fp32 range: one multiply by a power of two where 2^-e is a normal
+// float, ldexpf beyond
+__device__ __forceinline__ float unscale(float x, int e) {
+  return (unsigned)(e + 126) <= 252u ? x * __uint_as_float((uint32_t)(127 - e) << 23) : ldexpf(x, -e);
+}
+
+// F16 = false: tf32 hi/lo operands (m64n128k8); F16 = true: fp16 head/tail operands of rows and columns scaled by 2^ea,
+// 2^eb (m64n128k16), unscaled in the epilogue.
+// Persistent: each CTA walks the output tiles blockIdx.x, + gridDim.x, ... (N tiles fastest, then M tiles, then
+// splits), and the ring of stages runs on across tiles, so that the producer fills the next tile's first stages while
+// the consumers store the last one.  `it` counts the k-blocks a CTA has passed through the ring.
+template <bool F16>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
                const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo,
@@ -125,14 +161,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
   // SWIZZLE_128B needs 1024-byte aligned tiles
   uint8_t* tiles = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   constexpr int NACC = TC_BN / 2;                       // accumulators per consumer thread (m64 x 128 over 128 threads)
+  constexpr int BK = F16 ? TC_BK_F16 : TC_BK;           // values per 128-byte row
   unsigned long long* bars = reinterpret_cast<unsigned long long*>(tiles + (size_t)TC_STAGES * TC_STAGE_BYTES);
   // bars[0..S): full (TMA bytes landed), bars[S..2S): empty (both consumer warpgroups are done with the slot)
 
   const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
-  const int n0 = blockIdx.x * TC_BN, m0 = blockIdx.y * TC_BM;
-  const int kb0 = blockIdx.z * p.kb_per_split;
-  const int nkb = min(p.kb_per_split, p.K / TC_BK - kb0);
-  p.C += (long long)blockIdx.z * p.c_split_stride;
+  const int total_kb = p.K / BK;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < TC_STAGES; ++s) {
@@ -146,17 +180,23 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
   if (wg == 0) {
     // ===== TMA producer =====
     if (t == 0) {
-      for (int kb = 0; kb < nkb; ++kb) {
-        const int s = kb % TC_STAGES;
-        const uint32_t ph = (uint32_t)((kb / TC_STAGES) & 1);
-        bar_wait(smem_addr(&bars[TC_STAGES + s]), ph ^ 1u);       // slot free (first round passes immediately)
-        const uint32_t full = smem_addr(&bars[s]);
-        bar_expect_tx(full, TC_STAGE_BYTES);
-        const uint32_t base = smem_addr(tiles + (size_t)s * TC_STAGE_BYTES);
-        tma_load_2d(base + 0 * TC_TILE_BYTES, &map_a_hi, (kb0 + kb) * TC_BK, m0, full);
-        tma_load_2d(base + 1 * TC_TILE_BYTES, &map_a_lo, (kb0 + kb) * TC_BK, m0, full);
-        tma_load_2d(base + 2 * TC_TILE_BYTES, &map_b_hi, (kb0 + kb) * TC_BK, n0, full);
-        tma_load_2d(base + 3 * TC_TILE_BYTES, &map_b_lo, (kb0 + kb) * TC_BK, n0, full);
+      uint32_t it = 0;
+      for (int tile = blockIdx.x; tile < p.tiles; tile += gridDim.x) {
+        const int n0 = (tile % p.tiles_n) * TC_BN, m0 = (tile / p.tiles_n % p.tiles_m) * TC_BM;
+        const int kb0 = tile / (p.tiles_n * p.tiles_m) * p.kb_per_split;
+        const int nkb = min(p.kb_per_split, total_kb - kb0);
+        for (int kb = 0; kb < nkb; ++kb, ++it) {
+          const uint32_t s = it % TC_STAGES;
+          const uint32_t ph = (it / TC_STAGES) & 1u;
+          bar_wait(smem_addr(&bars[TC_STAGES + s]), ph ^ 1u);       // slot free (first round passes immediately)
+          const uint32_t full = smem_addr(&bars[s]);
+          bar_expect_tx(full, TC_STAGE_BYTES);
+          const uint32_t base = smem_addr(tiles + (size_t)s * TC_STAGE_BYTES);
+          tma_load_2d(base + 0 * TC_TILE_BYTES, &map_a_hi, (kb0 + kb) * BK, m0, full);
+          tma_load_2d(base + 1 * TC_TILE_BYTES, &map_a_lo, (kb0 + kb) * BK, m0, full);
+          tma_load_2d(base + 2 * TC_TILE_BYTES, &map_b_hi, (kb0 + kb) * BK, n0, full);
+          tma_load_2d(base + 3 * TC_TILE_BYTES, &map_b_lo, (kb0 + kb) * BK, n0, full);
+        }
       }
     }
     return;
@@ -164,48 +204,149 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
 
   // ===== consumers: warpgroup wg - 1 owns rows [64 (wg - 1), +64) of the tile =====
   const uint32_t a_off = (uint32_t)(wg - 1) * 64 * 128;          // 64 rows of 128 bytes into each A tile
-  float acc[NACC];
-#pragma unroll
-  for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
-  for (int kb = 0; kb < nkb; ++kb) {
-    const int s = kb % TC_STAGES;
-    bar_wait(smem_addr(&bars[s]), (uint32_t)((kb / TC_STAGES) & 1));
-    const uint32_t base = smem_addr(tiles + (size_t)s * TC_STAGE_BYTES);
-    const uint64_t da_hi = make_smem_desc(base + 0 * TC_TILE_BYTES + a_off), da_lo = make_smem_desc(base + 1 * TC_TILE_BYTES + a_off);
-    const uint64_t db_hi = make_smem_desc(base + 2 * TC_TILE_BYTES), db_lo = make_smem_desc(base + 3 * TC_TILE_BYTES);
-    wgmma_fence();
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {                      // 4 k-steps of 32 bytes per 128-byte row
-      const uint64_t adv = (uint64_t)(k * 2);
-      wgmma_tf32_n128(acc, da_lo + adv, db_hi + adv, 1u);     // small terms first
-      wgmma_tf32_n128(acc, da_hi + adv, db_lo + adv, 1u);
-      wgmma_tf32_n128(acc, da_hi + adv, db_hi + adv, 1u);
-    }
-    wgmma_commit();
-    // the products of stage kb - 1 have retired: its slot goes back to the producer
-    wgmma_wait<1>();
-    acc_fence(acc);
-    if (kb > 0 && t == 0) bar_arrive(smem_addr(&bars[TC_STAGES + (kb - 1) % TC_STAGES]));
-  }
-  wgmma_wait<0>();
-  acc_fence(acc);
-
-  // ===== epilogue: accumulator fragment -> global (+bias).  Register 4j + {0,1}: row 16 warp + lane / 4, columns
-  // 8j + 2 (lane % 4) + {0,1}; register 4j + {2,3}: the same columns 8 rows further down. =====
   const int warp = t >> 5, lane = t & 31;
-  const int r0 = m0 + (wg - 1) * 64 + warp * 16 + (lane >> 2);
-  const int cbase = n0 + 2 * (lane & 3);
+  uint32_t it = 0;
+  for (int tile = blockIdx.x; tile < p.tiles; tile += gridDim.x) {
+    const int n0 = (tile % p.tiles_n) * TC_BN, m0 = (tile / p.tiles_n % p.tiles_m) * TC_BM;
+    const int split = tile / (p.tiles_n * p.tiles_m);
+    const int nkb = min(p.kb_per_split, total_kb - split * p.kb_per_split);
+    float acc[NACC];
 #pragma unroll
-  for (int j = 0; j < TC_BN / 8; ++j) {
-    const int col = cbase + 8 * j;
-    float2 b = make_float2(0.f, 0.f);
-    if (p.bias) b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+    for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
+    for (int kb = 0; kb < nkb; ++kb, ++it) {
+      const uint32_t s = it % TC_STAGES;
+      bar_wait(smem_addr(&bars[s]), (it / TC_STAGES) & 1u);
+      const uint32_t base = smem_addr(tiles + (size_t)s * TC_STAGE_BYTES);
+      const uint64_t da_hi = make_smem_desc(base + 0 * TC_TILE_BYTES + a_off), da_lo = make_smem_desc(base + 1 * TC_TILE_BYTES + a_off);
+      const uint64_t db_hi = make_smem_desc(base + 2 * TC_TILE_BYTES), db_lo = make_smem_desc(base + 3 * TC_TILE_BYTES);
+      wgmma_fence();
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int row = r0 + 8 * h;
-      const float x = acc[4 * j + 2 * h], y = acc[4 * j + 2 * h + 1];
-      if (row < p.M) *reinterpret_cast<float2*>(p.C + (long long)row * p.ldc + col) = make_float2(x + b.x, y + b.y);
+      for (int k = 0; k < 4; ++k) {                      // 4 k-steps of 32 bytes per 128-byte row
+        const uint64_t adv = (uint64_t)(k * 2);
+        wgmma_n128<F16>(acc, da_lo + adv, db_hi + adv, 1u);     // small terms first
+        wgmma_n128<F16>(acc, da_hi + adv, db_lo + adv, 1u);
+        wgmma_n128<F16>(acc, da_hi + adv, db_hi + adv, 1u);
+      }
+      wgmma_commit();
+      // the products of the previous k-block have retired: its slot goes back to the producer
+      wgmma_wait<1>();
+      acc_fence(acc);
+      if (kb > 0 && t == 0) bar_arrive(smem_addr(&bars[TC_STAGES + (it - 1) % TC_STAGES]));
     }
+    wgmma_wait<0>();
+    acc_fence(acc);
+    if (t == 0) bar_arrive(smem_addr(&bars[TC_STAGES + (it - 1) % TC_STAGES]));   // the tile's last slot
+
+    // ===== epilogue: accumulator fragment -> global (+bias).  Register 4j + {0,1}: row 16 warp + lane / 4, columns
+    // 8j + 2 (lane % 4) + {0,1}; register 4j + {2,3}: the same columns 8 rows further down. =====
+    float* C = p.C + (long long)split * p.c_split_stride;
+    const int r0 = m0 + (wg - 1) * 64 + warp * 16 + (lane >> 2);
+    const int cbase = n0 + 2 * (lane & 3);
+    // every load of the epilogue is issued before the first store: one L2 round trip per tile, not one per column pair
+    float2 bias[TC_BN / 8];
+    int2 eb[TC_BN / 8];
+    int ea[2] = {0, 0};
+#pragma unroll
+    for (int j = 0; j < TC_BN / 8; ++j) {
+      bias[j] = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + cbase + 8 * j)) : make_float2(0.f, 0.f);
+      eb[j] = F16 ? __ldg(reinterpret_cast<const int2*>(p.eb + cbase + 8 * j)) : make_int2(0, 0);
+    }
+    if constexpr (F16) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) ea[h] = r0 + 8 * h < p.M ? __ldg(p.ea + r0 + 8 * h) : 0;
+    }
+#pragma unroll
+    for (int j = 0; j < TC_BN / 8; ++j) {
+      const int col = cbase + 8 * j;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = r0 + 8 * h;
+        float x = acc[4 * j + 2 * h], y = acc[4 * j + 2 * h + 1];
+        if constexpr (F16) {
+          x = unscale(x, ea[h] + eb[j].x);
+          y = unscale(y, ea[h] + eb[j].y);
+        }
+        if (row < p.M) *reinterpret_cast<float2*>(C + (long long)row * p.ldc + col) = make_float2(x + bias[j].x, y + bias[j].y);
+      }
+    }
+  }
+}
+
+// ---- fp16 operands: power-of-two range scaling and the head/tail split -------------------------------------------------
+// Exponent e that puts max_abs * 2^e into [2^13, 2^14): 140 - the biased exponent of max_abs.  All-zero vectors get 0;
+// e <= 127 keeps 2^e a normal float (vectors whose largest value is below 2^-114 are scaled less far), and e >= -115
+// holds for every finite max_abs, so x * 2^e is exact and the epilogue's unscale by 2^-(e_row + e_col) is too.
+__device__ __forceinline__ int f16_range_exponent(float max_abs) {
+  if (max_abs == 0.f) return 0;
+  return min(140 - (int)((__float_as_uint(max_abs) >> 23) & 0xFFu), 127);
+}
+__device__ __forceinline__ float exp2_int(int e) { return __uint_as_float((uint32_t)(e + 127) << 23); }   // e in [-126, 127]
+// y = x * 2^e = head + tail: |y| < 2^14 keeps head finite, y - head is exact in fp32
+__device__ __forceinline__ void split_f16(float y, __half& head, __half& tail) {
+  head = __float2half_rn(y);
+  tail = __float2half_rn(y - __half2float(head));
+}
+
+// one warp per row of x [M, K] (K % 64 == 0): e[r], head / tail [M, K] of row r scaled by 2^e[r]
+__global__ void split_rows_f16_kernel(const float* __restrict__ x, __half* __restrict__ head, __half* __restrict__ tail,
+                                      int* __restrict__ e, long long M, int K) {
+  const long long r = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (r >= M) return;
+  const float2* row = reinterpret_cast<const float2*>(x + r * K);
+  float mx = 0.f;
+  for (int i = lane; i < K / 2; i += 32) {
+    const float2 v = row[i];
+    mx = fmaxf(mx, fmaxf(fabsf(v.x), fabsf(v.y)));
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  const int er = f16_range_exponent(mx);
+  const float s = exp2_int(er);
+  if (lane == 0) e[r] = er;
+  __half2* h2 = reinterpret_cast<__half2*>(head + r * K);
+  __half2* t2 = reinterpret_cast<__half2*>(tail + r * K);
+  for (int i = lane; i < K / 2; i += 32) {             // the row is in L1 from the first pass
+    const float2 v = row[i];
+    __half hx, hy, tx, ty;
+    split_f16(v.x * s, hx, tx);
+    split_f16(v.y * s, hy, ty);
+    h2[i] = __halves2half2(hx, hy);
+    t2[i] = __halves2half2(tx, ty);
+  }
+}
+
+// W [K, N] row-major -> K-major head / tail [N, K] of every column n scaled by 2^e[n] (weights, once per finalize).
+// One block of 32 x 8 threads per 32 columns: the column maxima first, then 32 x 32 tiles through shared memory.
+__global__ void transpose_split_f16_kernel(const float* __restrict__ W, __half* __restrict__ head, __half* __restrict__ tail,
+                                           int* __restrict__ e, int K, int N) {
+  __shared__ float tile[32][33];
+  __shared__ float scale[32];
+  const int n0 = blockIdx.x * 32, tx = threadIdx.x, ty = threadIdx.y;
+  const int n = n0 + tx;
+  float mx = 0.f;
+  if (n < N)
+    for (int k = ty; k < K; k += 8) mx = fmaxf(mx, fabsf(W[(long long)k * N + n]));
+  tile[ty][tx] = mx;
+  __syncthreads();
+  if (ty == 0) {
+    for (int i = 1; i < 8; ++i) mx = fmaxf(mx, tile[i][tx]);
+    const int en = f16_range_exponent(mx);
+    if (n < N) e[n] = en;
+    scale[tx] = exp2_int(en);
+  }
+  __syncthreads();
+  for (int k0 = 0; k0 < K; k0 += 32) {
+    for (int i = ty; i < 32; i += 8) {
+      const int k = k0 + i;
+      tile[i][tx] = (k < K && n < N) ? W[(long long)k * N + n] * scale[tx] : 0.f;
+    }
+    __syncthreads();
+    for (int i = ty; i < 32; i += 8) {
+      const int nn = n0 + i, k = k0 + tx;
+      if (nn < N && k < K) split_f16(tile[tx][i], head[(long long)nn * K + k], tail[(long long)nn * K + k]);
+    }
+    __syncthreads();
   }
 }
 
@@ -282,16 +423,56 @@ int get_encode() {
   return 0;
 }
 
-// 2-D fp32 tensor [rows, K] (K contiguous), box = [128 rows, 32 floats], 128-byte swizzle
-int make_map(CUtensorMap* map, const float* ptr, long long rows, int K, int box_rows = TC_BM) {
+// 2-D fp32 or fp16 tensor [rows, K] (K contiguous), box = [128 rows, one 128-byte row: 32 floats or 64 halves],
+// 128-byte swizzle
+int make_map(CUtensorMap* map, const void* ptr, long long rows, int K, bool f16) {
+  const size_t esize = f16 ? sizeof(__half) : sizeof(float);
   cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)K * sizeof(float)};
-  cuuint32_t box[2] = {(cuuint32_t)TC_BK, (cuuint32_t)box_rows};
+  cuuint64_t strides[1] = {(cuuint64_t)K * esize};
+  cuuint32_t box[2] = {(cuuint32_t)(128 / esize), (cuuint32_t)TC_BM};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = g_encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(ptr), dims, strides, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CUresult r = g_encode(map, f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2,
+                        const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                        CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   LVSR_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d)", (int)r);
+  return 0;
+}
+
+// C = A . B^T (+ bias) on the presplit K-major operands of either kind; K is a multiple of the kind's k-block
+template <bool F16>
+int launch_tc(const void* A_hi, const void* A_lo, const int* ea, int M, const void* B_hi, const void* B_lo, const int* eb,
+              int N, int K, const float* bias, float* C, int ldc, int splits, long long split_stride, cudaStream_t stream) {
+  ProfScope prof("gemm", stream);
+  constexpr int BK = F16 ? TC_BK_F16 : TC_BK;
+  LVSR_CHECK(M >= 1 && N % TC_BN == 0 && K % BK == 0 && K >= BK && splits >= 1,
+             "gemm_tc: unsupported shape M=%d N=%d K=%d (%s operands)", M, N, K, F16 ? "fp16" : "tf32");
+  if (int rc = get_encode()) return rc;
+  CUtensorMap ma_hi, ma_lo, mb_hi, mb_lo;
+  if (int rc = make_map(&ma_hi, A_hi, M, K, F16)) return rc;
+  if (int rc = make_map(&ma_lo, A_lo, M, K, F16)) return rc;
+  if (int rc = make_map(&mb_hi, B_hi, N, K, F16)) return rc;
+  if (int rc = make_map(&mb_lo, B_lo, N, K, F16)) return rc;
+  static bool configured[LVSR_MAX_DEVICES] = {false};
+  const int dev = current_device();
+  if (!configured[dev]) {
+    LVSR_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM));
+    configured[dev] = true;
+  }
+  const int total_kb = K / BK;
+  splits = std::min(splits, total_kb);
+  TcGemmParams p;
+  p.C = C; p.bias = bias; p.ea = ea; p.eb = eb; p.M = M; p.N = N; p.K = K; p.ldc = ldc;
+  p.kb_per_split = ceil_div(total_kb, splits);
+  p.c_split_stride = split_stride;
+  p.tiles_n = N / TC_BN;
+  p.tiles_m = ceil_div(M, TC_BM);
+  const long long tiles = (long long)p.tiles_n * p.tiles_m * ceil_div(total_kb, p.kb_per_split);
+  LVSR_CHECK(tiles <= INT32_MAX, "gemm_tc: too many tiles (M=%d N=%d)", M, N);
+  p.tiles = (int)tiles;
+  // one CTA per SM (TC_SMEM), each walking tiles
+  const int grid = (int)std::min<long long>(tiles, device_sm_count());
+  gemm_tc_kernel<F16><<<grid, TC_THREADS, TC_SMEM, stream>>>(ma_hi, ma_lo, mb_hi, mb_lo, p);
+  LVSR_LAUNCH_CHECK();
   return 0;
 }
 
@@ -342,30 +523,7 @@ int gemm_tc_splits_launched(int Kpad, int splits) {
 // result z goes to C + z * split_stride (the caller adds them up).
 int gemm_tc_presplit(const float* A_hi, const float* A_lo, int M, const float* B_hi, const float* B_lo, int N, int Kpad,
                      const float* bias, float* C, int ldc, int splits, long long split_stride, cudaStream_t stream) {
-  ProfScope prof("gemm", stream);
-  LVSR_CHECK(M >= 1 && N % TC_BN == 0 && Kpad % TC_BK == 0 && Kpad >= TC_BK && splits >= 1, "gemm_tc_presplit: unsupported shape M=%d N=%d K=%d", M, N, Kpad);
-  if (int rc = get_encode()) return rc;
-  CUtensorMap ma_hi, ma_lo, mb_hi, mb_lo;
-  if (int rc = make_map(&ma_hi, A_hi, M, Kpad)) return rc;
-  if (int rc = make_map(&ma_lo, A_lo, M, Kpad)) return rc;
-  if (int rc = make_map(&mb_hi, B_hi, N, Kpad)) return rc;
-  if (int rc = make_map(&mb_lo, B_lo, N, Kpad)) return rc;
-  static bool configured[LVSR_MAX_DEVICES] = {false};
-  const int dev = current_device();
-  if (!configured[dev]) {
-    LVSR_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM));
-    configured[dev] = true;
-  }
-  const int total_kb = Kpad / TC_BK;
-  splits = std::min(splits, total_kb);
-  TcGemmParams p;
-  p.C = C; p.bias = bias; p.M = M; p.N = N; p.K = Kpad; p.ldc = ldc;
-  p.kb_per_split = ceil_div(total_kb, splits);
-  p.c_split_stride = split_stride;
-  dim3 grid(N / TC_BN, ceil_div(M, TC_BM), ceil_div(total_kb, p.kb_per_split));
-  gemm_tc_kernel<<<grid, TC_THREADS, TC_SMEM, stream>>>(ma_hi, ma_lo, mb_hi, mb_lo, p);
-  LVSR_LAUNCH_CHECK();
-  return 0;
+  return launch_tc<false>(A_hi, A_lo, nullptr, M, B_hi, B_lo, nullptr, N, Kpad, bias, C, ldc, splits, split_stride, stream);
 }
 
 // C[M,N] = A[M,K] . W + bias with W given as the K-major hi/lo pair produced by split_weight_tf32.
@@ -385,6 +543,28 @@ int gemm_tc(const float* A, float* A_hi, float* A_lo, int M, int K, const float*
   }
   LVSR_LAUNCH_CHECK();
   return gemm_tc_presplit(A_hi, A_lo, M, Wt_hi, Wt_lo, N, Kpad, bias, C, ldc, 1, 0, stream);
+}
+
+bool gemm_f16_supported(int M, int N, int K) { return M >= 1 && N % TC_BN == 0 && K >= TC_BK_F16 && K % TC_BK_F16 == 0; }
+
+// W [K, N] row-major -> Wt_head / Wt_tail [N, K] halves and ew [N]
+int split_weight_f16(const float* W, int K, int N, __half* Wt_head, __half* Wt_tail, int* ew, cudaStream_t stream) {
+  LVSR_CHECK(K % TC_BK_F16 == 0 && K > 0 && N > 0, "split_weight_f16: unsupported shape K=%d N=%d", K, N);
+  transpose_split_f16_kernel<<<ceil_div(N, 32), dim3(32, 8), 0, stream>>>(W, Wt_head, Wt_tail, ew, K, N);
+  LVSR_LAUNCH_CHECK();
+  return 0;
+}
+
+// C[M,N] = A[M,K] . W + bias on fp16 head/tail operands, W as split_weight_f16 left it.  A_head / A_tail (M * K halves
+// each) and ea (M ints): caller-provided scratch for the split of A.
+int gemm_f16(const float* A, __half* A_head, __half* A_tail, int* ea, int M, int K, const __half* Wt_head,
+             const __half* Wt_tail, const int* ew, int N, const float* bias, float* C, int ldc, cudaStream_t stream) {
+  LVSR_CHECK(gemm_f16_supported(M, N, K), "gemm_f16: unsupported shape M=%d N=%d K=%d", M, N, K);
+  constexpr int ROWS_PER_BLOCK = 8;
+  split_rows_f16_kernel<<<ceil_div(M, ROWS_PER_BLOCK), 32 * ROWS_PER_BLOCK, 0, stream>>>(
+      A, A_head, A_tail, ea, M, K);
+  LVSR_LAUNCH_CHECK();
+  return launch_tc<true>(A_head, A_tail, ea, M, Wt_head, Wt_tail, ew, N, K, bias, C, ldc, 1, 0, stream);
 }
 
 }  // namespace lvsr

@@ -1,5 +1,7 @@
 // Internal (C++) launch interfaces of the kernels behind the C ABI in include/lvsr_b200.h.
 #pragma once
+#include <cuda_fp16.h>
+
 #include "common.cuh"
 
 namespace lvsr {
@@ -28,7 +30,7 @@ inline GemmArgs make_gemm(const float* A, int M, int K, const float* W, int N, c
   return g;
 }
 
-// ---- gemm_tc.cu: wgmma / TMA path (3xTF32 split) -----------------------------------------
+// ---- gemm_tc.cu: wgmma / TMA path (3xTF32 split, or fp16 head/tail split when K % 64 == 0) -------------
 bool gemm_tc_supported(int M, int N, int K);
 int gemm_tc_kpad(int K);                 // contraction dimension as stored in the hi/lo operands (multiple of 32)
 int split_weight_tf32(const float* W, int K, int N, float* Wt_hi, float* Wt_lo, cudaStream_t stream);
@@ -39,6 +41,10 @@ int gemm_tc_presplit(const float* A_hi, const float* A_lo, int M, const float* B
 int gemm_tc_splits_launched(int Kpad, int splits);   // how many partial outputs gemm_tc_presplit writes
 int gemm_tc(const float* A, float* A_hi, float* A_lo, int M, int K, const float* Wt_hi, const float* Wt_lo, int N,
             const float* bias, float* C, int ldc, cudaStream_t stream);
+bool gemm_f16_supported(int M, int N, int K);      // K a multiple of 64: fp16 operands, no padding
+int split_weight_f16(const float* W, int K, int N, __half* Wt_head, __half* Wt_tail, int* ew, cudaStream_t stream);
+int gemm_f16(const float* A, __half* A_head, __half* A_tail, int* ea, int M, int K, const __half* Wt_head,
+             const __half* Wt_tail, const int* ew, int N, const float* bias, float* C, int ldc, cudaStream_t stream);
 
 // ---- bigru.cu -----------------------------------------------------------------------
 struct BiGruArgs {

@@ -87,6 +87,16 @@ struct Arena {
   }
 };
 
+// One projection's weights [K, N] packed for the tensor-core GEMM, K-major: fp16 head / tail planes [N, K] with the
+// exponent of every column (K a multiple of 64), else tf32 hi / lo planes [N, gemm_tc_kpad(K)].  mem == null: the
+// shape has no tensor-core form.
+struct TcWeights {
+  void* mem = nullptr;                              // the one allocation the planes below live in
+  __half *head = nullptr, *tail = nullptr;
+  int* ew = nullptr;
+  float *hi = nullptr, *lo = nullptr;
+};
+
 struct Param {
   std::string name;
   int64_t shape[2];
@@ -117,9 +127,9 @@ struct lvsr_model {
   float* Wff_cat = nullptr;         // [Cfb, 3C] = [fork gate_inputs | fork inputs]
   float* bff_cat = nullptr;         // [3C]
   float* FF = nullptr;              // [(V+1), 3C] = lookup . Wff_cat + bff_cat
-  // K-major tf32 hi/lo splits of the dense-projection weights (wgmma path); null = SIMT path
-  std::vector<float*> Wcat_hi, Wcat_lo;
-  float *Wp_hi = nullptr, *Wp_lo = nullptr;
+  // dense-projection weights as the tensor-core GEMM reads them (wgmma path); empty = SIMT path
+  std::vector<TcWeights> Wcat_tc;
+  TcWeights Wp_tc;
   bool use_tc = true;
   float v_bias = 0.f;               // host copy of energy_comp/linear.b
   unsigned* status = nullptr;       // device word: launch status of the data-flow decoder (common.cuh LVSR_FLOW_*)
@@ -128,7 +138,7 @@ struct lvsr_model {
   int32_t dec_plan[16] = {0};       // plan of the last lvsr_cost_matrix (lvsr_model_decoder_plan, LVSR_PLAN_* slots)
   int att_cs = 0;                   // cluster size of the last attention_step launch
   int32_t enc_plan[LVSR_MAX_LAYERS][16] = {};   // per layer: lvsr_model_encoder_plan's LVSR_ENC_* slots
-  int32_t pre_plan[2] = {0, 0};     // last lvsr_preprocess: path (LVSR_ENC_PATH_*), Kpad
+  int32_t pre_plan[3] = {0, 0, 0};  // last lvsr_preprocess: path (LVSR_ENC_PATH_*), Kpad, operands (LVSR_ENC_OPS_*)
   bool finalized = false;
   // ---- FST language model (lvsr_model_set_lm); lm_off == nullptr: none attached ----
   long long* lm_off = nullptr;
@@ -227,10 +237,11 @@ int finalize_on_stream(lvsr_model* m, cudaStream_t st, bool synchronise);
 // the training stores; with one, tape[l] records layer l's buffers (and allocates hext) for the backward pass.
 int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int T, int B, float* attended,
                 float* attended_mask, LayerTape* tape, cudaStream_t st);
-// out[M, N] = A[M, K] . W + bias on the tensor cores when W_hi / W_lo are given and the shape suits them, else on FFMA
-// tiles; *kpad (may be null) = the contraction as the tensor-core GEMM stored it, 0 on FFMA
-int projection_gemm(Arena& ws, const float* A, int M, int K, const float* W, const float* W_hi, const float* W_lo, int N,
-                    const float* bias, float* out, cudaStream_t st, int* kpad = nullptr);
+// out[M, N] = A[M, K] . W + bias on the tensor cores when tw holds a packed form and the shape suits it, else on FFMA
+// tiles; *kpad (may be null) = the contraction as the tensor-core GEMM stored it, 0 on FFMA; *operands (may be null) =
+// LVSR_ENC_OPS_* of the kernel that ran
+int projection_gemm(Arena& ws, const float* A, int M, int K, const float* W, const TcWeights* tw, int N,
+                    const float* bias, float* out, cudaStream_t st, int* kpad = nullptr, int* operands = nullptr);
 int readout_merged(lvsr_model* m, int R, const float* states, const float* ctx, float* merged, cudaStream_t st);
 ReadoutArgs readout_args(lvsr_model* m, int R, const float* merged);
 // language model (api.cu): the device view of the attached FST, the fusion fields of a readout, and the LM status

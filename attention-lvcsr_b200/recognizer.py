@@ -441,12 +441,14 @@ class SpeechRecognizer(object):
         for k in ("proj", "wgrad", "dx"):
             plan[k] = _lib.ENC_PATHS[plan[k]]
         plan["bigru"] = _lib.ENC_BIGRU_KERNELS[plan["bigru"]]
+        plan["operands"] = _lib.ENC_OPERANDS[plan["operands"]]
         plan["tape"] = bool(plan["tape"])
         return plan
 
     def encoder_plan(self):
         """What the encoder ran (lvsr_model_encoder_plan), one dict per layer.  Of the last encoder forward: proj (fork
-        projection GEMM: "tc" or "ffma"), kpad (its contraction as the tensor-core GEMM stores it, 0 on FFMA), bigru
+        projection GEMM: "tc" or "ffma"), kpad (its contraction as the tensor-core GEMM stores it, 0 on FFMA), operands
+        (of that tensor-core GEMM: "f16x3" when the contraction is a multiple of 64, else "tf32x3"; None on FFMA), bigru
         ("mma" or "ffma"), tape (a training forward), rb and cs (rows and CTAs per cluster), clusters, resident (clusters
         of that kernel the device holds at once), waves and T (frames scanned).  Of the last training step: bwd_cs
         (CTAs per cluster of the reverse-time scan), wgrad ("tc" or "ffma"), wgrad_splits, wgrad_kpad (the padded

@@ -128,12 +128,13 @@ int lvsr_model_decoder_plan(const lvsr_model* m, int32_t out[16]);
  * LVSR_ENC_T describe the LAST encoder forward on this handle (lvsr_encoder_forward, lvsr_recognizer_cost_host or the
  * forward of a training step), slots LVSR_ENC_BWD_CS .. LVSR_ENC_DX the backward pass of the LAST
  * lvsr_train_cost_and_grads (all zero before the first).  layer = -1 reports the last lvsr_preprocess (it also runs
- * inside every cost and training call) in LVSR_ENC_PROJ and LVSR_ENC_KPAD, every other slot zero.  The switches
+ * inside every cost and training call) in LVSR_ENC_PROJ, LVSR_ENC_KPAD and LVSR_ENC_OPERANDS, every other slot zero.  The switches
  * LVSR_BIGRU_MMA, LVSR_BIGRU_RB and LVSR_NO_TC_GEMM (DESIGN §7; the last one is read by lvsr_model_finalize) force
  * the choices; this report says what ran. */
 enum {
   LVSR_ENC_PROJ = 0,          /* fork projection GEMM: LVSR_ENC_PATH_*                                         */
-  LVSR_ENC_KPAD = 1,          /* its contraction as the tensor-core GEMM stores it (multiple of 32; 0 on FFMA) */
+  LVSR_ENC_KPAD = 1,          /* its contraction as the tensor-core GEMM stores it (0 on FFMA): unpadded on fp16
+                                 operands (a multiple of 64), padded to a multiple of 32 on tf32 operands       */
   LVSR_ENC_BIGRU = 2,         /* LVSR_ENC_BIGRU_*: the scan kernel                                             */
   LVSR_ENC_TAPE = 3,          /* 1: the scan kept the tape of a training step                                  */
   LVSR_ENC_RB = 4,            /* batch rows per cluster                                                        */
@@ -146,9 +147,13 @@ enum {
   LVSR_ENC_WGRAD = 11,        /* weight gradients X^T dY: LVSR_ENC_PATH_*                                      */
   LVSR_ENC_WGRAD_SPLITS = 12, /* partial products the contraction over T_l * B rows was split into             */
   LVSR_ENC_WGRAD_KPAD = 13,   /* that contraction as the tensor-core operands store it (0 on FFMA)             */
-  LVSR_ENC_DX = 14            /* input gradient dY W^T: LVSR_ENC_PATH_* (NONE for layer 0)                     */
+  LVSR_ENC_DX = 14,           /* input gradient dY W^T: LVSR_ENC_PATH_* (NONE for layer 0)                     */
+  LVSR_ENC_OPERANDS = 15      /* operands of the tensor-core projection GEMM: LVSR_ENC_OPS_*                   */
 };
 enum { LVSR_ENC_PATH_NONE = 0, LVSR_ENC_PATH_TC = 1, LVSR_ENC_PATH_FFMA = 2 };
+/* LVSR_ENC_OPS_TF32X3: tf32 hi/lo split, three products; LVSR_ENC_OPS_F16X3: fp16 head/tail split of rows and columns
+ * scaled by powers of two, three products (forward projections whose contraction is a multiple of 64) */
+enum { LVSR_ENC_OPS_NONE = 0, LVSR_ENC_OPS_TF32X3 = 1, LVSR_ENC_OPS_F16X3 = 2 };
 enum { LVSR_ENC_BIGRU_NONE = 0, LVSR_ENC_BIGRU_FFMA = 1, LVSR_ENC_BIGRU_MMA = 2 };
 int lvsr_model_encoder_plan(const lvsr_model* m, int32_t layer, int32_t out[16]);
 
