@@ -97,6 +97,8 @@ SIGNATURES = {
     "lvsr_model_status": (C.c_int, [_P, C.POINTER(C.c_int32), C.POINTER(C.c_int64)]),
     "lvsr_model_decoder_plan": (C.c_int, [_P, C.POINTER(C.c_int32)]),
     "lvsr_model_encoder_plan": (C.c_int, [_P, _I, C.POINTER(C.c_int32)]),
+    "lvsr_model_encoder_overlap": (C.c_int, [_P, _I, C.POINTER(C.c_int32)]),
+    "lvsr_model_encoder_overlap_claims": (C.c_int, [_P, _I, C.POINTER(C.c_int32), C.c_int64]),
     "lvsr_encoded_length": (C.c_int, [_P, _I]),
     "lvsr_encoded_dim": (C.c_int, [_P]),
     "lvsr_encoder_forward": (C.c_int, [_P, _P, _P, _I, _I, _P, _P, _P]),

@@ -246,6 +246,7 @@ size_t encoder_ws_bytes(const lvsr_model* m, int T, int B) {
     const int Tout = ceil_div(Tl, k);
     total += ((size_t)Tl * B * 6 * D + (size_t)Tout * B * 2 * D) * sizeof(float) + 1024;
     total += (size_t)2 * Tl * B * gemm_tc_kpad(l == 0 ? m->cfg.num_features : 2 * m->cfg.dims_bidir[l - 1]) * sizeof(float) + 1024;
+    total += gemm_f16_stream_sync_ints(Tl * B) * sizeof(int) + 1024;   // scheduling area of a streamed projection
     Tl = Tout;
   }
   return total + (1 << 16);
@@ -383,6 +384,8 @@ int lvsr_model_destroy(lvsr_model* m) {
   if (m->bff_cat) cudaFree(m->bff_cat);
   if (m->FF) cudaFree(m->FF);
   if (m->status) cudaFree(m->status);
+  if (m->enc_tiles) cudaFree(m->enc_tiles);
+  if (m->enc_claims) cudaFree(m->enc_claims);
   if (m->opt_velocity) cudaFree(m->opt_velocity);
   if (m->opt_ms_step) cudaFree(m->opt_ms_step);
   if (m->opt_ms_dx) cudaFree(m->opt_ms_dx);
@@ -421,6 +424,36 @@ int lvsr_model_encoder_plan(const lvsr_model* m, int32_t layer, int32_t out[16])
     out[LVSR_ENC_KPAD] = m->pre_plan[1];
     out[LVSR_ENC_OPERANDS] = m->pre_plan[2];
   }
+  return 0;
+}
+
+int lvsr_model_encoder_overlap(lvsr_model* m, int32_t layer, int32_t out[3]) {
+  LVSR_CHECK(m && out, "null argument");
+  LVSR_CHECK(layer >= 0 && layer < m->cfg.num_layers, "encoder_overlap: layer %d outside [0, %d)", layer, m->cfg.num_layers);
+  DeviceGuard device_guard(m);
+  out[0] = m->enc_overlap[layer];
+  out[1] = out[2] = 0;
+  if (out[0]) {
+    int tiles[2];
+    LVSR_CUDA_OK(cudaDeviceSynchronize());
+    LVSR_CUDA_OK(cudaMemcpy(tiles, m->enc_tiles + 2 * layer, sizeof(tiles), cudaMemcpyDeviceToHost));
+    out[1] = tiles[0];
+    out[2] = tiles[1];
+  }
+  return 0;
+}
+
+int lvsr_model_encoder_overlap_claims(lvsr_model* m, int32_t layer, int32_t* out, int64_t count) {
+  LVSR_CHECK(m && out, "null argument");
+  LVSR_CHECK(layer >= 1 && layer < m->cfg.num_layers && m->enc_overlap[layer],
+             "encoder_overlap_claims: layer %d did not overlap in the last encoder forward", layer);
+  const size_t end = layer + 1 < m->cfg.num_layers ? m->enc_claims_off[layer + 1] : m->enc_claims_cap;
+  const size_t n = end - m->enc_claims_off[layer];
+  LVSR_CHECK(count >= 0 && (size_t)count <= n, "encoder_overlap_claims: %lld ints asked, layer %d has %zu",
+             (long long)count, layer, n);
+  DeviceGuard device_guard(m);
+  LVSR_CUDA_OK(cudaDeviceSynchronize());
+  LVSR_CUDA_OK(cudaMemcpy(out, m->enc_claims + m->enc_claims_off[layer], (size_t)count * sizeof(int), cudaMemcpyDeviceToHost));
   return 0;
 }
 
@@ -672,6 +705,9 @@ int projection_gemm(Arena& ws, const float* A, int M, int K, const float* W, con
   return gemm_bias(make_gemm(A, M, K, W, N, bias, out), st);
 }
 
+// The SMs a scan must leave free for the projection behind it to run beside it (api.cu: run_encoder)
+constexpr int ENC_OVERLAP_MIN_SMS = 16;
+
 int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int T, int B, float* attended,
                 float* attended_mask, LayerTape* tape, cudaStream_t st) {
   const lvsr_config& c = m->cfg;
@@ -682,24 +718,53 @@ int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int
   for (int l = 0; l < c.num_layers; ++l) {
     for (int s = LVSR_ENC_PROJ; s <= LVSR_ENC_T; ++s) m->enc_plan[l][s] = 0;
     m->enc_plan[l][LVSR_ENC_OPERANDS] = 0;
+    m->enc_overlap[l] = 0;
   }
+  // LVSR_ENC_OVERLAP=0: every projection after the scan before it; LVSR_ENC_OVERLAP_SPIN_LIMIT: polls without scan
+  // progress after which the projection beside a scan stops claiming tiles (0: at its first tile that is not final)
+  const char* ov = getenv("LVSR_ENC_OVERLAP");
+  const bool overlap_on = m->use_tc && !(ov && atoi(ov) == 0);
+  const char* sl = getenv("LVSR_ENC_OVERLAP_SPIN_LIMIT");
+  const unsigned spin_limit = sl ? (unsigned)strtoul(sl, nullptr, 10) : LVSR_SPIN_LIMIT;
+  if (overlap_on && c.num_layers > 1) {
+    if (!m->enc_tiles) LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->enc_tiles), LVSR_MAX_LAYERS * 2 * sizeof(int)));
+    LVSR_CUDA_OK(cudaMemsetAsync(m->enc_tiles, 0, LVSR_MAX_LAYERS * 2 * sizeof(int), st));
+    // the claim records of every layer's projection (lvsr_model_encoder_overlap_claims)
+    size_t need = 0;
+    for (int l = 1, Tp = ceil_div(T, c.subsample[0]); l < c.num_layers; Tp = ceil_div(Tp, c.subsample[l]), ++l) {
+      m->enc_claims_off[l] = need;
+      need += 3 * (size_t)ceil_div(Tp * B, 128) * (6 * c.dims_bidir[l] / 128);
+    }
+    if (need > m->enc_claims_cap) {
+      if (m->enc_claims) LVSR_CUDA_OK(cudaFree(m->enc_claims));
+      m->enc_claims = nullptr;
+      m->enc_claims_cap = 0;
+      LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->enc_claims), need * sizeof(int)));
+      m->enc_claims_cap = need;
+    }
+    LVSR_CUDA_OK(cudaMemsetAsync(m->enc_claims, 0, need * sizeof(int), st));
+  }
+  float* pre_done = nullptr;   // this layer's pre-activations, when they were projected beside the previous scan
   for (int l = 0; l < c.num_layers; ++l) {
     const int D = c.dims_bidir[l], k = c.subsample[l];
     const int rows = Tl * B, Tout = ceil_div(Tl, k);
-    float* pre = ws.f32((size_t)rows * 6 * D);
+    float* pre = pre_done ? pre_done : ws.f32((size_t)rows * 6 * D);
     float* hext = tape ? ws.f32((size_t)(Tl + 2) * B * 2 * D) : nullptr;
     LVSR_CHECK(pre && (hext || !tape), "out of device memory (encoder pre-activations)");
-    // finalize splits the fork weights only while the tensor-core GEMM is on (null entry: a shape it refuses)
-    const size_t mark = ws.off;
     int32_t* plan = m->enc_plan[l];
-    int kpad = 0, operands = 0;
-    if (int rc = projection_gemm(ws, cur, rows, din, m->Wcat[l], m->use_tc ? &m->Wcat_tc[l] : nullptr, 6 * D, m->bcat[l],
-                                 pre, st, &kpad, &operands))
-      return rc;
-    plan[LVSR_ENC_PROJ] = kpad ? LVSR_ENC_PATH_TC : LVSR_ENC_PATH_FFMA;
-    plan[LVSR_ENC_KPAD] = kpad;
-    plan[LVSR_ENC_OPERANDS] = operands;
-    if (ws.off <= ws.cap) ws.off = mark;     // the split scratch is dead once the GEMM is enqueued (stream order)
+    if (!pre_done) {
+      // finalize splits the fork weights only while the tensor-core GEMM is on (null entry: a shape it refuses)
+      const size_t mark = ws.off;
+      int kpad = 0, operands = 0;
+      if (int rc = projection_gemm(ws, cur, rows, din, m->Wcat[l], m->use_tc ? &m->Wcat_tc[l] : nullptr, 6 * D, m->bcat[l],
+                                   pre, st, &kpad, &operands))
+        return rc;
+      plan[LVSR_ENC_PROJ] = kpad ? LVSR_ENC_PATH_TC : LVSR_ENC_PATH_FFMA;
+      plan[LVSR_ENC_KPAD] = kpad;
+      plan[LVSR_ENC_OPERANDS] = operands;
+      if (ws.off <= ws.cap) ws.off = mark;     // the split scratch is dead once the GEMM is enqueued (stream order)
+    }
+    pre_done = nullptr;
     float* out = (l == c.num_layers - 1) ? attended : ws.f32((size_t)Tout * B * 2 * D);
     LVSR_CHECK(out, "out of device memory (encoder layer output)");
     BiGruArgs a = {};
@@ -712,8 +777,60 @@ int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int
       a.tape = pre; a.hext = hext;
       tape[l] = {cur, pre, hext, out, Tl, Tout, din, D, k, mstride};
     }
+    // Layer l + 1's projection reads only this scan's output: its tiles can run beside the scan, on the SMs the scan
+    // leaves idle, as their rows become final -- when the scan runs in one wave of tensor-core clusters that leaves
+    // ENC_OVERLAP_MIN_SMS free and the projection takes fp16 operands
     BiGruPlan bp;
-    if (int rc = bigru_layer(a, st, &bp)) return rc;
+    if (int rc = bigru_plan(a, &bp)) return rc;
+    const int scan_ctas = bp.clusters * bp.cs, free_sms = device_sm_count() - scan_ctas;
+    const int l1 = l + 1, D1 = l1 < c.num_layers ? c.dims_bidir[l1] : 0, rows1 = Tout * B;
+    const bool overlap = overlap_on && l1 < c.num_layers && bp.kernel == LVSR_ENC_BIGRU_MMA && bp.waves == 1 &&
+                         free_sms >= ENC_OVERLAP_MIN_SMS && scan_ctas <= gemm_f16_stream_max_scan_ctas() &&
+                         m->Wcat_tc[l1].head && gemm_f16_stream_supported(rows1, 6 * D1, 2 * D);
+    if (!overlap) {
+      ProfScope prof("bigru", st);
+      if (int rc = bigru_layer(a, st, &bp)) return rc;
+    } else {
+      // the same arena order as without the overlap (pre-activations of l + 1 right after this layer's output), the
+      // split planes as projection_gemm takes them, then the scheduling area; all but the pre-activations dead after
+      float* pre1 = ws.f32((size_t)rows1 * 6 * D1);
+      const size_t mark = ws.off;
+      const int K1 = 2 * D;
+      float* a_hi = ws.f32((size_t)rows1 * K1);
+      float* a_lo = ws.f32((size_t)rows1 * K1);
+      int* sync = reinterpret_cast<int*>(ws.f32(gemm_f16_stream_sync_ints(rows1)));
+      LVSR_CHECK(pre1 && a_hi && a_lo && sync, "out of device memory (streamed projection)");
+      LVSR_CUDA_OK(cudaMemsetAsync(sync, 0, gemm_f16_stream_sync_ints(rows1) * sizeof(int), st));
+      a.progress = gemm_f16_stream_progress(sync);
+      __half* a_head = reinterpret_cast<__half*>(a_hi);
+      const TcWeights& tw = m->Wcat_tc[l1];
+      ProjStream ps = {sync, a.progress, scan_ctas, bp.cs, Tl, k, B, spin_limit, m->enc_tiles + 2 * l1,
+                       m->enc_claims + m->enc_claims_off[l1]};
+      {
+        // no event between the two launches: the projection must directly follow the scan in the stream.  The
+        // profiled "bigru" time therefore covers the scan and the projection tiles done beside it.
+        ProfScope prof("bigru", st);
+        if (int rc = bigru_layer(a, st, &bp)) return rc;
+        if (int rc = gemm_f16_stream(out, a_head, a_head + (size_t)rows1 * K1, reinterpret_cast<int*>(a_lo), rows1, K1,
+                                     tw.head, tw.tail, tw.ew, 6 * D1, m->bcat[l1], pre1, 6 * D1, ps, free_sms, st))
+          return rc;
+      }
+      {
+        ProfScope prof("gemm", st);
+        ps.progress = nullptr;
+        ps.tiles_done = m->enc_tiles + 2 * l1 + 1;
+        if (int rc = gemm_f16_stream(out, a_head, a_head + (size_t)rows1 * K1, reinterpret_cast<int*>(a_lo), rows1, K1,
+                                     tw.head, tw.tail, tw.ew, 6 * D1, m->bcat[l1], pre1, 6 * D1, ps, device_sm_count(), st))
+          return rc;
+      }
+      if (ws.off <= ws.cap) ws.off = mark;
+      int32_t* plan1 = m->enc_plan[l1];
+      plan1[LVSR_ENC_PROJ] = LVSR_ENC_PATH_TC;
+      plan1[LVSR_ENC_KPAD] = K1;
+      plan1[LVSR_ENC_OPERANDS] = LVSR_ENC_OPS_F16X3;
+      m->enc_overlap[l1] = 1;
+      pre_done = pre1;
+    }
     plan[LVSR_ENC_BIGRU] = bp.kernel;
     plan[LVSR_ENC_TAPE] = tape ? 1 : 0;
     plan[LVSR_ENC_RB] = bp.rb;

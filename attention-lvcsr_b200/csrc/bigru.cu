@@ -533,6 +533,7 @@ constexpr int MMA_CS = 4, MMA_WARPS = 8, EW_WARPS = 4, MMA_THREADS = (MMA_WARPS 
 // setmaxnreg redistributes the registers the CTA was LAUNCHED with (384 threads x 168), not the SM's whole file:
 // 256 * 224 + 128 * 56 = 64512 = 384 * 168
 constexpr int MMA_REGS = 224, EW_REGS = 56;
+constexpr int PROGRESS_EVERY = 16;   // steps between two publications of BiGruArgs::progress
 
 // Largest magnitude among the weights one warp turns into A fragments -> power-of-two scale that keeps the fp16 heads
 // far inside the fp16 range (|w| * scale <= 2^14); the warp multiplies its partial sums by the inverse.  Parameters of
@@ -609,6 +610,9 @@ bigru_mma_kernel(BiGruArgs a) {
   // every CTA of the cluster must be resident (and its mbarriers initialised) before any remote copy is issued
   __syncthreads();
   cluster_sync_all();
+  // a projection launched behind this scan as a programmatic dependent may start once every CTA of the scan runs: it
+  // then only takes SMs this launch does not need
+  asm volatile("griddepcontrol.launch_dependents;\n" ::: "memory");
   const bool tracing = g_bigru_trace_on && blockIdx.x == 0;
   const long long t_loop = clock64();
 
@@ -950,6 +954,15 @@ bigru_mma_kernel(BiGruArgs a) {
           if (pm_ptr) pm = __ldg(pm_ptr);
         }
       }
+      // every PROGRESS_EVERY steps and after the last: the output stores of the elementwise warps so far are visible
+      // at gpu scope, then one relaxed store says how many steps that covers (only these warps wait for it)
+      if (a.progress && ((s % PROGRESS_EVERY) == PROGRESS_EVERY - 1 || !more)) {
+        named_bar_sync(3, EW_WARPS * 32);
+        if (tid == 0) {
+          __threadfence();
+          asm volatile("st.relaxed.gpu.global.b32 [%0], %1;\n" ::"l"(a.progress + blockIdx.x), "r"(s + 1) : "memory");
+        }
+      }
       BG_STAMP(9);
       // advance t % subsample and t / subsample without dividing
       if (dir == 0) {
@@ -1078,9 +1091,8 @@ int launch_bigru_mma(const BiGruArgs& a, cudaStream_t stream, BiGruPlan* plan) {
 
 bool bigru_supported(int D) { return D == 128 || D == 256; }
 
-int bigru_layer(const BiGruArgs& a, cudaStream_t stream, BiGruPlan* plan) {
-  ProfScope prof("bigru", stream);
-  if (plan) *plan = {};
+int bigru_plan(const BiGruArgs& a, BiGruPlan* plan) {
+  *plan = {};
   if (a.T <= 0 || a.B <= 0) return 0;
   // hidden size 256: tensor-core products.  Clusters never talk to each other, so a batch with more clusters than the
   // device holds at once (mma_clusters_resident, from the occupancy query) simply runs in waves -- still
@@ -1097,13 +1109,28 @@ int bigru_layer(const BiGruArgs& a, cudaStream_t stream, BiGruPlan* plan) {
       rb = atoi(e);
       if (rb != 4 && rb != 8) return set_error("bigru: LVSR_BIGRU_RB=%s (expected 4 or 8)", e);
     }
-    return rb == 8 ? launch_bigru_mma<256, 8>(a, stream, plan) : launch_bigru_mma<256, 4>(a, stream, plan);
+    const int clusters = ceil_div(a.B, rb) * 2;
+    *plan = rb == 8 ? BiGruPlan{LVSR_ENC_BIGRU_MMA, 8, MMA_CS, clusters, mma_clusters_resident<256, 8>(), mma_waves<256, 8>(a.B)}
+                    : BiGruPlan{LVSR_ENC_BIGRU_MMA, 4, MMA_CS, clusters, mma_clusters_resident<256, 4>(), mma_waves<256, 4>(a.B)};
+    return 0;
   }
+  LVSR_CHECK(a.D == 128 || a.D == 256, "bigru: unsupported hidden size %d (supported: 128, 256)", a.D);
+  // the FFMA kernel's occupancy (resident, waves) is queried when it is launched
+  *plan = {LVSR_ENC_BIGRU_FFMA, RB, a.D == 256 ? 8 : 4, 2 * ceil_div(a.B, RB), 0, 0};
+  return 0;
+}
+
+// The FFMA kernel publishes no progress (BiGruArgs::progress is for the tensor-core kernel only).
+int bigru_layer(const BiGruArgs& a, cudaStream_t stream, BiGruPlan* plan) {
+  BiGruPlan pl;
+  if (plan) *plan = {};
+  if (int rc = bigru_plan(a, &pl)) return rc;
+  if (a.T <= 0 || a.B <= 0) return 0;
+  if (pl.kernel == LVSR_ENC_BIGRU_MMA)
+    return pl.rb == 8 ? launch_bigru_mma<256, 8>(a, stream, plan) : launch_bigru_mma<256, 4>(a, stream, plan);
   switch (a.D) {
     case 128: return launch_bigru<128, 4, 8>(a, stream, plan);
-    case 256: return launch_bigru<256, 8, 8>(a, stream, plan);
-    default:
-      return set_error("bigru: unsupported hidden size %d (supported: 128, 256)", a.D);
+    default: return launch_bigru<256, 8, 8>(a, stream, plan);
   }
 }
 

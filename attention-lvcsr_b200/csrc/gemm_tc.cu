@@ -28,6 +28,9 @@
 // projections of the metric configuration than this shape (tf32 operands).
 #include <cuda.h>
 #include <cuda_fp16.h>
+#include <limits.h>
+
+#include <algorithm>
 
 #include "kernels.h"
 
@@ -147,66 +150,38 @@ __device__ __forceinline__ float unscale(float x, int e) {
   return (unsigned)(e + 126) <= 252u ? x * __uint_as_float((uint32_t)(127 - e) << 23) : ldexpf(x, -e);
 }
 
-// F16 = false: tf32 hi/lo operands (m64n128k8); F16 = true: fp16 head/tail operands of rows and columns scaled by 2^ea,
-// 2^eb (m64n128k16), unscaled in the epilogue.
-// Persistent: each CTA walks the output tiles blockIdx.x, + gridDim.x, ... (N tiles fastest, then M tiles, then
-// splits), and the ring of stages runs on across tiles, so that the producer fills the next tile's first stages while
-// the consumers store the last one.  `it` counts the k-blocks a CTA has passed through the ring.
-template <bool F16>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
-               const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo,
-               TcGemmParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  // SWIZZLE_128B needs 1024-byte aligned tiles
-  uint8_t* tiles = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+// TMA producer, one thread: the k-blocks [kb0, kb0 + nkb) of output tile (m0, n0) into the ring of stages.  `it` counts
+// the k-blocks this CTA has passed through the ring.
+template <int BK>
+__device__ __forceinline__ void load_tile(const CUtensorMap* map_a_hi, const CUtensorMap* map_a_lo,
+                                          const CUtensorMap* map_b_hi, const CUtensorMap* map_b_lo, uint8_t* tiles,
+                                          unsigned long long* bars, int m0, int n0, int kb0, int nkb, uint32_t& it) {
+  for (int kb = 0; kb < nkb; ++kb, ++it) {
+    const uint32_t s = it % TC_STAGES;
+    const uint32_t ph = (it / TC_STAGES) & 1u;
+    bar_wait(smem_addr(&bars[TC_STAGES + s]), ph ^ 1u);       // slot free (first round passes immediately)
+    const uint32_t full = smem_addr(&bars[s]);
+    bar_expect_tx(full, TC_STAGE_BYTES);
+    const uint32_t base = smem_addr(tiles + (size_t)s * TC_STAGE_BYTES);
+    tma_load_2d(base + 0 * TC_TILE_BYTES, map_a_hi, (kb0 + kb) * BK, m0, full);
+    tma_load_2d(base + 1 * TC_TILE_BYTES, map_a_lo, (kb0 + kb) * BK, m0, full);
+    tma_load_2d(base + 2 * TC_TILE_BYTES, map_b_hi, (kb0 + kb) * BK, n0, full);
+    tma_load_2d(base + 3 * TC_TILE_BYTES, map_b_lo, (kb0 + kb) * BK, n0, full);
+  }
+}
+
+// Consumer warpgroup wg - 1 (rows [64 (wg - 1), +64) of the tile), thread t: the products of one output tile (N tiles
+// fastest, then M tiles, then splits) and its epilogue.  LDG_EA: the row exponents were written before this launch and
+// may come through the read-only cache; the streamed kernel writes them while it runs and reads them from L2.
+template <bool F16, bool LDG_EA>
+__device__ __forceinline__ void mma_store_tile(const TcGemmParams& p, uint8_t* tiles, unsigned long long* bars, int tile,
+                                               int wg, int t, uint32_t& it) {
   constexpr int NACC = TC_BN / 2;                       // accumulators per consumer thread (m64 x 128 over 128 threads)
   constexpr int BK = F16 ? TC_BK_F16 : TC_BK;           // values per 128-byte row
-  unsigned long long* bars = reinterpret_cast<unsigned long long*>(tiles + (size_t)TC_STAGES * TC_STAGE_BYTES);
-  // bars[0..S): full (TMA bytes landed), bars[S..2S): empty (both consumer warpgroups are done with the slot)
-
-  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
   const int total_kb = p.K / BK;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < TC_STAGES; ++s) {
-      bar_init(smem_addr(&bars[s]), 1);
-      bar_init(smem_addr(&bars[TC_STAGES + s]), 2);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
-  }
-  __syncthreads();
-
-  if (wg == 0) {
-    // ===== TMA producer =====
-    if (t == 0) {
-      uint32_t it = 0;
-      for (int tile = blockIdx.x; tile < p.tiles; tile += gridDim.x) {
-        const int n0 = (tile % p.tiles_n) * TC_BN, m0 = (tile / p.tiles_n % p.tiles_m) * TC_BM;
-        const int kb0 = tile / (p.tiles_n * p.tiles_m) * p.kb_per_split;
-        const int nkb = min(p.kb_per_split, total_kb - kb0);
-        for (int kb = 0; kb < nkb; ++kb, ++it) {
-          const uint32_t s = it % TC_STAGES;
-          const uint32_t ph = (it / TC_STAGES) & 1u;
-          bar_wait(smem_addr(&bars[TC_STAGES + s]), ph ^ 1u);       // slot free (first round passes immediately)
-          const uint32_t full = smem_addr(&bars[s]);
-          bar_expect_tx(full, TC_STAGE_BYTES);
-          const uint32_t base = smem_addr(tiles + (size_t)s * TC_STAGE_BYTES);
-          tma_load_2d(base + 0 * TC_TILE_BYTES, &map_a_hi, (kb0 + kb) * BK, m0, full);
-          tma_load_2d(base + 1 * TC_TILE_BYTES, &map_a_lo, (kb0 + kb) * BK, m0, full);
-          tma_load_2d(base + 2 * TC_TILE_BYTES, &map_b_hi, (kb0 + kb) * BK, n0, full);
-          tma_load_2d(base + 3 * TC_TILE_BYTES, &map_b_lo, (kb0 + kb) * BK, n0, full);
-        }
-      }
-    }
-    return;
-  }
-
-  // ===== consumers: warpgroup wg - 1 owns rows [64 (wg - 1), +64) of the tile =====
   const uint32_t a_off = (uint32_t)(wg - 1) * 64 * 128;          // 64 rows of 128 bytes into each A tile
   const int warp = t >> 5, lane = t & 31;
-  uint32_t it = 0;
-  for (int tile = blockIdx.x; tile < p.tiles; tile += gridDim.x) {
+  {
     const int n0 = (tile % p.tiles_n) * TC_BN, m0 = (tile / p.tiles_n % p.tiles_m) * TC_BM;
     const int split = tile / (p.tiles_n * p.tiles_m);
     const int nkb = min(p.kb_per_split, total_kb - split * p.kb_per_split);
@@ -253,7 +228,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
     }
     if constexpr (F16) {
 #pragma unroll
-      for (int h = 0; h < 2; ++h) ea[h] = r0 + 8 * h < p.M ? __ldg(p.ea + r0 + 8 * h) : 0;
+      for (int h = 0; h < 2; ++h)
+        ea[h] = r0 + 8 * h < p.M ? (LDG_EA ? __ldg(p.ea + r0 + 8 * h) : __ldcg(p.ea + r0 + 8 * h)) : 0;
     }
 #pragma unroll
     for (int j = 0; j < TC_BN / 8; ++j) {
@@ -270,6 +246,55 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
       }
     }
   }
+}
+
+__device__ __forceinline__ void init_ring(unsigned long long* bars) {
+  for (int s = 0; s < TC_STAGES; ++s) {
+    bar_init(smem_addr(&bars[s]), 1);
+    bar_init(smem_addr(&bars[TC_STAGES + s]), 2);
+  }
+}
+
+// F16 = false: tf32 hi/lo operands (m64n128k8); F16 = true: fp16 head/tail operands of rows and columns scaled by 2^ea,
+// 2^eb (m64n128k16), unscaled in the epilogue.
+// Persistent: each CTA walks the output tiles blockIdx.x, + gridDim.x, ... (N tiles fastest, then M tiles, then
+// splits), and the ring of stages runs on across tiles, so that the producer fills the next tile's first stages while
+// the consumers store the last one.
+template <bool F16>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
+               const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo,
+               TcGemmParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  // SWIZZLE_128B needs 1024-byte aligned tiles
+  uint8_t* tiles = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  constexpr int BK = F16 ? TC_BK_F16 : TC_BK;           // values per 128-byte row
+  unsigned long long* bars = reinterpret_cast<unsigned long long*>(tiles + (size_t)TC_STAGES * TC_STAGE_BYTES);
+  // bars[0..S): full (TMA bytes landed), bars[S..2S): empty (both consumer warpgroups are done with the slot)
+
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
+  const int total_kb = p.K / BK;
+
+  if (threadIdx.x == 0) {
+    init_ring(bars);
+    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+  }
+  __syncthreads();
+
+  uint32_t it = 0;
+  if (wg == 0) {
+    // ===== TMA producer =====
+    if (t == 0) {
+      for (int tile = blockIdx.x; tile < p.tiles; tile += gridDim.x) {
+        const int n0 = (tile % p.tiles_n) * TC_BN, m0 = (tile / p.tiles_n % p.tiles_m) * TC_BM;
+        const int kb0 = tile / (p.tiles_n * p.tiles_m) * p.kb_per_split;
+        load_tile<BK>(&map_a_hi, &map_a_lo, &map_b_hi, &map_b_lo, tiles, bars, m0, n0, kb0,
+                      min(p.kb_per_split, total_kb - kb0), it);
+      }
+    }
+    return;
+  }
+  for (int tile = blockIdx.x; tile < p.tiles; tile += gridDim.x) mma_store_tile<F16, true>(p, tiles, bars, tile, wg, t, it);
 }
 
 // ---- fp16 operands: power-of-two range scaling and the head/tail split -------------------------------------------------
@@ -314,6 +339,284 @@ __global__ void split_rows_f16_kernel(const float* __restrict__ x, __half* __res
     h2[i] = __halves2half2(hx, hy);
     t2[i] = __halves2half2(tx, ty);
   }
+}
+
+// ---- streamed fp16 projection ---------------------------------------------------------------------------------------
+// The fork GEMM of encoder layer l + 1 while the BiGRU scan of layer l still runs (api.cu: run_encoder).  Input frame t
+// of layer l + 1 is final once the forward scan has stored step t and the backward scan step T - 1 - t; the scan
+// publishes how many steps each of its CTAs has stored (bigru.cu).  gemm_f16_stream_kernel is gemm_tc_kernel<true> with
+// a dynamic tile schedule: warps 1..3 of the producer warpgroup claim output tiles from one counter, in the order their
+// rows become final (the middle m-tile first, then outward), split the tile's rows of A into fp16 head / tail planes and
+// exponents (split_rows_f16_kernel's rule) and hand the tile to the TMA thread and the consumers through a one-slot
+// queue; the split of an m-tile is shared out in 8-row chunks among the CTAs that claim its n-tiles.  Launched beside
+// the scan it claims only tiles whose rows are final and stops claiming when the scan has finished or has not
+// progressed for spin_limit polls; a second, stream-ordered launch on every SM (progress == null) runs the rest.
+// Every tile is computed exactly as gemm_tc_kernel<true> computes it, so the result does not depend on which launch did
+// which tile.
+constexpr int STREAM_CHUNK = 8;                          // rows per split work item
+constexpr int STREAM_CHUNKS = TC_BM / STREAM_CHUNK;      // ... per m-tile
+constexpr int STREAM_MAX_K = 1024;                       // a lane holds K / 128 float4 of each of two rows
+constexpr int STREAM_PROGRESS_MAX = 1024;                // scan CTAs that can publish progress
+
+struct StreamSched {
+  const float* A;          // [M, K] fp32 rows
+  __half *a_head, *a_tail; // [M, K] split planes (p.ea: the row exponents)
+  const int* progress;     // [nscan] steps stored per scan CTA; null: every row is final
+  int nscan, scan_cs;      // scan CTA i runs direction (i / scan_cs) & 1
+  int T, k, B;             // frames scanned, subsampling (output frame f = scan frame f k), batch rows per frame
+  int mid;                 // m-tile whose rows become final first
+  unsigned spin_limit;     // polls without progress before a launch beside the scan stops claiming
+  int* claim;              // next claim index
+  int* chunk_next;         // [tiles_m] split chunks handed out
+  int* chunk_done;         // [tiles_m] split chunks finished
+  int* tiles_done;         // tiles this launch claimed are added here
+  int* claims;             // [3 tiles] or null: (m-tile + 1, fwd, bwd) of each tile claimed beside the scan, with the
+                           // progress its rows were found final at
+};
+
+__device__ __forceinline__ int ld_acquire_i32(const int* p) {
+  int v;
+  asm volatile("ld.acquire.gpu.global.b32 %0, [%1];\n" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ int ld_relaxed_i32(const int* p) {
+  int v;
+  asm volatile("ld.relaxed.gpu.global.b32 %0, [%1];\n" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+// generic-proxy writes of the split planes <-> TMA (async-proxy) reads of them
+__device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;\n" ::: "memory"); }
+__device__ __forceinline__ void named_sync(int id, int count) { asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(count) : "memory"); }
+// mbarrier wait without the trap of bar_wait: the tile queue may wait for as long as the scan takes to make rows final
+__device__ __forceinline__ void bar_wait_sleep(uint32_t bar, uint32_t parity) {
+  uint32_t ok = 0;
+  while (true) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+        "selp.u32 %0, 1, 0, p;\n\t}\n"
+        : "=r"(ok)
+        : "r"(bar), "r"(parity)
+        : "memory");
+    if (ok) break;
+    __nanosleep(64);
+  }
+}
+
+// claim index i (in units of whole m-tiles) -> m-tile: mid, then alternately one further right and one further left
+__device__ __forceinline__ int stream_m_tile(int i, int mid, int tiles_m) {
+  if (i == 0) return mid;
+  const int j = i - 1, left = mid, right = tiles_m - 1 - mid, both = min(left, right);
+  if (j < 2 * both) return (j & 1) ? mid - 1 - (j >> 1) : mid + 1 + (j >> 1);
+  return right > left ? mid + 1 + j - both : mid - 1 - (j - both);
+}
+
+// One warp: the fewest steps any forward / backward scan CTA has published; spins counts the polls since they changed
+__device__ __forceinline__ void stream_poll(const StreamSched& s, int lane, int& fwd, int& bwd, unsigned& spins) {
+  int f = INT_MAX, b = INT_MAX;
+  for (int i = lane; i < s.nscan; i += 32) {
+    const int v = ld_acquire_i32(s.progress + i);
+    if ((i / s.scan_cs) & 1) b = min(b, v); else f = min(f, v);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    f = min(f, __shfl_xor_sync(0xffffffffu, f, o));
+    b = min(b, __shfl_xor_sync(0xffffffffu, b, o));
+  }
+  spins = (f == fwd && b == bwd) ? spins + 1 : 0;
+  fwd = f;
+  bwd = b;
+}
+__device__ __forceinline__ bool stream_ready(const StreamSched& s, const TcGemmParams& p, int c, int fwd, int bwd) {
+  const int m = stream_m_tile(c / p.tiles_n, s.mid, p.tiles_m);
+  const int r0 = m * TC_BM, r1 = min(r0 + TC_BM, p.M) - 1;
+  return fwd >= (r1 / s.B) * s.k + 1 && bwd >= s.T - (r0 / s.B) * s.k;
+}
+
+// One warp: claims the next tile (-1: none for this launch).  Beside the scan (s.progress set) a tile is claimed only
+// once the next one in claim order has its rows final, and no tile once the scan has finished or has not progressed for
+// spin_limit polls.  fwd / bwd / spins: stream_poll's state; polls_due: claims so far.
+__device__ int stream_claim(const StreamSched& s, const TcGemmParams& p, int lane, int& fwd, int& bwd, unsigned& spins,
+                           unsigned& polls_due) {
+  const int total = p.tiles_m * p.tiles_n;
+  if (!s.progress) {
+    const int c = __shfl_sync(0xffffffffu, lane == 0 ? atomicAdd(s.claim, 1) : 0, 0);
+    return c < total ? c : -1;
+  }
+  // the progress words are polled only when the last answer does not cover the next tile, and at every 4th claim to
+  // notice the end of the scan: every poll is 2 loads per lane of lines the scan writes
+  bool poll = (++polls_due & 3) == 0;
+  while (true) {
+    if (poll) stream_poll(s, lane, fwd, bwd, spins);
+    // the scan is done (or stalled and was waited for below): the launch on every SM takes the rest
+    if (fwd >= s.T && bwd >= s.T) return -1;
+    const int head = __shfl_sync(0xffffffffu, lane == 0 ? ld_relaxed_i32(s.claim) : 0, 0);
+    if (head >= total) return -1;
+    if (stream_ready(s, p, head, fwd, bwd)) break;
+    if (poll && spins >= s.spin_limit) return -1;
+    if (poll) __nanosleep(256);
+    poll = true;
+  }
+  const int c = __shfl_sync(0xffffffffu, lane == 0 ? atomicAdd(s.claim, 1) : 0, 0);
+  if (c >= total) return -1;
+  // other CTAs may have claimed the tiles up to c since the head was seen final: c follows within a few steps
+  while (!stream_ready(s, p, c, fwd, bwd)) {
+    if (spins >= s.spin_limit) {
+      // the scan stalls: this tile is claimed, so wait for the scan to end (its rows are final then); fwd = bwd = T
+      // makes the next stream_claim of this warp return -1, so the CTA stops after this tile
+      asm volatile("griddepcontrol.wait;\n" ::: "memory");
+      fwd = bwd = s.T;
+      break;
+    }
+    __nanosleep(256);
+    stream_poll(s, lane, fwd, bwd, spins);
+  }
+  if (lane == 0 && s.claims) {
+    s.claims[3LL * c] = stream_m_tile(c / p.tiles_n, s.mid, p.tiles_m) + 1;
+    s.claims[3LL * c + 1] = fwd;
+    s.claims[3LL * c + 2] = bwd;
+  }
+  return c;
+}
+
+// rows r0, r0 + 1 of A (r < M): exponent, head, tail -- split_rows_f16_kernel's rule, with both rows' loads in flight
+// at once and every load from L2 (other SMs wrote A while this kernel runs)
+__device__ __forceinline__ void stream_split_pair(const StreamSched& s, int* ea, long long r0, long long M, int K, int lane) {
+  constexpr int MAXV = STREAM_MAX_K / 128;
+  const int nv = K / 128;
+  float4 v[2][MAXV];
+#pragma unroll
+  for (int q = 0; q < 2; ++q)
+#pragma unroll
+    for (int i = 0; i < MAXV; ++i)
+      if (i < nv && r0 + q < M) v[q][i] = __ldcg(reinterpret_cast<const float4*>(s.A + (r0 + q) * K) + lane + 32 * i);
+#pragma unroll
+  for (int q = 0; q < 2; ++q) {
+    if (r0 + q >= M) break;
+    float mx = 0.f;
+#pragma unroll
+    for (int i = 0; i < MAXV; ++i)
+      if (i < nv) mx = fmaxf(mx, fmaxf(fmaxf(fabsf(v[q][i].x), fabsf(v[q][i].y)), fmaxf(fabsf(v[q][i].z), fabsf(v[q][i].w))));
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    const int er = f16_range_exponent(mx);
+    const float sc = exp2_int(er);
+    if (lane == 0) ea[r0 + q] = er;
+    uint2* h = reinterpret_cast<uint2*>(s.a_head + (r0 + q) * K);
+    uint2* tl = reinterpret_cast<uint2*>(s.a_tail + (r0 + q) * K);
+#pragma unroll
+    for (int i = 0; i < MAXV; ++i) {
+      if (i >= nv) break;
+      __half hx, hy, hz, hw, tx, ty, tz, tw;
+      split_f16(v[q][i].x * sc, hx, tx);
+      split_f16(v[q][i].y * sc, hy, ty);
+      split_f16(v[q][i].z * sc, hz, tz);
+      split_f16(v[q][i].w * sc, hw, tw);
+      const __half2 h01 = __halves2half2(hx, hy), h23 = __halves2half2(hz, hw);
+      const __half2 t01 = __halves2half2(tx, ty), t23 = __halves2half2(tz, tw);
+      h[lane + 32 * i] = make_uint2(*reinterpret_cast<const uint32_t*>(&h01), *reinterpret_cast<const uint32_t*>(&h23));
+      tl[lane + 32 * i] = make_uint2(*reinterpret_cast<const uint32_t*>(&t01), *reinterpret_cast<const uint32_t*>(&t23));
+    }
+  }
+}
+
+// One warp: takes 8-row chunks of m-tile m until none is left, then waits until every chunk (its own and those other
+// warps or CTAs took) is split
+__device__ __forceinline__ void stream_split_tile(const StreamSched& s, const TcGemmParams& p, int m, int lane) {
+  while (true) {
+    const int ch = __shfl_sync(0xffffffffu, lane == 0 ? atomicAdd(s.chunk_next + m, 1) : 0, 0);
+    if (ch >= STREAM_CHUNKS) break;
+    const long long r = (long long)m * TC_BM + ch * STREAM_CHUNK;
+    for (int q = 0; q < STREAM_CHUNK; q += 2) stream_split_pair(s, const_cast<int*>(p.ea), r + q, p.M, p.K, lane);
+    fence_proxy_async_global();
+    __syncwarp();
+    if (lane == 0) {
+      __threadfence();
+      atomicAdd(s.chunk_done + m, 1);
+    }
+  }
+  if (lane == 0)
+    while (ld_acquire_i32(s.chunk_done + m) < STREAM_CHUNKS) __nanosleep(128);
+  __syncwarp();
+}
+
+__global__ void __launch_bounds__(TC_THREADS, 1)
+gemm_f16_stream_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
+                       const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo,
+                       TcGemmParams p, StreamSched s) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* tiles = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  unsigned long long* bars = reinterpret_cast<unsigned long long*>(tiles + (size_t)TC_STAGES * TC_STAGE_BYTES);
+  // bars[0..2S): the ring as in gemm_tc_kernel; bars[2S]: a tile id is in the queue slot, bars[2S + 1]: the TMA thread
+  // and all 256 consumer threads have read it
+  volatile int* q_tile = reinterpret_cast<volatile int*>(bars + 2 * TC_STAGES + 2);
+  volatile int* q_claim = q_tile + 1;
+  const uint32_t q_full = smem_addr(&bars[2 * TC_STAGES]), q_empty = smem_addr(&bars[2 * TC_STAGES + 1]);
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+
+  if (threadIdx.x == 0) {
+    init_ring(bars);
+    bar_init(q_full, 1);
+    bar_init(q_empty, 1 + 256);
+    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+  }
+  __syncthreads();
+
+  uint32_t it = 0;
+  if (warp == 0) {
+    // ===== TMA thread =====
+    if (lane == 0) {
+      for (uint32_t n = 0;; ++n) {
+        bar_wait_sleep(q_full, n & 1u);
+        const int tile = *q_tile;
+        bar_arrive(q_empty);
+        if (tile < 0) break;
+        fence_proxy_async_global();
+        load_tile<TC_BK_F16>(&map_a_hi, &map_a_lo, &map_b_hi, &map_b_lo, tiles, bars, (tile / p.tiles_n) * TC_BM,
+                             (tile % p.tiles_n) * TC_BN, 0, p.K / TC_BK_F16, it);
+      }
+    }
+  } else if (wg == 0) {
+    // ===== warps 1..3: claim, split, queue =====
+    int fwd = -1, bwd = -1, claimed = 0;
+    unsigned spins = 0, polls_due = 0;
+    for (uint32_t n = 0;; ++n) {
+      bar_wait_sleep(q_empty, (n & 1u) ^ 1u);            // the slot is free (first round passes immediately)
+      if (warp == 1) {
+        const int c = stream_claim(s, p, lane, fwd, bwd, spins, polls_due);
+        if (lane == 0) *q_claim = c;
+      }
+      named_sync(1, 96);
+      const int c = *q_claim;
+      int tile = -1;
+      if (c >= 0) {
+        const int m = stream_m_tile(c / p.tiles_n, s.mid, p.tiles_m);
+        tile = m * p.tiles_n + c % p.tiles_n;
+        stream_split_tile(s, p, m, lane);
+      }
+      named_sync(1, 96);                                   // q_claim read by all, every chunk of the tile split
+      if (warp == 1 && lane == 0) {
+        *q_tile = tile;
+        bar_arrive(q_full);
+      }
+      if (c < 0) break;
+      ++claimed;
+    }
+    if (warp == 1 && lane == 0 && claimed) atomicAdd(s.tiles_done, claimed);
+  } else {
+    // ===== consumers =====
+    for (uint32_t n = 0;; ++n) {
+      bar_wait_sleep(q_full, n & 1u);
+      const int tile = *q_tile;
+      bar_arrive(q_empty);
+      if (tile < 0) break;
+      mma_store_tile<true, false>(p, tiles, bars, tile, wg, t, it);
+    }
+  }
+  // launched beside the scan: this kernel completes only after the scan has (no-op for a stream-ordered launch).  The
+  // whole warp waits together: lanes that reached the wait early would otherwise hold back a lane still issuing loads.
+  __syncwarp();
+  asm volatile("griddepcontrol.wait;\n" ::: "memory");
 }
 
 // W [K, N] row-major -> K-major head / tail [N, K] of every column n scaled by 2^e[n] (weights, once per finalize).
@@ -565,6 +868,76 @@ int gemm_f16(const float* A, __half* A_head, __half* A_tail, int* ea, int M, int
       A, A_head, A_tail, ea, M, K);
   LVSR_LAUNCH_CHECK();
   return launch_tc<true>(A_head, A_tail, ea, M, Wt_head, Wt_tail, ew, N, K, bias, C, ldc, 1, 0, stream);
+}
+
+// stream_split_pair moves whole float4 groups, K / 128 per lane and row
+bool gemm_f16_stream_supported(int M, int N, int K) {
+  return gemm_f16_supported(M, N, K) && K % 128 == 0 && K <= STREAM_MAX_K;
+}
+
+// [claim | pad | progress [STREAM_PROGRESS_MAX] | chunk_next [tiles_m] | chunk_done [tiles_m]]
+size_t gemm_f16_stream_sync_ints(int M) { return 32 + STREAM_PROGRESS_MAX + 2 * (size_t)ceil_div(M, TC_BM); }
+int* gemm_f16_stream_progress(int* sync) { return sync + 32; }
+int gemm_f16_stream_max_scan_ctas() { return STREAM_PROGRESS_MAX; }
+
+int gemm_f16_stream(const float* A, __half* A_head, __half* A_tail, int* ea, int M, int K, const __half* Wt_head,
+                    const __half* Wt_tail, const int* ew, int N, const float* bias, float* C, int ldc,
+                    const ProjStream& ps, int grid, cudaStream_t stream) {
+  LVSR_CHECK(gemm_f16_stream_supported(M, N, K) && ps.nscan <= STREAM_PROGRESS_MAX && grid >= 1 && ps.k >= 1 &&
+                 (long long)ceil_div(ps.T, ps.k) * ps.B == M,
+             "gemm_f16_stream: unsupported shape M=%d N=%d K=%d (T=%d k=%d B=%d)", M, N, K, ps.T, ps.k, ps.B);
+  if (int rc = get_encode()) return rc;
+  CUtensorMap ma_hi, ma_lo, mb_hi, mb_lo;
+  if (int rc = make_map(&ma_hi, A_head, M, K, true)) return rc;
+  if (int rc = make_map(&ma_lo, A_tail, M, K, true)) return rc;
+  if (int rc = make_map(&mb_hi, Wt_head, N, K, true)) return rc;
+  if (int rc = make_map(&mb_lo, Wt_tail, N, K, true)) return rc;
+  static bool configured[LVSR_MAX_DEVICES] = {false};
+  const int dev = current_device();
+  if (!configured[dev]) {
+    LVSR_CUDA_OK(cudaFuncSetAttribute(gemm_f16_stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM));
+    configured[dev] = true;
+  }
+  TcGemmParams p;
+  p.C = C; p.bias = bias; p.ea = ea; p.eb = ew; p.M = M; p.N = N; p.K = K; p.ldc = ldc;
+  p.kb_per_split = K / TC_BK_F16;
+  p.c_split_stride = 0;
+  p.tiles_n = N / TC_BN;
+  p.tiles_m = ceil_div(M, TC_BM);
+  LVSR_CHECK((long long)p.tiles_n * p.tiles_m <= INT32_MAX, "gemm_f16_stream: too many tiles (M=%d N=%d)", M, N);
+  p.tiles = p.tiles_n * p.tiles_m;
+  StreamSched s;
+  s.A = A; s.a_head = A_head; s.a_tail = A_tail;
+  s.progress = ps.progress;
+  s.nscan = ps.nscan; s.scan_cs = ps.scan_cs; s.T = ps.T; s.k = ps.k; s.B = ps.B;
+  // the frame the two scan directions finish first: the fewest steps max(f k + 1, T - f k) of both
+  int best = INT_MAX, fmid = 0;
+  for (int f = 0; f * ps.k < ps.T; ++f) {
+    const int ready = std::max(f * ps.k + 1, ps.T - f * ps.k);
+    if (ready < best) { best = ready; fmid = f; }
+  }
+  s.mid = std::min((int)((long long)fmid * ps.B / TC_BM), p.tiles_m - 1);
+  s.spin_limit = ps.spin_limit;
+  s.claim = ps.sync;
+  s.chunk_next = ps.sync + 32 + STREAM_PROGRESS_MAX;
+  s.chunk_done = s.chunk_next + p.tiles_m;
+  s.tiles_done = ps.tiles_done;
+  s.claims = ps.progress ? ps.claims : nullptr;
+  // beside the scan: a programmatic dependent launch, started once every scan CTA runs (griddepcontrol.launch_dependents
+  // after its entry barrier), so its CTAs only take SMs the scan does not need
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(std::min(grid, p.tiles));
+  cfg.blockDim = dim3(TC_THREADS);
+  cfg.dynamicSmemBytes = TC_SMEM;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = ps.progress ? 1 : 0;
+  LVSR_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_f16_stream_kernel, ma_hi, ma_lo, mb_hi, mb_lo, p, s));
+  LVSR_LAUNCH_CHECK();
+  return 0;
 }
 
 }  // namespace lvsr

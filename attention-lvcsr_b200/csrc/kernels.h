@@ -45,6 +45,28 @@ bool gemm_f16_supported(int M, int N, int K);      // K a multiple of 64: fp16 o
 int split_weight_f16(const float* W, int K, int N, __half* Wt_head, __half* Wt_tail, int* ew, cudaStream_t stream);
 int gemm_f16(const float* A, __half* A_head, __half* A_tail, int* ea, int M, int K, const __half* Wt_head,
              const __half* Wt_tail, const int* ew, int N, const float* bias, float* C, int ldc, cudaStream_t stream);
+// The same product streamed behind the BiGRU scan that writes A (gemm_tc.cu: gemm_f16_stream_kernel): the kernel splits
+// A itself, tile by tile, once the tile's rows are final.  A = the scan's output [ceil(T / k), B, K].  Two launches
+// share one zeroed scheduling area `sync` (gemm_f16_stream_sync_ints(M) ints, zeroed before the scan starts): with
+// `progress` set, right after the scan and beside it, on the SMs the scan leaves free; then with progress == null, on
+// every SM, for the tiles the first launch did not claim.  Each adds the tiles it claimed to *tiles_done.
+struct ProjStream {
+  int* sync;
+  const int* progress;     // gemm_f16_stream_progress(sync), handed to the scan (BiGruArgs::progress), or null
+  int nscan, scan_cs;      // CTAs of the scan and CTAs per cluster (scan CTA i runs direction (i / scan_cs) & 1)
+  int T, k, B;             // frames the scan runs, its subsampling, batch rows
+  unsigned spin_limit;     // polls without progress before the launch beside the scan stops claiming
+  int* tiles_done;
+  int* claims;             // [3 x tiles] or null: the launch beside the scan records (m-tile + 1, forward and backward
+                           // progress) of each tile it claims, at the progress it found the tile's rows final
+};
+bool gemm_f16_stream_supported(int M, int N, int K);
+size_t gemm_f16_stream_sync_ints(int M);
+int* gemm_f16_stream_progress(int* sync);
+int gemm_f16_stream_max_scan_ctas();
+int gemm_f16_stream(const float* A, __half* A_head, __half* A_tail, int* ea, int M, int K, const __half* Wt_head,
+                    const __half* Wt_tail, const int* ew, int N, const float* bias, float* C, int ldc,
+                    const ProjStream& ps, int grid, cudaStream_t stream);
 
 // ---- bigru.cu -----------------------------------------------------------------------
 struct BiGruArgs {
@@ -59,11 +81,15 @@ struct BiGruArgs {
   float* tape;             // = pre, written in place: candidate c over the inputs slot, z / r over the gate slots
   float* hext;             // [(T+2), B, 2D]: slot t+1 = states after time t; slot 0 (forward half) and slot T+1
                            // (backward half) = the broadcast initial states
+  // optional, tensor-core kernel only: progress[cta] = time steps whose output stores that CTA has made visible at gpu
+  // scope (published every few steps and after the last), for a projection streamed behind the scan
+  int* progress;
 };
 bool bigru_supported(int D);
 // what bigru_layer launched (lvsr_model_encoder_plan): kernel LVSR_ENC_BIGRU_*, rows and CTAs per cluster, clusters,
 // the clusters of that kernel the device holds at once (occupancy query) and the waves that makes
 struct BiGruPlan { int kernel, rb, cs, clusters, resident, waves; };
+int bigru_plan(const BiGruArgs& a, BiGruPlan* plan);   // what bigru_layer would launch for a, without launching
 int bigru_layer(const BiGruArgs& a, cudaStream_t stream, BiGruPlan* plan = nullptr);
 
 // ---- bigru_bwd.cu: reverse-time scan of one layer (training) ------------------------------

@@ -138,6 +138,12 @@ struct lvsr_model {
   int32_t dec_plan[16] = {0};       // plan of the last lvsr_cost_matrix (lvsr_model_decoder_plan, LVSR_PLAN_* slots)
   int att_cs = 0;                   // cluster size of the last attention_step launch
   int32_t enc_plan[LVSR_MAX_LAYERS][16] = {};   // per layer: lvsr_model_encoder_plan's LVSR_ENC_* slots
+  // per layer: 1 when the last encoder forward streamed its projection behind the previous layer's scan
+  int32_t enc_overlap[LVSR_MAX_LAYERS] = {};
+  int* enc_tiles = nullptr;         // device [LVSR_MAX_LAYERS][2]: tiles of those projections done beside / after the scan
+  int* enc_claims = nullptr;        // device: ProjStream::claims of every layer, layer l at enc_claims_off[l]
+  size_t enc_claims_cap = 0;        // ints allocated
+  size_t enc_claims_off[LVSR_MAX_LAYERS] = {};
   int32_t pre_plan[3] = {0, 0, 0};  // last lvsr_preprocess: path (LVSR_ENC_PATH_*), Kpad, operands (LVSR_ENC_OPS_*)
   bool finalized = false;
   // ---- FST language model (lvsr_model_set_lm); lm_off == nullptr: none attached ----

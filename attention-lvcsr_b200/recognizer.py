@@ -443,16 +443,33 @@ class SpeechRecognizer(object):
         plan["bigru"] = _lib.ENC_BIGRU_KERNELS[plan["bigru"]]
         plan["operands"] = _lib.ENC_OPERANDS[plan["operands"]]
         plan["tape"] = bool(plan["tape"])
+        if layer >= 0:
+            ov = (C.c_int32 * 3)()
+            _lib.check(lib.lvsr_model_encoder_overlap(h, int(layer), ov))
+            plan["overlap"], plan["tiles_beside"], plan["tiles_after"] = bool(ov[0]), int(ov[1]), int(ov[2])
         return plan
+
+    def encoder_overlap_claims(self, layer, tiles):
+        """lvsr_model_encoder_overlap_claims: int32 [tiles, 3], row c = (m-tile + 1, forward and backward scan progress)
+        at which the projection of `layer` claimed its tile c beside the previous scan (zeros: done after the scan)."""
+        import ctypes as C
+        import numpy as np
+        lib, h = _lib.load(), self._require_ready()
+        out = np.zeros((int(tiles), 3), dtype=np.int32)
+        _lib.check(lib.lvsr_model_encoder_overlap_claims(h, int(layer), out.ctypes.data_as(C.POINTER(C.c_int32)),
+                                                         out.size))
+        return out
 
     def encoder_plan(self):
         """What the encoder ran (lvsr_model_encoder_plan), one dict per layer.  Of the last encoder forward: proj (fork
         projection GEMM: "tc" or "ffma"), kpad (its contraction as the tensor-core GEMM stores it, 0 on FFMA), operands
         (of that tensor-core GEMM: "f16x3" when the contraction is a multiple of 64, else "tf32x3"; None on FFMA), bigru
         ("mma" or "ffma"), tape (a training forward), rb and cs (rows and CTAs per cluster), clusters, resident (clusters
-        of that kernel the device holds at once), waves and T (frames scanned).  Of the last training step: bwd_cs
-        (CTAs per cluster of the reverse-time scan), wgrad ("tc" or "ffma"), wgrad_splits, wgrad_kpad (the padded
-        contraction over T*B rows, 0 on FFMA) and dx ("tc", "ffma", or None for layer 0).  None / 0: not run."""
+        of that kernel the device holds at once), waves and T (frames scanned); overlap (the projection ran beside the
+        previous layer's scan, lvsr_model_encoder_overlap), tiles_beside and tiles_after (its output tiles computed
+        beside that scan and after it).  Of the last training step: bwd_cs (CTAs per cluster of the reverse-time scan),
+        wgrad ("tc" or "ffma"), wgrad_splits, wgrad_kpad (the padded contraction over T*B rows, 0 on FFMA) and dx ("tc",
+        "ffma", or None for layer 0).  None / 0: not run."""
         return [self._encoder_plan_row(l) for l in range(len(self.net["dims_bidir"]))]
 
     def preprocess_plan(self):

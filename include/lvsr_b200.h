@@ -156,6 +156,15 @@ enum { LVSR_ENC_PATH_NONE = 0, LVSR_ENC_PATH_TC = 1, LVSR_ENC_PATH_FFMA = 2 };
 enum { LVSR_ENC_OPS_NONE = 0, LVSR_ENC_OPS_TF32X3 = 1, LVSR_ENC_OPS_F16X3 = 2 };
 enum { LVSR_ENC_BIGRU_NONE = 0, LVSR_ENC_BIGRU_FFMA = 1, LVSR_ENC_BIGRU_MMA = 2 };
 int lvsr_model_encoder_plan(const lvsr_model* m, int32_t layer, int32_t out[16]);
+/* Projection of encoder layer 1 <= layer < num_layers in the LAST encoder forward (synchronises with the device):
+ * out[0] = 1 when it ran beside the BiGRU scan of layer - 1, streamed tile by tile as the scan's output became final
+ * (DESIGN §4; LVSR_ENC_OVERLAP=0 turns that off), else 0; out[1] / out[2] = its 128 x 128 output tiles computed beside
+ * the scan / by the launch on every SM after it (both 0 when out[0] is 0).  Layer 0 always reports zeros. */
+int lvsr_model_encoder_overlap(lvsr_model* m, int32_t layer, int32_t out[3]);
+/* For such a layer (out[0] == 1): per output tile c in claim order, out[3 c .. 3 c + 2] = (m-tile + 1, forward and backward
+ * scan progress) at which the launch beside the scan found the tile's rows final and claimed it, zeros for the tiles
+ * the launch after the scan did; count ints, at most 3 x the layer's tiles.  Synchronises with the device. */
+int lvsr_model_encoder_overlap_claims(lvsr_model* m, int32_t layer, int32_t* out, int64_t count);
 
 /* ---- encoder: BeamSearch.context_computer / Encoder.apply -------------------------
  * (libs/blocks/blocks/search.py:97-99; lvsr/bricks/__init__.py:71-78).
