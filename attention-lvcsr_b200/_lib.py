@@ -65,6 +65,15 @@ class LvsrTrainConfig(C.Structure):
                 ("epsilon", C.c_float), ("max_norm", C.c_float), ("burn_in_steps", C.c_int32), ("decay", C.c_float)]
 
 
+class LvsrAdaptiveNoise(C.Structure):
+    """Mirror of ``lvsr_adaptive_noise`` (include/lvsr_b200.h)."""
+    _fields_ = [("init_sigma", C.c_double), ("model_cost_coefficient", C.c_double), ("num_examples", C.c_int64),
+                ("seed", C.c_uint64)]
+
+
+# slots of lvsr_train_noise_stats (LVSR_NOISE_*), under the reference's monitor names (lvsr/main.py:440-460)
+NOISE_STATS = ("model_cost", "model_prior_mean", "model_prior_variance")
+
 LM_MAX_STATES = 7
 
 
@@ -122,6 +131,13 @@ SIGNATURES = {
     "lvsr_train_apply_updates": (C.c_int, [_P, _P, C.c_float, C.POINTER(LvsrTrainConfig), _P]),
     "lvsr_train_gradient_norm": (C.c_int, [_P, C.POINTER(C.c_float)]),
     "lvsr_train_reset": (C.c_int, [_P]),
+    "lvsr_train_set_adaptive_noise": (C.c_int, [_P, C.POINTER(LvsrAdaptiveNoise)]),
+    "lvsr_train_get_noise_param": (C.c_int, [_P, C.c_int, _P, C.c_int64]),
+    "lvsr_train_set_noise_param": (C.c_int, [_P, C.c_int, _P, C.c_int64]),
+    "lvsr_train_noise_stats": (C.c_int, [_P, C.POINTER(C.c_double)]),
+    "lvsr_train_noise_sample": (C.c_int, [_P, C.c_int64, _P, _P]),
+    "lvsr_train_noise_params": (C.c_int, [_P, _P, _P]),
+    "lvsr_train_noise_gradients": (C.c_int, [_P, _P, C.c_float, _P, _P]),
     "lvsr_launch_count": (C.c_int64, [C.c_int]),
     "lvsr_profile_enable": (C.c_int, [C.c_int]),
     "lvsr_profile_read": (C.c_int, [C.c_char_p, C.POINTER(C.c_double), C.POINTER(C.c_int64)]),

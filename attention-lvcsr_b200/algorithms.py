@@ -14,11 +14,26 @@ flat gradient buffer together with the local batch size and cost, and every repl
 update with 1 / (global batch size).
 """
 import ctypes as C
+import logging
 from collections import OrderedDict
 
 import numpy as np
 
 from . import _lib
+
+logger = logging.getLogger(__name__)
+
+# Adaptive weight noise (lvsr/graph.py:71-251): the log-variance of parameter p belongs to the top-level
+# NoiseBrick(name='adaptive_noise') and is named after p's owner path without the leading slash (graph.py:57-68,
+# 173-177), so Model.get_parameter_dict (B/model.py:78-88, B/select.py:199-220) calls it
+# "/adaptive_noise.recognizer/encoder/bidir0/forward/fork/fork_inputs.W".
+NOISE_BRICK = "adaptive_noise"
+ADAPTIVE_NOISE_DEFAULTS = dict(init_sigma=1e-6, model_cost_coefficient=1.0, seed=None)   # graph.py:71-80
+
+
+def noise_parameter_name(name):
+    """Blocks name of the adaptive-noise log-variance of the parameter called `name`."""
+    return "/%s.%s" % (NOISE_BRICK, name.lstrip("/"))
 
 
 class StepRule(object):
@@ -183,10 +198,18 @@ class GradientDescent(object):
     ``last_cost`` after ``process_batch`` is the reference's ``sequence_total_cost``, sum(cost_matrix) / batch size
     (lvsr/main.py:340-344), WITHOUT the decay term: the gradient includes decay * ||WEIGHT parameters||^2, the reported
     cost does not (it is ``train_cost`` minus that penalty), so costs stay comparable across decay settings and
-    no extra reduction over the parameters runs per step."""
+    no extra reduction over the parameters runs per step.
+
+    adaptive_noise: config['regularization']['adaptive_noise'] plus ``num_examples`` (lvsr/main.py:425-437):
+    dict(num_examples, init_sigma=1e-6, model_cost_coefficient=1.0, seed=None); seed None or 0 is Blocks'
+    default_seed, 1.  Every step then runs forward and backward on parameters perturbed by Gaussian noise whose
+    log-variances are trained with the parameters (lvsr/graph.py:71-251; include/lvsr_b200.h).  Decay has no effect
+    on the step under adaptive noise: like the reference, an error is logged and decay is dropped.  ``last_cost``
+    stays the task cost; ``last_model_cost``, ``model_prior_mean`` and ``model_prior_variance`` report the rest.
+    Inference (cost, search, sampling) always uses the means."""
 
     def __init__(self, recognizer=None, step_rule=None, decay=0.0, cost=None, parameters=None, gradients=None,
-                 on_unused_sources="warn", **kwargs):
+                 on_unused_sources="warn", adaptive_noise=None, **kwargs):
         if recognizer is None:
             raise ValueError("GradientDescent needs the recognizer (no symbolic cost exists in the CUDA path)")
         if getattr(recognizer, "lm", None):
@@ -195,6 +218,21 @@ class GradientDescent(object):
                                       "inference only)")
         self.recognizer = recognizer
         self.step_rule = step_rule if step_rule is not None else CompositeRule([Scale(), RemoveNotFinite(0.0)])
+        self.adaptive_noise = None
+        if adaptive_noise:
+            unknown = set(adaptive_noise) - set(ADAPTIVE_NOISE_DEFAULTS) - {"num_examples"}
+            if unknown:
+                raise TypeError("adaptive_noise: unknown arguments %s" % sorted(unknown))
+            if "num_examples" not in adaptive_noise:
+                raise ValueError("adaptive_noise needs num_examples, the size of the training set (lvsr/main.py:434)")
+            an = dict(ADAPTIVE_NOISE_DEFAULTS, **adaptive_noise)
+            self.adaptive_noise = dict(num_examples=int(an["num_examples"]), init_sigma=float(an["init_sigma"]),
+                                       model_cost_coefficient=float(an["model_cost_coefficient"]),
+                                       seed=int(an["seed"] or 1))
+            if decay > 0:
+                # lvsr/main.py:427-430; the gradients are those of the cost without the decay term (:431-437)
+                logger.error("using  adaptive noise with alignment weight panalty or weight decay is probably stupid")
+                decay = 0.0
         self._tc = _to_train_config(self.step_rule, decay)
         self.on_unused_sources = on_unused_sources
         self._grads = None
@@ -216,6 +254,12 @@ class GradientDescent(object):
         self._cost = torch.zeros((1,), dtype=torch.float32, device=rec.device)
         self._n = n
         _lib.check(lib.lvsr_train_reset(h))
+        if self.adaptive_noise:
+            an = self.adaptive_noise
+            cfg = _lib.LvsrAdaptiveNoise(init_sigma=an["init_sigma"], model_cost_coefficient=an["model_cost_coefficient"],
+                                         num_examples=an["num_examples"], seed=an["seed"])
+            _lib.check(lib.lvsr_train_set_adaptive_noise(h, C.byref(cfg)))
+            self._noise_grads = torch.zeros((n,), dtype=torch.float32, device=rec.device)
 
     def _world(self):
         import torch.distributed as dist
@@ -224,20 +268,88 @@ class GradientDescent(object):
         return None, 1
 
     def cost_and_gradients(self, batch):
-        """(cost, {parameter name: gradient}) of sum(cost_matrix)/B for this batch on this GPU (no update)."""
+        """(cost, {parameter name: gradient}) of sum(cost_matrix)/B for this batch on this GPU (no update).  Under
+        adaptive noise: the gradients of the reference (lvsr/graph.py:238-249) at this update's noise, the means'
+        first, then the log-variances' under their Blocks names."""
         rec = self.recognizer
         if self._buf is None:
             self.initialize()
         B = self._forward_backward(batch, None)
         import ctypes as C_
         lib, h = _lib.load(), rec._require_ready()
+        if self.adaptive_noise:
+            _lib.check(lib.lvsr_train_noise_gradients(h, self._buf.data_ptr(), 1.0, self._noise_grads.data_ptr(),
+                                                      rec._stream()))
         flat = self._buf[:self._n].cpu().numpy()
         out = OrderedDict()
-        for i, (name, shape) in enumerate(rec.parameter_shapes().items()):
-            off, cnt = C_.c_int64(), C_.c_int64()
-            _lib.check(lib.lvsr_model_param_offset(h, i, C_.byref(off), C_.byref(cnt)))
-            out[name] = flat[off.value:off.value + cnt.value].reshape(shape).copy()
+        for (name, (off, cnt)), shape in zip(self._offsets().items(), rec.parameter_shapes().values()):
+            out[name] = flat[off:off + cnt].reshape(shape).copy()
+        if self.adaptive_noise:
+            flat = self._noise_grads.cpu().numpy()
+            for (name, (off, cnt)), shape in zip(self._offsets().items(), rec.parameter_shapes().values()):
+                out[noise_parameter_name(name)] = flat[off:off + cnt].reshape(shape).copy()
         return float(self._cost.item()), out
+
+    def _offsets(self):
+        """{parameter name: (flat offset, element count)}."""
+        lib, h = _lib.load(), self.recognizer._require_ready()
+        out = OrderedDict()
+        for i in range(lib.lvsr_model_num_params(h)):
+            off, cnt = C.c_int64(), C.c_int64()
+            _lib.check(lib.lvsr_model_param_offset(h, i, C.byref(off), C.byref(cnt)))
+            out[lib.lvsr_model_param_name(h, i).decode()] = (off.value, cnt.value)
+        return out
+
+    # ---- adaptive weight noise ------------------------------------------------------------------------------------
+    def _require_noise(self):
+        if not self.adaptive_noise:
+            raise RuntimeError("adaptive noise is off (GradientDescent(adaptive_noise=...))")
+        if self._buf is None:
+            self.initialize()
+        return _lib.load(), self.recognizer._require_ready()
+
+    def noise_parameter_values(self):
+        """{Blocks name of the noise parameter ("/adaptive_noise.recognizer/..."): log-variance ndarray}."""
+        lib, h = self._require_noise()
+        out = OrderedDict()
+        for i, (name, shape) in enumerate(self.recognizer.parameter_shapes().items()):
+            arr = np.empty(shape, dtype=np.float32)
+            _lib.check(lib.lvsr_train_get_noise_param(h, i, arr.ctypes.data, arr.size))
+            out[noise_parameter_name(name)] = arr
+        return out
+
+    def set_noise_parameter_values(self, values):
+        """Set log-variances by their Blocks names; the others keep their values."""
+        lib, h = self._require_noise()
+        index = OrderedDict((noise_parameter_name(n), (i, s))
+                            for i, (n, s) in enumerate(self.recognizer.parameter_shapes().items()))
+        for name, value in values.items():
+            if name not in index:
+                raise KeyError("unknown noise parameter %s" % name)
+            i, shape = index[name]
+            arr = np.ascontiguousarray(value, dtype=np.float32)
+            if tuple(arr.shape) != shape:
+                raise ValueError("noise parameter %s: expected shape %s, got %s" % (name, shape, arr.shape))
+            _lib.check(lib.lvsr_train_set_noise_param(h, i, arr.ctypes.data, arr.size))
+
+    def noise_stats(self):
+        """{model_cost, model_prior_mean, model_prior_variance} of the last training forward (synchronises)."""
+        lib, h = self._require_noise()
+        out = (C.c_double * 3)()
+        _lib.check(lib.lvsr_train_noise_stats(h, out))
+        return OrderedDict(zip(_lib.NOISE_STATS, (float(v) for v in out)))
+
+    @property
+    def last_model_cost(self):
+        return self.noise_stats()["model_cost"] if self.adaptive_noise else None
+
+    @property
+    def model_prior_mean(self):
+        return self.noise_stats()["model_prior_mean"] if self.adaptive_noise else None
+
+    @property
+    def model_prior_variance(self):
+        return self.noise_stats()["model_prior_variance"] if self.adaptive_noise else None
 
     def _forward_backward(self, batch, gscale):
         rec = self.recognizer

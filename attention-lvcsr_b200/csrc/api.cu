@@ -392,6 +392,7 @@ int lvsr_model_destroy(lvsr_model* m) {
   if (m->opt_scratch) cudaFree(m->opt_scratch);
   if (m->opt_desc) cudaFree(m->opt_desc);
   lvsr_model_clear_lm(m);
+  noise_free(m);
   m->tws.destroy();
   m->ws.destroy();
   delete m;

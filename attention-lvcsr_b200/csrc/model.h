@@ -160,6 +160,25 @@ struct lvsr_model {
   float* opt_scratch = nullptr;     // [1024 partial sums | norm]
   void* opt_desc = nullptr;         // device copy of the per-parameter table (train::ParamDesc)
   long long burn_in_left = -1;      // BurnIn counter (-1: not started)
+  // ---- adaptive weight noise (noise.cu; lvsr_train_set_adaptive_noise) ----
+  struct Noise {
+    bool on = false;
+    lvsr_adaptive_noise cfg = {};
+    long long update = 0;           // update counter of the eps draw; advanced by lvsr_train_apply_updates
+    bool sampled = false;           // a sample pass ran since the last update (its priors feed the gradients)
+    bool stale = false;             // an update left the packed weights un-built (the next training forward packs
+                                    // its noisy copy; any other entry point first waits for the update, check_ready)
+    float* mem = nullptr;           // the one allocation of the buffers below (flat layout each, padding zero)
+    float* ls2 = nullptr;           // log-variance parameters
+    float* noisy = nullptr;         // means + eps * sigma of the current step
+    float* gls2 = nullptr;          // gradients, then steps, of ls2
+    float *velocity = nullptr, *ms_step = nullptr, *ms_dx = nullptr;   // optimizer state of ls2
+    void* aux = nullptr;            // the one allocation of the tables below
+    void* spans = nullptr;          // device [params]: (offset, count) of every parameter, padding excluded
+    double* stats = nullptr;        // device [LVSR_NOISE_*]: model cost, prior mean, prior variance, element count
+    double* part = nullptr;         // device partial sums of the sample pass
+    float* norm_part = nullptr;     // device partial squared norms of the gradient transform
+  } noise;
 
   float* P(const std::string& n) const {
     auto it = index.find(n);
@@ -222,7 +241,13 @@ struct ArenaScope {
 
 static inline int check_ready(lvsr_model* m) {
   LVSR_CHECK(m != nullptr, "null model");
-  if (!m->finalized) return lvsr_model_finalize(m);
+  if (!m->finalized) {
+    if (m->noise.stale) {             // the update may still run on its own stream: pack the means once it is done
+      LVSR_CUDA_OK(cudaDeviceSynchronize());
+      m->noise.stale = false;
+    }
+    return lvsr_model_finalize(m);
+  }
   return 0;
 }
 
@@ -238,6 +263,12 @@ struct LayerTape {
 
 // shared orchestration pieces (api.cu)
 int finalize_on_stream(lvsr_model* m, cudaStream_t st, bool synchronise);
+// adaptive weight noise (noise.cu): the sample pass of a training forward (noisy parameters + priors + model cost)
+// and the gradient transform of an update (both gradient groups; *nparts partial sums of squares of their union in
+// noise.norm_part when nparts is not null).  noise_free releases the handle's noise buffers.
+int noise_sample(lvsr_model* m, cudaStream_t st);
+int noise_gradients(lvsr_model* m, float* grads, float gscale, float* gls2, cudaStream_t st, int* nparts);
+void noise_free(lvsr_model* m);
 // Every encoder layer (fork projection + BiGRU scan) and the mask of the encoded frames: attended [Tp, B, E] (the last
 // layer writes it), attended_mask [Tp, B].  Buffers come from `ws`.  Without a tape (inference) the BiGRU runs without
 // the training stores; with one, tape[l] records layer l's buffers (and allocates hext) for the backward pass.

@@ -1,0 +1,318 @@
+// Adaptive weight noise (Graves 2011, "Practical Variational Inference for Neural Networks"): apply_adaptive_noise of
+// lvsr/graph.py:71-251 as lvsr/main.py:425-460 applies it to every parameter of the recognizer.
+//
+// Per parameter p (every entry of the flat layout, padding excluded) a log-variance ls2 of the same shape
+// (graph.py:173-179), S = 2048 (log_sigma_scale, :159):
+//   s2 = exp(S ls2),  p_noisy = p + eps sqrt(s2), eps ~ N(0, 1) fresh every update                      :178-183
+//   prior_u = sum(p) / n,  prior_s2 = (sum(s2) + sum((p - prior_u)^2)) / n   over ALL parameters      :186-198
+//   LC = coef / N sum[0.5 (log prior_s2 - S ls2) + ((p - prior_u)^2 + s2 - prior_s2) / (2 prior_s2)]   :206-214
+//   grad p   = coef (p - prior_u) / (N prior_s2) + g                                                   :240-241
+//   grad ls2 = coef 0.5 S / N (s2 / prior_s2 - 1) + 0.5 S s2 g^2                                       :243-247
+// with g the task gradient at p_noisy, the priors constants of the gradients, and g^2 the reference's "diagonal
+// Hessian" (not the reparameterisation gradient eps g).  The reference draws eps from Theano's MRG31k3p streams;
+// here it is Philox-4x32-10 keyed by (seed, update counter, flat index), Box-Muller in fp32, so that every
+// data-parallel rank draws the same noise without communication.
+//
+// The sample pass (one read of p and ls2, one write of p_noisy) also accumulates float64 partial sums of p, p^2, s2
+// and ls2 per CTA; one CTA then reduces them in a fixed order, so priors and model cost are deterministic.
+#include <curand_kernel.h>
+
+#include <cmath>
+#include <vector>
+
+#include "model.h"
+
+using namespace lvsr;
+
+namespace {
+
+constexpr double kLogSigmaScale = 2048.0;      // graph.py:159
+constexpr int kThreads = 256;
+constexpr int kCtasPerParam = 32;              // grid (kCtasPerParam, parameters); the partial sums follow this grid
+
+struct Span { long long offset, count; };
+
+__device__ __forceinline__ float2 box_muller(unsigned x, unsigned y) {
+  const float u = ((float)(x >> 8) + 0.5f) * (1.f / 16777216.f);    // (0, 1): log(u) is finite
+  const float v = (float)(y >> 8) * (1.f / 16777216.f);
+  const float r = sqrtf(-2.f * logf(u));
+  float s, c;
+  sincospif(2.f * v, &s, &c);
+  return make_float2(r * c, r * s);
+}
+
+// eps of the four flat elements 4q .. 4q+3 (a parameter starts at a multiple of 64, so a group never straddles two)
+__device__ __forceinline__ void eps4(unsigned long long seed, unsigned long long update, unsigned long long q, float e[4]) {
+  const uint4 ctr = make_uint4((unsigned)q, (unsigned)(q >> 32), (unsigned)update, (unsigned)(update >> 32));
+  const uint4 r = curand_Philox4x32_10(ctr, make_uint2((unsigned)seed, (unsigned)(seed >> 32)));
+  const float2 a = box_muller(r.x, r.y), b = box_muller(r.z, r.w);
+  e[0] = a.x; e[1] = a.y; e[2] = b.x; e[3] = b.y;
+}
+
+__device__ __forceinline__ double block_sum(double v, double* red) {
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  double s = 0.0;
+  for (int w = 0; w < kThreads / 32; ++w) s += red[w];
+  return s;
+}
+
+// p_noisy = p + eps exp(1024 ls2) (= eps sqrt(s2)); per CTA the sums of p, p^2, s2, ls2 -> part[4 * cta + k]
+__global__ void __launch_bounds__(kThreads) noise_sample_kernel(const float* __restrict__ mean, const float* __restrict__ ls2,
+                                                                float* __restrict__ noisy, const Span* spans,
+                                                                unsigned long long seed, unsigned long long update,
+                                                                double* part) {
+  __shared__ double red[kThreads / 32];
+  const Span sp = spans[blockIdx.y];
+  double sp1 = 0.0, sp2 = 0.0, ss2 = 0.0, sl = 0.0;
+  const long long groups = (sp.count + 3) >> 2;
+  for (long long gq = blockIdx.x * (long long)kThreads + threadIdx.x; gq < groups; gq += (long long)gridDim.x * kThreads) {
+    const long long i0 = sp.offset + 4 * gq;
+    const float4 p4 = *reinterpret_cast<const float4*>(mean + i0);
+    const float4 l4 = *reinterpret_cast<const float4*>(ls2 + i0);
+    const float p[4] = {p4.x, p4.y, p4.z, p4.w}, l[4] = {l4.x, l4.y, l4.z, l4.w};
+    float e[4], o[4];
+    eps4(seed, update, (unsigned long long)i0 >> 2, e);
+    const long long valid = sp.count - 4 * gq;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      o[j] = 0.f;                                   // the padding after a parameter stays zero
+      if (j < valid) {
+        const float sigma = expf(1024.f * l[j]);
+        o[j] = fmaf(sigma, e[j], p[j]);
+        sp1 += p[j];
+        sp2 += (double)p[j] * p[j];
+        ss2 += (double)sigma * sigma;
+        sl += l[j];
+      }
+    }
+    *reinterpret_cast<float4*>(noisy + i0) = make_float4(o[0], o[1], o[2], o[3]);
+  }
+  const double t0 = block_sum(sp1, red), t1 = block_sum(sp2, red), t2 = block_sum(ss2, red), t3 = block_sum(sl, red);
+  if (threadIdx.x == 0) {
+    double* out = part + 4 * ((size_t)blockIdx.y * gridDim.x + blockIdx.x);
+    out[0] = t0; out[1] = t1; out[2] = t2; out[3] = t3;
+  }
+}
+
+// fixed-order reduction of the partial sums -> stats [model cost, prior mean, prior variance, n]
+__global__ void __launch_bounds__(kThreads) noise_prior_kernel(const double* part, int nparts, double n, double coef_over_n,
+                                                               double* stats) {
+  __shared__ double red[kThreads / 32];
+  double s[4] = {0.0, 0.0, 0.0, 0.0};
+  for (int i = threadIdx.x; i < nparts; i += kThreads)
+    for (int k = 0; k < 4; ++k) s[k] += part[4 * (size_t)i + k];
+  double t[4];
+  for (int k = 0; k < 4; ++k) t[k] = block_sum(s[k], red);
+  if (threadIdx.x == 0) {
+    const double u = t[0] / n;
+    const double dev2 = t[1] - 2.0 * u * t[0] + n * u * u;      // sum (p - prior_u)^2
+    const double ps2 = (t[2] + dev2) / n;
+    stats[LVSR_NOISE_MODEL_COST] = coef_over_n * (0.5 * (n * log(ps2) - kLogSigmaScale * t[3]) + (dev2 + t[2] - n * ps2) / (2.0 * ps2));
+    stats[LVSR_NOISE_PRIOR_MEAN] = u;
+    stats[LVSR_NOISE_PRIOR_VARIANCE] = ps2;
+    stats[3] = n;
+  }
+}
+
+// both gradient groups from g = gscale * grads (the mean gradient at the noisy parameters); per CTA the sum of squares
+// of the two into norm_part (null: not needed)
+__global__ void __launch_bounds__(kThreads) noise_grad_kernel(float* __restrict__ grads, float* __restrict__ gls2,
+                                                              const float* __restrict__ mean, const float* __restrict__ ls2,
+                                                              const Span* spans, const double* stats, float gscale,
+                                                              float coef_over_n, float* norm_part) {
+  __shared__ double red[kThreads / 32];
+  const Span sp = spans[blockIdx.y];
+  const float u = (float)stats[LVSR_NOISE_PRIOR_MEAN];
+  const float ps2 = (float)stats[LVSR_NOISE_PRIOR_VARIANCE];
+  const float a = coef_over_n / ps2;
+  const float half_s = 0.5f * (float)kLogSigmaScale;
+  float sq = 0.f;
+  for (long long i = blockIdx.x * (long long)kThreads + threadIdx.x; i < sp.count; i += (long long)gridDim.x * kThreads) {
+    const long long o = sp.offset + i;
+    const float g = grads[o] * gscale;
+    const float s2 = expf((float)kLogSigmaScale * ls2[o]);
+    const float gp = fmaf(a, mean[o] - u, g);
+    const float gl = coef_over_n * half_s * (s2 / ps2 - 1.f) + half_s * s2 * g * g;
+    grads[o] = gp;
+    gls2[o] = gl;
+    sq = fmaf(gp, gp, fmaf(gl, gl, sq));
+  }
+  if (!norm_part) return;
+  const double t = block_sum(sq, red);
+  if (threadIdx.x == 0) norm_part[(size_t)blockIdx.y * gridDim.x + blockIdx.x] = (float)t;
+}
+
+__global__ void __launch_bounds__(kThreads) noise_eps_kernel(float* __restrict__ eps, const Span* spans, unsigned long long seed,
+                                                             unsigned long long update) {
+  const Span sp = spans[blockIdx.y];
+  const long long groups = (sp.count + 3) >> 2;
+  for (long long gq = blockIdx.x * (long long)kThreads + threadIdx.x; gq < groups; gq += (long long)gridDim.x * kThreads) {
+    const long long i0 = sp.offset + 4 * gq;
+    float e[4];
+    eps4(seed, update, (unsigned long long)i0 >> 2, e);
+    for (int j = 0; j < 4 && 4 * gq + j < sp.count; ++j) eps[i0 + j] = e[j];
+  }
+}
+
+__global__ void noise_fill_kernel(float* x, const Span* spans, float v) {
+  const Span sp = spans[blockIdx.y];
+  for (long long i = blockIdx.x * (long long)kThreads + threadIdx.x; i < sp.count; i += (long long)gridDim.x * kThreads)
+    x[sp.offset + i] = v;
+}
+
+inline dim3 param_grid(const lvsr_model* m) { return dim3(kCtasPerParam, (unsigned)m->params.size()); }
+inline const Span* spans_of(const lvsr_model* m) { return static_cast<const Span*>(m->noise.spans); }
+
+int check_index(const lvsr_model* m, int index, int64_t count) {
+  LVSR_CHECK(m && m->noise.on, "adaptive noise is off (lvsr_train_set_adaptive_noise)");
+  LVSR_CHECK(index >= 0 && index < (int)m->params.size(), "bad parameter index %d", index);
+  LVSR_CHECK(count == m->params[index].count, "parameter '%s' holds %lld values, got %lld", m->params[index].name.c_str(),
+             (long long)m->params[index].count, (long long)count);
+  return 0;
+}
+
+}  // namespace
+
+namespace lvsr {
+
+void noise_free(lvsr_model* m) {
+  if (m->noise.mem) cudaFree(m->noise.mem);
+  if (m->noise.aux) cudaFree(m->noise.aux);
+  m->noise = lvsr_model::Noise();
+}
+
+int noise_sample(lvsr_model* m, cudaStream_t st) {
+  ProfScope prof("noise", st);
+  lvsr_model::Noise& z = m->noise;
+  noise_sample_kernel<<<param_grid(m), kThreads, 0, st>>>(m->flat, z.ls2, z.noisy, spans_of(m), z.cfg.seed,
+                                                          (unsigned long long)z.update, z.part);
+  LVSR_LAUNCH_CHECK();
+  double n = 0.0;
+  for (const Param& p : m->params) n += (double)p.count;
+  const int nparts = kCtasPerParam * (int)m->params.size();
+  noise_prior_kernel<<<1, kThreads, 0, st>>>(z.part, nparts, n, z.cfg.model_cost_coefficient / (double)z.cfg.num_examples, z.stats);
+  LVSR_LAUNCH_CHECK();
+  z.sampled = true;
+  return 0;
+}
+
+int noise_gradients(lvsr_model* m, float* grads, float gscale, float* gls2, cudaStream_t st, int* nparts) {
+  lvsr_model::Noise& z = m->noise;
+  LVSR_CHECK(z.sampled, "adaptive noise: no training forward since the last update (its priors form the gradients)");
+  ProfScope prof("noise", st);
+  noise_grad_kernel<<<param_grid(m), kThreads, 0, st>>>(grads, gls2, m->flat, z.ls2, spans_of(m), z.stats, gscale,
+                                                        (float)(z.cfg.model_cost_coefficient / (double)z.cfg.num_examples),
+                                                        nparts ? z.norm_part : nullptr);
+  LVSR_LAUNCH_CHECK();
+  if (nparts) *nparts = kCtasPerParam * (int)m->params.size();
+  return 0;
+}
+
+}  // namespace lvsr
+
+extern "C" {
+
+int lvsr_train_set_adaptive_noise(lvsr_model* m, const lvsr_adaptive_noise* cfg) {
+  LVSR_CHECK(m, "null model");
+  DeviceGuard device_guard(m);
+  if (!cfg) {
+    LVSR_CUDA_OK(cudaDeviceSynchronize());        // a training call may still read the buffers
+    noise_free(m);
+    return 0;
+  }
+  LVSR_CHECK(cfg->init_sigma > 0.0 && std::isfinite(cfg->init_sigma), "adaptive noise: init_sigma must be > 0");
+  LVSR_CHECK(cfg->model_cost_coefficient >= 0.0 && std::isfinite(cfg->model_cost_coefficient),
+             "adaptive noise: model_cost_coefficient must be >= 0");
+  LVSR_CHECK(cfg->num_examples > 0, "adaptive noise: num_examples must be > 0");
+  lvsr_model::Noise& z = m->noise;
+  const size_t n = (size_t)m->flat_count, np = m->params.size();
+  const size_t nparts = (size_t)kCtasPerParam * np;
+  if (!z.mem) {
+    LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&z.mem), 6 * n * sizeof(float)));
+    const size_t span_bytes = (np * sizeof(Span) + 255) & ~(size_t)255;
+    LVSR_CUDA_OK(cudaMalloc(&z.aux, span_bytes + (4 + 4 * nparts) * sizeof(double) + nparts * sizeof(float)));
+    z.ls2 = z.mem; z.noisy = z.mem + n; z.gls2 = z.mem + 2 * n;
+    z.velocity = z.mem + 3 * n; z.ms_step = z.mem + 4 * n; z.ms_dx = z.mem + 5 * n;
+    z.spans = z.aux;
+    z.stats = reinterpret_cast<double*>(static_cast<char*>(z.aux) + span_bytes);
+    z.part = z.stats + 4;
+    z.norm_part = reinterpret_cast<float*>(z.part + 4 * nparts);
+    std::vector<Span> h(np);
+    for (size_t i = 0; i < np; ++i) h[i] = Span{m->params[i].offset, m->params[i].count};
+    LVSR_CUDA_OK(cudaMemcpy(z.spans, h.data(), np * sizeof(Span), cudaMemcpyHostToDevice));
+  } else {
+    LVSR_CUDA_OK(cudaDeviceSynchronize());
+  }
+  LVSR_CUDA_OK(cudaMemset(z.mem, 0, 6 * n * sizeof(float)));
+  LVSR_CUDA_OK(cudaMemset(z.stats, 0, 4 * sizeof(double)));
+  // graph.py:173-175: ls2 = log(init_sigma) * 2 / log_sigma_scale, in float32
+  noise_fill_kernel<<<param_grid(m), kThreads>>>(z.ls2, spans_of(m), (float)(log(cfg->init_sigma) * 2.0 / kLogSigmaScale));
+  LVSR_LAUNCH_CHECK();
+  LVSR_CUDA_OK(cudaDeviceSynchronize());
+  z.cfg = *cfg;
+  z.on = true;
+  z.update = 0;
+  z.sampled = false;
+  return 0;
+}
+
+int lvsr_train_get_noise_param(const lvsr_model* m, int index, float* host, int64_t count) {
+  if (int rc = check_index(m, index, count)) return rc;
+  LVSR_CHECK(host, "null argument");
+  DeviceGuard device_guard(m);
+  LVSR_CUDA_OK(cudaMemcpy(host, m->noise.ls2 + m->params[index].offset, (size_t)count * sizeof(float), cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+int lvsr_train_set_noise_param(lvsr_model* m, int index, const float* host, int64_t count) {
+  if (int rc = check_index(m, index, count)) return rc;
+  LVSR_CHECK(host, "null argument");
+  DeviceGuard device_guard(m);
+  LVSR_CUDA_OK(cudaMemcpy(m->noise.ls2 + m->params[index].offset, host, (size_t)count * sizeof(float), cudaMemcpyHostToDevice));
+  m->noise.sampled = false;
+  return 0;
+}
+
+int lvsr_train_noise_stats(lvsr_model* m, double out[3]) {
+  LVSR_CHECK(m && out, "null argument");
+  LVSR_CHECK(m->noise.on, "adaptive noise is off (lvsr_train_set_adaptive_noise)");
+  DeviceGuard device_guard(m);
+  LVSR_CUDA_OK(cudaDeviceSynchronize());
+  LVSR_CUDA_OK(cudaMemcpy(out, m->noise.stats, 3 * sizeof(double), cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+int lvsr_train_noise_sample(lvsr_model* m, int64_t update, float* eps_dev, void* stream) {
+  LVSR_CHECK(m && eps_dev && update >= 0, "train_noise_sample: bad arguments");
+  LVSR_CHECK(m->noise.on, "adaptive noise is off (lvsr_train_set_adaptive_noise)");
+  DeviceGuard device_guard(m);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  ProfScope prof("noise", st);
+  LVSR_CUDA_OK(cudaMemsetAsync(eps_dev, 0, (size_t)m->flat_count * sizeof(float), st));
+  noise_eps_kernel<<<param_grid(m), kThreads, 0, st>>>(eps_dev, spans_of(m), m->noise.cfg.seed, (unsigned long long)update);
+  LVSR_LAUNCH_CHECK();
+  return 0;
+}
+
+int lvsr_train_noise_params(lvsr_model* m, float* out_dev, void* stream) {
+  LVSR_CHECK(m && out_dev, "train_noise_params: null argument");
+  LVSR_CHECK(m->noise.on, "adaptive noise is off (lvsr_train_set_adaptive_noise)");
+  DeviceGuard device_guard(m);
+  LVSR_CUDA_OK(cudaMemcpyAsync(out_dev, m->noise.noisy, (size_t)m->flat_count * sizeof(float), cudaMemcpyDeviceToDevice,
+                               static_cast<cudaStream_t>(stream)));
+  return 0;
+}
+
+int lvsr_train_noise_gradients(lvsr_model* m, float* grads_dev, float gscale, float* ls2_grads_dev, void* stream) {
+  LVSR_CHECK(m && grads_dev && ls2_grads_dev, "train_noise_gradients: null argument");
+  LVSR_CHECK(m->noise.on, "adaptive noise is off (lvsr_train_set_adaptive_noise)");
+  DeviceGuard device_guard(m);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  LVSR_CUDA_OK(cudaMemsetAsync(ls2_grads_dev, 0, (size_t)m->flat_count * sizeof(float), st));
+  return noise_gradients(m, grads_dev, gscale, ls2_grads_dev, st, nullptr);
+}
+
+}  // extern "C"

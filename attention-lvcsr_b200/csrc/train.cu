@@ -144,13 +144,9 @@ float* grad_of(lvsr_model* m, float* grads, const std::string& name) {
   return it == m->index.end() ? nullptr : grads + m->params[it->second].offset;
 }
 
-}  // namespace
-
-extern "C" {
-
-int lvsr_train_cost_and_grads(lvsr_model* m, const float* x, const float* mask, const int64_t* labels, const float* lmask,
-                              int32_t T, int32_t B, int32_t L, float gscale, float* cost_out, float* grads, void* stream) {
-  DeviceGuard device_guard(m);
+// forward + backward of one batch on the parameters Param::dev points at and the weights packed from them
+int forward_backward(lvsr_model* m, const float* x, const float* mask, const int64_t* labels, const float* lmask,
+                     int32_t T, int32_t B, int32_t L, float gscale, float* cost_out, float* grads, void* stream) {
   if (int rc = check_ready(m)) return rc;
   LVSR_CHECK(x && labels && cost_out && grads && T > 0 && B > 0 && L > 0, "train_cost_and_grads: bad arguments");
   LVSR_CHECK(!lm_attached(m), "train_cost_and_grads: shallow fusion is inference only (detach the language model)");
@@ -537,6 +533,31 @@ int lvsr_train_cost_and_grads(lvsr_model* m, const float* x, const float* mask, 
   return 0;
 }
 
+}  // namespace
+
+extern "C" {
+
+int lvsr_train_cost_and_grads(lvsr_model* m, const float* x, const float* mask, const int64_t* labels, const float* lmask,
+                              int32_t T, int32_t B, int32_t L, float gscale, float* cost_out, float* grads, void* stream) {
+  DeviceGuard device_guard(m);
+  if (!m || !m->noise.on) return forward_backward(m, x, mask, labels, lmask, T, B, L, gscale, cost_out, grads, stream);
+  // adaptive weight noise (noise.cu): the step runs on p + eps sqrt(s2).  Every parameter pointer is re-pointed at
+  // the noisy copy and the kernel-side weights are re-packed from it; on every way out the pointers go back to the
+  // means and the handle is marked un-finalized, so any other entry point re-packs from the means first.
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (int rc = noise_sample(m, st)) return rc;
+  struct Restore {
+    lvsr_model* m;
+    ~Restore() {
+      for (Param& p : m->params) p.dev = m->flat + p.offset;
+      m->finalized = false;
+      m->noise.stale = true;         // the step may still read the noisy packing on its own stream (check_ready)
+    }
+  } restore{m};
+  for (Param& p : m->params) p.dev = m->noise.noisy + p.offset;
+  if (int rc = finalize_on_stream(m, st, false)) return rc;
+  return forward_backward(m, x, mask, labels, lmask, T, B, L, gscale, cost_out, grads, stream);
+}
 
 // Parameters with the WEIGHT role, the subjects of weight decay and max-norm (lvsr/main.py:418-420,493): Linear and
 // LookupTable W and the recurrent matrices.  The conv filters carry no role of their own (lvsr/bricks/attention.py:31-33).
@@ -552,6 +573,9 @@ int lvsr_train_apply_updates(lvsr_model* m, float* grads, float gscale, const lv
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long long n = m->flat_count;
   const int np = (int)m->params.size();
+  lvsr_model::Noise& z = m->noise;
+  // adaptive noise takes the gradients of the cost without the decay term (lvsr/main.py:425-437)
+  LVSR_CHECK(!(z.on && tc->decay > 0.f), "train_apply_updates: weight decay has no effect under adaptive noise: pass decay = 0");
   if (!m->opt_desc) {
     std::vector<ParamDesc> h(np);
     for (int i = 0; i < np; ++i) {
@@ -580,11 +604,20 @@ int lvsr_train_apply_updates(lvsr_model* m, float* grads, float gscale, const lv
   }
   float* part = m->opt_scratch;
   float* norm = m->opt_scratch + 1024;
-  const int nparts = (int)std::min<long long>(1024, std::max<long long>(1, n / 4096));
-  sqnorm_partial_kernel<<<nparts, 256, 0, st>>>(grads, n, part);
-  LVSR_LAUNCH_CHECK();
-  sqnorm_final_kernel<<<1, 32, 0, st>>>(part, nparts, gscale, norm);
-  LVSR_LAUNCH_CHECK();
+  if (z.on) {
+    // both gradient groups of adaptive noise (noise.cu), already multiplied by gscale; one clipping norm over both
+    int nparts = 0;
+    if (int rc = noise_gradients(m, grads, gscale, z.gls2, st, &nparts)) return rc;
+    sqnorm_final_kernel<<<1, 32, 0, st>>>(z.norm_part, nparts, 1.f, norm);
+    LVSR_LAUNCH_CHECK();
+    gscale = 1.f;
+  } else {
+    const int nparts = (int)std::min<long long>(1024, std::max<long long>(1, n / 4096));
+    sqnorm_partial_kernel<<<nparts, 256, 0, st>>>(grads, n, part);
+    LVSR_LAUNCH_CHECK();
+    sqnorm_final_kernel<<<1, 32, 0, st>>>(part, nparts, gscale, norm);
+    LVSR_LAUNCH_CHECK();
+  }
   StepArgs a = {};
   a.grads = grads; a.params = m->flat; a.velocity = m->opt_velocity; a.ms_step = m->opt_ms_step; a.ms_dx = m->opt_ms_dx;
   a.norm = norm; a.n = n; a.gscale = gscale; a.decay = tc->decay; a.threshold = tc->gradient_threshold;
@@ -592,6 +625,12 @@ int lvsr_train_apply_updates(lvsr_model* m, float* grads, float gscale, const lv
   a.use_adadelta = tc->use_adadelta; a.decay_rate = tc->decay_rate; a.epsilon = tc->epsilon;
   step_rules_kernel<<<grid1d(n, 256, 1184), 256, 0, st>>>(a);
   LVSR_LAUNCH_CHECK();
+  if (z.on) {          // the same rules over the ls2 block, with its own optimizer state
+    StepArgs b = a;
+    b.grads = z.gls2; b.params = z.ls2; b.velocity = z.velocity; b.ms_step = z.ms_step; b.ms_dx = z.ms_dx;
+    step_rules_kernel<<<grid1d(n, 256, 1184), 256, 0, st>>>(b);
+    LVSR_LAUNCH_CHECK();
+  }
   if (tc->max_norm > 0.f) {
     dim3 grid(32, np);
     max_norm_kernel<<<grid, 256, 0, st>>>(grads, m->flat, desc, tc->max_norm);
@@ -602,6 +641,17 @@ int lvsr_train_apply_updates(lvsr_model* m, float* grads, float gscale, const lv
     if (m->burn_in_left < 0) m->burn_in_left = tc->burn_in_steps;
     burn_mult = m->burn_in_left <= 0 ? 1.f : 0.f;
     m->burn_in_left = std::max<long long>(0, m->burn_in_left - 1);
+  }
+  if (z.on) {          // RemoveNotFinite per tensor: every ls2 is a tensor of its own; no max-norm (PARAMETER role only)
+    apply_update_pair_kernel<<<2 * np, 256, 0, st>>>(m->flat, grads, z.ls2, z.gls2, desc, np, burn_mult);
+    LVSR_LAUNCH_CHECK();
+    z.update++;
+    z.sampled = false;
+    // the next training forward packs the weights from its noisy copy; packing the means here as well would cost a
+    // second re-pack per step, so they are packed when another entry point needs them (check_ready)
+    z.stale = true;
+    m->finalized = false;
+    return 0;
   }
   apply_update_kernel<<<np, 256, 0, st>>>(m->flat, grads, desc, burn_mult);
   LVSR_LAUNCH_CHECK();
@@ -622,6 +672,7 @@ int lvsr_train_reset(lvsr_model* m) {
   if (m->opt_velocity) LVSR_CUDA_OK(cudaMemset(m->opt_velocity, 0, bytes));
   if (m->opt_ms_step) LVSR_CUDA_OK(cudaMemset(m->opt_ms_step, 0, bytes));
   if (m->opt_ms_dx) LVSR_CUDA_OK(cudaMemset(m->opt_ms_dx, 0, bytes));
+  if (m->noise.on) LVSR_CUDA_OK(cudaMemset(m->noise.velocity, 0, 3 * bytes));     // velocity | ms_step | ms_dx of ls2
   m->burn_in_left = -1;
   return 0;
 }

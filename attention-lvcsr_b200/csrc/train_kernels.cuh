@@ -908,9 +908,8 @@ __global__ void __launch_bounds__(256) max_norm_kernel(float* step, const float*
     }
   }
 }
-// RemoveNotFinite(0.0) + BurnIn + the update: one CTA per parameter.
-__global__ void __launch_bounds__(256) apply_update_kernel(float* params, const float* step, const ParamDesc* desc, float burn_mult) {
-  const ParamDesc d = desc[blockIdx.x];
+// RemoveNotFinite(0.0) + BurnIn + the update of one parameter by one CTA.
+__device__ __forceinline__ void apply_update_param(float* params, const float* step, const ParamDesc d, float burn_mult) {
   const long long cnt = (long long)d.rows * d.cols;
   __shared__ float red[8];
   __shared__ int bad;
@@ -931,6 +930,17 @@ __global__ void __launch_bounds__(256) apply_update_kernel(float* params, const 
     const float st = bad ? params[o] : step[o];
     params[o] = params[o] - st * burn_mult;
   }
+}
+__global__ void __launch_bounds__(256) apply_update_kernel(float* params, const float* step, const ParamDesc* desc, float burn_mult) {
+  apply_update_param(params, step, desc[blockIdx.x], burn_mult);
+}
+// Adaptive noise: the updates of the means (CTAs [0, nparams)) and of their log-variances (CTAs [nparams, 2 nparams))
+// in one grid, so that the CTA of a large log-variance runs beside, not after, the CTA of its large mean.
+__global__ void __launch_bounds__(256) apply_update_pair_kernel(float* params, const float* step, float* params2,
+                                                                const float* step2, const ParamDesc* desc, int nparams,
+                                                                float burn_mult) {
+  const bool second = (int)blockIdx.x >= nparams;
+  apply_update_param(second ? params2 : params, second ? step2 : step, desc[blockIdx.x - (second ? nparams : 0)], burn_mult);
 }
 
 }  // namespace train

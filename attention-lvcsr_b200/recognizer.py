@@ -341,13 +341,7 @@ class SpeechRecognizer(object):
         libs/blocks/blocks/serialization.py:264-282,606-610) or a plain .npz.  Like
         Model.set_parameter_values (libs/blocks/blocks/model.py:120-146) unknown names and missing parameters
         are LOGGED, not raised; missing parameters keep their current values."""
-        data = None
-        if tarfile.is_tarfile(path):
-            with tarfile.open(path) as tar:
-                data = np.load(io.BytesIO(tar.extractfile("_parameters").read()))
-        else:
-            data = np.load(path)
-        values = {k.replace("|", "/"): data[k] for k in data.files}
+        values = self.load_checkpoint_values(path)
         shapes = self.parameter_shapes()
         unknown = sorted(set(values) - set(shapes))
         missing = sorted(set(shapes) - set(values))
@@ -358,13 +352,26 @@ class SpeechRecognizer(object):
         self.set_parameter_values({k: v for k, v in values.items() if k in shapes})
         return dict(unknown=unknown, missing=missing)
 
-    def save_params(self, path):
+    @staticmethod
+    def load_checkpoint_values(path):
+        """{Blocks parameter name: array} of a checkpoint load_params reads, every name it holds."""
+        if tarfile.is_tarfile(path):
+            with tarfile.open(path) as tar:
+                data = np.load(io.BytesIO(tar.extractfile("_parameters").read()))
+        else:
+            data = np.load(path)
+        return {k.replace("|", "/"): data[k] for k in data.files}
+
+    def save_params(self, path, extra=None):
         """Write the parameters the way blocks.serialization.dump stores them separately: a tar archive with one
         member ``_parameters`` = numpy.savez of {brick path with '|' for '/': array}
         (libs/blocks/blocks/serialization.py:136,264-282,493-500,606-610) -- readable by the reference's
-        load_parameters and by load_params above."""
+        load_parameters and by load_params above.  ``extra``: more {Blocks name: array} of the same model, such as
+        the adaptive-noise parameters of GradientDescent.noise_parameter_values()."""
+        values = OrderedDict(self.get_parameter_values())
+        values.update(extra or {})
         buf = io.BytesIO()
-        np.savez(buf, **{k.replace("/", "|"): v for k, v in self.get_parameter_values().items()})
+        np.savez(buf, **{k.replace("/", "|"): v for k, v in values.items()})
         payload = buf.getvalue()
         with tarfile.open(path, "w") as tar:
             info = tarfile.TarInfo("_parameters")

@@ -61,10 +61,22 @@ def train(config, save_path, bokeh_name="", params=None, bokeh_server=None, boke
     data = Data(**config["data"])
     recognizer = create_model(config, data, params)
     train_conf = config["training"]
+    reg_conf = config.get("regularization", {})
+    adaptive_noise = None
+    if reg_conf.get("adaptive_noise"):
+        # lvsr/main.py:425-437: every parameter gets trained Gaussian noise; N is the size of the training set
+        logger.info("apply adaptive noise")
+        adaptive_noise = dict(reg_conf["adaptive_noise"], num_examples=data.get_dataset("train").num_examples)
     algorithm = pkg.GradientDescent(recognizer=recognizer,
-                                    step_rule=pkg.step_rule_from_config(train_conf, config.get("regularization", {})),
-                                    decay=config.get("regularization", {}).get("decay", 0.0))
+                                    step_rule=pkg.step_rule_from_config(train_conf, reg_conf),
+                                    decay=reg_conf.get("decay", 0.0), adaptive_noise=adaptive_noise)
     algorithm.initialize()
+    if adaptive_noise and params:
+        _load_noise_parameters(algorithm, params)
+
+    def save(path):
+        recognizer.save_params(path, extra=algorithm.noise_parameter_values() if adaptive_noise else None)
+
     num_batches = train_conf.get("num_batches")
     done = 0
     for epoch in range(int(train_conf.get("num_epochs", 1))):
@@ -76,16 +88,35 @@ def train(config, save_path, bokeh_name="", params=None, bokeh_server=None, boke
             # the quantities lvsr/main.py:340-345,357-372 monitors every batch
             logger.info("batch %d: sequence_total_cost %.6f total_gradient_norm %.6f time_train_this_batch %.4f",
                         done, cost, algorithm.total_gradient_norm(), time.time() - t0)
+            if adaptive_noise:
+                # lvsr/main.py:456-460
+                stats = algorithm.noise_stats()
+                logger.info("batch %d: task_cost %.6f model_cost %.6f model_prior_mean %.6g model_prior_variance %.6g",
+                            done, cost, stats["model_cost"], stats["model_prior_mean"], stats["model_prior_variance"])
             every = train_conf.get("save_every_n_batches")
             if every and done % every == 0 and save_path:
-                recognizer.save_params(save_path)
+                save(save_path)
             if num_batches and done >= num_batches:
                 break
         if num_batches and done >= num_batches:
             break
     if save_path:
-        recognizer.save_params(save_path)
+        save(save_path)
     return recognizer
+
+
+def _load_noise_parameters(algorithm, path):
+    """The adaptive-noise parameters of a checkpoint, as Model.set_parameter_values loads them
+    (lvsr/main.py:462-470, B/model.py:120-146): the ones present are set, missing ones are logged and keep
+    init_sigma (a checkpoint of a stage without adaptive noise has none)."""
+    values = algorithm.recognizer.load_checkpoint_values(path)
+    want = algorithm.noise_parameter_values()
+    found = {k: v for k, v in values.items() if k in want}
+    missing = sorted(set(want) - set(found))
+    if missing:
+        logger.error("missing values for parameters: {}\n".format(missing))
+    algorithm.set_noise_parameter_values(found)
+    return missing
 
 
 def train_multistage(config, save_path, bokeh_name, params, start_stage, **kwargs):

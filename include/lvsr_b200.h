@@ -310,13 +310,50 @@ int lvsr_train_apply_updates(lvsr_model* m, float* grads_dev, float gscale, cons
 int lvsr_train_gradient_norm(lvsr_model* m, float* norm_host);   /* total_gradient_norm of the last update (synchronises) */
 int lvsr_train_reset(lvsr_model* m);
 
+/* ---- adaptive weight noise (Graves 2011): apply_adaptive_noise, lvsr/graph.py:71-251, as lvsr/main.py:425-460
+ * applies it to every parameter).  Each parameter p gets a log-variance ls2 of its shape, s2 = exp(2048 ls2).
+ * While it is on:
+ *   lvsr_train_cost_and_grads draws eps ~ N(0, 1) per element (Philox-4x32-10 keyed by (seed, update counter, flat
+ *     index), Box-Muller in fp32: the same draw on every data-parallel rank), runs forward and backward on
+ *     p + eps sqrt(s2), and computes from the means prior_u = mean(p), prior_s2 = mean(s2 + (p - prior_u)^2) and the
+ *     model cost LC = coef / N * sum[0.5 (log prior_s2 - 2048 ls2) + ((p - prior_u)^2 + s2 - prior_s2) / (2 prior_s2)].
+ *     Every other entry point sees the means and weights packed from them.  The cost it reports is the task cost.
+ *   lvsr_train_apply_updates first forms, from g = gscale * grads_dev (the mean gradient at the noisy parameters),
+ *     grad p = coef (p - prior_u) / (N prior_s2) + g and grad ls2 = coef 1024 / N (s2 / prior_s2 - 1) + 1024 s2 g^2,
+ *     then runs the step rules over both groups: one clipping norm, optimizer state for both, RemoveNotFinite and
+ *     BurnIn per tensor, max-norm on the WEIGHT means only.  It refuses decay > 0 (the reference takes the gradients
+ *     of the cost without the decay term, lvsr/main.py:427-432).  The update counter then advances.  The weights
+ *     are not re-packed from the new means: the next training forward packs its noisy copy, and any other entry
+ *     point synchronises the device and packs the means first.
+ * lvsr_train_set_adaptive_noise turns it on (NULL: off), sets every ls2 to log(init_sigma) / 1024, clears the ls2
+ * optimizer state and the update counter.  lvsr_train_get/set_noise_param copy the ls2 of parameter `index`.
+ * lvsr_train_noise_stats (synchronises): out[LVSR_NOISE_*] of the last training forward.
+ * lvsr_train_noise_sample writes the eps of update `update` in the flat layout (padding zero).
+ * lvsr_train_noise_params copies the noisy parameters the last training forward ran on (flat layout, padding zero).
+ * lvsr_train_noise_gradients forms both gradient groups in place of grads_dev / into ls2_grads_dev (flat layout)
+ *   without an update, with the priors of the last training forward. */
+typedef struct {
+  double init_sigma;               /* initial standard deviation of the noise (reference default 1e-6)          */
+  double model_cost_coefficient;   /* coef (1.0)                                                                 */
+  int64_t num_examples;            /* N: utterances in the training set                                          */
+  uint64_t seed;                   /* key of the draw (the reference's default seed is 1)                         */
+} lvsr_adaptive_noise;
+enum { LVSR_NOISE_MODEL_COST = 0, LVSR_NOISE_PRIOR_MEAN = 1, LVSR_NOISE_PRIOR_VARIANCE = 2 };
+int lvsr_train_set_adaptive_noise(lvsr_model* m, const lvsr_adaptive_noise* cfg);
+int lvsr_train_get_noise_param(const lvsr_model* m, int index, float* values_host, int64_t count);
+int lvsr_train_set_noise_param(lvsr_model* m, int index, const float* values_host, int64_t count);
+int lvsr_train_noise_stats(lvsr_model* m, double out[3]);
+int lvsr_train_noise_sample(lvsr_model* m, int64_t update, float* eps_dev, void* stream);
+int lvsr_train_noise_params(lvsr_model* m, float* noisy_dev, void* stream);
+int lvsr_train_noise_gradients(lvsr_model* m, float* grads_dev, float gscale, float* ls2_grads_dev, void* stream);
+
 /* Counters for bench.py: number of kernels this library launched since the last reset. */
 int64_t lvsr_launch_count(int reset);
 
 /* Per-kernel-class device timing (CUDA events recorded on the launching stream around every
  * launch of that class) -- the analogue of the reference's Theano ProfileStats
  * (libs/Theano/theano/compile/profiling.py:97).  Classes: "gemm", "bigru", "attention",
- * "window", "dense", "readout", "lm".  lvsr_profile_read synchronises the device, returns the
+ * "window", "dense", "readout", "lm", "noise" (adaptive weight noise).  lvsr_profile_read synchronises the device, returns the
  * summed milliseconds and launch count recorded since the last read of that class. */
 int lvsr_profile_enable(int on);
 int lvsr_profile_read(const char* kernel_class, double* total_ms, int64_t* count);
