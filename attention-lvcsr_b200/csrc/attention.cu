@@ -137,11 +137,17 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) att_content_step_kernel(AttSte
 
 int num_sms() { return device_sm_count(); }
 
-int launch_att(const AttStepArgs& a, bool loc, int cs, cudaStream_t stream) {
+constexpr size_t ATT_SMEM_MAX = 227 * 1024;   // dynamic shared memory one CTA may opt in to on sm_90
+
+// Dynamic shared memory (bytes) of one attention-step CTA when clusters of cs CTAs split a row of T' positions.
+size_t att_step_smem(const AttStepArgs& a, bool loc, int cs) {
   const int tc_cap = ceil_div(a.Tp, cs);
-  const size_t smem = (loc ? att_smem_floats(a.M, a.E, a.K, a.n, tc_cap, cs) : att_smem_floats<false>(a.M, a.E, 0, 0, tc_cap, cs)) *
-                      sizeof(float);
-  LVSR_CHECK(smem <= 227 * 1024, "attention_step: shared memory %zu B exceeds 227 KB (Tp=%d, cs=%d)", smem, a.Tp, cs);
+  return (loc ? att_smem_floats(a.M, a.E, a.K, a.n, tc_cap, cs) : att_smem_floats<false>(a.M, a.E, 0, 0, tc_cap, cs)) *
+         sizeof(float);
+}
+
+int launch_att(const AttStepArgs& a, bool loc, int cs, size_t smem, cudaStream_t stream) {
+  const int tc_cap = ceil_div(a.Tp, cs);
   static size_t configured[2][LVSR_MAX_DEVICES] = {{0}};
   const int dev = current_device();
   void (*kernel)(AttStepArgs, int) = loc ? att_step_kernel : att_content_step_kernel;
@@ -186,19 +192,23 @@ int attention_step(const AttStepArgs& a, bool location, int* cs_out, cudaStream_
   int cs = 1;
   const int sms = num_sms();
   while (cs < 8 && a.R * cs * 2 <= sms && ceil_div(a.Tp, cs * 2) >= 16) cs *= 2;
-  // LVSR_ATT_CS=1|2|4|8 (DESIGN §7, read on every call) replaces the one-wave choice above when the forced size keeps
-  // ceil(T'/cs) >= 16 and its shared memory fits; otherwise it is declined.  Clusters of one step never wait for each
-  // other, so the grid need not be co-resident.
+  // a row longer than one CTA's shared memory holds is split further.  Clusters of one step never wait for each other,
+  // so the grid need not be co-resident and a larger cluster than one wave allows always runs.
+  while (cs < 8 && att_step_smem(a, location, cs) > ATT_SMEM_MAX && ceil_div(a.Tp, cs * 2) >= 16) cs *= 2;
+  // LVSR_ATT_CS=1|2|4|8 (DESIGN §7, read on every call) replaces the choice above when the forced size keeps
+  // ceil(T'/cs) >= 16 and its shared memory fits; otherwise it is declined.
   if (const char* s = getenv("LVSR_ATT_CS")) {
     const int f = atoi(s);
     LVSR_CHECK(f == 1 || f == 2 || f == 4 || f == 8, "LVSR_ATT_CS=%s: expected 1, 2, 4 or 8", s);
-    const int cap = ceil_div(a.Tp, f);
-    const size_t smem = (location ? att_smem_floats(a.M, a.E, a.K, a.n, cap, f) : att_smem_floats<false>(a.M, a.E, 0, 0, cap, f)) *
-                        sizeof(float);
-    if ((f == 1 || cap >= 16) && smem <= 227 * 1024) cs = f;
+    if ((f == 1 || ceil_div(a.Tp, f) >= 16) && att_step_smem(a, location, f) <= ATT_SMEM_MAX) cs = f;
   }
+  const size_t smem = att_step_smem(a, location, cs);
+  LVSR_CHECK(smem <= ATT_SMEM_MAX,
+             "attention_step: T'=%d positions do not fit in shared memory at any cluster size: %zu B per CTA in "
+             "clusters of %d (M=%d, E=%d, conv_num_filters=%d, conv_n=%d) exceeds the 227 KB limit",
+             a.Tp, smem, cs, a.M, a.E, location ? a.K : 0, location ? a.n : 0);
   *cs_out = cs;
-  return launch_att(a, location, cs, stream);
+  return launch_att(a, location, cs, smem, stream);
 }
 
 }  // namespace lvsr
