@@ -82,6 +82,11 @@ class Uniform(NdarrayInitialization):
         self.width = np.sqrt(12) * std if std is not None else width
         self.mean = mean
 
+    def __setstate__(self, state):
+        # a YAML mapping (`!!python/object:blocks.initialization.Uniform {width: 0.1}`, exp/wsj/configs/
+        # wsj_jan_bhd04.yaml) builds the object without __init__: the mapping is taken as the constructor's arguments
+        self.__init__(**state)
+
     def generate(self, rng, shape):
         w = self.width / 2
         return rng.uniform(self.mean - w, self.mean + w, size=shape).astype(np.float32)

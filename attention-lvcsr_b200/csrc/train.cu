@@ -151,8 +151,6 @@ int forward_backward(lvsr_model* m, const float* x, const float* mask, const int
   LVSR_CHECK(x && labels && cost_out && grads && T > 0 && B > 0 && L > 0, "train_cost_and_grads: bad arguments");
   LVSR_CHECK(!lm_attached(m), "train_cost_and_grads: shallow fusion is inference only (detach the language model)");
   const lvsr_config& c = m->cfg;
-  LVSR_CHECK(c.energy_normalizer == LVSR_NORM_SOFTMAX,
-             "training supports the softmax energy normaliser only (logistic / relu: inference only)");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int C = c.dim_dec, E = m->E, M = c.dim_matcher, K = c.conv_num_filters, n = c.conv_n, w = 2 * n + 1;
   const int V = c.num_phonemes, Cfb = c.dim_feedback, Cpm = c.post_merge_dim, Hd = Cpm / c.maxout_pieces;
@@ -162,6 +160,8 @@ int forward_backward(lvsr_model* m, const float* x, const float* mask, const int
   const size_t ro_smem = (size_t)8 * (Hd + 128) * sizeof(float);
   LVSR_CHECK(ro_smem <= 48 * 1024 && V <= 128, "readout backward: post_merge_dim / num_phonemes too large");
   const bool content = content_attention(m);
+  // the logistic and relu energy gradients read the step's energies, which the softmax one does not need
+  const bool keep_energies = c.energy_normalizer != LVSR_NORM_SOFTMAX;
   const int tc_cap = ceil_div(Tp, AB_CS);
   const size_t ab_smem = (content ? att_bwd_content_smem_floats(E, tc_cap) : att_bwd_smem_floats(M, E, K, n, tc_cap)) * sizeof(float);
   LVSR_CHECK(ab_smem <= 227 * 1024 && M <= AB_NT && M % 128 == 0 && K <= 16 && E % 4 == 0,
@@ -182,6 +182,7 @@ int forward_backward(lvsr_model* m, const float* x, const float* mask, const int
     }
     bytes += ((size_t)Tp * B * (2 * M + 2 * E) + (size_t)R * (Tp + 8 * C + 3 * E + 2 * M + 3 * Cpm + V + 16) + (size_t)4 * B * Tp +
               (size_t)2 * B * (M + (size_t)K * M + (size_t)K * w) + (size_t)4 * (E + C) * 3 * C + (size_t)80 * E * M) * sizeof(float);
+    if (keep_energies) bytes += ((size_t)R * Tp + (size_t)AB_CS * B) * sizeof(float);
     ws.reserve(bytes, st);
   }
   ArenaScope scope(ws, st);
@@ -199,8 +200,9 @@ int forward_backward(lvsr_model* m, const float* x, const float* mask, const int
   float* W_all = ws.f32((size_t)R * Tp);        // alignments alpha_i
   float* S_prev = ws.f32((size_t)R * C);        // s_{i-1}
   float* CTX = ws.f32((size_t)R * E);           // weighted averages
-  LVSR_CHECK(costs && W_all && S_prev && CTX, "out of device memory (decoder tape)");
-  if (int rc = lvsr_cost_matrix(m, Hatt, attm, Tp, B, labels, lmask, L, costs, W_all, nullptr, S_prev, CTX, stream)) return rc;
+  float* E_all = keep_energies ? ws.f32((size_t)R * Tp) : nullptr;     // energies e_i, bias included
+  LVSR_CHECK(costs && W_all && S_prev && CTX && (E_all || !keep_energies), "out of device memory (decoder tape)");
+  if (int rc = lvsr_cost_matrix(m, Hatt, attm, Tp, B, labels, lmask, L, costs, W_all, E_all, S_prev, CTX, stream)) return rc;
   sum_all_kernel<<<1, 1024, 0, st>>>(costs, R, cost_out, gscale);
   LVSR_LAUNCH_CHECK();
 
@@ -287,10 +289,12 @@ int forward_backward(lvsr_model* m, const float* x, const float* mask, const int
   float* acc_v = ws.f32((size_t)nct * M);
   float* acc_Wh = ws.f32((size_t)nct * K * M);
   float* acc_filt = ws.f32((size_t)nct * K * w);
+  float* acc_b = keep_energies ? ws.f32((size_t)nct) : nullptr;
   int* win = ws.i32(2);
   float* lohi = ws.f32((size_t)2 * B);
   LVSR_CHECK(G && Z && Rg && HR && Cc && Q && P && dP && dG && dCTX && dQp && dsbuf[0] && dsbuf[1] && keep && dHR && dspart &&
-                 dAbuf[0] && dAbuf[1] && w0 && acc_v && (content || (acc_Wh && acc_filt)) && win && lohi,
+                 dAbuf[0] && dAbuf[1] && w0 && acc_v && (content || (acc_Wh && acc_filt)) && (acc_b || !keep_energies) &&
+                 win && lohi,
              "out of device memory (decoder backward)");
   if (int rc = lvsr_preprocess(m, Hatt, Tp, B, P, stream)) return rc;
   if (int rc = gemm_nn(CTX, R, E, E, m->Wd_cat, 3 * C, 3 * C, nullptr, G, 3 * C, false, st)) return rc;
@@ -313,13 +317,21 @@ int forward_backward(lvsr_model* m, const float* x, const float* mask, const int
     LVSR_CUDA_OK(cudaMemsetAsync(acc_Wh, 0, (size_t)nct * K * M * sizeof(float), st));
     LVSR_CUDA_OK(cudaMemsetAsync(acc_filt, 0, (size_t)nct * K * w * sizeof(float), st));
   }
+  if (acc_b) LVSR_CUDA_OK(cudaMemsetAsync(acc_b, 0, (size_t)nct * sizeof(float), st));
   LVSR_CUDA_OK(cudaMemsetAsync(dsbuf[0], 0, (size_t)B * C * sizeof(float), st));
   if (int rc = onehot_rows(w0, B, Tp, st)) return rc;
   {
-    const bool kp12 = att_bwd_kp(K) == 12;
-    LVSR_CUDA_OK(cudaFuncSetAttribute(att_bwd_kernel<12>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ab_smem));
-    LVSR_CUDA_OK(cudaFuncSetAttribute(att_bwd_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ab_smem));
-    LVSR_CUDA_OK(cudaFuncSetAttribute(att_bwd_content_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ab_smem));
+    void (*att_bwd)(AttBwdArgs, int) = att_bwd_content_kernel;
+    if (!content) {
+      const bool kp12 = att_bwd_kp(K) == 12;
+      if (c.energy_normalizer == LVSR_NORM_LOGISTIC)
+        att_bwd = kp12 ? att_bwd_kernel<12, LVSR_NORM_LOGISTIC> : att_bwd_kernel<16, LVSR_NORM_LOGISTIC>;
+      else if (c.energy_normalizer == LVSR_NORM_RELU)
+        att_bwd = kp12 ? att_bwd_kernel<12, LVSR_NORM_RELU> : att_bwd_kernel<16, LVSR_NORM_RELU>;
+      else
+        att_bwd = kp12 ? att_bwd_kernel<12, LVSR_NORM_SOFTMAX> : att_bwd_kernel<16, LVSR_NORM_SOFTMAX>;
+    }
+    LVSR_CUDA_OK(cudaFuncSetAttribute(att_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ab_smem));
     const int ew = ceil_div(B * C, 256);
     for (int i = L - 1; i >= 0; --i) {
       ProfScope prof("dec_bwd_step", st);
@@ -353,11 +365,10 @@ int forward_backward(lvsr_model* m, const float* x, const float* mask, const int
       ab.dP = dP; ab.dq_part = dQp + (size_t)i * 2 * B * M; ab.dA_out = dAbuf[(L - i) & 1];
       ab.acc_v = acc_v; ab.acc_Wh = acc_Wh; ab.acc_filt = acc_filt;
       ab.B = B; ab.Tp = Tp; ab.M = M; ab.E = E; ab.K = K; ab.n = n;
+      ab.e_cur = E_all ? E_all + (size_t)i * B * Tp : nullptr; ab.acc_b = acc_b;
       {
         ProfScope prof_ab("att_bwd", st);
-        if (content) att_bwd_content_kernel<<<nct, AB_NT, ab_smem, st>>>(ab, tc_cap);
-        else if (kp12) att_bwd_kernel<12><<<nct, AB_NT, ab_smem, st>>>(ab, tc_cap);
-        else att_bwd_kernel<16><<<nct, AB_NT, ab_smem, st>>>(ab, tc_cap);
+        att_bwd<<<nct, AB_NT, ab_smem, st>>>(ab, tc_cap);
         LVSR_LAUNCH_CHECK();
       }
       // ds_{i-1} = gates/elementwise part + dq . W_s^T (two partials) + readout of step i (which saw s_{i-1})
@@ -424,6 +435,10 @@ int forward_backward(lvsr_model* m, const float* x, const float* mask, const int
       reduce_partials_kernel<<<grid1d((long long)K * M), 256, 0, st>>>(acc_Wh, nct, (long long)K * M, grad_of(m, grads, at + "/handler.W"));
       LVSR_LAUNCH_CHECK();
       reduce_partials_kernel<<<grid1d((long long)K * w), 256, 0, st>>>(acc_filt, nct, (long long)K * w, grad_of(m, grads, at + "/conv1d.filters"));
+      LVSR_LAUNCH_CHECK();
+    }
+    if (acc_b) {
+      reduce_partials_kernel<<<1, 256, 0, st>>>(acc_b, nct, 1, grad_of(m, grads, at + "/energy_comp/linear.b"));
       LVSR_LAUNCH_CHECK();
     }
   }

@@ -443,7 +443,14 @@ __global__ void __launch_bounds__(256) dh_from_ctx_kernel(const float* W_all, co
 
 // ------------------------------------------------------------------------------------------
 // Attention step backward for one decoder step: 2 CTAs per batch row (halves of the window).
-// Forward math: lvsr/bricks/attention.py:98-114,165-183,191-213 (softmax normaliser only).
+// Forward math: lvsr/bricks/attention.py:98-114,165-183,191-213.
+// With g[t] = dctx . H[t] + carry[t] the gradient reaching alpha_i[t] and S = sum_t alpha_i[t] g[t], the energy
+// gradient of each normaliser (e includes the energy bias; the window mask m is folded into alpha):
+//   softmax   alpha = exp(e) m / N:        de = alpha (g - S)
+//   logistic  alpha = sigma(e) m / N:      de = alpha (1 - sigma(e)) (g - S)
+//   relu      alpha = max(e/1000, 0) m / N: de = m [e > 0] (g - S) / (1000 N) = (g - S) alpha / e where e > 0, else 0
+// N is the same for every position of a row, so the relu rule reads 1 / (1000 N) off the alignment instead of
+// re-forming the window's mask and sum.  The energy bias b enters every energy: db = sum of de.
 // ------------------------------------------------------------------------------------------
 constexpr int AB_NT = 512;
 constexpr int AB_CS = 2;
@@ -466,6 +473,8 @@ struct AttBwdArgs {
   float* acc_Wh;             // [2B][K][M]
   float* acc_filt;           // [2B][K][w]
   int B, Tp, M, E, K, n;
+  const float* e_cur;        // [B, Tp]  energies of step i, bias included (logistic / relu only)
+  float* acc_b;              // [2B]     per-CTA partial sums of de (logistic / relu only)
 };
 
 __host__ __device__ inline int att_bwd_kp(int K) { return K <= 12 ? 12 : 16; }     // padded row of K filter values (float4 loads)
@@ -500,7 +509,8 @@ __device__ __forceinline__ float block_sum_512(float v, float* scratch) {
 
 // KP: padded filter-row length (12 or 16).  Everything indexed by the filter k is held as KP-wide float4 rows so the
 // inner loops are vector shared-memory loads + FMAs; the handler column of a thread lives in registers.
-template <int KP>
+// NORM: the energy normaliser (LVSR_NORM_*); it changes the energy gradient and adds the bias partial only.
+template <int KP, int NORM>
 __global__ void __launch_bounds__(AB_NT, 1) att_bwd_kernel(AttBwdArgs a, int tc_cap) {
   extern __shared__ __align__(16) float smem[];
   constexpr int KV = KP / 4;
@@ -541,7 +551,7 @@ __global__ void __launch_bounds__(AB_NT, 1) att_bwd_kernel(AttBwdArgs a, int tc_
     }
   const float S = block_sum_512(part, sred);      // (contains the __syncthreads that publish the staging)
 
-  // ---- de[t] = alpha_i[t] (dctx . H[t] + carry[t] - S) for the owned positions: one warp per position ----
+  // ---- de[t] for the owned positions (softmax: alpha_i[t] (dctx . H[t] + carry[t] - S)): one warp per position ----
   for (int t = warp; t < nt; t += AB_NT / 32) {
     const long long pos = b0 + t0 + t;
     const float* hrow = a.H + (pos * B + b) * E;
@@ -555,7 +565,14 @@ __global__ void __launch_bounds__(AB_NT, 1) att_bwd_kernel(AttBwdArgs a, int tc_
     if (lane == 0) {
       const long long o = (long long)b * Tp + pos;
       const float carry = a.dA_in ? (a.dA_in[o] + a.dA_in[(long long)B * Tp + o]) : 0.f;
-      sde[t] = a.w_cur[o] * (d + carry - S);
+      if constexpr (NORM == LVSR_NORM_SOFTMAX) {
+        sde[t] = a.w_cur[o] * (d + carry - S);
+      } else if constexpr (NORM == LVSR_NORM_LOGISTIC) {
+        sde[t] = a.w_cur[o] * (1.f / (1.f + expf(a.e_cur[o]))) * (d + carry - S);      // 1 - sigma(e) = sigma(-e)
+      } else {
+        const float e = a.e_cur[o];
+        sde[t] = e > 0.f ? (d + carry - S) * (a.w_cur[o] / e) : 0.f;
+      }
     }
   }
   // ---- location features of the owned positions: F[t,k] = sum_j alpha_cut[t + n - j] filt[k, j];
@@ -670,6 +687,15 @@ __global__ void __launch_bounds__(AB_NT, 1) att_bwd_kernel(AttBwdArgs a, int tc_
 #pragma unroll
     for (int k = 0; k < KP; ++k)
       if (k < K) a.acc_Wh[((long long)blockIdx.x * K + k) * M + m] += dWh[k];
+  }
+  if constexpr (NORM != LVSR_NORM_SOFTMAX) {
+    // energy bias: the owned positions' de, summed by the last warp in a fixed order
+    if (warp == AB_NT / 32 - 1) {
+      float s = 0.f;
+      for (int t = lane; t < nt; t += 32) s += sde[t];
+      s = warp_sum(s);
+      if (lane == 0) a.acc_b[blockIdx.x] += s;
+    }
   }
   // gradient of alpha_{i-1}: dalpha_cut[t'] = sum_j dF[t' - n + j, :] . filt[:, j] over the OWNED t = t' - n + j
   for (int pidx = tid; pidx < Tp; pidx += AB_NT) {

@@ -124,6 +124,7 @@ class SpeechRecognizer(object):
         self.initial_states_init = None
         self.weights_init = None
         self.biases_init = None
+        self._brick_schemes = OrderedDict()          # {brick path below /recognizer: {scheme: value}}
 
         act = post_merge_activation if post_merge_activation is not None else _bricks.Tanh()
         if dim_matcher is None:
@@ -310,31 +311,76 @@ class SpeechRecognizer(object):
             out[name] = arr
         return out
 
-    def initialize(self, seed=1):
-        """Blocks ``initialize()``: one RandomState walked in brick order; a recurrent
-        brick takes rec_weights_init for all three matrices, initial states take
-        initial_states_init (lvsr/bricks/recognizer.py:363-373; B/bricks/recurrent.py:568-580)."""
+    _ROOT_SCHEMES = ("weights_init", "biases_init", "rec_weights_init", "initial_states_init")
+    _BRICK_SCHEMES = ("weights_init", "biases_init")
+
+    def set_initialization(self, path, **schemes):
+        """Initialisation schemes of the Blocks brick at `path`, as one entry of config['initialization'] sets them
+        (lvsr/main.py:223-231).  '/recognizer' takes the four schemes of the recognizer itself; a deeper path takes
+        weights_init / biases_init, which initialize() applies to the parameters of that brick and of the bricks
+        below it, overriding every shallower path's.  A path naming no brick of the model is refused by initialize().
+        """
+        root = "/" + self.name
+        allowed = self._ROOT_SCHEMES if path == root else self._BRICK_SCHEMES
+        unknown = sorted(set(schemes) - set(allowed))
+        if unknown:
+            raise TypeError("initialization of %s: %s not supported (only %s)" % (path, unknown, ", ".join(allowed)))
+        if path == root:
+            for attr, value in schemes.items():
+                setattr(self, attr, value)
+        else:
+            self._brick_schemes.setdefault(path, {}).update(schemes)
+
+    def initial_values(self, shapes, seed=1):
+        """The values initialize() sets, for the parameters `shapes` ({Blocks name: shape} in brick order):
+        Blocks ``initialize()`` with one RandomState walked in brick order; a recurrent brick takes
+        rec_weights_init for all three matrices, initial states take initial_states_init
+        (lvsr/bricks/recognizer.py:363-373; B/bricks/recurrent.py:568-580).  The schemes of set_initialization's
+        deeper paths are pushed after those of /recognizer (lvsr/main.py:223-231, sorted by depth), so the deepest
+        path holding a parameter's brick decides that parameter's scheme.  Such a push sets weights_init only, so
+        under it a recurrent brick's gate matrices follow the path while state_to_state keeps rec_weights_init
+        (its recurrent_weights_init) when /recognizer sets one."""
         w_init = self.weights_init or _bricks.IsotropicGaussian(0.01)
         b_init = self.biases_init or _bricks.Constant(0.0)
         rec_init = self.rec_weights_init or w_init
         h0_init = self.initial_states_init or _bricks.Constant(0.0)
+        overrides = self._brick_schemes
+        bricks = set()
+        for name in shapes:
+            parts = name.rsplit(".", 1)[0].split("/")
+            bricks.update("/".join(parts[:i]) for i in range(2, len(parts) + 1))
+        for path in overrides:
+            if path not in bricks:
+                # the reference's `brick, = Selector(recognizer).select(path).bricks` finds no brick
+                raise ValueError("initialization: no brick of the model at %s" % path)
+
+        def scheme(name, attr, default):
+            brick = name.rsplit(".", 1)[0]
+            holders = [p for p, s in overrides.items() if attr in s and (brick == p or brick.startswith(p + "/"))]
+            return overrides[max(holders, key=lambda p: p.count("/"))][attr] if holders else default
+
         rng = np.random.RandomState(seed)
         values = OrderedDict()
-        for name, shape in self.parameter_shapes().items():
+        for name, shape in shapes.items():
             leaf = name.rsplit(".", 1)[1]
             if leaf == "b":
-                v = b_init.generate(rng, shape)
+                v = scheme(name, "biases_init", b_init).generate(rng, shape)
             elif leaf == "state_to_state":
-                v = rec_init.generate(rng, shape)
+                v = (self.rec_weights_init or scheme(name, "weights_init", w_init)).generate(rng, shape)
             elif leaf == "state_to_gates":
                 d = shape[0]
-                v = np.hstack([rec_init.generate(rng, (d, d)), rec_init.generate(rng, (d, d))])
+                init = scheme(name, "weights_init", rec_init)
+                v = np.hstack([init.generate(rng, (d, d)), init.generate(rng, (d, d))])
             elif leaf == "initial_state":
                 v = h0_init.generate(rng, shape)
             else:
-                v = w_init.generate(rng, shape)
+                v = scheme(name, "weights_init", w_init).generate(rng, shape)
             values[name] = np.asarray(v, dtype=np.float32).reshape(shape)
-        self.set_parameter_values(values)
+        return values
+
+    def initialize(self, seed=1):
+        """Blocks ``initialize()``: the parameters become initial_values(parameter_shapes(), seed)."""
+        self.set_parameter_values(self.initial_values(self.parameter_shapes(), seed))
 
     def load_params(self, path):
         """Blocks checkpoint (tar with a ``_parameters`` npz whose keys use '|' for '/':

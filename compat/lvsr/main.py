@@ -34,7 +34,7 @@ def wer(truth, hyp):
 
 def create_model(config, data, load_path=None, test_tag=False):
     """lvsr/main.py:206-250: SpeechRecognizer(input dims from the data, **config['net']), the initialisation
-    schemes of config['initialization'] pushed onto '/recognizer', initialize(), optional parameter load."""
+    schemes of config['initialization'] set on the bricks their paths name, initialize(), optional parameter load."""
     net = dict(config["net"])
     for unused in ("bottom_class",):
         net.get("bottom", {}).pop(unused, None) if isinstance(net.get("bottom"), dict) else None
@@ -42,12 +42,8 @@ def create_model(config, data, load_path=None, test_tag=False):
         input_dims={"recordings": data.num_features}, input_num_chars={}, eos_label=data.eos_label,
         num_phonemes=data.num_labels, name="recognizer", data_prepend_eos=data.prepend_eos,
         character_map=data.character_map, **net)
-    for path, inits in sorted(config.get("initialization", {}).items()):
-        if path != "/recognizer":
-            logger.warning("initialization for %s ignored: only /recognizer is addressable here", path)
-            continue
-        for attr, value in inits.items():
-            setattr(recognizer, attr, value)
+    for path, inits in config.get("initialization", {}).items():
+        recognizer.set_initialization(path, **inits)
     recognizer.initialize()
     if load_path:
         recognizer.load_params(load_path)

@@ -286,7 +286,9 @@ int lvsr_recognizer_cost_host(lvsr_model* m, const float* recordings_host, const
  *     lvsr_cost_matrix).  cost_dev[0] = gscale * sum(cost_matrix); grads_dev (lvsr_model_flat_size floats, flat
  *     parameter layout) = gscale * d sum(cost_matrix) / d parameter.  Single GPU: gscale = 1/B gives the reference's
  *     cost = sum / batch_size.  N GPUs: pass gscale = 1, all-reduce(sum) grads_dev, then apply with
- *     gscale = 1 / global batch (SURVEY.md 8e).  Softmax energy normaliser only.
+ *     gscale = 1 / global batch (SURVEY.md 8e).  Every energy normaliser: with logistic / relu the gradient of
+ *     energy_comp/linear.b is formed too.  A relu row whose window holds no positive energy is 0 / 0 in the forward,
+ *     as in the reference: its cost and the gradients are not finite (the update then follows RemoveNotFinite(0.0)).
  *   lvsr_train_apply_updates: grads_dev *= gscale (+ 2 decay W on WEIGHT parameters), then the CompositeRule of
  *     lvsr/main.py:509-516: StepClipping(gradient_threshold) -> Momentum(scale, momentum) -> AdaDelta(decay_rate,
  *     epsilon) -> Restrict(VariableClipping(max_norm, axis=0), WEIGHT parameters) -> RemoveNotFinite(0.0) -> BurnIn,
