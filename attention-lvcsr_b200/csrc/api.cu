@@ -114,13 +114,23 @@ void build_param_table(lvsr_model* m) {
   add_param(m, t + "/distribute/fork_gate_inputs.W", E, 2 * C);
 }
 
-int copy_cols(float* dst, int ld_dst, int col0, const float* src, int rows, int cols, cudaStream_t s) {
-  LVSR_CUDA_OK(cudaMemcpy2DAsync(dst + col0, (size_t)ld_dst * sizeof(float), src, (size_t)cols * sizeof(float),
-                                 (size_t)cols * sizeof(float), rows, cudaMemcpyDeviceToDevice, s));
+int copy2d(float* dst, int ld_dst, const float* src, int ld_src, int rows, int cols, cudaStream_t st) {
+  LVSR_CUDA_OK(cudaMemcpy2DAsync(dst, (size_t)ld_dst * sizeof(float), src, (size_t)ld_src * sizeof(float),
+                                 (size_t)cols * sizeof(float), rows, cudaMemcpyDeviceToDevice, st));
   return 0;
 }
 
-
+int fork_copy(lvsr_model* m, const ForkLayout& f, float* W, float* b, float* grads, cudaStream_t st) {
+  for (int bias = 0; bias < 2; ++bias)
+    for (const auto& k : f.block) {
+      const Param* p = m->param(f.fork + "/" + k.param + (bias ? ".b" : ".W"));
+      LVSR_CHECK(p, "fork_copy: %s has no parameter %s", f.fork.c_str(), k.param);
+      float* packed = (bias ? b : W) + k.col;
+      if (int rc = grads ? copy2d(grads + p->offset, k.cols, packed, f.ld, bias ? 1 : f.rows, k.cols, st)   // scatter gradients
+                         : copy2d(packed, f.ld, p->dev, k.cols, bias ? 1 : f.rows, k.cols, st)) return rc;   // pack parameters
+    }
+  return 0;
+}
 
 // take_glimpses for R rows: q = s.W_state, window, attention step.
 struct Segments {           // batched beam search: hypotheses of one utterance = one segment (the reference's batch)
@@ -481,22 +491,20 @@ float* lvsr_model_flat_params(lvsr_model* m) { return m ? m->flat : nullptr; }
 int lvsr_model_set_param(lvsr_model* m, const char* name, const float* host, int64_t count) {
   DeviceGuard device_guard(m);
   LVSR_CHECK(m && name && host, "null argument");
-  auto it = m->index.find(name);
-  LVSR_CHECK(it != m->index.end(), "unknown parameter '%s'", name);
-  Param& p = m->params[it->second];
-  LVSR_CHECK(count == p.count, "parameter '%s' expects %lld values, got %lld", name, (long long)p.count, (long long)count);
-  LVSR_CUDA_OK(cudaMemcpy(p.dev, host, (size_t)count * sizeof(float), cudaMemcpyHostToDevice));
+  const Param* p = m->param(name);
+  LVSR_CHECK(p, "unknown parameter '%s'", name);
+  LVSR_CHECK(count == p->count, "parameter '%s' expects %lld values, got %lld", name, (long long)p->count, (long long)count);
+  LVSR_CUDA_OK(cudaMemcpy(p->dev, host, (size_t)count * sizeof(float), cudaMemcpyHostToDevice));
   m->finalized = false;
   return 0;
 }
 int lvsr_model_get_param(const lvsr_model* m, const char* name, float* host, int64_t count) {
   DeviceGuard device_guard(m);
   LVSR_CHECK(m && name && host, "null argument");
-  auto it = m->index.find(name);
-  LVSR_CHECK(it != m->index.end(), "unknown parameter '%s'", name);
-  const Param& p = m->params[it->second];
-  LVSR_CHECK(count == p.count, "parameter '%s' holds %lld values, asked for %lld", name, (long long)p.count, (long long)count);
-  LVSR_CUDA_OK(cudaMemcpy(host, p.dev, (size_t)count * sizeof(float), cudaMemcpyDeviceToHost));
+  const Param* p = m->param(name);
+  LVSR_CHECK(p, "unknown parameter '%s'", name);
+  LVSR_CHECK(count == p->count, "parameter '%s' holds %lld values, asked for %lld", name, (long long)p->count, (long long)count);
+  LVSR_CUDA_OK(cudaMemcpy(host, p->dev, (size_t)count * sizeof(float), cudaMemcpyDeviceToHost));
   return 0;
 }
 
@@ -605,15 +613,13 @@ static int pack_tc_weights(TcWeights& tw, const float* W, int K, int N, cudaStre
 int finalize_on_stream(lvsr_model* m, cudaStream_t st, bool synchronise) {
   const lvsr_config& c = m->cfg;
   if (m->Wcat.empty()) {
-    int din = c.num_features;
     for (int l = 0; l < c.num_layers; ++l) {
-      const int D = c.dims_bidir[l];
+      const ForkLayout f = encoder_fork(c, l, 0);       // Wcat[l] [rows, ld], bcat[l] [ld]
       float *W = nullptr, *b = nullptr;
-      LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&W), (size_t)din * 6 * D * sizeof(float)));
-      LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&b), (size_t)6 * D * sizeof(float)));
+      LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&W), (size_t)f.rows * f.ld * sizeof(float)));
+      LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&b), (size_t)f.ld * sizeof(float)));
       m->Wcat.push_back(W);
       m->bcat.push_back(b);
-      din = 2 * D;
     }
     const int C = c.dim_dec;
     LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->Wd_cat), (size_t)m->E * 3 * C * sizeof(float)));
@@ -622,39 +628,25 @@ int finalize_on_stream(lvsr_model* m, cudaStream_t st, bool synchronise) {
     LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->bff_cat), (size_t)3 * C * sizeof(float)));
     LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->FF), (size_t)(c.num_phonemes + 1) * 3 * C * sizeof(float)));
   }
-  int din = c.num_features;
-  for (int l = 0; l < c.num_layers; ++l) {
-    const int D = c.dims_bidir[l];
-    for (int dir = 0; dir < 2; ++dir) {
-      const std::string b = enc_base(l, dir);
-      const int c0 = dir * 3 * D;   // per direction: [inputs D | gate_inputs 2D (update | reset)]
-      if (int rc = copy_cols(m->Wcat[l], 6 * D, c0, m->P(b + "/fork/fork_inputs.W"), din, D, st)) return rc;
-      if (int rc = copy_cols(m->Wcat[l], 6 * D, c0 + D, m->P(b + "/fork/fork_gate_inputs.W"), din, 2 * D, st)) return rc;
-      if (int rc = copy_cols(m->bcat[l], 6 * D, c0, m->P(b + "/fork/fork_inputs.b"), 1, D, st)) return rc;
-      if (int rc = copy_cols(m->bcat[l], 6 * D, c0 + D, m->P(b + "/fork/fork_gate_inputs.b"), 1, 2 * D, st)) return rc;
-    }
-    din = 2 * D;
-  }
+  for (int l = 0; l < c.num_layers; ++l)
+    for (int dir = 0; dir < 2; ++dir)
+      if (int rc = fork_copy(m, encoder_fork(c, l, dir), m->Wcat[l], m->bcat[l], nullptr, st)) return rc;
   const int C = c.dim_dec, Cfb = c.dim_feedback, V = c.num_phonemes;
   const std::string g = GEN, t = TR;
   // decoder-side packing: gate columns first (update | reset), then the candidate inputs
-  if (int rc = copy_cols(m->Wd_cat, 3 * C, 0, m->P(t + "/distribute/fork_gate_inputs.W"), m->E, 2 * C, st)) return rc;
-  if (int rc = copy_cols(m->Wd_cat, 3 * C, 2 * C, m->P(t + "/distribute/fork_inputs.W"), m->E, C, st)) return rc;
+  if (int rc = copy2d(m->Wd_cat, 3 * C, m->P(t + "/distribute/fork_gate_inputs.W"), 2 * C, m->E, 2 * C, st)) return rc;
+  if (int rc = copy2d(m->Wd_cat + 2 * C, 3 * C, m->P(t + "/distribute/fork_inputs.W"), C, m->E, C, st)) return rc;
   LVSR_CUDA_OK(cudaMemsetAsync(m->Wb1, 0, (size_t)(m->E + C) * 3 * C * sizeof(float), st));
-  if (int rc = copy_cols(m->Wb1, 3 * C, 0, m->Wd_cat, m->E, 3 * C, st)) return rc;
-  if (int rc = copy_cols(m->Wb1 + (size_t)m->E * 3 * C, 3 * C, 0, m->P(t + "/transition.state_to_gates"), C, 2 * C, st)) return rc;
-  if (int rc = copy_cols(m->Wff_cat, 3 * C, 0, m->P(g + "/fork/fork_gate_inputs.W"), Cfb, 2 * C, st)) return rc;
-  if (int rc = copy_cols(m->Wff_cat, 3 * C, 2 * C, m->P(g + "/fork/fork_inputs.W"), Cfb, C, st)) return rc;
-  if (int rc = copy_cols(m->bff_cat, 3 * C, 0, m->P(g + "/fork/fork_gate_inputs.b"), 1, 2 * C, st)) return rc;
-  if (int rc = copy_cols(m->bff_cat, 3 * C, 2 * C, m->P(g + "/fork/fork_inputs.b"), 1, C, st)) return rc;
+  if (int rc = copy2d(m->Wb1, 3 * C, m->Wd_cat, 3 * C, m->E, 3 * C, st)) return rc;
+  if (int rc = copy2d(m->Wb1 + (size_t)m->E * 3 * C, 3 * C, m->P(t + "/transition.state_to_gates"), 2 * C, C, 2 * C, st)) return rc;
+  if (int rc = fork_copy(m, feedback_fork(c), m->Wff_cat, m->bff_cat, nullptr, st)) return rc;
   // tensor-core operands of the fork and preprocess weights (K-major fp16 head/tail planes or tf32 hi/lo pairs)
   m->use_tc = getenv("LVSR_NO_TC_GEMM") == nullptr;
   if (m->use_tc) {
     m->Wcat_tc.resize(c.num_layers);
-    int dk = c.num_features;
     for (int l = 0; l < c.num_layers; ++l) {
-      if (int rc = pack_tc_weights(m->Wcat_tc[l], m->Wcat[l], dk, 6 * c.dims_bidir[l], st)) return rc;
-      dk = 2 * c.dims_bidir[l];
+      const ForkLayout f = encoder_fork(c, l, 0);
+      if (int rc = pack_tc_weights(m->Wcat_tc[l], m->Wcat[l], f.rows, f.ld, st)) return rc;
     }
     if (int rc = pack_tc_weights(m->Wp_tc, m->P(att_base(m) + "/preprocess.W"), m->E, c.dim_matcher, st)) return rc;
   }
@@ -755,7 +747,7 @@ int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int
     int32_t* plan = m->enc_plan[l];
     if (!pre_done) {
       // finalize splits the fork weights only while the tensor-core GEMM is on (null entry: a shape it refuses)
-      const size_t mark = ws.off;
+      ArenaMark mark{ws};      // the split scratch is dead once the GEMM is enqueued (stream order)
       int kpad = 0, operands = 0;
       if (int rc = projection_gemm(ws, cur, rows, din, m->Wcat[l], m->use_tc ? &m->Wcat_tc[l] : nullptr, 6 * D, m->bcat[l],
                                    pre, st, &kpad, &operands))
@@ -763,7 +755,6 @@ int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int
       plan[LVSR_ENC_PROJ] = kpad ? LVSR_ENC_PATH_TC : LVSR_ENC_PATH_FFMA;
       plan[LVSR_ENC_KPAD] = kpad;
       plan[LVSR_ENC_OPERANDS] = operands;
-      if (ws.off <= ws.cap) ws.off = mark;     // the split scratch is dead once the GEMM is enqueued (stream order)
     }
     pre_done = nullptr;
     float* out = (l == c.num_layers - 1) ? attended : ws.f32((size_t)Tout * B * 2 * D);
@@ -776,7 +767,7 @@ int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int
     a.out = out; a.T = Tl; a.B = B; a.D = D; a.subsample = k;
     if (tape) {
       a.tape = pre; a.hext = hext;
-      tape[l] = {cur, pre, hext, out, Tl, Tout, din, D, k, mstride};
+      tape[l] = {cur, pre, hext, Tl, din, D, k, mstride};
     }
     // Layer l + 1's projection reads only this scan's output: its tiles can run beside the scan, on the SMs the scan
     // leaves idle, as their rows become final -- when the scan runs in one wave of tensor-core clusters that leaves
@@ -795,7 +786,7 @@ int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int
       // the same arena order as without the overlap (pre-activations of l + 1 right after this layer's output), the
       // split planes as projection_gemm takes them, then the scheduling area; all but the pre-activations dead after
       float* pre1 = ws.f32((size_t)rows1 * 6 * D1);
-      const size_t mark = ws.off;
+      ArenaMark mark{ws};
       const int K1 = 2 * D;
       float* a_hi = ws.f32((size_t)rows1 * K1);
       float* a_lo = ws.f32((size_t)rows1 * K1);
@@ -824,7 +815,6 @@ int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int
                                      tw.head, tw.tail, tw.ew, 6 * D1, m->bcat[l1], pre1, 6 * D1, ps, device_sm_count(), st))
           return rc;
       }
-      if (ws.off <= ws.cap) ws.off = mark;
       int32_t* plan1 = m->enc_plan[l1];
       plan1[LVSR_ENC_PROJ] = LVSR_ENC_PATH_TC;
       plan1[LVSR_ENC_KPAD] = K1;
@@ -1053,11 +1043,10 @@ int lvsr_cost_matrix(lvsr_model* m, const float* attended, const float* attended
     float* e_i = energies_out ? energies_out + (size_t)i * B * Tp : e_scratch;
     float* ctx_i = ctx_all + (size_t)i * B * E;
     const float* s_i = s_all + (size_t)i * B * C;
-    const size_t mark = ws.off;
+    ArenaMark mark{ws};   // per-step scratch is reusable (stream order): rewound at the end of every step
     if (int rc = glimpses(m, attended, P, attended_mask, Tp, B, nullptr, B, s_i, w_prev, nullptr, i, w_i, e_i, ctx_i, st)) return rc;
     if (int rc = transition(m, B, s_i, ctx_i, lab + (size_t)i * B, labels_mask ? labels_mask + (size_t)i * B : nullptr,
                             s_all + (size_t)(i + 1) * B * C, st)) return rc;
-    if (ws.off <= ws.cap) ws.off = mark;   // per-step scratch is reusable (stream order)
     w_prev = w_i;
   }
   // the language model's cost rows in force before each label (sequence_generators.py:284-289), then fused below

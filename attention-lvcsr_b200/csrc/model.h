@@ -121,10 +121,10 @@ struct lvsr_model {
   float* flat = nullptr;
   int64_t flat_count = 0;
   // packed, kernel-side weights (rebuilt by finalize)
-  std::vector<float*> Wcat, bcat;   // per encoder layer: [Din, 6D], [6D]
+  std::vector<float*> Wcat, bcat;   // per encoder layer: [Din, 6D], [6D] (encoder_fork)
   float* Wd_cat = nullptr;          // [E, 3C] = [distribute gate_inputs (2C) | distribute inputs (C)]
   float* Wb1 = nullptr;             // [E+C, 3C] = Wd_cat stacked on [state_to_gates | 0] (persistent decoder)
-  float* Wff_cat = nullptr;         // [Cfb, 3C] = [fork gate_inputs | fork inputs]
+  float* Wff_cat = nullptr;         // [Cfb, 3C] (feedback_fork)
   float* bff_cat = nullptr;         // [3C]
   float* FF = nullptr;              // [(V+1), 3C] = lookup . Wff_cat + bff_cat
   // dense-projection weights as the tensor-core GEMM reads them (wgmma path); empty = SIMT path
@@ -180,10 +180,11 @@ struct lvsr_model {
     float* norm_part = nullptr;     // device partial squared norms of the gradient transform
   } noise;
 
-  float* P(const std::string& n) const {
+  const Param* param(const std::string& n) const {     // null when the model has no such parameter
     auto it = index.find(n);
-    return it == index.end() ? nullptr : params[it->second].dev;
+    return it == index.end() ? nullptr : &params[it->second];
   }
+  float* P(const std::string& n) const { const Param* p = param(n); return p ? p->dev : nullptr; }
 };
 
 
@@ -239,6 +240,21 @@ struct ArenaScope {
   ~ArenaScope() { ws.leave(st); }
 };
 
+// Rewinds the workspace to its construction-time offset when the scope ends, unless it overflowed (off > cap)
+struct ArenaMark { Arena& ws; const size_t off = ws.off; ~ArenaMark() { if (ws.off <= ws.cap) ws.off = off; } };
+
+// A packed fork, blocks in column order: <fork>/<param>.W fills columns [col, col + cols) of W [rows, ld], .b those of b [ld]
+struct ForkLayout { std::string fork; int rows, ld; struct { const char* param; int col, cols; } block[2]; };
+// encoder layer l, direction dir, in Wcat[l] / bcat[l]: per direction [inputs D | gate_inputs 2D (update | reset)]
+static inline ForkLayout encoder_fork(const lvsr_config& c, int l, int dir) {
+  const int D = c.dims_bidir[l], c0 = dir * 3 * D, din = l ? 2 * c.dims_bidir[l - 1] : c.num_features;
+  return {enc_base(l, dir) + "/fork", din, 6 * D, {{"fork_inputs", c0, D}, {"fork_gate_inputs", c0 + D, 2 * D}}};
+}
+// fork(feedback(y)) in Wff_cat / bff_cat: [gate_inputs 2C | inputs C]
+static inline ForkLayout feedback_fork(const lvsr_config& c) {
+  return {std::string(GEN) + "/fork", c.dim_feedback, 3 * c.dim_dec, {{"fork_gate_inputs", 0, 2 * c.dim_dec}, {"fork_inputs", 2 * c.dim_dec, c.dim_dec}}};
+}
+
 static inline int check_ready(lvsr_model* m) {
   LVSR_CHECK(m != nullptr, "null model");
   if (!m->finalized) {
@@ -256,13 +272,15 @@ struct LayerTape {
   const float* X;      // input of the layer [T*B, Din]
   float* pre;          // [T*B, 6D] forward tape, then dPre
   float* hext;         // [(T+2), B, 2D]
-  float* out;          // [Tout, B, 2D]
-  int T, Tout, Din, D, k;
+  int T, Din, D, k;
   long long mstride;
 };
 
 // shared orchestration pieces (api.cu)
 int finalize_on_stream(lvsr_model* m, cudaStream_t st, bool synchronise);
+int copy2d(float* dst, int ld_dst, const float* src, int ld_src, int rows, int cols, cudaStream_t st);   // float matrices
+// a packed fork's blocks, W first: parameters -> W / b (grads null), or W / b (gradients) -> the flat gradient buffer
+int fork_copy(lvsr_model* m, const ForkLayout& f, float* W, float* b, float* grads, cudaStream_t st);
 // adaptive weight noise (noise.cu): the sample pass of a training forward (noisy parameters + priors + model cost)
 // and the gradient transform of an update (both gradient groups; *nparts partial sums of squares of their union in
 // noise.norm_part when nparts is not null).  noise_free releases the handle's noise buffers.

@@ -7,14 +7,11 @@
 // -> BurnIn and the in-place update.  The gradient buffer uses the flat parameter layout, so a data-parallel
 // caller all-reduces ONE buffer between lvsr_train_cost_and_grads and lvsr_train_apply_updates (SURVEY.md 8e).
 //
-// Structure of the backward pass:
-//   * everything that does not depend on the recurrence is a LARGE GEMM over all steps at once
-//     (weight gradients X^T dY as split-R TN products, input gradients dY W^T, the decoder's gate values
-//     re-computed for all L steps from the saved states and glimpses);
-//   * the two recurrences are reverse-time scans: bigru_bwd.cu (persistent cluster kernel, same DSMEM
-//     all-gathers as the forward) and the decoder loop below (per step: 4 skinny products, the attention
-//     backward kernel -- 2 CTAs per utterance re-computing tanh(match) instead of storing [L,T',B,M] --
-//     and two element-wise kernels).
+// TrainStep::run: taped forward (DecTape), the transposed weights (made in run, ahead of the readout's buffers, for their
+// place in the arena), readout backward, decoder backward (the reverse-time loop: DecGrads), decoder weight gradients,
+// gradient of the attended sequence, encoder backward.  Work off the recurrences is LARGE GEMMs over all steps.  The
+// recurrences are reverse-time scans: bigru_bwd.cu (persistent cluster kernel) and the decoder loop (per step: 4 skinny
+// products, the attention backward re-computing tanh(match) instead of storing [L,T',B,M], two element-wise kernels).
 #include <stdlib.h>
 
 #include <algorithm>
@@ -44,7 +41,7 @@ int gemm_tn(Arena& ws, const float* A, int lda, const float* B, int ldb, int R, 
   int rps = ceil_div(ceil_div(R, splits), TN_BK) * TN_BK;
   splits = ceil_div(R, rps);
   if (splits_out) *splits_out = splits;
-  const size_t mark = ws.off;
+  ArenaMark mark{ws};                       // partials are dead once the reduce is enqueued (stream order)
   float* part = ws.f32((size_t)splits * Mo * N);
   LVSR_CHECK(part, "out of device memory (TN partials)");
   TnArgs g;
@@ -56,7 +53,6 @@ int gemm_tn(Arena& ws, const float* A, int lda, const float* B, int ldb, int R, 
   LVSR_LAUNCH_CHECK();
   tn_reduce_kernel<<<grid1d((long long)Mo * N), 256, 0, st>>>(part, splits, Mo, N, C, ldc, accumulate ? 1 : 0);
   LVSR_LAUNCH_CHECK();
-  if (ws.off <= ws.cap) ws.off = mark;      // partials are dead once the reduce is enqueued (stream order)
   return 0;
 }
 
@@ -99,18 +95,11 @@ int skinny(const float* X0, int K0, int ldx0, const float* W0, const float* X1, 
   return 0;
 }
 
-int copy2d(float* dst, int ld_dst, const float* src, int ld_src, int rows, int cols, cudaStream_t st) {
-  LVSR_CUDA_OK(cudaMemcpy2DAsync(dst, (size_t)ld_dst * sizeof(float), src, (size_t)ld_src * sizeof(float),
-                                 (size_t)cols * sizeof(float), rows, cudaMemcpyDeviceToDevice, st));
-  return 0;
-}
-
 // K-major (contraction-major) tf32 hi/lo operand of the tensor-core GEMM: [rows, Kpad] built from a [K, rows] matrix
-struct TcOperand { float* hi = nullptr; float* lo = nullptr; int rows = 0, Kpad = 0; };
+struct TcOperand { float* hi = nullptr; float* lo = nullptr; int Kpad = 0; };
 
 // src [R, cols] (leading dimension ld) -> transposed hi/lo pair [cols, kpad(R)]
 int make_tc_operand(Arena& ws, const float* src, int R, int cols, int ld, TcOperand* out, cudaStream_t st) {
-  out->rows = cols;
   out->Kpad = gemm_tc_kpad(R);
   out->hi = ws.f32((size_t)cols * out->Kpad);
   out->lo = ws.f32((size_t)cols * out->Kpad);
@@ -128,49 +117,51 @@ int gemm_tn_tc(Arena& ws, const TcOperand& A, int a0, int Mo, const TcOperand& B
   const int want = std::max(1, std::min(32, ceil_div(device_sm_count(), tiles)));
   const int splits = gemm_tc_splits_launched(A.Kpad, want);
   if (splits_out) *splits_out = splits;
-  const size_t mark = ws.off;
+  ArenaMark mark{ws};
   float* part = ws.f32((size_t)splits * Mo * N);
   LVSR_CHECK(part, "out of device memory (TN partials)");
   if (int rc = gemm_tc_presplit(A.hi + (size_t)a0 * A.Kpad, A.lo + (size_t)a0 * A.Kpad, Mo, B.hi + (size_t)b0 * B.Kpad,
                                 B.lo + (size_t)b0 * B.Kpad, N, A.Kpad, nullptr, part, N, want, (long long)Mo * N, st)) return rc;
   tn_reduce_kernel<<<grid1d((long long)Mo * N), 256, 0, st>>>(part, splits, Mo, N, C, ldc, accumulate ? 1 : 0);
   LVSR_LAUNCH_CHECK();
-  if (ws.off <= ws.cap) ws.off = mark;
   return 0;
 }
 
-float* grad_of(lvsr_model* m, float* grads, const std::string& name) {
-  auto it = m->index.find(name);
-  return it == m->index.end() ? nullptr : grads + m->params[it->second].offset;
-}
+// The decoder's tape: attended sequence and mask, per step costs, alignments, energies (softmax: null), s_{i-1}, glimpses
+struct DecTape { float *Hatt, *attm, *costs, *W_all, *E_all, *S_prev, *CTX; };
+// Decoder backward's results: [dGz|dGr|dA], re-computed HR, dCTX, dq partials [L][2][B][M], dP, attention-constant partials
+struct DecGrads { float *dG, *HR, *dCTX, *dQp, *dP, *acc_v, *acc_Wh, *acc_filt, *acc_b; };
 
-// forward + backward of one batch on the parameters Param::dev points at and the weights packed from them
-int forward_backward(lvsr_model* m, const float* x, const float* mask, const int64_t* labels, const float* lmask,
-                     int32_t T, int32_t B, int32_t L, float gscale, float* cost_out, float* grads, void* stream) {
-  if (int rc = check_ready(m)) return rc;
-  LVSR_CHECK(x && labels && cost_out && grads && T > 0 && B > 0 && L > 0, "train_cost_and_grads: bad arguments");
-  LVSR_CHECK(!lm_attached(m), "train_cost_and_grads: shallow fusion is inference only (detach the language model)");
+// One training step's shapes and handles; phases read parameters via m->P as they run (adaptive noise re-points them)
+struct TrainStep {
+  lvsr_model* m;
+  cudaStream_t st;
+  const int64_t* labels;
+  const float* lmask;
+  float* grads;
+  float gscale;
+  int B, L, Tp;
   const lvsr_config& c = m->cfg;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  Arena& ws = m->tws;
+  const long long* lab = reinterpret_cast<const long long*>(labels);
   const int C = c.dim_dec, E = m->E, M = c.dim_matcher, K = c.conv_num_filters, n = c.conv_n, w = 2 * n + 1;
   const int V = c.num_phonemes, Cfb = c.dim_feedback, Cpm = c.post_merge_dim, Hd = Cpm / c.maxout_pieces;
-  const int Tp = lvsr_encoded_length(m, T);
-  const int R = L * B;
-  // shapes the backward kernels cannot take are refused before any work is enqueued
-  const size_t ro_smem = (size_t)8 * (Hd + 128) * sizeof(float);
-  LVSR_CHECK(ro_smem <= 48 * 1024 && V <= 128, "readout backward: post_merge_dim / num_phonemes too large");
+  const int R = L * B, nct = AB_CS * B, tc_cap = ceil_div(Tp, AB_CS);
   const bool content = content_attention(m);
   // the logistic and relu energy gradients read the step's energies, which the softmax one does not need
   const bool keep_energies = c.energy_normalizer != LVSR_NORM_SOFTMAX;
-  const int tc_cap = ceil_div(Tp, AB_CS);
+  const size_t ro_smem = (size_t)8 * (Hd + 128) * sizeof(float);
   const size_t ab_smem = (content ? att_bwd_content_smem_floats(E, tc_cap) : att_bwd_smem_floats(M, E, K, n, tc_cap)) * sizeof(float);
-  LVSR_CHECK(ab_smem <= 227 * 1024 && M <= AB_NT && M % 128 == 0 && K <= 16 && E % 4 == 0,
-             "attention backward: shape unsupported (Tp=%d M=%d)", Tp, M);
-  LVSR_CHECK(E <= 1024, "encoded dim %d > 1024 unsupported in training", E);
-  const long long* lab = reinterpret_cast<const long long*>(labels);
-  Arena& ws = m->tws;
-  // size the tape arena once per shape
-  {
+  const std::string g = GEN, t = TR, at = att_base(m);
+  float* grad(const std::string& name) const { const Param* p = m->param(name); return p ? grads + p->offset : nullptr; }
+
+  int run(const float* x, const float* mask, int T, float* cost_out) const {
+    // shapes the backward kernels cannot take are refused before any work is enqueued
+    LVSR_CHECK(ro_smem <= 48 * 1024 && V <= 128, "readout backward: post_merge_dim / num_phonemes too large");
+    LVSR_CHECK(ab_smem <= 227 * 1024 && M <= AB_NT && M % 128 == 0 && K <= 16 && E % 4 == 0,
+               "attention backward: shape unsupported (Tp=%d M=%d)", Tp, M);
+    LVSR_CHECK(E <= 1024, "encoded dim %d > 1024 unsupported in training", E);
+    // size the tape arena once per shape
     size_t bytes = (size_t)64 << 20;
     int Tl = T, din = c.num_features;
     for (int l = 0; l < c.num_layers; ++l) {
@@ -184,69 +175,74 @@ int forward_backward(lvsr_model* m, const float* x, const float* mask, const int
               (size_t)2 * B * (M + (size_t)K * M + (size_t)K * w) + (size_t)4 * (E + C) * 3 * C + (size_t)80 * E * M) * sizeof(float);
     if (keep_energies) bytes += ((size_t)R * Tp + (size_t)AB_CS * B) * sizeof(float);
     ws.reserve(bytes, st);
+    ArenaScope scope(ws, st);
+    for (int l = 0; l < c.num_layers; ++l)
+      for (int s = LVSR_ENC_BWD_CS; s <= LVSR_ENC_DX; ++s) m->enc_plan[l][s] = 0;
+    LVSR_CUDA_OK(cudaMemsetAsync(grads, 0, (size_t)m->flat_count * sizeof(float), st));
+    std::vector<LayerTape> tape(c.num_layers);
+    DecTape d;
+    if (int rc = taped_forward(x, mask, T, tape.data(), cost_out, d)) return rc;
+    // dY . W^T right-hand sides, transposed here, not in the phases that read them, to keep their arena place ahead of
+    // the readout's and decoder backward's buffers: placement can move the step time (DESIGN.md section 6, item 4)
+    float* WmsT = c.use_states_for_readout ? ws.f32((size_t)Cpm * C) : nullptr;     // [Cpm, C]
+    float* WmcT = ws.f32((size_t)Cpm * E);
+    float* WstateT = ws.f32((size_t)C * C);
+    float* WgT = ws.f32((size_t)2 * C * C);             // [2C, C]
+    float* WdcatT = ws.f32((size_t)3 * C * E);          // [3C, E]
+    float* WsT = ws.f32((size_t)M * C);                 // [M, C]
+    float* WpT = ws.f32((size_t)M * E);                 // [M, E]
+    LVSR_CHECK(WmcT && WstateT && WgT && WdcatT && WsT && WpT, "out of device memory (transposed weights)");
+    if (WmsT) if (int rc = transpose(m->P(g + "/readout/merge/transform_states.W"), WmsT, C, Cpm, st)) return rc;
+    if (int rc = transpose(m->P(g + "/readout/merge/transform_weighted_averages.W"), WmcT, E, Cpm, st)) return rc;
+    if (int rc = transpose(m->P(t + "/transition.state_to_state"), WstateT, C, C, st)) return rc;
+    if (int rc = transpose(m->P(t + "/transition.state_to_gates"), WgT, C, 2 * C, st)) return rc;
+    if (int rc = transpose(m->Wd_cat, WdcatT, E, 3 * C, st)) return rc;
+    // [dG (3C)] . WcombT [3C, C + E] = [ grad of s_{i-1} through the gates | grad of the glimpse ]: one product per step
+    float* WcombT = ws.f32((size_t)3 * C * (C + E));
+    LVSR_CHECK(WcombT, "out of device memory (transposed weights)");
+    LVSR_CUDA_OK(cudaMemsetAsync(WcombT, 0, (size_t)3 * C * (C + E) * sizeof(float), st));
+    if (int rc = copy2d(WcombT, C + E, WgT, C, 2 * C, C, st)) return rc;
+    if (int rc = copy2d(WcombT + C, C + E, WdcatT, E, 3 * C, E, st)) return rc;
+    if (int rc = transpose(m->P(at + "/state_trans/transform_states.W"), WsT, C, M, st)) return rc;
+    if (int rc = transpose(m->P(at + "/preprocess.W"), WpT, E, M, st)) return rc;
+    float *dS_ro, *dCtx_ro, *dH;
+    DecGrads dg;
+    if (int rc = readout_backward(d, WmsT, WmcT, dS_ro, dCtx_ro)) return rc;
+    if (int rc = decoder_backward(d, WstateT, WcombT, WsT, dS_ro, dCtx_ro, dg)) return rc;
+    if (int rc = decoder_weight_grads(d, dg)) return rc;
+    if (int rc = attended_grad(d, dg, WpT, dH)) return rc;
+    return encoder_backward(tape.data(), mask, dH);
   }
-  ArenaScope scope(ws, st);
-  for (int l = 0; l < c.num_layers; ++l)
-    for (int s = LVSR_ENC_BWD_CS; s <= LVSR_ENC_DX; ++s) m->enc_plan[l][s] = 0;
-  LVSR_CUDA_OK(cudaMemsetAsync(grads, 0, (size_t)m->flat_count * sizeof(float), st));
-
-  // =========================== forward, keeping the tape ===========================
-  float* Hatt = ws.f32((size_t)Tp * B * E);                  // attended [Tp, B, E]
-  float* attm = ws.f32((size_t)Tp * B);
-  LVSR_CHECK(Hatt && attm, "out of device memory (encoder output)");
-  std::vector<LayerTape> tape(c.num_layers);
-  if (int rc = run_encoder(m, ws, x, mask, T, B, Hatt, attm, tape.data(), st)) return rc;
-  float* costs = ws.f32((size_t)R);
-  float* W_all = ws.f32((size_t)R * Tp);        // alignments alpha_i
-  float* S_prev = ws.f32((size_t)R * C);        // s_{i-1}
-  float* CTX = ws.f32((size_t)R * E);           // weighted averages
-  float* E_all = keep_energies ? ws.f32((size_t)R * Tp) : nullptr;     // energies e_i, bias included
-  LVSR_CHECK(costs && W_all && S_prev && CTX && (E_all || !keep_energies), "out of device memory (decoder tape)");
-  if (int rc = lvsr_cost_matrix(m, Hatt, attm, Tp, B, labels, lmask, L, costs, W_all, E_all, S_prev, CTX, stream)) return rc;
-  sum_all_kernel<<<1, 1024, 0, st>>>(costs, R, cost_out, gscale);
-  LVSR_LAUNCH_CHECK();
-
-  // =========================== backward ===========================
-  const std::string g = GEN, t = TR, at = att_base(m);
-  // ---- transposed weights used as right-hand sides of dY . W^T -------------------------------
-  float* WoT_unused = nullptr; (void)WoT_unused;
-  float* WmsT = c.use_states_for_readout ? ws.f32((size_t)Cpm * C) : nullptr;     // [Cpm, C]
-  float* WmcT = ws.f32((size_t)Cpm * E);
-  float* WstateT = ws.f32((size_t)C * C);
-  float* WgT = ws.f32((size_t)2 * C * C);             // [2C, C]
-  float* WdcatT = ws.f32((size_t)3 * C * E);          // [3C, E]
-  float* WsT = ws.f32((size_t)M * C);                 // [M, C]
-  float* WpT = ws.f32((size_t)M * E);                 // [M, E]
-  LVSR_CHECK(WmcT && WstateT && WgT && WdcatT && WsT && WpT, "out of device memory (transposed weights)");
-  if (WmsT) if (int rc = transpose(m->P(g + "/readout/merge/transform_states.W"), WmsT, C, Cpm, st)) return rc;
-  if (int rc = transpose(m->P(g + "/readout/merge/transform_weighted_averages.W"), WmcT, E, Cpm, st)) return rc;
-  if (int rc = transpose(m->P(t + "/transition.state_to_state"), WstateT, C, C, st)) return rc;
-  if (int rc = transpose(m->P(t + "/transition.state_to_gates"), WgT, C, 2 * C, st)) return rc;
-  if (int rc = transpose(m->Wd_cat, WdcatT, E, 3 * C, st)) return rc;
-  // [dG (3C)] . WcombT [3C, C + E] = [ grad of s_{i-1} through the gates | grad of the glimpse ]: one product per step
-  float* WcombT = ws.f32((size_t)3 * C * (C + E));
-  LVSR_CHECK(WcombT, "out of device memory (transposed weights)");
-  LVSR_CUDA_OK(cudaMemsetAsync(WcombT, 0, (size_t)3 * C * (C + E) * sizeof(float), st));
-  if (int rc = copy2d(WcombT, C + E, WgT, C, 2 * C, C, st)) return rc;
-  if (int rc = copy2d(WcombT + C, C + E, WdcatT, E, 3 * C, E, st)) return rc;
-  if (int rc = transpose(m->P(at + "/state_trans/transform_states.W"), WsT, C, M, st)) return rc;
-  if (int rc = transpose(m->P(at + "/preprocess.W"), WpT, E, M, st)) return rc;
-
-  // ---- readout + emitter backward (all steps at once) ----------------------------------------
-  float* merged = ws.f32((size_t)R * Cpm);
-  float* hid = ws.f32((size_t)R * Hd);
-  float* dlogits = ws.f32((size_t)R * V);
-  float* dmerged = ws.f32((size_t)R * Cpm);
-  float* dS_ro = ws.f32((size_t)R * C);
-  float* dCtx_ro = ws.f32((size_t)R * E);
-  LVSR_CHECK(merged && hid && dlogits && dmerged && dS_ro && dCtx_ro, "out of device memory (readout backward)");
-  {
-    bool acc = false;
-    if (c.use_states_for_readout) {
-      if (int rc = gemm_nn(S_prev, R, C, C, m->P(g + "/readout/merge/transform_states.W"), Cpm, Cpm, nullptr, merged, Cpm, false, st)) return rc;
-      acc = true;
-    }
-    if (int rc = gemm_nn(CTX, R, E, E, m->P(g + "/readout/merge/transform_weighted_averages.W"), Cpm, Cpm, nullptr, merged, Cpm, acc, st)) return rc;
+  // Taped forward: the encoder keeping its tape, then the teacher-forced decoder; *cost_out = sum(costs) * gscale
+  int taped_forward(const float* x, const float* mask, int T, LayerTape* tape, float* cost_out, DecTape& d) const {
+    d.Hatt = ws.f32((size_t)Tp * B * E);                  // attended [Tp, B, E]
+    d.attm = ws.f32((size_t)Tp * B);
+    LVSR_CHECK(d.Hatt && d.attm, "out of device memory (encoder output)");
+    if (int rc = run_encoder(m, ws, x, mask, T, B, d.Hatt, d.attm, tape, st)) return rc;
+    d.costs = ws.f32((size_t)R);
+    d.W_all = ws.f32((size_t)R * Tp);        // alignments alpha_i
+    d.S_prev = ws.f32((size_t)R * C);        // s_{i-1}
+    d.CTX = ws.f32((size_t)R * E);           // weighted averages
+    d.E_all = keep_energies ? ws.f32((size_t)R * Tp) : nullptr;     // energies e_i, bias included
+    LVSR_CHECK(d.costs && d.W_all && d.S_prev && d.CTX && (d.E_all || !keep_energies), "out of device memory (decoder tape)");
+    if (int rc = lvsr_cost_matrix(m, d.Hatt, d.attm, Tp, B, labels, lmask, L, d.costs, d.W_all, d.E_all, d.S_prev, d.CTX, st)) return rc;
+    sum_all_kernel<<<1, 1024, 0, st>>>(d.costs, R, cost_out, gscale);
+    LVSR_LAUNCH_CHECK();
+    return 0;
+  }
+  // Readout + emitter backward, all steps at once; dS_ro / dCtx_ro: its gradients of the states and the glimpses
+  int readout_backward(const DecTape& d, const float* WmsT, const float* WmcT, float*& dS_ro, float*& dCtx_ro) const {
+    float* merged = ws.f32((size_t)R * Cpm);
+    float* hid = ws.f32((size_t)R * Hd);
+    float* dlogits = ws.f32((size_t)R * V);
+    float* dmerged = ws.f32((size_t)R * Cpm);
+    dS_ro = ws.f32((size_t)R * C);
+    dCtx_ro = ws.f32((size_t)R * E);
+    LVSR_CHECK(merged && hid && dlogits && dmerged && dS_ro && dCtx_ro, "out of device memory (readout backward)");
+    if (c.use_states_for_readout)
+      if (int rc = gemm_nn(d.S_prev, R, C, C, m->P(g + "/readout/merge/transform_states.W"), Cpm, Cpm, nullptr, merged, Cpm, false, st)) return rc;
+    if (int rc = gemm_nn(d.CTX, R, E, E, m->P(g + "/readout/merge/transform_weighted_averages.W"), Cpm, Cpm, nullptr, merged, Cpm,
+                         c.use_states_for_readout, st)) return rc;
     ReadoutBwdArgs rb = {};
     rb.merged = merged; rb.b_pm = m->P(g + "/readout/post_merge/bias.b"); rb.Wo = m->P(g + "/readout/post_merge/mlp/linear_0.W");
     rb.bo = m->P(g + "/readout/post_merge/mlp/linear_0.b");
@@ -254,82 +250,78 @@ int forward_backward(lvsr_model* m, const float* x, const float* mask, const int
     rb.labels = lab; rb.lmask = lmask; rb.gscale = gscale; rb.hid = hid; rb.dlogits = dlogits; rb.dmerged = dmerged;
     readout_bwd_kernel<<<ceil_div(R, 8), 256, ro_smem, st>>>(rb);
     LVSR_LAUNCH_CHECK();
-    if (int rc = gemm_tn(ws, hid, Hd, dlogits, V, R, Hd, V, grad_of(m, grads, g + "/readout/post_merge/mlp/linear_0.W"), V, false, st)) return rc;
-    if (int rc = colsum(dlogits, R, V, V, grad_of(m, grads, g + "/readout/post_merge/mlp/linear_0.b"), false, st)) return rc;
-    if (int rc = colsum(dmerged, R, Cpm, Cpm, grad_of(m, grads, g + "/readout/post_merge/bias.b"), false, st)) return rc;
-    if (int rc = gemm_tn(ws, CTX, E, dmerged, Cpm, R, E, Cpm, grad_of(m, grads, g + "/readout/merge/transform_weighted_averages.W"), Cpm, false, st)) return rc;
+    if (int rc = gemm_tn(ws, hid, Hd, dlogits, V, R, Hd, V, grad(g + "/readout/post_merge/mlp/linear_0.W"), V, false, st)) return rc;
+    if (int rc = colsum(dlogits, R, V, V, grad(g + "/readout/post_merge/mlp/linear_0.b"), false, st)) return rc;
+    if (int rc = colsum(dmerged, R, Cpm, Cpm, grad(g + "/readout/post_merge/bias.b"), false, st)) return rc;
+    if (int rc = gemm_tn(ws, d.CTX, E, dmerged, Cpm, R, E, Cpm, grad(g + "/readout/merge/transform_weighted_averages.W"), Cpm, false, st)) return rc;
     if (int rc = gemm_nn(dmerged, R, Cpm, Cpm, WmcT, E, E, nullptr, dCtx_ro, E, false, st)) return rc;
     if (c.use_states_for_readout) {
-      if (int rc = gemm_tn(ws, S_prev, C, dmerged, Cpm, R, C, Cpm, grad_of(m, grads, g + "/readout/merge/transform_states.W"), Cpm, false, st)) return rc;
+      if (int rc = gemm_tn(ws, d.S_prev, C, dmerged, Cpm, R, C, Cpm, grad(g + "/readout/merge/transform_states.W"), Cpm, false, st)) return rc;
       if (int rc = gemm_nn(dmerged, R, Cpm, Cpm, WmsT, C, C, nullptr, dS_ro, C, false, st)) return rc;
     } else {
       LVSR_CUDA_OK(cudaMemsetAsync(dS_ro, 0, (size_t)R * C * sizeof(float), st));
     }
+    return 0;
   }
-
-  // ---- decoder: gate values of all steps, then the reverse-time loop --------------------------
-  float* G = ws.f32((size_t)R * 3 * C);          // pre-activations -> third block keeps the candidate input
-  float* Z = ws.f32((size_t)R * C);
-  float* Rg = ws.f32((size_t)R * C);
-  float* HR = ws.f32((size_t)R * C);
-  float* Cc = ws.f32((size_t)R * C);
-  float* Q = ws.f32((size_t)R * M);
-  float* P = ws.f32((size_t)Tp * B * M);
-  float* dP = ws.f32((size_t)Tp * B * M);
-  float* dG = ws.f32((size_t)R * 3 * C);         // [dGz | dGr | dA] of every step
-  float* dCTX = ws.f32((size_t)R * E);
-  float* dQp = ws.f32((size_t)2 * R * M);        // the two CTAs' partial dq of every step
-  float* dsbuf[2] = {ws.f32((size_t)B * C), ws.f32((size_t)B * C)};
-  float* keep = ws.f32((size_t)B * C);
-  float* dHR = ws.f32((size_t)B * C);
-  float* dspart = ws.f32((size_t)B * C);
-  float* dAbuf[2] = {ws.f32((size_t)2 * B * Tp), ws.f32((size_t)2 * B * Tp)};
-  float* w0 = ws.f32((size_t)B * Tp);
-  const int nct = AB_CS * B;
-  float* acc_v = ws.f32((size_t)nct * M);
-  float* acc_Wh = ws.f32((size_t)nct * K * M);
-  float* acc_filt = ws.f32((size_t)nct * K * w);
-  float* acc_b = keep_energies ? ws.f32((size_t)nct) : nullptr;
-  int* win = ws.i32(2);
-  float* lohi = ws.f32((size_t)2 * B);
-  LVSR_CHECK(G && Z && Rg && HR && Cc && Q && P && dP && dG && dCTX && dQp && dsbuf[0] && dsbuf[1] && keep && dHR && dspart &&
-                 dAbuf[0] && dAbuf[1] && w0 && acc_v && (content || (acc_Wh && acc_filt)) && (acc_b || !keep_energies) &&
-                 win && lohi,
-             "out of device memory (decoder backward)");
-  if (int rc = lvsr_preprocess(m, Hatt, Tp, B, P, stream)) return rc;
-  if (int rc = gemm_nn(CTX, R, E, E, m->Wd_cat, 3 * C, 3 * C, nullptr, G, 3 * C, false, st)) return rc;
-  if (int rc = gemm_nn(S_prev, R, C, C, m->P(t + "/transition.state_to_gates"), 2 * C, 2 * C, nullptr, G, 3 * C, true, st)) return rc;
-  dec_gates_kernel<<<grid1d((long long)R * 3 * C), 256, 0, st>>>(G, m->FF, lab, S_prev, R, C, Z, Rg, HR);
-  LVSR_LAUNCH_CHECK();
-  {
-    const size_t mark = ws.off;
-    float* Cpre = ws.f32((size_t)R * C);
-    LVSR_CHECK(Cpre, "out of device memory");
-    if (int rc = gemm_nn(HR, R, C, C, m->P(t + "/transition.state_to_state"), C, C, nullptr, Cpre, C, false, st)) return rc;
-    dec_cand_kernel<<<grid1d((long long)R * C), 256, 0, st>>>(Cpre, G, R, C, Cc);
+  // Decoder backward: gate values of all steps re-computed, then the reverse-time loop; writes the initial state's gradient
+  int decoder_backward(const DecTape& d, const float* WstateT, const float* WcombT, const float* WsT, const float* dS_ro,
+                       const float* dCtx_ro, DecGrads& out) const {
+    float* G = ws.f32((size_t)R * 3 * C);          // pre-activations -> third block keeps the candidate input
+    float* Z = ws.f32((size_t)R * C);
+    float* Rg = ws.f32((size_t)R * C);
+    float* HR = ws.f32((size_t)R * C);
+    float* Cc = ws.f32((size_t)R * C);
+    float* Q = ws.f32((size_t)R * M);
+    float* P = ws.f32((size_t)Tp * B * M);
+    float* dP = ws.f32((size_t)Tp * B * M);
+    float* dG = ws.f32((size_t)R * 3 * C);         // [dGz | dGr | dA] of every step
+    float* dCTX = ws.f32((size_t)R * E);
+    float* dQp = ws.f32((size_t)2 * R * M);        // the two CTAs' partial dq of every step
+    float* dsbuf[2] = {ws.f32((size_t)B * C), ws.f32((size_t)B * C)};
+    float* keep = ws.f32((size_t)B * C);
+    float* dHR = ws.f32((size_t)B * C);
+    float* dspart = ws.f32((size_t)B * C);
+    float* dAbuf[2] = {ws.f32((size_t)2 * B * Tp), ws.f32((size_t)2 * B * Tp)};
+    float* w0 = ws.f32((size_t)B * Tp);
+    float* acc_v = ws.f32((size_t)nct * M);
+    float* acc_Wh = ws.f32((size_t)nct * K * M);
+    float* acc_filt = ws.f32((size_t)nct * K * w);
+    float* acc_b = keep_energies ? ws.f32((size_t)nct) : nullptr;
+    int* win = ws.i32(2);
+    float* lohi = ws.f32((size_t)2 * B);
+    LVSR_CHECK(G && Z && Rg && HR && Cc && Q && P && dP && dG && dCTX && dQp && dsbuf[0] && dsbuf[1] && keep && dHR && dspart &&
+                   dAbuf[0] && dAbuf[1] && w0 && acc_v && (content || (acc_Wh && acc_filt)) && (acc_b || !keep_energies) &&
+                   win && lohi,
+               "out of device memory (decoder backward)");
+    if (int rc = lvsr_preprocess(m, d.Hatt, Tp, B, P, st)) return rc;
+    if (int rc = gemm_nn(d.CTX, R, E, E, m->Wd_cat, 3 * C, 3 * C, nullptr, G, 3 * C, false, st)) return rc;
+    if (int rc = gemm_nn(d.S_prev, R, C, C, m->P(t + "/transition.state_to_gates"), 2 * C, 2 * C, nullptr, G, 3 * C, true, st)) return rc;
+    dec_gates_kernel<<<grid1d((long long)R * 3 * C), 256, 0, st>>>(G, m->FF, lab, d.S_prev, R, C, Z, Rg, HR);
     LVSR_LAUNCH_CHECK();
-    if (ws.off <= ws.cap) ws.off = mark;
-  }
-  if (int rc = gemm_nn(S_prev, R, C, C, m->P(at + "/state_trans/transform_states.W"), M, M, nullptr, Q, M, false, st)) return rc;
-  LVSR_CUDA_OK(cudaMemsetAsync(dP, 0, (size_t)Tp * B * M * sizeof(float), st));
-  LVSR_CUDA_OK(cudaMemsetAsync(acc_v, 0, (size_t)nct * M * sizeof(float), st));
-  if (!content) {
-    LVSR_CUDA_OK(cudaMemsetAsync(acc_Wh, 0, (size_t)nct * K * M * sizeof(float), st));
-    LVSR_CUDA_OK(cudaMemsetAsync(acc_filt, 0, (size_t)nct * K * w * sizeof(float), st));
-  }
-  if (acc_b) LVSR_CUDA_OK(cudaMemsetAsync(acc_b, 0, (size_t)nct * sizeof(float), st));
-  LVSR_CUDA_OK(cudaMemsetAsync(dsbuf[0], 0, (size_t)B * C * sizeof(float), st));
-  if (int rc = onehot_rows(w0, B, Tp, st)) return rc;
-  {
+    {
+      ArenaMark mark{ws};
+      float* Cpre = ws.f32((size_t)R * C);
+      LVSR_CHECK(Cpre, "out of device memory");
+      if (int rc = gemm_nn(HR, R, C, C, m->P(t + "/transition.state_to_state"), C, C, nullptr, Cpre, C, false, st)) return rc;
+      dec_cand_kernel<<<grid1d((long long)R * C), 256, 0, st>>>(Cpre, G, R, C, Cc);
+      LVSR_LAUNCH_CHECK();
+    }
+    if (int rc = gemm_nn(d.S_prev, R, C, C, m->P(at + "/state_trans/transform_states.W"), M, M, nullptr, Q, M, false, st)) return rc;
+    LVSR_CUDA_OK(cudaMemsetAsync(dP, 0, (size_t)Tp * B * M * sizeof(float), st));
+    LVSR_CUDA_OK(cudaMemsetAsync(acc_v, 0, (size_t)nct * M * sizeof(float), st));
+    if (!content) {
+      LVSR_CUDA_OK(cudaMemsetAsync(acc_Wh, 0, (size_t)nct * K * M * sizeof(float), st));
+      LVSR_CUDA_OK(cudaMemsetAsync(acc_filt, 0, (size_t)nct * K * w * sizeof(float), st));
+    }
+    if (acc_b) LVSR_CUDA_OK(cudaMemsetAsync(acc_b, 0, (size_t)nct * sizeof(float), st));
+    LVSR_CUDA_OK(cudaMemsetAsync(dsbuf[0], 0, (size_t)B * C * sizeof(float), st));
+    if (int rc = onehot_rows(w0, B, Tp, st)) return rc;
     void (*att_bwd)(AttBwdArgs, int) = att_bwd_content_kernel;
     if (!content) {
       const bool kp12 = att_bwd_kp(K) == 12;
-      if (c.energy_normalizer == LVSR_NORM_LOGISTIC)
-        att_bwd = kp12 ? att_bwd_kernel<12, LVSR_NORM_LOGISTIC> : att_bwd_kernel<16, LVSR_NORM_LOGISTIC>;
-      else if (c.energy_normalizer == LVSR_NORM_RELU)
-        att_bwd = kp12 ? att_bwd_kernel<12, LVSR_NORM_RELU> : att_bwd_kernel<16, LVSR_NORM_RELU>;
-      else
-        att_bwd = kp12 ? att_bwd_kernel<12, LVSR_NORM_SOFTMAX> : att_bwd_kernel<16, LVSR_NORM_SOFTMAX>;
+      if (c.energy_normalizer == LVSR_NORM_LOGISTIC) att_bwd = kp12 ? att_bwd_kernel<12, LVSR_NORM_LOGISTIC> : att_bwd_kernel<16, LVSR_NORM_LOGISTIC>;
+      else if (c.energy_normalizer == LVSR_NORM_RELU) att_bwd = kp12 ? att_bwd_kernel<12, LVSR_NORM_RELU> : att_bwd_kernel<16, LVSR_NORM_RELU>;
+      else att_bwd = kp12 ? att_bwd_kernel<12, LVSR_NORM_SOFTMAX> : att_bwd_kernel<16, LVSR_NORM_SOFTMAX>;
     }
     LVSR_CUDA_OK(cudaFuncSetAttribute(att_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ab_smem));
     const int ew = ceil_div(B * C, 256);
@@ -339,7 +331,7 @@ int forward_backward(lvsr_model* m, const float* x, const float* mask, const int
       float* ds_next = dsbuf[(L - i) & 1];
       const float* lm_i = lmask ? lmask + (size_t)i * B : nullptr;
       float* dG_i = dG + (size_t)i * B * 3 * C;
-      const float* Sp_i = S_prev + (size_t)i * B * C;
+      const float* Sp_i = d.S_prev + (size_t)i * B * C;
       dec_bwd_a_kernel<<<ew, 256, 0, st>>>(ds, Z + (size_t)i * B * C, Cc + (size_t)i * B * C, Sp_i, lm_i, B, C, dG_i, keep);
       LVSR_LAUNCH_CHECK();
       if (int rc = skinny(dG_i + 2 * C, C, 3 * C, WstateT, nullptr, 0, 0, nullptr, nullptr, 0, nullptr, 0, dHR, C, B, C, st)) return rc;
@@ -350,22 +342,22 @@ int forward_backward(lvsr_model* m, const float* x, const float* mask, const int
       if (int rc = skinny(dG_i, 3 * C, 3 * C, WcombT, nullptr, 0, 0, nullptr, keep, C, dCtx_ro + (size_t)i * B * E, E, dspart, C, B, C + E, st,
                           C, dctx_i, E)) return rc;
       // attention backward
-      const float* w_prev = i == 0 ? w0 : W_all + (size_t)(i - 1) * B * Tp;
+      const float* w_prev = i == 0 ? w0 : d.W_all + (size_t)(i - 1) * B * Tp;
       if (!content) {                     // content attention attends every frame: no window
         WindowArgs wa = {};
         wa.weights = w_prev; wa.step = nullptr; wa.step_offset = i; wa.R = B; wa.Tp = Tp; wa.prior = prior_of(c); wa.win = win; wa.lohi = lohi;
         if (int rc = attention_window(wa, st)) return rc;
       }
       AttBwdArgs ab = {};
-      ab.P = P; ab.H = Hatt; ab.maskH = attm; ab.q = Q + (size_t)i * B * M; ab.w_prev = w_prev; ab.w_cur = W_all + (size_t)i * B * Tp;
-      ab.ctx = CTX + (size_t)i * B * E; ab.dctx = dctx_i;
+      ab.P = P; ab.H = d.Hatt; ab.maskH = d.attm; ab.q = Q + (size_t)i * B * M; ab.w_prev = w_prev; ab.w_cur = d.W_all + (size_t)i * B * Tp;
+      ab.ctx = d.CTX + (size_t)i * B * E; ab.dctx = dctx_i;
       ab.dA_in = (i == L - 1) ? nullptr : dAbuf[(L - 1 - i) & 1];
       ab.win = win;
       ab.filt = m->P(at + "/conv1d.filters"); ab.Wh = m->P(at + "/handler.W"); ab.v = m->P(at + "/energy_comp/linear.W");
       ab.dP = dP; ab.dq_part = dQp + (size_t)i * 2 * B * M; ab.dA_out = dAbuf[(L - i) & 1];
       ab.acc_v = acc_v; ab.acc_Wh = acc_Wh; ab.acc_filt = acc_filt;
       ab.B = B; ab.Tp = Tp; ab.M = M; ab.E = E; ab.K = K; ab.n = n;
-      ab.e_cur = E_all ? E_all + (size_t)i * B * Tp : nullptr; ab.acc_b = acc_b;
+      ab.e_cur = d.E_all ? d.E_all + (size_t)i * B * Tp : nullptr; ab.acc_b = acc_b;
       {
         ProfScope prof_ab("att_bwd", st);
         att_bwd<<<nct, AB_NT, ab_smem, st>>>(ab, tc_cap);
@@ -375,41 +367,38 @@ int forward_backward(lvsr_model* m, const float* x, const float* mask, const int
       const float* q0 = dQp + (size_t)i * 2 * B * M;
       if (int rc = skinny(q0, M, M, WsT, q0 + (size_t)B * M, M, M, WsT, dspart, C, dS_ro + (size_t)i * B * C, C, ds_next, C, B, C, st)) return rc;
     }
+    // dsbuf[L & 1]: gradient of the broadcast initial state, per row
+    if (int rc = colsum(dsbuf[L & 1], B, C, C, grad(t + "/transition.initial_state"), false, st)) return rc;
+    out = {dG, HR, dCTX, dQp, dP, acc_v, acc_Wh, acc_filt, acc_b};
+    return 0;
   }
-  const float* ds_init = dsbuf[L & 1];                    // gradient of the broadcast initial state, per row
-  if (int rc = colsum(ds_init, B, C, C, grad_of(m, grads, t + "/transition.initial_state"), false, st)) return rc;
-
-  // ---- decoder weight gradients: large GEMMs over all steps -----------------------------------
-  {
+  // Decoder weight gradients: large GEMMs over all steps, the feedback fork, and the sums of the attention constants
+  int decoder_weight_grads(const DecTape& d, const DecGrads& dg) const {
     // state_to_state = HR^T dA ; state_to_gates = S_prev^T [dGz|dGr] ; distribute = CTX^T dG (gate columns first in Wd_cat)
-    if (int rc = gemm_tn(ws, HR, C, dG + 2 * C, 3 * C, R, C, C, grad_of(m, grads, t + "/transition.state_to_state"), C, false, st)) return rc;
-    if (int rc = gemm_tn(ws, S_prev, C, dG, 3 * C, R, C, 2 * C, grad_of(m, grads, t + "/transition.state_to_gates"), 2 * C, false, st)) return rc;
-    if (int rc = gemm_tn(ws, CTX, E, dG, 3 * C, R, E, 2 * C, grad_of(m, grads, t + "/distribute/fork_gate_inputs.W"), 2 * C, false, st)) return rc;
-    if (int rc = gemm_tn(ws, CTX, E, dG + 2 * C, 3 * C, R, E, C, grad_of(m, grads, t + "/distribute/fork_inputs.W"), C, false, st)) return rc;
+    if (int rc = gemm_tn(ws, dg.HR, C, dg.dG + 2 * C, 3 * C, R, C, C, grad(t + "/transition.state_to_state"), C, false, st)) return rc;
+    if (int rc = gemm_tn(ws, d.S_prev, C, dg.dG, 3 * C, R, C, 2 * C, grad(t + "/transition.state_to_gates"), 2 * C, false, st)) return rc;
+    if (int rc = gemm_tn(ws, d.CTX, E, dg.dG, 3 * C, R, E, 2 * C, grad(t + "/distribute/fork_gate_inputs.W"), 2 * C, false, st)) return rc;
+    if (int rc = gemm_tn(ws, d.CTX, E, dg.dG + 2 * C, 3 * C, R, E, C, grad(t + "/distribute/fork_inputs.W"), C, false, st)) return rc;
     // state transformer: S_prev^T dQ (two partials)
-    float* gWs = grad_of(m, grads, at + "/state_trans/transform_states.W");
     {
       // dQp is [L][2][B][M]: view partial p as rows of length M with stride 2*B*M per step -> gather into [R, M] first
-      const size_t mark = ws.off;
+      ArenaMark mark{ws};
       float* dQ = ws.f32((size_t)R * M);
       LVSR_CHECK(dQ, "out of device memory");
       for (int p = 0; p < 2; ++p) {
         // rows of step i live at dQp + (i*2 + p)*B*M: a 2-D copy with pitch 2*B*M
-        LVSR_CUDA_OK(cudaMemcpy2DAsync(dQ, (size_t)B * M * sizeof(float), dQp + (size_t)p * B * M, (size_t)2 * B * M * sizeof(float),
-                                       (size_t)B * M * sizeof(float), L, cudaMemcpyDeviceToDevice, st));
-        if (int rc = gemm_tn(ws, S_prev, C, dQ, M, R, C, M, gWs, M, p == 1, st)) return rc;
+        if (int rc = copy2d(dQ, B * M, dg.dQp + (size_t)p * B * M, 2 * B * M, L, B * M, st)) return rc;
+        if (int rc = gemm_tn(ws, d.S_prev, C, dQ, M, R, C, M, grad(at + "/state_trans/transform_states.W"), M, p == 1, st)) return rc;
       }
-      if (ws.off <= ws.cap) ws.off = mark;
     }
-    // fork(feedback(y)): dFF by label, then lookup / fork weights / biases
-    const size_t mark = ws.off;
+    // fork(feedback(y)): dFF by label, then lookup / fork weights / biases; the scratch is rewound when the phase returns
+    ArenaMark mark{ws};
     float* dFF = ws.f32((size_t)(V + 1) * 3 * C);
     float* WffT = ws.f32((size_t)3 * C * Cfb);
-    float* dlook = ws.f32((size_t)(V + 1) * Cfb);
     float* dWff = ws.f32((size_t)Cfb * 3 * C);
     float* dbff = ws.f32((size_t)3 * C);
-    LVSR_CHECK(dFF && WffT && dlook && dWff && dbff, "out of device memory (feedback gradients)");
-    scatter_rows_kernel<<<V + 1, 256, 0, st>>>(dG, lab, R, 3 * C, dFF);
+    LVSR_CHECK(dFF && WffT && dWff && dbff, "out of device memory (feedback gradients)");
+    scatter_rows_kernel<<<V + 1, 256, 0, st>>>(dg.dG, lab, R, 3 * C, dFF);
     LVSR_LAUNCH_CHECK();
     if (c.one_of_n_feedback) {
       // FF[y] = W_fork[y, :] + b: the gradient of the fork weights IS dFF
@@ -417,135 +406,138 @@ int forward_backward(lvsr_model* m, const float* x, const float* mask, const int
     } else {
       if (int rc = transpose(m->Wff_cat, WffT, Cfb, 3 * C, st)) return rc;
       const float* look = m->P(g + "/readout/lookupfeedback/lookuptable.W");
-      if (int rc = gemm_nn(dFF, V + 1, 3 * C, 3 * C, WffT, Cfb, Cfb, nullptr, grad_of(m, grads, g + "/readout/lookupfeedback/lookuptable.W"), Cfb, false, st)) return rc;
+      if (int rc = gemm_nn(dFF, V + 1, 3 * C, 3 * C, WffT, Cfb, Cfb, nullptr, grad(g + "/readout/lookupfeedback/lookuptable.W"), Cfb, false, st)) return rc;
       if (int rc = gemm_tn(ws, look, Cfb, dFF, 3 * C, V + 1, Cfb, 3 * C, dWff, 3 * C, false, st)) return rc;
     }
     if (int rc = colsum(dFF, V + 1, 3 * C, 3 * C, dbff, false, st)) return rc;
-    // Wff_cat columns: [gate_inputs 2C | inputs C]
-    if (int rc = copy2d(grad_of(m, grads, g + "/fork/fork_gate_inputs.W"), 2 * C, dWff, 3 * C, Cfb, 2 * C, st)) return rc;
-    if (int rc = copy2d(grad_of(m, grads, g + "/fork/fork_inputs.W"), C, dWff + 2 * C, 3 * C, Cfb, C, st)) return rc;
-    if (int rc = copy2d(grad_of(m, grads, g + "/fork/fork_gate_inputs.b"), 2 * C, dbff, 3 * C, 1, 2 * C, st)) return rc;
-    if (int rc = copy2d(grad_of(m, grads, g + "/fork/fork_inputs.b"), C, dbff + 2 * C, 3 * C, 1, C, st)) return rc;
-    (void)dlook;
-    if (ws.off <= ws.cap) ws.off = mark;
+    if (int rc = fork_copy(m, feedback_fork(c), dWff, dbff, grads, st)) return rc;
     // attention constants: sums of the per-CTA partials
-    reduce_partials_kernel<<<grid1d(M), 256, 0, st>>>(acc_v, nct, M, grad_of(m, grads, at + "/energy_comp/linear.W"));
+    reduce_partials_kernel<<<grid1d(M), 256, 0, st>>>(dg.acc_v, nct, M, grad(at + "/energy_comp/linear.W"));
     LVSR_LAUNCH_CHECK();
     if (!content) {
-      reduce_partials_kernel<<<grid1d((long long)K * M), 256, 0, st>>>(acc_Wh, nct, (long long)K * M, grad_of(m, grads, at + "/handler.W"));
+      reduce_partials_kernel<<<grid1d((long long)K * M), 256, 0, st>>>(dg.acc_Wh, nct, (long long)K * M, grad(at + "/handler.W"));
       LVSR_LAUNCH_CHECK();
-      reduce_partials_kernel<<<grid1d((long long)K * w), 256, 0, st>>>(acc_filt, nct, (long long)K * w, grad_of(m, grads, at + "/conv1d.filters"));
-      LVSR_LAUNCH_CHECK();
-    }
-    if (acc_b) {
-      reduce_partials_kernel<<<1, 256, 0, st>>>(acc_b, nct, 1, grad_of(m, grads, at + "/energy_comp/linear.b"));
+      reduce_partials_kernel<<<grid1d((long long)K * w), 256, 0, st>>>(dg.acc_filt, nct, (long long)K * w, grad(at + "/conv1d.filters"));
       LVSR_LAUNCH_CHECK();
     }
+    if (dg.acc_b) {
+      reduce_partials_kernel<<<1, 256, 0, st>>>(dg.acc_b, nct, 1, grad(at + "/energy_comp/linear.b"));
+      LVSR_LAUNCH_CHECK();
+    }
+    return 0;
   }
-  // ---- gradient of the attended sequence: glimpses + preprocess --------------------------------
-  float* dH = ws.f32((size_t)Tp * B * E);
-  LVSR_CHECK(dH, "out of device memory (dH)");
-  {
+  // Gradient of the attended sequence (dH) through the glimpses and the preprocess, with the preprocess's gradients
+  int attended_grad(const DecTape& d, const DecGrads& dg, const float* WpT, float*& dH) const {
+    dH = ws.f32((size_t)Tp * B * E);
+    LVSR_CHECK(dH, "out of device memory (dH)");
     dim3 grid(ceil_div(Tp, 8), B);
-    dh_from_ctx_kernel<<<grid, 256, 0, st>>>(W_all, dCTX, L, B, Tp, E, dH, 0);
+    dh_from_ctx_kernel<<<grid, 256, 0, st>>>(d.W_all, dg.dCTX, L, B, Tp, E, dH, 0);
     LVSR_LAUNCH_CHECK();
-    if (int rc = gemm_nn(dP, Tp * B, M, M, WpT, E, E, nullptr, dH, E, true, st)) return rc;
-    if (int rc = gemm_tn(ws, Hatt, E, dP, M, Tp * B, E, M, grad_of(m, grads, at + "/preprocess.W"), M, false, st)) return rc;
-    if (int rc = colsum(dP, Tp * B, M, M, grad_of(m, grads, at + "/preprocess.b"), false, st)) return rc;
+    if (int rc = gemm_nn(dg.dP, Tp * B, M, M, WpT, E, E, nullptr, dH, E, true, st)) return rc;
+    if (int rc = gemm_tn(ws, d.Hatt, E, dg.dP, M, Tp * B, E, M, grad(at + "/preprocess.W"), M, false, st)) return rc;
+    if (int rc = colsum(dg.dP, Tp * B, M, M, grad(at + "/preprocess.b"), false, st)) return rc;
+    return 0;
   }
-
-  // ---- encoder: reverse-time scans and their GEMMs, top layer first ----------------------------
-  const float* dout = dH;
-  for (int l = c.num_layers - 1; l >= 0; --l) {
-    LayerTape& tp = tape[l];
-    const int D = tp.D, rows = tp.T * B;
-    float* hr = ws.f32((size_t)rows * 2 * D);
-    float* dh0 = ws.f32((size_t)2 * B * D);
-    LVSR_CHECK(hr && dh0, "out of device memory (encoder backward)");
-    BiGruBwdArgs a = {};
-    a.tape = tp.pre; a.hext = tp.hext; a.mask = mask; a.mask_tstride = tp.mstride; a.dout = dout;
-    const std::string bf = enc_base(l, 0), bb = enc_base(l, 1);
-    a.Wg_f = m->P(bf + "/gatedrecurrent.state_to_gates"); a.Ws_f = m->P(bf + "/gatedrecurrent.state_to_state");
-    a.Wg_b = m->P(bb + "/gatedrecurrent.state_to_gates"); a.Ws_b = m->P(bb + "/gatedrecurrent.state_to_state");
-    a.hr_out = hr; a.dh0 = dh0; a.T = tp.T; a.B = B; a.D = D; a.subsample = tp.k;
-    int32_t* plan = m->enc_plan[l];
-    int bwd_cs = 0, wsplits = 0;
-    if (int rc = bigru_layer_backward(a, st, &bwd_cs)) return rc;
-    plan[LVSR_ENC_BWD_CS] = bwd_cs;
-    // fork: dWcat = X^T dPre, dbcat = colsum(dPre); columns per direction [inputs D | gate_inputs 2D]
-    {
-      const size_t mark = ws.off;
-      float* dWcat = ws.f32((size_t)tp.Din * 6 * D);
-      float* dbcat = ws.f32((size_t)6 * D);
-      LVSR_CHECK(dWcat && dbcat, "out of device memory (fork gradients)");
-      // tensor-core path: every operand transposed once into K-major tf32 hi/lo pairs (the contraction runs over the
-      // T*B rows), then five split-K tensor-core products share them; FFMA tiles for small problems / LVSR_NO_TC_GEMM
-      const bool tc = m->use_tc && rows >= 2048 && D % 128 == 0;
-      TcOperand dPreT, XT, hrT, hpT[2];
-      if (tc) {
-        if (int rc = make_tc_operand(ws, tp.pre, rows, 6 * D, 6 * D, &dPreT, st)) return rc;
-        if (int rc = make_tc_operand(ws, tp.X, rows, tp.Din, tp.Din, &XT, st)) return rc;
-        if (int rc = make_tc_operand(ws, hr, rows, 2 * D, 2 * D, &hrT, st)) return rc;
-        for (int dir = 0; dir < 2; ++dir) {
-          const float* hprev = tp.hext + (size_t)(dir ? 2 : 0) * B * 2 * D + dir * D;
-          if (int rc = make_tc_operand(ws, hprev, rows, D, 2 * D, &hpT[dir], st)) return rc;
-        }
-        if (int rc = gemm_tn_tc(ws, XT, 0, tp.Din, dPreT, 0, 6 * D, dWcat, 6 * D, false, st, &wsplits)) return rc;
-      } else {
-        if (int rc = gemm_tn(ws, tp.X, tp.Din, tp.pre, 6 * D, rows, tp.Din, 6 * D, dWcat, 6 * D, false, st, &wsplits)) return rc;
-      }
-      plan[LVSR_ENC_WGRAD] = tc ? LVSR_ENC_PATH_TC : LVSR_ENC_PATH_FFMA;
-      plan[LVSR_ENC_WGRAD_SPLITS] = wsplits;
-      plan[LVSR_ENC_WGRAD_KPAD] = tc ? dPreT.Kpad : 0;
-      if (int rc = colsum(tp.pre, rows, 6 * D, 6 * D, dbcat, false, st)) return rc;
-      for (int dir = 0; dir < 2; ++dir) {
-        const std::string b = enc_base(l, dir);
-        const int c0 = dir * 3 * D;
-        if (int rc = copy2d(grad_of(m, grads, b + "/fork/fork_inputs.W"), D, dWcat + c0, 6 * D, tp.Din, D, st)) return rc;
-        if (int rc = copy2d(grad_of(m, grads, b + "/fork/fork_gate_inputs.W"), 2 * D, dWcat + c0 + D, 6 * D, tp.Din, 2 * D, st)) return rc;
-        if (int rc = copy2d(grad_of(m, grads, b + "/fork/fork_inputs.b"), D, dbcat + c0, 6 * D, 1, D, st)) return rc;
-        if (int rc = copy2d(grad_of(m, grads, b + "/fork/fork_gate_inputs.b"), 2 * D, dbcat + c0 + D, 6 * D, 1, 2 * D, st)) return rc;
-        // recurrent weights: state_to_state = (h*r)^T dA ; state_to_gates = H_prev^T [dGz|dGr]
-        float* gWs = grad_of(m, grads, b + "/gatedrecurrent.state_to_state");
-        float* gWg = grad_of(m, grads, b + "/gatedrecurrent.state_to_gates");
+  // Encoder backward, top layer first: scan, weight and input gradients; plan slots LVSR_ENC_BWD_CS .. LVSR_ENC_DX
+  int encoder_backward(const LayerTape* tape, const float* mask, const float* dH) const {
+    const float* dout = dH;
+    for (int l = c.num_layers - 1; l >= 0; --l) {
+      const LayerTape& tp = tape[l];
+      const int D = tp.D, rows = tp.T * B;
+      float* hr = ws.f32((size_t)rows * 2 * D);
+      float* dh0 = ws.f32((size_t)2 * B * D);
+      LVSR_CHECK(hr && dh0, "out of device memory (encoder backward)");
+      BiGruBwdArgs a = {};
+      a.tape = tp.pre; a.hext = tp.hext; a.mask = mask; a.mask_tstride = tp.mstride; a.dout = dout;
+      const std::string bf = enc_base(l, 0), bb = enc_base(l, 1);
+      a.Wg_f = m->P(bf + "/gatedrecurrent.state_to_gates"); a.Ws_f = m->P(bf + "/gatedrecurrent.state_to_state");
+      a.Wg_b = m->P(bb + "/gatedrecurrent.state_to_gates"); a.Ws_b = m->P(bb + "/gatedrecurrent.state_to_state");
+      a.hr_out = hr; a.dh0 = dh0; a.T = tp.T; a.B = B; a.D = D; a.subsample = tp.k;
+      int32_t* plan = m->enc_plan[l];
+      int bwd_cs = 0, wsplits = 0;
+      if (int rc = bigru_layer_backward(a, st, &bwd_cs)) return rc;
+      plan[LVSR_ENC_BWD_CS] = bwd_cs;
+      // fork: dWcat = X^T dPre, dbcat = colsum(dPre), scattered to the parameters by the layer's fork layout
+      {
+        ArenaMark mark{ws};
+        float* dWcat = ws.f32((size_t)tp.Din * 6 * D);
+        float* dbcat = ws.f32((size_t)6 * D);
+        LVSR_CHECK(dWcat && dbcat, "out of device memory (fork gradients)");
+        // tensor-core path: every operand transposed once into K-major tf32 hi/lo pairs (the contraction runs over the
+        // T*B rows), then five split-K tensor-core products share them; FFMA tiles for small problems / LVSR_NO_TC_GEMM
+        const bool tc = m->use_tc && rows >= 2048 && D % 128 == 0;
+        // H_prev of each direction: slot t (forward) / t+2 (backward) of hext
+        const float* hprev[2] = {tp.hext, tp.hext + (size_t)2 * B * 2 * D + D};
+        TcOperand dPreT, XT, hrT, hpT[2];
         if (tc) {
-          if (int rc = gemm_tn_tc(ws, hrT, dir * D, D, dPreT, c0, D, gWs, D, false, st)) return rc;
-          if (int rc = gemm_tn_tc(ws, hpT[dir], 0, D, dPreT, c0 + D, 2 * D, gWg, 2 * D, false, st)) return rc;
+          if (int rc = make_tc_operand(ws, tp.pre, rows, 6 * D, 6 * D, &dPreT, st)) return rc;
+          if (int rc = make_tc_operand(ws, tp.X, rows, tp.Din, tp.Din, &XT, st)) return rc;
+          if (int rc = make_tc_operand(ws, hr, rows, 2 * D, 2 * D, &hrT, st)) return rc;
+          for (int dir = 0; dir < 2; ++dir)
+            if (int rc = make_tc_operand(ws, hprev[dir], rows, D, 2 * D, &hpT[dir], st)) return rc;
+          if (int rc = gemm_tn_tc(ws, XT, 0, tp.Din, dPreT, 0, 6 * D, dWcat, 6 * D, false, st, &wsplits)) return rc;
         } else {
-          if (int rc = gemm_tn(ws, hr + dir * D, 2 * D, tp.pre + c0, 6 * D, rows, D, D, gWs, D, false, st)) return rc;
-          const float* hprev = tp.hext + (size_t)(dir ? 2 : 0) * B * 2 * D + dir * D;     // slot t (forward) / t+2 (backward)
-          if (int rc = gemm_tn(ws, hprev, 2 * D, tp.pre + c0 + D, 6 * D, rows, D, 2 * D, gWg, 2 * D, false, st)) return rc;
+          if (int rc = gemm_tn(ws, tp.X, tp.Din, tp.pre, 6 * D, rows, tp.Din, 6 * D, dWcat, 6 * D, false, st, &wsplits)) return rc;
         }
-        if (int rc = colsum(dh0 + (size_t)dir * B * D, B, D, D, grad_of(m, grads, b + "/gatedrecurrent.initial_state"), false, st)) return rc;
+        plan[LVSR_ENC_WGRAD] = tc ? LVSR_ENC_PATH_TC : LVSR_ENC_PATH_FFMA;
+        plan[LVSR_ENC_WGRAD_SPLITS] = wsplits;
+        plan[LVSR_ENC_WGRAD_KPAD] = tc ? dPreT.Kpad : 0;
+        if (int rc = colsum(tp.pre, rows, 6 * D, 6 * D, dbcat, false, st)) return rc;
+        for (int dir = 0; dir < 2; ++dir) {
+          const std::string b = enc_base(l, dir);
+          const ForkLayout f = encoder_fork(c, l, dir);
+          const int cA = f.block[0].col, cG = f.block[1].col;      // columns of dA (fork_inputs) and [dGz|dGr]
+          if (int rc = fork_copy(m, f, dWcat, dbcat, grads, st)) return rc;
+          // recurrent weights: state_to_state = (h*r)^T dA ; state_to_gates = H_prev^T [dGz|dGr]
+          float* gWs = grad(b + "/gatedrecurrent.state_to_state");
+          float* gWg = grad(b + "/gatedrecurrent.state_to_gates");
+          if (tc) {
+            if (int rc = gemm_tn_tc(ws, hrT, dir * D, D, dPreT, cA, D, gWs, D, false, st)) return rc;
+            if (int rc = gemm_tn_tc(ws, hpT[dir], 0, D, dPreT, cG, 2 * D, gWg, 2 * D, false, st)) return rc;
+          } else {
+            if (int rc = gemm_tn(ws, hr + dir * D, 2 * D, tp.pre + cA, 6 * D, rows, D, D, gWs, D, false, st)) return rc;
+            if (int rc = gemm_tn(ws, hprev[dir], 2 * D, tp.pre + cG, 6 * D, rows, D, 2 * D, gWg, 2 * D, false, st)) return rc;
+          }
+          if (int rc = colsum(dh0 + (size_t)dir * B * D, B, D, D, grad(b + "/gatedrecurrent.initial_state"), false, st)) return rc;
+        }
       }
-      if (ws.off <= ws.cap) ws.off = mark;
-    }
-    // gradient of the layer input = gradient of the (subsampled) output of the layer below
-    if (l > 0) {
-      float* dX = ws.f32((size_t)rows * tp.Din);
-      float* WcatT = ws.f32((size_t)6 * D * tp.Din);
-      LVSR_CHECK(dX && WcatT, "out of device memory (dX)");
-      if (m->use_tc && gemm_tc_supported(rows, tp.Din, 6 * D) && (6 * D) % 32 == 0) {
-        // dX = dPre . Wcat^T: the K-major form of the right-hand side [N = Din, K = 6D] is Wcat itself
-        const size_t mark = ws.off;
-        float* a_hi = ws.f32((size_t)rows * 6 * D);
-        float* a_lo = ws.f32((size_t)rows * 6 * D);
-        float* w_hi = ws.f32((size_t)tp.Din * 6 * D);
-        float* w_lo = ws.f32((size_t)tp.Din * 6 * D);
-        LVSR_CHECK(a_hi && a_lo && w_hi && w_lo, "out of device memory (dX operands)");
-        if (int rc = split_tf32(m->Wcat[l], w_hi, w_lo, (long long)tp.Din * 6 * D, st)) return rc;
-        if (int rc = gemm_tc(tp.pre, a_hi, a_lo, rows, 6 * D, w_hi, w_lo, tp.Din, nullptr, dX, tp.Din, st)) return rc;
-        if (ws.off <= ws.cap) ws.off = mark;
-        plan[LVSR_ENC_DX] = LVSR_ENC_PATH_TC;
-      } else {
-        if (int rc = transpose(m->Wcat[l], WcatT, tp.Din, 6 * D, st)) return rc;
-        if (int rc = gemm_nn(tp.pre, rows, 6 * D, 6 * D, WcatT, tp.Din, tp.Din, nullptr, dX, tp.Din, false, st)) return rc;
-        plan[LVSR_ENC_DX] = LVSR_ENC_PATH_FFMA;
+      // gradient of the layer input = gradient of the (subsampled) output of the layer below
+      if (l > 0) {
+        float* dX = ws.f32((size_t)rows * tp.Din);
+        LVSR_CHECK(dX, "out of device memory (dX)");
+        if (m->use_tc && gemm_tc_supported(rows, tp.Din, 6 * D) && (6 * D) % 32 == 0) {
+          // dX = dPre . Wcat^T: the K-major form of the right-hand side [N = Din, K = 6D] is Wcat itself
+          ArenaMark mark{ws};
+          float* a_hi = ws.f32((size_t)rows * 6 * D);
+          float* a_lo = ws.f32((size_t)rows * 6 * D);
+          float* w_hi = ws.f32((size_t)tp.Din * 6 * D);
+          float* w_lo = ws.f32((size_t)tp.Din * 6 * D);
+          LVSR_CHECK(a_hi && a_lo && w_hi && w_lo, "out of device memory (dX operands)");
+          if (int rc = split_tf32(m->Wcat[l], w_hi, w_lo, (long long)tp.Din * 6 * D, st)) return rc;
+          if (int rc = gemm_tc(tp.pre, a_hi, a_lo, rows, 6 * D, w_hi, w_lo, tp.Din, nullptr, dX, tp.Din, st)) return rc;
+          plan[LVSR_ENC_DX] = LVSR_ENC_PATH_TC;
+        } else {
+          float* WcatT = ws.f32((size_t)6 * D * tp.Din);
+          LVSR_CHECK(WcatT, "out of device memory (dX)");
+          if (int rc = transpose(m->Wcat[l], WcatT, tp.Din, 6 * D, st)) return rc;
+          if (int rc = gemm_nn(tp.pre, rows, 6 * D, 6 * D, WcatT, tp.Din, tp.Din, nullptr, dX, tp.Din, false, st)) return rc;
+          plan[LVSR_ENC_DX] = LVSR_ENC_PATH_FFMA;
+        }
+        dout = dX;
       }
-      dout = dX;
     }
+    return 0;
   }
-  return 0;
+};
+
+// forward + backward of one batch on the parameters Param::dev points at and the weights packed from them
+int forward_backward(lvsr_model* m, const float* x, const float* mask, const int64_t* labels, const float* lmask,
+                     int32_t T, int32_t B, int32_t L, float gscale, float* cost_out, float* grads, void* stream) {
+  if (int rc = check_ready(m)) return rc;
+  LVSR_CHECK(x && labels && cost_out && grads && T > 0 && B > 0 && L > 0, "train_cost_and_grads: bad arguments");
+  LVSR_CHECK(!lm_attached(m), "train_cost_and_grads: shallow fusion is inference only (detach the language model)");
+  return TrainStep{m, static_cast<cudaStream_t>(stream), labels, lmask, grads, gscale, B, L, lvsr_encoded_length(m, T)}
+      .run(x, mask, T, cost_out);
 }
 
 }  // namespace
