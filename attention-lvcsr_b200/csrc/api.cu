@@ -244,7 +244,7 @@ static int lm_sync_status(lvsr_model* m, cudaStream_t st) {
   unsigned h = 0;
   LVSR_CUDA_OK(cudaMemcpyAsync(&h, m->lm_status, sizeof(h), cudaMemcpyDeviceToHost, st));
   LVSR_CUDA_OK(cudaStreamSynchronize(st));
-  if (h) LVSR_CUDA_OK(cudaMemset(m->lm_status, 0, sizeof(unsigned)));
+  if (h) LVSR_CUDA_OK(cudaMemsetAsync(m->lm_status, 0, sizeof(unsigned), st));
   return lm_report(h);
 }
 
@@ -375,6 +375,7 @@ int lvsr_model_create(const lvsr_config* cfg, lvsr_model** out) {
     return set_error("cudaMalloc(status) failed");
   }
   cudaMemset(m->status, 0, 64);
+  cudaDeviceSynchronize();      // the zeroed buffers are in place before a call on any stream reads them
   *out = m;
   return 0;
 }
@@ -413,7 +414,7 @@ int lvsr_model_status(lvsr_model* m, int32_t* launch_status, int64_t* stepwise_f
   DeviceGuard device_guard(m);
   LVSR_CHECK(m && launch_status, "null argument");
   unsigned hst = 0;
-  LVSR_CUDA_OK(cudaMemcpy(&hst, m->status, sizeof(hst), cudaMemcpyDeviceToHost));   // synchronises with the device
+  if (int rc = copy_on_handle(m, &hst, m->status, sizeof(hst), cudaMemcpyDeviceToHost)) return rc;   // after the handle's work
   *launch_status = (int32_t)hst;
   if (stepwise_fallbacks) *stepwise_fallbacks = m->dec_fallbacks;
   return 0;
@@ -494,7 +495,7 @@ int lvsr_model_set_param(lvsr_model* m, const char* name, const float* host, int
   const Param* p = m->param(name);
   LVSR_CHECK(p, "unknown parameter '%s'", name);
   LVSR_CHECK(count == p->count, "parameter '%s' expects %lld values, got %lld", name, (long long)p->count, (long long)count);
-  LVSR_CUDA_OK(cudaMemcpy(p->dev, host, (size_t)count * sizeof(float), cudaMemcpyHostToDevice));
+  if (int rc = copy_on_handle(m, p->dev, host, (size_t)count * sizeof(float), cudaMemcpyHostToDevice)) return rc;
   m->finalized = false;
   return 0;
 }
@@ -504,14 +505,14 @@ int lvsr_model_get_param(const lvsr_model* m, const char* name, float* host, int
   const Param* p = m->param(name);
   LVSR_CHECK(p, "unknown parameter '%s'", name);
   LVSR_CHECK(count == p->count, "parameter '%s' holds %lld values, asked for %lld", name, (long long)p->count, (long long)count);
-  LVSR_CUDA_OK(cudaMemcpy(host, p->dev, (size_t)count * sizeof(float), cudaMemcpyDeviceToHost));
+  if (int rc = copy_on_handle(m, host, p->dev, (size_t)count * sizeof(float), cudaMemcpyDeviceToHost)) return rc;
   return 0;
 }
 
 int lvsr_model_finalize(lvsr_model* m) {
   DeviceGuard device_guard(m);
   LVSR_CHECK(m, "null model");
-  return finalize_on_stream(m, 0, true);
+  return finalize_on_stream(m, m->stream, true);      // after the work queued on the handle
 }
 
 int lvsr_model_clear_lm(lvsr_model* m) {
@@ -546,17 +547,20 @@ int lvsr_model_set_lm(lvsr_model* m, int32_t num_states, int32_t start, const in
   if (int rc = lvsr_model_clear_lm(m)) return rc;
   const size_t na = (size_t)std::max<int64_t>(num_arcs, 1);
   LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->lm_status), sizeof(unsigned)));
-  LVSR_CUDA_OK(cudaMemset(m->lm_status, 0, sizeof(unsigned)));
   LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->lm_off), (size_t)(num_states + 1) * sizeof(long long)));
   LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->lm_label), na * sizeof(int)));
   LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->lm_next), na * sizeof(int)));
   LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->lm_weight), na * sizeof(float)));
-  LVSR_CUDA_OK(cudaMemcpy(m->lm_off, off, (size_t)(num_states + 1) * sizeof(long long), cudaMemcpyHostToDevice));
+  // on the handle's stream, complete before the host tables may go away
+  cudaStream_t st = m->stream;
+  LVSR_CUDA_OK(cudaMemsetAsync(m->lm_status, 0, sizeof(unsigned), st));
+  LVSR_CUDA_OK(cudaMemcpyAsync(m->lm_off, off, (size_t)(num_states + 1) * sizeof(long long), cudaMemcpyHostToDevice, st));
   if (num_arcs > 0) {
-    LVSR_CUDA_OK(cudaMemcpy(m->lm_label, label, (size_t)num_arcs * sizeof(int), cudaMemcpyHostToDevice));
-    LVSR_CUDA_OK(cudaMemcpy(m->lm_next, next, (size_t)num_arcs * sizeof(int), cudaMemcpyHostToDevice));
-    LVSR_CUDA_OK(cudaMemcpy(m->lm_weight, weight, (size_t)num_arcs * sizeof(float), cudaMemcpyHostToDevice));
+    LVSR_CUDA_OK(cudaMemcpyAsync(m->lm_label, label, (size_t)num_arcs * sizeof(int), cudaMemcpyHostToDevice, st));
+    LVSR_CUDA_OK(cudaMemcpyAsync(m->lm_next, next, (size_t)num_arcs * sizeof(int), cudaMemcpyHostToDevice, st));
+    LVSR_CUDA_OK(cudaMemcpyAsync(m->lm_weight, weight, (size_t)num_arcs * sizeof(float), cudaMemcpyHostToDevice, st));
   }
+  LVSR_CUDA_OK(cudaStreamSynchronize(st));
   m->lm_start = start;
   m->lm_fusion = *fusion;
   return 0;
@@ -567,6 +571,7 @@ int lvsr_lm_initial_states(lvsr_model* m, int32_t R, int32_t* states, double* we
   LVSR_CHECK(m && lm_attached(m), "lm_initial_states: no language model attached");
   LVSR_CHECK(states && weights && add && R > 0, "lm_initial_states: bad arguments");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (int rc = bind_stream(m, st)) return rc;
   if (int rc = lm_step(lm_fst(m), R, nullptr, nullptr, nullptr, nullptr, states, weights, add, st)) return rc;
   return lm_sync_status(m, st);
 }
@@ -578,6 +583,7 @@ int lvsr_lm_next_states(lvsr_model* m, int32_t R, const int32_t* states, const d
   LVSR_CHECK(states && weights && outputs && next_states && next_weights && next_add && R > 0,
              "lm_next_states: bad arguments");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (int rc = bind_stream(m, st)) return rc;
   if (int rc = lm_step(lm_fst(m), R, states, weights, nullptr, reinterpret_cast<const long long*>(outputs), next_states,
                        next_weights, next_add, st)) return rc;
   return lm_sync_status(m, st);
@@ -660,9 +666,12 @@ int finalize_on_stream(lvsr_model* m, cudaStream_t st, bool synchronise) {
     if (int rc = gemm_bias(ff, st)) return rc;
   }
   m->v_bias = 0.f;
-  if (c.energy_normalizer != LVSR_NORM_SOFTMAX)
-    LVSR_CUDA_OK(cudaMemcpy(&m->v_bias, m->P(att_base(m) + "/energy_comp/linear.b"), sizeof(float),
-                            cudaMemcpyDeviceToHost));
+  if (c.energy_normalizer != LVSR_NORM_SOFTMAX) {
+    // a kernel argument: read in st's order (after an update enqueued there), so the host waits for st
+    LVSR_CUDA_OK(cudaMemcpyAsync(&m->v_bias, m->P(att_base(m) + "/energy_comp/linear.b"), sizeof(float),
+                                 cudaMemcpyDeviceToHost, st));
+    LVSR_CUDA_OK(cudaStreamSynchronize(st));
+  }
   if (synchronise) LVSR_CUDA_OK(cudaStreamSynchronize(st));
   m->finalized = true;
   return 0;
@@ -854,6 +863,7 @@ int lvsr_encoded_dim(const lvsr_model* m) { return m ? m->E : 0; }
 int lvsr_encoder_forward(lvsr_model* m, const float* x, const float* mask, int32_t T, int32_t B,
                          float* attended, float* attended_mask, void* stream) {
   DeviceGuard device_guard(m);
+  if (int rc = bind_stream(m, static_cast<cudaStream_t>(stream))) return rc;
   if (int rc = check_ready(m)) return rc;
   LVSR_CHECK(x && attended && attended_mask && T > 0 && B > 0, "encoder_forward: bad arguments");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -864,6 +874,7 @@ int lvsr_encoder_forward(lvsr_model* m, const float* x, const float* mask, int32
 
 int lvsr_preprocess(lvsr_model* m, const float* attended, int32_t Tp, int32_t U, float* out, void* stream) {
   DeviceGuard device_guard(m);
+  if (int rc = bind_stream(m, static_cast<cudaStream_t>(stream))) return rc;
   if (int rc = check_ready(m)) return rc;
   LVSR_CHECK(attended && out && Tp > 0 && U > 0, "preprocess: bad arguments");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -884,6 +895,7 @@ int lvsr_cost_matrix(lvsr_model* m, const float* attended, const float* attended
                      const int64_t* labels, const float* labels_mask, int32_t L, float* costs,
                      float* weights_out, float* energies_out, float* states_out, float* wavg_out, void* stream) {
   DeviceGuard device_guard(m);
+  if (int rc = bind_stream(m, static_cast<cudaStream_t>(stream))) return rc;
   if (int rc = check_ready(m)) return rc;
   LVSR_CHECK(attended && attended_mask && labels && costs && Tp > 0 && B > 0 && L > 0, "cost_matrix: bad arguments");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1084,6 +1096,7 @@ int lvsr_cost_matrix(lvsr_model* m, const float* attended, const float* attended
 int lvsr_initial_states(lvsr_model* m, int32_t Tp, int32_t R, float* states, int64_t* outputs, float* wavg,
                         float* weights, float* energies, int64_t* step, void* stream) {
   DeviceGuard device_guard(m);
+  if (int rc = bind_stream(m, static_cast<cudaStream_t>(stream))) return rc;
   if (int rc = check_ready(m)) return rc;
   LVSR_CHECK(states && outputs && wavg && weights && energies && step && Tp > 0 && R > 0, "initial_states: bad arguments");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1105,6 +1118,7 @@ int lvsr_logprobs(lvsr_model* m, const float* attended, const float* preprocesse
                   int32_t Tp, int32_t U, const int32_t* row_utt, int32_t R, const float* states,
                   const float* weights, const int64_t* step, float* out, void* stream) {
   DeviceGuard device_guard(m);
+  if (int rc = bind_stream(m, static_cast<cudaStream_t>(stream))) return rc;
   if (int rc = check_ready(m)) return rc;
   LVSR_CHECK(attended && attended_mask && states && weights && step && out && Tp > 0 && U > 0 && R > 0,
              "logprobs: bad arguments");
@@ -1138,6 +1152,7 @@ int lvsr_next_states(lvsr_model* m, const float* attended, const float* preproce
                      const float* weights, const int64_t* step, const int64_t* outputs, float* next_states,
                      float* next_wavg, float* next_weights, float* next_energies, int64_t* next_step, void* stream) {
   DeviceGuard device_guard(m);
+  if (int rc = bind_stream(m, static_cast<cudaStream_t>(stream))) return rc;
   if (int rc = check_ready(m)) return rc;
   LVSR_CHECK(attended && attended_mask && states && weights && step && outputs && next_states && next_wavg &&
                  next_weights && next_energies && next_step && Tp > 0 && U > 0 && R > 0,
@@ -1230,6 +1245,7 @@ extern "C" {
 int lvsr_recognizer_cost_host(lvsr_model* m, const float* x_h, const float* mask_h, const int64_t* labels_h,
                               const float* lmask_h, int32_t T, int32_t B, int32_t L, float* costs_h, void* stream) {
   DeviceGuard device_guard(m);
+  if (int rc = bind_stream(m, static_cast<cudaStream_t>(stream))) return rc;
   if (int rc = check_ready(m)) return rc;
   LVSR_CHECK(x_h && labels_h && costs_h && T > 0 && B > 0 && L > 0, "recognizer_cost_host: bad arguments");
   for (long long i = 0; i < (long long)L * B; ++i)       // host memory: the lookup's IndexError, up front

@@ -12,21 +12,14 @@ namespace lvsr {
 
 // Stack-style device workspace.  Top-level API calls bump-allocate from one block; when
 // the block is too small the overflow is served by separate cudaMallocs and the block is
-// regrown at the end of the call, so a steady-state workload never allocates.
+// regrown at the end of the call, so a steady-state workload never allocates.  The arena is
+// rewound when a call returns while its kernels may still be in flight: safe because every call
+// on the handle runs on the handle's bound stream (bind_stream below).
 struct Arena {
   char* base = nullptr;
   size_t cap = 0, off = 0, overflow_bytes = 0;
   int depth = 0;
   std::vector<void*> overflow;
-  // the arena is rewound when a call returns while its kernels may still be in flight: safe only if the next call
-  // is enqueued on the SAME stream.  A call on another stream first waits for everything the previous one enqueued.
-  cudaStream_t last_stream = nullptr;
-  bool used = false;
-  void bind_stream(cudaStream_t st) {
-    if (depth == 0 && used && st != last_stream) cudaStreamSynchronize(last_stream);
-    last_stream = st;
-    used = true;
-  }
 
   void* alloc(size_t bytes) {
     bytes = (bytes + 255) & ~(size_t)255;
@@ -153,6 +146,9 @@ struct lvsr_model {
   int lm_start = 0;
   lvsr_lm_fusion lm_fusion = {};
   unsigned* lm_status = nullptr;
+  // The stream of the last call that enqueued work on the handle (bind_stream).  Both arenas, the device words above
+  // and the parameter and optimizer buffers are only ever touched in this stream's order.
+  cudaStream_t stream = nullptr;
   Arena ws;
   // ---- training (train.cu) ----
   Arena tws;                        // tape + backward workspace
@@ -232,11 +228,31 @@ struct DeviceGuard {
   ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
 };
 
+// Every entry point that takes a stream binds it first, before it sizes a workspace or touches per-handle device
+// state: a call on another stream than the last one first waits for everything the handle enqueued there, so two
+// streams never share the arenas, the status and claim words or the parameters at once.
+static inline int bind_stream(lvsr_model* m, cudaStream_t st) {
+  LVSR_CHECK(m != nullptr, "null model");
+  if (st != m->stream) {
+    LVSR_CUDA_OK(cudaStreamSynchronize(m->stream));
+    m->stream = st;
+  }
+  return 0;
+}
+
+// Host calls without a stream take effect after all work queued on the handle: they copy on its bound stream and,
+// when the copy touches host memory, wait for it.
+static inline int copy_on_handle(const lvsr_model* m, void* dst, const void* src, size_t bytes, cudaMemcpyKind kind) {
+  LVSR_CUDA_OK(cudaMemcpyAsync(dst, src, bytes, kind, m->stream));
+  LVSR_CUDA_OK(cudaStreamSynchronize(m->stream));
+  return 0;
+}
+
 struct ArenaScope {
   Arena& ws;
   cudaStream_t st;
-  ArenaScope(lvsr_model* mm, cudaStream_t s) : ws(mm->ws), st(s) { ws.bind_stream(s); ws.enter(); }
-  ArenaScope(Arena& a, cudaStream_t s) : ws(a), st(s) { ws.bind_stream(s); ws.enter(); }
+  ArenaScope(lvsr_model* mm, cudaStream_t s) : ws(mm->ws), st(s) { ws.enter(); }
+  ArenaScope(Arena& a, cudaStream_t s) : ws(a), st(s) { ws.enter(); }
   ~ArenaScope() { ws.leave(st); }
 };
 

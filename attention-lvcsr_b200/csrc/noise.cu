@@ -230,6 +230,7 @@ int lvsr_train_set_adaptive_noise(lvsr_model* m, const lvsr_adaptive_noise* cfg)
   lvsr_model::Noise& z = m->noise;
   const size_t n = (size_t)m->flat_count, np = m->params.size();
   const size_t nparts = (size_t)kCtasPerParam * np;
+  LVSR_CUDA_OK(cudaDeviceSynchronize());          // after every call queued on the handle, on any stream
   if (!z.mem) {
     LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&z.mem), 6 * n * sizeof(float)));
     const size_t span_bytes = (np * sizeof(Span) + 255) & ~(size_t)255;
@@ -243,8 +244,6 @@ int lvsr_train_set_adaptive_noise(lvsr_model* m, const lvsr_adaptive_noise* cfg)
     std::vector<Span> h(np);
     for (size_t i = 0; i < np; ++i) h[i] = Span{m->params[i].offset, m->params[i].count};
     LVSR_CUDA_OK(cudaMemcpy(z.spans, h.data(), np * sizeof(Span), cudaMemcpyHostToDevice));
-  } else {
-    LVSR_CUDA_OK(cudaDeviceSynchronize());
   }
   LVSR_CUDA_OK(cudaMemset(z.mem, 0, 6 * n * sizeof(float)));
   LVSR_CUDA_OK(cudaMemset(z.stats, 0, 4 * sizeof(double)));
@@ -263,15 +262,16 @@ int lvsr_train_get_noise_param(const lvsr_model* m, int index, float* host, int6
   if (int rc = check_index(m, index, count)) return rc;
   LVSR_CHECK(host, "null argument");
   DeviceGuard device_guard(m);
-  LVSR_CUDA_OK(cudaMemcpy(host, m->noise.ls2 + m->params[index].offset, (size_t)count * sizeof(float), cudaMemcpyDeviceToHost));
-  return 0;
+  return copy_on_handle(m, host, m->noise.ls2 + m->params[index].offset, (size_t)count * sizeof(float),
+                        cudaMemcpyDeviceToHost);
 }
 
 int lvsr_train_set_noise_param(lvsr_model* m, int index, const float* host, int64_t count) {
   if (int rc = check_index(m, index, count)) return rc;
   LVSR_CHECK(host, "null argument");
   DeviceGuard device_guard(m);
-  LVSR_CUDA_OK(cudaMemcpy(m->noise.ls2 + m->params[index].offset, host, (size_t)count * sizeof(float), cudaMemcpyHostToDevice));
+  if (int rc = copy_on_handle(m, m->noise.ls2 + m->params[index].offset, host, (size_t)count * sizeof(float),
+                              cudaMemcpyHostToDevice)) return rc;
   m->noise.sampled = false;
   return 0;
 }
@@ -290,6 +290,7 @@ int lvsr_train_noise_sample(lvsr_model* m, int64_t update, float* eps_dev, void*
   LVSR_CHECK(m->noise.on, "adaptive noise is off (lvsr_train_set_adaptive_noise)");
   DeviceGuard device_guard(m);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (int rc = bind_stream(m, st)) return rc;
   ProfScope prof("noise", st);
   LVSR_CUDA_OK(cudaMemsetAsync(eps_dev, 0, (size_t)m->flat_count * sizeof(float), st));
   noise_eps_kernel<<<param_grid(m), kThreads, 0, st>>>(eps_dev, spans_of(m), m->noise.cfg.seed, (unsigned long long)update);
@@ -301,8 +302,10 @@ int lvsr_train_noise_params(lvsr_model* m, float* out_dev, void* stream) {
   LVSR_CHECK(m && out_dev, "train_noise_params: null argument");
   LVSR_CHECK(m->noise.on, "adaptive noise is off (lvsr_train_set_adaptive_noise)");
   DeviceGuard device_guard(m);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (int rc = bind_stream(m, st)) return rc;
   LVSR_CUDA_OK(cudaMemcpyAsync(out_dev, m->noise.noisy, (size_t)m->flat_count * sizeof(float), cudaMemcpyDeviceToDevice,
-                               static_cast<cudaStream_t>(stream)));
+                               st));
   return 0;
 }
 
@@ -311,6 +314,7 @@ int lvsr_train_noise_gradients(lvsr_model* m, float* grads_dev, float gscale, fl
   LVSR_CHECK(m->noise.on, "adaptive noise is off (lvsr_train_set_adaptive_noise)");
   DeviceGuard device_guard(m);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (int rc = bind_stream(m, st)) return rc;
   LVSR_CUDA_OK(cudaMemsetAsync(ls2_grads_dev, 0, (size_t)m->flat_count * sizeof(float), st));
   return noise_gradients(m, grads_dev, gscale, ls2_grads_dev, st, nullptr);
 }

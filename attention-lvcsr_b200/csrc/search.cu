@@ -63,6 +63,7 @@ int lvsr_beam_search_many(lvsr_model* m, const float* attended, const float* pre
                           double round_to_inf, int32_t stop_on_optimistic, lvsr_validate_fn validate, void* validate_user,
                           lvsr_search_result** result, void* stream) {
   DeviceGuard device_guard(m);
+  if (int rc = bind_stream(m, static_cast<cudaStream_t>(stream))) return rc;
   if (int rc = check_ready(m)) return rc;
   LVSR_CHECK(attended && preprocessed && attended_mask && utt_len_host && max_length_host && result && Tp > 0 && U > 0 && beam_size > 0,
              "beam_search_many: bad arguments");
@@ -140,7 +141,7 @@ int lvsr_beam_search_many(lvsr_model* m, const float* attended, const float* pre
   auto lm_check = [&]() -> int {
     if (!lm || *h_lm == 0) return 0;
     const unsigned s = *h_lm;
-    LVSR_CUDA_OK(cudaMemset(m->lm_status, 0, sizeof(unsigned)));
+    LVSR_CUDA_OK(cudaMemsetAsync(m->lm_status, 0, sizeof(unsigned), st));
     return lm_report(s);
   };
 

@@ -547,7 +547,8 @@ extern "C" {
 int lvsr_train_cost_and_grads(lvsr_model* m, const float* x, const float* mask, const int64_t* labels, const float* lmask,
                               int32_t T, int32_t B, int32_t L, float gscale, float* cost_out, float* grads, void* stream) {
   DeviceGuard device_guard(m);
-  if (!m || !m->noise.on) return forward_backward(m, x, mask, labels, lmask, T, B, L, gscale, cost_out, grads, stream);
+  if (int rc = bind_stream(m, static_cast<cudaStream_t>(stream))) return rc;
+  if (!m->noise.on) return forward_backward(m, x, mask, labels, lmask, T, B, L, gscale, cost_out, grads, stream);
   // adaptive weight noise (noise.cu): the step runs on p + eps sqrt(s2).  Every parameter pointer is re-pointed at
   // the noisy copy and the kernel-side weights are re-packed from it; on every way out the pointers go back to the
   // means and the handle is marked un-finalized, so any other entry point re-packs from the means first.
@@ -578,6 +579,7 @@ int lvsr_train_apply_updates(lvsr_model* m, float* grads, float gscale, const lv
   LVSR_CHECK(m && grads && tc, "train_apply_updates: null argument");
   LVSR_CHECK(!(tc->decay_rate < 0.f || tc->decay_rate > 1.f), "decay rate needs to be in [0, 1]");   // B/algorithms/__init__.py:481-482
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (int rc = bind_stream(m, st)) return rc;
   const long long n = m->flat_count;
   const int np = (int)m->params.size();
   lvsr_model::Noise& z = m->noise;
@@ -592,7 +594,8 @@ int lvsr_train_apply_updates(lvsr_model* m, float* grads, float gscale, const lv
       h[i].is_weight = is_weight_name(m->params[i].name) ? 1 : 0;
     }
     LVSR_CUDA_OK(cudaMalloc(&m->opt_desc, sizeof(ParamDesc) * np));
-    LVSR_CUDA_OK(cudaMemcpy(m->opt_desc, h.data(), sizeof(ParamDesc) * np, cudaMemcpyHostToDevice));
+    LVSR_CUDA_OK(cudaMemcpyAsync(m->opt_desc, h.data(), sizeof(ParamDesc) * np, cudaMemcpyHostToDevice, st));
+    LVSR_CUDA_OK(cudaStreamSynchronize(st));         // h goes away on return (once per handle)
     LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->opt_scratch), 1032 * sizeof(float)));
   }
   auto lazy = [&](float** p) -> int {
@@ -668,18 +671,18 @@ int lvsr_train_apply_updates(lvsr_model* m, float* grads, float gscale, const lv
 int lvsr_train_gradient_norm(lvsr_model* m, float* norm_host) {
   LVSR_CHECK(m && norm_host && m->opt_scratch, "train_gradient_norm: no update has run yet");
   DeviceGuard device_guard(m);
-  LVSR_CUDA_OK(cudaMemcpy(norm_host, m->opt_scratch + 1024, sizeof(float), cudaMemcpyDeviceToHost));
-  return 0;
+  return copy_on_handle(m, norm_host, m->opt_scratch + 1024, sizeof(float), cudaMemcpyDeviceToHost);   // after the update
 }
 
 int lvsr_train_reset(lvsr_model* m) {
   LVSR_CHECK(m, "null model");
   DeviceGuard device_guard(m);
   const size_t bytes = (size_t)m->flat_count * sizeof(float);
-  if (m->opt_velocity) LVSR_CUDA_OK(cudaMemset(m->opt_velocity, 0, bytes));
-  if (m->opt_ms_step) LVSR_CUDA_OK(cudaMemset(m->opt_ms_step, 0, bytes));
-  if (m->opt_ms_dx) LVSR_CUDA_OK(cudaMemset(m->opt_ms_dx, 0, bytes));
-  if (m->noise.on) LVSR_CUDA_OK(cudaMemset(m->noise.velocity, 0, 3 * bytes));     // velocity | ms_step | ms_dx of ls2
+  cudaStream_t st = m->stream;     // after every update queued on the handle, before the next one
+  if (m->opt_velocity) LVSR_CUDA_OK(cudaMemsetAsync(m->opt_velocity, 0, bytes, st));
+  if (m->opt_ms_step) LVSR_CUDA_OK(cudaMemsetAsync(m->opt_ms_step, 0, bytes, st));
+  if (m->opt_ms_dx) LVSR_CUDA_OK(cudaMemsetAsync(m->opt_ms_dx, 0, bytes, st));
+  if (m->noise.on) LVSR_CUDA_OK(cudaMemsetAsync(m->noise.velocity, 0, 3 * bytes, st));     // velocity | ms_step | ms_dx of ls2
   m->burn_in_left = -1;
   return 0;
 }

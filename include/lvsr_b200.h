@@ -13,9 +13,22 @@
  *     layouts the reference feeds its compiled functions
  *     (lvsr/datasets/__init__.py:22-29,308; lvsr/bricks/recognizer.py:129-133,353-361).
  *   - `*_dev` pointers are device pointers on the model's GPU, `*_host` are host pointers.
- *   - `stream` is a cudaStream_t passed as void* (NULL = default stream).  Calls are
- *     stream-ordered and never synchronise, except the `*_host` convenience calls,
- *     which copy H2D, compute, copy D2H and synchronise the stream before returning.
+ *   - `stream` is a cudaStream_t passed as void* (NULL = default stream); blocking and
+ *     non-blocking streams are both fine.  A call that takes a stream is ordered on it.  The
+ *     handle is bound to the stream of its last such call: a call on a different stream first
+ *     synchronises the previous one, so the handle's workspace, device words and parameters are
+ *     never used from two streams at once.  The caller orders its own buffers between streams,
+ *     and keeps the bound stream alive until the handle's next call on another one.
+ *   - host calls without a stream (get/set_param, finalize, status, train_gradient_norm,
+ *     get/set_noise_param) act after all work queued on the handle: they synchronise its bound
+ *     stream.  train_reset is enqueued on that stream without waiting.
+ *   - calls with a stream do not synchronise, except: the `*_host` convenience calls (copy H2D,
+ *     compute, copy D2H, synchronise the stream); a call that needs a larger workspace than the
+ *     handle holds (it is regrown); the first call after parameters changed (it re-packs the
+ *     weights, like lvsr_model_finalize); the LM calls noted below; and, with the logistic or
+ *     relu normaliser, the call that re-packs the weights after an update, which reads the energy
+ *     bias back to the host as a kernel argument: lvsr_train_apply_updates without adaptive
+ *     noise, lvsr_train_cost_and_grads (for the noisy bias) with it.
  *   - every call returns 0 on success, non-zero on error; lvsr_last_error() then
  *     describes the failure (thread-local).
  *   - one model handle per GPU; a handle is not thread-safe.
@@ -94,7 +107,7 @@ float* lvsr_model_flat_params(lvsr_model* m);     /* device pointer; call lvsr_m
 /* Re-derive the packed kernel-side weights after parameters changed. */
 int lvsr_model_finalize(lvsr_model* m);
 /* Launch status of the persistent teacher-forced decoder of the LAST lvsr_cost_matrix call on this
- * handle (synchronises with the device): 0 = ok, 2 = a hand-over value never arrived within the
+ * handle (synchronises the handle's stream): 0 = ok, 2 = a hand-over value never arrived within the
  * polling limit, 3 = the launch lost its cluster shape.  On a non-zero status the costs of that call
  * are NaN (never plausible garbage); lvsr_recognizer_cost_host re-runs such a call on the step-wise
  * kernels by itself and counts it in *stepwise_fallbacks (may be NULL).  No reference counterpart:
@@ -309,8 +322,9 @@ int lvsr_train_cost_and_grads(lvsr_model* m, const float* recordings_dev, const 
                               int32_t L, float gscale, float* cost_dev, float* grads_dev, void* stream);
 int lvsr_train_apply_updates(lvsr_model* m, float* grads_dev, float gscale, const lvsr_train_config* tc,
                              void* stream);
-int lvsr_train_gradient_norm(lvsr_model* m, float* norm_host);   /* total_gradient_norm of the last update (synchronises) */
-int lvsr_train_reset(lvsr_model* m);
+int lvsr_train_gradient_norm(lvsr_model* m, float* norm_host);   /* total_gradient_norm of the last update (synchronises
+                                                                    the handle's stream) */
+int lvsr_train_reset(lvsr_model* m);     /* zero the optimizer state, enqueued on the handle's stream after its updates */
 
 /* ---- adaptive weight noise (Graves 2011): apply_adaptive_noise, lvsr/graph.py:71-251, as lvsr/main.py:425-460
  * applies it to every parameter).  Each parameter p gets a log-variance ls2 of its shape, s2 = exp(2048 ls2).
