@@ -12,10 +12,11 @@ from .bricks import (Constant, GatedRecurrent, Identity, IsotropicGaussian, Maxo
                      Orthogonal, Rectifier, Tanh, Uniform)
 from . import algorithms  # noqa: F401
 from .algorithms import (AdaDelta, BurnIn, CompositeRule, GradientDescent, Momentum, RemoveNotFinite,  # noqa: F401
-                         Restrict, Scale, StepClipping, VariableClipping, step_rule_from_config)
+                         Restrict, Scale, StepClipping, VariableClipping, adaptive_clipping, clipping_rule,
+                         step_rule_from_config)
 from .recognizer import SpeechRecognizer  # noqa: F401
 from .search import BeamSearch, CandidateNotFoundError  # noqa: F401
 
 __all__ = ["GradientDescent", "CompositeRule", "StepClipping", "Momentum", "AdaDelta", "VariableClipping", "Restrict",
-           "RemoveNotFinite", "BurnIn", "Scale", "step_rule_from_config", "SpeechRecognizer", "BeamSearch", "CandidateNotFoundError", "Maxout", "Rectifier", "Tanh",
+           "RemoveNotFinite", "BurnIn", "Scale", "adaptive_clipping", "clipping_rule", "step_rule_from_config", "SpeechRecognizer", "BeamSearch", "CandidateNotFoundError", "Maxout", "Rectifier", "Tanh",
            "Identity", "GatedRecurrent", "IsotropicGaussian", "Constant", "Orthogonal", "Uniform"]

@@ -71,6 +71,11 @@ class LvsrAdaptiveNoise(C.Structure):
                 ("seed", C.c_uint64)]
 
 
+class LvsrAdaptiveClipping(C.Structure):
+    """Mirror of ``lvsr_adaptive_clipping`` (include/lvsr_b200.h)."""
+    _fields_ = [("initial_threshold", C.c_double), ("decay_rate", C.c_double), ("burnin_period", C.c_int32)]
+
+
 # slots of lvsr_train_noise_stats (LVSR_NOISE_*), under the reference's monitor names (lvsr/main.py:440-460)
 NOISE_STATS = ("model_cost", "model_prior_mean", "model_prior_variance")
 
@@ -131,6 +136,9 @@ SIGNATURES = {
     "lvsr_train_apply_updates": (C.c_int, [_P, _P, C.c_float, C.POINTER(LvsrTrainConfig), _P]),
     "lvsr_train_gradient_norm": (C.c_int, [_P, C.POINTER(C.c_float)]),
     "lvsr_train_reset": (C.c_int, [_P]),
+    "lvsr_train_set_adaptive_clipping": (C.c_int, [_P, C.POINTER(LvsrAdaptiveClipping)]),
+    "lvsr_train_clipping_threshold": (C.c_int, [_P, C.POINTER(C.c_double)]),
+    "lvsr_alignment_stats": (C.c_int, [_P, _P, _P, _I, _I, _I, _P, _P]),
     "lvsr_train_set_adaptive_noise": (C.c_int, [_P, C.POINTER(LvsrAdaptiveNoise)]),
     "lvsr_train_get_noise_param": (C.c_int, [_P, C.c_int, _P, C.c_int64]),
     "lvsr_train_set_noise_param": (C.c_int, [_P, C.c_int, _P, C.c_int64]),

@@ -41,10 +41,48 @@ class StepRule(object):
 
 
 class StepClipping(StepRule):
-    """B/algorithms/__init__.py:610-643."""
+    """B/algorithms/__init__.py:610-643.
+
+    ``adaptive`` (set by ``adaptive_clipping``): None, or dict(burnin_period, decay_rate) of the AdaptiveClipping
+    extension that resets this rule's threshold after every batch (lvsr/extensions.py:64-91); ``threshold`` is then its
+    initial threshold."""
 
     def __init__(self, threshold=None):
         self.threshold = threshold
+        self.adaptive = None
+        self._recognizer = None
+
+    def current_threshold(self):
+        """The threshold the next update uses: under adaptive clipping the device value once a GradientDescent has
+        been initialised with this rule (lvsr_train_clipping_threshold; synchronises), else ``threshold``."""
+        if self.adaptive is None or self._recognizer is None:
+            return None if self.threshold is None else float(self.threshold)
+        v = C.c_double()
+        _lib.check(_lib.load().lvsr_train_clipping_threshold(self._recognizer._require_ready(), C.byref(v)))
+        return float(v.value)
+
+
+def adaptive_clipping(step_rule, burnin_period=100, decay_rate=0.99):
+    """Mark the StepClipping of `step_rule` (a StepClipping, or a CompositeRule holding one) as adaptive, as
+    ``AdaptiveClipping(total_gradient_norm, clipping, gradient_threshold, decay_rate, burnin_period)`` does in
+    lvsr/main.py:616-619 (defaults: lvsr/extensions.py:66-67; lvsr/main.py passes 0.998 and 500).  Returns `step_rule`.
+    GradientDescent.initialize() then keeps the threshold's statistics on the device (include/lvsr_b200.h)."""
+    comps = step_rule.components if isinstance(step_rule, CompositeRule) else [step_rule]
+    clips = [c for c in comps if isinstance(c, StepClipping)]
+    if len(clips) != 1:
+        raise ValueError("adaptive_clipping needs exactly one StepClipping in the rule, found %d" % len(clips))
+    if not clips[0].threshold or clips[0].threshold <= 0:
+        raise ValueError("adaptive_clipping needs an initial threshold > 0, got %r" % (clips[0].threshold,))
+    if int(burnin_period) < 1 or not 0.0 <= float(decay_rate) <= 1.0:
+        raise ValueError("adaptive_clipping: burnin_period >= 1 and decay_rate in [0, 1] expected")
+    clips[0].adaptive = dict(burnin_period=int(burnin_period), decay_rate=float(decay_rate))
+    return step_rule
+
+
+def clipping_rule(step_rule):
+    """The StepClipping of `step_rule`, or None."""
+    comps = step_rule.components if isinstance(step_rule, CompositeRule) else [step_rule]
+    return next((c for c in comps if isinstance(c, StepClipping)), None)
 
 
 class Scale(StepRule):
@@ -254,6 +292,15 @@ class GradientDescent(object):
         self._cost = torch.zeros((1,), dtype=torch.float32, device=rec.device)
         self._n = n
         _lib.check(lib.lvsr_train_reset(h))
+        clip = clipping_rule(self.step_rule)
+        if clip is not None and getattr(clip, "adaptive", None) is not None:
+            cfg = _lib.LvsrAdaptiveClipping(initial_threshold=float(clip.threshold),
+                                            decay_rate=clip.adaptive["decay_rate"],
+                                            burnin_period=clip.adaptive["burnin_period"])
+            _lib.check(lib.lvsr_train_set_adaptive_clipping(h, C.byref(cfg)))
+            clip._recognizer = rec
+        else:
+            _lib.check(lib.lvsr_train_set_adaptive_clipping(h, None))
         if self.adaptive_noise:
             an = self.adaptive_noise
             cfg = _lib.LvsrAdaptiveNoise(init_sigma=an["init_sigma"], model_cost_coefficient=an["model_cost_coefficient"],

@@ -402,6 +402,8 @@ int lvsr_model_destroy(lvsr_model* m) {
   if (m->opt_ms_dx) cudaFree(m->opt_ms_dx);
   if (m->opt_scratch) cudaFree(m->opt_scratch);
   if (m->opt_desc) cudaFree(m->opt_desc);
+  if (m->clip) cudaFree(m->clip);
+  if (m->align_mem) cudaFree(m->align_mem);
   lvsr_model_clear_lm(m);
   noise_free(m);
   m->tws.destroy();

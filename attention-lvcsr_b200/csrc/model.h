@@ -156,6 +156,11 @@ struct lvsr_model {
   float* opt_scratch = nullptr;     // [1024 partial sums | norm]
   void* opt_desc = nullptr;         // device copy of the per-parameter table (train::ParamDesc)
   long long burn_in_left = -1;      // BurnIn counter (-1: not started)
+  double* clip = nullptr;           // device train::CLIP_* words of adaptive clipping (nullptr: off)
+  double clip_init[8] = {};         // their values after lvsr_train_set_adaptive_clipping / lvsr_train_reset
+  // ---- lvsr_alignment_stats (stats.cu): [finished-CTA count | 256-byte pad | 2 doubles per batch row] ----
+  void* align_mem = nullptr;
+  int align_rows = 0;               // batch rows it holds
   // ---- adaptive weight noise (noise.cu; lvsr_train_set_adaptive_noise) ----
   struct Noise {
     bool on = false;

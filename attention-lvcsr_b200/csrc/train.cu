@@ -15,6 +15,7 @@
 #include <stdlib.h>
 
 #include <algorithm>
+#include <cmath>
 #include <string>
 #include <vector>
 
@@ -618,19 +619,20 @@ int lvsr_train_apply_updates(lvsr_model* m, float* grads, float gscale, const lv
     // both gradient groups of adaptive noise (noise.cu), already multiplied by gscale; one clipping norm over both
     int nparts = 0;
     if (int rc = noise_gradients(m, grads, gscale, z.gls2, st, &nparts)) return rc;
-    sqnorm_final_kernel<<<1, 32, 0, st>>>(z.norm_part, nparts, 1.f, norm);
+    sqnorm_final_kernel<<<1, 32, 0, st>>>(z.norm_part, nparts, 1.f, norm, m->clip);
     LVSR_LAUNCH_CHECK();
     gscale = 1.f;
   } else {
     const int nparts = (int)std::min<long long>(1024, std::max<long long>(1, n / 4096));
     sqnorm_partial_kernel<<<nparts, 256, 0, st>>>(grads, n, part);
     LVSR_LAUNCH_CHECK();
-    sqnorm_final_kernel<<<1, 32, 0, st>>>(part, nparts, gscale, norm);
+    sqnorm_final_kernel<<<1, 32, 0, st>>>(part, nparts, gscale, norm, m->clip);
     LVSR_LAUNCH_CHECK();
   }
   StepArgs a = {};
   a.grads = grads; a.params = m->flat; a.velocity = m->opt_velocity; a.ms_step = m->opt_ms_step; a.ms_dx = m->opt_ms_dx;
   a.norm = norm; a.n = n; a.gscale = gscale; a.decay = tc->decay; a.threshold = tc->gradient_threshold;
+  a.clip = m->clip;
   a.use_momentum = tc->use_momentum; a.learning_rate = tc->scale; a.momentum = tc->momentum;
   a.use_adadelta = tc->use_adadelta; a.decay_rate = tc->decay_rate; a.epsilon = tc->epsilon;
   step_rules_kernel<<<grid1d(n, 256, 1184), 256, 0, st>>>(a);
@@ -683,8 +685,43 @@ int lvsr_train_reset(lvsr_model* m) {
   if (m->opt_ms_step) LVSR_CUDA_OK(cudaMemsetAsync(m->opt_ms_step, 0, bytes, st));
   if (m->opt_ms_dx) LVSR_CUDA_OK(cudaMemsetAsync(m->opt_ms_dx, 0, bytes, st));
   if (m->noise.on) LVSR_CUDA_OK(cudaMemsetAsync(m->noise.velocity, 0, 3 * bytes, st));     // velocity | ms_step | ms_dx of ls2
+  if (m->clip) LVSR_CUDA_OK(cudaMemcpyAsync(m->clip, m->clip_init, sizeof(m->clip_init), cudaMemcpyHostToDevice, st));
   m->burn_in_left = -1;
   return 0;
+}
+
+int lvsr_train_set_adaptive_clipping(lvsr_model* m, const lvsr_adaptive_clipping* cfg) {
+  LVSR_CHECK(m, "null model");
+  DeviceGuard device_guard(m);
+  static_assert(sizeof(m->clip_init) == CLIP_WORDS * sizeof(double), "clip_init holds the CLIP_* words");
+  if (!cfg) {
+    if (m->clip) {
+      LVSR_CUDA_OK(cudaStreamSynchronize(m->stream));     // an update queued on the handle may still read the state
+      cudaFree(m->clip);
+      m->clip = nullptr;
+    }
+    return 0;
+  }
+  LVSR_CHECK(cfg->initial_threshold > 0.0 && std::isfinite(cfg->initial_threshold),
+             "adaptive clipping: initial_threshold must be > 0");
+  LVSR_CHECK(cfg->decay_rate >= 0.0 && cfg->decay_rate <= 1.0, "adaptive clipping: decay_rate must be in [0, 1]");
+  LVSR_CHECK(cfg->burnin_period > 0, "adaptive clipping: burnin_period must be > 0");
+  double* c = m->clip_init;
+  for (int i = 0; i < CLIP_WORDS; ++i) c[i] = 0.0;
+  c[CLIP_THR] = c[CLIP_NEXT] = c[CLIP_THR0] = cfg->initial_threshold;
+  c[CLIP_DECAY] = cfg->decay_rate;
+  c[CLIP_BURNIN] = (double)cfg->burnin_period;
+  if (!m->clip) LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->clip), sizeof(m->clip_init)));
+  // after every update queued on the handle; the host image lives in the handle, so the copy needs no wait
+  LVSR_CUDA_OK(cudaMemcpyAsync(m->clip, c, sizeof(m->clip_init), cudaMemcpyHostToDevice, m->stream));
+  return 0;
+}
+
+int lvsr_train_clipping_threshold(lvsr_model* m, double* threshold_host) {
+  LVSR_CHECK(m && threshold_host, "null argument");
+  LVSR_CHECK(m->clip, "adaptive clipping is off (lvsr_train_set_adaptive_clipping)");
+  DeviceGuard device_guard(m);
+  return copy_on_handle(m, threshold_host, m->clip + CLIP_NEXT, sizeof(double), cudaMemcpyDeviceToHost);
 }
 
 }  // extern "C"

@@ -860,11 +860,39 @@ __global__ void __launch_bounds__(256) sqnorm_partial_kernel(const float* g, lon
     part[blockIdx.x] = v;
   }
 }
-__global__ void sqnorm_final_kernel(const float* part, int nparts, float gscale, float* norm_out) {
+// Adaptive clipping (lvsr/extensions.py:64-91 as lvsr/main.py:616-619 installs it; lvsr_train_set_adaptive_clipping):
+// device doubles.  CLIP_THR is the threshold of the step being applied, CLIP_NEXT the one the next step will use.
+enum { CLIP_MU = 0, CLIP_MU2 = 1, CLIP_N = 2, CLIP_THR = 3, CLIP_NEXT = 4, CLIP_THR0 = 5, CLIP_DECAY = 6, CLIP_BURNIN = 7,
+       CLIP_WORDS = 8 };
+
+// AdaptiveClipping.after_batch for the batch whose gradient norm is `norm`, in float64.  A zero norm (math.log(0) raises
+// in the reference) leaves the moments as they were; the count still advances, as iterations_done does.
+__device__ inline void adaptive_clip_update(double* c, double norm) {
+  c[CLIP_THR] = c[CLIP_NEXT];
+  const double d = c[CLIP_DECAY], thr0 = c[CLIP_THR0], burnin = c[CLIP_BURNIN];
+  const double n = c[CLIP_N] + 1.0;
+  c[CLIP_N] = n;
+  if (norm != 0.0) {
+    const double L = log(norm);
+    c[CLIP_MU] = d * c[CLIP_MU] + (1.0 - d) * L;
+    c[CLIP_MU2] = d * c[CLIP_MU2] + (1.0 - d) * L * L;
+  }
+  const double mu = c[CLIP_MU], var = c[CLIP_MU2] - mu * mu;
+  const double sigma = sqrt(var < 0.0 ? 0.0 : var);          // rounding below 0 only; a NaN passes through
+  const double conf = fmin(burnin, n) / burnin;
+  const double thr = conf * exp(mu + sigma) + (1.0 - conf) * thr0;
+  const double cap = 5.0 * thr0;
+  c[CLIP_NEXT] = cap < thr ? cap : thr;                       // Python's min(thr, cap): a NaN threshold stays NaN
+}
+
+// clip: adaptive clipping state or nullptr (off)
+__global__ void sqnorm_final_kernel(const float* part, int nparts, float gscale, float* norm_out, double* clip) {
   if (threadIdx.x == 0 && blockIdx.x == 0) {
     double s = 0.0;
     for (int i = 0; i < nparts; ++i) s += (double)part[i];
-    norm_out[0] = (float)(sqrt(s) * (double)gscale);
+    const float norm = (float)(sqrt(s) * (double)gscale);
+    norm_out[0] = norm;
+    if (clip) adaptive_clip_update(clip, (double)norm);
   }
 }
 
@@ -880,10 +908,17 @@ struct StepArgs {
   int use_momentum; float learning_rate, momentum;
   int use_adadelta; float decay_rate, epsilon;
   const unsigned char* is_weight_map;   // per element or nullptr
+  const double* clip;        // adaptive clipping state or nullptr: the threshold is clip[CLIP_THR], not `threshold`
 };
 __global__ void step_rules_kernel(StepArgs a) {
   const float norm = a.norm[0];
-  const float mult = (a.threshold > 0.f && !(norm < a.threshold)) ? a.threshold / norm : 1.f;
+  float mult;
+  if (a.clip) {              // StepClipping with its shared float32 threshold: switch(norm < thr, 1, thr / norm)
+    const float thr = (float)a.clip[CLIP_THR];
+    mult = norm < thr ? 1.f : thr / norm;
+  } else {
+    mult = (a.threshold > 0.f && !(norm < a.threshold)) ? a.threshold / norm : 1.f;
+  }
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < a.n; i += (long long)gridDim.x * blockDim.x) {
     float s = a.grads[i] * a.gscale * mult;
     if (a.use_momentum) {

@@ -610,6 +610,49 @@ class SpeechRecognizer(object):
             return extra
         return costs
 
+    def alignment_statistics(self, weights, labels_mask, out):
+        """lvsr_alignment_stats: out[0] = sum of mask * sum_t w log(w + 1e-7), out[1] = the monotonicity penalty
+        (lvsr/expressions.py:14-25) of weights [L,B,T'] on the device; out is a float64 device tensor of >= 2."""
+        torch = self._torch()
+        lib, h = _lib.load(), self._require_ready()
+        L, B, Tp = weights.shape
+        if weights.dtype != torch.float32 or not weights.is_contiguous():
+            raise ValueError("alignment_statistics: contiguous float32 weights expected")
+        if labels_mask is not None and (tuple(labels_mask.shape) != (L, B) or labels_mask.dtype != torch.float32):
+            raise ValueError("alignment_statistics: labels_mask must be float32 [%d, %d]" % (L, B))
+        if out.dtype != torch.float64 or out.numel() < 2:
+            raise ValueError("alignment_statistics: out must be a float64 tensor of at least 2 elements")
+        _lib.check(lib.lvsr_alignment_stats(h, _ptr(weights), _ptr(labels_mask), L, B, Tp, _ptr(out), self._stream()))
+        return out
+
+    def validation_statistics(self, recordings, recordings_mask, labels, labels_mask):
+        """What one batch of the reference's validation (lvsr/main.py:550-568) accumulates: dict(cost = sum of the cost
+        matrix, weights_entropy, weights_penalty (the sums of lvsr/expressions.py:14-25), num_labels = sum of the label
+        mask, batch_size).  The encoder, the teacher-forced decoder with its alignment, and the statistics kernel run on
+        device buffers; the results come back in one copy."""
+        torch = self._torch()
+        att, attm = self.encode(recordings, recordings_mask)
+        self._check_labels(labels)
+        y = self._dev(labels, torch.int64)
+        ym = self._dev(labels_mask, torch.float32)
+        L, B = y.shape
+        # [entropy, penalty | costs [L, B] as float32]: one read-back
+        buf = torch.empty((2 + (L * B + 1) // 2,), dtype=torch.float64, device=self.device)
+        costs = buf[2:].view(torch.float32)[:L * B].view(L, B)
+        weights = torch.empty((L, B, att.shape[0]), dtype=torch.float32, device=self.device)
+        lib, h = _lib.load(), self._require_ready()
+        if ym is not None and tuple(ym.shape) != (L, B):
+            raise ValueError("validation_statistics: labels_mask must be [%d, %d], got %s" % (L, B, tuple(ym.shape)))
+        _lib.check(lib.lvsr_cost_matrix(h, _ptr(att), _ptr(attm), att.shape[0], B, _ptr(y), _ptr(ym), L, _ptr(costs),
+                                        _ptr(weights), None, None, None, self._stream()))
+        self.alignment_statistics(weights, ym, buf)
+        host = buf.cpu().numpy()
+        host_costs = host[2:].view(np.float32)[:L * B]
+        num_labels = float(L * B) if labels_mask is None else float(np.asarray(
+            labels_mask.cpu() if isinstance(labels_mask, torch.Tensor) else labels_mask, dtype=np.float64).sum())
+        return dict(cost=float(host_costs.astype(np.float64).sum()), weights_entropy=float(host[0]),
+                    weights_penalty=float(host[1]), num_labels=num_labels, batch_size=int(B))
+
     # ------------------------------------------------------------------------------
     # reference-facing methods (numpy in, numpy out)
     # ------------------------------------------------------------------------------

@@ -37,11 +37,13 @@ class NpzAudioDataset(object):
 
 class Data(object):
     def __init__(self, dataset_filename=None, path=None, name_mapping=None, add_eos=True, prepend_eos=False,
-                 batch_size=10, sort_k_batches=None, max_length=None, **unused):
+                 batch_size=10, validation_batch_size=None, sort_k_batches=None, max_length=None, **unused):
         self.path = path or dataset_filename
         self.name_mapping = name_mapping or {}
         self.add_eos, self.prepend_eos = add_eos, prepend_eos
         self.batch_size, self.sort_k_batches, self.max_length = batch_size, sort_k_batches, max_length
+        # lvsr/datasets/__init__.py: the batch size of the validation stream, batch_size when not given
+        self.validation_batch_size = validation_batch_size or batch_size
         self.info_dataset = self.get_dataset("train")
         self.num_labels = self.info_dataset.num_labels
         self.num_features = self.info_dataset.num_features
@@ -65,16 +67,17 @@ class Data(object):
                 continue
             yield ex
 
-    def batches(self, part, shuffle=True, seed=1):
-        """Padded, masked, time-major batches (lvsr/datasets/__init__.py:281-309); sort_k_batches groups
-        utterances of similar length."""
+    def batches(self, part, shuffle=True, seed=1, batch_size=None):
+        """Padded, masked, time-major batches (lvsr/datasets/__init__.py:281-309) of batch_size (default: the data's)
+        utterances; sort_k_batches groups utterances of similar length."""
         exs = list(self.examples(part, shuffle=shuffle, seed=seed))
+        bs = batch_size or self.batch_size
         k = self.sort_k_batches or 1
         out = []
-        for s in range(0, len(exs), self.batch_size * k):
-            chunk = sorted(exs[s:s + self.batch_size * k], key=lambda e: len(e["recordings"]))
-            for b in range(0, len(chunk), self.batch_size):
-                out.append(chunk[b:b + self.batch_size])
+        for s in range(0, len(exs), bs * k):
+            chunk = sorted(exs[s:s + bs * k], key=lambda e: len(e["recordings"]))
+            for b in range(0, len(chunk), bs):
+                out.append(chunk[b:b + bs])
         for group in out:
             B = len(group)
             T = max(len(e["recordings"]) for e in group)

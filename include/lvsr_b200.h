@@ -204,6 +204,16 @@ int lvsr_cost_matrix(lvsr_model* m, const float* attended_dev, const float* atte
                      int32_t L, float* costs_dev, float* weights_dev, float* energies_dev,
                      float* states_dev, float* weighted_averages_dev, void* stream);
 
+/* ---- alignment statistics of validation: weights_entropy and weights_penalty -------------------------------------
+ * (lvsr/expressions.py:4-25 as lvsr/main.py:385-388 monitors them) of the weights lvsr_cost_matrix writes,
+ * weights [L,B,T'], labels_mask [L,B] (NULL = all ones).  out_dev (float64, device):
+ *   out[0] = sum_{i,b} mask[i,b] sum_t w log(w + 1e-7)
+ *   out[1] = sum_{i>=1,b} mask[i,b] sum_t max(C_i[t] - C_{i-1}[t], 0),  C_i[t] = sum_{t'<=t} w[i,b,t']
+ * One launch; float64 sums in a fixed order, so the result is deterministic.  T' is limited by the shared memory of a
+ * CTA (8 bytes per position: about 29000 on an H100). */
+int lvsr_alignment_stats(lvsr_model* m, const float* weights_dev, const float* labels_mask_dev, int32_t L, int32_t B,
+                         int32_t Tp, double* out_dev, void* stream);
+
 /* ---- the BeamSearch state functions (libs/blocks/blocks/search.py:101-142) ---------
  * R rows (beam hypotheses); row r attends utterance row_utt[r] of `attended` [T',U,E]
  * (row_utt NULL = identity, U == R: the reference's replicated-context call).
@@ -325,6 +335,30 @@ int lvsr_train_apply_updates(lvsr_model* m, float* grads_dev, float gscale, cons
 int lvsr_train_gradient_norm(lvsr_model* m, float* norm_host);   /* total_gradient_norm of the last update (synchronises
                                                                     the handle's stream) */
 int lvsr_train_reset(lvsr_model* m);     /* zero the optimizer state, enqueued on the handle's stream after its updates */
+
+/* ---- adaptive clipping: AdaptiveClipping (lvsr/extensions.py:64-91), which lvsr/main.py:616-619 always installs ----
+ * While it is on, the StepClipping threshold of lvsr_train_apply_updates is the device value below, not
+ * gradient_threshold.  After the norm of update n (n = 1, 2, ..., the float32 value lvsr_train_gradient_norm reports)
+ * is reduced, the same kernel updates, in float64, with L = log(norm) and d = decay_rate:
+ *   mu  <- d mu  + (1 - d) L          mu2 <- d mu2 + (1 - d) L^2          sigma = sqrt(mu2 - mu^2)
+ *   c = min(burnin_period, n) / burnin_period
+ *   threshold of update n + 1 = min(c exp(mu + sigma) + (1 - c) initial_threshold, 5 initial_threshold)
+ * mu and mu2 start at 0 and update 1 clips with initial_threshold.  No launch, host copy or synchronisation is added
+ * to the update; every data-parallel rank reduces the same all-reduced norm and so gets the same threshold.
+ *   - a NaN norm makes the state and every later threshold NaN, as in the reference; a step clipped by a NaN threshold
+ *     is NaN, so RemoveNotFinite(0.0) zeroes every parameter.
+ *   - a zero norm (the reference raises on log(0)) leaves mu and mu2 unchanged; n still advances.
+ *   - rounding that makes mu2 - mu^2 negative gives sigma = 0.
+ * lvsr_train_set_adaptive_clipping turns it on (NULL: off) and resets the state; lvsr_train_reset resets it too.
+ * lvsr_train_clipping_threshold returns the threshold the next update will use (synchronises the handle's stream;
+ * an error while it is off). */
+typedef struct {
+  double initial_threshold;        /* thr_0: the StepClipping threshold (config['training']['gradient_threshold']) */
+  double decay_rate;               /* d (lvsr/main.py: 0.998)                                                     */
+  int32_t burnin_period;           /* (lvsr/main.py: 500)                                                          */
+} lvsr_adaptive_clipping;
+int lvsr_train_set_adaptive_clipping(lvsr_model* m, const lvsr_adaptive_clipping* cfg);
+int lvsr_train_clipping_threshold(lvsr_model* m, double* threshold_host);
 
 /* ---- adaptive weight noise (Graves 2011): apply_adaptive_noise, lvsr/graph.py:71-251, as lvsr/main.py:425-460
  * applies it to every parameter).  Each parameter p gets a log-variance ls2 of its shape, s2 = exp(2048 ls2).
