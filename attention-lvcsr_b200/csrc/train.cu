@@ -108,14 +108,22 @@ int make_tc_operand(Arena& ws, const float* src, int R, int cols, int ld, TcOper
   return transpose_split_tf32(src, R, cols, ld, out->hi, out->lo, st);
 }
 
+// Rows of the contraction one split of gemm_tn_tc adds up in its tensor-core accumulators, at most, and the most splits
+// the training step's arena holds partials for (TrainStep::run).  The error of a split grows with the rows it adds, far
+// faster than that of an fp32 FFMA sum: on the benchmarked training batch (T * B = 96,000 rows) the fork weight
+// gradients of encoder layers 1 and 2 were off by up to 1.4e-4 of their largest entry at 16,000 rows per split and by
+// 4e-5 at 2048 (H100 SXM, 700 W).  The partials are summed in fp32.
+constexpr int TC_SPLIT_ROWS = 2048, TC_MAX_SPLITS = 80;
+
 // C[Mo, N] (ldc) (+)= A^T B on the tensor cores: A, B given as K-major operands (rows a0.. / b0..), split-K over the
-// contraction (R) so that every SM gets a tile; partials are summed in a fixed order.  *splits_out (may be null) = the
-// partial products launched.
+// contraction (R) so that every SM gets a tile and no split adds more than TC_SPLIT_ROWS rows; partials are summed in a
+// fixed order.  *splits_out (may be null) = the partial products launched.
 int gemm_tn_tc(Arena& ws, const TcOperand& A, int a0, int Mo, const TcOperand& B, int b0, int N, float* C, int ldc,
                bool accumulate, cudaStream_t st, int* splits_out = nullptr) {
   ProfScope prof("gemm_tn", st);
   const int tiles = ceil_div(Mo, 128) * (N / (N % 256 == 0 ? 256 : 128));
-  const int want = std::max(1, std::min(32, ceil_div(device_sm_count(), tiles)));
+  const int want = std::min(TC_MAX_SPLITS, std::max({1, std::min(32, ceil_div(device_sm_count(), tiles)),
+                                                     ceil_div(A.Kpad, TC_SPLIT_ROWS)}));
   const int splits = gemm_tc_splits_launched(A.Kpad, want);
   if (splits_out) *splits_out = splits;
   ArenaMark mark{ws};
