@@ -3,6 +3,8 @@
 // Host-side orchestration only: which kernel runs when, on which buffers.  The
 // compiled-function seam it replaces is SURVEY.md section 8b tier b3
 // (libs/blocks/blocks/search.py:97-142; lvsr/bricks/recognizer.py:375-390,490-494).
+// The persistent decoder's hand-over buffers, their sentinel pre-fill, its plan and its debug switches are
+// dec_scan.cu's (run_dec_scan); lvsr_cost_matrix only chooses between it and the step-wise kernels.
 #include "lvsr_b200.h"
 
 #include <stdarg.h>
@@ -927,7 +929,7 @@ int lvsr_cost_matrix(lvsr_model* m, const float* attended, const float* attended
   for (int32_t& v : m->dec_plan) v = 0;
   LVSR_CUDA_OK(cudaMemsetAsync(m->status, 0, sizeof(unsigned), st));
   if (getenv("LVSR_NO_DEC_SCAN") == nullptr && !m->force_stepwise) {
-    DecScanArgs d = {};
+    DecScanInputs d = {};
     d.P = P; d.H = attended; d.maskH = attended_mask;
     d.filt = m->P(att_base(m) + "/conv1d.filters");     // null for content attention
     d.Wh = m->P(att_base(m) + "/handler.W");
@@ -939,117 +941,14 @@ int lvsr_cost_matrix(lvsr_model* m, const float* attended, const float* attended
     d.Ws = m->P(att_base(m) + "/state_trans/transform_states.W");
     d.FF = m->FF;
     d.labels = lab; d.lmask = labels_mask;
-    d.s_all = s_all; d.ctx_all = ctx_all; d.w0 = w0;
+    d.s_all = s_all; d.ctx_all = ctx_all; d.w0 = w0; d.w_all = weights_out;
     d.e_seq = energies_out; d.e_scratch = e_scratch;
     d.status = m->status;
     d.Tp = Tp; d.B = B; d.L = L; d.M = M; d.E = E; d.C = C; d.K = c.conv_num_filters; d.n = c.conv_n;
     d.normalizer = c.energy_normalizer;
     d.V = c.num_phonemes;
-    // per-step hand-over buffers of the data-flow decoder; everything another CTA polls starts
-    // as the sentinel (0xFF bytes)
-    d.w_all = weights_out ? weights_out : ws.f32((size_t)L * B * Tp);
-    d.q_all = ws.f32((size_t)L * B * M);
-    d.hr_all = ws.f32((size_t)L * B * C);
-    d.rowpos_all = ws.f32((size_t)(L + 1) * B);
-    LVSR_CHECK(d.w_all && d.q_all && d.hr_all && d.rowpos_all,
-               "out of device memory (decoder scan workspace)");
-    LVSR_CUDA_OK(cudaMemsetAsync(d.w_all, 0xFF, (size_t)L * B * Tp * sizeof(float), st));
-    LVSR_CUDA_OK(cudaMemsetAsync(d.q_all, 0xFF, (size_t)L * B * M * sizeof(float), st));
-    LVSR_CUDA_OK(cudaMemsetAsync(d.hr_all, 0xFF, (size_t)L * B * C * sizeof(float), st));
-    LVSR_CUDA_OK(cudaMemsetAsync(d.rowpos_all + B, 0xFF, (size_t)L * B * sizeof(float), st));
-    LVSR_CUDA_OK(cudaMemsetAsync(d.rowpos_all, 0, (size_t)B * sizeof(float), st));
-    LVSR_CUDA_OK(cudaMemsetAsync(s_all + (size_t)B * C, 0xFF, (size_t)L * B * C * sizeof(float), st));
-    LVSR_CUDA_OK(cudaMemsetAsync(ctx_all, 0xFF, (size_t)L * B * E * sizeof(float), st));
-    const bool trace = getenv("LVSR_DEC_TRACE") != nullptr;
-    if (trace) {
-      d.trace = reinterpret_cast<unsigned long long*>(ws.i64((size_t)2 * L * 9 + (size_t)L * 12 + (size_t)L * B));
-      LVSR_CUDA_OK(cudaMemsetAsync(d.trace, 0, ((size_t)2 * L * 9 + (size_t)L * 12 + (size_t)L * B) * 8, st));
-    }
-    int supported = 0, grid = 0, max_clusters = 0;
-    if (int rc = dec_scan_try(d, !content_attention(m), &supported, &grid, &max_clusters, st)) return rc;
-    scanned = supported != 0;
-    int32_t* p = m->dec_plan;
-    p[LVSR_PLAN_MAX_CLUSTERS] = max_clusters;
-    if (scanned) {
-      p[LVSR_PLAN_RAN] = 1;
-      p[LVSR_PLAN_KERNEL] = content_attention(m) ? LVSR_PLAN_DEC_CONTENT : d.wh_rows != 16 ? LVSR_PLAN_DEC_SCAN_COMPACT
-                                                                                            : LVSR_PLAN_DEC_SCAN;
-      p[LVSR_PLAN_CS] = d.cs; p[LVSR_PLAN_GRID] = grid; p[LVSR_PLAN_NISL] = d.nisl; p[LVSR_PLAN_NRG] = d.nrg;
-      p[LVSR_PLAN_NCG] = d.ncg; p[LVSR_PLAN_NC1] = d.nc1; p[LVSR_PLAN_NC2] = d.nc2; p[LVSR_PLAN_NC3] = d.nc3;
-      p[LVSR_PLAN_TC_CAP] = d.tc_cap; p[LVSR_PLAN_WH_ROWS] = d.wh_rows; p[LVSR_PLAN_RED_ALIAS] = d.red_alias;
-    }
-    if (scanned && getenv("LVSR_DEC_CHECK") != nullptr) {
-      // debug post-condition: the launch reported success and every hand-over word was written
-      LVSR_CUDA_OK(cudaStreamSynchronize(st));
-      unsigned hst = 0;
-      LVSR_CUDA_OK(cudaMemcpy(&hst, m->status, sizeof(hst), cudaMemcpyDeviceToHost));
-      LVSR_CHECK(hst == 0, "LVSR_DEC_CHECK: persistent decoder launch status %u (2 = a value never arrived, "
-                 "3 = launched without its cluster shape)", hst);
-      struct { const char* name; const float* p; size_t n; } bufs[] = {
-          {"weights", d.w_all, (size_t)L * B * Tp}, {"queries", d.q_all, (size_t)L * B * M},
-          {"reset-gated states", d.hr_all, (size_t)L * B * C}, {"states", s_all, (size_t)(L + 1) * B * C},
-          {"weighted averages", ctx_all, (size_t)L * B * E},
-          {"row positions", d.rowpos_all, c.prior_type == LVSR_PRIOR_EXPANDING ? (size_t)B : (size_t)(L + 1) * B}};
-      for (auto& b : bufs) {
-        long long left = 0;
-        if (int rc = count_sentinels(b.p, (long long)b.n, &left, st)) return rc;
-        // the query of step L is never needed; everything else must have been produced
-        LVSR_CHECK(left == 0, "LVSR_DEC_CHECK: %lld sentinel words left in the %s buffer", left, b.name);
-      }
-    }
-    if (trace && scanned) {
-      std::vector<unsigned long long> h((size_t)2 * L * 9 + (size_t)L * 12 + (size_t)L * B);
-      LVSR_CUDA_OK(cudaMemcpyAsync(h.data(), d.trace, h.size() * 8, cudaMemcpyDeviceToHost, st));
-      LVSR_CUDA_OK(cudaStreamSynchronize(st));
-      const char* names[8] = {"A", "syncA", "B1", "sync1", "B2", "sync2", "B3", "sync3"};
-      for (int slot = 0; slot < 2; ++slot) {
-        double sum[8] = {0};
-        int n = 0;
-        for (int i = 1; i + 1 < L; ++i, ++n)
-          for (int j = 0; j < 8; ++j) sum[j] += (double)(h[((size_t)slot * L + i) * 9 + j + 1] - h[((size_t)slot * L + i) * 9 + j]);
-        fprintf(stderr, "[dec_scan trace] CTA %s:", slot == 0 ? "first" : "last");
-        for (int j = 0; j < 8; ++j) fprintf(stderr, " %s=%.2fus", names[j], n ? sum[j] / n * 1e-3 : 0.0);
-        fprintf(stderr, "\n");
-      }
-      {
-        const char* an[7] = {"stage", "conv", "energy", "stats", "ctx", "exchange", "combine"};
-        double sum[7] = {0};
-        int n = 0;
-        for (int i = 1; i + 1 < L; ++i, ++n)
-          for (int j = 0; j < 7; ++j)
-            sum[j] += (double)(h[(size_t)2 * L * 9 + (size_t)i * 8 + j + 1] - h[(size_t)2 * L * 9 + (size_t)i * 8 + j]);
-        fprintf(stderr, "[dec_scan trace] attention row 0:");
-        for (int j = 0; j < 7; ++j) fprintf(stderr, " %s=%.2fus", an[j], n ? sum[j] / n * 1e-3 : 0.0);
-        fprintf(stderr, "\n");
-      }
-      {
-        // gate tile of CTA 0: start of B1 -> x arrived -> products done -> cross-warp sums done -> end of B1
-        double sum[4] = {0};
-        int n = 0;
-        for (int i = 1; i + 1 < L; ++i, ++n) {
-          const unsigned long long* b = &h[(size_t)0 * L * 9 + (size_t)i * 9];
-          const unsigned long long* t = &h[(size_t)2 * L * 9 + (size_t)L * 8 + (size_t)i * 4];
-          sum[0] += (double)(t[0] - b[2]); sum[1] += (double)(t[1] - t[0]);
-          sum[2] += (double)(t[2] - t[1]); sum[3] += (double)(b[3] - t[2]);
-        }
-        {
-          // when each row's attention phase ended, relative to row 0 (mean over steps)
-          fprintf(stderr, "[dec_scan trace] end of attention vs row 0 (us):");
-          for (int r = 0; r < B; ++r) {
-            double acc = 0;
-            for (int i = 1; i + 1 < L; ++i) {
-              const unsigned long long* e = &h[(size_t)2 * L * 9 + (size_t)L * 12 + (size_t)i * B];
-              acc += (double)((long long)e[r] - (long long)e[0]);
-            }
-            fprintf(stderr, " %.1f", acc / (L - 2) * 1e-3);
-          }
-          fprintf(stderr, "\n");
-        }
-        fprintf(stderr, "[dec_scan trace] gate tile: wait_x=%.2fus products=%.2fus sums=%.2fus epilogue=%.2fus\n",
-                n ? sum[0] / n * 1e-3 : 0.0, n ? sum[1] / n * 1e-3 : 0.0, n ? sum[2] / n * 1e-3 : 0.0,
-                n ? sum[3] / n * 1e-3 : 0.0);
-      }
-    }
+    // the persistent decoder's buffers follow `merged` and the preprocess's split scratch in the workspace
+    if (int rc = run_dec_scan(d, !content_attention(m), ws, m->dec_plan, &scanned, st)) return rc;
   }
   const float* w_prev = w0;
   for (int i = 0; i < L && !scanned; ++i) {

@@ -18,13 +18,40 @@
 //     (query, context, h*r, next state, alignment, position statistic) lives in a per-step
 //     buffer the host fills with 0xFF bytes and is polled by its consumers until it is no longer
 //     the sentinel (common.cuh: ld_flow / st_flow).  One store + one load per hand-over.
+//     The host half of this protocol is run_dec_scan, at the end of this file.
 //   * the window statistics of the next step (mean / median position) ride on the attention
 //     exchange, so the windowing priors need no extra pass and no host round trip.
 #include <string.h>
 
 #include "attention_row.cuh"
+#include "model.h"
 
 namespace lvsr {
+
+// The kernels' argument: DecScanInputs' fields (kernels.h; same order and meaning), the hand-over buffers run_dec_scan
+// adds and the fields the planner derives.  Every buffer another CTA reads is per-step and pre-filled with the
+// sentinel, except step 0 (s_all[0], rowpos_all[0], w0): written once, polled by consumers.
+struct DecScanArgs {
+  const float *P, *H, *maskH;
+  const float *filt, *Wh, *v;
+  float v_bias;
+  PriorParams prior;
+  const float *Wb1, *Wstate, *Ws, *FF;
+  const long long* labels; const float* lmask;
+  float *s_all, *ctx_all; const float* w0;
+  float *w_all, *e_seq, *e_scratch;
+  float* q_all;                        // [L, B, M]
+  float* hr_all;                       // [L, B, C] reset-gated states (the only gate value that crosses CTAs)
+  float* rowpos_all;                   // [L+1, B]; rowpos_all[0] = 0
+  unsigned long long* trace;           // LVSR_DEC_TRACE stamps (layout: trace_att and below), or nullptr
+  unsigned* status;
+  int Tp, B, L, M, E, C, K, n, normalizer, V;
+  // derived by the planner
+  int cs, tc_cap, nrg, nc1, nc2, nc3;
+  int nisl, ncg;                       // nisl > 0: islands of <= 16 rows whose CTAs own their dense tiles
+  int wh_rows;                         // handler rows in shared memory: 16 (fast) or K (compact, long utterances)
+  int red_alias;                       // dense-tile scratch shares the attention reduction scratch (long utterances)
+};
 
 namespace {
 
@@ -205,6 +232,17 @@ __device__ __forceinline__ void dense_dispatch(int nq, const DenseIO& d, const f
   __trap();   // plan() only admits the shapes above
 }
 
+// LVSR_DEC_TRACE buffer: global_ns() stamps of one call, in four regions
+//   [2][L][DS_STAMPS]  DS_STAMP(j) of the first (slot 0) and the last CTA (slot 1), at each step's phase boundaries
+//   [L][8]             the attention row's stamps (AttRowIO::trace) of CTA 0's row, from trace_att(L)
+//   [L][4]             the DenseIO::tr stamps of CTA 0's gate tile, from trace_gate(L)
+//   [L][B]             the end of each row's attention phase (rank 0 of the row's cluster), from trace_rowend(L)
+constexpr int DS_STAMPS = 9;
+__host__ __device__ __forceinline__ size_t trace_att(int L) { return (size_t)2 * L * DS_STAMPS; }
+__host__ __device__ __forceinline__ size_t trace_gate(int L) { return trace_att(L) + (size_t)L * 8; }
+__host__ __device__ __forceinline__ size_t trace_rowend(int L) { return trace_att(L) + (size_t)L * 12; }
+__host__ __device__ __forceinline__ size_t trace_words(int L, int B) { return trace_rowend(L) + (size_t)L * B; }
+
 // COMPACT: the handler copy in shared memory holds only its K rows (a.wh_rows == K); a separate instantiation so that
 // the default kernel's energy loop stays exactly the unpredicated code (it is sensitive to every extra register).
 // LOC = false: content-only attention (no previous alignment, conv or handler; see attention_row).
@@ -302,7 +340,7 @@ __device__ __forceinline__ void dec_scan_body(const DecScanArgs& a) {
 #define DS_STAMP(j)                                                                         \
   do {                                                                                      \
     if (a.trace && trace_slot >= 0 && tid == 0)                                             \
-      a.trace[((size_t)trace_slot * a.L + i) * 9 + (j)] = global_ns();                      \
+      a.trace[((size_t)trace_slot * a.L + i) * DS_STAMPS + (j)] = global_ns();              \
   } while (0)
   for (int i = 0; i < a.L; ++i) {
 #ifdef LVSR_DEC_DEBUG
@@ -375,12 +413,12 @@ __device__ __forceinline__ void dec_scan_body(const DecScanArgs& a) {
       io.b0 = b0; io.b1 = b1; io.lo = lo; io.hi = hi;
       io.rowpos_out = (a.prior.type == LVSR_PRIOR_EXPANDING) ? nullptr : (rowpos_wr + row);
       io.rowpos_mode = a.prior.type;
-      io.trace = (a.trace && bid == 0) ? a.trace + (size_t)2 * a.L * 9 + (size_t)i * 8 : nullptr;
+      io.trace = (a.trace && bid == 0) ? a.trace + trace_att(a.L) + (size_t)i * 8 : nullptr;
       attention_row<COMPACT, LOC>(io, att, a.tc_cap, rank, cs, true, true, false);
     }
     DS_STAMP(1);
     if (a.trace && rank == 0 && tid == 0 && cluster_id < R)
-      a.trace[(size_t)2 * a.L * 9 + (size_t)a.L * 12 + (size_t)i * R + cluster_id] = global_ns();
+      a.trace[trace_rowend(a.L) + (size_t)i * R + cluster_id] = global_ns();
     DS_STAMP(2);
 
     // ================= phase B1: gates + candidate inputs ==============================
@@ -388,7 +426,7 @@ __device__ __forceinline__ void dec_scan_body(const DecScanArgs& a) {
       DenseIO d = {};
       d.X1 = ctx_cur; d.K1 = E; d.X2 = s_cur; d.K2 = C; d.R = Rlim; d.N = 3 * C; d.mode = EP_GATES; d.C = C;
       d.add = a.FF; d.arow = a.labels + (size_t)i * R; d.add_rows = a.V + 1; d.hr = hr_cur; d.loc = loc; d.ncu = a.nc2;
-      d.tr = (a.trace && bid == 0) ? a.trace + (size_t)2 * a.L * 9 + (size_t)a.L * 8 + (size_t)i * 4 : nullptr;
+      d.tr = (a.trace && bid == 0) ? a.trace + trace_gate(a.L) + (size_t)i * 4 : nullptr;
       dense_dispatch(a.nc1 / 8, d, w1s, ws1, r0, cgi * a.nc2, red);
     }
     DS_STAMP(3);
@@ -604,14 +642,136 @@ int plan_and_launch(DecScanArgs& a, bool loc, int* supported, int* grid, int* ma
   return 0;
 }
 
+__global__ void count_sentinels_kernel(const unsigned* p, long long n, unsigned long long* out) {
+  unsigned long long c = 0;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    c += p[i] == LVSR_SENTINEL ? 1u : 0u;
+  if (c) atomicAdd(out, c);
+}
+
+// *host_count = the words of p[0, n) that still hold the sentinel (synchronises)
+int count_sentinels(const float* p, long long n, long long* host_count, cudaStream_t stream) {
+  unsigned long long* d = nullptr;
+  LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&d), sizeof(*d)));
+  cudaMemsetAsync(d, 0, sizeof(*d), stream);
+  const int grid = (int)std::min<long long>(2048, (n + 255) / 256);
+  if (n > 0) count_sentinels_kernel<<<grid, 256, 0, stream>>>(reinterpret_cast<const unsigned*>(p), n, d);
+  unsigned long long h = 0;
+  cudaError_t e = cudaMemcpyAsync(&h, d, sizeof(h), cudaMemcpyDeviceToHost, stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
+  cudaFree(d);
+  if (e != cudaSuccess) return set_error("count_sentinels failed: %s", cudaGetErrorString(e));
+  *host_count = (long long)h;
+  return 0;
+}
+
+// LVSR_DEC_TRACE: the mean phase times over steps 1 .. L-2 on stderr
+int print_trace(const unsigned long long* trace, int L, int B, cudaStream_t st) {
+  std::vector<unsigned long long> h(trace_words(L, B));
+  LVSR_CUDA_OK(cudaMemcpyAsync(h.data(), trace, h.size() * 8, cudaMemcpyDeviceToHost, st));
+  LVSR_CUDA_OK(cudaStreamSynchronize(st));
+  // mean of h[hi + i * hs] - h[lo + i * ls] over the steps, in us
+  auto us = [&](size_t hi, size_t hs, size_t lo, size_t ls) {
+    double sum = 0;
+    int n = 0;
+    for (int i = 1; i + 1 < L; ++i, ++n) sum += (double)(h[hi + i * hs] - h[lo + i * ls]);
+    return n ? sum / n * 1e-3 : 0.0;
+  };
+  const char* names[8] = {"A", "syncA", "B1", "sync1", "B2", "sync2", "B3", "sync3"};
+  for (int slot = 0; slot < 2; ++slot) {
+    const size_t s0 = (size_t)slot * L * DS_STAMPS;
+    fprintf(stderr, "[dec_scan trace] CTA %s:", slot == 0 ? "first" : "last");
+    for (int j = 0; j < 8; ++j) fprintf(stderr, " %s=%.2fus", names[j], us(s0 + j + 1, DS_STAMPS, s0 + j, DS_STAMPS));
+    fprintf(stderr, "\n");
+  }
+  const char* an[7] = {"stage", "conv", "energy", "stats", "ctx", "exchange", "combine"};
+  fprintf(stderr, "[dec_scan trace] attention row 0:");
+  for (int j = 0; j < 7; ++j) fprintf(stderr, " %s=%.2fus", an[j], us(trace_att(L) + j + 1, 8, trace_att(L) + j, 8));
+  // when each row's attention phase ended, relative to row 0 (mean over steps)
+  fprintf(stderr, "\n[dec_scan trace] end of attention vs row 0 (us):");
+  for (int r = 0; r < B; ++r) {
+    double acc = 0;
+    for (int i = 1; i + 1 < L; ++i) {
+      const unsigned long long* e = &h[trace_rowend(L) + (size_t)i * B];
+      acc += (double)((long long)e[r] - (long long)e[0]);
+    }
+    fprintf(stderr, " %.1f", acc / (L - 2) * 1e-3);
+  }
+  // gate tile of CTA 0: start of B1 -> x arrived -> products done -> cross-warp sums done -> end of B1
+  const size_t g = trace_gate(L);
+  fprintf(stderr, "\n[dec_scan trace] gate tile: wait_x=%.2fus products=%.2fus sums=%.2fus epilogue=%.2fus\n",
+          us(g, 4, 2, DS_STAMPS), us(g + 1, 4, g, 4), us(g + 2, 4, g + 1, 4), us(3, DS_STAMPS, g + 2, 4));
+  return 0;
+}
+
 }  // namespace
 
-// Runs the persistent decoder if the shapes fit (*supported = 1, the derived fields of `a` and *grid describe the
-// launched plan); otherwise leaves the buffers untouched (*supported = 0) and the caller falls back to the per-step
-// kernels.  *max_clusters = the answer of the last occupancy query (0 if none was made).
-int dec_scan_try(DecScanArgs& a, bool location, int* supported, int* grid, int* max_clusters, cudaStream_t stream) {
-  ProfScope prof("dec_scan", stream);
-  return plan_and_launch(a, location, supported, grid, max_clusters, stream);
+// The host half of the hand-over protocol (file header).  The buffers come from `ws` in this order: w_all (unless the
+// caller gave one), q_all, hr_all, rowpos_all, the trace; their place in the workspace moves the decoder's step time.
+int run_dec_scan(const DecScanInputs& in, bool location, Arena& ws, int32_t* plan, bool* ran, cudaStream_t st) {
+  *ran = false;
+  const int Tp = in.Tp, B = in.B, L = in.L, M = in.M, E = in.E, C = in.C;
+  DecScanArgs a = {};
+  a.P = in.P; a.H = in.H; a.maskH = in.maskH; a.filt = in.filt; a.Wh = in.Wh; a.v = in.v; a.v_bias = in.v_bias;
+  a.prior = in.prior; a.Wb1 = in.Wb1; a.Wstate = in.Wstate; a.Ws = in.Ws; a.FF = in.FF;
+  a.labels = in.labels; a.lmask = in.lmask; a.s_all = in.s_all; a.ctx_all = in.ctx_all; a.w0 = in.w0;
+  a.e_seq = in.e_seq; a.e_scratch = in.e_scratch; a.status = in.status;
+  a.Tp = Tp; a.B = B; a.L = L; a.M = M; a.E = E; a.C = C; a.K = in.K; a.n = in.n; a.normalizer = in.normalizer;
+  a.V = in.V;
+  a.w_all = in.w_all ? in.w_all : ws.f32((size_t)L * B * Tp);
+  a.q_all = ws.f32((size_t)L * B * M);
+  a.hr_all = ws.f32((size_t)L * B * C);
+  a.rowpos_all = ws.f32((size_t)(L + 1) * B);
+  LVSR_CHECK(a.w_all && a.q_all && a.hr_all && a.rowpos_all, "out of device memory (decoder scan workspace)");
+  // Each buffer: `head` words of step 0 (s_all: the caller's initial states; rowpos_all: zeroed here), then `filled`
+  // words that start as the sentinel (0xFF bytes).  LVSR_DEC_CHECK counts the sentinels left in the first `checked`
+  // words: under the expanding prior no row position is handed over.
+  struct HandOver { const char* name; float* p; size_t head, filled, checked; bool zero_head; };
+  const HandOver bufs[] = {
+      {"weights", a.w_all, 0, (size_t)L * B * Tp, (size_t)L * B * Tp, false},
+      {"queries", a.q_all, 0, (size_t)L * B * M, (size_t)L * B * M, false},
+      {"reset-gated states", a.hr_all, 0, (size_t)L * B * C, (size_t)L * B * C, false},
+      {"row positions", a.rowpos_all, (size_t)B, (size_t)L * B,
+       a.prior.type == LVSR_PRIOR_EXPANDING ? (size_t)B : (size_t)(L + 1) * B, true},
+      {"states", a.s_all, (size_t)B * C, (size_t)L * B * C, (size_t)(L + 1) * B * C, false},
+      {"weighted averages", a.ctx_all, 0, (size_t)L * B * E, (size_t)L * B * E, false}};
+  for (const HandOver& b : bufs) {
+    LVSR_CUDA_OK(cudaMemsetAsync(b.p + b.head, 0xFF, b.filled * sizeof(float), st));
+    if (b.zero_head) LVSR_CUDA_OK(cudaMemsetAsync(b.p, 0, b.head * sizeof(float), st));
+  }
+  const bool trace = getenv("LVSR_DEC_TRACE") != nullptr;
+  if (trace) {
+    a.trace = reinterpret_cast<unsigned long long*>(ws.i64(trace_words(L, B)));
+    LVSR_CUDA_OK(cudaMemsetAsync(a.trace, 0, trace_words(L, B) * 8, st));
+  }
+  int supported = 0, grid = 0, max_clusters = 0;
+  {
+    ProfScope prof("dec_scan", st);
+    if (int rc = plan_and_launch(a, location, &supported, &grid, &max_clusters, st)) return rc;
+  }
+  plan[LVSR_PLAN_MAX_CLUSTERS] = max_clusters;
+  if (!supported) return 0;
+  *ran = true;
+  plan[LVSR_PLAN_RAN] = 1;
+  plan[LVSR_PLAN_KERNEL] = !location ? LVSR_PLAN_DEC_CONTENT
+                                      : a.wh_rows != 16 ? LVSR_PLAN_DEC_SCAN_COMPACT : LVSR_PLAN_DEC_SCAN;
+  plan[LVSR_PLAN_CS] = a.cs; plan[LVSR_PLAN_GRID] = grid; plan[LVSR_PLAN_NISL] = a.nisl; plan[LVSR_PLAN_NRG] = a.nrg;
+  plan[LVSR_PLAN_NCG] = a.ncg; plan[LVSR_PLAN_NC1] = a.nc1; plan[LVSR_PLAN_NC2] = a.nc2; plan[LVSR_PLAN_NC3] = a.nc3;
+  plan[LVSR_PLAN_TC_CAP] = a.tc_cap; plan[LVSR_PLAN_WH_ROWS] = a.wh_rows; plan[LVSR_PLAN_RED_ALIAS] = a.red_alias;
+  if (getenv("LVSR_DEC_CHECK") != nullptr) {
+    // debug post-condition: the launch reported success and every hand-over word was written
+    LVSR_CUDA_OK(cudaStreamSynchronize(st));
+    unsigned hst = 0;
+    LVSR_CUDA_OK(cudaMemcpy(&hst, a.status, sizeof(hst), cudaMemcpyDeviceToHost));
+    LVSR_CHECK(hst == 0, "LVSR_DEC_CHECK: persistent decoder launch status %u (2 = a value never arrived, "
+               "3 = launched without its cluster shape)", hst);
+    for (const HandOver& b : bufs) {
+      long long left = 0;
+      if (int rc = count_sentinels(b.p, (long long)b.checked, &left, st)) return rc;
+      LVSR_CHECK(left == 0, "LVSR_DEC_CHECK: %lld sentinel words left in the %s buffer", left, b.name);
+    }
+  }
+  return trace ? print_trace(a.trace, L, B, st) : 0;
 }
 
 }  // namespace lvsr

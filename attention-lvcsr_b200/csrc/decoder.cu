@@ -245,13 +245,6 @@ __global__ void gather_time_kernel(float* dst, const float* src, int Tout, int k
   }
 }
 
-__global__ void count_sentinels_kernel(const unsigned* p, long long n, unsigned long long* out) {
-  unsigned long long c = 0;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-    c += p[i] == LVSR_SENTINEL ? 1u : 0u;
-  if (c) atomicAdd(out, c);
-}
-
 __global__ void gather_rows_kernel(float* dst, const float* src, const int* idx, long long total, int N) {
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x)
     dst[i] = src[(long long)idx[i / N] * N + i % N];
@@ -374,19 +367,6 @@ int onehot_rows(float* dst, int R, int N, cudaStream_t stream) {
   if (total <= 0) return 0;
   onehot_rows_kernel<<<grid_for(total), 256, 0, stream>>>(dst, total, N);
   LVSR_LAUNCH_CHECK();
-  return 0;
-}
-int count_sentinels(const float* p, long long n, long long* host_count, cudaStream_t stream) {
-  unsigned long long* d = nullptr;
-  LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&d), sizeof(*d)));
-  cudaMemsetAsync(d, 0, sizeof(*d), stream);
-  if (n > 0) count_sentinels_kernel<<<grid_for(n), 256, 0, stream>>>(reinterpret_cast<const unsigned*>(p), n, d);
-  unsigned long long h = 0;
-  cudaError_t e = cudaMemcpyAsync(&h, d, sizeof(h), cudaMemcpyDeviceToHost, stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
-  cudaFree(d);
-  if (e != cudaSuccess) return set_error("count_sentinels failed: %s", cudaGetErrorString(e));
-  *host_count = (long long)h;
   return 0;
 }
 int gather_rows(float* dst, const float* src, const int* idx, int Rn, int N, cudaStream_t stream) {

@@ -219,7 +219,9 @@ int lm_gather(int* states, double* weights, float* add, const int* src_states, c
               const float* src_add, const int* idx, int Rn, int V, cudaStream_t stream);
 
 // ---- dec_scan.cu: persistent teacher-forced decoder -----------------------------------
-struct DecScanArgs {
+// The caller's inputs.  The hand-over protocol between the kernel's CTAs is dec_scan.cu's alone: run_dec_scan takes
+// the per-step hand-over buffers from the workspace and pre-fills them, s_all and ctx_all with the sentinel.
+struct DecScanInputs {
   const float *P, *H, *maskH;          // [Tp,B,M], [Tp,B,E], [Tp,B]
   const float *filt, *Wh, *v;          // attention constants
   float v_bias;
@@ -230,35 +232,26 @@ struct DecScanArgs {
   const float* FF;                     // [(V+1), 3C] fork(feedback(y)), gate columns first
   const long long* labels;             // [L, B]
   const float* lmask;                  // [L, B] or nullptr
-  // Every buffer another CTA reads is per-step and pre-filled with the sentinel (0xFF bytes) by
-  // the host, except step 0 (s_all[0], rowpos_all[0], w0): written once, polled by consumers.
   float* s_all;                        // [(L+1), B, C]; s_all[0] = initial states on entry
   float* ctx_all;                      // [L, B, E]
   const float* w0;                     // [B, Tp] initial alignment
-  float* w_all;                        // [L, B, Tp] alignments (the caller's weights output or scratch)
+  float* w_all;                        // [L, B, Tp] alignments: the caller's weights output, or nullptr (scratch)
   float* e_seq;                        // [L, B, Tp] or nullptr
   float* e_scratch;                    // [B, Tp]
-  float* q_all;                        // [L, B, M]
-  float* hr_all;                       // [L, B, C] reset-gated states (the only gate value that crosses CTAs)
-  float* rowpos_all;                   // [L+1, B]; rowpos_all[0] = 0
-  unsigned long long* trace;           // optional debug stamps, or nullptr
   unsigned* status;                    // launch status word (common.cuh: LVSR_FLOW_*), zeroed by the caller
   int Tp, B, L, M, E, C, K, n, normalizer;
   int V;                               // num_phonemes: the feedback table FF has V + 1 rows
-  // derived by the planner
-  int cs, tc_cap, nrg, nc1, nc2, nc3;
-  int nisl, ncg;                       // nisl > 0: islands of <= 16 rows whose CTAs own their dense tiles
-  int wh_rows;                         // handler rows in shared memory: 16 (fast) or K (compact, long utterances)
-  int red_alias;                       // dense-tile scratch shares the attention reduction scratch (long utterances)
 };
-int dec_scan_try(DecScanArgs& a, bool location, int* supported, int* grid, int* max_clusters, cudaStream_t stream);
+struct Arena;
+// Runs the persistent decoder when a plan fits (*ran = true, plan[LVSR_PLAN_*] describe it); else *ran = false, only
+// plan[LVSR_PLAN_MAX_CLUSTERS] is set and the caller runs the step-wise kernels.  location = false: content attention.
+int run_dec_scan(const DecScanInputs& in, bool location, Arena& ws, int32_t* plan, bool* ran, cudaStream_t stream);
 
 // small utility kernels
 int fill_f32(float* p, long long n, float v, cudaStream_t stream);
 int fill_i64(long long* p, long long n, long long v, cudaStream_t stream);
 int broadcast_rows(float* dst, const float* src, int R, int N, cudaStream_t stream);   // dst[r,:] = src[:]
 int onehot_rows(float* dst, int R, int N, cudaStream_t stream);                         // dst[r,:] = e_0
-int count_sentinels(const float* p, long long n, long long* host_count, cudaStream_t stream);   // synchronises
 int gather_rows(float* dst, const float* src, const int* idx, int Rn, int N, cudaStream_t stream);   // dst[r,:] = src[idx[r],:]
 int gather_i64(long long* dst, const long long* src, const int* idx, int Rn, long long inc, cudaStream_t stream);
 // k smallest of cost_so_far[r] + neglogp[r, v] over the rows of each segment (B/search.py:341-344)
