@@ -17,7 +17,7 @@ PRIORS = {"expanding": 0, "window_around_mean": 1, "window_around_median": 2}
 ATTENTION_TYPES = {"content_and_conv": 0, "content": 1}
 # slots of lvsr_model_decoder_plan's report (LVSR_PLAN_*) and the kernel names of its `kernel` slot (LVSR_PLAN_DEC_*)
 PLAN_SLOTS = ("ran", "kernel", "cs", "grid", "nisl", "nrg", "ncg", "nc1", "nc2", "nc3", "tc_cap", "wh_rows", "red_alias",
-              "att_cs", "max_clusters")
+              "att_cs", "max_clusters", "l2_evict_first_kb")
 PLAN_KERNELS = ("stepwise", "dec_scan", "dec_scan<COMPACT>", "dec_content")
 # slots of lvsr_model_encoder_plan's report (LVSR_ENC_*), the GEMM paths (LVSR_ENC_PATH_*), the operands of the
 # tensor-core projection (LVSR_ENC_OPS_*) and the scan kernels (LVSR_ENC_BIGRU_*)

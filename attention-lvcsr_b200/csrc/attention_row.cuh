@@ -19,7 +19,8 @@
 //     the next tile does not fit: at 512 threads the kernels run at the 128-register cap, the buffer
 //     was spilled right after its loads were issued (the spill store waits for the data, so nothing
 //     overlapped), and local memory lives in L2 because shared memory takes nearly all of L1;
-//   * context: 8 independent 16-byte loads in flight per thread up to the last position, 512 threads.
+//   * context: 8 independent 16-byte loads in flight per thread up to the last position, 512 threads;
+//   * L2HINT (persistent decoder): the P and H loads carry an L2 eviction policy (dec_scan.cu l2_plan).
 #pragma once
 #include <cuda_bf16.h>
 
@@ -89,7 +90,29 @@ struct AttRowIO {
   float* rowpos_out = nullptr;
   int rowpos_mode = 0;
   unsigned long long* trace = nullptr;   // optional [8] globaltimer stamps (debug)
+  // L2 eviction policies of the loads of P and H (l2_policy); read only by attention_row<..., L2HINT = true>
+  unsigned long long pol_p = 0, pol_h = 0;
 };
+
+// A cache policy for ld.global...L2::cache_hint: the fraction f of the lines (chosen by address, so the same lines on
+// every pass) keeps the normal eviction priority and the rest is evicted first (f = 0: every line evicted first).
+__device__ __forceinline__ unsigned long long l2_policy(float f) {
+  unsigned long long p;
+  if (f > 0.f) asm("createpolicy.fractional.L2::evict_normal.L2::evict_first.b64 %0, %1;\n" : "=l"(p) : "f"(f));
+  else asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;\n" : "=l"(p));
+  return p;
+}
+__device__ __forceinline__ float2 ldg_hint(const float2* p, unsigned long long pol) {
+  float2 v;
+  asm("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.f32 {%0, %1}, [%2], %3;\n" : "=f"(v.x), "=f"(v.y) : "l"(p), "l"(pol));
+  return v;
+}
+__device__ __forceinline__ float4 ldg_hint(const float4* p, unsigned long long pol) {
+  float4 v;
+  asm("ld.global.nc.L1::no_allocate.L2::cache_hint.v4.f32 {%0, %1, %2, %3}, [%4], %5;\n"
+      : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p), "l"(pol));
+  return v;
+}
 
 __device__ __forceinline__ unsigned long long att_global_ns() {
   unsigned long long t;
@@ -179,7 +202,7 @@ __device__ __forceinline__ void mma_bf16_16816(float (&d)[4], const uint32_t (&a
 
 // NTW: 8-column tiles of the matcher dimension per warp (M = 128 * NTW).  LOC = false (content-only attention):
 // e[t] = v . tanh(P[t] + q) on the FP32 pipes, same accumulator layout without the handler product.
-template <int NTW, bool COMPACT, bool LOC = true>
+template <int NTW, bool COMPACT, bool LOC, bool L2HINT>
 __device__ __forceinline__ void att_energies(const AttRowIO& a, const AttSmem& s, int nt, int t0, int tc_cap) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int g = lane >> 2, tig = lane & 3;
@@ -214,8 +237,15 @@ __device__ __forceinline__ void att_energies(const AttRowIO& a, const AttSmem& s
     const int r0 = min(tile * 16 + g, nt - 1), r1 = min(tile * 16 + g + 8, nt - 1);   // clamp: tail rows are discarded
 #pragma unroll
     for (int j = 0; j < NTW; ++j) {
-      dst[j][0] = __ldg(reinterpret_cast<const float2*>(pbase + r0 * prow + j * 8));
-      dst[j][1] = __ldg(reinterpret_cast<const float2*>(pbase + r1 * prow + j * 8));
+      const float2* p0 = reinterpret_cast<const float2*>(pbase + r0 * prow + j * 8);
+      const float2* p1 = reinterpret_cast<const float2*>(pbase + r1 * prow + j * 8);
+      if constexpr (L2HINT) {
+        dst[j][0] = ldg_hint(p0, a.pol_p);
+        dst[j][1] = ldg_hint(p1, a.pol_p);
+      } else {
+        dst[j][0] = __ldg(p0);
+        dst[j][1] = __ldg(p1);
+      }
     }
   };
   for (int tile = 0; tile < ntile; ++tile) {
@@ -270,7 +300,9 @@ __device__ __forceinline__ float gmax_of(const float* xs, int cs) {
 // `entry_wait_pending`: the caller issued barrier.cluster.arrive at kernel entry.
 // LOC = false: content-only attention (B/bricks/attention.py:259-414): no previous alignment, conv or handler, so in
 // flow mode only the query is waited for; e_out receives zeros (the reference keeps no energies for it).
-template <bool COMPACT = false, bool LOC = true>
+// L2HINT: the loads of P and H carry the L2 policies a.pol_p / a.pol_h (the persistent decoder when l2_plan turns the
+// hints on); otherwise plain loads.
+template <bool COMPACT = false, bool LOC = true, bool L2HINT = false>
 __device__ __forceinline__ void attention_row(const AttRowIO& a, float* smem, int tc_cap, int rank, int cs,
                                               bool constants_staged, bool flow,
                                               bool entry_wait_pending) {
@@ -385,9 +417,9 @@ __device__ __forceinline__ void attention_row(const AttRowIO& a, float* smem, in
     for (int l = tid; l < nt * lines; l += NT)
       asm volatile("prefetch.global.L2 [%0];\n" ::"l"(pb + (long long)(l / lines) * U * M + (l % lines) * 32));
   }
-  if (M == 512) att_energies<4, COMPACT, LOC>(a, s, nt, t0, tc_cap);
-  else if (M == 256) att_energies<2, COMPACT, LOC>(a, s, nt, t0, tc_cap);
-  else att_energies<1, COMPACT, LOC>(a, s, nt, t0, tc_cap);
+  if (M == 512) att_energies<4, COMPACT, LOC, L2HINT>(a, s, nt, t0, tc_cap);
+  else if (M == 256) att_energies<2, COMPACT, LOC, L2HINT>(a, s, nt, t0, tc_cap);
+  else att_energies<1, COMPACT, LOC, L2HINT>(a, s, nt, t0, tc_cap);
   __syncthreads();
   {
     // e[t] = the 16 warps' partial sums, added in a fixed order
@@ -459,8 +491,10 @@ __device__ __forceinline__ void attention_row(const AttRowIO& a, float* smem, in
       for (int t = g; t < nt; t += 8 * ng) {
         float4 h[8];
 #pragma unroll
-        for (int q = 0; q < 8; ++q)
-          h[q] = __ldg(reinterpret_cast<const float4*>(hbase + (long long)min(t + q * ng, nt - 1) * hstride));
+        for (int q = 0; q < 8; ++q) {
+          const float4* p = reinterpret_cast<const float4*>(hbase + (long long)min(t + q * ng, nt - 1) * hstride);
+          h[q] = L2HINT ? ldg_hint(p, a.pol_h) : __ldg(p);
+        }
 #pragma unroll
         for (int q = 0; q < 8; ++q) {
           if (t + q * ng < nt) {

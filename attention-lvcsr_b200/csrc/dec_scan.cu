@@ -51,6 +51,8 @@ struct DecScanArgs {
   int nisl, ncg;                       // nisl > 0: islands of <= 16 rows whose CTAs own their dense tiles
   int wh_rows;                         // handler rows in shared memory: 16 (fast) or K (compact, long utterances)
   int red_alias;                       // dense-tile scratch shares the attention reduction scratch (long utterances)
+  int l2_hint;                         // l2_plan: 1 = the kernel instantiation whose P and H loads carry L2 policies:
+  float l2_fp, l2_fh;                  // these fractions of their lines keep the normal priority, the rest evict-first
 };
 
 namespace {
@@ -246,7 +248,9 @@ __host__ __device__ __forceinline__ size_t trace_words(int L, int B) { return tr
 // COMPACT: the handler copy in shared memory holds only its K rows (a.wh_rows == K); a separate instantiation so that
 // the default kernel's energy loop stays exactly the unpredicated code (it is sensitive to every extra register).
 // LOC = false: content-only attention (no previous alignment, conv or handler; see attention_row).
-template <bool COMPACT, bool LOC>
+// HINT: the loads of P and H carry the L2 policies of a.l2_fp / a.l2_fh (l2_plan); a separate instantiation, so that
+// the kernel without them is exactly the plain-load code.
+template <bool COMPACT, bool LOC, bool HINT>
 __device__ __forceinline__ void dec_scan_body(const DecScanArgs& a) {
   extern __shared__ __align__(16) float smem[];
   cg::cluster_group cluster = cg::this_cluster();
@@ -291,6 +295,7 @@ __device__ __forceinline__ void dec_scan_body(const DecScanArgs& a) {
   // a CTA's gate tile (B1) and candidate tile (B2) cover the same nc2 units of the same rows, so
   // the update gate, the candidate input and the state itself never leave its shared memory
   const bool in2 = cgi < a.ncg && cgi * a.nc2 < C, in1 = in2, in3 = cgi < a.ncg && cgi * a.nc3 < M;
+  const unsigned long long pol_p = HINT ? l2_policy(a.l2_fp) : 0, pol_h = HINT ? l2_policy(a.l2_fh) : 0;
 
   // ---- shared memory: [attention region][w1][w2][w3][red] -----------------------------
   float* att = smem;
@@ -414,7 +419,8 @@ __device__ __forceinline__ void dec_scan_body(const DecScanArgs& a) {
       io.rowpos_out = (a.prior.type == LVSR_PRIOR_EXPANDING) ? nullptr : (rowpos_wr + row);
       io.rowpos_mode = a.prior.type;
       io.trace = (a.trace && bid == 0) ? a.trace + trace_att(a.L) + (size_t)i * 8 : nullptr;
-      attention_row<COMPACT, LOC>(io, att, a.tc_cap, rank, cs, true, true, false);
+      io.pol_p = pol_p; io.pol_h = pol_h;
+      attention_row<COMPACT, LOC, HINT>(io, att, a.tc_cap, rank, cs, true, true, false);
     }
     DS_STAMP(1);
     if (a.trace && rank == 0 && tid == 0 && cluster_id < R)
@@ -459,11 +465,12 @@ __device__ __forceinline__ void dec_scan_body(const DecScanArgs& a) {
   cluster.sync();   // no CTA exits while a peer may still address its shared memory
 }
 
-template <bool COMPACT>
-__global__ void __launch_bounds__(DS_THREADS, 1) dec_scan_kernel(DecScanArgs a) { dec_scan_body<COMPACT, true>(a); }
+template <bool COMPACT, bool HINT>
+__global__ void __launch_bounds__(DS_THREADS, 1) dec_scan_kernel(DecScanArgs a) { dec_scan_body<COMPACT, true, HINT>(a); }
 
 // content-only attention: the persistent decoder hands over only the query between the dense phases and the attention
-__global__ void __launch_bounds__(DS_THREADS, 1) dec_content_kernel(DecScanArgs a) { dec_scan_body<false, false>(a); }
+template <bool HINT>
+__global__ void __launch_bounds__(DS_THREADS, 1) dec_content_kernel(DecScanArgs a) { dec_scan_body<false, false, HINT>(a); }
 
 using DecKernel = void (*)(DecScanArgs);
 
@@ -540,6 +547,55 @@ int read_dec_force(DecForce* f) {
   return 0;
 }
 
+int device_l2_bytes() {
+  static int l2[LVSR_MAX_DEVICES] = {0};
+  const int dev = current_device();
+  if (l2[dev] == 0) {
+    cudaDeviceGetAttribute(&l2[dev], cudaDevAttrL2CacheSize, dev);
+    if (l2[dev] <= 0) l2[dev] = 50 << 20;
+  }
+  return l2[dev];
+}
+
+// L2 priority of P and H.  Under the expanding prior every step reads its whole window of P (energies) and H (context)
+// again.  When the widest window of the two is larger than the L2, a cyclic read like this gets no hits from one step
+// to the next at the normal priority; it only evicts everything else the step touches (hand-over buffers, weights,
+// alignments, the kernel's stack).  Then every load of P and H is marked evict-first (DESIGN §5: keeping any share of
+// them at the normal priority measured slower, in proportion to the share).  Plain loads when the two fit in the L2,
+// and under the window-around priors, whose windows follow the alignment so that plain LRU keeps most of a step's
+// lines for the next.  LVSR_DEC_L2=off|<fP>,<fH> (DESIGN §7), read on every call, replaces the automatic plan: the
+// shares fP of P's and fH of H's lines keep the normal priority.  *kb: the KB of P and H per step loaded evict-first
+// (0: none).
+int l2_plan(DecScanArgs& a, int* kb) {
+  int positions = a.Tp;
+  if (a.prior.type == LVSR_PRIOR_EXPANDING) {
+    positions = 0;
+    for (int i = 0; i < a.L; ++i) {     // the kernel's window of step i
+      const double bb = fmax(0.0, fmin((double)(a.Tp - 1), a.prior.initial_begin + i * a.prior.min_speed));
+      const double ee = fmax(0.0, fmin((double)a.Tp, a.prior.initial_end + i * a.prior.max_speed));
+      positions = std::max(positions, (int)ceil(ee) - (int)floor(bb));
+    }
+  }
+  const double bp = (double)positions * a.B * a.M * 4, bh = (double)positions * a.B * a.E * 4;
+  bool on = false;
+  double fp = 0, fh = 0;
+  if (const char* s = getenv("LVSR_DEC_L2")) {
+    char tail = 0;
+    if (strcmp(s, "off") != 0) {
+      LVSR_CHECK(sscanf(s, "%lf,%lf%c", &fp, &fh, &tail) == 2 && fp >= 0 && fp <= 1 && fh >= 0 && fh <= 1,
+                 "LVSR_DEC_L2=%s: expected off or <fP>,<fH> with fractions in [0, 1]", s);
+      on = true;
+    }
+  } else {
+    on = a.prior.type == LVSR_PRIOR_EXPANDING && bp + bh > device_l2_bytes();
+  }
+  a.l2_hint = on ? 1 : 0;
+  a.l2_fp = (float)fp;
+  a.l2_fh = (float)fh;
+  *kb = on ? (int)(((1 - fp) * bp + (1 - fh) * bh) / 1024) : 0;
+  return 0;
+}
+
 int plan_and_launch(DecScanArgs& a, bool loc, int* supported, int* grid, int* max_clusters_seen, cudaStream_t stream) {
   *supported = 0;
   *grid = 0;
@@ -557,9 +613,13 @@ int plan_and_launch(DecScanArgs& a, bool loc, int* supported, int* grid, int* ma
     if (force.cs > 1 && ceil_div(a.Tp, force.cs) < 16) return 0;
     cs = force.cs;
   }
-  LVSR_CUDA_OK(cudaFuncSetAttribute(dec_scan_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-  LVSR_CUDA_OK(cudaFuncSetAttribute(dec_scan_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-  if (!loc) LVSR_CUDA_OK(cudaFuncSetAttribute(dec_content_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+  const bool hint = a.l2_hint != 0;
+  const DecKernel k_pad = hint ? dec_scan_kernel<false, true> : dec_scan_kernel<false, false>;
+  const DecKernel k_compact = hint ? dec_scan_kernel<true, true> : dec_scan_kernel<true, false>;
+  const DecKernel k_content = hint ? dec_content_kernel<true> : dec_content_kernel<false>;
+  LVSR_CUDA_OK(cudaFuncSetAttribute(k_pad, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+  LVSR_CUDA_OK(cudaFuncSetAttribute(k_compact, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+  if (!loc) LVSR_CUDA_OK(cudaFuncSetAttribute(k_content, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
   for (; cs >= 1; cs >>= 1) {
     if (force.cs && cs != force.cs) break;
     // prefer islands (grid = one cluster per row); fall back to one global island on all SMs
@@ -591,7 +651,7 @@ int plan_and_launch(DecScanArgs& a, bool loc, int* supported, int* grid, int* ma
     cfg.attrs = attr;
     cfg.numAttrs = 1;
     int max_clusters = 0;
-    const DecKernel kernel = !loc ? dec_content_kernel : a.wh_rows != 16 ? dec_scan_kernel<true> : dec_scan_kernel<false>;
+    const DecKernel kernel = !loc ? k_content : a.wh_rows != 16 ? k_compact : k_pad;
     if (cudaOccupancyMaxActiveClusters(&max_clusters, kernel, &cfg) != cudaSuccess) {
       cudaGetLastError();
       continue;
@@ -744,7 +804,8 @@ int run_dec_scan(const DecScanInputs& in, bool location, Arena& ws, int32_t* pla
     a.trace = reinterpret_cast<unsigned long long*>(ws.i64(trace_words(L, B)));
     LVSR_CUDA_OK(cudaMemsetAsync(a.trace, 0, trace_words(L, B) * 8, st));
   }
-  int supported = 0, grid = 0, max_clusters = 0;
+  int supported = 0, grid = 0, max_clusters = 0, l2_kb = 0;
+  if (int rc = l2_plan(a, &l2_kb)) return rc;
   {
     ProfScope prof("dec_scan", st);
     if (int rc = plan_and_launch(a, location, &supported, &grid, &max_clusters, st)) return rc;
@@ -758,6 +819,7 @@ int run_dec_scan(const DecScanInputs& in, bool location, Arena& ws, int32_t* pla
   plan[LVSR_PLAN_CS] = a.cs; plan[LVSR_PLAN_GRID] = grid; plan[LVSR_PLAN_NISL] = a.nisl; plan[LVSR_PLAN_NRG] = a.nrg;
   plan[LVSR_PLAN_NCG] = a.ncg; plan[LVSR_PLAN_NC1] = a.nc1; plan[LVSR_PLAN_NC2] = a.nc2; plan[LVSR_PLAN_NC3] = a.nc3;
   plan[LVSR_PLAN_TC_CAP] = a.tc_cap; plan[LVSR_PLAN_WH_ROWS] = a.wh_rows; plan[LVSR_PLAN_RED_ALIAS] = a.red_alias;
+  plan[LVSR_PLAN_L2_KB] = l2_kb;
   if (getenv("LVSR_DEC_CHECK") != nullptr) {
     // debug post-condition: the launch reported success and every hand-over word was written
     LVSR_CUDA_OK(cudaStreamSynchronize(st));

@@ -474,8 +474,8 @@ class SpeechRecognizer(object):
     def decoder_plan(self):
         """Plan of the last cost_matrix (lvsr_model_decoder_plan) as a dict: ran (the persistent decoder ran),
         kernel ("dec_scan", "dec_scan<COMPACT>", "dec_content" or "stepwise"), cs, grid, nisl, nrg, ncg, nc1, nc2,
-        nc3, tc_cap, wh_rows, red_alias, max_clusters (the planner's last occupancy answer) and att_cs (cluster
-        size of the last attention step)."""
+        nc3, tc_cap, wh_rows, red_alias, max_clusters (the planner's last occupancy answer), att_cs (cluster
+        size of the last attention step) and l2_evict_first_kb (KB of P and H per step loaded L2 evict-first; 0: none)."""
         import ctypes as C
         lib, h = _lib.load(), self._require_ready()
         out = (C.c_int32 * 16)()

@@ -133,7 +133,8 @@ enum {
   LVSR_PLAN_WH_ROWS = 11,     /* handler rows in shared memory: 16 (padded) or K (compact)                     */
   LVSR_PLAN_RED_ALIAS = 12,   /* 1: the dense tiles' scratch shares the attention reduction scratch            */
   LVSR_PLAN_ATT_CS = 13,      /* cluster size of the last attention step launch                                */
-  LVSR_PLAN_MAX_CLUSTERS = 14 /* answer of the planner's last occupancy query (0: none made)                   */
+  LVSR_PLAN_MAX_CLUSTERS = 14,/* answer of the planner's last occupancy query (0: none made)                   */
+  LVSR_PLAN_L2_KB = 15        /* KB of P and H per step the decoder loads with L2 evict-first (0: plain loads)  */
 };
 enum { LVSR_PLAN_STEPWISE = 0, LVSR_PLAN_DEC_SCAN = 1, LVSR_PLAN_DEC_SCAN_COMPACT = 2, LVSR_PLAN_DEC_CONTENT = 3 };
 int lvsr_model_decoder_plan(const lvsr_model* m, int32_t out[16]);
