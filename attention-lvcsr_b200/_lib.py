@@ -55,6 +55,7 @@ class LvsrConfig(C.Structure):
         ("prior_after", C.c_double),
         ("one_of_n_feedback", C.c_int32),
         ("attention_type", C.c_int32),
+        ("dec_stack", C.c_int32),
     ]
 
 

@@ -226,6 +226,14 @@ def allreduce_step_buffer(buf, n, local_batch, local_cost, dist):
     return buf[n], buf[n + 1]
 
 
+def check_trainable_net(net):
+    """Refuse a config['net'] the training step cannot run: a stacked decoder (dec_stack > 1) decodes and scores,
+    but has no backward pass through the RecurrentStack."""
+    if net.get("dec_stack", 1) != 1:
+        raise NotImplementedError("attention-lvcsr_b200: training with dec_stack=%d (a stacked decoder is inference "
+                                  "only: cost, analyze, beam search and sampling)" % net["dec_stack"])
+
+
 class GradientDescent(object):
     """``GradientDescent(cost=..., parameters=..., step_rule=...)`` of the reference with the recognizer in
     place of the symbolic cost (there is no graph to differentiate: the backward pass is part of the library).
@@ -254,6 +262,7 @@ class GradientDescent(object):
             # with an LM the reference's emitter is LMEmitter, whose costs are the fused readout's: inference only
             raise NotImplementedError("attention-lvcsr_b200: training with a language model (shallow fusion is "
                                       "inference only)")
+        check_trainable_net(getattr(recognizer, "net", {}))
         self.recognizer = recognizer
         self.step_rule = step_rule if step_rule is not None else CompositeRule([Scale(), RemoveNotFinite(0.0)])
         self.adaptive_noise = None

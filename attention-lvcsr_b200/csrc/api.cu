@@ -90,8 +90,14 @@ void build_param_table(lvsr_model* m) {
   const int E = m->E, C = c.dim_dec, M = c.dim_matcher, K = c.conv_num_filters, w = 2 * c.conv_n + 1;
   const int V = c.num_phonemes, Cfb = c.dim_feedback, Cpm = c.post_merge_dim;
   const std::string g = GEN, t = TR, a = att_base(m);
+  // dec_stack 2: every consumer of the states takes one more input, "states#1", and every consumer of the
+  // transition's sequences "inputs#1" / "gate_inputs#1" (the RecurrentStack's names for layer 1, recurrent.py:819-820)
+  const bool stack = c.dec_stack == 2;
   if (!c.one_of_n_feedback) add_param(m, g + "/readout/lookupfeedback/lookuptable.W", V + 1, Cfb);
-  if (c.use_states_for_readout) add_param(m, g + "/readout/merge/transform_states.W", C, Cpm);
+  if (c.use_states_for_readout) {
+    add_param(m, g + "/readout/merge/transform_states.W", C, Cpm);
+    if (stack) add_param(m, g + "/readout/merge/transform_states#1.W", C, Cpm);
+  }
   add_param(m, g + "/readout/merge/transform_weighted_averages.W", E, Cpm);
   add_param(m, g + "/readout/post_merge/bias.b", Cpm);
   add_param(m, g + "/readout/post_merge/mlp/linear_0.b", V);
@@ -100,10 +106,25 @@ void build_param_table(lvsr_model* m) {
   add_param(m, g + "/fork/fork_inputs.W", Cfb, C);
   add_param(m, g + "/fork/fork_gate_inputs.b", 2 * C);
   add_param(m, g + "/fork/fork_gate_inputs.W", Cfb, 2 * C);
-  add_param(m, t + "/transition.state_to_state", C, C);
-  add_param(m, t + "/transition.state_to_gates", C, 2 * C);
-  add_param(m, t + "/transition.initial_state", C);
+  if (stack) {
+    add_param(m, g + "/fork/fork_inputs#1.b", C);
+    add_param(m, g + "/fork/fork_inputs#1.W", Cfb, C);
+    add_param(m, g + "/fork/fork_gate_inputs#1.b", 2 * C);
+    add_param(m, g + "/fork/fork_gate_inputs#1.W", Cfb, 2 * C);
+  }
+  // AttentionRecurrent.children = [transition, attention, distribute]; RecurrentStack.children = transitions + forks,
+  // and fork_1 (outputs: layer 1's own sequence names) has no bias under skip_connections (recurrent.py:818-831)
+  for (int l = 0; l < c.dec_stack; ++l) {
+    add_param(m, dec_gru(m, l) + ".state_to_state", C, C);
+    add_param(m, dec_gru(m, l) + ".state_to_gates", C, 2 * C);
+    add_param(m, dec_gru(m, l) + ".initial_state", C);
+  }
+  if (stack) {
+    add_param(m, t + "/recurrentstack/fork_1/fork_inputs.W", C, C);
+    add_param(m, t + "/recurrentstack/fork_1/fork_gate_inputs.W", C, 2 * C);
+  }
   add_param(m, a + "/state_trans/transform_states.W", C, M);
+  if (stack) add_param(m, a + "/state_trans/transform_states#1.W", C, M);
   add_param(m, a + "/preprocess.b", M);
   add_param(m, a + "/preprocess.W", E, M);
   if (c.energy_normalizer != LVSR_NORM_SOFTMAX) add_param(m, a + "/energy_comp/linear.b", 1);
@@ -114,6 +135,10 @@ void build_param_table(lvsr_model* m) {
   }
   add_param(m, t + "/distribute/fork_inputs.W", E, C);
   add_param(m, t + "/distribute/fork_gate_inputs.W", E, 2 * C);
+  if (stack) {
+    add_param(m, t + "/distribute/fork_inputs#1.W", E, C);
+    add_param(m, t + "/distribute/fork_gate_inputs#1.W", E, 2 * C);
+  }
 }
 
 int copy2d(float* dst, int ld_dst, const float* src, int ld_src, int rows, int cols, cudaStream_t st) {
@@ -134,6 +159,19 @@ int fork_copy(lvsr_model* m, const ForkLayout& f, float* W, float* b, float* gra
   return 0;
 }
 
+// The weights that map a decoder state row to the attention's match space and to the readout's merge.  With
+// dec_stack 2 the state is [s0 | s1] and both bricks sum one Linear per state (lvsr/bricks/attention.py:103-104,
+// Merge of lvsr/bricks/recognizer.py:298-301): one product with the row-stacked weights finalize packs.
+static const float* att_state_weights(const lvsr_model* m) {
+  return m->cfg.dec_stack == 2 ? m->stack.Ws : m->P(att_base(m) + "/state_trans/transform_states.W");
+}
+static const float* readout_state_weights(const lvsr_model* m) {
+  return m->cfg.dec_stack == 2 ? m->stack.Wm : m->P(std::string(GEN) + "/readout/merge/transform_states.W");
+}
+static const float* initial_state_row(const lvsr_model* m) {
+  return m->cfg.dec_stack == 2 ? m->stack.h0 : m->P(dec_gru(m, 0) + ".initial_state");
+}
+
 // take_glimpses for R rows: q = s.W_state, window, attention step.
 struct Segments {           // batched beam search: hypotheses of one utterance = one segment (the reference's batch)
   const int* seg_start = nullptr; int nseg = 0; const int* seg_len = nullptr; const int* row_seg = nullptr;
@@ -148,7 +186,7 @@ int glimpses(lvsr_model* m, const float* H, const float* P, const float* maskH, 
   float* lohi = ws.f32((size_t)2 * R);
   LVSR_CHECK(q && win && lohi, "out of device memory (workspace)");
   DenseArgs d = {};
-  d.X1 = states; d.K1 = c.dim_dec; d.W1 = m->P(att_base(m) + "/state_trans/transform_states.W");
+  d.X1 = states; d.K1 = state_dim(m); d.W1 = att_state_weights(m);
   d.R = R; d.N = c.dim_matcher; d.mode = DENSE_PLAIN; d.out = q;
   if (int rc = dense_step(d, st)) return rc;
   WindowArgs wa = {};
@@ -181,15 +219,48 @@ int transition(lvsr_model* m, int R, const float* states, const float* ctx, cons
   LVSR_CHECK(z && hr && ai, "out of device memory (workspace)");
   DenseArgs g = {};
   g.X1 = ctx; g.K1 = m->E; g.W1 = m->Wd_cat;
-  g.X2 = states; g.K2 = C; g.W2 = m->P(std::string(TR) + "/transition.state_to_gates"); g.N2 = 2 * C;
+  g.X2 = states; g.K2 = C; g.W2 = m->P(dec_gru(m, 0) + ".state_to_gates"); g.N2 = 2 * C;
   g.add = m->FF; g.arow = outputs; g.add_rows = c.num_phonemes + 1; g.R = R; g.N = 3 * C; g.mode = DENSE_GATES;
   g.s = states; g.z = z; g.hr = hr; g.ai = ai; g.C = C;
   if (int rc = dense_step(g, st)) return rc;
   DenseArgs k = {};
-  k.X1 = hr; k.K1 = C; k.W1 = m->P(std::string(TR) + "/transition.state_to_state");
+  k.X1 = hr; k.K1 = C; k.W1 = m->P(dec_gru(m, 0) + ".state_to_state");
   k.add = ai; k.arow = nullptr; k.R = R; k.N = C; k.mode = DENSE_CAND;
   k.s = states; k.z = z; k.rmask = rmask; k.out = next_states; k.C = C;
   return dense_step(k, st);
+}
+
+// RecurrentStack.apply of dec_stack 2 for R wide state rows [s0 | s1] (row stride 2C): layer 0 is transition() on a
+// contiguous copy of s0, layer 1 then takes layer 0's new state through fork_1 (recurrent.py:925-950).
+static int stack_transition(lvsr_model* m, int R, const float* states, const float* ctx, const long long* outputs,
+                            const float* rmask, float* next_states, cudaStream_t st) {
+  const lvsr_config& c = m->cfg;
+  Arena& ws = m->ws;
+  const int C = c.dim_dec, S = 2 * C;
+  float* s0 = ws.f32((size_t)R * C);
+  float* s0n = ws.f32((size_t)R * C);
+  float* z = ws.f32((size_t)R * C);
+  float* hr = ws.f32((size_t)R * C);
+  float* ai = ws.f32((size_t)R * C);
+  LVSR_CHECK(s0 && s0n && z && hr && ai, "out of device memory (workspace)");
+  if (int rc = copy2d(s0, C, states, S, R, C, st)) return rc;
+  if (int rc = transition(m, R, s0, ctx, outputs, rmask, s0n, st)) return rc;
+  StackUpperArgs u = {};
+  u.R = R; u.C = C; u.E = m->E;
+  u.ctx = ctx; u.s0n = s0n; u.ld_s0n = C; u.s1 = states + C; u.ld_s1 = S;
+  u.outputs = outputs; u.ff_rows = c.num_phonemes + 1; u.rmask = rmask;
+  u.Wd = m->stack.Wd; u.FF = m->stack.FF; u.F = m->stack.F;
+  u.U = m->P(dec_gru(m, 1) + ".state_to_gates"); u.W = m->P(dec_gru(m, 1) + ".state_to_state");
+  u.z = z; u.hr = hr; u.ai = ai; u.out = next_states + C; u.ld_out = S;
+  if (int rc = stack_upper_step(u, st)) return rc;
+  return copy2d(next_states, S, s0n, C, R, C, st);
+}
+
+// compute_states of the decoder, whatever its depth
+static int dec_transition(lvsr_model* m, int R, const float* states, const float* ctx, const long long* outputs,
+                          const float* rmask, float* next_states, cudaStream_t st) {
+  if (m->cfg.dec_stack == 2) return stack_transition(m, R, states, ctx, outputs, rmask, next_states, st);
+  return transition(m, R, states, ctx, outputs, rmask, next_states, st);
 }
 
 int readout_merged(lvsr_model* m, int R, const float* states, const float* ctx, float* merged, cudaStream_t st) {
@@ -197,7 +268,7 @@ int readout_merged(lvsr_model* m, int R, const float* states, const float* ctx, 
   DenseArgs d = {};
   d.X1 = ctx; d.K1 = m->E; d.W1 = m->P(std::string(GEN) + "/readout/merge/transform_weighted_averages.W");
   if (c.use_states_for_readout) {
-    d.X2 = states; d.K2 = c.dim_dec; d.W2 = m->P(std::string(GEN) + "/readout/merge/transform_states.W");
+    d.X2 = states; d.K2 = state_dim(m); d.W2 = readout_state_weights(m);
     d.N2 = c.post_merge_dim;
   }
   d.R = R; d.N = c.post_merge_dim; d.mode = DENSE_PLAIN; d.out = merged;
@@ -265,10 +336,13 @@ size_t encoder_ws_bytes(const lvsr_model* m, int T, int B) {
 }
 size_t cost_ws_bytes(const lvsr_model* m, int Tp, int B, int L) {
   const lvsr_config& c = m->cfg;
-  size_t f = (size_t)Tp * B * c.dim_matcher + (size_t)2 * Tp * B * m->E + (size_t)(L + 1) * B * c.dim_dec + (size_t)L * B * m->E +
+  const size_t S = state_dim(m);
+  // a stacked step takes s0, s0' and the upper layer's z / hr / ai beside the lower layer's three [B, C] buffers
+  const size_t step_rows = 3 + (size_t)5 * (c.dec_stack - 1);
+  size_t f = (size_t)Tp * B * c.dim_matcher + (size_t)2 * Tp * B * m->E + (size_t)(L + 1) * B * S + (size_t)L * B * m->E +
              (size_t)4 * B * Tp + (size_t)L * B * c.post_merge_dim + (size_t)B * c.dim_matcher +
-             (size_t)L * B * (Tp + c.dim_matcher + c.dim_dec + 1) +
-             (size_t)3 * B * c.dim_dec + 4 * B + 64;
+             (size_t)L * B * (Tp + c.dim_matcher + S + 1) +
+             step_rows * B * c.dim_dec + 4 * B + 64;
   return f * sizeof(float) + (1 << 16);
 }
 
@@ -337,11 +411,13 @@ int lvsr_model_create(const lvsr_config* cfg, lvsr_model** out) {
   // the centre crop [:, :, n:-n] of the reference is EMPTY for n = 0 (lvsr/bricks/attention.py:109-110)
   LVSR_CHECK(content || cfg->conv_n >= 1, "conv_n must be >= 1 (got %d)", cfg->conv_n);
   LVSR_CHECK(cfg->num_phonemes >= 1 && cfg->num_phonemes <= 128, "num_phonemes out of range");
+  LVSR_CHECK(cfg->dec_stack >= 0 && cfg->dec_stack <= 2, "dec_stack %d unsupported (1 or 2)", cfg->dec_stack);
   int dev_count = 0;
   LVSR_CUDA_OK(cudaGetDeviceCount(&dev_count));
   LVSR_CHECK(dev_count > 0, "no CUDA device: the GPU path has no CPU fallback");
   lvsr_model* m = new lvsr_model();
   m->cfg = *cfg;
+  if (m->cfg.dec_stack == 0) m->cfg.dec_stack = 1;     // callers that predate the field zero-fill it
   if (content) {
     // SequenceContentAttention takes none of these (lvsr/bricks/recognizer.py:261-265): softmax weights over every
     // frame, which is the expanding window [0, length) that never moves
@@ -396,6 +472,7 @@ int lvsr_model_destroy(lvsr_model* m) {
   if (m->Wff_cat) cudaFree(m->Wff_cat);
   if (m->bff_cat) cudaFree(m->bff_cat);
   if (m->FF) cudaFree(m->FF);
+  if (m->stack.mem) cudaFree(m->stack.mem);
   if (m->status) cudaFree(m->status);
   if (m->enc_tiles) cudaFree(m->enc_tiles);
   if (m->enc_claims) cudaFree(m->enc_claims);
@@ -637,6 +714,18 @@ int finalize_on_stream(lvsr_model* m, cudaStream_t st, bool synchronise) {
     LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->Wff_cat), (size_t)c.dim_feedback * 3 * C * sizeof(float)));
     LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->bff_cat), (size_t)3 * C * sizeof(float)));
     LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->FF), (size_t)(c.num_phonemes + 1) * 3 * C * sizeof(float)));
+    if (c.dec_stack == 2) {
+      lvsr_model::Stack& s = m->stack;
+      const size_t n[8] = {(size_t)2 * C * c.dim_matcher, (size_t)2 * C * c.post_merge_dim, (size_t)2 * C,
+                           (size_t)m->E * 3 * C, (size_t)c.dim_feedback * 3 * C, (size_t)3 * C,
+                           (size_t)(c.num_phonemes + 1) * 3 * C, (size_t)C * 3 * C};
+      size_t total = 0;
+      for (size_t k : n) total += (k + 63) & ~(size_t)63;      // 256-byte aligned pieces
+      LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&s.mem), total * sizeof(float)));
+      float** piece[8] = {&s.Ws, &s.Wm, &s.h0, &s.Wd, &s.Wff, &s.bff, &s.FF, &s.F};
+      float* p = s.mem;
+      for (int i = 0; i < 8; ++i) { *piece[i] = p; p += (n[i] + 63) & ~(size_t)63; }
+    }
   }
   for (int l = 0; l < c.num_layers; ++l)
     for (int dir = 0; dir < 2; ++dir)
@@ -648,7 +737,7 @@ int finalize_on_stream(lvsr_model* m, cudaStream_t st, bool synchronise) {
   if (int rc = copy2d(m->Wd_cat + 2 * C, 3 * C, m->P(t + "/distribute/fork_inputs.W"), C, m->E, C, st)) return rc;
   LVSR_CUDA_OK(cudaMemsetAsync(m->Wb1, 0, (size_t)(m->E + C) * 3 * C * sizeof(float), st));
   if (int rc = copy2d(m->Wb1, 3 * C, m->Wd_cat, 3 * C, m->E, 3 * C, st)) return rc;
-  if (int rc = copy2d(m->Wb1 + (size_t)m->E * 3 * C, 3 * C, m->P(t + "/transition.state_to_gates"), 2 * C, C, 2 * C, st)) return rc;
+  if (int rc = copy2d(m->Wb1 + (size_t)m->E * 3 * C, 3 * C, m->P(dec_gru(m, 0) + ".state_to_gates"), 2 * C, C, 2 * C, st)) return rc;
   if (int rc = fork_copy(m, feedback_fork(c), m->Wff_cat, m->bff_cat, nullptr, st)) return rc;
   // tensor-core operands of the fork and preprocess weights (K-major fp16 head/tail planes or tf32 hi/lo pairs)
   m->use_tc = getenv("LVSR_NO_TC_GEMM") == nullptr;
@@ -668,6 +757,32 @@ int finalize_on_stream(lvsr_model* m, cudaStream_t st, bool synchronise) {
     GemmArgs ff = make_gemm(m->P(g + "/readout/lookupfeedback/lookuptable.W"), V + 1, Cfb, m->Wff_cat, 3 * C,
                             m->bff_cat, m->FF);
     if (int rc = gemm_bias(ff, st)) return rc;
+  }
+  if (c.dec_stack == 2) {
+    // the wide state's row-stacked weights [W ; W#1], both initial states, and layer 1's counterparts of Wd_cat / FF
+    lvsr_model::Stack& s = m->stack;
+    const int M = c.dim_matcher, Cpm = c.post_merge_dim;
+    const std::string a = att_base(m), r = t + "/recurrentstack";
+    if (int rc = copy2d(s.Ws, M, m->P(a + "/state_trans/transform_states.W"), M, C, M, st)) return rc;
+    if (int rc = copy2d(s.Ws + (size_t)C * M, M, m->P(a + "/state_trans/transform_states#1.W"), M, C, M, st)) return rc;
+    if (c.use_states_for_readout) {
+      if (int rc = copy2d(s.Wm, Cpm, m->P(g + "/readout/merge/transform_states.W"), Cpm, C, Cpm, st)) return rc;
+      if (int rc = copy2d(s.Wm + (size_t)C * Cpm, Cpm, m->P(g + "/readout/merge/transform_states#1.W"), Cpm, C, Cpm, st))
+        return rc;
+    }
+    if (int rc = copy2d(s.h0, C, m->P(dec_gru(m, 0) + ".initial_state"), C, 1, C, st)) return rc;
+    if (int rc = copy2d(s.h0 + C, C, m->P(dec_gru(m, 1) + ".initial_state"), C, 1, C, st)) return rc;
+    if (int rc = copy2d(s.Wd, 3 * C, m->P(t + "/distribute/fork_gate_inputs#1.W"), 2 * C, m->E, 2 * C, st)) return rc;
+    if (int rc = copy2d(s.Wd + 2 * C, 3 * C, m->P(t + "/distribute/fork_inputs#1.W"), C, m->E, C, st)) return rc;
+    if (int rc = copy2d(s.F, 3 * C, m->P(r + "/fork_1/fork_gate_inputs.W"), 2 * C, C, 2 * C, st)) return rc;
+    if (int rc = copy2d(s.F + 2 * C, 3 * C, m->P(r + "/fork_1/fork_inputs.W"), C, C, C, st)) return rc;
+    if (int rc = fork_copy(m, stack_feedback_fork(c), s.Wff, s.bff, nullptr, st)) return rc;
+    if (c.one_of_n_feedback) {
+      if (int rc = add_bias_rows(s.FF, s.Wff, s.bff, V + 1, 3 * C, st)) return rc;
+    } else {
+      GemmArgs ff = make_gemm(m->P(g + "/readout/lookupfeedback/lookuptable.W"), V + 1, Cfb, s.Wff, 3 * C, s.bff, s.FF);
+      if (int rc = gemm_bias(ff, st)) return rc;
+    }
   }
   m->v_bias = 0.f;
   if (c.energy_normalizer != LVSR_NORM_SOFTMAX) {
@@ -907,11 +1022,11 @@ int lvsr_cost_matrix(lvsr_model* m, const float* attended, const float* attended
   ArenaScope scope(m, st);
   const lvsr_config& c = m->cfg;
   Arena& ws = m->ws;
-  const int C = c.dim_dec, E = m->E, M = c.dim_matcher;
+  const int C = c.dim_dec, E = m->E, M = c.dim_matcher, S = state_dim(m);
   const long long* lab = reinterpret_cast<const long long*>(labels);
 
   float* P = ws.f32((size_t)Tp * B * M);
-  float* s_all = ws.f32((size_t)(L + 1) * B * C);
+  float* s_all = ws.f32((size_t)(L + 1) * B * S);
   float* ctx_all = wavg_out ? wavg_out : ws.f32((size_t)L * B * E);
   float* w0 = ws.f32((size_t)B * Tp);
   float* wpp[2] = {ws.f32((size_t)B * Tp), ws.f32((size_t)B * Tp)};   // step-wise fallback only
@@ -921,14 +1036,15 @@ int lvsr_cost_matrix(lvsr_model* m, const float* attended, const float* attended
              "out of device memory (decoder workspace)");
 
   if (int rc = lvsr_preprocess(m, attended, Tp, B, P, stream)) return rc;          // hoisted: B/bricks/attention.py:733-738
-  if (int rc = broadcast_rows(s_all, m->P(std::string(TR) + "/transition.initial_state"), B, C, st)) return rc;
+  if (int rc = broadcast_rows(s_all, initial_state_row(m), B, S, st)) return rc;
   if (int rc = onehot_rows(w0, B, Tp, st)) return rc;                               // lvsr/bricks/attention.py:215-222
   if (int rc = fill_f32(costs, (long long)L * B, 0.f, st)) return rc;
 
   bool scanned = false;
   for (int32_t& v : m->dec_plan) v = 0;
   LVSR_CUDA_OK(cudaMemsetAsync(m->status, 0, sizeof(unsigned), st));
-  if (getenv("LVSR_NO_DEC_SCAN") == nullptr && !m->force_stepwise) {
+  // the persistent decoder holds one GRU layer: a stacked decoder runs on the step-wise kernels
+  if (getenv("LVSR_NO_DEC_SCAN") == nullptr && !m->force_stepwise && c.dec_stack == 1) {
     DecScanInputs d = {};
     d.P = P; d.H = attended; d.maskH = attended_mask;
     d.filt = m->P(att_base(m) + "/conv1d.filters");     // null for content attention
@@ -937,7 +1053,7 @@ int lvsr_cost_matrix(lvsr_model* m, const float* attended, const float* attended
     d.v_bias = m->v_bias;
     d.prior = prior_of(c);
     d.Wb1 = m->Wb1;
-    d.Wstate = m->P(std::string(TR) + "/transition.state_to_state");
+    d.Wstate = m->P(dec_gru(m, 0) + ".state_to_state");
     d.Ws = m->P(att_base(m) + "/state_trans/transform_states.W");
     d.FF = m->FF;
     d.labels = lab; d.lmask = labels_mask;
@@ -955,11 +1071,11 @@ int lvsr_cost_matrix(lvsr_model* m, const float* attended, const float* attended
     float* w_i = weights_out ? weights_out + (size_t)i * B * Tp : wpp[i & 1];
     float* e_i = energies_out ? energies_out + (size_t)i * B * Tp : e_scratch;
     float* ctx_i = ctx_all + (size_t)i * B * E;
-    const float* s_i = s_all + (size_t)i * B * C;
+    const float* s_i = s_all + (size_t)i * B * S;
     ArenaMark mark{ws};   // per-step scratch is reusable (stream order): rewound at the end of every step
     if (int rc = glimpses(m, attended, P, attended_mask, Tp, B, nullptr, B, s_i, w_prev, nullptr, i, w_i, e_i, ctx_i, st)) return rc;
-    if (int rc = transition(m, B, s_i, ctx_i, lab + (size_t)i * B, labels_mask ? labels_mask + (size_t)i * B : nullptr,
-                            s_all + (size_t)(i + 1) * B * C, st)) return rc;
+    if (int rc = dec_transition(m, B, s_i, ctx_i, lab + (size_t)i * B, labels_mask ? labels_mask + (size_t)i * B : nullptr,
+                                s_all + (size_t)(i + 1) * B * S, st)) return rc;
     w_prev = w_i;
   }
   // the language model's cost rows in force before each label (sequence_generators.py:284-289), then fused below
@@ -976,7 +1092,7 @@ int lvsr_cost_matrix(lvsr_model* m, const float* attended, const float* attended
     const std::string g = GEN;
     bool acc = false;
     if (c.use_states_for_readout) {
-      GemmArgs a = make_gemm(s_all, R, C, m->P(g + "/readout/merge/transform_states.W"), c.post_merge_dim, nullptr, merged);
+      GemmArgs a = make_gemm(s_all, R, S, readout_state_weights(m), c.post_merge_dim, nullptr, merged);
       if (int rc = gemm_bias(a, st)) return rc;
       acc = true;
     }
@@ -990,7 +1106,7 @@ int lvsr_cost_matrix(lvsr_model* m, const float* attended, const float* attended
     if (int rc = readout_costs(r, st)) return rc;
   }
   if (states_out)
-    LVSR_CUDA_OK(cudaMemcpyAsync(states_out, s_all, (size_t)L * B * C * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    LVSR_CUDA_OK(cudaMemcpyAsync(states_out, s_all, (size_t)L * B * S * sizeof(float), cudaMemcpyDeviceToDevice, st));
   return 0;
 }
 
@@ -1002,7 +1118,7 @@ int lvsr_initial_states(lvsr_model* m, int32_t Tp, int32_t R, float* states, int
   LVSR_CHECK(states && outputs && wavg && weights && energies && step && Tp > 0 && R > 0, "initial_states: bad arguments");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const lvsr_config& c = m->cfg;
-  if (int rc = broadcast_rows(states, m->P(std::string(TR) + "/transition.initial_state"), R, c.dim_dec, st)) return rc;
+  if (int rc = broadcast_rows(states, initial_state_row(m), R, state_dim(m), st)) return rc;
   if (int rc = fill_i64(reinterpret_cast<long long*>(outputs), R, c.num_phonemes, st)) return rc;   // recognizer.py:286
   if (int rc = fill_f32(wavg, (long long)R * m->E, 0.f, st)) return rc;
   if (content_attention(m)) {             // B/bricks/attention.py:392-395: zero weights; no energies state
@@ -1072,7 +1188,8 @@ int lvsr_next_states(lvsr_model* m, const float* attended, const float* preproce
   }
   if (int rc = glimpses(m, attended, P, attended_mask, Tp, U, row_utt, R, states, weights,
                         reinterpret_cast<const long long*>(step), 0, next_weights, next_energies, next_wavg, st)) return rc;
-  if (int rc = transition(m, R, states, next_wavg, reinterpret_cast<const long long*>(outputs), nullptr, next_states, st)) return rc;
+  if (int rc = dec_transition(m, R, states, next_wavg, reinterpret_cast<const long long*>(outputs), nullptr, next_states, st))
+    return rc;
   return add_i64(reinterpret_cast<long long*>(next_step), reinterpret_cast<const long long*>(step), R, 1, st);
 }
 
@@ -1114,10 +1231,10 @@ int search_advance(lvsr_model* m, const float* attended, const float* preprocess
   ArenaScope scope(m, st);
   const lvsr_config& c = m->cfg;
   Arena& ws = m->ws;
-  const int C = c.dim_dec, E = m->E;
-  float* s_sel = ws.f32((size_t)Rn * C);
+  const int S = state_dim(m), E = m->E;
+  float* s_sel = ws.f32((size_t)Rn * S);
   LVSR_CHECK(s_sel, "out of device memory (search workspace)");
-  if (int rc = gather_rows(s_sel, states, parent, Rn, C, st)) return rc;
+  if (int rc = gather_rows(s_sel, states, parent, Rn, S, st)) return rc;
   if (c.prior_type == LVSR_PRIOR_EXPANDING) {
     if (int rc = gather_rows(n_wavg, wavg, parent, Rn, E, st)) return rc;
     if (int rc = gather_rows(n_weights, new_weights, parent, Rn, Tp, st)) return rc;
@@ -1135,7 +1252,7 @@ int search_advance(lvsr_model* m, const float* attended, const float* preprocess
     if (int rc = glimpses(m, attended, preprocessed, attended_mask, Tp, U, row_utt, Rn, s_sel, w_sel, st_sel, 0, n_weights,
                           n_energies, n_wavg, st, sg)) return rc;
   }
-  if (int rc = transition(m, Rn, s_sel, n_wavg, symbols, nullptr, n_states, st)) return rc;
+  if (int rc = dec_transition(m, Rn, s_sel, n_wavg, symbols, nullptr, n_states, st)) return rc;
   return gather_i64(n_step, step, parent, Rn, 1, st);
 }
 

@@ -218,6 +218,28 @@ int lm_path(const LmFst& f, int L, int B, const long long* labels, const float* 
 int lm_gather(int* states, double* weights, float* add, const int* src_states, const double* src_weights,
               const float* src_add, const int* idx, int Rn, int V, cudaStream_t stream);
 
+// ---- dec_stack.cu: upper GRU of a two-layer RecurrentStack with skip connections (dec_stack 2) -------------------
+// One step of layer 1 for R rows (libs/blocks/blocks/bricks/recurrent.py:925-950, B/bricks/recurrent.py:608-620):
+//   gate inputs  g = ctx.Wd[:, :2C] + FF[y, :2C] + s0n.F[:, :2C] + s1.U        (U = state_to_gates [C, 2C])
+//   inputs       a = ctx.Wd[:, 2C:] + FF[y, 2C:] + s0n.F[:, 2C:]
+//   z, r = sigmoid(g); c = tanh((s1 * r).W + a); s1' = c z + s1 (1 - z), blended by the row mask
+// s0n is layer 0's new state of the same step.  The states live in the wide rows [s0 | s1]: s1, s0n and out carry
+// their own row strides.  Two launches (gates, candidate) of the dense tiling of decoder.cu.
+struct StackUpperArgs {
+  int R, C, E;
+  const float* ctx;                 // [R, E] glimpses of the step
+  const float* s0n; int ld_s0n;     // [R, C] layer 0's new state
+  const float* s1; int ld_s1;       // [R, C] layer 1's state
+  const long long* outputs;         // [R] fed-back symbols: rows of FF (clamped into [0, ff_rows))
+  int ff_rows;
+  const float* rmask;               // [R] or nullptr
+  const float *Wd, *FF, *F;         // [E, 3C], [ff_rows, 3C], [C, 3C]: gate columns first, then the inputs
+  const float *U, *W;               // state_to_gates [C, 2C], state_to_state [C, C]
+  float *z, *hr, *ai;               // [R, C] scratch each
+  float* out; int ld_out;           // [R, C] layer 1's new state
+};
+int stack_upper_step(const StackUpperArgs& a, cudaStream_t stream);
+
 // ---- dec_scan.cu: persistent teacher-forced decoder -----------------------------------
 // The caller's inputs.  The hand-over protocol between the kernel's CTAs is dec_scan.cu's alone: run_dec_scan takes
 // the per-step hand-over buffers from the workspace and pre-fills them, s_all and ctx_all with the sentinel.

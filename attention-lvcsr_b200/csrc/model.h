@@ -120,6 +120,19 @@ struct lvsr_model {
   float* Wff_cat = nullptr;         // [Cfb, 3C] (feedback_fork)
   float* bff_cat = nullptr;         // [3C]
   float* FF = nullptr;              // [(V+1), 3C] = lookup . Wff_cat + bff_cat
+  // dec_stack 2 (finalize; all inside stack_mem): the attention and the readout see the wide state [s0 | s1] through
+  // row-stacked weights, and the upper layer's packed inputs mirror Wd_cat / FF of the lower one
+  struct Stack {
+    float* mem = nullptr;           // the one allocation of the buffers below
+    float* Ws = nullptr;            // [2C, M]   state_trans/transform_states.W ; transform_states#1.W
+    float* Wm = nullptr;            // [2C, Cpm] readout/merge/transform_states.W ; transform_states#1.W
+    float* h0 = nullptr;            // [2C]      initial_state of both layers
+    float* Wd = nullptr;            // [E, 3C]   distribute [fork_gate_inputs#1 | fork_inputs#1]
+    float* Wff = nullptr;           // [Cfb, 3C] generator fork [fork_gate_inputs#1 | fork_inputs#1]
+    float* bff = nullptr;           // [3C]
+    float* FF = nullptr;            // [(V+1), 3C] = feedback . Wff + bff
+    float* F = nullptr;             // [C, 3C]   recurrentstack/fork_1 [fork_gate_inputs | fork_inputs] (no bias)
+  } stack;
   // dense-projection weights as the tensor-core GEMM reads them (wgmma path); empty = SIMT path
   std::vector<TcWeights> Wcat_tc;
   TcWeights Wp_tc;
@@ -200,6 +213,15 @@ static inline bool content_attention(const lvsr_model* m) { return m->cfg.attent
 // brick path of the attention's parameters
 static inline std::string att_base(const lvsr_model* m) { return content_attention(m) ? CONT : ATT; }
 
+// Width of a decoder state row: dec_stack * C ([s0 | s1] with two layers; lvsr_model_create reads dec_stack 0 as 1)
+static inline int state_dim(const lvsr_model* m) { return m->cfg.dec_stack * m->cfg.dim_dec; }
+// brick path of the decoder GRU of stack level l: "transition", or inside the RecurrentStack "transition_<l>#<l>"
+// (RecurrentStack renames its layers, libs/blocks/blocks/bricks/recurrent.py:819-820)
+static inline std::string dec_gru(const lvsr_model* m, int level) {
+  if (m->cfg.dec_stack == 1) return std::string(TR) + "/transition";
+  return std::string(TR) + "/recurrentstack/transition_" + std::to_string(level) + "#" + std::to_string(level);
+}
+
 static inline std::string enc_base(int l, int dir) {
   char buf[128];
   snprintf(buf, sizeof(buf), "/recognizer/encoder/bidir%d/%s", l, dir ? "backward" : "forward");
@@ -274,6 +296,10 @@ static inline ForkLayout encoder_fork(const lvsr_config& c, int l, int dir) {
 // fork(feedback(y)) in Wff_cat / bff_cat: [gate_inputs 2C | inputs C]
 static inline ForkLayout feedback_fork(const lvsr_config& c) {
   return {std::string(GEN) + "/fork", c.dim_feedback, 3 * c.dim_dec, {{"fork_gate_inputs", 0, 2 * c.dim_dec}, {"fork_inputs", 2 * c.dim_dec, c.dim_dec}}};
+}
+// the same for the upper layer of dec_stack 2 (outputs "inputs#1", "gate_inputs#1"), in Stack::Wff / Stack::bff
+static inline ForkLayout stack_feedback_fork(const lvsr_config& c) {
+  return {std::string(GEN) + "/fork", c.dim_feedback, 3 * c.dim_dec, {{"fork_gate_inputs#1", 0, 2 * c.dim_dec}, {"fork_inputs#1", 2 * c.dim_dec, c.dim_dec}}};
 }
 
 static inline int check_ready(lvsr_model* m) {

@@ -69,7 +69,7 @@ int lvsr_beam_search_many(lvsr_model* m, const float* attended, const float* pre
              "beam_search_many: bad arguments");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const lvsr_config& c = m->cfg;
-  const int C = c.dim_dec, E = m->E, V = c.num_phonemes, k = beam_size;
+  const int C = state_dim(m), E = m->E, V = c.num_phonemes, k = beam_size;     // C: floats of a state row
   const int Rmax = U * k;
 
   // ---- device state: two sets of (states, weights, step) + the per-step outputs, one allocation -----------------

@@ -556,6 +556,9 @@ extern "C" {
 int lvsr_train_cost_and_grads(lvsr_model* m, const float* x, const float* mask, const int64_t* labels, const float* lmask,
                               int32_t T, int32_t B, int32_t L, float gscale, float* cost_out, float* grads, void* stream) {
   DeviceGuard device_guard(m);
+  LVSR_CHECK(!m || m->cfg.dec_stack == 1,
+             "train_cost_and_grads: a stacked decoder (dec_stack %d) is inference only: no backward pass through the "
+             "RecurrentStack", m ? m->cfg.dec_stack : 0);
   if (int rc = bind_stream(m, static_cast<cudaStream_t>(stream))) return rc;
   if (!m->noise.on) return forward_backward(m, x, mask, labels, lmask, T, B, L, gscale, cost_out, grads, stream);
   // adaptive weight noise (noise.cu): the step runs on p + eps sqrt(s2).  Every parameter pointer is re-pointed at

@@ -100,8 +100,10 @@ class SpeechRecognizer(object):
             unsupported("unidirectional encoder")
         if dims_top:
             unsupported("dims_top")
-        if dec_stack != 1:
-            unsupported("dec_stack > 1")
+        if dec_stack not in (1, 2):
+            # RecurrentStack of GatedRecurrent layers (lvsr/bricks/recognizer.py:250-259): one or two; two decode and
+            # score only (GradientDescent refuses them)
+            unsupported("dec_stack=%r (1 or 2)" % (dec_stack,))
         if criterion is not None and criterion.get("name", "log_likelihood") != "log_likelihood":
             unsupported("criterion %r" % criterion.get("name"))
         if bottom and bottom.get("dims"):
@@ -150,7 +152,8 @@ class SpeechRecognizer(object):
             post_merge_dim=int(post_merge_dims[0]) if post_merge_dims else int(num_phonemes),
             post_merge_activation=act.kind, maxout_pieces=int(getattr(act, "num_pieces", 1)),
             use_states_for_readout=bool(use_states_for_readout),
-            energy_normalizer=energy_normalizer or "softmax", prior=prior, attention_type=attention_type)
+            energy_normalizer=energy_normalizer or "softmax", prior=prior, attention_type=attention_type,
+            dec_stack=int(dec_stack))
         if not post_merge_dims:
             # Readout's default post_merge is a bare Bias on readout_dim (sequence_generators.py:596-599)
             self.net["post_merge_activation"] = "identity"
@@ -230,6 +233,7 @@ class SpeechRecognizer(object):
         cfg.prior_before = float(p.get("before", 0))
         cfg.prior_after = float(p.get("after", 0))
         cfg.one_of_n_feedback = 0 if n.get("embed_outputs", True) else 1
+        cfg.dec_stack = n.get("dec_stack", 1)
         return cfg
 
     def _require_ready(self):
@@ -537,6 +541,12 @@ class SpeechRecognizer(object):
     def dim_encoded(self):
         return 2 * self.net["dims_bidir"][-1]
 
+    @property
+    def dim_state(self):
+        """Floats of a decoder state row: dim_dec, or with dec_stack 2 the states of both layers [s0 | s1]
+        (the reference's "states" and "states#1")."""
+        return self.net.get("dec_stack", 1) * self.net["dim_dec"]
+
     def encode(self, recordings, recordings_mask=None):
         """Encoder.apply (lvsr/bricks/__init__.py:71-78): [T,B,F], [T,B] -> ([T',B,E], [T',B])."""
         torch = self._torch()
@@ -598,7 +608,7 @@ class SpeechRecognizer(object):
         if return_all:
             extra = dict(weights=torch.empty((L, B, Tp), dtype=torch.float32, device=self.device),
                          energies=torch.empty((L, B, Tp), dtype=torch.float32, device=self.device),
-                         states=torch.empty((L, B, self.net["dim_dec"]), dtype=torch.float32, device=self.device),
+                         states=torch.empty((L, B, self.dim_state), dtype=torch.float32, device=self.device),
                          weighted_averages=torch.empty((L, B, self.dim_encoded), dtype=torch.float32,
                                                        device=self.device))
         _lib.check(lib.lvsr_cost_matrix(
@@ -736,7 +746,7 @@ class SpeechRecognizer(object):
         feedback -> next state.  ``sample=True`` emits from the softmax like SoftmaxEmitter.emit
         (sequence_generators.py:772-778; a seeded Philox stream on the device instead of Theano's MRG stream, so
         draws differ from the reference while their distribution does not), ``sample=False`` emits the arg-max.
-        Returns dict(outputs [n,B] int64, costs [n,B] = -log p(emitted), states [n,B,C], weights [n,B,T'])."""
+        Returns dict(outputs [n,B] int64, costs [n,B] = -log p(emitted), states [n,B,dim_state], weights [n,B,T'])."""
         if self.lm:
             # LMEmitter.emit returns zeros in the reference: generating with an LM is not defined there
             raise NotImplementedError("attention-lvcsr_b200: generate / sample with a language model")
@@ -795,7 +805,7 @@ class SpeechRecognizer(object):
         lib, h = _lib.load(), self._require_ready()
         dev = self.device
         st = OrderedDict(
-            states=torch.empty((R, self.net["dim_dec"]), dtype=torch.float32, device=dev),
+            states=torch.empty((R, self.dim_state), dtype=torch.float32, device=dev),
             outputs=torch.empty((R,), dtype=torch.int64, device=dev),
             weighted_averages=torch.empty((R, self.dim_encoded), dtype=torch.float32, device=dev),
             weights=torch.empty((R, Tp), dtype=torch.float32, device=dev),

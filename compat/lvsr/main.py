@@ -182,6 +182,7 @@ def train(config, save_path, bokeh_name="", params=None, bokeh_server=None, boke
     device), FinishAfter(num_batches, num_epochs; default 1 epoch) and the stop on a NaN gradient norm, the `_best` /
     `_best_ll` checkpoints, Patience.  Monitoring runs only when config['monitoring'] has validate_every_* /
     search_every_* keys.  Parameters are saved in Blocks checkpoint format."""
+    pkg.algorithms.check_trainable_net(config["net"])     # before the model and the data are built
     data = Data(**config["data"])
     recognizer = create_model(config, data, params)
     train_conf = config["training"]

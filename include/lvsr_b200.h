@@ -79,6 +79,10 @@ typedef struct {
                                       1: OneOfNFeedback(V+1) (embed_outputs=False, lvsr/bricks/__init__.py:86-109;
                                       exp/wsj/configs/wsj_jan_new.yaml:46): feedback = one-hot, dim_feedback = V+1  */
   int32_t attention_type;          /* LVSR_ATT_* (0, the zeroed default: content_and_conv)                      */
+  int32_t dec_stack;               /* GRU layers of the decoder: 1 (0, the zeroed default, reads as 1) or 2, a
+                                      RecurrentStack with skip connections (lvsr/bricks/recognizer.py:250-259).  With 2
+                                      the decoder state of a row is [s0 | s1], 2 * dim_dec floats, wherever the ABI
+                                      takes or returns states; training refuses it (inference only).              */
 } lvsr_config;
 
 const char* lvsr_last_error(void);
@@ -198,8 +202,8 @@ int lvsr_preprocess(lvsr_model* m, const float* attended_dev, int32_t Tp, int32_
  * (libs/blocks/blocks/bricks/sequence_generators.py:254-326).
  * labels int64 [L,B], every entry in [0, num_phonemes) -- device memory, NOT range-checked here
  * (lvsr_recognizer_cost_host checks its host copy); labels_mask [L,B] or NULL.  Outputs: costs [L,B]; optional (NULL to
- * skip) weights [L,B,T'], energies [L,B,T'], states [L,B,C] (= s_{i-1}),
- * weighted_averages [L,B,E]. */
+ * skip) weights [L,B,T'], energies [L,B,T'], states [L,B,S] (= s_{i-1}; S = dec_stack * C, [s0 | s1] rows with
+ * dec_stack 2), weighted_averages [L,B,E].  dec_stack 2 always runs on the step-wise kernels. */
 int lvsr_cost_matrix(lvsr_model* m, const float* attended_dev, const float* attended_mask_dev,
                      int32_t Tp, int32_t B, const int64_t* labels_dev, const float* labels_mask_dev,
                      int32_t L, float* costs_dev, float* weights_dev, float* energies_dev,
@@ -218,6 +222,8 @@ int lvsr_alignment_stats(lvsr_model* m, const float* weights_dev, const float* l
 /* ---- the BeamSearch state functions (libs/blocks/blocks/search.py:101-142) ---------
  * R rows (beam hypotheses); row r attends utterance row_utt[r] of `attended` [T',U,E]
  * (row_utt NULL = identity, U == R: the reference's replicated-context call).
+ * states and next_states are [R, dec_stack * C]: with dec_stack 2 each row is [s0 | s1], the states of both layers
+ * (the reference's "states" and "states#1").
  * `preprocessed` may be NULL: it is then recomputed, as the reference does on every call.
  * Content attention: the initial weights and energies are zeros (libs/blocks/blocks/bricks/attention.py:392-395), and
  * every energies output (here and in lvsr_cost_matrix) is zeros (lvsr/bricks/recognizer.py:475-478). */
@@ -310,7 +316,8 @@ int lvsr_recognizer_cost_host(lvsr_model* m, const float* recordings_host, const
  *     lvsr_cost_matrix).  cost_dev[0] = gscale * sum(cost_matrix); grads_dev (lvsr_model_flat_size floats, flat
  *     parameter layout) = gscale * d sum(cost_matrix) / d parameter.  Single GPU: gscale = 1/B gives the reference's
  *     cost = sum / batch_size.  N GPUs: pass gscale = 1, all-reduce(sum) grads_dev, then apply with
- *     gscale = 1 / global batch (SURVEY.md 8e).  Every energy normaliser: with logistic / relu the gradient of
+ *     gscale = 1 / global batch (SURVEY.md 8e).  A model with dec_stack 2 is refused before any work is enqueued
+ *     (no backward pass through the stack).  Every energy normaliser: with logistic / relu the gradient of
  *     energy_comp/linear.b is formed too.  A relu row whose window holds no positive energy is 0 / 0 in the forward,
  *     as in the reference: its cost and the gradients are not finite (the update then follows RemoveNotFinite(0.0)).
  *   lvsr_train_apply_updates: grads_dev *= gscale (+ 2 decay W on WEIGHT parameters), then the CompositeRule of
