@@ -17,6 +17,7 @@ def package():
 
 
 def make_recognizer(cfg, params=None):
+    """A SpeechRecognizer of the oracle config `cfg` (stack_oracle's configs carry dec_stack 2)."""
     pkg = package()
     act = {"maxout": pkg.Maxout(cfg["maxout_pieces"]), "relu": pkg.Rectifier(), "tanh": pkg.Tanh(),
            "identity": pkg.Identity()}[cfg["post_merge_activation"]]
@@ -29,7 +30,7 @@ def make_recognizer(cfg, params=None):
         embed_outputs=cfg.get("embed_outputs", True), prior=cfg["prior"], energy_normalizer=cfg["energy_normalizer"],
         use_states_for_readout=cfg["use_states_for_readout"],
         max_decoded_length_scale=cfg["max_decoded_length_scale"],
-        attention_type=cfg.get("attention_type", "content_and_conv"),
+        attention_type=cfg.get("attention_type", "content_and_conv"), dec_stack=cfg.get("dec_stack", 1),
         enc_transition=pkg.GatedRecurrent, dec_transition=pkg.GatedRecurrent, data_prepend_eos=False)
     if params is not None:
         rec.set_parameter_values(params)

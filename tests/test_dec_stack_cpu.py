@@ -12,6 +12,7 @@ from numpy.testing import assert_allclose
 from oracle import lvsr_oracle as O
 import content_oracle as CO
 import stack_oracle as SO
+import test_gpu_widths as W
 from compat_helpers import COMPAT, write_experiment
 from helpers import ROOT, package
 
@@ -50,6 +51,35 @@ def test_zero_upper_layer_is_the_single_layer_model(attention_type, extra):
     assert_allclose(got["states"][..., :C], want["states"], rtol=0, atol=1e-12)
     assert SO.beam_search(cfg2, stack, x[:, 0], 3, max_length=6) == M1.beam_search(cfg1, single, x[:, 0], 3,
                                                                                     max_length=6)
+
+
+WIDTHS = [(c, True) for c in W.CASES] + [("ragged_k", False), ("odd_c", False)]
+
+
+@pytest.mark.parametrize("case,states_readout", WIDTHS,
+                         ids=[c + ("" if s else "-no_states_readout") for c, s in WIDTHS])
+def test_zero_upper_layer_at_every_width(case, states_readout):
+    """The same at the widths of test_gpu_widths.CASES (C = 8 to 512, E = 256 and 512, one-hot feedback, Maxout(3),
+    Tanh, Rectifier, Identity, V = 2 to 128, content attention) and without the states in the readout, on the
+    teacher-forced decoder alone."""
+    net, prior = W.CASES[case]
+    kw = dict(W.COMMON, **net, use_states_for_readout=states_readout)
+    if case.startswith("content"):
+        cfg1, M1, cfg2 = CO.make_config(**kw), CO, SO.make_config("content", **kw)
+    else:
+        cfg1, M1, cfg2 = O.make_config(prior=prior, **kw), O, SO.make_config(prior=prior, **kw)
+    single = M1.init_params(cfg1, seed=3, scale=10.0)
+    stack = SO.from_single(cfg2, single)
+    assert any("readout/merge/transform_states#1" in k for k in stack) == states_readout
+    att, attm, labels, lm = W._inputs(cfg1, 3, 14, 6, seed=4)
+    want = M1.cost_matrix(cfg1, single, att, attm, labels, lm, return_all=True)
+    got = SO.cost_matrix(cfg2, stack, att, attm, labels, lm, return_all=True)
+    C = cfg1["dim_dec"]
+    assert got["states"].shape == want["states"].shape[:2] + (2 * C,)
+    assert not np.any(got["states"][..., C:])
+    for key in ("costs", "weights", "energies", "weighted_averages"):
+        assert_allclose(got[key], want[key], rtol=0, atol=1e-12, err_msg=key)
+    assert_allclose(got["states"][..., :C], want["states"], rtol=0, atol=1e-12)
 
 
 def test_transition_is_blocks_recurrent_stack_with_skip_connections():
