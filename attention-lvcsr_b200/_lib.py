@@ -59,6 +59,17 @@ class LvsrConfig(C.Structure):
     ]
 
 
+LVSR_MAX_BOTTOM = 4
+LVSR_MAX_BOTTOM_DIM = 4096
+# activations of the bottom MLP (LVSR_ACT_* values of lvsr_bottom_config.activation)
+BOTTOM_ACTIVATIONS = {"relu": 1, "tanh": 2}
+
+
+class LvsrBottomConfig(C.Structure):
+    """Mirror of ``lvsr_bottom_config`` (include/lvsr_b200.h)."""
+    _fields_ = [("num_layers", C.c_int32), ("dims", C.c_int32 * LVSR_MAX_BOTTOM), ("activation", C.c_int32)]
+
+
 class LvsrTrainConfig(C.Structure):
     """Mirror of ``lvsr_train_config`` (include/lvsr_b200.h)."""
     _fields_ = [("gradient_threshold", C.c_float), ("use_momentum", C.c_int32), ("scale", C.c_float),
@@ -99,6 +110,7 @@ SIGNATURES = {
     "lvsr_last_error": (C.c_char_p, []),
     "lvsr_version": (C.c_int, []),
     "lvsr_model_create": (C.c_int, [C.POINTER(LvsrConfig), C.POINTER(_P)]),
+    "lvsr_model_create_bottom": (C.c_int, [C.POINTER(LvsrConfig), C.POINTER(LvsrBottomConfig), C.POINTER(_P)]),
     "lvsr_model_destroy": (C.c_int, [_P]),
     "lvsr_model_num_params": (C.c_int, [_P]),
     "lvsr_model_param_name": (C.c_char_p, [_P, C.c_int]),

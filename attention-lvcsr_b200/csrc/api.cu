@@ -72,7 +72,7 @@ void add_param(lvsr_model* m, const std::string& name, int64_t d0, int64_t d1 = 
 // Blocks initialisation order (oracle/lvsr_oracle.py: param_shapes)
 void build_param_table(lvsr_model* m) {
   const lvsr_config& c = m->cfg;
-  int din = c.num_features;
+  int din = encoder_input_dim(m);
   for (int l = 0; l < c.num_layers; ++l) {
     const int D = c.dims_bidir[l];
     for (int dir = 0; dir < 2; ++dir) {
@@ -86,6 +86,12 @@ void build_param_table(lvsr_model* m) {
       add_param(m, b + "/fork/fork_gate_inputs.W", din, 2 * D);
     }
     din = 2 * D;
+  }
+  // SpeechRecognizer.children = [encoder, top, bottom, generator] (lvsr/bricks/recognizer.py:350); Linear._allocate
+  // makes W before b (libs/blocks/blocks/bricks/simple.py)
+  for (int i = 0; i < m->bottom.num_layers; ++i) {
+    add_param(m, bottom_linear(i) + ".W", bottom_input_dim(m, i), m->bottom.dims[i]);
+    add_param(m, bottom_linear(i) + ".b", m->bottom.dims[i]);
   }
   const int E = m->E, C = c.dim_dec, M = c.dim_matcher, K = c.conv_num_filters, w = 2 * c.conv_n + 1;
   const int V = c.num_phonemes, Cfb = c.dim_feedback, Cpm = c.post_merge_dim;
@@ -328,11 +334,11 @@ size_t encoder_ws_bytes(const lvsr_model* m, int T, int B) {
     const int D = m->cfg.dims_bidir[l], k = m->cfg.subsample[l];
     const int Tout = ceil_div(Tl, k);
     total += ((size_t)Tl * B * 6 * D + (size_t)Tout * B * 2 * D) * sizeof(float) + 1024;
-    total += (size_t)2 * Tl * B * gemm_tc_kpad(l == 0 ? m->cfg.num_features : 2 * m->cfg.dims_bidir[l - 1]) * sizeof(float) + 1024;
+    total += (size_t)2 * Tl * B * gemm_tc_kpad(l == 0 ? encoder_input_dim(m) : 2 * m->cfg.dims_bidir[l - 1]) * sizeof(float) + 1024;
     total += gemm_f16_stream_sync_ints(Tl * B) * sizeof(int) + 1024;   // scheduling area of a streamed projection
     Tl = Tout;
   }
-  return total + (1 << 16);
+  return total + bottom_ws_bytes(m, T * B) + (1 << 16);
 }
 size_t cost_ws_bytes(const lvsr_model* m, int Tp, int B, int L) {
   const lvsr_config& c = m->cfg;
@@ -386,8 +392,19 @@ int lvsr_profile_read(const char* kernel_class, double* total_ms, int64_t* count
   return 0;
 }
 
-int lvsr_model_create(const lvsr_config* cfg, lvsr_model** out) {
+int lvsr_model_create(const lvsr_config* cfg, lvsr_model** out) { return lvsr_model_create_bottom(cfg, nullptr, out); }
+
+int lvsr_model_create_bottom(const lvsr_config* cfg, const lvsr_bottom_config* bottom, lvsr_model** out) {
   LVSR_CHECK(cfg && out, "null argument");
+  if (bottom) {
+    LVSR_CHECK(bottom->num_layers >= 0 && bottom->num_layers <= LVSR_MAX_BOTTOM, "bottom MLP: %d layers (0 .. %d)",
+               bottom->num_layers, (int)LVSR_MAX_BOTTOM);
+    for (int i = 0; i < bottom->num_layers; ++i)
+      LVSR_CHECK(bottom->dims[i] >= 1 && bottom->dims[i] <= LVSR_MAX_BOTTOM_DIM, "bottom MLP: width %d of layer %d (1 .. %d)",
+                 bottom->dims[i], i, (int)LVSR_MAX_BOTTOM_DIM);
+    LVSR_CHECK(bottom->num_layers == 0 || bottom->activation == LVSR_ACT_RELU || bottom->activation == LVSR_ACT_TANH,
+               "bottom MLP: activation %d unsupported (Rectifier or Tanh)", bottom->activation);
+  }
   LVSR_CHECK(cfg->num_layers >= 1 && cfg->num_layers <= LVSR_MAX_LAYERS, "num_layers %d out of range", cfg->num_layers);
   for (int l = 0; l < cfg->num_layers; ++l) {
     LVSR_CHECK(bigru_supported(cfg->dims_bidir[l]), "encoder dim %d unsupported (128 or 256)", cfg->dims_bidir[l]);
@@ -417,6 +434,7 @@ int lvsr_model_create(const lvsr_config* cfg, lvsr_model** out) {
   LVSR_CHECK(dev_count > 0, "no CUDA device: the GPU path has no CPU fallback");
   lvsr_model* m = new lvsr_model();
   m->cfg = *cfg;
+  if (bottom && bottom->num_layers > 0) m->bottom = *bottom;
   if (m->cfg.dec_stack == 0) m->cfg.dec_stack = 1;     // callers that predate the field zero-fill it
   if (content) {
     // SequenceContentAttention takes none of these (lvsr/bricks/recognizer.py:261-265): softmax weights over every
@@ -466,6 +484,7 @@ int lvsr_model_destroy(lvsr_model* m) {
   for (float* p : m->Wcat) if (p) cudaFree(p);
   for (float* p : m->bcat) if (p) cudaFree(p);
   for (TcWeights& t : m->Wcat_tc) if (t.mem) cudaFree(t.mem);
+  for (TcWeights& t : m->bottom_tc) if (t.mem) cudaFree(t.mem);
   if (m->Wp_tc.mem) cudaFree(m->Wp_tc.mem);
   if (m->Wd_cat) cudaFree(m->Wd_cat);
   if (m->Wb1) cudaFree(m->Wb1);
@@ -701,7 +720,7 @@ int finalize_on_stream(lvsr_model* m, cudaStream_t st, bool synchronise) {
   const lvsr_config& c = m->cfg;
   if (m->Wcat.empty()) {
     for (int l = 0; l < c.num_layers; ++l) {
-      const ForkLayout f = encoder_fork(c, l, 0);       // Wcat[l] [rows, ld], bcat[l] [ld]
+      const ForkLayout f = encoder_fork(m, l, 0);       // Wcat[l] [rows, ld], bcat[l] [ld]
       float *W = nullptr, *b = nullptr;
       LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&W), (size_t)f.rows * f.ld * sizeof(float)));
       LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&b), (size_t)f.ld * sizeof(float)));
@@ -729,7 +748,7 @@ int finalize_on_stream(lvsr_model* m, cudaStream_t st, bool synchronise) {
   }
   for (int l = 0; l < c.num_layers; ++l)
     for (int dir = 0; dir < 2; ++dir)
-      if (int rc = fork_copy(m, encoder_fork(c, l, dir), m->Wcat[l], m->bcat[l], nullptr, st)) return rc;
+      if (int rc = fork_copy(m, encoder_fork(m, l, dir), m->Wcat[l], m->bcat[l], nullptr, st)) return rc;
   const int C = c.dim_dec, Cfb = c.dim_feedback, V = c.num_phonemes;
   const std::string g = GEN, t = TR;
   // decoder-side packing: gate columns first (update | reset), then the candidate inputs
@@ -744,10 +763,15 @@ int finalize_on_stream(lvsr_model* m, cudaStream_t st, bool synchronise) {
   if (m->use_tc) {
     m->Wcat_tc.resize(c.num_layers);
     for (int l = 0; l < c.num_layers; ++l) {
-      const ForkLayout f = encoder_fork(c, l, 0);
+      const ForkLayout f = encoder_fork(m, l, 0);
       if (int rc = pack_tc_weights(m->Wcat_tc[l], m->Wcat[l], f.rows, f.ld, st)) return rc;
     }
     if (int rc = pack_tc_weights(m->Wp_tc, m->P(att_base(m) + "/preprocess.W"), m->E, c.dim_matcher, st)) return rc;
+    m->bottom_tc.resize(m->bottom.num_layers);
+    for (int i = 0; i < m->bottom.num_layers; ++i)
+      if (int rc = pack_tc_weights(m->bottom_tc[i], m->P(bottom_linear(i) + ".W"), bottom_input_dim(m, i), m->bottom.dims[i],
+                                   st))
+        return rc;
   }
   // fork(feedback(y)) for every symbol y, once: [(V+1), 3C]
   if (c.one_of_n_feedback) {
@@ -830,10 +854,18 @@ int projection_gemm(Arena& ws, const float* A, int M, int K, const float* W, con
 constexpr int ENC_OVERLAP_MIN_SMS = 16;
 
 int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int T, int B, float* attended,
-                float* attended_mask, LayerTape* tape, cudaStream_t st) {
+                float* attended_mask, LayerTape* tape, cudaStream_t st, const float** bottom_out) {
   const lvsr_config& c = m->cfg;
   const float* cur = x;
-  int Tl = T, din = c.num_features;
+  int Tl = T, din = encoder_input_dim(m);
+  if (m->bottom.num_layers) {
+    // every frame, padded ones included: the BiGRU's mask keeps them out of the states and their gradients
+    const float* y[LVSR_MAX_BOTTOM] = {};
+    if (int rc = bottom_forward(m, ws, x, T * B, y, st)) return rc;
+    cur = y[m->bottom.num_layers - 1];
+    if (bottom_out)
+      for (int i = 0; i < m->bottom.num_layers; ++i) bottom_out[i] = y[i];
+  }
   long long mstride = B;
   int kcum = 1;
   for (int l = 0; l < c.num_layers; ++l) {

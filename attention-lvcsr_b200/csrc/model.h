@@ -105,6 +105,7 @@ using namespace lvsr;
 
 struct lvsr_model {
   lvsr_config cfg;
+  lvsr_bottom_config bottom = {};   // the bottom MLP in front of the encoder (num_layers 0: none)
   int device = 0;                   // the GPU this handle lives on (current device at lvsr_model_create)
   int E;
   std::vector<Param> params;
@@ -135,6 +136,7 @@ struct lvsr_model {
   } stack;
   // dense-projection weights as the tensor-core GEMM reads them (wgmma path); empty = SIMT path
   std::vector<TcWeights> Wcat_tc;
+  std::vector<TcWeights> bottom_tc; // per bottom layer: linear_<i>.W [d_in, d_out]
   TcWeights Wp_tc;
   bool use_tc = true;
   float v_bias = 0.f;               // host copy of energy_comp/linear.b
@@ -286,11 +288,20 @@ struct ArenaScope {
 // Rewinds the workspace to its construction-time offset when the scope ends, unless it overflowed (off > cap)
 struct ArenaMark { Arena& ws; const size_t off = ws.off; ~ArenaMark() { if (ws.off <= ws.cap) ws.off = off; } };
 
+// Features encoder layer 0 takes: the bottom MLP's last width, or the recordings' features without one
+static inline int encoder_input_dim(const lvsr_model* m) {
+  return m->bottom.num_layers ? m->bottom.dims[m->bottom.num_layers - 1] : m->cfg.num_features;
+}
+// Bottom layer i: its Blocks path (MLP "bottom" of the brick "bottom", linears "linear_<i>") and input width
+static inline std::string bottom_linear(int i) { return "/recognizer/bottom/bottom/linear_" + std::to_string(i); }
+static inline int bottom_input_dim(const lvsr_model* m, int i) { return i ? m->bottom.dims[i - 1] : m->cfg.num_features; }
+
 // A packed fork, blocks in column order: <fork>/<param>.W fills columns [col, col + cols) of W [rows, ld], .b those of b [ld]
 struct ForkLayout { std::string fork; int rows, ld; struct { const char* param; int col, cols; } block[2]; };
 // encoder layer l, direction dir, in Wcat[l] / bcat[l]: per direction [inputs D | gate_inputs 2D (update | reset)]
-static inline ForkLayout encoder_fork(const lvsr_config& c, int l, int dir) {
-  const int D = c.dims_bidir[l], c0 = dir * 3 * D, din = l ? 2 * c.dims_bidir[l - 1] : c.num_features;
+static inline ForkLayout encoder_fork(const lvsr_model* m, int l, int dir) {
+  const lvsr_config& c = m->cfg;
+  const int D = c.dims_bidir[l], c0 = dir * 3 * D, din = l ? 2 * c.dims_bidir[l - 1] : encoder_input_dim(m);
   return {enc_base(l, dir) + "/fork", din, 6 * D, {{"fork_inputs", c0, D}, {"fork_gate_inputs", c0 + D, 2 * D}}};
 }
 // fork(feedback(y)) in Wff_cat / bff_cat: [gate_inputs 2C | inputs C]
@@ -337,8 +348,15 @@ void noise_free(lvsr_model* m);
 // Every encoder layer (fork projection + BiGRU scan) and the mask of the encoded frames: attended [Tp, B, E] (the last
 // layer writes it), attended_mask [Tp, B].  Buffers come from `ws`.  Without a tape (inference) the BiGRU runs without
 // the training stores; with one, tape[l] records layer l's buffers (and allocates hext) for the backward pass.
+// With a bottom MLP it runs first, on all T*B frames; with a tape, bottom_out[i] (LVSR_MAX_BOTTOM entries) records
+// the output of its layer i, after the activation, for the backward pass.
 int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int T, int B, float* attended,
-                float* attended_mask, LayerTape* tape, cudaStream_t st);
+                float* attended_mask, LayerTape* tape, cudaStream_t st, const float** bottom_out = nullptr);
+// The bottom MLP (bottom.cu): out[i] = act(X_i W_i + b_i) for every layer over `rows` frames, buffers from `ws`
+int bottom_forward(lvsr_model* m, Arena& ws, const float* x, int rows, const float** out, cudaStream_t st);
+// dY [rows, n] <- dY * act'(Y) in place, from the layer's output Y = act(pre) (bottom.cu)
+int bottom_act_backward(float* dY, const float* Y, long long n, int activation, cudaStream_t st);
+size_t bottom_ws_bytes(const lvsr_model* m, int rows);
 // out[M, N] = A[M, K] . W + bias on the tensor cores when tw holds a packed form and the shape suits it, else on FFMA
 // tiles; *kpad (may be null) = the contraction as the tensor-core GEMM stored it, 0 on FFMA; *operands (may be null) =
 // LVSR_ENC_OPS_* of the kernel that ran

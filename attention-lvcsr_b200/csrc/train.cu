@@ -172,7 +172,13 @@ struct TrainStep {
     LVSR_CHECK(E <= 1024, "encoded dim %d > 1024 unsupported in training", E);
     // size the tape arena once per shape
     size_t bytes = (size_t)64 << 20;
-    int Tl = T, din = c.num_features;
+    int Tl = T, din = encoder_input_dim(m);
+    for (int i = 0; i < m->bottom.num_layers; ++i) {
+      // output, forward split, K-major operands, TN partials and the input gradient with its operands
+      const size_t rows = (size_t)T * B, di = bottom_input_dim(m, i), d = m->bottom.dims[i];
+      bytes += (rows * d + 2 * rows * gemm_tc_kpad((int)di) + 2 * (di + d + 32) * (rows + 32) + (size_t)80 * di * d +
+                rows * di + 2 * rows * d + 2 * di * d) * sizeof(float);
+    }
     for (int l = 0; l < c.num_layers; ++l) {
       const int D = c.dims_bidir[l], Tout = ceil_div(Tl, c.subsample[l]);
       bytes += ((size_t)Tl * B * 6 * D * 2 + (size_t)(Tl + 2) * B * 2 * D * 2 + (size_t)Tout * B * 2 * D * 2 + (size_t)3 * Tl * B * gemm_tc_kpad(din)) * sizeof(float);
@@ -189,8 +195,9 @@ struct TrainStep {
       for (int s = LVSR_ENC_BWD_CS; s <= LVSR_ENC_DX; ++s) m->enc_plan[l][s] = 0;
     LVSR_CUDA_OK(cudaMemsetAsync(grads, 0, (size_t)m->flat_count * sizeof(float), st));
     std::vector<LayerTape> tape(c.num_layers);
+    const float* bottom_out[LVSR_MAX_BOTTOM] = {};
     DecTape d;
-    if (int rc = taped_forward(x, mask, T, tape.data(), cost_out, d)) return rc;
+    if (int rc = taped_forward(x, mask, T, tape.data(), bottom_out, cost_out, d)) return rc;
     // dY . W^T right-hand sides, transposed here, not in the phases that read them, to keep their arena place ahead of
     // the readout's and decoder backward's buffers: placement can move the step time (DESIGN.md section 6, item 4)
     float* WmsT = c.use_states_for_readout ? ws.f32((size_t)Cpm * C) : nullptr;     // [Cpm, C]
@@ -220,14 +227,15 @@ struct TrainStep {
     if (int rc = decoder_backward(d, WstateT, WcombT, WsT, dS_ro, dCtx_ro, dg)) return rc;
     if (int rc = decoder_weight_grads(d, dg)) return rc;
     if (int rc = attended_grad(d, dg, WpT, dH)) return rc;
-    return encoder_backward(tape.data(), mask, dH);
+    return encoder_backward(tape.data(), mask, dH, x, bottom_out);
   }
   // Taped forward: the encoder keeping its tape, then the teacher-forced decoder; *cost_out = sum(costs) * gscale
-  int taped_forward(const float* x, const float* mask, int T, LayerTape* tape, float* cost_out, DecTape& d) const {
+  int taped_forward(const float* x, const float* mask, int T, LayerTape* tape, const float** bottom_out, float* cost_out,
+                    DecTape& d) const {
     d.Hatt = ws.f32((size_t)Tp * B * E);                  // attended [Tp, B, E]
     d.attm = ws.f32((size_t)Tp * B);
     LVSR_CHECK(d.Hatt && d.attm, "out of device memory (encoder output)");
-    if (int rc = run_encoder(m, ws, x, mask, T, B, d.Hatt, d.attm, tape, st)) return rc;
+    if (int rc = run_encoder(m, ws, x, mask, T, B, d.Hatt, d.attm, tape, st, bottom_out)) return rc;
     d.costs = ws.f32((size_t)R);
     d.W_all = ws.f32((size_t)R * Tp);        // alignments alpha_i
     d.S_prev = ws.f32((size_t)R * C);        // s_{i-1}
@@ -447,9 +455,67 @@ struct TrainStep {
     if (int rc = colsum(dg.dP, Tp * B, M, M, grad(at + "/preprocess.b"), false, st)) return rc;
     return 0;
   }
-  // Encoder backward, top layer first: scan, weight and input gradients; plan slots LVSR_ENC_BWD_CS .. LVSR_ENC_DX
-  int encoder_backward(const LayerTape* tape, const float* mask, const float* dH) const {
+  // dX [rows, N] = dY [rows, K] . W^T for a layer's weights W [N, K] (row-major, so W is the K-major form of the
+  // right-hand side): on the tensor cores when the shape suits them, else W transposed onto the FFMA tiles
+  int input_grad(const float* dY, int rows, int K, const float* W, int N, float* dX, int32_t* path) const {
+    if (m->use_tc && gemm_tc_supported(rows, N, K) && K % 32 == 0) {
+      ArenaMark mark{ws};
+      float* a_hi = ws.f32((size_t)rows * K);
+      float* a_lo = ws.f32((size_t)rows * K);
+      float* w_hi = ws.f32((size_t)N * K);
+      float* w_lo = ws.f32((size_t)N * K);
+      LVSR_CHECK(a_hi && a_lo && w_hi && w_lo, "out of device memory (dX operands)");
+      if (int rc = split_tf32(W, w_hi, w_lo, (long long)N * K, st)) return rc;
+      if (int rc = gemm_tc(dY, a_hi, a_lo, rows, K, w_hi, w_lo, N, nullptr, dX, N, st)) return rc;
+      *path = LVSR_ENC_PATH_TC;
+    } else {
+      float* WT = ws.f32((size_t)K * N);
+      LVSR_CHECK(WT, "out of device memory (dX)");
+      if (int rc = transpose(W, WT, N, K, st)) return rc;
+      if (int rc = gemm_nn(dY, rows, K, K, WT, N, N, nullptr, dX, N, false, st)) return rc;
+      *path = LVSR_ENC_PATH_FFMA;
+    }
+    return 0;
+  }
+  // The bottom MLP, top layer first, from dY = the gradient of its output (overwritten): dZ = dY * act'(Y) in place,
+  // dW_i = X_i^T dZ on the products of the fork weights, db_i = colsum(dZ), and dX_i = dZ W_i^T below the top layer.
+  // Padded frames carry exactly zero dY (the BiGRU backward gives them no dPre), so they add nothing.
+  int bottom_backward(const float* x, const float* const* Y, float* dY, int rows) const {
+    ProfScope prof("bottom_bwd", st);
+    const lvsr_bottom_config& bt = m->bottom;
+    for (int i = bt.num_layers - 1; i >= 0; --i) {
+      const int din = bottom_input_dim(m, i), d = bt.dims[i];
+      const float* X = i ? Y[i - 1] : x;
+      const std::string lin = bottom_linear(i);
+      if (int rc = bottom_act_backward(dY, Y[i], (long long)rows * d, bt.activation, st)) return rc;
+      {
+        ArenaMark mark{ws};
+        if (m->use_tc && rows >= 2048 && d % 128 == 0) {
+          TcOperand dZT, XT;
+          if (int rc = make_tc_operand(ws, dY, rows, d, d, &dZT, st)) return rc;
+          if (int rc = make_tc_operand(ws, X, rows, din, din, &XT, st)) return rc;
+          if (int rc = gemm_tn_tc(ws, XT, 0, din, dZT, 0, d, grad(lin + ".W"), d, false, st)) return rc;
+        } else {
+          if (int rc = gemm_tn(ws, X, din, dY, d, rows, din, d, grad(lin + ".W"), d, false, st)) return rc;
+        }
+      }
+      if (int rc = colsum(dY, rows, d, d, grad(lin + ".b"), false, st)) return rc;
+      if (i > 0) {
+        float* dX = ws.f32((size_t)rows * din);
+        LVSR_CHECK(dX, "out of device memory (bottom dX)");
+        int32_t path = 0;
+        if (int rc = input_grad(dY, rows, d, m->P(lin + ".W"), din, dX, &path)) return rc;
+        dY = dX;
+      }
+    }
+    return 0;
+  }
+  // Encoder backward, top layer first: scan, weight and input gradients; plan slots LVSR_ENC_BWD_CS .. LVSR_ENC_DX.
+  // With a bottom MLP, layer 0's input gradient feeds its backward (x: the recordings, bottom_out: its layers' outputs).
+  int encoder_backward(const LayerTape* tape, const float* mask, const float* dH, const float* x,
+                       const float* const* bottom_out) const {
     const float* dout = dH;
+    float* dX0 = nullptr;
     for (int l = c.num_layers - 1; l >= 0; --l) {
       const LayerTape& tp = tape[l];
       const int D = tp.D, rows = tp.T * B;
@@ -494,7 +560,7 @@ struct TrainStep {
         if (int rc = colsum(tp.pre, rows, 6 * D, 6 * D, dbcat, false, st)) return rc;
         for (int dir = 0; dir < 2; ++dir) {
           const std::string b = enc_base(l, dir);
-          const ForkLayout f = encoder_fork(c, l, dir);
+          const ForkLayout f = encoder_fork(m, l, dir);
           const int cA = f.block[0].col, cG = f.block[1].col;      // columns of dA (fork_inputs) and [dGz|dGr]
           if (int rc = fork_copy(m, f, dWcat, dbcat, grads, st)) return rc;
           // recurrent weights: state_to_state = (h*r)^T dA ; state_to_gates = H_prev^T [dGz|dGr]
@@ -510,32 +576,16 @@ struct TrainStep {
           if (int rc = colsum(dh0 + (size_t)dir * B * D, B, D, D, grad(b + "/gatedrecurrent.initial_state"), false, st)) return rc;
         }
       }
-      // gradient of the layer input = gradient of the (subsampled) output of the layer below
-      if (l > 0) {
+      // gradient of the layer input = gradient of the (subsampled) output of the layer below, or of the bottom MLP's
+      if (l > 0 || m->bottom.num_layers) {
         float* dX = ws.f32((size_t)rows * tp.Din);
         LVSR_CHECK(dX, "out of device memory (dX)");
-        if (m->use_tc && gemm_tc_supported(rows, tp.Din, 6 * D) && (6 * D) % 32 == 0) {
-          // dX = dPre . Wcat^T: the K-major form of the right-hand side [N = Din, K = 6D] is Wcat itself
-          ArenaMark mark{ws};
-          float* a_hi = ws.f32((size_t)rows * 6 * D);
-          float* a_lo = ws.f32((size_t)rows * 6 * D);
-          float* w_hi = ws.f32((size_t)tp.Din * 6 * D);
-          float* w_lo = ws.f32((size_t)tp.Din * 6 * D);
-          LVSR_CHECK(a_hi && a_lo && w_hi && w_lo, "out of device memory (dX operands)");
-          if (int rc = split_tf32(m->Wcat[l], w_hi, w_lo, (long long)tp.Din * 6 * D, st)) return rc;
-          if (int rc = gemm_tc(tp.pre, a_hi, a_lo, rows, 6 * D, w_hi, w_lo, tp.Din, nullptr, dX, tp.Din, st)) return rc;
-          plan[LVSR_ENC_DX] = LVSR_ENC_PATH_TC;
-        } else {
-          float* WcatT = ws.f32((size_t)6 * D * tp.Din);
-          LVSR_CHECK(WcatT, "out of device memory (dX)");
-          if (int rc = transpose(m->Wcat[l], WcatT, tp.Din, 6 * D, st)) return rc;
-          if (int rc = gemm_nn(tp.pre, rows, 6 * D, 6 * D, WcatT, tp.Din, tp.Din, nullptr, dX, tp.Din, false, st)) return rc;
-          plan[LVSR_ENC_DX] = LVSR_ENC_PATH_FFMA;
-        }
-        dout = dX;
+        // dX = dPre . Wcat^T: the K-major form of the right-hand side [N = Din, K = 6D] is Wcat itself
+        if (int rc = input_grad(tp.pre, rows, 6 * D, m->Wcat[l], tp.Din, dX, &plan[LVSR_ENC_DX])) return rc;
+        dout = dX0 = dX;
       }
     }
-    return 0;
+    return m->bottom.num_layers ? bottom_backward(x, bottom_out, dX0, tape[0].T * B) : 0;
   }
 };
 

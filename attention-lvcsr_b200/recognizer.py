@@ -106,8 +106,15 @@ class SpeechRecognizer(object):
             unsupported("dec_stack=%r (1 or 2)" % (dec_stack,))
         if criterion is not None and criterion.get("name", "log_likelihood") != "log_likelihood":
             unsupported("criterion %r" % criterion.get("name"))
-        if bottom and bottom.get("dims"):
-            unsupported("bottom MLP")
+        # SpeechBottom (lvsr/bricks/recognizer.py:105-157): an MLP of one Linear + activation per entry of dims, Tanh
+        # when the activation is None; Identity when dims is empty
+        bottom = dict(bottom or {})
+        bottom.pop("bottom_class", None)
+        bottom_dims = [int(d) for d in (bottom.get("dims") or [])]
+        bottom_act = bottom.get("activation")
+        bottom_kind = "tanh" if bottom_act is None else getattr(bottom_act, "kind", None)
+        if bottom_dims and bottom_kind not in _lib.BOTTOM_ACTIVATIONS:
+            unsupported("bottom MLP activation %r (Rectifier or Tanh)" % (bottom_act,))
         for tr in (enc_transition, dec_transition):
             if tr is not None and getattr(tr, "__name__", type(tr).__name__) != "GatedRecurrent":
                 unsupported("transition %r" % tr)
@@ -154,6 +161,8 @@ class SpeechRecognizer(object):
             use_states_for_readout=bool(use_states_for_readout),
             energy_normalizer=energy_normalizer or "softmax", prior=prior, attention_type=attention_type,
             dec_stack=int(dec_stack))
+        if bottom_dims:
+            self.net["bottom"] = dict(dims=bottom_dims, activation=bottom_kind)
         if not post_merge_dims:
             # Readout's default post_merge is a bare Bias on readout_dim (sequence_generators.py:596-599)
             self.net["post_merge_activation"] = "identity"
@@ -236,6 +245,21 @@ class SpeechRecognizer(object):
         cfg.dec_stack = n.get("dec_stack", 1)
         return cfg
 
+    def _make_bottom_config(self):
+        """lvsr_bottom_config of the bottom MLP, None without one."""
+        b = self.net.get("bottom")
+        if not b:
+            return None
+        if len(b["dims"]) > _lib.LVSR_MAX_BOTTOM:
+            raise NotImplementedError("attention-lvcsr_b200: a bottom MLP of %d layers (at most %d)"
+                                      % (len(b["dims"]), _lib.LVSR_MAX_BOTTOM))
+        out = _lib.LvsrBottomConfig()
+        out.num_layers = len(b["dims"])
+        for i, d in enumerate(b["dims"]):
+            out.dims[i] = d
+        out.activation = _lib.BOTTOM_ACTIVATIONS[b["activation"]]
+        return out
+
     def _require_ready(self):
         if self._handle is None:
             import ctypes as C
@@ -244,7 +268,11 @@ class SpeechRecognizer(object):
             with torch.cuda.device(self.device):
                 h = C.c_void_p()
                 cfg = self._make_config()
-                _lib.check(lib.lvsr_model_create(C.byref(cfg), C.byref(h)))
+                bottom = self._make_bottom_config()
+                if bottom is None:
+                    _lib.check(lib.lvsr_model_create(C.byref(cfg), C.byref(h)))
+                else:
+                    _lib.check(lib.lvsr_model_create_bottom(C.byref(cfg), C.byref(bottom), C.byref(h)))
             self._handle = h
             if self.lm:
                 self._attach_lm(lib, h)
@@ -526,7 +554,7 @@ class SpeechRecognizer(object):
         previous layer's scan, lvsr_model_encoder_overlap), tiles_beside and tiles_after (its output tiles computed
         beside that scan and after it).  Of the last training step: bwd_cs (CTAs per cluster of the reverse-time scan),
         wgrad ("tc" or "ffma"), wgrad_splits, wgrad_kpad (the padded contraction over T*B rows, 0 on FFMA) and dx ("tc",
-        "ffma", or None for layer 0).  None / 0: not run."""
+        "ffma", or None for layer 0 without a bottom MLP).  None / 0: not run."""
         return [self._encoder_plan_row(l) for l in range(len(self.net["dims_bidir"]))]
 
     def preprocess_plan(self):

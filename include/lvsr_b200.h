@@ -85,6 +85,18 @@ typedef struct {
                                       takes or returns states; training refuses it (inference only).              */
 } lvsr_config;
 
+/* The bottom MLP of config['net']['bottom'] (SpeechBottom, lvsr/bricks/recognizer.py:105-157): with num_layers = k > 0
+ * every frame passes x_{i+1} = act(x_i W_i + b_i), i = 0 .. k-1, before encoder layer 0, which then takes dims[k-1]
+ * features.  x_0 is the recordings (num_features); activation is LVSR_ACT_RELU (Rectifier) or LVSR_ACT_TANH.  Its
+ * parameters are "/recognizer/bottom/bottom/linear_<i>.W" [d_in, dims[i]] and ".b" [dims[i]], after the encoder's and
+ * before the generator's in the parameter table.  num_layers = 0 is the Identity bottom (dims: []). */
+enum { LVSR_MAX_BOTTOM = 4, LVSR_MAX_BOTTOM_DIM = 4096 };
+typedef struct {
+  int32_t num_layers;              /* k = len(dims), 0 .. LVSR_MAX_BOTTOM                                        */
+  int32_t dims[LVSR_MAX_BOTTOM];   /* 1 .. LVSR_MAX_BOTTOM_DIM each                                              */
+  int32_t activation;              /* LVSR_ACT_RELU or LVSR_ACT_TANH (the reference's default for None)          */
+} lvsr_bottom_config;
+
 const char* lvsr_last_error(void);
 int lvsr_version(void);
 
@@ -92,6 +104,9 @@ int lvsr_version(void);
 /* SpeechRecognizer(**config['net']) + allocate(): lvsr/main.py:213-221. Uses the
  * CUDA device current on the calling thread. */
 int lvsr_model_create(const lvsr_config* cfg, lvsr_model** out);
+/* The same with a bottom MLP (NULL: none, which is lvsr_model_create).  Every entry point that takes recordings runs
+ * it; a depth, width or activation outside lvsr_bottom_config's ranges is refused here. */
+int lvsr_model_create_bottom(const lvsr_config* cfg, const lvsr_bottom_config* bottom, lvsr_model** out);
 int lvsr_model_destroy(lvsr_model* m);
 
 /* Parameter table in Blocks order/names ("/recognizer/encoder/bidir0/forward/fork/fork_inputs.W"
@@ -165,7 +180,7 @@ enum {
   LVSR_ENC_WGRAD = 11,        /* weight gradients X^T dY: LVSR_ENC_PATH_*                                      */
   LVSR_ENC_WGRAD_SPLITS = 12, /* partial products the contraction over T_l * B rows was split into             */
   LVSR_ENC_WGRAD_KPAD = 13,   /* that contraction as the tensor-core operands store it (0 on FFMA)             */
-  LVSR_ENC_DX = 14,           /* input gradient dY W^T: LVSR_ENC_PATH_* (NONE for layer 0)                     */
+  LVSR_ENC_DX = 14,           /* input gradient dY W^T: LVSR_ENC_PATH_* (NONE for layer 0 without a bottom MLP)*/
   LVSR_ENC_OPERANDS = 15      /* operands of the tensor-core projection GEMM: LVSR_ENC_OPS_*                   */
 };
 enum { LVSR_ENC_PATH_NONE = 0, LVSR_ENC_PATH_TC = 1, LVSR_ENC_PATH_FFMA = 2 };
@@ -411,7 +426,8 @@ int64_t lvsr_launch_count(int reset);
 /* Per-kernel-class device timing (CUDA events recorded on the launching stream around every
  * launch of that class) -- the analogue of the reference's Theano ProfileStats
  * (libs/Theano/theano/compile/profiling.py:97).  Classes: "gemm", "bigru", "attention",
- * "window", "dense", "readout", "lm", "noise" (adaptive weight noise).  lvsr_profile_read synchronises the device, returns the
+ * "window", "dense", "readout", "lm", "noise" (adaptive weight noise), "bottom" (the bottom MLP's forward, its
+ * GEMMs included) and "bottom_bwd" (its backward).  lvsr_profile_read synchronises the device, returns the
  * summed milliseconds and launch count recorded since the last read of that class. */
 int lvsr_profile_enable(int on);
 int lvsr_profile_read(const char* kernel_class, double* total_ms, int64_t* count);
