@@ -157,7 +157,7 @@ int fork_copy(lvsr_model* m, const ForkLayout& f, float* W, float* b, float* gra
   for (int bias = 0; bias < 2; ++bias)
     for (const auto& k : f.block) {
       const Param* p = m->param(f.fork + "/" + k.param + (bias ? ".b" : ".W"));
-      LVSR_CHECK(p, "fork_copy: %s has no parameter %s", f.fork.c_str(), k.param);
+      LVSR_CHECK(p, "fork_copy: %s has no parameter %s", f.fork.c_str(), k.param.c_str());
       float* packed = (bias ? b : W) + k.col;
       if (int rc = grads ? copy2d(grads + p->offset, k.cols, packed, f.ld, bias ? 1 : f.rows, k.cols, st)   // scatter gradients
                          : copy2d(packed, f.ld, p->dev, k.cols, bias ? 1 : f.rows, k.cols, st)) return rc;   // pack parameters
@@ -192,7 +192,7 @@ int glimpses(lvsr_model* m, const float* H, const float* P, const float* maskH, 
   float* lohi = ws.f32((size_t)2 * R);
   LVSR_CHECK(q && win && lohi, "out of device memory (workspace)");
   DenseArgs d = {};
-  d.X1 = states; d.K1 = state_dim(m); d.W1 = att_state_weights(m);
+  d.op[0] = {states, state_dim(m), state_dim(m), att_state_weights(m), c.dim_matcher};
   d.R = R; d.N = c.dim_matcher; d.mode = DENSE_PLAIN; d.out = q;
   if (int rc = dense_step(d, st)) return rc;
   WindowArgs wa = {};
@@ -213,71 +213,46 @@ int glimpses(lvsr_model* m, const float* H, const float* P, const float* maskH, 
   return attention_step(a, !content_attention(m), &m->att_cs, st);
 }
 
-// compute_states for R rows: distribute + fork(feedback) + GRU step.
-int transition(lvsr_model* m, int R, const float* states, const float* ctx, const long long* outputs,
-               const float* rmask, float* next_states, cudaStream_t st) {
+// compute_states for R state rows of stride S = state_dim(m): distribute + fork(feedback) + GRU step, layer by layer.
+// Layer l reads states[:, lC : (l+1)C] and writes next_states[:, lC : (l+1)C]; with dec_stack 2, layer 1 also takes
+// layer 0's new state next_states[:, :C] through the RecurrentStack's bias-free fork_1 (recurrent.py:925-950).  The
+// layers share one z / hr / ai scratch set (stream order).  next_states may be states: each launch reads a state
+// element before the launch that overwrites it, or in the thread that overwrites it.
+static int transition(lvsr_model* m, int R, const float* states, const float* ctx, const long long* outputs,
+                      const float* rmask, float* next_states, cudaStream_t st) {
   const lvsr_config& c = m->cfg;
   Arena& ws = m->ws;
-  const int C = c.dim_dec;
+  const int C = c.dim_dec, S = state_dim(m);
   float* z = ws.f32((size_t)R * C);
   float* hr = ws.f32((size_t)R * C);
   float* ai = ws.f32((size_t)R * C);
   LVSR_CHECK(z && hr && ai, "out of device memory (workspace)");
-  DenseArgs g = {};
-  g.X1 = ctx; g.K1 = m->E; g.W1 = m->Wd_cat;
-  g.X2 = states; g.K2 = C; g.W2 = m->P(dec_gru(m, 0) + ".state_to_gates"); g.N2 = 2 * C;
-  g.add = m->FF; g.arow = outputs; g.add_rows = c.num_phonemes + 1; g.R = R; g.N = 3 * C; g.mode = DENSE_GATES;
-  g.s = states; g.z = z; g.hr = hr; g.ai = ai; g.C = C;
-  if (int rc = dense_step(g, st)) return rc;
-  DenseArgs k = {};
-  k.X1 = hr; k.K1 = C; k.W1 = m->P(dec_gru(m, 0) + ".state_to_state");
-  k.add = ai; k.arow = nullptr; k.R = R; k.N = C; k.mode = DENSE_CAND;
-  k.s = states; k.z = z; k.rmask = rmask; k.out = next_states; k.C = C;
-  return dense_step(k, st);
-}
-
-// RecurrentStack.apply of dec_stack 2 for R wide state rows [s0 | s1] (row stride 2C): layer 0 is transition() on a
-// contiguous copy of s0, layer 1 then takes layer 0's new state through fork_1 (recurrent.py:925-950).
-static int stack_transition(lvsr_model* m, int R, const float* states, const float* ctx, const long long* outputs,
-                            const float* rmask, float* next_states, cudaStream_t st) {
-  const lvsr_config& c = m->cfg;
-  Arena& ws = m->ws;
-  const int C = c.dim_dec, S = 2 * C;
-  float* s0 = ws.f32((size_t)R * C);
-  float* s0n = ws.f32((size_t)R * C);
-  float* z = ws.f32((size_t)R * C);
-  float* hr = ws.f32((size_t)R * C);
-  float* ai = ws.f32((size_t)R * C);
-  LVSR_CHECK(s0 && s0n && z && hr && ai, "out of device memory (workspace)");
-  if (int rc = copy2d(s0, C, states, S, R, C, st)) return rc;
-  if (int rc = transition(m, R, s0, ctx, outputs, rmask, s0n, st)) return rc;
-  StackUpperArgs u = {};
-  u.R = R; u.C = C; u.E = m->E;
-  u.ctx = ctx; u.s0n = s0n; u.ld_s0n = C; u.s1 = states + C; u.ld_s1 = S;
-  u.outputs = outputs; u.ff_rows = c.num_phonemes + 1; u.rmask = rmask;
-  u.Wd = m->stack.Wd; u.FF = m->stack.FF; u.F = m->stack.F;
-  u.U = m->P(dec_gru(m, 1) + ".state_to_gates"); u.W = m->P(dec_gru(m, 1) + ".state_to_state");
-  u.z = z; u.hr = hr; u.ai = ai; u.out = next_states + C; u.ld_out = S;
-  if (int rc = stack_upper_step(u, st)) return rc;
-  return copy2d(next_states, S, s0n, C, R, C, st);
-}
-
-// compute_states of the decoder, whatever its depth
-static int dec_transition(lvsr_model* m, int R, const float* states, const float* ctx, const long long* outputs,
-                          const float* rmask, float* next_states, cudaStream_t st) {
-  if (m->cfg.dec_stack == 2) return stack_transition(m, R, states, ctx, outputs, rmask, next_states, st);
-  return transition(m, R, states, ctx, outputs, rmask, next_states, st);
+  for (int l = 0; l < c.dec_stack; ++l) {
+    const lvsr_model::DecLayer& in = m->dec[l];
+    const float* s = states + (size_t)l * C;
+    DenseArgs g = {};
+    g.op[0] = {ctx, m->E, m->E, in.Wd, 3 * C};
+    if (l == 1) g.op[1] = {next_states, C, S, m->stack.F, 3 * C};
+    g.op[l + 1] = {s, C, S, m->P(dec_gru(m, l) + ".state_to_gates"), 2 * C};   // the layer's own state comes last
+    g.add = in.FF; g.arow = outputs; g.add_rows = c.num_phonemes + 1; g.R = R; g.N = 3 * C; g.mode = DENSE_GATES;
+    g.s = s; g.ld_s = S; g.z = z; g.hr = hr; g.ai = ai; g.C = C;
+    if (int rc = dense_step(g, st)) return rc;
+    DenseArgs k = {};
+    k.op[0] = {hr, C, C, m->P(dec_gru(m, l) + ".state_to_state"), C};
+    k.add = ai; k.arow = nullptr; k.R = R; k.N = C; k.mode = DENSE_CAND;
+    k.s = s; k.ld_s = S; k.z = z; k.rmask = rmask; k.out = next_states + (size_t)l * C; k.ld_out = S; k.C = C;
+    if (int rc = dense_step(k, st)) return rc;
+  }
+  return 0;
 }
 
 int readout_merged(lvsr_model* m, int R, const float* states, const float* ctx, float* merged, cudaStream_t st) {
   const lvsr_config& c = m->cfg;
   DenseArgs d = {};
-  d.X1 = ctx; d.K1 = m->E; d.W1 = m->P(std::string(GEN) + "/readout/merge/transform_weighted_averages.W");
-  if (c.use_states_for_readout) {
-    d.X2 = states; d.K2 = state_dim(m); d.W2 = readout_state_weights(m);
-    d.N2 = c.post_merge_dim;
-  }
-  d.R = R; d.N = c.post_merge_dim; d.mode = DENSE_PLAIN; d.out = merged;
+  const int S = state_dim(m), N = c.post_merge_dim;
+  d.op[0] = {ctx, m->E, m->E, m->P(std::string(GEN) + "/readout/merge/transform_weighted_averages.W"), N};
+  if (c.use_states_for_readout) d.op[1] = {states, S, S, readout_state_weights(m), N};
+  d.R = R; d.N = N; d.mode = DENSE_PLAIN; d.out = merged;
   return dense_step(d, st);
 }
 
@@ -343,12 +318,10 @@ size_t encoder_ws_bytes(const lvsr_model* m, int T, int B) {
 size_t cost_ws_bytes(const lvsr_model* m, int Tp, int B, int L) {
   const lvsr_config& c = m->cfg;
   const size_t S = state_dim(m);
-  // a stacked step takes s0, s0' and the upper layer's z / hr / ai beside the lower layer's three [B, C] buffers
-  const size_t step_rows = 3 + (size_t)5 * (c.dec_stack - 1);
   size_t f = (size_t)Tp * B * c.dim_matcher + (size_t)2 * Tp * B * m->E + (size_t)(L + 1) * B * S + (size_t)L * B * m->E +
              (size_t)4 * B * Tp + (size_t)L * B * c.post_merge_dim + (size_t)B * c.dim_matcher +
              (size_t)L * B * (Tp + c.dim_matcher + S + 1) +
-             step_rows * B * c.dim_dec + 4 * B + 64;
+             (size_t)3 * B * c.dim_dec + 4 * B + 64;
   return f * sizeof(float) + (1 << 16);
 }
 
@@ -486,11 +459,9 @@ int lvsr_model_destroy(lvsr_model* m) {
   for (TcWeights& t : m->Wcat_tc) if (t.mem) cudaFree(t.mem);
   for (TcWeights& t : m->bottom_tc) if (t.mem) cudaFree(t.mem);
   if (m->Wp_tc.mem) cudaFree(m->Wp_tc.mem);
-  if (m->Wd_cat) cudaFree(m->Wd_cat);
+  for (const lvsr_model::DecLayer& d : m->dec)
+    for (float* p : {d.Wd, d.Wff, d.bff, d.FF}) if (p) cudaFree(p);
   if (m->Wb1) cudaFree(m->Wb1);
-  if (m->Wff_cat) cudaFree(m->Wff_cat);
-  if (m->bff_cat) cudaFree(m->bff_cat);
-  if (m->FF) cudaFree(m->FF);
   if (m->stack.mem) cudaFree(m->stack.mem);
   if (m->status) cudaFree(m->status);
   if (m->enc_tiles) cudaFree(m->enc_tiles);
@@ -728,22 +699,24 @@ int finalize_on_stream(lvsr_model* m, cudaStream_t st, bool synchronise) {
       m->bcat.push_back(b);
     }
     const int C = c.dim_dec;
-    LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->Wd_cat), (size_t)m->E * 3 * C * sizeof(float)));
+    for (int l = 0; l < c.dec_stack; ++l) {
+      lvsr_model::DecLayer& d = m->dec[l];
+      LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&d.Wd), (size_t)m->E * 3 * C * sizeof(float)));
+      LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&d.Wff), (size_t)c.dim_feedback * 3 * C * sizeof(float)));
+      LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&d.bff), (size_t)3 * C * sizeof(float)));
+      LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&d.FF), (size_t)(c.num_phonemes + 1) * 3 * C * sizeof(float)));
+    }
     LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->Wb1), (size_t)(m->E + C) * 3 * C * sizeof(float)));
-    LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->Wff_cat), (size_t)c.dim_feedback * 3 * C * sizeof(float)));
-    LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->bff_cat), (size_t)3 * C * sizeof(float)));
-    LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->FF), (size_t)(c.num_phonemes + 1) * 3 * C * sizeof(float)));
     if (c.dec_stack == 2) {
       lvsr_model::Stack& s = m->stack;
-      const size_t n[8] = {(size_t)2 * C * c.dim_matcher, (size_t)2 * C * c.post_merge_dim, (size_t)2 * C,
-                           (size_t)m->E * 3 * C, (size_t)c.dim_feedback * 3 * C, (size_t)3 * C,
-                           (size_t)(c.num_phonemes + 1) * 3 * C, (size_t)C * 3 * C};
+      const size_t n[4] = {(size_t)2 * C * c.dim_matcher, (size_t)2 * C * c.post_merge_dim, (size_t)2 * C,
+                           (size_t)C * 3 * C};
       size_t total = 0;
       for (size_t k : n) total += (k + 63) & ~(size_t)63;      // 256-byte aligned pieces
       LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&s.mem), total * sizeof(float)));
-      float** piece[8] = {&s.Ws, &s.Wm, &s.h0, &s.Wd, &s.Wff, &s.bff, &s.FF, &s.F};
+      float** piece[4] = {&s.Ws, &s.Wm, &s.h0, &s.F};
       float* p = s.mem;
-      for (int i = 0; i < 8; ++i) { *piece[i] = p; p += (n[i] + 63) & ~(size_t)63; }
+      for (int i = 0; i < 4; ++i) { *piece[i] = p; p += (n[i] + 63) & ~(size_t)63; }
     }
   }
   for (int l = 0; l < c.num_layers; ++l)
@@ -751,13 +724,26 @@ int finalize_on_stream(lvsr_model* m, cudaStream_t st, bool synchronise) {
       if (int rc = fork_copy(m, encoder_fork(m, l, dir), m->Wcat[l], m->bcat[l], nullptr, st)) return rc;
   const int C = c.dim_dec, Cfb = c.dim_feedback, V = c.num_phonemes;
   const std::string g = GEN, t = TR;
-  // decoder-side packing: gate columns first (update | reset), then the candidate inputs
-  if (int rc = copy2d(m->Wd_cat, 3 * C, m->P(t + "/distribute/fork_gate_inputs.W"), 2 * C, m->E, 2 * C, st)) return rc;
-  if (int rc = copy2d(m->Wd_cat + 2 * C, 3 * C, m->P(t + "/distribute/fork_inputs.W"), C, m->E, C, st)) return rc;
+  // decoder-side packing, per layer: gate columns first (update | reset), then the candidate inputs
+  for (int l = 0; l < c.dec_stack; ++l) {
+    const lvsr_model::DecLayer& d = m->dec[l];
+    const std::string x = layer_suffix(l);
+    const std::string dist = t + "/distribute/";
+    if (int rc = copy2d(d.Wd, 3 * C, m->P(dist + "fork_gate_inputs" + x + ".W"), 2 * C, m->E, 2 * C, st)) return rc;
+    if (int rc = copy2d(d.Wd + 2 * C, 3 * C, m->P(dist + "fork_inputs" + x + ".W"), C, m->E, C, st)) return rc;
+    if (int rc = fork_copy(m, feedback_fork(c, l), d.Wff, d.bff, nullptr, st)) return rc;
+    // fork(feedback(y)) for every symbol y, once: [(V+1), 3C]
+    if (c.one_of_n_feedback) {
+      // one-hot feedback: fork(feedback(y)) is row y of the fork weights plus the bias
+      if (int rc = add_bias_rows(d.FF, d.Wff, d.bff, V + 1, 3 * C, st)) return rc;
+    } else {
+      GemmArgs ff = make_gemm(m->P(g + "/readout/lookupfeedback/lookuptable.W"), V + 1, Cfb, d.Wff, 3 * C, d.bff, d.FF);
+      if (int rc = gemm_bias(ff, st)) return rc;
+    }
+  }
   LVSR_CUDA_OK(cudaMemsetAsync(m->Wb1, 0, (size_t)(m->E + C) * 3 * C * sizeof(float), st));
-  if (int rc = copy2d(m->Wb1, 3 * C, m->Wd_cat, 3 * C, m->E, 3 * C, st)) return rc;
+  if (int rc = copy2d(m->Wb1, 3 * C, m->dec[0].Wd, 3 * C, m->E, 3 * C, st)) return rc;
   if (int rc = copy2d(m->Wb1 + (size_t)m->E * 3 * C, 3 * C, m->P(dec_gru(m, 0) + ".state_to_gates"), 2 * C, C, 2 * C, st)) return rc;
-  if (int rc = fork_copy(m, feedback_fork(c), m->Wff_cat, m->bff_cat, nullptr, st)) return rc;
   // tensor-core operands of the fork and preprocess weights (K-major fp16 head/tail planes or tf32 hi/lo pairs)
   m->use_tc = getenv("LVSR_NO_TC_GEMM") == nullptr;
   if (m->use_tc) {
@@ -773,17 +759,8 @@ int finalize_on_stream(lvsr_model* m, cudaStream_t st, bool synchronise) {
                                    st))
         return rc;
   }
-  // fork(feedback(y)) for every symbol y, once: [(V+1), 3C]
-  if (c.one_of_n_feedback) {
-    // one-hot feedback: fork(feedback(y)) is row y of the fork weights plus the bias
-    if (int rc = add_bias_rows(m->FF, m->Wff_cat, m->bff_cat, V + 1, 3 * C, st)) return rc;
-  } else {
-    GemmArgs ff = make_gemm(m->P(g + "/readout/lookupfeedback/lookuptable.W"), V + 1, Cfb, m->Wff_cat, 3 * C,
-                            m->bff_cat, m->FF);
-    if (int rc = gemm_bias(ff, st)) return rc;
-  }
   if (c.dec_stack == 2) {
-    // the wide state's row-stacked weights [W ; W#1], both initial states, and layer 1's counterparts of Wd_cat / FF
+    // the wide state's row-stacked weights [W ; W#1], both initial states, and fork_1 of layer 0's new state
     lvsr_model::Stack& s = m->stack;
     const int M = c.dim_matcher, Cpm = c.post_merge_dim;
     const std::string a = att_base(m), r = t + "/recurrentstack";
@@ -796,17 +773,8 @@ int finalize_on_stream(lvsr_model* m, cudaStream_t st, bool synchronise) {
     }
     if (int rc = copy2d(s.h0, C, m->P(dec_gru(m, 0) + ".initial_state"), C, 1, C, st)) return rc;
     if (int rc = copy2d(s.h0 + C, C, m->P(dec_gru(m, 1) + ".initial_state"), C, 1, C, st)) return rc;
-    if (int rc = copy2d(s.Wd, 3 * C, m->P(t + "/distribute/fork_gate_inputs#1.W"), 2 * C, m->E, 2 * C, st)) return rc;
-    if (int rc = copy2d(s.Wd + 2 * C, 3 * C, m->P(t + "/distribute/fork_inputs#1.W"), C, m->E, C, st)) return rc;
     if (int rc = copy2d(s.F, 3 * C, m->P(r + "/fork_1/fork_gate_inputs.W"), 2 * C, C, 2 * C, st)) return rc;
     if (int rc = copy2d(s.F + 2 * C, 3 * C, m->P(r + "/fork_1/fork_inputs.W"), C, C, C, st)) return rc;
-    if (int rc = fork_copy(m, stack_feedback_fork(c), s.Wff, s.bff, nullptr, st)) return rc;
-    if (c.one_of_n_feedback) {
-      if (int rc = add_bias_rows(s.FF, s.Wff, s.bff, V + 1, 3 * C, st)) return rc;
-    } else {
-      GemmArgs ff = make_gemm(m->P(g + "/readout/lookupfeedback/lookuptable.W"), V + 1, Cfb, s.Wff, 3 * C, s.bff, s.FF);
-      if (int rc = gemm_bias(ff, st)) return rc;
-    }
   }
   m->v_bias = 0.f;
   if (c.energy_normalizer != LVSR_NORM_SOFTMAX) {
@@ -1087,7 +1055,7 @@ int lvsr_cost_matrix(lvsr_model* m, const float* attended, const float* attended
     d.Wb1 = m->Wb1;
     d.Wstate = m->P(dec_gru(m, 0) + ".state_to_state");
     d.Ws = m->P(att_base(m) + "/state_trans/transform_states.W");
-    d.FF = m->FF;
+    d.FF = m->dec[0].FF;
     d.labels = lab; d.lmask = labels_mask;
     d.s_all = s_all; d.ctx_all = ctx_all; d.w0 = w0; d.w_all = weights_out;
     d.e_seq = energies_out; d.e_scratch = e_scratch;
@@ -1106,8 +1074,8 @@ int lvsr_cost_matrix(lvsr_model* m, const float* attended, const float* attended
     const float* s_i = s_all + (size_t)i * B * S;
     ArenaMark mark{ws};   // per-step scratch is reusable (stream order): rewound at the end of every step
     if (int rc = glimpses(m, attended, P, attended_mask, Tp, B, nullptr, B, s_i, w_prev, nullptr, i, w_i, e_i, ctx_i, st)) return rc;
-    if (int rc = dec_transition(m, B, s_i, ctx_i, lab + (size_t)i * B, labels_mask ? labels_mask + (size_t)i * B : nullptr,
-                                s_all + (size_t)(i + 1) * B * S, st)) return rc;
+    if (int rc = transition(m, B, s_i, ctx_i, lab + (size_t)i * B, labels_mask ? labels_mask + (size_t)i * B : nullptr,
+                            s_all + (size_t)(i + 1) * B * S, st)) return rc;
     w_prev = w_i;
   }
   // the language model's cost rows in force before each label (sequence_generators.py:284-289), then fused below
@@ -1220,7 +1188,7 @@ int lvsr_next_states(lvsr_model* m, const float* attended, const float* preproce
   }
   if (int rc = glimpses(m, attended, P, attended_mask, Tp, U, row_utt, R, states, weights,
                         reinterpret_cast<const long long*>(step), 0, next_weights, next_energies, next_wavg, st)) return rc;
-  if (int rc = dec_transition(m, R, states, next_wavg, reinterpret_cast<const long long*>(outputs), nullptr, next_states, st))
+  if (int rc = transition(m, R, states, next_wavg, reinterpret_cast<const long long*>(outputs), nullptr, next_states, st))
     return rc;
   return add_i64(reinterpret_cast<long long*>(next_step), reinterpret_cast<const long long*>(step), R, 1, st);
 }
@@ -1284,7 +1252,7 @@ int search_advance(lvsr_model* m, const float* attended, const float* preprocess
     if (int rc = glimpses(m, attended, preprocessed, attended_mask, Tp, U, row_utt, Rn, s_sel, w_sel, st_sel, 0, n_weights,
                           n_energies, n_wavg, st, sg)) return rc;
   }
-  if (int rc = dec_transition(m, Rn, s_sel, n_wavg, symbols, nullptr, n_states, st)) return rc;
+  if (int rc = transition(m, Rn, s_sel, n_wavg, symbols, nullptr, n_states, st)) return rc;
   return gather_i64(n_step, step, parent, Rn, 1, st);
 }
 

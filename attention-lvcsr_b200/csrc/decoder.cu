@@ -6,6 +6,8 @@
 //   Distribute + GatedRecurrent step    ctx.W_d + fork(feedback) -> gates -> candidate -> blend
 //                                        (B/bricks/attention.py:625-662, B/bricks/parallel.py:249-265,
 //                                         B/bricks/recurrent.py:608-620)
+//   RecurrentStack step (dec_stack 2)   each layer as above; layer 1 adds fork_1 of layer 0's new state
+//                                        (B/bricks/recurrent.py:925-950)
 // and, once per sequence / search step, Readout.readout + SoftmaxEmitter
 //   (B/bricks/sequence_generators.py:614-619, 780-795; lvsr/bricks/recognizer.py:298-320;
 //    B/bricks/simple.py:175-181, 335-371).
@@ -37,14 +39,14 @@ __global__ void __launch_bounds__(256) dense_kernel(DenseArgs a) {
 #pragma unroll
     for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
 
-  auto run = [&](const float* X, int K, const float* W, int ldw, int ncols) {
-    if (X == nullptr || c0 >= ncols) return;
+  auto run = [&](const DenseOperand& p) {
+    if (p.X == nullptr || c0 >= p.ncols) return;
     // warp `warp` owns k in [k_lo, k_hi), a multiple-of-4 aligned slice
-    const int kq = (K / 4 + 7) / 8;            // float4 groups per warp
-    const int k_lo = min(K, warp * kq * 4), k_hi = min(K, k_lo + kq * 4);
+    const int kq = (p.K / 4 + 7) / 8;          // float4 groups per warp
+    const int k_lo = min(p.K, warp * kq * 4), k_hi = min(p.K, k_lo + kq * 4);
     const float* xr[4];
 #pragma unroll
-    for (int i = 0; i < 4; ++i) xr[i] = X + (long long)min(rbase + i, a.R - 1) * K;
+    for (int i = 0; i < 4; ++i) xr[i] = p.X + (long long)min(rbase + i, a.R - 1) * p.ldx;
     int k = k_lo;
     for (; k + 4 <= k_hi; k += 4) {
       float4 xv[4];
@@ -52,7 +54,7 @@ __global__ void __launch_bounds__(256) dense_kernel(DenseArgs a) {
       for (int i = 0; i < 4; ++i) xv[i] = *reinterpret_cast<const float4*>(xr[i] + k);
       float4 wv[4];
 #pragma unroll
-      for (int kk = 0; kk < 4; ++kk) wv[kk] = __ldg(reinterpret_cast<const float4*>(W + (long long)(k + kk) * ldw + c0));
+      for (int kk = 0; kk < 4; ++kk) wv[kk] = __ldg(reinterpret_cast<const float4*>(p.W + (long long)(k + kk) * p.ncols + c0));
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         const float xs[4] = {xv[i].x, xv[i].y, xv[i].z, xv[i].w};
@@ -66,8 +68,9 @@ __global__ void __launch_bounds__(256) dense_kernel(DenseArgs a) {
       }
     }
   };
-  run(a.X1, a.K1, a.W1, a.N, a.N);
-  run(a.X2, a.K2, a.W2, a.N2, a.N2);
+  run(a.op[0]);
+  run(a.op[1]);
+  run(a.op[2]);
 
 #pragma unroll
   for (int i = 0; i < 4; ++i)
@@ -95,7 +98,7 @@ __global__ void __launch_bounds__(256) dense_kernel(DenseArgs a) {
         a.z[(long long)r * C + c] = sigmoidf_acc(v);
       } else if (c < 2 * C) {
         const int uu = c - C;
-        a.hr[(long long)r * C + uu] = a.s[(long long)r * C + uu] * sigmoidf_acc(v);
+        a.hr[(long long)r * C + uu] = a.s[(long long)r * a.ld_s + uu] * sigmoidf_acc(v);
       } else {
         a.ai[(long long)r * C + (c - 2 * C)] = v;
       }
@@ -103,13 +106,13 @@ __global__ void __launch_bounds__(256) dense_kernel(DenseArgs a) {
       const int C = a.C;
       const float cand = tanhf_acc(v);
       const float z = a.z[(long long)r * C + c];
-      const float sold = a.s[(long long)r * C + c];
+      const float sold = a.s[(long long)r * a.ld_s + c];
       float sn = cand * z + sold * (1.f - z);
       if (a.rmask) {
         const float m = a.rmask[r];
         sn = m * sn + (1.f - m) * sold;
       }
-      a.out[(long long)r * C + c] = sn;
+      a.out[(long long)r * a.ld_out + c] = sn;
     }
   }
 }
@@ -316,8 +319,10 @@ inline int grid_for(long long n) { return (int)std::min<long long>(2048, std::ma
 int dense_step(const DenseArgs& a, cudaStream_t stream) {
   ProfScope prof("dense", stream);
   if (a.R <= 0) return 0;
-  LVSR_CHECK(a.N % 4 == 0 && a.K1 % 4 == 0 && (a.X2 == nullptr || (a.K2 % 4 == 0 && a.N2 % 4 == 0)),
-             "dense_step: dimensions must be multiples of 4 (N=%d K1=%d K2=%d)", a.N, a.K1, a.K2);
+  LVSR_CHECK(a.N % 4 == 0, "dense_step: N=%d is not a multiple of 4", a.N);
+  for (const DenseOperand& p : a.op)
+    LVSR_CHECK(!p.X || (p.K % 4 == 0 && p.ldx % 4 == 0 && p.ncols % 4 == 0),
+               "dense_step: dimensions and strides must be multiples of 4 (K=%d ldx=%d ncols=%d)", p.K, p.ldx, p.ncols);
   dim3 grid(ceil_div(a.N, DN), ceil_div(a.R, DR));
   dense_kernel<<<grid, 256, 0, stream>>>(a);
   LVSR_LAUNCH_CHECK();

@@ -155,11 +155,14 @@ int attention_step(const AttStepArgs& a, bool location, int* cs_out, cudaStream_
 int attention_max_cluster();
 
 // ---- decoder.cu ---------------------------------------------------------------------
-// out[R,N] = epilogue( X1[R,K1].W1[K1,N] (+ X2[R,K2].W2[K2,N2], columns < N2 only) + add[arow[r]] )
+// out[R,N] = epilogue( sum over the operands, in order, of X[R,K].W[K,ncols] (columns < ncols only) + add[arow[r]] )
 enum { DENSE_PLAIN = 0, DENSE_GATES = 1, DENSE_CAND = 2 };
+struct DenseOperand {
+  const float* X; int K, ldx;   // X [R, K], row stride ldx; null: no operand
+  const float* W; int ncols;    // W [K, ncols], ncols <= N
+};
 struct DenseArgs {
-  const float* X1; int K1; const float* W1;        // W1 [K1, N]
-  const float* X2; int K2; const float* W2; int N2; // W2 [K2, N2], may be null
+  DenseOperand op[3];
   const float* add;        // [*, N] addend rows or nullptr
   const long long* arow;   // [R] row index into add (labels) or nullptr (identity)
   long long add_rows;      // rows of `add` when arow is given (0 = unknown): indices are clamped into the table
@@ -167,11 +170,11 @@ struct DenseArgs {
   // DENSE_PLAIN: out[R,N]
   float* out;
   // DENSE_GATES (N = 3C): cols [0,C) update -> z[R,C]; [C,2C) reset -> hr[R,C] = s*r; [2C,3C) -> ai[R,C]
-  // DENSE_CAND  (N = C):  c = tanh(acc + ai); s' = c*z + s*(1-z); optional row mask blend -> out[R,C]
-  const float* s;          // [R, C] current states
+  // DENSE_CAND  (N = C):  c = tanh(acc + ai); s' = c*z + s*(1-z); optional row mask blend -> out[R,C], row stride ld_out
+  const float* s; int ld_s;   // [R, C] current states, row stride ld_s
   float* z; float* hr; float* ai;
   const float* rmask;      // [R] or nullptr
-  int C;
+  int C, ld_out;
 };
 int dense_step(const DenseArgs& a, cudaStream_t stream);
 
@@ -217,28 +220,6 @@ int lm_path(const LmFst& f, int L, int B, const long long* labels, const float* 
 // dst row r = src row idx[r] of the (states, weights, add) triple
 int lm_gather(int* states, double* weights, float* add, const int* src_states, const double* src_weights,
               const float* src_add, const int* idx, int Rn, int V, cudaStream_t stream);
-
-// ---- dec_stack.cu: upper GRU of a two-layer RecurrentStack with skip connections (dec_stack 2) -------------------
-// One step of layer 1 for R rows (libs/blocks/blocks/bricks/recurrent.py:925-950, B/bricks/recurrent.py:608-620):
-//   gate inputs  g = ctx.Wd[:, :2C] + FF[y, :2C] + s0n.F[:, :2C] + s1.U        (U = state_to_gates [C, 2C])
-//   inputs       a = ctx.Wd[:, 2C:] + FF[y, 2C:] + s0n.F[:, 2C:]
-//   z, r = sigmoid(g); c = tanh((s1 * r).W + a); s1' = c z + s1 (1 - z), blended by the row mask
-// s0n is layer 0's new state of the same step.  The states live in the wide rows [s0 | s1]: s1, s0n and out carry
-// their own row strides.  Two launches (gates, candidate) of the dense tiling of decoder.cu.
-struct StackUpperArgs {
-  int R, C, E;
-  const float* ctx;                 // [R, E] glimpses of the step
-  const float* s0n; int ld_s0n;     // [R, C] layer 0's new state
-  const float* s1; int ld_s1;       // [R, C] layer 1's state
-  const long long* outputs;         // [R] fed-back symbols: rows of FF (clamped into [0, ff_rows))
-  int ff_rows;
-  const float* rmask;               // [R] or nullptr
-  const float *Wd, *FF, *F;         // [E, 3C], [ff_rows, 3C], [C, 3C]: gate columns first, then the inputs
-  const float *U, *W;               // state_to_gates [C, 2C], state_to_state [C, C]
-  float *z, *hr, *ai;               // [R, C] scratch each
-  float* out; int ld_out;           // [R, C] layer 1's new state
-};
-int stack_upper_step(const StackUpperArgs& a, cudaStream_t stream);
 
 // ---- dec_scan.cu: persistent teacher-forced decoder -----------------------------------
 // The caller's inputs.  The hand-over protocol between the kernel's CTAs is dec_scan.cu's alone: run_dec_scan takes

@@ -116,22 +116,22 @@ struct lvsr_model {
   int64_t flat_count = 0;
   // packed, kernel-side weights (rebuilt by finalize)
   std::vector<float*> Wcat, bcat;   // per encoder layer: [Din, 6D], [6D] (encoder_fork)
-  float* Wd_cat = nullptr;          // [E, 3C] = [distribute gate_inputs (2C) | distribute inputs (C)]
-  float* Wb1 = nullptr;             // [E+C, 3C] = Wd_cat stacked on [state_to_gates | 0] (persistent decoder)
-  float* Wff_cat = nullptr;         // [Cfb, 3C] (feedback_fork)
-  float* bff_cat = nullptr;         // [3C]
-  float* FF = nullptr;              // [(V+1), 3C] = lookup . Wff_cat + bff_cat
-  // dec_stack 2 (finalize; all inside stack_mem): the attention and the readout see the wide state [s0 | s1] through
-  // row-stacked weights, and the upper layer's packed inputs mirror Wd_cat / FF of the lower one
+  // the packed inputs of decoder layer l < dec_stack (finalize), gate columns first (update | reset), then the
+  // candidate inputs; the parameters of layer l > 0 carry the suffix "#l" (layer_suffix)
+  struct DecLayer {
+    float* Wd = nullptr;            // [E, 3C]     distribute [fork_gate_inputs | fork_inputs]
+    float* Wff = nullptr;           // [Cfb, 3C]   generator fork (feedback_fork)
+    float* bff = nullptr;           // [3C]
+    float* FF = nullptr;            // [(V+1), 3C] = feedback . Wff + bff
+  } dec[2];
+  float* Wb1 = nullptr;             // [E+C, 3C] = dec[0].Wd stacked on [state_to_gates | 0] (persistent decoder)
+  // dec_stack 2 (finalize; all inside mem): the attention and the readout see the wide state [s0 | s1] through
+  // row-stacked weights
   struct Stack {
     float* mem = nullptr;           // the one allocation of the buffers below
     float* Ws = nullptr;            // [2C, M]   state_trans/transform_states.W ; transform_states#1.W
     float* Wm = nullptr;            // [2C, Cpm] readout/merge/transform_states.W ; transform_states#1.W
     float* h0 = nullptr;            // [2C]      initial_state of both layers
-    float* Wd = nullptr;            // [E, 3C]   distribute [fork_gate_inputs#1 | fork_inputs#1]
-    float* Wff = nullptr;           // [Cfb, 3C] generator fork [fork_gate_inputs#1 | fork_inputs#1]
-    float* bff = nullptr;           // [3C]
-    float* FF = nullptr;            // [(V+1), 3C] = feedback . Wff + bff
     float* F = nullptr;             // [C, 3C]   recurrentstack/fork_1 [fork_gate_inputs | fork_inputs] (no bias)
   } stack;
   // dense-projection weights as the tensor-core GEMM reads them (wgmma path); empty = SIMT path
@@ -297,20 +297,21 @@ static inline std::string bottom_linear(int i) { return "/recognizer/bottom/bott
 static inline int bottom_input_dim(const lvsr_model* m, int i) { return i ? m->bottom.dims[i - 1] : m->cfg.num_features; }
 
 // A packed fork, blocks in column order: <fork>/<param>.W fills columns [col, col + cols) of W [rows, ld], .b those of b [ld]
-struct ForkLayout { std::string fork; int rows, ld; struct { const char* param; int col, cols; } block[2]; };
+struct ForkLayout { std::string fork; int rows, ld; struct { std::string param; int col, cols; } block[2]; };
 // encoder layer l, direction dir, in Wcat[l] / bcat[l]: per direction [inputs D | gate_inputs 2D (update | reset)]
 static inline ForkLayout encoder_fork(const lvsr_model* m, int l, int dir) {
   const lvsr_config& c = m->cfg;
   const int D = c.dims_bidir[l], c0 = dir * 3 * D, din = l ? 2 * c.dims_bidir[l - 1] : encoder_input_dim(m);
   return {enc_base(l, dir) + "/fork", din, 6 * D, {{"fork_inputs", c0, D}, {"fork_gate_inputs", c0 + D, 2 * D}}};
 }
-// fork(feedback(y)) in Wff_cat / bff_cat: [gate_inputs 2C | inputs C]
-static inline ForkLayout feedback_fork(const lvsr_config& c) {
-  return {std::string(GEN) + "/fork", c.dim_feedback, 3 * c.dim_dec, {{"fork_gate_inputs", 0, 2 * c.dim_dec}, {"fork_inputs", 2 * c.dim_dec, c.dim_dec}}};
-}
-// the same for the upper layer of dec_stack 2 (outputs "inputs#1", "gate_inputs#1"), in Stack::Wff / Stack::bff
-static inline ForkLayout stack_feedback_fork(const lvsr_config& c) {
-  return {std::string(GEN) + "/fork", c.dim_feedback, 3 * c.dim_dec, {{"fork_gate_inputs#1", 0, 2 * c.dim_dec}, {"fork_inputs#1", 2 * c.dim_dec, c.dim_dec}}};
+// Suffix of the names of decoder layer l's inputs: "" for layer 0, "#<l>" above it (the RecurrentStack's names of
+// layer l's sequences, libs/blocks/blocks/bricks/recurrent.py:819-820)
+static inline std::string layer_suffix(int l) { return l ? "#" + std::to_string(l) : ""; }
+// fork(feedback(y)) of decoder layer l in dec[l].Wff / dec[l].bff: [gate_inputs 2C | inputs C]
+static inline ForkLayout feedback_fork(const lvsr_config& c, int l) {
+  const std::string x = layer_suffix(l);
+  return {std::string(GEN) + "/fork", c.dim_feedback, 3 * c.dim_dec,
+          {{"fork_gate_inputs" + x, 0, 2 * c.dim_dec}, {"fork_inputs" + x, 2 * c.dim_dec, c.dim_dec}}};
 }
 
 static inline int check_ready(lvsr_model* m) {

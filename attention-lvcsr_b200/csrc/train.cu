@@ -212,7 +212,7 @@ struct TrainStep {
     if (int rc = transpose(m->P(g + "/readout/merge/transform_weighted_averages.W"), WmcT, E, Cpm, st)) return rc;
     if (int rc = transpose(m->P(t + "/transition.state_to_state"), WstateT, C, C, st)) return rc;
     if (int rc = transpose(m->P(t + "/transition.state_to_gates"), WgT, C, 2 * C, st)) return rc;
-    if (int rc = transpose(m->Wd_cat, WdcatT, E, 3 * C, st)) return rc;
+    if (int rc = transpose(m->dec[0].Wd, WdcatT, E, 3 * C, st)) return rc;
     // [dG (3C)] . WcombT [3C, C + E] = [ grad of s_{i-1} through the gates | grad of the glimpse ]: one product per step
     float* WcombT = ws.f32((size_t)3 * C * (C + E));
     LVSR_CHECK(WcombT, "out of device memory (transposed weights)");
@@ -311,9 +311,9 @@ struct TrainStep {
                    win && lohi,
                "out of device memory (decoder backward)");
     if (int rc = lvsr_preprocess(m, d.Hatt, Tp, B, P, st)) return rc;
-    if (int rc = gemm_nn(d.CTX, R, E, E, m->Wd_cat, 3 * C, 3 * C, nullptr, G, 3 * C, false, st)) return rc;
+    if (int rc = gemm_nn(d.CTX, R, E, E, m->dec[0].Wd, 3 * C, 3 * C, nullptr, G, 3 * C, false, st)) return rc;
     if (int rc = gemm_nn(d.S_prev, R, C, C, m->P(t + "/transition.state_to_gates"), 2 * C, 2 * C, nullptr, G, 3 * C, true, st)) return rc;
-    dec_gates_kernel<<<grid1d((long long)R * 3 * C), 256, 0, st>>>(G, m->FF, lab, d.S_prev, R, C, Z, Rg, HR);
+    dec_gates_kernel<<<grid1d((long long)R * 3 * C), 256, 0, st>>>(G, m->dec[0].FF, lab, d.S_prev, R, C, Z, Rg, HR);
     LVSR_LAUNCH_CHECK();
     {
       ArenaMark mark{ws};
@@ -391,7 +391,7 @@ struct TrainStep {
   }
   // Decoder weight gradients: large GEMMs over all steps, the feedback fork, and the sums of the attention constants
   int decoder_weight_grads(const DecTape& d, const DecGrads& dg) const {
-    // state_to_state = HR^T dA ; state_to_gates = S_prev^T [dGz|dGr] ; distribute = CTX^T dG (gate columns first in Wd_cat)
+    // state_to_state = HR^T dA ; state_to_gates = S_prev^T [dGz|dGr] ; distribute = CTX^T dG (gate columns first in dec[0].Wd)
     if (int rc = gemm_tn(ws, dg.HR, C, dg.dG + 2 * C, 3 * C, R, C, C, grad(t + "/transition.state_to_state"), C, false, st)) return rc;
     if (int rc = gemm_tn(ws, d.S_prev, C, dg.dG, 3 * C, R, C, 2 * C, grad(t + "/transition.state_to_gates"), 2 * C, false, st)) return rc;
     if (int rc = gemm_tn(ws, d.CTX, E, dg.dG, 3 * C, R, E, 2 * C, grad(t + "/distribute/fork_gate_inputs.W"), 2 * C, false, st)) return rc;
@@ -421,13 +421,13 @@ struct TrainStep {
       // FF[y] = W_fork[y, :] + b: the gradient of the fork weights IS dFF
       LVSR_CUDA_OK(cudaMemcpyAsync(dWff, dFF, (size_t)(V + 1) * 3 * C * sizeof(float), cudaMemcpyDeviceToDevice, st));
     } else {
-      if (int rc = transpose(m->Wff_cat, WffT, Cfb, 3 * C, st)) return rc;
+      if (int rc = transpose(m->dec[0].Wff, WffT, Cfb, 3 * C, st)) return rc;
       const float* look = m->P(g + "/readout/lookupfeedback/lookuptable.W");
       if (int rc = gemm_nn(dFF, V + 1, 3 * C, 3 * C, WffT, Cfb, Cfb, nullptr, grad(g + "/readout/lookupfeedback/lookuptable.W"), Cfb, false, st)) return rc;
       if (int rc = gemm_tn(ws, look, Cfb, dFF, 3 * C, V + 1, Cfb, 3 * C, dWff, 3 * C, false, st)) return rc;
     }
     if (int rc = colsum(dFF, V + 1, 3 * C, 3 * C, dbff, false, st)) return rc;
-    if (int rc = fork_copy(m, feedback_fork(c), dWff, dbff, grads, st)) return rc;
+    if (int rc = fork_copy(m, feedback_fork(c, 0), dWff, dbff, grads, st)) return rc;
     // attention constants: sums of the per-CTA partials
     reduce_partials_kernel<<<grid1d(M), 256, 0, st>>>(dg.acc_v, nct, M, grad(at + "/energy_comp/linear.W"));
     LVSR_LAUNCH_CHECK();

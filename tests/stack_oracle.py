@@ -10,7 +10,7 @@ attention, tests/content_oracle.py's); only what the stack changes is restated h
     skip connections and is named after layer 1's own sequences (fork_inputs, fork_gate_inputs); every brick that
     took "states" or "inputs" / "gate_inputs" takes "states#1" / "inputs#1" / "gate_inputs#1" too: the attention's
     state_trans, the readout's merge, the generator's fork (with bias) and the distribute fork;
-  * transition (stack_transition): layer 0 is the single-layer GRU step; layer 1's inputs are the distributed
+  * transition (recurrent_stack_step): layer 0 is the single-layer GRU step; layer 1's inputs are the distributed
     glimpses + the feedback fork#1 + fork_1 of layer 0's NEW state (recurrent.py:925-950); both take the row mask;
   * attention and readout receive both states and sum one Linear per state (lvsr/bricks/attention.py:103-106,
     the Merge of lvsr/bricks/recognizer.py:298-301).  That sum is [s0 | s1] . [W ; W#1]: wide_params() stacks the
@@ -126,7 +126,7 @@ def wide_params(cfg, params):
 # --------------------------------------------------------------------------
 
 
-def stack_transition(layers, forks, states, inputs, mask=None):
+def recurrent_stack_step(layers, forks, states, inputs, mask=None):
     """RecurrentStack.do_apply with skip_connections=True for one step (recurrent.py:919-961) of GatedRecurrent
     layers.  layers[l] = dict(state_to_state, state_to_gates); forks[l - 1] = dict(inputs=W, gate_inputs=W), the
     bias-free fork_l of layer l - 1's new state; states[l] [B, C_l]; inputs[l] = (inputs, gate_inputs), layer l's
@@ -165,7 +165,7 @@ def compute_states(cfg, params, states, fed, weighted_averages, mask=None):
     layers = [dict(state_to_state=params[lay + ".state_to_state"], state_to_gates=params[lay + ".state_to_gates"])
               for lay in LAYER]
     forks = [dict(inputs=params[RS + "/fork_1/fork_inputs.W"], gate_inputs=params[RS + "/fork_1/fork_gate_inputs.W"])]
-    s0, s1 = stack_transition(layers, forks, [states[:, :C], states[:, C:]], inputs, mask)
+    s0, s1 = recurrent_stack_step(layers, forks, [states[:, :C], states[:, C:]], inputs, mask)
     return np.concatenate([s0, s1], axis=1)
 
 

@@ -120,7 +120,7 @@ def test_transition_is_blocks_recurrent_stack_with_skip_connections():
     states = [np.zeros((4, D))] * depth
     for i in range(24):
         inputs = [(x_val[i][:, :D], x_val[i][:, D:3 * D])] * depth
-        states = SO.stack_transition(layers, forks, states, inputs, mask_val[i])
+        states = SO.recurrent_stack_step(layers, forks, states, inputs, mask_val[i])
         for d in range(depth):
             assert_allclose(states[d], h_val[d][i + 1], rtol=1e-13, atol=0)
     assert np.all(h_val[:, 13:, 3] == h_val[:, 12:13, 3])         # masked steps keep the state

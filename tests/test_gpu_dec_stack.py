@@ -3,8 +3,8 @@ parameter table, the teacher-forced cost matrix with both layers' states, the Be
 sampled generation, beam search one utterance at a time and in lock-step (with and without an FST language model),
 and a Blocks checkpoint round trip.
 
-The attention and the readout see the wide state rows [s0 | s1]; layer 1 runs on dec_stack.cu's kernels after the
-single-layer step of layer 0, always step-wise (the persistent decoder holds one layer).  Element-wise bounds are
+The attention and the readout see the wide state rows [s0 | s1]; both layers step on decoder.cu's dense_kernel, layer 1
+after layer 0, always step-wise (the persistent decoder holds one layer).  Element-wise bounds are
 test_gpu_attention_plans.py's (DESIGN section 2): weights 5e-5 per element, energies 2e-5 of their scale, costs 1e-5,
 states and weighted averages 1e-4, each with a floor of 0.1 of the tensor's scale.  The oracle decodes the GPU's own
 encoder output, so the comparison measures the decoder alone.

@@ -1,7 +1,7 @@
 """The stacked decoder (net.dec_stack: 2) at the widths, row counts, encoded lengths, streams and entry points the
 single-layer decoder is tested at, against the float64 stack oracle (tests/stack_oracle.py) element by element.
 
-Layer 1 runs on dec_stack.cu's stack_dense_kernel: a CTA owns 8 output columns of a block of 64 rows, its 8 warps split
+Both layers run on decoder.cu's dense_kernel: a CTA owns 8 output columns of a block of 64 rows, its 8 warps split
 each contraction (E, C, C for the gates, C for the candidate) into slices of ceil(K / 32) float4 groups.  The widths of
 test_gpu_widths.py (C = 8, 72 and 200 leave ragged or empty slices) are run here with a stack, both readout settings
 (use_states_for_readout=False drops the merge's two state weights, which finalize then leaves unpacked), every readout
@@ -9,8 +9,8 @@ activation, one-hot feedback and V = 2 to 128; row counts around the kernel's 64
 with ragged label masks, whose masked steps must leave both layers' states bit for bit; 72 rows past the longest row
 one attention CTA holds (cs 2 at T' = 1289 and 2000, bench.NET's decoder widths); greedy and sampled generation at 100
 rows; search_many over the configs[2] shape of bench.py and over long utterances; teacher forcing with an FST language
-model; the stream contract on a non-blocking stream (stack_transition adds two copy2d calls and five workspace buffers to
-every step); validation_statistics, analyze, pickling and compat's search and sample.
+model; the stream contract on a non-blocking stream; validation_statistics, analyze, pickling and compat's search and
+sample.
 
 Every teacher-forced case asserts through SpeechRecognizer.decoder_plan() that the step-wise kernels ran (the persistent
 decoder holds one layer).  Bounds are test_gpu_attention_plans.py's TOL (weights 5e-5 relative per element, energies
@@ -22,14 +22,7 @@ Worst errors measured over this file on an H100 80GB HBM3 (700 W power limit): w
 weighted averages 2.1e-5 (72 rows at T' = 1289), weight sums 2.0e-7, costs 2.5e-6, states 4.9e-5 (E = C = 512, state
 rows of 1024), search costs 6.6e-6, LM-fused costs 3.3e-6 (bound: test_gpu_lm.py's 1e-4), validation_statistics'
 cost sum 7.3e-9, entropy 7.6e-8 and penalty 4.4e-5 relative (bound: 1e-5, 5e-5 and the gate, 1e-4).  The file runs
-in about a minute there, 35 s of it in the two large searches, most of that the oracle's.
-
-Value-only and ordering mutants, each applied alone, fail tests here: stack_dense_kernel slicing K into K / 32
-float4 groups per warp (8 failures: C = 8, 72 and 200; test_gpu_dec_stack.py, the only other file with stacked
-models, passes with it), the
-candidate launch without the row mask (20), finalize packing the readout's stacked weight from transform_states#1.W
-twice (30), and stack_transition copying layer 0's new state into the wide rows with a synchronous cudaMemcpy2D
-(1: the non-blocking stream)."""
+in about a minute there, 35 s of it in the two large searches, most of that the oracle's."""
 import pickle
 import sys
 
