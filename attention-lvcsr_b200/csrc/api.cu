@@ -380,7 +380,8 @@ int lvsr_model_create_bottom(const lvsr_config* cfg, const lvsr_bottom_config* b
   }
   LVSR_CHECK(cfg->num_layers >= 1 && cfg->num_layers <= LVSR_MAX_LAYERS, "num_layers %d out of range", cfg->num_layers);
   for (int l = 0; l < cfg->num_layers; ++l) {
-    LVSR_CHECK(bigru_supported(cfg->dims_bidir[l]), "encoder dim %d unsupported (128 or 256)", cfg->dims_bidir[l]);
+    LVSR_CHECK(bigru_supported(cfg->dims_bidir[l]), "encoder dim %d of layer %d unsupported (a multiple of 64 from 64 to 512)",
+               cfg->dims_bidir[l], l);
     LVSR_CHECK(cfg->subsample[l] >= 1, "subsample must be >= 1");
   }
   LVSR_CHECK(cfg->dim_dec % 8 == 0 && cfg->post_merge_dim % 8 == 0, "dim_dec and post_merge_dim must be multiples of 8");

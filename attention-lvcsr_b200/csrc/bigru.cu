@@ -88,6 +88,12 @@ __device__ __forceinline__ void st_async_v4(uint32_t remote_addr, float x, float
                : "memory");
 }
 
+// float4 groups of a lane's gate-weight k range (D / 64 of them) that the FFMA kernel keeps in registers: all of them at
+// D = 64, 128 and 256 (as the kernel always did), one at the other widths -- two already spill at
+// __launch_bounds__(256, 2), and the rolled loop over the shared-memory groups keeps their loads from being hoisted.
+template <int D>
+__host__ __device__ constexpr int ffma_qreg() { return D <= 128 || D == 256 ? D / 64 : 1; }
+
 // D: hidden units per direction; CS: CTAs per cluster.
 //
 // Work split inside a warp: lane = kg * CG + cg.
@@ -101,7 +107,11 @@ __device__ __forceinline__ void st_async_v4(uint32_t remote_addr, float x, float
 // 72 loads per warp and step; k over 32 lanes: 24 loads but 46 exchanges and ~1000 instructions
 // per warp and step (issue-bound); 16 lanes sits between.
 //
-// Shapes: <256, 8 CTAs, 8 warps> and <128, 4 CTAs, 8 warps> = 256 threads, two CTAs (two different clusters) per SM.
+// Shapes: <D, D / 32 CTAs, 8 warps> = 256 threads for every D = 64, 128, ..., 512 (32 units per CTA, so 2 to 16 CTAs per
+// cluster; above 8 the cluster size is non-portable), two CTAs (two different clusters) per SM where shared memory
+// allows it (up to D = 192; the shared-memory weights of wider layers leave room for one CTA per SM).  At D = 64, 128
+// and 256 a lane's gate slice (4 * D/16 floats) stays in registers; at the other widths the first float4 group of its
+// k range does and the rest sits in shared memory beside the state_to_state slice (see ffma_qreg).
 // TAPE: training forward (stores c / z / r over the pre-activations and every frame of h); compiled out for inference
 template <int D, int CS, int NWARP, bool TAPE>
 __global__ void __launch_bounds__(NWARP * 32, 2)
@@ -117,20 +127,28 @@ bigru_kernel(BiGruArgs a) {
   constexpr int CPL2 = NC2 / CG;      // candidate columns per lane
   static_assert(D % (CS * NWARP) == 0 && D % (4 * KL) == 0, "unsupported D / cluster size");
   static_assert(NC2 % CG == 0 && CPL2 == 2 && CPL1 == 4, "lane roles below assume 4 gate / 2 candidate columns per lane");
-  static_assert(KPG <= 32 && 32 % KPG == 0, "a lane's k range sits inside one 32-unit chunk");
+  static_assert(KPG <= 32, "a lane's k range sits inside one chunk of h");
+  static_assert(CS <= 16, "sender lanes reach at most 16 peers");
+  constexpr int QREG = ffma_qreg<D>();   // float4 groups of the gate slice held in registers, the rest in shared memory
   constexpr int N1 = RB * CPL1, N2 = RB * CPL2;        // per-lane partial sums of the two phases
   constexpr uint32_t FULL_BYTES = RB * D * sizeof(float);
 
   // h and h*r of all units, in chunks of 32 units: chunk c holds [RB][32] floats + 16 bytes of pad.
   // The 8 kg lanes of a warp read 8 different chunks (or half chunks) at the same offset; without
-  // the pad that is an 8-way bank conflict on every load.
-  constexpr int CH = 32, NCH = D / CH, SLOT = RB * CH + 4;
+  // the pad that is an 8-way bank conflict on every load.  Where a lane's k range does not divide 32 (D = 192, 320,
+  // 384, 448) a chunk is one lane's k range instead, so no float4 group straddles two chunks; the pad keeps the
+  // 4 kg lanes of a load phase on distinct banks there too.
+  constexpr int CH = 32 % KPG == 0 ? 32 : KPG, NCH = D / CH, SLOT = RB * CH + 4;
   __shared__ __align__(128) float hbuf[NCH][SLOT];
   __shared__ __align__(128) float hrbuf[NCH][SLOT];
   // state_to_state slice: [warp][q][lane][4 k] so a lane fetches four k of its column as one
   // vector; read in the candidate loop (the gate slice lives in registers for the whole sequence)
   extern __shared__ __align__(16) float w2s_dyn[];
   float (*w2s)[KQ][CPL2][32][4] = reinterpret_cast<float (*)[KQ][CPL2][32][4]>(w2s_dyn);
+  // gate slice beyond the register-resident groups: [warp][q - QREG][j][lane][4 k], one float4 per lane and column
+  // (the warp stride must be what ffma_smem_bytes allocates; QS = 1 only stands in for an empty slice)
+  constexpr int QS = KQ > QREG ? KQ - QREG : 1;
+  float (*w1s)[QS][CPL1][32][4] = reinterpret_cast<float (*)[QS][CPL1][32][4]>(w2s_dyn + (size_t)NWARP * KQ * CPL2 * 32 * 4);
   __shared__ __align__(8) unsigned long long mbar[2];   // [0]: h arrivals, [1]: h*r arrivals
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -142,7 +160,7 @@ bigru_kernel(BiGruArgs a) {
   const int row0 = (cluster_id >> 1) * RB;    // first batch row of this cluster
   const int ul_warp = warp * NC2;             // first owned unit of this warp, local index
   const int u_warp = rank * UC + ul_warp;     // ... global unit index
-  const int kpeer = (kg * KPG) / 32, koff = (kg * KPG) % 32;   // chunk and offset of this lane's k range
+  const int kpeer = (kg * KPG) / CH, koff = (kg * KPG) % CH;   // chunk and offset of this lane's k range
 
   const float* Wg = dir ? a.Wg_b : a.Wg_f;    // [D, 2D]  cols [update | reset]
   const float* Ws = dir ? a.Ws_b : a.Ws_f;    // [D, D]
@@ -152,15 +170,19 @@ bigru_kernel(BiGruArgs a) {
   // gate column cl of the warp (0..NC1): cl < NC2 -> update gate of unit u_warp + cl, else reset gate
   // pairs (k, k+1): the even-k and the odd-k partial sum of a column advance side by side (fma2) --
   // h arrives as (k, k+1) register pairs from the 16-byte loads anyway
-  float2 w1[CPL1][KPG / 2];
+  float2 w1[CPL1][QREG * 2];
 #pragma unroll
   for (int j = 0; j < CPL1; ++j) {
     const int cl = cg * CPL1 + j;
     const int col = (cl < NC2) ? (u_warp + cl) : (D + u_warp + (cl - NC2));
 #pragma unroll
-    for (int kk = 0; kk < KPG / 2; ++kk)
+    for (int kk = 0; kk < QREG * 2; ++kk)
       w1[j][kk] = make_float2(Wg[(long long)(kg * KPG + 2 * kk) * (2 * D) + col],
                               Wg[(long long)(kg * KPG + 2 * kk + 1) * (2 * D) + col]);
+#pragma unroll
+    for (int q = QREG; q < KQ; ++q)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) w1s[warp][q - QREG][j][lane][i] = Wg[(long long)(kg * KPG + q * 4 + i) * (2 * D) + col];
   }
 #pragma unroll
   for (int q = 0; q < KQ; ++q)
@@ -189,6 +211,7 @@ bigru_kernel(BiGruArgs a) {
   // sender role: lane = rowg * 8 + peer ships row rowg of this warp's 4 units to CTA `peer`
   const int rowg = lane >> 3, peer = lane & 7;
   const bool sender = peer < CS;
+  const bool sender2 = peer + 8 < CS;   // clusters above 8 CTAs: lanes also ship to peer + 8
   int src_hr[4], src_h[4];
 #pragma unroll
   for (int u = 0; u < 4; ++u) {
@@ -200,6 +223,14 @@ bigru_kernel(BiGruArgs a) {
   const uint32_t dst_h = map_to_rank(smem_u32(&hbuf[u_warp / CH][rowg * CH + u_warp % CH]), sender ? peer : 0);
   const uint32_t dst_hr = map_to_rank(smem_u32(&hrbuf[u_warp / CH][rowg * CH + u_warp % CH]), sender ? peer : 0);
   const uint32_t rbar_h = map_to_rank(bar_h, sender ? peer : 0), rbar_hr = map_to_rank(bar_hr, sender ? peer : 0);
+  uint32_t dst_h2 = 0, dst_hr2 = 0, rbar_h2 = 0, rbar_hr2 = 0;
+  if constexpr (CS > 8) {
+    const int p2 = sender2 ? peer + 8 : 0;
+    dst_h2 = map_to_rank(smem_u32(&hbuf[u_warp / CH][rowg * CH + u_warp % CH]), p2);
+    dst_hr2 = map_to_rank(smem_u32(&hrbuf[u_warp / CH][rowg * CH + u_warp % CH]), p2);
+    rbar_h2 = map_to_rank(bar_h, p2);
+    rbar_hr2 = map_to_rank(bar_hr, p2);
+  }
   if (tid == 0) {
     mbar_init(bar_h, 1);
     mbar_init(bar_hr, 1);
@@ -279,7 +310,7 @@ bigru_kernel(BiGruArgs a) {
 #pragma unroll
       for (int i = 0; i < N1; ++i) ap[i] = make_float2(0.f, 0.f);
 #pragma unroll
-      for (int q = 0; q < KQ; ++q) {
+      for (int q = 0; q < QREG; ++q) {
 #pragma unroll
         for (int r = 0; r < RB; ++r) {
           const float4 v = *reinterpret_cast<const float4*>(&hbuf[kpeer][r * CH + koff + q * 4]);
@@ -288,6 +319,23 @@ bigru_kernel(BiGruArgs a) {
             float2 sacc = ap[r * CPL1 + j];
             sacc = fma2(make_float2(v.x, v.y), w1[j][q * 2 + 0], sacc);
             sacc = fma2(make_float2(v.z, v.w), w1[j][q * 2 + 1], sacc);
+            ap[r * CPL1 + j] = sacc;
+          }
+        }
+      }
+#pragma unroll 1
+      for (int q = QREG; q < KQ; ++q) {   // rolled: unrolled, the loads of later groups are hoisted and spill
+        float4 w[CPL1];
+#pragma unroll
+        for (int j = 0; j < CPL1; ++j) w[j] = *reinterpret_cast<const float4*>(&w1s[warp][q - QREG][j][lane][0]);
+#pragma unroll
+        for (int r = 0; r < RB; ++r) {
+          const float4 v = *reinterpret_cast<const float4*>(&hbuf[kpeer][r * CH + koff + q * 4]);
+#pragma unroll
+          for (int j = 0; j < CPL1; ++j) {
+            float2 sacc = ap[r * CPL1 + j];
+            sacc = fma2(make_float2(v.x, v.y), make_float2(w[j].x, w[j].y), sacc);
+            sacc = fma2(make_float2(v.z, v.w), make_float2(w[j].z, w[j].w), sacc);
             ap[r * CPL1 + j] = sacc;
           }
         }
@@ -307,6 +355,8 @@ bigru_kernel(BiGruArgs a) {
       const float x = __shfl_sync(0xffffffffu, hr_mine, src_hr[0]), y = __shfl_sync(0xffffffffu, hr_mine, src_hr[1]);
       const float z = __shfl_sync(0xffffffffu, hr_mine, src_hr[2]), w = __shfl_sync(0xffffffffu, hr_mine, src_hr[3]);
       if (sender) st_async_v4(dst_hr, x, y, z, w, rbar_hr);
+      if constexpr (CS > 8)
+        if (sender2) st_async_v4(dst_hr2, x, y, z, w, rbar_hr2);
     }
 
     BG_STAMP(2);
@@ -353,6 +403,8 @@ bigru_kernel(BiGruArgs a) {
       const float x = __shfl_sync(0xffffffffu, hn, src_h[0]), y = __shfl_sync(0xffffffffu, hn, src_h[1]);
       const float z = __shfl_sync(0xffffffffu, hn, src_h[2]), w = __shfl_sync(0xffffffffu, hn, src_h[3]);
       if (sender) st_async_v4(dst_h, x, y, z, w, rbar_h);
+      if constexpr (CS > 8)
+        if (sender2) st_async_v4(dst_h2, x, y, z, w, rbar_h2);
       if (sub_phase == 0 && peer == 0 && row0 + rowg < B)
         *reinterpret_cast<float4*>(a.out + ((long long)t_out * B + row0 + rowg) * (2 * D) + dir * D + u_warp) =
             make_float4(x, y, z, w);
@@ -379,18 +431,37 @@ bigru_kernel(BiGruArgs a) {
   cluster_sync_all();
 }
 
-// dynamic shared memory of bigru_kernel<D, CS, NWARP, *>
+// dynamic shared memory of bigru_kernel<D, CS, NWARP, *>: the state_to_state slice, then the gate slice's groups beyond
+// ffma_qreg
 template <int D, int NWARP>
-constexpr size_t ffma_smem_bytes() { return (size_t)NWARP * (D / 16 / 4) * 2 * 32 * 4 * sizeof(float); }
+constexpr size_t ffma_smem_bytes() {
+  return (size_t)NWARP * (D / 16 / 4) * 2 * 32 * 4 * sizeof(float) +
+         (size_t)NWARP * (D / 64 - ffma_qreg<D>()) * 4 * 32 * 4 * sizeof(float);
+}
 
-// how many clusters of the FFMA kernel the device holds at once (encoder plan report only: the FFMA kernel is never
-// chosen by it)
+// once per device: the dynamic shared memory, and clusters above 8 CTAs (D > 256) are non-portable
+template <int D, int CS, int NWARP, bool TAPE>
+int ffma_configure() {
+  static bool configured[LVSR_MAX_DEVICES] = {false};
+  const int dev = current_device();
+  if (!configured[dev]) {
+    LVSR_CUDA_OK(cudaFuncSetAttribute(bigru_kernel<D, CS, NWARP, TAPE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)ffma_smem_bytes<D, NWARP>()));
+    if (CS > 8)
+      LVSR_CUDA_OK(cudaFuncSetAttribute(bigru_kernel<D, CS, NWARP, TAPE>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    configured[dev] = true;
+  }
+  return 0;
+}
+
+// how many clusters of the FFMA kernel the device holds at once (0: none, the launch is refused)
 template <int D, int CS, int NWARP, bool TAPE>
 int ffma_clusters_resident() {
   static int per_dev[LVSR_MAX_DEVICES];
   static bool known[LVSR_MAX_DEVICES] = {false};
   const int dev = current_device();
   if (!known[dev]) {
+    if (ffma_configure<D, CS, NWARP, TAPE>()) return 0;
     known[dev] = true;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(CS * 64);
@@ -416,13 +487,11 @@ int ffma_clusters_resident() {
 template <int D, int CS, int NWARP, bool TAPE>
 int launch_bigru_t(const BiGruArgs& a, cudaStream_t stream, BiGruPlan* plan) {
   constexpr size_t W2S_BYTES = ffma_smem_bytes<D, NWARP>();
-  static bool configured[LVSR_MAX_DEVICES] = {false};
-  const int dev = current_device();
-  if (!configured[dev]) {
-    LVSR_CUDA_OK(cudaFuncSetAttribute(bigru_kernel<D, CS, NWARP, TAPE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)W2S_BYTES));
-    configured[dev] = true;
-  }
+  if (int rc = ffma_configure<D, CS, NWARP, TAPE>()) return rc;
+  const int resident = ffma_clusters_resident<D, CS, NWARP, TAPE>();
+  if (resident <= 0)
+    return set_error("bigru: this device holds no cluster of %d CTAs of the hidden-size-%d scan (%zu bytes of shared memory "
+                     "each)", CS, D, W2S_BYTES);
   const int groups = ceil_div(a.B, RB);
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(CS * groups * 2);
@@ -443,10 +512,7 @@ int launch_bigru_t(const BiGruArgs& a, cudaStream_t stream, BiGruPlan* plan) {
   }
   LVSR_CUDA_OK(cudaLaunchKernelEx(&cfg, bigru_kernel<D, CS, NWARP, TAPE>, a));
   g_launch_count++;
-  if (plan) {
-    const int resident = ffma_clusters_resident<D, CS, NWARP, TAPE>();
-    *plan = {LVSR_ENC_BIGRU_FFMA, RB, CS, 2 * groups, resident, resident > 0 ? ceil_div(2 * groups, resident) : 0};
-  }
+  if (plan) *plan = {LVSR_ENC_BIGRU_FFMA, RB, CS, 2 * groups, resident, ceil_div(2 * groups, resident)};
   if (trace) {
     unsigned long long h[8] = {0};
     LVSR_CUDA_OK(cudaMemcpyFromSymbolAsync(h, g_bigru_trace, sizeof(h), 0, cudaMemcpyDeviceToHost, stream));
@@ -1089,7 +1155,7 @@ int launch_bigru_mma(const BiGruArgs& a, cudaStream_t stream, BiGruPlan* plan) {
 
 }  // namespace
 
-bool bigru_supported(int D) { return D == 128 || D == 256; }
+bool bigru_supported(int D) { return D >= 64 && D <= 512 && D % 64 == 0; }
 
 int bigru_plan(const BiGruArgs& a, BiGruPlan* plan) {
   *plan = {};
@@ -1114,9 +1180,9 @@ int bigru_plan(const BiGruArgs& a, BiGruPlan* plan) {
                     : BiGruPlan{LVSR_ENC_BIGRU_MMA, 4, MMA_CS, clusters, mma_clusters_resident<256, 4>(), mma_waves<256, 4>(a.B)};
     return 0;
   }
-  LVSR_CHECK(a.D == 128 || a.D == 256, "bigru: unsupported hidden size %d (supported: 128, 256)", a.D);
+  LVSR_CHECK(bigru_supported(a.D), "bigru: unsupported hidden size %d (supported: multiples of 64 from 64 to 512)", a.D);
   // the FFMA kernel's occupancy (resident, waves) is queried when it is launched
-  *plan = {LVSR_ENC_BIGRU_FFMA, RB, a.D == 256 ? 8 : 4, 2 * ceil_div(a.B, RB), 0, 0};
+  *plan = {LVSR_ENC_BIGRU_FFMA, RB, a.D / 32, 2 * ceil_div(a.B, RB), 0, 0};
   return 0;
 }
 
@@ -1129,8 +1195,14 @@ int bigru_layer(const BiGruArgs& a, cudaStream_t stream, BiGruPlan* plan) {
   if (pl.kernel == LVSR_ENC_BIGRU_MMA)
     return pl.rb == 8 ? launch_bigru_mma<256, 8>(a, stream, plan) : launch_bigru_mma<256, 4>(a, stream, plan);
   switch (a.D) {
+    case 64: return launch_bigru<64, 2, 8>(a, stream, plan);
     case 128: return launch_bigru<128, 4, 8>(a, stream, plan);
-    default: return launch_bigru<256, 8, 8>(a, stream, plan);
+    case 192: return launch_bigru<192, 6, 8>(a, stream, plan);
+    case 256: return launch_bigru<256, 8, 8>(a, stream, plan);
+    case 320: return launch_bigru<320, 10, 8>(a, stream, plan);
+    case 384: return launch_bigru<384, 12, 8>(a, stream, plan);
+    case 448: return launch_bigru<448, 14, 8>(a, stream, plan);
+    default: return launch_bigru<512, 16, 8>(a, stream, plan);
   }
 }
 

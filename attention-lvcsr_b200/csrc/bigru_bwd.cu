@@ -20,6 +20,8 @@
 // mbarrier -- the all-gather machinery of the forward kernel.  W_s^T slice in registers, W_g^T
 // slice in shared memory (k-major, padded so the 8 k-groups of a warp hit distinct banks);
 // thread = (k-group 0..7, unit), 4 rows per thread, cross-k reduction by shuffles.
+// Every D = 64, 128, ..., 512 runs, with CS = D / 32 (clusters above 8 CTAs are non-portable); from D = 384 on the
+// shared memory leaves room for one CTA per SM.
 #include "kernels.h"
 
 namespace lvsr {
@@ -69,8 +71,15 @@ __device__ __forceinline__ void st_async_v4(uint32_t remote_addr, float4 v, uint
                : "memory");
 }
 
+__host__ __device__ constexpr size_t bwd_smem_bytes(int D) {
+  return ((size_t)2 * D * WSTR) * sizeof(float) + ((size_t)3 * D + 2 * UC) * sizeof(float4);
+}
+// CTAs per SM the shared memory allows (228 KB per SM, 1 KB of it reserved per CTA); the register budget follows it, so
+// the wide layers, which hold one CTA per SM anyway, get the registers that keep them from spilling
+__host__ __device__ constexpr int bwd_min_blocks(int D) { return 2 * (bwd_smem_bytes(D) + 1024) <= 228 * 1024 ? 2 : 1; }
+
 template <int D, int CS>
-__global__ void __launch_bounds__(NT, 2) bigru_bwd_kernel(BiGruBwdArgs a) {
+__global__ void __launch_bounds__(NT, bwd_min_blocks(D)) bigru_bwd_kernel(BiGruBwdArgs a) {
   static_assert(D == CS * UC, "32 units per CTA");
   constexpr int KA = D / 8;         // k values per thread, first product  (K = D)
   constexpr int KB = 2 * D / 8;     // second product (K = 2D)
@@ -137,9 +146,13 @@ __global__ void __launch_bounds__(NT, 2) bigru_bwd_kernel(BiGruBwdArgs a) {
   };
   if (warp == 0) prefetch(t);
 
-  uint32_t dstA[CS], dstB0[CS], dstB1[CS], rbarA[CS], rbarB[CS];
+  // remote addresses: held in registers at CS = 2, 4 and 8 (as the kernel always did); at the other sizes 5 * CS of them
+  // would spill, and `mapa` in the loop is cheap
+  constexpr bool REMOTE_REGS = CS <= 4 || CS == 8;
+  constexpr int NR = REMOTE_REGS ? CS : 1;
+  uint32_t dstA[NR], dstB0[NR], dstB1[NR], rbarA[NR], rbarB[NR];
 #pragma unroll
-  for (int p = 0; p < CS; ++p) {
+  for (int p = 0; p < NR; ++p) {
     dstA[p] = map_to_rank(smem_u32(&bufA[ju]), p);
     dstB0[p] = map_to_rank(smem_u32(&bufB[ju]), p);
     dstB1[p] = map_to_rank(smem_u32(&bufB[D + ju]), p);
@@ -166,8 +179,13 @@ __global__ void __launch_bounds__(NT, 2) bigru_bwd_kernel(BiGruBwdArgs a) {
         daz[q] = dz * z[q] * (1.f - z[q]);
       }
       const float4 v = make_float4(dac[0], dac[1], dac[2], dac[3]);
+      if constexpr (REMOTE_REGS) {
 #pragma unroll
-      for (int p = 0; p < CS; ++p) st_async_v4(dstA[p], v, rbarA[p]);
+        for (int p = 0; p < CS; ++p) st_async_v4(dstA[p], v, rbarA[p]);
+      } else {
+#pragma unroll
+        for (int p = 0; p < CS; ++p) st_async_v4(map_to_rank(smem_u32(&bufA[ju]), p), v, map_to_rank(barA, p));
+      }
       // dA of this step: in place over the saved candidate
 #pragma unroll
       for (int q = 0; q < RB; ++q)
@@ -204,10 +222,19 @@ __global__ void __launch_bounds__(NT, 2) bigru_bwd_kernel(BiGruBwdArgs a) {
         hr[q] = h[q] * r[q];
       }
       const float4 vz = make_float4(daz[0], daz[1], daz[2], daz[3]), vr = make_float4(dar[0], dar[1], dar[2], dar[3]);
+      if constexpr (REMOTE_REGS) {
 #pragma unroll
-      for (int p = 0; p < CS; ++p) {
-        st_async_v4(dstB0[p], vz, rbarB[p]);
-        st_async_v4(dstB1[p], vr, rbarB[p]);
+        for (int p = 0; p < CS; ++p) {
+          st_async_v4(dstB0[p], vz, rbarB[p]);
+          st_async_v4(dstB1[p], vr, rbarB[p]);
+        }
+      } else {
+#pragma unroll
+        for (int p = 0; p < CS; ++p) {
+          const uint32_t rbar = map_to_rank(barB, p);
+          st_async_v4(map_to_rank(smem_u32(&bufB[ju]), p), vz, rbar);
+          st_async_v4(map_to_rank(smem_u32(&bufB[D + ju]), p), vr, rbar);
+        }
       }
 #pragma unroll
       for (int q = 0; q < RB; ++q) {
@@ -254,15 +281,18 @@ __global__ void __launch_bounds__(NT, 2) bigru_bwd_kernel(BiGruBwdArgs a) {
 
 template <int D, int CS>
 int launch_bwd(const BiGruBwdArgs& a, cudaStream_t stream) {
-  constexpr size_t SMEM = ((size_t)2 * D * WSTR) * sizeof(float) + ((size_t)3 * D + 2 * UC) * sizeof(float4);
+  constexpr size_t SMEM = bwd_smem_bytes(D);
   static bool configured[LVSR_MAX_DEVICES] = {false};
+  static int resident[LVSR_MAX_DEVICES];
   const int dev = current_device();
-  if (!configured[dev]) {
-    LVSR_CUDA_OK(cudaFuncSetAttribute(bigru_bwd_kernel<D, CS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM));
-    configured[dev] = true;
-  }
   const int groups = ceil_div(a.B, RB);
   cudaLaunchConfig_t cfg = {};
+  if (!configured[dev]) {
+    LVSR_CUDA_OK(cudaFuncSetAttribute(bigru_bwd_kernel<D, CS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM));
+    if (CS > 8) LVSR_CUDA_OK(cudaFuncSetAttribute(bigru_bwd_kernel<D, CS>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    configured[dev] = true;
+    resident[dev] = -1;
+  }
   cfg.gridDim = dim3(CS * groups * 2);
   cfg.blockDim = dim3(NT);
   cfg.dynamicSmemBytes = SMEM;
@@ -274,6 +304,17 @@ int launch_bwd(const BiGruBwdArgs& a, cudaStream_t stream) {
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
+  if (resident[dev] < 0) {
+    int k = 0;
+    if (cudaOccupancyMaxActiveClusters(&k, bigru_bwd_kernel<D, CS>, &cfg) != cudaSuccess) {
+      cudaGetLastError();
+      k = 0;
+    }
+    resident[dev] = k;
+  }
+  if (resident[dev] <= 0)
+    return set_error("bigru backward: this device holds no cluster of %d CTAs of the hidden-size-%d scan (%zu bytes of "
+                     "shared memory each)", CS, D, SMEM);
   LVSR_CUDA_OK(cudaLaunchKernelEx(&cfg, bigru_bwd_kernel<D, CS>, a));
   g_launch_count++;
   return 0;
@@ -285,12 +326,21 @@ int bigru_layer_backward(const BiGruBwdArgs& a, cudaStream_t stream, int* cs_out
   ProfScope prof("bigru_bwd", stream);
   if (cs_out) *cs_out = 0;
   if (a.T <= 0 || a.B <= 0) return 0;
-  if (cs_out && bigru_supported(a.D)) *cs_out = a.D / UC;
+  int rc;
   switch (a.D) {
-    case 128: return launch_bwd<128, 4>(a, stream);
-    case 256: return launch_bwd<256, 8>(a, stream);
-    default: return set_error("bigru backward: unsupported hidden size %d (supported: 128, 256)", a.D);
+    case 64: rc = launch_bwd<64, 2>(a, stream); break;
+    case 128: rc = launch_bwd<128, 4>(a, stream); break;
+    case 192: rc = launch_bwd<192, 6>(a, stream); break;
+    case 256: rc = launch_bwd<256, 8>(a, stream); break;
+    case 320: rc = launch_bwd<320, 10>(a, stream); break;
+    case 384: rc = launch_bwd<384, 12>(a, stream); break;
+    case 448: rc = launch_bwd<448, 14>(a, stream); break;
+    case 512: rc = launch_bwd<512, 16>(a, stream); break;
+    default:
+      return set_error("bigru backward: unsupported hidden size %d (supported: multiples of 64 from 64 to 512)", a.D);
   }
+  if (rc == 0 && cs_out) *cs_out = a.D / UC;   // the cluster size that ran
+  return rc;
 }
 
 }  // namespace lvsr
