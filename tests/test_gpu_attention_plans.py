@@ -20,8 +20,9 @@ an H100 80GB HBM3 (700 W power limit); none is looser than 1e-4, the project's g
 averages carry absolute errors of about 1e-6 of their scale, so their per-element floor is 0.1 of the scale.  The
 file runs in about 20 s on that GPU.
 
-Content-and-conv attention only exists with an encoded dimension of 256 or 512 (BiGRU(128) or BiGRU(256)), so the
-gate product's K = E + C = 512 is reached as E = 256, C = 256 only; E = 384 cannot be built.
+The cases here use E = 256 (BiGRU(128)), where the gate product's K = E + C = 512 is reached as C = 256.  The encoder
+gives every E that is a multiple of 128 from 128 to 1024; the other encoded widths, among them E + C = 512 as 384 + 128
+and 256 as 128 + 128, are covered by test_gpu_encoded_widths.py.
 """
 import math
 

@@ -63,12 +63,13 @@ def _smem_bytes(Tp, cs, loc=True, M=512, E=512, K=10, n=100):
     return 4 * f
 
 
-def _longest_row(cs, loc=True):
-    """The largest T' a cluster of cs CTAs holds: the largest multiple of cs whose chunk fits."""
+def _longest_row(cs, loc=True, **widths):
+    """The largest T' a cluster of cs CTAs holds: the largest multiple of cs whose chunk fits.  `widths`: M, E, K, n
+    of _smem_bytes (bench.NET's by default)."""
     lo, hi = 1, 1 << 20
     while lo < hi:
         mid = (lo + hi + 1) // 2
-        lo, hi = (mid, hi) if _smem_bytes(mid * cs, cs, loc) <= SMEM_MAX else (lo, mid - 1)
+        lo, hi = (mid, hi) if _smem_bytes(mid * cs, cs, loc, **widths) <= SMEM_MAX else (lo, mid - 1)
     return lo * cs
 
 
@@ -77,11 +78,11 @@ def _sms():
     return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
 
 
-def _expected_cs(R, Tp, loc=True):
+def _expected_cs(R, Tp, loc=True, **widths):
     cs = 1
     while cs < 8 and R * cs * 2 <= _sms() and -(-Tp // (cs * 2)) >= 16:
         cs *= 2
-    while cs < 8 and _smem_bytes(Tp, cs, loc) > SMEM_MAX and -(-Tp // (cs * 2)) >= 16:
+    while cs < 8 and _smem_bytes(Tp, cs, loc, **widths) > SMEM_MAX and -(-Tp // (cs * 2)) >= 16:
         cs *= 2
     return cs
 
