@@ -652,14 +652,25 @@ def _take_states(st, idx):
 def beam_search(cfg, params, recordings, beam_size, eol_symbol=None, max_length=None,
                 ignore_first_eol=False, char_discount=0, round_to_inf=1e9,
                 stop_on="patience", validate_solution_function=None,
-                computers=None, as_arrays=False):
+                computers=None, as_arrays=False, stats=None):
     """BeamSearch.search for ONE utterance, B/search.py:244-407, driven the way
     SpeechRecognizer.beam_search does (lvsr/bricks/recognizer.py:513-533):
     recordings [T,F] -> batch axis inserted, max_length = int(T / scale).
 
     ``computers`` lets a test substitute the four device functions (same
     signatures as the oracle's) while keeping this host logic as the checker.
+    ``stats`` (a dict) receives what the settings decided: "steps" run, "stop"
+    ("patience" / "optimistic" when a criterion ended the loop, else None),
+    "finished" (hypotheses added to done), "eol_removed" (eol hypotheses whose
+    step cost reached round_to_inf), "eol_kept_first" (eol hypotheses kept in
+    the beam at step 0 by ignore_first_eol) and "rejected" (by the validator).
+
+    The ranking key is float64 whatever the cost dtype, as under numpy 1.x
+    where the reference ran (a float32 scalar minus a Python float was
+    float64 there; NEP 50 makes it float32).
     """
+    if stats is not None:
+        stats.update(steps=0, stop=None, finished=0, eol_removed=0, eol_kept_first=0, rejected=0)
     c = computers or {}
     f_ctx = c.get("context", lambda x: context_computer(cfg, params, x))
     f_init = c.get("initial", lambda att: initial_states(cfg, params, 1, att))
@@ -681,7 +692,7 @@ def beam_search(cfg, params, recordings, beam_size, eol_symbol=None, max_length=
     patience = None
 
     def rank(item):
-        return item[1][-1] - char_discount * len(item[1])
+        return float(item[1][-1]) - char_discount * len(item[1])
 
     for i in range(max_length):
         width = st["states"].shape[0]
@@ -697,12 +708,15 @@ def beam_search(cfg, params, recordings, beam_size, eol_symbol=None, max_length=
                 else:
                     patience -= 1
                     if patience == 0:
+                        if stats is not None:
+                            stats["stop"] = "patience"
                         break
         elif stop_on == "optimistic_future_cost":
             if len(done) >= beam_size:
-                optimistic = all_costs[-1, :].min() - char_discount * max_length
-                last = done[beam_size - 1][1]
-                if last[-1] - char_discount * len(last) < optimistic:
+                optimistic = float(all_costs[-1, :].min()) - char_discount * max_length
+                if rank(done[beam_size - 1]) < optimistic:
+                    if stats is not None:
+                        stats["stop"] = "optimistic"
                     break
         else:
             raise ValueError("Unknown stopping criterion {}".format(stop_on))
@@ -736,6 +750,16 @@ def beam_search(cfg, params, recordings, beam_size, eol_symbol=None, max_length=
             if (validate_solution_function is None or
                     validate_solution_function(recordings, all_outputs[:, idx])):
                 done.append((all_outputs[:, idx], all_costs[:, idx]))
+                if stats is not None:
+                    stats["finished"] += 1
+            elif stats is not None:
+                stats["rejected"] += 1
+        if stats is not None:
+            n_eol = int(np.count_nonzero(all_outputs[-1] == eol_symbol))
+            stats["steps"] = i + 1
+            stats["eol_removed"] += n_eol - len(finished)
+            if ignore_first_eol and i == 0:
+                stats["eol_kept_first"] += n_eol
         unfinished = np.where(mask == 1)[0]
         st = _take_states(st, unfinished)
         all_outputs = np.take(all_outputs, unfinished, axis=1)

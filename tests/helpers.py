@@ -16,8 +16,9 @@ def package():
     return graft.load_package()
 
 
-def make_recognizer(cfg, params=None):
-    """A SpeechRecognizer of the oracle config `cfg` (stack_oracle's configs carry dec_stack 2)."""
+def make_recognizer(cfg, params=None, **extra):
+    """A SpeechRecognizer of the oracle config `cfg` (stack_oracle's configs carry dec_stack 2); `extra` goes to the
+    constructor (e.g. lm and character_map)."""
     pkg = package()
     act = {"maxout": pkg.Maxout(cfg["maxout_pieces"]), "relu": pkg.Rectifier(), "tanh": pkg.Tanh(),
            "identity": pkg.Identity()}[cfg["post_merge_activation"]]
@@ -31,7 +32,7 @@ def make_recognizer(cfg, params=None):
         use_states_for_readout=cfg["use_states_for_readout"],
         max_decoded_length_scale=cfg["max_decoded_length_scale"],
         attention_type=cfg.get("attention_type", "content_and_conv"), dec_stack=cfg.get("dec_stack", 1),
-        enc_transition=pkg.GatedRecurrent, dec_transition=pkg.GatedRecurrent, data_prepend_eos=False)
+        enc_transition=pkg.GatedRecurrent, dec_transition=pkg.GatedRecurrent, data_prepend_eos=False, **extra)
     if params is not None:
         rec.set_parameter_values(params)
     return rec
