@@ -88,6 +88,11 @@ class LvsrAdaptiveClipping(C.Structure):
     _fields_ = [("initial_threshold", C.c_double), ("decay_rate", C.c_double), ("burnin_period", C.c_int32)]
 
 
+class LvsrRegularization(C.Structure):
+    """Mirror of ``lvsr_regularization`` (include/lvsr_b200.h)."""
+    _fields_ = [("dropout", C.c_int32), ("noise_level", C.c_double), ("penalty_coof", C.c_double), ("seed", C.c_uint64)]
+
+
 # slots of lvsr_train_noise_stats (LVSR_NOISE_*), under the reference's monitor names (lvsr/main.py:440-460)
 NOISE_STATS = ("model_cost", "model_prior_mean", "model_prior_variance")
 
@@ -159,6 +164,11 @@ SIGNATURES = {
     "lvsr_train_noise_sample": (C.c_int, [_P, C.c_int64, _P, _P]),
     "lvsr_train_noise_params": (C.c_int, [_P, _P, _P]),
     "lvsr_train_noise_gradients": (C.c_int, [_P, _P, C.c_float, _P, _P]),
+    "lvsr_train_set_regularization": (C.c_int, [_P, C.POINTER(LvsrRegularization)]),
+    "lvsr_train_set_utterance_offset": (C.c_int, [_P, C.c_int64]),
+    "lvsr_train_dropout_mask": (C.c_int, [_P, C.c_int64, C.c_int64, _I, _I, _I, _P, _P]),
+    "lvsr_train_weight_noise_sample": (C.c_int, [_P, C.c_int64, _P, _P]),
+    "lvsr_train_penalty_sum": (C.c_int, [_P, _P, _P]),
     "lvsr_launch_count": (C.c_int64, [C.c_int]),
     "lvsr_profile_enable": (C.c_int, [C.c_int]),
     "lvsr_profile_read": (C.c_int, [C.c_char_p, C.POINTER(C.c_double), C.POINTER(C.c_int64)]),

@@ -29,6 +29,9 @@ logger = logging.getLogger(__name__)
 # "/adaptive_noise.recognizer/encoder/bidir0/forward/fork/fork_inputs.W".
 NOISE_BRICK = "adaptive_noise"
 ADAPTIVE_NOISE_DEFAULTS = dict(init_sigma=1e-6, model_cost_coefficient=1.0, seed=None)   # graph.py:71-80
+# regularization.dropout / noise / penalty_coof (lvsr/main.py:400-417); seed None or 0 is Blocks' default_seed, 1
+REGULARIZATION_DEFAULTS = dict(dropout=False, noise=0.0, penalty_coof=0.0, seed=None)
+ADAPTIVE_NOISE_ERROR = "using  adaptive noise with alignment weight panalty or weight decay is probably stupid"
 
 
 def noise_parameter_name(name):
@@ -226,6 +229,32 @@ def allreduce_step_buffer(buf, n, local_batch, local_cost, dist):
     return buf[n], buf[n + 1]
 
 
+def _regularization(reg):
+    """The checked `regularization` argument of GradientDescent -> dict(dropout, noise, penalty_coof, seed), or None
+    when none of the three is on.  Like lvsr/main.py:402-408, which builds the noisy graph from the clean one, weight
+    noise discards dropout: dropout is then logged and dropped."""
+    unknown = set(reg) - set(REGULARIZATION_DEFAULTS)
+    if unknown:
+        raise TypeError("regularization: unknown arguments %s" % sorted(unknown))
+    r = dict(REGULARIZATION_DEFAULTS, **reg)
+    if not isinstance(r["dropout"], bool):
+        raise TypeError("regularization: dropout must be a bool, got %r" % (r["dropout"],))
+    noise = float(r["noise"])
+    if not (np.isfinite(noise) and noise >= 0.0):
+        raise ValueError("regularization: noise must be a standard deviation >= 0, got %r" % (r["noise"],))
+    coof = float(r["penalty_coof"])
+    if not (np.isfinite(coof) and coof >= 0.0):
+        raise ValueError("regularization: penalty_coof must be >= 0, got %r" % (r["penalty_coof"],))
+    dropout = r["dropout"]
+    if dropout and noise > 0:
+        logger.warning("regularization: dropout has no effect with noise (the reference applies the noise to the graph "
+                       "without dropout, lvsr/main.py:402-408): dropped")
+        dropout = False
+    if not (dropout or noise > 0 or coof > 0):
+        return None
+    return dict(dropout=dropout, noise=noise, penalty_coof=coof, seed=int(r["seed"] or 1))
+
+
 def check_trainable_net(net):
     """Refuse a config['net'] the training step cannot run: a stacked decoder (dec_stack > 1) decodes and scores,
     but has no backward pass through the RecurrentStack."""
@@ -252,10 +281,24 @@ class GradientDescent(object):
     log-variances are trained with the parameters (lvsr/graph.py:71-251; include/lvsr_b200.h).  Decay has no effect
     on the step under adaptive noise: like the reference, an error is logged and decay is dropped.  ``last_cost``
     stays the task cost; ``last_model_cost``, ``model_prior_mean`` and ``model_prior_variance`` report the rest.
-    Inference (cost, search, sampling) always uses the means."""
+    Inference (cost, search, sampling) always uses the means.
+
+    regularization: config['regularization']'s dropout, noise and penalty_coof, plus a seed:
+    dict(dropout=False, noise=0.0, penalty_coof=0.0, seed=None) (lvsr/main.py:400-417).  ``dropout`` (a bool, the
+    schema's type) multiplies the encoder's input, the recordings or the bottom MLP's output, by Bernoulli(0.5) / 0.5
+    in every training step; ``noise`` > 0 adds N(0, noise^2) to every parameter outside the attention for forward and
+    backward, and the gradient there updates the clean parameters.  Fresh draws every update, keyed by (seed, update,
+    global utterance index) and (seed, update, parameter element); include/lvsr_b200.h.  With noise on, dropout is
+    dropped with a warning, as the reference builds its noisy graph from the graph without dropout.  ``penalty_coof``
+    > 0 adds penalty_coof * weights_penalty / B to the cost the gradient is taken of, weights_penalty being the
+    alignment monotonicity penalty of the regularised forward (lvsr/expressions.py:14-19, lvsr/main.py:411-417).
+    Under adaptive noise the reference trains on the clean graph, so all three are dropped with a logged error.
+    Data-parallel dropout needs equal shards: rank r's first utterance is utterance r * B of the global batch.
+    ``last_cost`` stays the task cost of the regularised forward; ``last_penalty`` is weights_penalty / B of the
+    last update (a device scalar; None when the penalty is off), all-reduced with the gradient."""
 
     def __init__(self, recognizer=None, step_rule=None, decay=0.0, cost=None, parameters=None, gradients=None,
-                 on_unused_sources="warn", adaptive_noise=None, **kwargs):
+                 on_unused_sources="warn", adaptive_noise=None, regularization=None, **kwargs):
         if recognizer is None:
             raise ValueError("GradientDescent needs the recognizer (no symbolic cost exists in the CUDA path)")
         if getattr(recognizer, "lm", None):
@@ -276,10 +319,17 @@ class GradientDescent(object):
             self.adaptive_noise = dict(num_examples=int(an["num_examples"]), init_sigma=float(an["init_sigma"]),
                                        model_cost_coefficient=float(an["model_cost_coefficient"]),
                                        seed=int(an["seed"] or 1))
-            if decay > 0:
-                # lvsr/main.py:427-430; the gradients are those of the cost without the decay term (:431-437)
-                logger.error("using  adaptive noise with alignment weight panalty or weight decay is probably stupid")
-                decay = 0.0
+        self.regularization = _regularization(regularization or {})
+        if self.adaptive_noise:
+            # lvsr/main.py:425-437: the cost and its gradients are rebuilt from the clean graph, so decay and the three
+            # regularisers have no effect; the reference logs the error below for the penalty and decay
+            coof = float((regularization or {}).get("penalty_coof", 0.0))
+            if decay > 0 or coof > 0:
+                logger.error(ADAPTIVE_NOISE_ERROR)
+            if self.regularization:
+                logger.error("regularization %s has no effect under adaptive noise: dropped", self.regularization)
+            decay = 0.0
+            self.regularization = None
         self._tc = _to_train_config(self.step_rule, decay)
         self.on_unused_sources = on_unused_sources
         self._grads = None
@@ -287,6 +337,7 @@ class GradientDescent(object):
         self._cost = None
         self.equal_shards = True
         self.last_cost = None
+        self.last_penalty = None
         self.last_batch_size = None
 
     SOURCES = ("recordings", "recordings_mask", "labels", "labels_mask")
@@ -296,7 +347,7 @@ class GradientDescent(object):
         torch = rec._torch()
         lib, h = _lib.load(), rec._require_ready()
         n = int(lib.lvsr_model_flat_size(h))
-        # [flat gradient | local batch size | local cost sum | padding]: one buffer, one all-reduce
+        # [flat gradient | local batch size | local cost sum | penalty sum | padding]: one buffer, one all-reduce
         self._buf = torch.zeros((n + 64,), dtype=torch.float32, device=rec.device)
         self._cost = torch.zeros((1,), dtype=torch.float32, device=rec.device)
         self._n = n
@@ -316,6 +367,13 @@ class GradientDescent(object):
                                          num_examples=an["num_examples"], seed=an["seed"])
             _lib.check(lib.lvsr_train_set_adaptive_noise(h, C.byref(cfg)))
             self._noise_grads = torch.zeros((n,), dtype=torch.float32, device=rec.device)
+        if self.regularization:
+            r = self.regularization
+            cfg = _lib.LvsrRegularization(dropout=int(r["dropout"]), noise_level=r["noise"],
+                                          penalty_coof=r["penalty_coof"], seed=r["seed"])
+            _lib.check(lib.lvsr_train_set_regularization(h, C.byref(cfg)))
+        else:
+            _lib.check(lib.lvsr_train_set_regularization(h, None))
 
     def _world(self):
         import torch.distributed as dist
@@ -407,7 +465,7 @@ class GradientDescent(object):
     def model_prior_variance(self):
         return self.noise_stats()["model_prior_variance"] if self.adaptive_noise else None
 
-    def _forward_backward(self, batch, gscale):
+    def _forward_backward(self, batch, gscale, utterance_offset=0):
         rec = self.recognizer
         torch = rec._torch()
         lib, h = _lib.load(), rec._require_ready()
@@ -432,9 +490,14 @@ class GradientDescent(object):
             raise ValueError("batch shapes disagree: recordings %s mask %s labels %s labels_mask %s" % (
                 tuple(x.shape), None if m is None else tuple(m.shape), tuple(y.shape), None if ym is None else tuple(ym.shape)))
         gs = (1.0 / B) if gscale is None else gscale
+        if self.regularization and self.regularization["dropout"]:
+            _lib.check(lib.lvsr_train_set_utterance_offset(h, int(utterance_offset)))
         _lib.check(lib.lvsr_train_cost_and_grads(
             h, x.data_ptr(), None if m is None else m.data_ptr(), y.data_ptr(), None if ym is None else ym.data_ptr(),
             T, B, L, float(gs), self._cost.data_ptr(), self._buf.data_ptr(), rec._stream()))
+        if self._penalty_on():
+            # the penalty sum rides in the step buffer's padding: the data-parallel step stays one all-reduce
+            _lib.check(lib.lvsr_train_penalty_sum(h, self._buf.data_ptr() + 4 * (self._n + 2), rec._stream()))
         return B
 
     def process_batch(self, batch):
@@ -449,8 +512,9 @@ class GradientDescent(object):
             _lib.check(lib.lvsr_train_apply_updates(h, self._buf.data_ptr(), 1.0, C.byref(self._tc), rec._stream()))
             self.last_batch_size = B
             self.last_cost = self._cost                       # device scalar; .item() synchronises
+            self.last_penalty = self._buf[self._n + 2] / B if self._penalty_on() else None
             return
-        B = self._forward_backward(batch, 1.0)                # gradient SUM over the local utterances
+        B = self._forward_backward(batch, 1.0, self._utterance_offset(dist, batch))   # gradient SUM over the local utterances
         bg_dev, cost_dev = allreduce_step_buffer(self._buf, self._n, B, self._cost, dist)   # the ONE collective of the step
         # the global batch size has to reach the host to become a kernel argument; every rank knows its own B and
         # shards are equal-sized in the data-parallel loop, so the common case needs no synchronisation
@@ -458,6 +522,21 @@ class GradientDescent(object):
         _lib.check(lib.lvsr_train_apply_updates(h, self._buf.data_ptr(), 1.0 / Bg, C.byref(self._tc), rec._stream()))
         self.last_batch_size = Bg
         self.last_cost = cost_dev / Bg
+        self.last_penalty = self._buf[self._n + 2] / Bg if self._penalty_on() else None
+
+    def _penalty_on(self):
+        return bool(self.regularization and self.regularization["penalty_coof"] > 0)
+
+    def _utterance_offset(self, dist, batch):
+        """Global index of this rank's first utterance, the key of its dropout mask: rank * B under equal shards."""
+        if not (self.regularization and self.regularization["dropout"]):
+            return 0
+        if not self.equal_shards:
+            # with unequal shards the offset takes a second collective (a scan of the shard sizes) besides the step's
+            # one all-reduce
+            raise NotImplementedError("data-parallel dropout keys its mask by global utterance index, which needs "
+                                      "equal shards (equal_shards=True): rank r's first utterance is r * B")
+        return dist.get_rank() * len(batch["recordings"][0])
 
     def total_gradient_norm(self):
         lib, h = _lib.load(), self.recognizer._require_ready()

@@ -476,6 +476,7 @@ int lvsr_model_destroy(lvsr_model* m) {
   if (m->align_mem) cudaFree(m->align_mem);
   lvsr_model_clear_lm(m);
   noise_free(m);
+  reg_free(m);
   m->tws.destroy();
   m->ws.destroy();
   delete m;
@@ -823,7 +824,8 @@ int projection_gemm(Arena& ws, const float* A, int M, int K, const float* W, con
 constexpr int ENC_OVERLAP_MIN_SMS = 16;
 
 int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int T, int B, float* attended,
-                float* attended_mask, LayerTape* tape, cudaStream_t st, const float** bottom_out) {
+                float* attended_mask, LayerTape* tape, cudaStream_t st, const float** bottom_out,
+                const DropoutKey* dropout) {
   const lvsr_config& c = m->cfg;
   const float* cur = x;
   int Tl = T, din = encoder_input_dim(m);
@@ -834,6 +836,12 @@ int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int
     cur = y[m->bottom.num_layers - 1];
     if (bottom_out)
       for (int i = 0; i < m->bottom.num_layers; ++i) bottom_out[i] = y[i];
+  }
+  if (dropout) {
+    float* dropped = ws.f32((size_t)T * B * din);
+    LVSR_CHECK(dropped, "out of device memory (dropout)");
+    if (int rc = dropout_apply(*dropout, cur, dropped, T, B, din, st)) return rc;
+    cur = dropped;
   }
   long long mstride = B;
   int kcum = 1;

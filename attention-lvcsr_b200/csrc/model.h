@@ -195,6 +195,18 @@ struct lvsr_model {
     double* part = nullptr;         // device partial sums of the sample pass
     float* norm_part = nullptr;     // device partial squared norms of the gradient transform
   } noise;
+  // ---- dropout and weight noise (noise.cu; lvsr_train_set_regularization) ----
+  struct Reg {
+    bool dropout = false;
+    float level = 0.f;              // weight noise standard deviation (0: off)
+    unsigned long long seed = 1;
+    long long update = 0;           // update counter of both draws; advanced by lvsr_train_apply_updates
+    long long utt_offset = 0;       // global index of the batch's first utterance (dropout key)
+    float* noisy = nullptr;         // flat layout: the means + level * eps of the current step (padding zero)
+    void* spans = nullptr;          // device [params]: (offset, count, subject): 0 for the attention's parameters
+    float penalty_coof = 0.f;       // alignment penalty coefficient (0: off)
+    float* penalty = nullptr;       // device: the penalty sum of the last training forward (penalty_coof > 0)
+  } reg;
 
   const Param* param(const std::string& n) const {     // null when the model has no such parameter
     auto it = index.find(n);
@@ -346,13 +358,22 @@ int fork_copy(lvsr_model* m, const ForkLayout& f, float* W, float* b, float* gra
 int noise_sample(lvsr_model* m, cudaStream_t st);
 int noise_gradients(lvsr_model* m, float* grads, float gscale, float* gls2, cudaStream_t st, int* nparts);
 void noise_free(lvsr_model* m);
+// dropout and weight noise (noise.cu): out = in * the dropout multiplier of update `update` over a [T, B, F] batch whose
+// first utterance has the global index utt_offset (in null: the multiplier itself; in == out is allowed), and the
+// noisy parameter copy reg.noisy of the handle's current update.  reg_free releases the handle's buffers.
+struct DropoutKey { unsigned long long seed; long long update, utt_offset; };
+int dropout_apply(const DropoutKey& key, const float* in, float* out, int T, int B, int F, cudaStream_t st);
+int weight_noise_sample(lvsr_model* m, cudaStream_t st);
+void reg_free(lvsr_model* m);
 // Every encoder layer (fork projection + BiGRU scan) and the mask of the encoded frames: attended [Tp, B, E] (the last
 // layer writes it), attended_mask [Tp, B].  Buffers come from `ws`.  Without a tape (inference) the BiGRU runs without
 // the training stores; with one, tape[l] records layer l's buffers (and allocates hext) for the backward pass.
 // With a bottom MLP it runs first, on all T*B frames; with a tape, bottom_out[i] (LVSR_MAX_BOTTOM entries) records
-// the output of its layer i, after the activation, for the backward pass.
+// the output of its layer i, after the activation, for the backward pass.  dropout (null: none) multiplies the input of
+// layer 0 by its mask, in a copy from `ws` that layer 0's tape records; bottom_out keeps the undropped outputs.
 int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int T, int B, float* attended,
-                float* attended_mask, LayerTape* tape, cudaStream_t st, const float** bottom_out = nullptr);
+                float* attended_mask, LayerTape* tape, cudaStream_t st, const float** bottom_out = nullptr,
+                const DropoutKey* dropout = nullptr);
 // The bottom MLP (bottom.cu): out[i] = act(X_i W_i + b_i) for every layer over `rows` frames, buffers from `ws`
 int bottom_forward(lvsr_model* m, Arena& ws, const float* x, int rows, const float** out, cudaStream_t st);
 // dY [rows, n] <- dY * act'(Y) in place, from the layer's output Y = act(pre) (bottom.cu)

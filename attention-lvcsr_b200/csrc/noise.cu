@@ -17,7 +17,9 @@
 // and ls2 per CTA; one CTA then reduces them in a fixed order, so priors and model cost are deterministic.
 #include <curand_kernel.h>
 
+#include <algorithm>
 #include <cmath>
+#include <string>
 #include <vector>
 
 #include "model.h"
@@ -41,9 +43,14 @@ __device__ __forceinline__ float2 box_muller(unsigned x, unsigned y) {
   return make_float2(r * c, r * s);
 }
 
+// Stream tags of the draws, in the high byte of the fourth Philox counter word (adaptive noise: 0, so its draws are
+// those of an update counter below 2^24 * 2^32)
+constexpr unsigned kTagDropout = 0xD0u << 24, kTagWeightNoise = 0x57u << 24;
+
 // eps of the four flat elements 4q .. 4q+3 (a parameter starts at a multiple of 64, so a group never straddles two)
-__device__ __forceinline__ void eps4(unsigned long long seed, unsigned long long update, unsigned long long q, float e[4]) {
-  const uint4 ctr = make_uint4((unsigned)q, (unsigned)(q >> 32), (unsigned)update, (unsigned)(update >> 32));
+__device__ __forceinline__ void eps4(unsigned long long seed, unsigned long long update, unsigned long long q, float e[4],
+                                     unsigned tag = 0) {
+  const uint4 ctr = make_uint4((unsigned)q, (unsigned)(q >> 32), (unsigned)update, (unsigned)(update >> 32) ^ tag);
   const uint4 r = curand_Philox4x32_10(ctr, make_uint2((unsigned)seed, (unsigned)(seed >> 32)));
   const float2 a = box_muller(r.x, r.y), b = box_muller(r.z, r.w);
   e[0] = a.x; e[1] = a.y; e[2] = b.x; e[3] = b.y;
@@ -163,6 +170,45 @@ __global__ void noise_fill_kernel(float* x, const Span* spans, float v) {
     x[sp.offset + i] = v;
 }
 
+// Dropout multiplier of element (t, b, f) of a [T, B, F] batch: bit f % 128 of the Philox draw keyed by (seed; t,
+// global utterance offset + b, update, tag | f / 128) -> 0 or 2.  in null: the multiplier itself; in may be out.
+__global__ void __launch_bounds__(kThreads) dropout_kernel(const float* in, float* out, long long n, int B, int F,
+                                                           unsigned long long seed, unsigned long long update,
+                                                           long long utt_offset) {
+  const uint2 key = make_uint2((unsigned)seed, (unsigned)(seed >> 32));
+  for (long long i = blockIdx.x * (long long)kThreads + threadIdx.x; i < n; i += (long long)gridDim.x * kThreads) {
+    const long long r = i / F, t = r / B;
+    const unsigned f = (unsigned)(i - r * F);
+    const uint4 ctr = make_uint4((unsigned)t, (unsigned)(utt_offset + (r - t * B)), (unsigned)update, kTagDropout | (f >> 7));
+    const uint4 w = curand_Philox4x32_10(ctr, key);
+    const unsigned q = (f >> 5) & 3u;
+    const unsigned word = q == 0 ? w.x : q == 1 ? w.y : q == 2 ? w.z : w.w;
+    const float mult = ((word >> (f & 31u)) & 1u) ? 2.f : 0.f;
+    out[i] = in ? in[i] * mult : mult;
+  }
+}
+
+// One parameter of the weight noise: its flat span and whether it is a subject (the attention's parameters are not)
+struct RegSpan { long long offset, count; int subject; };
+
+// mean null: eps of the subjects, 0 elsewhere (replay); else noisy = mean + level eps over the subjects, mean elsewhere.
+// The padding between parameters is not written.
+__global__ void __launch_bounds__(kThreads) weight_noise_kernel(const float* __restrict__ mean, float* __restrict__ out,
+                                                                const RegSpan* spans, float level, unsigned long long seed,
+                                                                unsigned long long update) {
+  const RegSpan sp = spans[blockIdx.y];
+  const long long groups = (sp.count + 3) >> 2;
+  for (long long gq = blockIdx.x * (long long)kThreads + threadIdx.x; gq < groups; gq += (long long)gridDim.x * kThreads) {
+    const long long i0 = sp.offset + 4 * gq;
+    float e[4];
+    eps4(seed, update, (unsigned long long)i0 >> 2, e, kTagWeightNoise);
+    for (int j = 0; j < 4 && 4 * gq + j < sp.count; ++j) {
+      if (!mean) out[i0 + j] = sp.subject ? e[j] : 0.f;
+      else out[i0 + j] = sp.subject ? fmaf(level, e[j], mean[i0 + j]) : mean[i0 + j];
+    }
+  }
+}
+
 inline dim3 param_grid(const lvsr_model* m) { return dim3(kCtasPerParam, (unsigned)m->params.size()); }
 inline const Span* spans_of(const lvsr_model* m) { return static_cast<const Span*>(m->noise.spans); }
 
@@ -209,6 +255,31 @@ int noise_gradients(lvsr_model* m, float* grads, float gscale, float* gls2, cuda
   LVSR_LAUNCH_CHECK();
   if (nparts) *nparts = kCtasPerParam * (int)m->params.size();
   return 0;
+}
+
+int dropout_apply(const DropoutKey& key, const float* in, float* out, int T, int B, int F, cudaStream_t st) {
+  ProfScope prof("dropout", st);
+  const long long n = (long long)T * B * F;
+  dropout_kernel<<<(unsigned)std::min<long long>(4096, (n + kThreads - 1) / kThreads), kThreads, 0, st>>>(
+      in, out, n, B, F, key.seed, (unsigned long long)key.update, key.utt_offset);
+  LVSR_LAUNCH_CHECK();
+  return 0;
+}
+
+int weight_noise_sample(lvsr_model* m, cudaStream_t st) {
+  ProfScope prof("weight_noise", st);
+  const lvsr_model::Reg& r = m->reg;
+  weight_noise_kernel<<<param_grid(m), kThreads, 0, st>>>(m->flat, r.noisy, static_cast<const RegSpan*>(r.spans), r.level,
+                                                          r.seed, (unsigned long long)r.update);
+  LVSR_LAUNCH_CHECK();
+  return 0;
+}
+
+void reg_free(lvsr_model* m) {
+  if (m->reg.noisy) cudaFree(m->reg.noisy);
+  if (m->reg.spans) cudaFree(m->reg.spans);
+  if (m->reg.penalty) cudaFree(m->reg.penalty);
+  m->reg = lvsr_model::Reg();
 }
 
 }  // namespace lvsr
@@ -317,6 +388,83 @@ int lvsr_train_noise_gradients(lvsr_model* m, float* grads_dev, float gscale, fl
   if (int rc = bind_stream(m, st)) return rc;
   LVSR_CUDA_OK(cudaMemsetAsync(ls2_grads_dev, 0, (size_t)m->flat_count * sizeof(float), st));
   return noise_gradients(m, grads_dev, gscale, ls2_grads_dev, st, nullptr);
+}
+
+int lvsr_train_set_regularization(lvsr_model* m, const lvsr_regularization* cfg) {
+  LVSR_CHECK(m, "null model");
+  DeviceGuard device_guard(m);
+  if (cfg) {
+    LVSR_CHECK(cfg->dropout == 0 || cfg->dropout == 1, "regularization: dropout must be 0 or 1");
+    LVSR_CHECK(cfg->noise_level >= 0.0 && std::isfinite(cfg->noise_level), "regularization: noise_level must be >= 0");
+    LVSR_CHECK(cfg->penalty_coof >= 0.0 && std::isfinite(cfg->penalty_coof), "regularization: penalty_coof must be >= 0");
+  }
+  if (m->reg.spans || m->reg.penalty) LVSR_CUDA_OK(cudaDeviceSynchronize());     // a training call may still read the buffers
+  reg_free(m);
+  if (!cfg) return 0;
+  lvsr_model::Reg& r = m->reg;
+  r.dropout = cfg->dropout != 0;
+  r.level = (float)cfg->noise_level;
+  r.seed = cfg->seed ? cfg->seed : 1;
+  r.penalty_coof = (float)cfg->penalty_coof;
+  if (r.penalty_coof > 0.f) {
+    LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&r.penalty), sizeof(float)));
+    LVSR_CUDA_OK(cudaMemset(r.penalty, 0, sizeof(float)));
+  }
+  if (r.level > 0.f) {
+    // Blocks' apply_noise subjects: every parameter outside Selector(generator.transition.attention) (lvsr/main.py:297)
+    const size_t np = m->params.size();
+    std::vector<RegSpan> h(np);
+    for (size_t i = 0; i < np; ++i) {
+      const std::string& name = m->params[i].name;
+      const bool attention = name.rfind(std::string(ATT) + "/", 0) == 0 || name.rfind(std::string(CONT) + "/", 0) == 0;
+      h[i] = RegSpan{m->params[i].offset, m->params[i].count, attention ? 0 : 1};
+    }
+    LVSR_CUDA_OK(cudaMalloc(&r.spans, np * sizeof(RegSpan)));
+    LVSR_CUDA_OK(cudaMemcpy(r.spans, h.data(), np * sizeof(RegSpan), cudaMemcpyHostToDevice));
+    LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&r.noisy), (size_t)m->flat_count * sizeof(float)));
+    LVSR_CUDA_OK(cudaMemset(r.noisy, 0, (size_t)m->flat_count * sizeof(float)));
+  }
+  return 0;
+}
+
+int lvsr_train_penalty_sum(lvsr_model* m, float* penalty_dev, void* stream) {
+  LVSR_CHECK(m && penalty_dev, "train_penalty_sum: null argument");
+  LVSR_CHECK(m->reg.penalty, "the alignment penalty is off (lvsr_train_set_regularization)");
+  DeviceGuard device_guard(m);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (int rc = bind_stream(m, st)) return rc;
+  LVSR_CUDA_OK(cudaMemcpyAsync(penalty_dev, m->reg.penalty, sizeof(float), cudaMemcpyDeviceToDevice, st));
+  return 0;
+}
+
+int lvsr_train_set_utterance_offset(lvsr_model* m, int64_t utterance_offset) {
+  LVSR_CHECK(m && utterance_offset >= 0, "train_set_utterance_offset: bad arguments");
+  m->reg.utt_offset = utterance_offset;        // a kernel argument of the next training forward: no wait needed
+  return 0;
+}
+
+int lvsr_train_dropout_mask(lvsr_model* m, int64_t update, int64_t utterance_offset, int32_t T, int32_t B, int32_t F,
+                            float* mult_dev, void* stream) {
+  LVSR_CHECK(m && mult_dev && update >= 0 && utterance_offset >= 0 && T > 0 && B > 0 && F > 0,
+             "train_dropout_mask: bad arguments");
+  DeviceGuard device_guard(m);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (int rc = bind_stream(m, st)) return rc;
+  return dropout_apply(DropoutKey{m->reg.seed, update, utterance_offset}, nullptr, mult_dev, T, B, F, st);
+}
+
+int lvsr_train_weight_noise_sample(lvsr_model* m, int64_t update, float* eps_dev, void* stream) {
+  LVSR_CHECK(m && eps_dev && update >= 0, "train_weight_noise_sample: bad arguments");
+  LVSR_CHECK(m->reg.spans, "weight noise is off (lvsr_train_set_regularization)");
+  DeviceGuard device_guard(m);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (int rc = bind_stream(m, st)) return rc;
+  ProfScope prof("weight_noise", st);
+  LVSR_CUDA_OK(cudaMemsetAsync(eps_dev, 0, (size_t)m->flat_count * sizeof(float), st));
+  weight_noise_kernel<<<param_grid(m), kThreads, 0, st>>>(nullptr, eps_dev, static_cast<const RegSpan*>(m->reg.spans),
+                                                          0.f, m->reg.seed, (unsigned long long)update);
+  LVSR_LAUNCH_CHECK();
+  return 0;
 }
 
 }  // extern "C"

@@ -150,6 +150,8 @@ struct TrainStep {
   float* grads;
   float gscale;
   int B, L, Tp;
+  const DropoutKey* drop;          // dropout on the encoder's input (null: off)
+  float penalty_coof;              // alignment penalty coefficient (0: off)
   const lvsr_config& c = m->cfg;
   Arena& ws = m->tws;
   const long long* lab = reinterpret_cast<const long long*>(labels);
@@ -189,6 +191,8 @@ struct TrainStep {
     bytes += ((size_t)Tp * B * (2 * M + 2 * E) + (size_t)R * (Tp + 8 * C + 3 * E + 2 * M + 3 * Cpm + V + 16) + (size_t)4 * B * Tp +
               (size_t)2 * B * (M + (size_t)K * M + (size_t)K * w) + (size_t)4 * (E + C) * 3 * C + (size_t)80 * E * M) * sizeof(float);
     if (keep_energies) bytes += ((size_t)R * Tp + (size_t)AB_CS * B) * sizeof(float);
+    if (drop) bytes += (size_t)T * B * encoder_input_dim(m) * sizeof(float);      // the dropped encoder input
+    if (penalty_coof > 0.f) bytes += (size_t)R * (Tp + 1) * sizeof(float);      // penalty gradient and row sums
     ws.reserve(bytes, st);
     ArenaScope scope(ws, st);
     for (int l = 0; l < c.num_layers; ++l)
@@ -235,7 +239,7 @@ struct TrainStep {
     d.Hatt = ws.f32((size_t)Tp * B * E);                  // attended [Tp, B, E]
     d.attm = ws.f32((size_t)Tp * B);
     LVSR_CHECK(d.Hatt && d.attm, "out of device memory (encoder output)");
-    if (int rc = run_encoder(m, ws, x, mask, T, B, d.Hatt, d.attm, tape, st, bottom_out)) return rc;
+    if (int rc = run_encoder(m, ws, x, mask, T, B, d.Hatt, d.attm, tape, st, bottom_out, drop)) return rc;
     d.costs = ws.f32((size_t)R);
     d.W_all = ws.f32((size_t)R * Tp);        // alignments alpha_i
     d.S_prev = ws.f32((size_t)R * C);        // s_{i-1}
@@ -333,6 +337,18 @@ struct TrainStep {
     if (acc_b) LVSR_CUDA_OK(cudaMemsetAsync(acc_b, 0, (size_t)nct * sizeof(float), st));
     LVSR_CUDA_OK(cudaMemsetAsync(dsbuf[0], 0, (size_t)B * C * sizeof(float), st));
     if (int rc = onehot_rows(w0, B, Tp, st)) return rc;
+    // the alignment penalty's gradient of every alpha_i (it reads only the taped alignments) and its sum
+    float* pen = nullptr;
+    if (penalty_coof > 0.f) {
+      ProfScope prof_pen("penalty", st);
+      pen = ws.f32((size_t)R * Tp);
+      float* rows = ws.f32((size_t)R);
+      LVSR_CHECK(pen && rows, "out of device memory (alignment penalty)");
+      penalty_grad_kernel<<<ceil_div(R, 256), 256, 0, st>>>(d.W_all, lmask, L, B, Tp, penalty_coof * gscale, pen, rows);
+      LVSR_LAUNCH_CHECK();
+      sum_all_kernel<<<1, 1024, 0, st>>>(rows, R, m->reg.penalty, 1.f);
+      LVSR_LAUNCH_CHECK();
+    }
     void (*att_bwd)(AttBwdArgs, int) = att_bwd_content_kernel;
     if (!content) {
       const bool kp12 = att_bwd_kp(K) == 12;
@@ -375,6 +391,7 @@ struct TrainStep {
       ab.acc_v = acc_v; ab.acc_Wh = acc_Wh; ab.acc_filt = acc_filt;
       ab.B = B; ab.Tp = Tp; ab.M = M; ab.E = E; ab.K = K; ab.n = n;
       ab.e_cur = d.E_all ? d.E_all + (size_t)i * B * Tp : nullptr; ab.acc_b = acc_b;
+      ab.pen = pen ? pen + (size_t)i * B * Tp : nullptr;
       {
         ProfScope prof_ab("att_bwd", st);
         att_bwd<<<nct, AB_NT, ab_smem, st>>>(ab, tc_cap);
@@ -585,18 +602,42 @@ struct TrainStep {
         dout = dX0 = dX;
       }
     }
-    return m->bottom.num_layers ? bottom_backward(x, bottom_out, dX0, tape[0].T * B) : 0;
+    if (!m->bottom.num_layers) return 0;
+    // the gradient of the bottom's output passes the multiplier that dropped it in the forward
+    if (drop) if (int rc = dropout_apply(*drop, dX0, dX0, tape[0].T, B, tape[0].Din, st)) return rc;
+    return bottom_backward(x, bottom_out, dX0, tape[0].T * B);
   }
 };
 
 // forward + backward of one batch on the parameters Param::dev points at and the weights packed from them
 int forward_backward(lvsr_model* m, const float* x, const float* mask, const int64_t* labels, const float* lmask,
-                     int32_t T, int32_t B, int32_t L, float gscale, float* cost_out, float* grads, void* stream) {
+                     int32_t T, int32_t B, int32_t L, float gscale, float* cost_out, float* grads, void* stream,
+                     const DropoutKey* drop) {
   if (int rc = check_ready(m)) return rc;
   LVSR_CHECK(x && labels && cost_out && grads && T > 0 && B > 0 && L > 0, "train_cost_and_grads: bad arguments");
   LVSR_CHECK(!lm_attached(m), "train_cost_and_grads: shallow fusion is inference only (detach the language model)");
-  return TrainStep{m, static_cast<cudaStream_t>(stream), labels, lmask, grads, gscale, B, L, lvsr_encoded_length(m, T)}
+  return TrainStep{m, static_cast<cudaStream_t>(stream), labels, lmask, grads, gscale, B, L, lvsr_encoded_length(m, T),
+                   drop, m->reg.penalty_coof}
       .run(x, mask, T, cost_out);
+}
+
+// forward_backward on the parameter copy `copy` (flat layout): every parameter pointer is re-pointed at it and the
+// kernel-side weights are re-packed from it; on every way out the pointers go back to the means and the handle is
+// marked un-finalized, so any other entry point re-packs from the means first.
+int forward_backward_on(lvsr_model* m, const float* copy, const float* x, const float* mask, const int64_t* labels,
+                        const float* lmask, int32_t T, int32_t B, int32_t L, float gscale, float* cost_out, float* grads,
+                        void* stream, const DropoutKey* drop) {
+  struct Restore {
+    lvsr_model* m;
+    ~Restore() {
+      for (Param& p : m->params) p.dev = m->flat + p.offset;
+      m->finalized = false;
+      m->noise.stale = true;         // the step may still read the noisy packing on its own stream (check_ready)
+    }
+  } restore{m};
+  for (Param& p : m->params) p.dev = const_cast<float*>(copy) + p.offset;
+  if (int rc = finalize_on_stream(m, static_cast<cudaStream_t>(stream), false)) return rc;
+  return forward_backward(m, x, mask, labels, lmask, T, B, L, gscale, cost_out, grads, stream, drop);
 }
 
 }  // namespace
@@ -610,23 +651,25 @@ int lvsr_train_cost_and_grads(lvsr_model* m, const float* x, const float* mask, 
              "train_cost_and_grads: a stacked decoder (dec_stack %d) is inference only: no backward pass through the "
              "RecurrentStack", m ? m->cfg.dec_stack : 0);
   if (int rc = bind_stream(m, static_cast<cudaStream_t>(stream))) return rc;
-  if (!m->noise.on) return forward_backward(m, x, mask, labels, lmask, T, B, L, gscale, cost_out, grads, stream);
-  // adaptive weight noise (noise.cu): the step runs on p + eps sqrt(s2).  Every parameter pointer is re-pointed at
-  // the noisy copy and the kernel-side weights are re-packed from it; on every way out the pointers go back to the
-  // means and the handle is marked un-finalized, so any other entry point re-packs from the means first.
+  const lvsr_model::Reg& r = m->reg;
+  const bool weight_noise = r.level > 0.f;
+  LVSR_CHECK(!(m->noise.on && (r.dropout || weight_noise || r.penalty_coof > 0.f)),
+             "train_cost_and_grads: dropout, weight noise and the alignment penalty have no effect under adaptive noise "
+             "(lvsr/main.py:425-437): turn them off (lvsr_train_set_regularization)");
+  const DropoutKey key{r.seed, r.update, r.utt_offset};
+  const DropoutKey* drop = r.dropout ? &key : nullptr;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (int rc = noise_sample(m, st)) return rc;
-  struct Restore {
-    lvsr_model* m;
-    ~Restore() {
-      for (Param& p : m->params) p.dev = m->flat + p.offset;
-      m->finalized = false;
-      m->noise.stale = true;         // the step may still read the noisy packing on its own stream (check_ready)
-    }
-  } restore{m};
-  for (Param& p : m->params) p.dev = m->noise.noisy + p.offset;
-  if (int rc = finalize_on_stream(m, st, false)) return rc;
-  return forward_backward(m, x, mask, labels, lmask, T, B, L, gscale, cost_out, grads, stream);
+  if (m->noise.on) {
+    // adaptive weight noise (noise.cu): the step runs on p + eps sqrt(s2)
+    if (int rc = noise_sample(m, st)) return rc;
+    return forward_backward_on(m, m->noise.noisy, x, mask, labels, lmask, T, B, L, gscale, cost_out, grads, stream, drop);
+  }
+  if (weight_noise) {
+    // weight noise (noise.cu): the step runs on p + level eps, the attention's parameters as they are
+    if (int rc = weight_noise_sample(m, st)) return rc;
+    return forward_backward_on(m, r.noisy, x, mask, labels, lmask, T, B, L, gscale, cost_out, grads, stream, drop);
+  }
+  return forward_backward(m, x, mask, labels, lmask, T, B, L, gscale, cost_out, grads, stream, drop);
 }
 
 // Parameters with the WEIGHT role, the subjects of weight decay and max-norm (lvsr/main.py:418-420,493): Linear and
@@ -715,6 +758,7 @@ int lvsr_train_apply_updates(lvsr_model* m, float* grads, float gscale, const lv
     burn_mult = m->burn_in_left <= 0 ? 1.f : 0.f;
     m->burn_in_left = std::max<long long>(0, m->burn_in_left - 1);
   }
+  m->reg.update++;     // the next step draws a fresh dropout mask and weight noise
   if (z.on) {          // RemoveNotFinite per tensor: every ls2 is a tensor of its own; no max-norm (PARAMETER role only)
     apply_update_pair_kernel<<<2 * np, 256, 0, st>>>(m->flat, grads, z.ls2, z.gls2, desc, np, burn_mult);
     LVSR_LAUNCH_CHECK();
@@ -728,6 +772,12 @@ int lvsr_train_apply_updates(lvsr_model* m, float* grads, float gscale, const lv
   }
   apply_update_kernel<<<np, 256, 0, st>>>(m->flat, grads, desc, burn_mult);
   LVSR_LAUNCH_CHECK();
+  if (m->reg.level > 0.f) {
+    // as under adaptive noise: the next training forward packs its noisy copy, other entry points pack the means
+    z.stale = true;
+    m->finalized = false;
+    return 0;
+  }
   return finalize_on_stream(m, st, false);             // re-pack the kernel-side weights from the new parameters
 }
 
@@ -748,6 +798,7 @@ int lvsr_train_reset(lvsr_model* m) {
   if (m->noise.on) LVSR_CUDA_OK(cudaMemsetAsync(m->noise.velocity, 0, 3 * bytes, st));     // velocity | ms_step | ms_dx of ls2
   if (m->clip) LVSR_CUDA_OK(cudaMemcpyAsync(m->clip, m->clip_init, sizeof(m->clip_init), cudaMemcpyHostToDevice, st));
   m->burn_in_left = -1;
+  m->reg.update = 0;
   return 0;
 }
 

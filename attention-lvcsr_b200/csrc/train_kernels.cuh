@@ -475,7 +475,47 @@ struct AttBwdArgs {
   int B, Tp, M, E, K, n;
   const float* e_cur;        // [B, Tp]  energies of step i, bias included (logistic / relu only)
   float* acc_b;              // [2B]     per-CTA partial sums of de (logistic / relu only)
+  const float* pen;          // [B, Tp]  gradient of the alignment penalty w.r.t. alpha_i, or nullptr (none)
 };
+
+// Alignment monotonicity penalty (lvsr/expressions.py:14-19) of the taped alignments W [L, B, Tp], c_i = cumsum_t w_i:
+//   P = sum_b sum_{i>=1} m[i,b] sum_t max(c_i[t] - c_{i-1}[t], 0)
+//   dP/dw_i[t'] = sum_{t>=t'} (m_i [c_i[t] >= c_{i-1}[t]] - m_{i+1} [c_{i+1}[t] >= c_i[t]])   (first term absent for
+//   i = 0, second for i = L-1; a tie counts as 1, the gradient of Theano's maximum)
+// One thread per (i, b) row: grad [L, B, Tp] = scale * dP/dw, row_sum [L * B] = the row's term of P (0 for i = 0).
+__global__ void __launch_bounds__(256) penalty_grad_kernel(const float* __restrict__ W, const float* __restrict__ lmask,
+                                                           int L, int B, int Tp, float scale, float* __restrict__ grad,
+                                                           float* __restrict__ row_sum) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= L * B) return;
+  const int i = r / B, b = r % B;
+  const float* wc = W + (size_t)r * Tp;
+  const float* wp = i > 0 ? wc - (size_t)B * Tp : nullptr;
+  const float* wn = i + 1 < L ? wc + (size_t)B * Tp : nullptr;
+  const float mi = i > 0 ? (lmask ? lmask[r] : 1.f) : 0.f;
+  const float mn = wn ? (lmask ? lmask[r + B] : 1.f) : 0.f;
+  float* g = grad + (size_t)r * Tp;
+  float cp = 0.f, cc = 0.f, cn = 0.f, sum = 0.f;
+  for (int t = 0; t < Tp; ++t) {
+    cc += wc[t];
+    float v = 0.f;
+    if (wp) {
+      cp += wp[t];
+      if (cc >= cp) { v += mi; sum += cc - cp; }
+    }
+    if (wn) {
+      cn += wn[t];
+      if (cn >= cc) v -= mn;
+    }
+    g[t] = v;
+  }
+  float acc = 0.f;
+  for (int t = Tp - 1; t >= 0; --t) {
+    acc += g[t];
+    g[t] = scale * acc;
+  }
+  row_sum[r] = mi * sum;
+}
 
 __host__ __device__ inline int att_bwd_kp(int K) { return K <= 12 ? 12 : 16; }     // padded row of K filter values (float4 loads)
 
@@ -549,6 +589,11 @@ __global__ void __launch_bounds__(AB_NT, 1) att_bwd_kernel(AttBwdArgs a, int tc_
       const long long o = (long long)b * Tp + b0 + t;
       part += a.w_cur[o] * (a.dA_in[o] + a.dA_in[(long long)B * Tp + o]);
     }
+  if (a.pen)           // the penalty's gradient of alpha_i joins the carry
+    for (int t = tid; t < Tw; t += AB_NT) {
+      const long long o = (long long)b * Tp + b0 + t;
+      part += a.w_cur[o] * a.pen[o];
+    }
   const float S = block_sum_512(part, sred);      // (contains the __syncthreads that publish the staging)
 
   // ---- de[t] for the owned positions (softmax: alpha_i[t] (dctx . H[t] + carry[t] - S)): one warp per position ----
@@ -564,7 +609,8 @@ __global__ void __launch_bounds__(AB_NT, 1) att_bwd_kernel(AttBwdArgs a, int tc_
     d = warp_sum(d);
     if (lane == 0) {
       const long long o = (long long)b * Tp + pos;
-      const float carry = a.dA_in ? (a.dA_in[o] + a.dA_in[(long long)B * Tp + o]) : 0.f;
+      float carry = a.dA_in ? (a.dA_in[o] + a.dA_in[(long long)B * Tp + o]) : 0.f;
+      if (a.pen) carry += a.pen[o];
       if constexpr (NORM == LVSR_NORM_SOFTMAX) {
         sde[t] = a.w_cur[o] * (d + carry - S);
       } else if constexpr (NORM == LVSR_NORM_LOGISTIC) {
@@ -767,9 +813,11 @@ __global__ void __launch_bounds__(AB_NT, 1) att_bwd_content_kernel(AttBwdArgs a,
   // S = sum_t alpha_i[t] dalpha_i[t] = dctx . ctx_i
   float part = 0.f;
   for (int i = tid; i < E; i += AB_NT) part += a.dctx[(long long)b * E + i] * a.ctx[(long long)b * E + i];
+  if (a.pen)           // + sum_t alpha_i[t] pen[t]: the penalty's gradient of alpha_i
+    for (int t = tid; t < Tp; t += AB_NT) part += a.w_cur[(long long)b * Tp + t] * a.pen[(long long)b * Tp + t];
   const float S = block_sum_512(part, sred);      // (contains the __syncthreads that publish the staging)
 
-  // ---- de[t] = alpha_i[t] (dctx . H[t] - S) for the owned positions: one warp per position ----
+  // ---- de[t] = alpha_i[t] (dctx . H[t] (+ pen[t]) - S) for the owned positions: one warp per position ----
   for (int t = warp; t < nt; t += AB_NT / 32) {
     const long long pos = t0 + t;
     const float* hrow = a.H + (pos * B + b) * E;
@@ -780,7 +828,10 @@ __global__ void __launch_bounds__(AB_NT, 1) att_bwd_content_kernel(AttBwdArgs a,
       d = fmaf(h4.x, c4.x, d); d = fmaf(h4.y, c4.y, d); d = fmaf(h4.z, c4.z, d); d = fmaf(h4.w, c4.w, d);
     }
     d = warp_sum(d);
-    if (lane == 0) sde[t] = a.w_cur[(long long)b * Tp + pos] * (d - S);
+    if (lane == 0) {
+      const long long o = (long long)b * Tp + pos;
+      sde[t] = a.pen ? a.w_cur[o] * (d + a.pen[o] - S) : a.w_cur[o] * (d - S);
+    }
   }
   __syncthreads();
 

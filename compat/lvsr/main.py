@@ -193,12 +193,21 @@ def train(config, save_path, bokeh_name="", params=None, bokeh_server=None, boke
         # lvsr/main.py:425-437: every parameter gets trained Gaussian noise; N is the size of the training set
         logger.info("apply adaptive noise")
         adaptive_noise = dict(reg_conf["adaptive_noise"], num_examples=data.get_dataset("train").num_examples)
+    # lvsr/main.py:400-417: dropout on the bottom's output, noise on every parameter outside the attention, the
+    # alignment penalty; a config that applies none of them trains exactly as without the keys
+    extra = {}
+    if reg_conf.get("dropout"):
+        logger.info("apply dropout")
+    if reg_conf.get("noise"):
+        logger.info("apply noise")
+    if reg_conf.get("dropout") or reg_conf.get("noise") or reg_conf.get("penalty_coof", 0.0) > 0:
+        extra["regularization"] = {k: reg_conf[k] for k in ("dropout", "noise", "penalty_coof") if k in reg_conf}
     step_rule = pkg.step_rule_from_config(train_conf, reg_conf)
     if train_conf.get("gradient_threshold"):
         pkg.adaptive_clipping(step_rule, burnin_period=CLIPPING_BURNIN_PERIOD, decay_rate=CLIPPING_DECAY_RATE)
     clipping = pkg.clipping_rule(step_rule)
     algorithm = pkg.GradientDescent(recognizer=recognizer, step_rule=step_rule,
-                                    decay=reg_conf.get("decay", 0.0), adaptive_noise=adaptive_noise)
+                                    decay=reg_conf.get("decay", 0.0), adaptive_noise=adaptive_noise, **extra)
     algorithm.initialize()
     if adaptive_noise and params:
         _load_noise_parameters(algorithm, params)

@@ -420,6 +420,46 @@ int lvsr_train_noise_sample(lvsr_model* m, int64_t update, float* eps_dev, void*
 int lvsr_train_noise_params(lvsr_model* m, float* noisy_dev, void* stream);
 int lvsr_train_noise_gradients(lvsr_model* m, float* grads_dev, float gscale, float* ls2_grads_dev, void* stream);
 
+/* ---- dropout and weight noise: regularization.dropout / regularization.noise (lvsr/main.py:400-408) ----
+ * While they are on, lvsr_train_cost_and_grads runs the step on regularised inputs; every other entry point
+ * (cost, search, sampling, validation statistics) never applies them.
+ *   dropout: the encoder's input (the recordings, or the bottom MLP's last output) is multiplied by Bernoulli(0.5) / 0.5
+ *     element-wise, padded frames included (Blocks' apply_dropout).  The multiplier of element (t, b, f) is 0 or 2,
+ *     drawn from Philox-4x32-10 keyed by (seed, update counter, global utterance index = utterance offset + b, t, f): a
+ *     data-parallel rank given the offset of its first utterance draws the mask the one-GPU step on the concatenated
+ *     batch draws.  The caller's recordings are not changed; with a bottom MLP its gradient passes the same multiplier.
+ *   noise_level > 0: every parameter outside the attention brick (conv_att / cont_att) is perturbed by
+ *     noise_level * eps, eps ~ N(0, 1) per element (Philox keyed by (seed, update counter, flat index), Box-Muller),
+ *     for forward and backward (Blocks' apply_noise); the gradient at the noisy point is applied to the clean means,
+ *     which decay and max-norm act on.  The attention's parameters are used as they are.
+ * The update counter is advanced by lvsr_train_apply_updates and cleared by lvsr_train_reset and by
+ * lvsr_train_set_regularization, so two lvsr_train_cost_and_grads calls between updates draw the same mask and noise.
+ * Refused together with adaptive noise, under which the reference trains on the clean graph (lvsr/main.py:425-437).
+ * lvsr_train_set_regularization sets them (NULL: both off); seed 0 means 1, Blocks' default seed.
+ * lvsr_train_set_utterance_offset sets the global index of the batch's first utterance for the next steps (0 after
+ *   lvsr_train_set_regularization).
+ * lvsr_train_dropout_mask writes the multiplier of update `update` for a [T, B, F] batch whose first utterance has
+ *   the global index `utterance_offset` (F: the encoder's input width).
+ * lvsr_train_weight_noise_sample writes the eps of update `update` in the flat layout, exactly 0 in the padding and
+ *   over the attention's parameters.
+ * penalty_coof > 0: the alignment monotonicity penalty (lvsr/expressions.py:14-19) of the regularised forward's
+ *   alignments w [L, B, T'], P = sum_b sum_{i>=1} m[i,b] sum_t max(c_i[t] - c_{i-1}[t], 0) with c_i = cumsum_t w_i and
+ *   m the labels mask, adds penalty_coof * gscale * dP/dw to the alignment gradients (a tie c_i = c_{i-1} counts as
+ *   increasing, as Theano's maximum does).  cost_dev stays the task cost; lvsr_train_penalty_sum copies P of the last
+ *   training forward (a float, unscaled) to a device address on the stream, e.g. a slot of the all-reduced buffer. */
+typedef struct {
+  int32_t dropout;                 /* 1: dropout on the encoder's input, keep probability 0.5               */
+  double noise_level;              /* standard deviation of the weight noise, 0 = off                        */
+  double penalty_coof;             /* coefficient of the alignment penalty, 0 = off                          */
+  uint64_t seed;                   /* key of both draws (0: 1)                                               */
+} lvsr_regularization;
+int lvsr_train_set_regularization(lvsr_model* m, const lvsr_regularization* cfg);
+int lvsr_train_set_utterance_offset(lvsr_model* m, int64_t utterance_offset);
+int lvsr_train_dropout_mask(lvsr_model* m, int64_t update, int64_t utterance_offset, int32_t T, int32_t B, int32_t F,
+                            float* mult_dev, void* stream);
+int lvsr_train_weight_noise_sample(lvsr_model* m, int64_t update, float* eps_dev, void* stream);
+int lvsr_train_penalty_sum(lvsr_model* m, float* penalty_dev, void* stream);
+
 /* Counters for bench.py: number of kernels this library launched since the last reset. */
 int64_t lvsr_launch_count(int reset);
 
@@ -427,7 +467,8 @@ int64_t lvsr_launch_count(int reset);
  * launch of that class) -- the analogue of the reference's Theano ProfileStats
  * (libs/Theano/theano/compile/profiling.py:97).  Classes: "gemm", "bigru", "attention",
  * "window", "dense", "readout", "lm", "noise" (adaptive weight noise), "bottom" (the bottom MLP's forward, its
- * GEMMs included) and "bottom_bwd" (its backward).  lvsr_profile_read synchronises the device, returns the
+ * GEMMs included), "bottom_bwd" (its backward), "dropout" (the training dropout's forward and backward) and
+ * "weight_noise" (the sample of regularization.noise) and "penalty" (the alignment penalty's gradient and sum).  lvsr_profile_read synchronises the device, returns the
  * summed milliseconds and launch count recorded since the last read of that class. */
 int lvsr_profile_enable(int on);
 int lvsr_profile_read(const char* kernel_class, double* total_ms, int64_t* count);
