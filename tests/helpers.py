@@ -204,3 +204,76 @@ PYRAMID = dict(num_features=40, dims_bidir=[128, 128, 128], subsample=[1, 2, 2],
                conv_n=12, conv_num_filters=10, num_phonemes=32, post_merge_dims=[128], maxout_pieces=2)
 WSJ = dict(num_features=40, dims_bidir=[256, 256, 256, 256], subsample=[1, 1, 2, 2], dim_dec=256, dim_matcher=512,
            conv_n=100, conv_num_filters=10, num_phonemes=32, post_merge_dims=[256], maxout_pieces=2)
+
+
+_READOUT = "/recognizer/generator/readout/post_merge/mlp/linear_0"
+
+
+def bottom_recognizer(cfg, params=None, lm=None, cmap=None):
+    """A SpeechRecognizer of a bottom_oracle config (a bottom MLP in front of the encoder)."""
+    pkg = package()
+    content = cfg.get("attention_type") == "content"
+    act = {"relu": pkg.Rectifier(), "tanh": pkg.Tanh()}[cfg["bottom"]["activation"]]
+    rec = pkg.SpeechRecognizer(
+        input_dims={"recordings": cfg["num_features"]}, input_num_chars={}, eos_label=cfg["eos_label"],
+        num_phonemes=cfg["num_phonemes"], dim_dec=cfg["dim_dec"], dims_bidir=cfg["dims_bidir"],
+        subsample=cfg["subsample"], conv_n=None if content else cfg["conv_n"],
+        conv_num_filters=cfg["conv_num_filters"], dim_matcher=cfg["dim_matcher"],
+        post_merge_dims=cfg["post_merge_dims"], post_merge_activation=pkg.Maxout(cfg["maxout_pieces"]),
+        dim_output_embedding=cfg["dim_feedback"] if cfg.get("embed_outputs", True) else None,
+        embed_outputs=cfg.get("embed_outputs", True), prior=None if content else cfg["prior"],
+        energy_normalizer=None if content else cfg["energy_normalizer"],
+        attention_type="content" if content else "content_and_conv",
+        max_decoded_length_scale=cfg["max_decoded_length_scale"], enc_transition=pkg.GatedRecurrent,
+        dec_transition=pkg.GatedRecurrent, data_prepend_eos=False, lm=lm, character_map=cmap,
+        dec_stack=cfg.get("dec_stack", 1), bottom=dict(dims=cfg["bottom"]["dims"], activation=act))
+    if params is not None:
+        rec.set_parameter_values(params)
+    return rec
+
+
+def bottom_params(cfg, seed, gain=1.0, eos_bias=None):
+    """Trained-like float32 parameters (scale 10) with biases of the bottom drawn too."""
+    import bottom_oracle
+    from collections import OrderedDict
+    p = bottom_oracle.init_params(cfg, seed=seed, scale=10.0)
+    rng = np.random.RandomState(seed + 100)
+    for i, d in enumerate(cfg["bottom"]["dims"]):
+        p[bottom_oracle.linear_name(i) + ".W"] *= 10.0 / np.sqrt(p[bottom_oracle.linear_name(i) + ".W"].shape[0])   # pre-activations O(1)
+        p[bottom_oracle.linear_name(i) + ".b"] = rng.normal(0, 0.3, size=d)
+    p[_READOUT + ".W"] = p[_READOUT + ".W"] * gain
+    if eos_bias is not None:
+        p[_READOUT + ".b"][cfg["eos_label"]] = eos_bias
+    return OrderedDict((k, f32(v)) for k, v in p.items())
+
+
+def check_overlap_claims(rec, plan, B, subsample):
+    """Every tile the launch beside a scan claimed had all its rows final at the progress it was claimed at: input frame
+    f of layer l is the scan's output frame f, stored at scan step f k by the forward direction and at step T - 1 - f k
+    by the backward one, so it is final once forward progress > f k and backward progress >= T - f k."""
+    for l, p in enumerate(plan):
+        if not p["overlap"]:
+            continue
+        T, k, M = plan[l - 1]["T"], subsample[l - 1], p["T"] * B
+        tiles = p["tiles_beside"] + p["tiles_after"]
+        rec_ = rec.encoder_overlap_claims(l, tiles).astype(np.int64)
+        rec_ = rec_[rec_[:, 0] > 0]
+        assert len(rec_) == p["tiles_beside"], (l, len(rec_), p)
+        r0 = (rec_[:, 0] - 1) * 128
+        r1 = np.minimum(r0 + 128, M) - 1
+        f_lo, f_hi = r0 // B, r1 // B
+        early = (rec_[:, 1] < f_hi * k + 1) | (rec_[:, 2] < T - f_lo * k)
+        assert not early.any(), ("layer %d: %d of %d tiles claimed before their rows were final" %
+                                 (l, early.sum(), len(rec_)), rec_[early][:5], f_lo[early][:5], f_hi[early][:5])
+
+
+def bench_recognizer():
+    """The recognizer bench.py --mode train builds (bench.NET at bench.TRAIN_WORKLOAD's features and vocabulary)."""
+    import bench
+    pkg = package()
+    W, N = bench.TRAIN_WORKLOAD, bench.NET
+    return pkg.SpeechRecognizer(
+        input_dims={"recordings": W["F"]}, input_num_chars={}, eos_label=W["V"] - 1, num_phonemes=W["V"],
+        dim_dec=N["dim_dec"], dims_bidir=N["dims_bidir"], subsample=N["subsample"], conv_n=N["conv_n"],
+        conv_num_filters=N["conv_num_filters"], dim_matcher=N["dim_matcher"], post_merge_dims=N["post_merge_dims"],
+        post_merge_activation=pkg.Maxout(2), enc_transition=pkg.GatedRecurrent, dec_transition=pkg.GatedRecurrent)

@@ -24,6 +24,7 @@ import lm_oracle as LO
 import stack_oracle as SO
 from compat_helpers import COMPAT, write_experiment
 from helpers import O, elementwise_err, f32, package, rel_err
+from helpers import bottom_params as _params, bottom_recognizer as _recognizer
 from oracle import lvsr_oracle_grad as G
 from test_gpu_attention_plans import TOL, _compare
 from test_gpu_widths import _same_up_to_near_ties
@@ -53,39 +54,6 @@ def _config(arch, dims, activation, attention_type="content_and_conv", dec_stack
     return BO.make_config(base, dims, activation)
 
 
-def _recognizer(cfg, params=None, lm=None, cmap=None):
-    pkg = package()
-    content = cfg.get("attention_type") == "content"
-    act = {"relu": pkg.Rectifier(), "tanh": pkg.Tanh()}[cfg["bottom"]["activation"]]
-    rec = pkg.SpeechRecognizer(
-        input_dims={"recordings": cfg["num_features"]}, input_num_chars={}, eos_label=cfg["eos_label"],
-        num_phonemes=cfg["num_phonemes"], dim_dec=cfg["dim_dec"], dims_bidir=cfg["dims_bidir"],
-        subsample=cfg["subsample"], conv_n=None if content else cfg["conv_n"],
-        conv_num_filters=cfg["conv_num_filters"], dim_matcher=cfg["dim_matcher"],
-        post_merge_dims=cfg["post_merge_dims"], post_merge_activation=pkg.Maxout(cfg["maxout_pieces"]),
-        dim_output_embedding=cfg["dim_feedback"] if cfg.get("embed_outputs", True) else None,
-        embed_outputs=cfg.get("embed_outputs", True), prior=None if content else cfg["prior"],
-        energy_normalizer=None if content else cfg["energy_normalizer"],
-        attention_type="content" if content else "content_and_conv",
-        max_decoded_length_scale=cfg["max_decoded_length_scale"], enc_transition=pkg.GatedRecurrent,
-        dec_transition=pkg.GatedRecurrent, data_prepend_eos=False, lm=lm, character_map=cmap,
-        dec_stack=cfg.get("dec_stack", 1), bottom=dict(dims=cfg["bottom"]["dims"], activation=act))
-    if params is not None:
-        rec.set_parameter_values(params)
-    return rec
-
-
-def _params(cfg, seed, gain=1.0, eos_bias=None):
-    """Trained-like float32 parameters (scale 10) with biases of the bottom drawn too."""
-    p = BO.init_params(cfg, seed=seed, scale=10.0)
-    rng = np.random.RandomState(seed + 100)
-    for i, d in enumerate(cfg["bottom"]["dims"]):
-        p[BO.linear_name(i) + ".W"] *= 10.0 / np.sqrt(p[BO.linear_name(i) + ".W"].shape[0])   # pre-activations O(1)
-        p[BO.linear_name(i) + ".b"] = rng.normal(0, 0.3, size=d)
-    p[_RO + ".W"] = p[_RO + ".W"] * gain
-    if eos_bias is not None:
-        p[_RO + ".b"][cfg["eos_label"]] = eos_bias
-    return OrderedDict((k, f32(v)) for k, v in p.items())
 
 
 def test_parameter_table_and_refusals():

@@ -6,6 +6,7 @@ import numpy as np
 import pytest
 
 from helpers import O, WSJ, check_grads, f32, make_recognizer
+from helpers import check_overlap_claims as _check_claims
 
 pytestmark = pytest.mark.gpu
 
@@ -20,26 +21,6 @@ def _torch():
 def _encode(rec, x, m):
     att, attm = rec.encode(x, m)
     return att.cpu().numpy(), attm.cpu().numpy(), rec.encoder_plan()
-
-
-def _check_claims(rec, plan, B, subsample):
-    """Every tile the launch beside a scan claimed had all its rows final at the progress it was claimed at: input frame
-    f of layer l is the scan's output frame f, stored at scan step f k by the forward direction and at step T - 1 - f k
-    by the backward one, so it is final once forward progress > f k and backward progress >= T - f k."""
-    for l, p in enumerate(plan):
-        if not p["overlap"]:
-            continue
-        T, k, M = plan[l - 1]["T"], subsample[l - 1], p["T"] * B
-        tiles = p["tiles_beside"] + p["tiles_after"]
-        rec_ = rec.encoder_overlap_claims(l, tiles).astype(np.int64)
-        rec_ = rec_[rec_[:, 0] > 0]
-        assert len(rec_) == p["tiles_beside"], (l, len(rec_), p)
-        r0 = (rec_[:, 0] - 1) * 128
-        r1 = np.minimum(r0 + 128, M) - 1
-        f_lo, f_hi = r0 // B, r1 // B
-        early = (rec_[:, 1] < f_hi * k + 1) | (rec_[:, 2] < T - f_lo * k)
-        assert not early.any(), ("layer %d: %d of %d tiles claimed before their rows were final" %
-                                 (l, early.sum(), len(rec_)), rec_[early][:5], f_lo[early][:5], f_hi[early][:5])
 
 
 def _case(net, B, T, seed, monkeypatch, one_frame=False, spin_limit=None, warm=False, reps=1):
