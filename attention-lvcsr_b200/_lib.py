@@ -116,6 +116,7 @@ SIGNATURES = {
     "lvsr_version": (C.c_int, []),
     "lvsr_model_create": (C.c_int, [C.POINTER(LvsrConfig), C.POINTER(_P)]),
     "lvsr_model_create_bottom": (C.c_int, [C.POINTER(LvsrConfig), C.POINTER(LvsrBottomConfig), C.POINTER(_P)]),
+    "lvsr_model_create_encoder": (C.c_int, [C.POINTER(LvsrConfig), C.POINTER(LvsrBottomConfig), C.c_int32, C.POINTER(_P)]),
     "lvsr_model_destroy": (C.c_int, [_P]),
     "lvsr_model_num_params": (C.c_int, [_P]),
     "lvsr_model_param_name": (C.c_char_p, [_P, C.c_int]),

@@ -75,8 +75,8 @@ void build_param_table(lvsr_model* m) {
   int din = encoder_input_dim(m);
   for (int l = 0; l < c.num_layers; ++l) {
     const int D = c.dims_bidir[l];
-    for (int dir = 0; dir < 2; ++dir) {
-      const std::string b = enc_base(l, dir);
+    for (int dir = 0; dir < encoder_dirs(m); ++dir) {
+      const std::string b = enc_base(m, l, dir);
       add_param(m, b + "/gatedrecurrent.state_to_state", D, D);
       add_param(m, b + "/gatedrecurrent.state_to_gates", D, 2 * D);
       add_param(m, b + "/gatedrecurrent.initial_state", D);
@@ -85,7 +85,7 @@ void build_param_table(lvsr_model* m) {
       add_param(m, b + "/fork/fork_gate_inputs.b", 2 * D);
       add_param(m, b + "/fork/fork_gate_inputs.W", din, 2 * D);
     }
-    din = 2 * D;
+    din = encoder_output_dim(m, l);
   }
   // SpeechRecognizer.children = [encoder, top, bottom, generator] (lvsr/bricks/recognizer.py:350); Linear._allocate
   // makes W before b (libs/blocks/blocks/bricks/simple.py)
@@ -306,10 +306,10 @@ size_t encoder_ws_bytes(const lvsr_model* m, int T, int B) {
   size_t total = 0;
   int Tl = T;
   for (int l = 0; l < m->cfg.num_layers; ++l) {
-    const int D = m->cfg.dims_bidir[l], k = m->cfg.subsample[l];
+    const int D = m->cfg.dims_bidir[l], k = m->cfg.subsample[l], nd = encoder_dirs(m);
     const int Tout = ceil_div(Tl, k);
-    total += ((size_t)Tl * B * 6 * D + (size_t)Tout * B * 2 * D) * sizeof(float) + 1024;
-    total += (size_t)2 * Tl * B * gemm_tc_kpad(l == 0 ? encoder_input_dim(m) : 2 * m->cfg.dims_bidir[l - 1]) * sizeof(float) + 1024;
+    total += ((size_t)Tl * B * 3 * nd * D + (size_t)Tout * B * nd * D) * sizeof(float) + 1024;
+    total += (size_t)2 * Tl * B * gemm_tc_kpad(l == 0 ? encoder_input_dim(m) : encoder_output_dim(m, l - 1)) * sizeof(float) + 1024;
     total += gemm_f16_stream_sync_ints(Tl * B) * sizeof(int) + 1024;   // scheduling area of a streamed projection
     Tl = Tout;
   }
@@ -365,10 +365,15 @@ int lvsr_profile_read(const char* kernel_class, double* total_ms, int64_t* count
   return 0;
 }
 
-int lvsr_model_create(const lvsr_config* cfg, lvsr_model** out) { return lvsr_model_create_bottom(cfg, nullptr, out); }
+int lvsr_model_create(const lvsr_config* cfg, lvsr_model** out) { return lvsr_model_create_encoder(cfg, nullptr, 1, out); }
 
 int lvsr_model_create_bottom(const lvsr_config* cfg, const lvsr_bottom_config* bottom, lvsr_model** out) {
+  return lvsr_model_create_encoder(cfg, bottom, 1, out);
+}
+
+int lvsr_model_create_encoder(const lvsr_config* cfg, const lvsr_bottom_config* bottom, int32_t bidir, lvsr_model** out) {
   LVSR_CHECK(cfg && out, "null argument");
+  LVSR_CHECK(bidir == 0 || bidir == 1, "bidir %d unsupported (1: bidirectional encoder, 0: forward-only encoder)", bidir);
   if (bottom) {
     LVSR_CHECK(bottom->num_layers >= 0 && bottom->num_layers <= LVSR_MAX_BOTTOM, "bottom MLP: %d layers (0 .. %d)",
                bottom->num_layers, (int)LVSR_MAX_BOTTOM);
@@ -408,6 +413,7 @@ int lvsr_model_create_bottom(const lvsr_config* cfg, const lvsr_bottom_config* b
   LVSR_CHECK(dev_count > 0, "no CUDA device: the GPU path has no CPU fallback");
   lvsr_model* m = new lvsr_model();
   m->cfg = *cfg;
+  m->ndir = bidir ? 2 : 1;
   if (bottom && bottom->num_layers > 0) m->bottom = *bottom;
   if (m->cfg.dec_stack == 0) m->cfg.dec_stack = 1;     // callers that predate the field zero-fill it
   if (content) {
@@ -423,7 +429,7 @@ int lvsr_model_create_bottom(const lvsr_config* cfg, const lvsr_bottom_config* b
     c.prior_before = c.prior_after = 0.0;
   }
   LVSR_CUDA_OK(cudaGetDevice(&m->device));
-  m->E = 2 * cfg->dims_bidir[cfg->num_layers - 1];
+  m->E = encoder_output_dim(m, cfg->num_layers - 1);
   build_param_table(m);
   int64_t total = 0;
   for (auto& p : m->params) {
@@ -722,7 +728,7 @@ int finalize_on_stream(lvsr_model* m, cudaStream_t st, bool synchronise) {
     }
   }
   for (int l = 0; l < c.num_layers; ++l)
-    for (int dir = 0; dir < 2; ++dir)
+    for (int dir = 0; dir < encoder_dirs(m); ++dir)
       if (int rc = fork_copy(m, encoder_fork(m, l, dir), m->Wcat[l], m->bcat[l], nullptr, st)) return rc;
   const int C = c.dim_dec, Cfb = c.dim_feedback, V = c.num_phonemes;
   const std::string g = GEN, t = TR;
@@ -863,7 +869,7 @@ int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int
     size_t need = 0;
     for (int l = 1, Tp = ceil_div(T, c.subsample[0]); l < c.num_layers; Tp = ceil_div(Tp, c.subsample[l]), ++l) {
       m->enc_claims_off[l] = need;
-      need += 3 * (size_t)ceil_div(Tp * B, 128) * (6 * c.dims_bidir[l] / 128);
+      need += 3 * (size_t)ceil_div(Tp * B, 128) * (encoder_fork(m, l, 0).ld / 128);
     }
     if (need > m->enc_claims_cap) {
       if (m->enc_claims) LVSR_CUDA_OK(cudaFree(m->enc_claims));
@@ -875,18 +881,19 @@ int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int
     LVSR_CUDA_OK(cudaMemsetAsync(m->enc_claims, 0, need * sizeof(int), st));
   }
   float* pre_done = nullptr;   // this layer's pre-activations, when they were projected beside the previous scan
+  const int nd = encoder_dirs(m);
   for (int l = 0; l < c.num_layers; ++l) {
-    const int D = c.dims_bidir[l], k = c.subsample[l];
+    const int D = c.dims_bidir[l], k = c.subsample[l], N = encoder_fork(m, l, 0).ld, Dout = encoder_output_dim(m, l);
     const int rows = Tl * B, Tout = ceil_div(Tl, k);
-    float* pre = pre_done ? pre_done : ws.f32((size_t)rows * 6 * D);
-    float* hext = tape ? ws.f32((size_t)(Tl + 2) * B * 2 * D) : nullptr;
+    float* pre = pre_done ? pre_done : ws.f32((size_t)rows * N);
+    float* hext = tape ? ws.f32((size_t)(Tl + 2) * B * Dout) : nullptr;
     LVSR_CHECK(pre && (hext || !tape), "out of device memory (encoder pre-activations)");
     int32_t* plan = m->enc_plan[l];
     if (!pre_done) {
       // finalize splits the fork weights only while the tensor-core GEMM is on (null entry: a shape it refuses)
       ArenaMark mark{ws};      // the split scratch is dead once the GEMM is enqueued (stream order)
       int kpad = 0, operands = 0;
-      if (int rc = projection_gemm(ws, cur, rows, din, m->Wcat[l], m->use_tc ? &m->Wcat_tc[l] : nullptr, 6 * D, m->bcat[l],
+      if (int rc = projection_gemm(ws, cur, rows, din, m->Wcat[l], m->use_tc ? &m->Wcat_tc[l] : nullptr, N, m->bcat[l],
                                    pre, st, &kpad, &operands))
         return rc;
       plan[LVSR_ENC_PROJ] = kpad ? LVSR_ENC_PATH_TC : LVSR_ENC_PATH_FFMA;
@@ -894,14 +901,16 @@ int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int
       plan[LVSR_ENC_OPERANDS] = operands;
     }
     pre_done = nullptr;
-    float* out = (l == c.num_layers - 1) ? attended : ws.f32((size_t)Tout * B * 2 * D);
+    float* out = (l == c.num_layers - 1) ? attended : ws.f32((size_t)Tout * B * Dout);
     LVSR_CHECK(out, "out of device memory (encoder layer output)");
     BiGruArgs a = {};
     a.pre = pre; a.mask = mask; a.mask_tstride = mstride;
-    const std::string bf = enc_base(l, 0) + "/gatedrecurrent", bb = enc_base(l, 1) + "/gatedrecurrent";
+    const std::string bf = enc_base(m, l, 0) + "/gatedrecurrent", bb = enc_base(m, l, 1) + "/gatedrecurrent";
     a.Wg_f = m->P(bf + ".state_to_gates"); a.Ws_f = m->P(bf + ".state_to_state"); a.h0_f = m->P(bf + ".initial_state");
-    a.Wg_b = m->P(bb + ".state_to_gates"); a.Ws_b = m->P(bb + ".state_to_state"); a.h0_b = m->P(bb + ".initial_state");
-    a.out = out; a.T = Tl; a.B = B; a.D = D; a.subsample = k;
+    if (nd == 2) {
+      a.Wg_b = m->P(bb + ".state_to_gates"); a.Ws_b = m->P(bb + ".state_to_state"); a.h0_b = m->P(bb + ".initial_state");
+    }
+    a.out = out; a.T = Tl; a.B = B; a.D = D; a.subsample = k; a.ndir = nd;
     if (tape) {
       a.tape = pre; a.hext = hext;
       tape[l] = {cur, pre, hext, Tl, din, D, k, mstride};
@@ -912,19 +921,19 @@ int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int
     BiGruPlan bp;
     if (int rc = bigru_plan(a, &bp)) return rc;
     const int scan_ctas = bp.clusters * bp.cs, free_sms = device_sm_count() - scan_ctas;
-    const int l1 = l + 1, D1 = l1 < c.num_layers ? c.dims_bidir[l1] : 0, rows1 = Tout * B;
+    const int l1 = l + 1, N1 = l1 < c.num_layers ? encoder_fork(m, l1, 0).ld : 0, rows1 = Tout * B;
     const bool overlap = overlap_on && l1 < c.num_layers && bp.kernel == LVSR_ENC_BIGRU_MMA && bp.waves == 1 &&
                          free_sms >= ENC_OVERLAP_MIN_SMS && scan_ctas <= gemm_f16_stream_max_scan_ctas() &&
-                         m->Wcat_tc[l1].head && gemm_f16_stream_supported(rows1, 6 * D1, 2 * D);
+                         m->Wcat_tc[l1].head && gemm_f16_stream_supported(rows1, N1, Dout);
     if (!overlap) {
       ProfScope prof("bigru", st);
       if (int rc = bigru_layer(a, st, &bp)) return rc;
     } else {
       // the same arena order as without the overlap (pre-activations of l + 1 right after this layer's output), the
       // split planes as projection_gemm takes them, then the scheduling area; all but the pre-activations dead after
-      float* pre1 = ws.f32((size_t)rows1 * 6 * D1);
+      float* pre1 = ws.f32((size_t)rows1 * N1);
       ArenaMark mark{ws};
-      const int K1 = 2 * D;
+      const int K1 = Dout;
       float* a_hi = ws.f32((size_t)rows1 * K1);
       float* a_lo = ws.f32((size_t)rows1 * K1);
       int* sync = reinterpret_cast<int*>(ws.f32(gemm_f16_stream_sync_ints(rows1)));
@@ -933,7 +942,7 @@ int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int
       a.progress = gemm_f16_stream_progress(sync);
       __half* a_head = reinterpret_cast<__half*>(a_hi);
       const TcWeights& tw = m->Wcat_tc[l1];
-      ProjStream ps = {sync, a.progress, scan_ctas, bp.cs, Tl, k, B, spin_limit, m->enc_tiles + 2 * l1,
+      ProjStream ps = {sync, a.progress, scan_ctas, bp.cs, nd, Tl, k, B, spin_limit, m->enc_tiles + 2 * l1,
                        m->enc_claims + m->enc_claims_off[l1]};
       {
         // no event between the two launches: the projection must directly follow the scan in the stream.  The
@@ -941,7 +950,7 @@ int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int
         ProfScope prof("bigru", st);
         if (int rc = bigru_layer(a, st, &bp)) return rc;
         if (int rc = gemm_f16_stream(out, a_head, a_head + (size_t)rows1 * K1, reinterpret_cast<int*>(a_lo), rows1, K1,
-                                     tw.head, tw.tail, tw.ew, 6 * D1, m->bcat[l1], pre1, 6 * D1, ps, free_sms, st))
+                                     tw.head, tw.tail, tw.ew, N1, m->bcat[l1], pre1, N1, ps, free_sms, st))
           return rc;
       }
       {
@@ -949,7 +958,7 @@ int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int
         ps.progress = nullptr;
         ps.tiles_done = m->enc_tiles + 2 * l1 + 1;
         if (int rc = gemm_f16_stream(out, a_head, a_head + (size_t)rows1 * K1, reinterpret_cast<int*>(a_lo), rows1, K1,
-                                     tw.head, tw.tail, tw.ew, 6 * D1, m->bcat[l1], pre1, 6 * D1, ps, device_sm_count(), st))
+                                     tw.head, tw.tail, tw.ew, N1, m->bcat[l1], pre1, N1, ps, device_sm_count(), st))
           return rc;
       }
       int32_t* plan1 = m->enc_plan[l1];
@@ -967,7 +976,7 @@ int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int
     plan[LVSR_ENC_RESIDENT] = bp.resident;
     plan[LVSR_ENC_WAVES] = bp.waves;
     plan[LVSR_ENC_T] = Tl;
-    cur = out; Tl = Tout; din = 2 * D; mstride *= k; kcum *= k;
+    cur = out; Tl = Tout; din = Dout; mstride *= k; kcum *= k;
   }
   if (mask) {
     if (int rc = gather_time_subsample(attended_mask, mask, Tl, kcum, B, st)) return rc;

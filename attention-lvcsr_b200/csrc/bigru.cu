@@ -112,8 +112,10 @@ __host__ __device__ constexpr int ffma_qreg() { return D <= 128 || D == 256 ? D 
 // allows it (up to D = 192; the shared-memory weights of wider layers leave room for one CTA per SM).  At D = 64, 128
 // and 256 a lane's gate slice (4 * D/16 floats) stays in registers; at the other widths the first float4 group of its
 // k range does and the rest sits in shared memory beside the state_to_state slice (see ffma_qreg).
+// NDIR: directions of the layer.  2: cluster c runs direction c & 1 on rows (c >> 1) * RB; 1 (net.bidir False): every
+// cluster runs the forward direction, on rows c * RB, and the pre-activations, outputs and hext hold one direction.
 // TAPE: training forward (stores c / z / r over the pre-activations and every frame of h); compiled out for inference
-template <int D, int CS, int NWARP, bool TAPE>
+template <int D, int CS, int NDIR, int NWARP, bool TAPE>
 __global__ void __launch_bounds__(NWARP * 32, 2)
 bigru_kernel(BiGruArgs a) {
   constexpr int UC = D / CS;          // units owned by this CTA
@@ -129,6 +131,7 @@ bigru_kernel(BiGruArgs a) {
   static_assert(NC2 % CG == 0 && CPL2 == 2 && CPL1 == 4, "lane roles below assume 4 gate / 2 candidate columns per lane");
   static_assert(KPG <= 32, "a lane's k range sits inside one chunk of h");
   static_assert(CS <= 16, "sender lanes reach at most 16 peers");
+  static_assert(NDIR == 1 || NDIR == 2, "one or two directions");
   constexpr int QREG = ffma_qreg<D>();   // float4 groups of the gate slice held in registers, the rest in shared memory
   constexpr int N1 = RB * CPL1, N2 = RB * CPL2;        // per-lane partial sums of the two phases
   constexpr uint32_t FULL_BYTES = RB * D * sizeof(float);
@@ -156,8 +159,8 @@ bigru_kernel(BiGruArgs a) {
   const int cluster_id = blockIdx.x / CS;
   unsigned rank;
   asm volatile("mov.u32 %0, %%cluster_ctarank;\n" : "=r"(rank));
-  const int dir = cluster_id & 1;             // 0 forward, 1 backward
-  const int row0 = (cluster_id >> 1) * RB;    // first batch row of this cluster
+  const int dir = NDIR == 2 ? cluster_id & 1 : 0;                          // 0 forward, 1 backward
+  const int row0 = (NDIR == 2 ? cluster_id >> 1 : cluster_id) * RB;       // first batch row of this cluster
   const int ul_warp = warp * NC2;             // first owned unit of this warp, local index
   const int u_warp = rank * UC + ul_warp;     // ... global unit index
   const int kpeer = (kg * KPG) / CH, koff = (kg * KPG) % CH;   // chunk and offset of this lane's k range
@@ -242,12 +245,12 @@ bigru_kernel(BiGruArgs a) {
     for (int i = tid; i < RB * UC; i += NWARP * 32) {
       const int r = i / UC, u = rank * UC + i % UC;
       if (row0 + r < a.B)
-        a.hext[((long long)(dir ? a.T + 1 : 0) * a.B + row0 + r) * (2 * D) + dir * D + u] = h0[u];
+        a.hext[((long long)(dir ? a.T + 1 : 0) * a.B + row0 + r) * (NDIR * D) + dir * D + u] = h0[u];
     }
   }
 
   const int T = a.T, B = a.B;
-  const long long pre_ld = 6LL * D;                       // [A | Gz | Gr] per direction
+  const long long pre_ld = 3LL * NDIR * D;                // [A | Gz | Gr] per direction
   const float* pre_dir = a.pre + (long long)dir * 3 * D;
   const int dt = dir ? -1 : 1;
   int t = dir ? (T - 1) : 0;
@@ -406,10 +409,10 @@ bigru_kernel(BiGruArgs a) {
       if constexpr (CS > 8)
         if (sender2) st_async_v4(dst_h2, x, y, z, w, rbar_h2);
       if (sub_phase == 0 && peer == 0 && row0 + rowg < B)
-        *reinterpret_cast<float4*>(a.out + ((long long)t_out * B + row0 + rowg) * (2 * D) + dir * D + u_warp) =
+        *reinterpret_cast<float4*>(a.out + ((long long)t_out * B + row0 + rowg) * (NDIR * D) + dir * D + u_warp) =
             make_float4(x, y, z, w);
       if (TAPE && peer == 0 && row0 + rowg < B)
-        *reinterpret_cast<float4*>(a.hext + ((long long)(t + 1) * B + row0 + rowg) * (2 * D) + dir * D + u_warp) =
+        *reinterpret_cast<float4*>(a.hext + ((long long)(t + 1) * B + row0 + rowg) * (NDIR * D) + dir * D + u_warp) =
             make_float4(x, y, z, w);
     }
     BG_STAMP(5);
@@ -440,28 +443,28 @@ constexpr size_t ffma_smem_bytes() {
 }
 
 // once per device: the dynamic shared memory, and clusters above 8 CTAs (D > 256) are non-portable
-template <int D, int CS, int NWARP, bool TAPE>
+template <int D, int CS, int NDIR, int NWARP, bool TAPE>
 int ffma_configure() {
   static bool configured[LVSR_MAX_DEVICES] = {false};
   const int dev = current_device();
   if (!configured[dev]) {
-    LVSR_CUDA_OK(cudaFuncSetAttribute(bigru_kernel<D, CS, NWARP, TAPE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    LVSR_CUDA_OK(cudaFuncSetAttribute(bigru_kernel<D, CS, NDIR, NWARP, TAPE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                       (int)ffma_smem_bytes<D, NWARP>()));
     if (CS > 8)
-      LVSR_CUDA_OK(cudaFuncSetAttribute(bigru_kernel<D, CS, NWARP, TAPE>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+      LVSR_CUDA_OK(cudaFuncSetAttribute(bigru_kernel<D, CS, NDIR, NWARP, TAPE>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
     configured[dev] = true;
   }
   return 0;
 }
 
 // how many clusters of the FFMA kernel the device holds at once (0: none, the launch is refused)
-template <int D, int CS, int NWARP, bool TAPE>
+template <int D, int CS, int NDIR, int NWARP, bool TAPE>
 int ffma_clusters_resident() {
   static int per_dev[LVSR_MAX_DEVICES];
   static bool known[LVSR_MAX_DEVICES] = {false};
   const int dev = current_device();
   if (!known[dev]) {
-    if (ffma_configure<D, CS, NWARP, TAPE>()) return 0;
+    if (ffma_configure<D, CS, NDIR, NWARP, TAPE>()) return 0;
     known[dev] = true;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(CS * 64);
@@ -475,7 +478,7 @@ int ffma_clusters_resident() {
     cfg.attrs = attr;
     cfg.numAttrs = 1;
     int k = 0;
-    if (cudaOccupancyMaxActiveClusters(&k, bigru_kernel<D, CS, NWARP, TAPE>, &cfg) != cudaSuccess) {
+    if (cudaOccupancyMaxActiveClusters(&k, bigru_kernel<D, CS, NDIR, NWARP, TAPE>, &cfg) != cudaSuccess) {
       cudaGetLastError();
       k = 0;
     }
@@ -484,17 +487,17 @@ int ffma_clusters_resident() {
   return per_dev[dev];
 }
 
-template <int D, int CS, int NWARP, bool TAPE>
+template <int D, int CS, int NDIR, int NWARP, bool TAPE>
 int launch_bigru_t(const BiGruArgs& a, cudaStream_t stream, BiGruPlan* plan) {
   constexpr size_t W2S_BYTES = ffma_smem_bytes<D, NWARP>();
-  if (int rc = ffma_configure<D, CS, NWARP, TAPE>()) return rc;
-  const int resident = ffma_clusters_resident<D, CS, NWARP, TAPE>();
+  if (int rc = ffma_configure<D, CS, NDIR, NWARP, TAPE>()) return rc;
+  const int resident = ffma_clusters_resident<D, CS, NDIR, NWARP, TAPE>();
   if (resident <= 0)
     return set_error("bigru: this device holds no cluster of %d CTAs of the hidden-size-%d scan (%zu bytes of shared memory "
                      "each)", CS, D, W2S_BYTES);
   const int groups = ceil_div(a.B, RB);
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(CS * groups * 2);
+  cfg.gridDim = dim3(CS * groups * NDIR);
   cfg.blockDim = dim3(NWARP * 32);
   cfg.dynamicSmemBytes = W2S_BYTES;
   cfg.stream = stream;
@@ -510,9 +513,9 @@ int launch_bigru_t(const BiGruArgs& a, cudaStream_t stream, BiGruPlan* plan) {
     const int on = 1;
     LVSR_CUDA_OK(cudaMemcpyToSymbolAsync(g_bigru_trace_on, &on, sizeof(on), 0, cudaMemcpyHostToDevice, stream));
   }
-  LVSR_CUDA_OK(cudaLaunchKernelEx(&cfg, bigru_kernel<D, CS, NWARP, TAPE>, a));
+  LVSR_CUDA_OK(cudaLaunchKernelEx(&cfg, bigru_kernel<D, CS, NDIR, NWARP, TAPE>, a));
   g_launch_count++;
-  if (plan) *plan = {LVSR_ENC_BIGRU_FFMA, RB, CS, 2 * groups, resident, ceil_div(2 * groups, resident)};
+  if (plan) *plan = {LVSR_ENC_BIGRU_FFMA, RB, CS, NDIR * groups, resident, ceil_div(NDIR * groups, resident)};
   if (trace) {
     unsigned long long h[8] = {0};
     LVSR_CUDA_OK(cudaMemcpyFromSymbolAsync(h, g_bigru_trace, sizeof(h), 0, cudaMemcpyDeviceToHost, stream));
@@ -615,7 +618,8 @@ __device__ __forceinline__ float range_scale(float warp_max_abs, float& inverse)
   return scale;
 }
 
-template <int D, bool TAPE, int RB>
+// NDIR as for bigru_kernel: 1 runs the forward direction in every cluster
+template <int D, int NDIR, bool TAPE, int RB>
 __global__ void __launch_bounds__(MMA_THREADS, 1)
 bigru_mma_kernel(BiGruArgs a) {
   constexpr int CS = MMA_CS;
@@ -654,8 +658,8 @@ bigru_mma_kernel(BiGruArgs a) {
   const int cluster_id = blockIdx.x / CS;
   unsigned rank;
   asm volatile("mov.u32 %0, %%cluster_ctarank;\n" : "=r"(rank));
-  const int dir = cluster_id & 1;
-  const int row0 = (cluster_id >> 1) * RB;
+  const int dir = NDIR == 2 ? cluster_id & 1 : 0;
+  const int row0 = (NDIR == 2 ? cluster_id >> 1 : cluster_id) * RB;
   const float* h0 = dir ? a.h0_b : a.h0_f;
   const uint32_t bar_h = smem_u32(&mbar[0]), bar_hr = smem_u32(&mbar[1]);
   const int T = a.T, B = a.B;
@@ -895,10 +899,10 @@ bigru_mma_kernel(BiGruArgs a) {
     for (int i = 0; i < 4; ++i) h_own[i] = h0[u_glob + i];
     if constexpr (TAPE) {
       if (writer)
-        *reinterpret_cast<float4*>(a.hext + ((long long)(dir ? T + 1 : 0) * B + row0 + erow) * (2 * D) + dir * D + u_glob) =
+        *reinterpret_cast<float4*>(a.hext + ((long long)(dir ? T + 1 : 0) * B + row0 + erow) * (NDIR * D) + dir * D + u_glob) =
             make_float4(h_own[0], h_own[1], h_own[2], h_own[3]);
     }
-    const long long pre_ld = 6LL * D;
+    const long long pre_ld = 3LL * NDIR * D;
     const int dt = dir ? -1 : 1;
     int t = dir ? (T - 1) : 0;
     // fork pre-activations of this thread's 4 units: [inputs | update | reset]; every slot is re-loaded for the next step
@@ -1006,10 +1010,10 @@ bigru_mma_kernel(BiGruArgs a) {
         if (writer) {
           const float4 hv = make_float4(h_own[0], h_own[1], h_own[2], h_own[3]);
           if (sub_phase == 0)
-            *reinterpret_cast<float4*>(a.out + ((long long)t_out * B + row0 + erow) * (2 * D) + dir * D + u_glob) = hv;
+            *reinterpret_cast<float4*>(a.out + ((long long)t_out * B + row0 + erow) * (NDIR * D) + dir * D + u_glob) = hv;
           if constexpr (TAPE) {
             *reinterpret_cast<float4*>(tape_ptr) = make_float4(sc[0], sc[1], sc[2], sc[3]);
-            *reinterpret_cast<float4*>(a.hext + ((long long)(t + 1) * B + row0 + erow) * (2 * D) + dir * D + u_glob) = hv;
+            *reinterpret_cast<float4*>(a.hext + ((long long)(t + 1) * B + row0 + erow) * (NDIR * D) + dir * D + u_glob) = hv;
           }
         }
         pre_ptr += pre_step;
@@ -1053,7 +1057,9 @@ bigru_mma_kernel(BiGruArgs a) {
 template <int D, int CS, int NWARP>
 int launch_bigru(const BiGruArgs& a, cudaStream_t stream, BiGruPlan* plan) {
   LVSR_CHECK((a.tape == nullptr) == (a.hext == nullptr), "bigru: tape and hext go together");
-  return a.tape ? launch_bigru_t<D, CS, NWARP, true>(a, stream, plan) : launch_bigru_t<D, CS, NWARP, false>(a, stream, plan);
+  if (a.ndir == 1)
+    return a.tape ? launch_bigru_t<D, CS, 1, NWARP, true>(a, stream, plan) : launch_bigru_t<D, CS, 1, NWARP, false>(a, stream, plan);
+  return a.tape ? launch_bigru_t<D, CS, 2, NWARP, true>(a, stream, plan) : launch_bigru_t<D, CS, 2, NWARP, false>(a, stream, plan);
 }
 
 template <int D, bool TAPE>
@@ -1073,7 +1079,7 @@ int mma_launch_config(cudaLaunchConfig_t& cfg, cudaLaunchAttribute* attr, int cl
 }
 
 // how many clusters of the tensor-core kernel the device holds at once (one CTA per SM, 4 SMs of one GPC per cluster)
-template <int D, int RB>
+template <int D, int NDIR, int RB>
 int mma_clusters_resident() {
   static int per_dev[LVSR_MAX_DEVICES];
   static bool known[LVSR_MAX_DEVICES] = {false};
@@ -1084,7 +1090,7 @@ int mma_clusters_resident() {
     cudaLaunchAttribute attr[1];
     int k = 0;
     if (mma_launch_config<D, false>(cfg, attr, 64, nullptr) != 0 ||
-        cudaOccupancyMaxActiveClusters(&k, bigru_mma_kernel<D, false, RB>, &cfg) != cudaSuccess) {
+        cudaOccupancyMaxActiveClusters(&k, bigru_mma_kernel<D, NDIR, false, RB>, &cfg) != cudaSuccess) {
       cudaGetLastError();
       k = 0;
     }
@@ -1095,24 +1101,24 @@ int mma_clusters_resident() {
 
 // waves of a launch of B rows: clusters never talk to each other, so a launch with more clusters than the device holds
 // at once runs them in turns, and every wave costs a whole sequence of steps (0: the kernel cannot be resident at all)
-template <int D, int RB>
+template <int D, int NDIR, int RB>
 int mma_waves(int B) {
-  const int resident = mma_clusters_resident<D, RB>();
-  return resident > 0 ? ceil_div(2 * ceil_div(B, RB), resident) : 0;
+  const int resident = mma_clusters_resident<D, NDIR, RB>();
+  return resident > 0 ? ceil_div(NDIR * ceil_div(B, RB), resident) : 0;
 }
 
-template <int D, bool TAPE, int RB>
+template <int D, int NDIR, bool TAPE, int RB>
 int launch_bigru_mma_t(const BiGruArgs& a, cudaStream_t stream) {
   cudaLaunchConfig_t cfg;
   cudaLaunchAttribute attr[1];
-  const int clusters = ceil_div(a.B, RB) * 2;
+  const int clusters = ceil_div(a.B, RB) * NDIR;
   if (int rc = mma_launch_config<D, TAPE>(cfg, attr, clusters, stream)) return rc;
   static const bool trace = getenv("LVSR_BIGRU_TRACE") != nullptr;
   if (trace) {
     const int on = 1;
     LVSR_CUDA_OK(cudaMemcpyToSymbolAsync(g_bigru_trace_on, &on, sizeof(on), 0, cudaMemcpyHostToDevice, stream));
   }
-  LVSR_CUDA_OK(cudaLaunchKernelEx(&cfg, bigru_mma_kernel<D, TAPE, RB>, a));
+  LVSR_CUDA_OK(cudaLaunchKernelEx(&cfg, bigru_mma_kernel<D, NDIR, TAPE, RB>, a));
   g_launch_count++;
   if (trace) {
     unsigned long long h[12] = {0};
@@ -1120,7 +1126,7 @@ int launch_bigru_mma_t(const BiGruArgs& a, cudaStream_t stream) {
     LVSR_CUDA_OK(cudaStreamSynchronize(stream));
     const double n = h[8] ? (double)h[8] : 1.0;
     fprintf(stderr, "[bigru trace] mma<%d> RB=%d B=%d clusters=%d resident=%d waves=%d\n", D, RB, a.B, clusters,
-            mma_clusters_resident<D, RB>(), mma_waves<D, RB>(a.B));
+            mma_clusters_resident<D, NDIR, RB>(), mma_waves<D, NDIR, RB>(a.B));
     fprintf(stderr,
             "[bigru trace] mma<%d> T=%llu cycles/step  MMA warp: wait_h=%.0f gates=%.0f wait_hr=%.0f cand=%.0f | elementwise: "
             "wait_gates=%.0f r+send(+z)=%.0f wait_cand=%.0f cand+send+stores=%.0f\n",
@@ -1144,12 +1150,34 @@ int launch_bigru_mma_t(const BiGruArgs& a, cudaStream_t stream) {
   return 0;
 }
 
-template <int D, int RB>
+template <int D, int NDIR, int RB>
 int launch_bigru_mma(const BiGruArgs& a, cudaStream_t stream, BiGruPlan* plan) {
   LVSR_CHECK((a.tape == nullptr) == (a.hext == nullptr), "bigru: tape and hext go together");
-  if (int rc = a.tape ? launch_bigru_mma_t<D, true, RB>(a, stream) : launch_bigru_mma_t<D, false, RB>(a, stream)) return rc;
+  if (int rc = a.tape ? launch_bigru_mma_t<D, NDIR, true, RB>(a, stream) : launch_bigru_mma_t<D, NDIR, false, RB>(a, stream))
+    return rc;
   if (plan)
-    *plan = {LVSR_ENC_BIGRU_MMA, RB, MMA_CS, ceil_div(a.B, RB) * 2, mma_clusters_resident<D, RB>(), mma_waves<D, RB>(a.B)};
+    *plan = {LVSR_ENC_BIGRU_MMA, RB, MMA_CS, ceil_div(a.B, RB) * NDIR, mma_clusters_resident<D, NDIR, RB>(),
+             mma_waves<D, NDIR, RB>(a.B)};
+  return 0;
+}
+
+// the tensor-core plan of a batch of B rows with NDIR directions: RB 4, or 8 where that saves a wave (see bigru_plan)
+template <int NDIR>
+int mma_plan(int B, BiGruPlan* plan) {
+  // 8-row clusters cost a third MMA per k-step and twice the elementwise work of a step, but halve the clusters:
+  // worth it only where that saves a wave
+  int rb = 4;
+  const int w8 = mma_waves<256, NDIR, 8>(B);
+  if (w8 > 0 && w8 < mma_waves<256, NDIR, 4>(B)) rb = 8;
+  if (const char* e = getenv("LVSR_BIGRU_RB")) {
+    rb = atoi(e);
+    if (rb != 4 && rb != 8) return set_error("bigru: LVSR_BIGRU_RB=%s (expected 4 or 8)", e);
+  }
+  const int clusters = ceil_div(B, rb) * NDIR;
+  *plan = rb == 8 ? BiGruPlan{LVSR_ENC_BIGRU_MMA, 8, MMA_CS, clusters, mma_clusters_resident<256, NDIR, 8>(),
+                              mma_waves<256, NDIR, 8>(B)}
+                  : BiGruPlan{LVSR_ENC_BIGRU_MMA, 4, MMA_CS, clusters, mma_clusters_resident<256, NDIR, 4>(),
+                              mma_waves<256, NDIR, 4>(B)};
   return 0;
 }
 
@@ -1160,29 +1188,16 @@ bool bigru_supported(int D) { return D >= 64 && D <= 512 && D % 64 == 0; }
 int bigru_plan(const BiGruArgs& a, BiGruPlan* plan) {
   *plan = {};
   if (a.T <= 0 || a.B <= 0) return 0;
+  LVSR_CHECK(a.ndir == 1 || a.ndir == 2, "bigru: %d directions (1 or 2)", a.ndir);
   // hidden size 256: tensor-core products.  Clusters never talk to each other, so a batch with more clusters than the
   // device holds at once (mma_clusters_resident, from the occupancy query) simply runs in waves -- still
   // ahead of the FFMA kernels, which would have to put two or more CTAs on every SM for such a batch.
-  bool mma = a.D == 256 && mma_clusters_resident<256, 4>() > 0;
+  bool mma = a.D == 256 && (a.ndir == 1 ? mma_clusters_resident<256, 1, 4>() : mma_clusters_resident<256, 2, 4>()) > 0;
   if (const char* e = getenv("LVSR_BIGRU_MMA")) mma = a.D == 256 && atoi(e) != 0;
-  if (mma) {
-    // 8-row clusters cost a third MMA per k-step and twice the elementwise work of a step, but halve the clusters:
-    // worth it only where that saves a wave
-    int rb = 4;
-    const int w8 = mma_waves<256, 8>(a.B);
-    if (w8 > 0 && w8 < mma_waves<256, 4>(a.B)) rb = 8;
-    if (const char* e = getenv("LVSR_BIGRU_RB")) {
-      rb = atoi(e);
-      if (rb != 4 && rb != 8) return set_error("bigru: LVSR_BIGRU_RB=%s (expected 4 or 8)", e);
-    }
-    const int clusters = ceil_div(a.B, rb) * 2;
-    *plan = rb == 8 ? BiGruPlan{LVSR_ENC_BIGRU_MMA, 8, MMA_CS, clusters, mma_clusters_resident<256, 8>(), mma_waves<256, 8>(a.B)}
-                    : BiGruPlan{LVSR_ENC_BIGRU_MMA, 4, MMA_CS, clusters, mma_clusters_resident<256, 4>(), mma_waves<256, 4>(a.B)};
-    return 0;
-  }
+  if (mma) return a.ndir == 1 ? mma_plan<1>(a.B, plan) : mma_plan<2>(a.B, plan);
   LVSR_CHECK(bigru_supported(a.D), "bigru: unsupported hidden size %d (supported: multiples of 64 from 64 to 512)", a.D);
   // the FFMA kernel's occupancy (resident, waves) is queried when it is launched
-  *plan = {LVSR_ENC_BIGRU_FFMA, RB, a.D / 32, 2 * ceil_div(a.B, RB), 0, 0};
+  *plan = {LVSR_ENC_BIGRU_FFMA, RB, a.D / 32, a.ndir * ceil_div(a.B, RB), 0, 0};
   return 0;
 }
 
@@ -1192,8 +1207,10 @@ int bigru_layer(const BiGruArgs& a, cudaStream_t stream, BiGruPlan* plan) {
   if (plan) *plan = {};
   if (int rc = bigru_plan(a, &pl)) return rc;
   if (a.T <= 0 || a.B <= 0) return 0;
-  if (pl.kernel == LVSR_ENC_BIGRU_MMA)
-    return pl.rb == 8 ? launch_bigru_mma<256, 8>(a, stream, plan) : launch_bigru_mma<256, 4>(a, stream, plan);
+  if (pl.kernel == LVSR_ENC_BIGRU_MMA) {
+    if (a.ndir == 1) return pl.rb == 8 ? launch_bigru_mma<256, 1, 8>(a, stream, plan) : launch_bigru_mma<256, 1, 4>(a, stream, plan);
+    return pl.rb == 8 ? launch_bigru_mma<256, 2, 8>(a, stream, plan) : launch_bigru_mma<256, 2, 4>(a, stream, plan);
+  }
   switch (a.D) {
     case 64: return launch_bigru<64, 2, 8>(a, stream, plan);
     case 128: return launch_bigru<128, 4, 8>(a, stream, plan);

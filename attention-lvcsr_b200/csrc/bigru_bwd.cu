@@ -21,7 +21,8 @@
 // slice in shared memory (k-major, padded so the 8 k-groups of a warp hit distinct banks);
 // thread = (k-group 0..7, unit), 4 rows per thread, cross-k reduction by shuffles.
 // Every D = 64, 128, ..., 512 runs, with CS = D / 32 (clusters above 8 CTAs are non-portable); from D = 384 on the
-// shared memory leaves room for one CTA per SM.
+// shared memory leaves room for one CTA per SM.  NDIR = 1 is the layer of a forward-only encoder (net.bidir False):
+// every cluster runs the forward direction and the tape, hext, dout and hr_out hold one direction.
 #include "kernels.h"
 
 namespace lvsr {
@@ -78,9 +79,10 @@ __host__ __device__ constexpr size_t bwd_smem_bytes(int D) {
 // the wide layers, which hold one CTA per SM anyway, get the registers that keep them from spilling
 __host__ __device__ constexpr int bwd_min_blocks(int D) { return 2 * (bwd_smem_bytes(D) + 1024) <= 228 * 1024 ? 2 : 1; }
 
-template <int D, int CS>
+template <int D, int CS, int NDIR>
 __global__ void __launch_bounds__(NT, bwd_min_blocks(D)) bigru_bwd_kernel(BiGruBwdArgs a) {
   static_assert(D == CS * UC, "32 units per CTA");
+  static_assert(NDIR == 1 || NDIR == 2, "one or two directions");
   constexpr int KA = D / 8;         // k values per thread, first product  (K = D)
   constexpr int KB = 2 * D / 8;     // second product (K = 2D)
   extern __shared__ __align__(16) float smem[];
@@ -96,8 +98,8 @@ __global__ void __launch_bounds__(NT, bwd_min_blocks(D)) bigru_bwd_kernel(BiGruB
   const int cluster_id = blockIdx.x / CS;
   unsigned rank;
   asm volatile("mov.u32 %0, %%cluster_ctarank;\n" : "=r"(rank));
-  const int dir = cluster_id & 1;
-  const int row0 = (cluster_id >> 1) * RB;
+  const int dir = NDIR == 2 ? cluster_id & 1 : 0;
+  const int row0 = (NDIR == 2 ? cluster_id >> 1 : cluster_id) * RB;
   const int u0 = rank * UC;
   const float* Wg = dir ? a.Wg_b : a.Wg_f;
   const float* Ws = dir ? a.Ws_b : a.Ws_f;
@@ -122,7 +124,7 @@ __global__ void __launch_bounds__(NT, bwd_min_blocks(D)) bigru_bwd_kernel(BiGruB
 
   // ---- element-wise owner: warp 0, lane = owned unit, all RB rows in registers ---------------
   const int ju = u0 + lane;                                 // global unit of this lane (warp 0)
-  const long long pre_ld = 6LL * D;
+  const long long pre_ld = 3LL * NDIR * D;
   const int dt = dir ? 1 : -1;                              // backward in the scan's own order
   int t = dir ? 0 : T - 1;
   float dh[RB] = {0.f, 0.f, 0.f, 0.f};
@@ -137,10 +139,10 @@ __global__ void __launch_bounds__(NT, bwd_min_blocks(D)) bigru_bwd_kernel(BiGruB
         const float* tp = a.tape + ((long long)tt * B + row) * pre_ld + (long long)dir * 3 * D;
         nc[r] = __ldg(tp + ju); nz[r] = __ldg(tp + D + ju); nr[r] = __ldg(tp + 2 * D + ju);
         // h_prev: forward direction = state after time tt-1 (slot tt), backward = after tt+1 (slot tt+2)
-        nh[r] = __ldg(a.hext + ((long long)(dir ? tt + 2 : tt) * B + row) * (2 * D) + dir * D + ju);
+        nh[r] = __ldg(a.hext + ((long long)(dir ? tt + 2 : tt) * B + row) * (NDIR * D) + dir * D + ju);
         if (a.mask) nm[r] = __ldg(a.mask + (long long)tt * a.mask_tstride + row);
         if (tt % a.subsample == 0)
-          ng[r] = __ldg(a.dout + ((long long)(tt / a.subsample) * B + row) * (2 * D) + dir * D + ju);
+          ng[r] = __ldg(a.dout + ((long long)(tt / a.subsample) * B + row) * (NDIR * D) + dir * D + ju);
       }
     }
   };
@@ -242,7 +244,7 @@ __global__ void __launch_bounds__(NT, bwd_min_blocks(D)) bigru_bwd_kernel(BiGruB
           float* tp = a.tape + ((long long)t * B + row0 + q) * pre_ld + (long long)dir * 3 * D;
           tp[D + ju] = daz[q];
           tp[2 * D + ju] = dar[q];
-          a.hr_out[((long long)t * B + row0 + q) * (2 * D) + dir * D + ju] = hr[q];
+          a.hr_out[((long long)t * B + row0 + q) * (NDIR * D) + dir * D + ju] = hr[q];
         }
       }
     }
@@ -279,7 +281,7 @@ __global__ void __launch_bounds__(NT, bwd_min_blocks(D)) bigru_bwd_kernel(BiGruB
   cluster_sync_all();   // no CTA exits while a peer may still address its shared memory
 }
 
-template <int D, int CS>
+template <int D, int CS, int NDIR>
 int launch_bwd(const BiGruBwdArgs& a, cudaStream_t stream) {
   constexpr size_t SMEM = bwd_smem_bytes(D);
   static bool configured[LVSR_MAX_DEVICES] = {false};
@@ -288,12 +290,12 @@ int launch_bwd(const BiGruBwdArgs& a, cudaStream_t stream) {
   const int groups = ceil_div(a.B, RB);
   cudaLaunchConfig_t cfg = {};
   if (!configured[dev]) {
-    LVSR_CUDA_OK(cudaFuncSetAttribute(bigru_bwd_kernel<D, CS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM));
-    if (CS > 8) LVSR_CUDA_OK(cudaFuncSetAttribute(bigru_bwd_kernel<D, CS>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    LVSR_CUDA_OK(cudaFuncSetAttribute(bigru_bwd_kernel<D, CS, NDIR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM));
+    if (CS > 8) LVSR_CUDA_OK(cudaFuncSetAttribute(bigru_bwd_kernel<D, CS, NDIR>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
     configured[dev] = true;
     resident[dev] = -1;
   }
-  cfg.gridDim = dim3(CS * groups * 2);
+  cfg.gridDim = dim3(CS * groups * NDIR);
   cfg.blockDim = dim3(NT);
   cfg.dynamicSmemBytes = SMEM;
   cfg.stream = stream;
@@ -306,7 +308,7 @@ int launch_bwd(const BiGruBwdArgs& a, cudaStream_t stream) {
   cfg.numAttrs = 1;
   if (resident[dev] < 0) {
     int k = 0;
-    if (cudaOccupancyMaxActiveClusters(&k, bigru_bwd_kernel<D, CS>, &cfg) != cudaSuccess) {
+    if (cudaOccupancyMaxActiveClusters(&k, bigru_bwd_kernel<D, CS, NDIR>, &cfg) != cudaSuccess) {
       cudaGetLastError();
       k = 0;
     }
@@ -315,9 +317,25 @@ int launch_bwd(const BiGruBwdArgs& a, cudaStream_t stream) {
   if (resident[dev] <= 0)
     return set_error("bigru backward: this device holds no cluster of %d CTAs of the hidden-size-%d scan (%zu bytes of "
                      "shared memory each)", CS, D, SMEM);
-  LVSR_CUDA_OK(cudaLaunchKernelEx(&cfg, bigru_bwd_kernel<D, CS>, a));
+  LVSR_CUDA_OK(cudaLaunchKernelEx(&cfg, bigru_bwd_kernel<D, CS, NDIR>, a));
   g_launch_count++;
   return 0;
+}
+
+template <int NDIR>
+int launch_bwd_width(const BiGruBwdArgs& a, cudaStream_t stream) {
+  switch (a.D) {
+    case 64: return launch_bwd<64, 2, NDIR>(a, stream);
+    case 128: return launch_bwd<128, 4, NDIR>(a, stream);
+    case 192: return launch_bwd<192, 6, NDIR>(a, stream);
+    case 256: return launch_bwd<256, 8, NDIR>(a, stream);
+    case 320: return launch_bwd<320, 10, NDIR>(a, stream);
+    case 384: return launch_bwd<384, 12, NDIR>(a, stream);
+    case 448: return launch_bwd<448, 14, NDIR>(a, stream);
+    case 512: return launch_bwd<512, 16, NDIR>(a, stream);
+    default:
+      return set_error("bigru backward: unsupported hidden size %d (supported: multiples of 64 from 64 to 512)", a.D);
+  }
 }
 
 }  // namespace
@@ -326,19 +344,8 @@ int bigru_layer_backward(const BiGruBwdArgs& a, cudaStream_t stream, int* cs_out
   ProfScope prof("bigru_bwd", stream);
   if (cs_out) *cs_out = 0;
   if (a.T <= 0 || a.B <= 0) return 0;
-  int rc;
-  switch (a.D) {
-    case 64: rc = launch_bwd<64, 2>(a, stream); break;
-    case 128: rc = launch_bwd<128, 4>(a, stream); break;
-    case 192: rc = launch_bwd<192, 6>(a, stream); break;
-    case 256: rc = launch_bwd<256, 8>(a, stream); break;
-    case 320: rc = launch_bwd<320, 10>(a, stream); break;
-    case 384: rc = launch_bwd<384, 12>(a, stream); break;
-    case 448: rc = launch_bwd<448, 14>(a, stream); break;
-    case 512: rc = launch_bwd<512, 16>(a, stream); break;
-    default:
-      return set_error("bigru backward: unsupported hidden size %d (supported: multiples of 64 from 64 to 512)", a.D);
-  }
+  LVSR_CHECK(a.ndir == 1 || a.ndir == 2, "bigru backward: %d directions (1 or 2)", a.ndir);
+  const int rc = a.ndir == 1 ? launch_bwd_width<1>(a, stream) : launch_bwd_width<2>(a, stream);
   if (rc == 0 && cs_out) *cs_out = a.D / UC;   // the cluster size that ran
   return rc;
 }

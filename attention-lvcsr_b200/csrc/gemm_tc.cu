@@ -362,7 +362,8 @@ struct StreamSched {
   const float* A;          // [M, K] fp32 rows
   __half *a_head, *a_tail; // [M, K] split planes (p.ea: the row exponents)
   const int* progress;     // [nscan] steps stored per scan CTA; null: every row is final
-  int nscan, scan_cs;      // scan CTA i runs direction (i / scan_cs) & 1
+  int nscan, scan_cs;      // scan CTA i runs direction (i / scan_cs) % ndir
+  int ndir;                // 1: every scan CTA runs forward (no backward progress to wait for)
   int T, k, B;             // frames scanned, subsampling (output frame f = scan frame f k), batch rows per frame
   int mid;                 // m-tile whose rows become final first
   unsigned spin_limit;     // polls without progress before a launch beside the scan stops claiming
@@ -416,7 +417,7 @@ __device__ __forceinline__ void stream_poll(const StreamSched& s, int lane, int&
   int f = INT_MAX, b = INT_MAX;
   for (int i = lane; i < s.nscan; i += 32) {
     const int v = ld_acquire_i32(s.progress + i);
-    if ((i / s.scan_cs) & 1) b = min(b, v); else f = min(f, v);
+    if (s.ndir == 2 && ((i / s.scan_cs) & 1)) b = min(b, v); else f = min(f, v);
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
@@ -909,7 +910,7 @@ int gemm_f16_stream(const float* A, __half* A_head, __half* A_tail, int* ea, int
   StreamSched s;
   s.A = A; s.a_head = A_head; s.a_tail = A_tail;
   s.progress = ps.progress;
-  s.nscan = ps.nscan; s.scan_cs = ps.scan_cs; s.T = ps.T; s.k = ps.k; s.B = ps.B;
+  s.nscan = ps.nscan; s.scan_cs = ps.scan_cs; s.ndir = ps.ndir; s.T = ps.T; s.k = ps.k; s.B = ps.B;
   // the frame the two scan directions finish first: the fewest steps max(f k + 1, T - f k) of both
   int best = INT_MAX, fmid = 0;
   for (int f = 0; f * ps.k < ps.T; ++f) {

@@ -53,7 +53,8 @@ int gemm_f16(const float* A, __half* A_head, __half* A_tail, int* ea, int M, int
 struct ProjStream {
   int* sync;
   const int* progress;     // gemm_f16_stream_progress(sync), handed to the scan (BiGruArgs::progress), or null
-  int nscan, scan_cs;      // CTAs of the scan and CTAs per cluster (scan CTA i runs direction (i / scan_cs) & 1)
+  int nscan, scan_cs;      // CTAs of the scan and CTAs per cluster (scan CTA i runs direction (i / scan_cs) % ndir)
+  int ndir;                // directions of the scan (1: every CTA runs forward)
   int T, k, B;             // frames the scan runs, its subsampling, batch rows
   unsigned spin_limit;     // polls without progress before the launch beside the scan stops claiming
   int* tiles_done;
@@ -70,16 +71,17 @@ int gemm_f16_stream(const float* A, __half* A_head, __half* A_tail, int* ea, int
 
 // ---- bigru.cu -----------------------------------------------------------------------
 struct BiGruArgs {
-  const float* pre;        // [T*B, 6D]: per direction [inputs D | update-gate D | reset-gate D], fwd then bwd
+  const float* pre;        // [T*B, 3 ndir D]: per direction [inputs D | update-gate D | reset-gate D], fwd then bwd
   const float* mask;       // [T, B] view (time stride mask_tstride) or nullptr
   long long mask_tstride;
   const float *Wg_f, *Ws_f, *h0_f;   // forward  state_to_gates [D,2D], state_to_state [D,D], initial_state [D]
-  const float *Wg_b, *Ws_b, *h0_b;   // backward
-  float* out;              // [ceil(T/subsample), B, 2D] (forward units first)
+  const float *Wg_b, *Ws_b, *h0_b;   // backward (unused when ndir is 1)
+  float* out;              // [ceil(T/subsample), B, ndir D] (forward units first)
   int T, B, D, subsample;
+  int ndir;                // 2: both directions, 1: forward only (net.bidir False)
   // training only (both null for inference): the tape the backward scan reads
   float* tape;             // = pre, written in place: candidate c over the inputs slot, z / r over the gate slots
-  float* hext;             // [(T+2), B, 2D]: slot t+1 = states after time t; slot 0 (forward half) and slot T+1
+  float* hext;             // [(T+2), B, ndir D]: slot t+1 = states after time t; slot 0 (forward half) and slot T+1
                            // (backward half) = the broadcast initial states
   // optional, tensor-core kernel only: progress[cta] = time steps whose output stores that CTA has made visible at gpu
   // scope (published every few steps and after the last), for a projection streamed behind the scan
@@ -94,15 +96,16 @@ int bigru_layer(const BiGruArgs& a, cudaStream_t stream, BiGruPlan* plan = nullp
 
 // ---- bigru_bwd.cu: reverse-time scan of one layer (training) ------------------------------
 struct BiGruBwdArgs {
-  float* tape;             // [T*B, 6D] in: c | z | r per direction (forward's tape); out: dA | dGz | dGr
-  const float* hext;       // [(T+2), B, 2D] (see BiGruArgs)
+  float* tape;             // [T*B, 3 ndir D] in: c | z | r per direction (forward's tape); out: dA | dGz | dGr
+  const float* hext;       // [(T+2), B, ndir D] (see BiGruArgs)
   const float* mask;       // [T, B] view or nullptr
   long long mask_tstride;
-  const float* dout;       // [ceil(T/subsample), B, 2D] gradient of the layer's (subsampled) output
+  const float* dout;       // [ceil(T/subsample), B, ndir D] gradient of the layer's (subsampled) output
   const float *Wg_f, *Ws_f, *Wg_b, *Ws_b;
-  float* hr_out;           // [T, B, 2D]: h_prev * r (operand of the state_to_state gradient)
-  float* dh0;              // [2, B, D]: gradient of the broadcast initial state, per direction and row
+  float* hr_out;           // [T, B, ndir D]: h_prev * r (operand of the state_to_state gradient)
+  float* dh0;              // [ndir, B, D]: gradient of the broadcast initial state, per direction and row
   int T, B, D, subsample;
+  int ndir;                // as BiGruArgs::ndir
 };
 int bigru_layer_backward(const BiGruBwdArgs& a, cudaStream_t stream, int* cs_out = nullptr);   // *cs_out: CTAs per cluster
 

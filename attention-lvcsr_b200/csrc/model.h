@@ -107,6 +107,7 @@ struct lvsr_model {
   lvsr_config cfg;
   lvsr_bottom_config bottom = {};   // the bottom MLP in front of the encoder (num_layers 0: none)
   int device = 0;                   // the GPU this handle lives on (current device at lvsr_model_create)
+  int ndir = 2;                     // encoder directions: 2 bidirectional, 1 forward only (read through encoder_dirs)
   int E;
   std::vector<Param> params;
   std::map<std::string, int> index;
@@ -115,7 +116,7 @@ struct lvsr_model {
   float* flat = nullptr;
   int64_t flat_count = 0;
   // packed, kernel-side weights (rebuilt by finalize)
-  std::vector<float*> Wcat, bcat;   // per encoder layer: [Din, 6D], [6D] (encoder_fork)
+  std::vector<float*> Wcat, bcat;   // per encoder layer: [Din, 3 ndir D], [3 ndir D] (encoder_fork)
   // the packed inputs of decoder layer l < dec_stack (finalize), gate columns first (update | reset), then the
   // candidate inputs; the parameters of layer l > 0 carry the suffix "#l" (layer_suffix)
   struct DecLayer {
@@ -236,9 +237,18 @@ static inline std::string dec_gru(const lvsr_model* m, int level) {
   return std::string(TR) + "/recurrentstack/transition_" + std::to_string(level) + "#" + std::to_string(level);
 }
 
-static inline std::string enc_base(int l, int dir) {
+// Directions of every encoder layer: 2 for Bidirectional, 1 for a forward-only RecurrentWithFork (net.bidir False,
+// lvsr/bricks/__init__.py:54-78).  Layer l's output, and layer l + 1's input, is encoder_dirs(m) * dims_bidir[l] wide.
+static inline int encoder_dirs(const lvsr_model* m) { return m->ndir; }
+static inline int encoder_output_dim(const lvsr_model* m, int l) { return encoder_dirs(m) * m->cfg.dims_bidir[l]; }
+
+// brick path of encoder layer l, direction dir: "bidir<l>/forward|backward", or "with_fork<l>" when unidirectional
+static inline std::string enc_base(const lvsr_model* m, int l, int dir) {
   char buf[128];
-  snprintf(buf, sizeof(buf), "/recognizer/encoder/bidir%d/%s", l, dir ? "backward" : "forward");
+  if (encoder_dirs(m) == 1)
+    snprintf(buf, sizeof(buf), "/recognizer/encoder/with_fork%d", l);
+  else
+    snprintf(buf, sizeof(buf), "/recognizer/encoder/bidir%d/%s", l, dir ? "backward" : "forward");
   return buf;
 }
 
@@ -310,11 +320,13 @@ static inline int bottom_input_dim(const lvsr_model* m, int i) { return i ? m->b
 
 // A packed fork, blocks in column order: <fork>/<param>.W fills columns [col, col + cols) of W [rows, ld], .b those of b [ld]
 struct ForkLayout { std::string fork; int rows, ld; struct { std::string param; int col, cols; } block[2]; };
-// encoder layer l, direction dir, in Wcat[l] / bcat[l]: per direction [inputs D | gate_inputs 2D (update | reset)]
+// encoder layer l, direction dir, in Wcat[l] / bcat[l]: per direction [inputs D | gate_inputs 2D (update | reset)],
+// encoder_dirs(m) directions side by side
 static inline ForkLayout encoder_fork(const lvsr_model* m, int l, int dir) {
   const lvsr_config& c = m->cfg;
-  const int D = c.dims_bidir[l], c0 = dir * 3 * D, din = l ? 2 * c.dims_bidir[l - 1] : encoder_input_dim(m);
-  return {enc_base(l, dir) + "/fork", din, 6 * D, {{"fork_inputs", c0, D}, {"fork_gate_inputs", c0 + D, 2 * D}}};
+  const int D = c.dims_bidir[l], c0 = dir * 3 * D, din = l ? encoder_output_dim(m, l - 1) : encoder_input_dim(m);
+  return {enc_base(m, l, dir) + "/fork", din, 3 * encoder_dirs(m) * D,
+          {{"fork_inputs", c0, D}, {"fork_gate_inputs", c0 + D, 2 * D}}};
 }
 // Suffix of the names of decoder layer l's inputs: "" for layer 0, "#<l>" above it (the RecurrentStack's names of
 // layer l's sequences, libs/blocks/blocks/bricks/recurrent.py:819-820)
@@ -341,8 +353,8 @@ static inline int check_ready(lvsr_model* m) {
 // One encoder layer as the training step's backward pass reads it.
 struct LayerTape {
   const float* X;      // input of the layer [T*B, Din]
-  float* pre;          // [T*B, 6D] forward tape, then dPre
-  float* hext;         // [(T+2), B, 2D]
+  float* pre;          // [T*B, 3 ndir D] forward tape, then dPre
+  float* hext;         // [(T+2), B, ndir D]
   int T, Din, D, k;
   long long mstride;
 };

@@ -182,11 +182,13 @@ struct TrainStep {
                 rows * di + 2 * rows * d + 2 * di * d) * sizeof(float);
     }
     for (int l = 0; l < c.num_layers; ++l) {
-      const int D = c.dims_bidir[l], Tout = ceil_div(Tl, c.subsample[l]);
-      bytes += ((size_t)Tl * B * 6 * D * 2 + (size_t)(Tl + 2) * B * 2 * D * 2 + (size_t)Tout * B * 2 * D * 2 + (size_t)3 * Tl * B * gemm_tc_kpad(din)) * sizeof(float);
-      bytes += (size_t)80 * std::max(din, 2 * D) * 6 * D * sizeof(float);      // TN partials
-      bytes += ((size_t)2 * (6 * D + din + 3 * D + 32) * (Tl * (size_t)B + 32) + (size_t)2 * Tl * B * 6 * D) * sizeof(float);   // K-major tf32 operands
-      Tl = Tout; din = 2 * D;
+      // N: the fork's columns (3 ndir D), Dout: the layer's output (ndir D)
+      const int D = c.dims_bidir[l], Tout = ceil_div(Tl, c.subsample[l]), N = encoder_fork(m, l, 0).ld;
+      const int Dout = encoder_output_dim(m, l);
+      bytes += ((size_t)Tl * B * N * 2 + (size_t)(Tl + 2) * B * Dout * 2 + (size_t)Tout * B * Dout * 2 + (size_t)3 * Tl * B * gemm_tc_kpad(din)) * sizeof(float);
+      bytes += (size_t)80 * std::max(din, Dout) * N * sizeof(float);      // TN partials
+      bytes += ((size_t)2 * (N + din + 3 * D + 32) * (Tl * (size_t)B + 32) + (size_t)2 * Tl * B * N) * sizeof(float);   // K-major tf32 operands
+      Tl = Tout; din = Dout;
     }
     bytes += ((size_t)Tp * B * (2 * M + 2 * E) + (size_t)R * (Tp + 8 * C + 3 * E + 2 * M + 3 * Cpm + V + 16) + (size_t)4 * B * Tp +
               (size_t)2 * B * (M + (size_t)K * M + (size_t)K * w) + (size_t)4 * (E + C) * 3 * C + (size_t)80 * E * M) * sizeof(float);
@@ -535,16 +537,19 @@ struct TrainStep {
     float* dX0 = nullptr;
     for (int l = c.num_layers - 1; l >= 0; --l) {
       const LayerTape& tp = tape[l];
-      const int D = tp.D, rows = tp.T * B;
-      float* hr = ws.f32((size_t)rows * 2 * D);
-      float* dh0 = ws.f32((size_t)2 * B * D);
+      // nd directions side by side: the tape's rows are N = 3 nd D wide, hext's and hr's Dout = nd D
+      const int D = tp.D, rows = tp.T * B, nd = encoder_dirs(m), N = 3 * nd * D, Dout = nd * D;
+      float* hr = ws.f32((size_t)rows * Dout);
+      float* dh0 = ws.f32((size_t)nd * B * D);
       LVSR_CHECK(hr && dh0, "out of device memory (encoder backward)");
       BiGruBwdArgs a = {};
       a.tape = tp.pre; a.hext = tp.hext; a.mask = mask; a.mask_tstride = tp.mstride; a.dout = dout;
-      const std::string bf = enc_base(l, 0), bb = enc_base(l, 1);
+      const std::string bf = enc_base(m, l, 0), bb = enc_base(m, l, 1);
       a.Wg_f = m->P(bf + "/gatedrecurrent.state_to_gates"); a.Ws_f = m->P(bf + "/gatedrecurrent.state_to_state");
-      a.Wg_b = m->P(bb + "/gatedrecurrent.state_to_gates"); a.Ws_b = m->P(bb + "/gatedrecurrent.state_to_state");
-      a.hr_out = hr; a.dh0 = dh0; a.T = tp.T; a.B = B; a.D = D; a.subsample = tp.k;
+      if (nd == 2) {
+        a.Wg_b = m->P(bb + "/gatedrecurrent.state_to_gates"); a.Ws_b = m->P(bb + "/gatedrecurrent.state_to_state");
+      }
+      a.hr_out = hr; a.dh0 = dh0; a.T = tp.T; a.B = B; a.D = D; a.subsample = tp.k; a.ndir = nd;
       int32_t* plan = m->enc_plan[l];
       int bwd_cs = 0, wsplits = 0;
       if (int rc = bigru_layer_backward(a, st, &bwd_cs)) return rc;
@@ -552,31 +557,31 @@ struct TrainStep {
       // fork: dWcat = X^T dPre, dbcat = colsum(dPre), scattered to the parameters by the layer's fork layout
       {
         ArenaMark mark{ws};
-        float* dWcat = ws.f32((size_t)tp.Din * 6 * D);
-        float* dbcat = ws.f32((size_t)6 * D);
+        float* dWcat = ws.f32((size_t)tp.Din * N);
+        float* dbcat = ws.f32((size_t)N);
         LVSR_CHECK(dWcat && dbcat, "out of device memory (fork gradients)");
         // tensor-core path: every operand transposed once into K-major tf32 hi/lo pairs (the contraction runs over the
         // T*B rows), then five split-K tensor-core products share them; FFMA tiles for small problems / LVSR_NO_TC_GEMM
         const bool tc = m->use_tc && rows >= 2048 && D % 128 == 0;
         // H_prev of each direction: slot t (forward) / t+2 (backward) of hext
-        const float* hprev[2] = {tp.hext, tp.hext + (size_t)2 * B * 2 * D + D};
+        const float* hprev[2] = {tp.hext, tp.hext + (size_t)2 * B * Dout + D};
         TcOperand dPreT, XT, hrT, hpT[2];
         if (tc) {
-          if (int rc = make_tc_operand(ws, tp.pre, rows, 6 * D, 6 * D, &dPreT, st)) return rc;
+          if (int rc = make_tc_operand(ws, tp.pre, rows, N, N, &dPreT, st)) return rc;
           if (int rc = make_tc_operand(ws, tp.X, rows, tp.Din, tp.Din, &XT, st)) return rc;
-          if (int rc = make_tc_operand(ws, hr, rows, 2 * D, 2 * D, &hrT, st)) return rc;
-          for (int dir = 0; dir < 2; ++dir)
-            if (int rc = make_tc_operand(ws, hprev[dir], rows, D, 2 * D, &hpT[dir], st)) return rc;
-          if (int rc = gemm_tn_tc(ws, XT, 0, tp.Din, dPreT, 0, 6 * D, dWcat, 6 * D, false, st, &wsplits)) return rc;
+          if (int rc = make_tc_operand(ws, hr, rows, Dout, Dout, &hrT, st)) return rc;
+          for (int dir = 0; dir < nd; ++dir)
+            if (int rc = make_tc_operand(ws, hprev[dir], rows, D, Dout, &hpT[dir], st)) return rc;
+          if (int rc = gemm_tn_tc(ws, XT, 0, tp.Din, dPreT, 0, N, dWcat, N, false, st, &wsplits)) return rc;
         } else {
-          if (int rc = gemm_tn(ws, tp.X, tp.Din, tp.pre, 6 * D, rows, tp.Din, 6 * D, dWcat, 6 * D, false, st, &wsplits)) return rc;
+          if (int rc = gemm_tn(ws, tp.X, tp.Din, tp.pre, N, rows, tp.Din, N, dWcat, N, false, st, &wsplits)) return rc;
         }
         plan[LVSR_ENC_WGRAD] = tc ? LVSR_ENC_PATH_TC : LVSR_ENC_PATH_FFMA;
         plan[LVSR_ENC_WGRAD_SPLITS] = wsplits;
         plan[LVSR_ENC_WGRAD_KPAD] = tc ? dPreT.Kpad : 0;
-        if (int rc = colsum(tp.pre, rows, 6 * D, 6 * D, dbcat, false, st)) return rc;
-        for (int dir = 0; dir < 2; ++dir) {
-          const std::string b = enc_base(l, dir);
+        if (int rc = colsum(tp.pre, rows, N, N, dbcat, false, st)) return rc;
+        for (int dir = 0; dir < nd; ++dir) {
+          const std::string b = enc_base(m, l, dir);
           const ForkLayout f = encoder_fork(m, l, dir);
           const int cA = f.block[0].col, cG = f.block[1].col;      // columns of dA (fork_inputs) and [dGz|dGr]
           if (int rc = fork_copy(m, f, dWcat, dbcat, grads, st)) return rc;
@@ -587,8 +592,8 @@ struct TrainStep {
             if (int rc = gemm_tn_tc(ws, hrT, dir * D, D, dPreT, cA, D, gWs, D, false, st)) return rc;
             if (int rc = gemm_tn_tc(ws, hpT[dir], 0, D, dPreT, cG, 2 * D, gWg, 2 * D, false, st)) return rc;
           } else {
-            if (int rc = gemm_tn(ws, hr + dir * D, 2 * D, tp.pre + cA, 6 * D, rows, D, D, gWs, D, false, st)) return rc;
-            if (int rc = gemm_tn(ws, hprev[dir], 2 * D, tp.pre + cG, 6 * D, rows, D, 2 * D, gWg, 2 * D, false, st)) return rc;
+            if (int rc = gemm_tn(ws, hr + dir * D, Dout, tp.pre + cA, N, rows, D, D, gWs, D, false, st)) return rc;
+            if (int rc = gemm_tn(ws, hprev[dir], Dout, tp.pre + cG, N, rows, D, 2 * D, gWg, 2 * D, false, st)) return rc;
           }
           if (int rc = colsum(dh0 + (size_t)dir * B * D, B, D, D, grad(b + "/gatedrecurrent.initial_state"), false, st)) return rc;
         }
@@ -597,8 +602,8 @@ struct TrainStep {
       if (l > 0 || m->bottom.num_layers) {
         float* dX = ws.f32((size_t)rows * tp.Din);
         LVSR_CHECK(dX, "out of device memory (dX)");
-        // dX = dPre . Wcat^T: the K-major form of the right-hand side [N = Din, K = 6D] is Wcat itself
-        if (int rc = input_grad(tp.pre, rows, 6 * D, m->Wcat[l], tp.Din, dX, &plan[LVSR_ENC_DX])) return rc;
+        // dX = dPre . Wcat^T: the K-major form of the right-hand side [N = Din, K = 3 nd D] is Wcat itself
+        if (int rc = input_grad(tp.pre, rows, N, m->Wcat[l], tp.Din, dX, &plan[LVSR_ENC_DX])) return rc;
         dout = dX0 = dX;
       }
     }

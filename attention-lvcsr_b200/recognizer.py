@@ -96,8 +96,10 @@ class SpeechRecognizer(object):
         if lm and character_map is None:
             unsupported("lm without a character_map")
         lm = _lm_config(lm) if lm else None
-        if not bidir:
-            unsupported("unidirectional encoder")
+        if bidir not in (True, False, 0, 1):
+            # net.bidir (lvsr/configs/schema.yaml:48-49) is a boolean
+            raise ValueError("bidir must be True (Bidirectional encoder layers) or False (forward-only "
+                             "RecurrentWithFork layers), got %r" % (bidir,))
         if dims_top:
             unsupported("dims_top")
         if dec_stack not in (1, 2):
@@ -160,7 +162,7 @@ class SpeechRecognizer(object):
             post_merge_activation=act.kind, maxout_pieces=int(getattr(act, "num_pieces", 1)),
             use_states_for_readout=bool(use_states_for_readout),
             energy_normalizer=energy_normalizer or "softmax", prior=prior, attention_type=attention_type,
-            dec_stack=int(dec_stack))
+            dec_stack=int(dec_stack), bidir=bool(bidir))
         if bottom_dims:
             self.net["bottom"] = dict(dims=bottom_dims, activation=bottom_kind)
         if not post_merge_dims:
@@ -269,7 +271,10 @@ class SpeechRecognizer(object):
                 h = C.c_void_p()
                 cfg = self._make_config()
                 bottom = self._make_bottom_config()
-                if bottom is None:
+                if not self.bidir:
+                    _lib.check(lib.lvsr_model_create_encoder(C.byref(cfg), None if bottom is None else C.byref(bottom),
+                                                             0, C.byref(h)))
+                elif bottom is None:
                     _lib.check(lib.lvsr_model_create(C.byref(cfg), C.byref(h)))
                 else:
                     _lib.check(lib.lvsr_model_create_bottom(C.byref(cfg), C.byref(bottom), C.byref(h)))
@@ -566,8 +571,14 @@ class SpeechRecognizer(object):
         return int(_lib.load().lvsr_encoded_length(self._require_ready(), int(T)))
 
     @property
+    def bidir(self):
+        """net.bidir: Bidirectional encoder layers (True) or forward-only ones (False)."""
+        return self.net.get("bidir", True)
+
+    @property
     def dim_encoded(self):
-        return 2 * self.net["dims_bidir"][-1]
+        """Width of the encoded frames: both directions' states of the last layer, or its one direction's."""
+        return (2 if self.bidir else 1) * self.net["dims_bidir"][-1]
 
     @property
     def dim_state(self):

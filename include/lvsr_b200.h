@@ -107,6 +107,12 @@ int lvsr_model_create(const lvsr_config* cfg, lvsr_model** out);
 /* The same with a bottom MLP (NULL: none, which is lvsr_model_create).  Every entry point that takes recordings runs
  * it; a depth, width or activation outside lvsr_bottom_config's ranges is refused here. */
 int lvsr_model_create_bottom(const lvsr_config* cfg, const lvsr_bottom_config* bottom, lvsr_model** out);
+/* The same with the encoder's direction count (net.bidir, lvsr/bricks/__init__.py:54-78): bidir 1 is the bidirectional
+ * encoder the two calls above build; bidir 0 makes every layer l one forward-only GatedRecurrent
+ * ("/recognizer/encoder/with_fork<l>/..."), layer l + 1 takes dims_bidir[l] features and the encoded width is
+ * dims_bidir[num_layers - 1].  Any other value is refused before any device work.  Added within version 104: detect it
+ * by its symbol. */
+int lvsr_model_create_encoder(const lvsr_config* cfg, const lvsr_bottom_config* bottom, int32_t bidir, lvsr_model** out);
 int lvsr_model_destroy(lvsr_model* m);
 
 /* Parameter table in Blocks order/names ("/recognizer/encoder/bidir0/forward/fork/fork_inputs.W"
