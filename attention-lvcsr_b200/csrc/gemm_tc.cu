@@ -343,10 +343,11 @@ __global__ void split_rows_f16_kernel(const float* __restrict__ x, __half* __res
 
 // ---- streamed fp16 projection ---------------------------------------------------------------------------------------
 // The fork GEMM of encoder layer l + 1 while the BiGRU scan of layer l still runs (api.cu: run_encoder).  Input frame t
-// of layer l + 1 is final once the forward scan has stored step t and the backward scan step T - 1 - t; the scan
-// publishes how many steps each of its CTAs has stored (bigru.cu).  gemm_f16_stream_kernel is gemm_tc_kernel<true> with
-// a dynamic tile schedule: warps 1..3 of the producer warpgroup claim output tiles from one counter, in the order their
-// rows become final (the middle m-tile first, then outward), split the tile's rows of A into fp16 head / tail planes and
+// of layer l + 1 is final once the forward scan has stored step t and the backward scan step T - 1 - t (a forward-only
+// scan: once it has stored step t); the scan publishes how many steps each of its CTAs has stored (bigru.cu).
+// gemm_f16_stream_kernel is gemm_tc_kernel<true> with a dynamic tile schedule: warps 1..3 of the producer warpgroup
+// claim output tiles from one counter, in the order their rows become final (two directions: the middle m-tile first,
+// then outward; forward only: m-tile 0 first, then upward), split the tile's rows of A into fp16 head / tail planes and
 // exponents (split_rows_f16_kernel's rule) and hand the tile to the TMA thread and the consumers through a one-slot
 // queue; the split of an m-tile is shared out in 8-row chunks among the CTAs that claim its n-tiles.  Launched beside
 // the scan it claims only tiles whose rows are final and stops claiming when the scan has finished or has not
@@ -911,10 +912,11 @@ int gemm_f16_stream(const float* A, __half* A_head, __half* A_tail, int* ea, int
   s.A = A; s.a_head = A_head; s.a_tail = A_tail;
   s.progress = ps.progress;
   s.nscan = ps.nscan; s.scan_cs = ps.scan_cs; s.ndir = ps.ndir; s.T = ps.T; s.k = ps.k; s.B = ps.B;
-  // the frame the two scan directions finish first: the fewest steps max(f k + 1, T - f k) of both
+  // the frame that becomes final first: the fewest scan steps max(f k + 1, T - f k) that both directions need, or
+  // f k + 1 when the scan runs forward only (frame 0, so the m-tiles are claimed in ascending order)
   int best = INT_MAX, fmid = 0;
   for (int f = 0; f * ps.k < ps.T; ++f) {
-    const int ready = std::max(f * ps.k + 1, ps.T - f * ps.k);
+    const int ready = ps.ndir == 1 ? f * ps.k + 1 : std::max(f * ps.k + 1, ps.T - f * ps.k);
     if (ready < best) { best = ready; fmid = f; }
   }
   s.mid = std::min((int)((long long)fmid * ps.B / TC_BM), p.tiles_m - 1);

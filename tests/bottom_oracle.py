@@ -12,7 +12,9 @@ table are restated here:
     and before the generator's (SpeechRecognizer.children = [encoder, top, bottom, generator], :350);
   * every entry point starting from recordings runs the inner model's on bottom(recordings): lvsr_oracle for
     content_and_conv attention, content_oracle for content attention, stack_oracle for dec_stack 2;
-  * the torch float64 mirror (cost_and_grads, train_step) puts the bottom in front of lvsr_oracle_grad's encoder.
+  * the torch float64 mirror (cost_and_grads, train_step) puts the bottom in front of lvsr_oracle_grad's encoder;
+  * a forward-only encoder (cfg["bidir"] False, unidirectional_oracle.make_config's configs) takes
+    unidirectional_oracle's table, encoder and decoder functions in place of lvsr_oracle's.
 
 tests/test_bottom_cpu.py pins this module: Blocks' test_mlp known answer, the Rectifier at 0, the mirror against the
 numpy functions, autograd against finite differences.
@@ -25,6 +27,7 @@ from oracle import lvsr_oracle as O
 from oracle import lvsr_oracle_grad as G
 import content_oracle as CO
 import stack_oracle as SO
+import unidirectional_oracle as U
 
 BOTTOM = "/recognizer/bottom/bottom"
 
@@ -45,7 +48,13 @@ def inner(cfg):
     return out
 
 
+def _unidirectional(cfg):
+    return cfg.get("bidir", True) is False
+
+
 def _module(cfg):
+    if _unidirectional(cfg):
+        return U
     if cfg.get("dec_stack", 1) == 2:
         return SO
     return CO if cfg.get("attention_type") == "content" else O
@@ -120,7 +129,7 @@ def bottom(cfg, params, x):
 
 
 def encoder(cfg, params, x, mask=None):
-    return O.encoder(inner(cfg), params, bottom(cfg, params, x), mask)
+    return (U if _unidirectional(cfg) else O).encoder(inner(cfg), params, bottom(cfg, params, x), mask)
 
 
 def recognizer_cost(cfg, params, recordings, recordings_mask, labels, labels_mask, return_all=False):
@@ -163,7 +172,11 @@ def cost_and_grads(cfg, params, recordings, recordings_mask, labels, labels_mask
     lm = None if labels_mask is None else torch.as_tensor(np.asarray(labels_mask, dtype=np.float64))
     labels = np.asarray(labels, dtype=np.int64)
     icfg = inner(cfg)
-    attended, amask = G._encoder(icfg, p, _bottom_torch(cfg, p, x), m)
+    if _unidirectional(cfg):
+        attended, amask = U._encoder_torch(icfg, p, _bottom_torch(cfg, p, x), m)
+        icfg = U.decoder_config(icfg)
+    else:
+        attended, amask = G._encoder(icfg, p, _bottom_torch(cfg, p, x), m)
     if cfg.get("attention_type") == "content":
         costs = CO._cost_matrix_torch(icfg, p, attended, amask, labels, lm)
     else:

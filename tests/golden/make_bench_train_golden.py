@@ -102,14 +102,25 @@ def crop(batch, b):
 _WORK = {}
 
 
-def _init_worker(cfg, params, batch):
+def _init_worker(cfg, params, batch, oracle=None):
     import torch
     torch.set_num_threads(1)           # one utterance is too small for threads to help; the workers share the cores
-    _WORK.update(cfg=cfg, params=params, batch=batch)
+    _WORK.update(cfg=cfg, params=params, batch=batch, oracle=oracle)
+
+
+def _oracles():
+    """(gradient oracle, forward oracle) of the model: oracle/lvsr_oracle{_grad}.py, or the importable module named by
+    `oracle` (one that has both cost_and_grads and recognizer_cost, e.g. tests/unidirectional_oracle.py)."""
+    if _WORK.get("oracle") is None:
+        from oracle import lvsr_oracle_grad as G
+        return G, O
+    import importlib
+    mod = importlib.import_module(_WORK["oracle"])
+    return mod, mod
 
 
 def _utterance(b):
-    from oracle import lvsr_oracle_grad as G
+    G, _ = _oracles()
     cost, grads, costs = G.cost_and_grads(_WORK["cfg"], _WORK["params"], *crop(_WORK["batch"], b), return_costs=True)
     return cost, grads, costs[:, 0]
 
@@ -119,7 +130,7 @@ def _readout_preactivations(b):
     cfg, p = _WORK["cfg"], _WORK["params"]
     p64 = {k: np.asarray(v, dtype=np.float64) for k, v in p.items()}
     x, m, labels, lm = crop(_WORK["batch"], b)
-    out = O.recognizer_cost(cfg, p64, x.astype(np.float64), m.astype(np.float64), labels, lm.astype(np.float64),
+    out = _oracles()[1].recognizer_cost(cfg, p64, x.astype(np.float64), m.astype(np.float64), labels, lm.astype(np.float64),
                             return_all=True)
     pre = out["weighted_averages"] @ p64[_RO + "/merge/transform_weighted_averages.W"] + p64[_RO + "/post_merge/bias.b"]
     if cfg["use_states_for_readout"]:
@@ -127,11 +138,11 @@ def _readout_preactivations(b):
     return pre[:, 0]
 
 
-def _pool(cfg, params, batch, workers):
+def _pool(cfg, params, batch, workers, oracle=None):
     if workers > 1:
         return multiprocessing.get_context("spawn").Pool(workers, initializer=_init_worker,
-                                                         initargs=(cfg, params, batch))
-    _WORK.update(cfg=cfg, params=params, batch=batch)
+                                                         initargs=(cfg, params, batch, oracle))
+    _WORK.update(cfg=cfg, params=params, batch=batch, oracle=oracle)
     return None
 
 
@@ -139,11 +150,11 @@ def _map(pool, fn, items):
     return pool.imap(fn, items) if pool is not None else map(fn, items)
 
 
-def maxout_gaps(cfg, params, batch, workers=1):
+def maxout_gaps(cfg, params, batch, workers=1, oracle=None):
     """float64 (first piece - second piece) of every two-piece maxout unit of the readout at every label-unmasked
-    row, [n_rows, units]."""
+    row, [n_rows, units]; oracle: as _oracles."""
     assert cfg["post_merge_activation"] == "maxout" and cfg["maxout_pieces"] == 2, cfg
-    pool = _pool(cfg, params, batch, workers)
+    pool = _pool(cfg, params, batch, workers, oracle)
     try:
         pre = np.concatenate(list(_map(pool, _readout_preactivations, range(np.asarray(batch[2]).shape[1]))))
     finally:
@@ -181,14 +192,14 @@ def apply_nudges(params, index, value):
     return out
 
 
-def mean_of_utterance_grads(cfg, params, batch, workers=1):
+def mean_of_utterance_grads(cfg, params, batch, workers=1, oracle=None):
     """float64 (sum(costs) / B, costs [L, B], gradient) of the batch, as the mean over its utterances run one at a time.
-    Summed in utterance order, so the result does not depend on `workers`."""
+    Summed in utterance order, so the result does not depend on `workers`; oracle: as _oracles."""
     check_prior(cfg)
     L, B = np.asarray(batch[2]).shape
     costs = np.zeros((L, B))
     total, grads = 0.0, None
-    pool = _pool(cfg, params, batch, workers)
+    pool = _pool(cfg, params, batch, workers, oracle)
     try:
         for b, (cost, g, c) in enumerate(_map(pool, _utterance, range(B))):
             total += cost
@@ -248,30 +259,37 @@ def meta():
     return dict(workload=bench.TRAIN_WORKLOAD, net=bench.NET, train_conf=bench.TRAIN_CONF, seed=SEED)
 
 
-def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--workers", type=int, default=min(8, os.cpu_count() or 1))
-    ap.add_argument("--out", default=PATH)
-    args = ap.parse_args()
-    cfg, batch, params = bench_inputs()
+def write_fixture(out, cfg, batch, params, meta, workers, oracle=None):
+    """The fixture of the training step of (cfg, params) on `batch` (the fields listed above) -> `out`; oracle: as
+    _oracles."""
     t0 = time.time()
     check_prior(cfg)
-    gaps = maxout_gaps(cfg, params, batch, workers=args.workers)
+    gaps = maxout_gaps(cfg, params, batch, workers=workers, oracle=oracle)
     nudges = kink_nudges(gaps)
     index = np.array([2 * j for j in sorted(nudges)], dtype=np.int64)             # the unit's first piece
     value = np.array([nudges[j] for j in sorted(nudges)], dtype=np.float32)
     moved = gaps.copy()
     moved[:, index // 2] += value.astype(np.float64)
     assert np.abs(moved).min() >= KINK_EPS
-    cost, costs, grads = mean_of_utterance_grads(cfg, apply_nudges(params, index, value), batch, workers=args.workers)
+    cost, costs, grads = mean_of_utterance_grads(cfg, apply_nudges(params, index, value), batch, workers=workers,
+                                                 oracle=oracle)
     norm = float(np.sqrt(sum((g * g).sum() for g in grads.values())))
-    np.savez_compressed(args.out, meta=np.array(json.dumps(meta(), sort_keys=True)),
+    np.savez_compressed(out, meta=np.array(json.dumps(meta, sort_keys=True)),
                         batch_sha256=np.array(batch_digests(batch)), params_sha256=np.array(params_digest(params)),
                         kink_eps=np.float64(KINK_EPS), nudge_index=index, nudge_value=value,
                         min_gap_before=np.float64(np.abs(gaps).min()), min_gap=np.float64(np.abs(moved).min()),
                         cost=np.float64(cost), costs=costs, grad_norm=np.float64(norm), **reduce_grads(grads))
     print("oracle %.0f s, %d maxout units moved off their kinks, cost %.6f, |g| %.6f -> %s (%.0f KB)" % (
-        time.time() - t0, len(index), cost, norm, args.out, os.path.getsize(args.out) / 1024))
+        time.time() - t0, len(index), cost, norm, out, os.path.getsize(out) / 1024))
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--workers", type=int, default=min(8, os.cpu_count() or 1))
+    ap.add_argument("--out", default=PATH)
+    args = ap.parse_args()
+    cfg, batch, params = bench_inputs()
+    write_fixture(args.out, cfg, batch, params, meta(), args.workers)
 
 
 if __name__ == "__main__":

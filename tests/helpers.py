@@ -210,7 +210,8 @@ _READOUT = "/recognizer/generator/readout/post_merge/mlp/linear_0"
 
 
 def bottom_recognizer(cfg, params=None, lm=None, cmap=None):
-    """A SpeechRecognizer of a bottom_oracle config (a bottom MLP in front of the encoder)."""
+    """A SpeechRecognizer of a bottom_oracle config (a bottom MLP in front of the encoder; forward-only encoder layers
+    when the config has bidir False)."""
     pkg = package()
     content = cfg.get("attention_type") == "content"
     act = {"relu": pkg.Rectifier(), "tanh": pkg.Tanh()}[cfg["bottom"]["activation"]]
@@ -226,7 +227,8 @@ def bottom_recognizer(cfg, params=None, lm=None, cmap=None):
         attention_type="content" if content else "content_and_conv",
         max_decoded_length_scale=cfg["max_decoded_length_scale"], enc_transition=pkg.GatedRecurrent,
         dec_transition=pkg.GatedRecurrent, data_prepend_eos=False, lm=lm, character_map=cmap,
-        dec_stack=cfg.get("dec_stack", 1), bottom=dict(dims=cfg["bottom"]["dims"], activation=act))
+        dec_stack=cfg.get("dec_stack", 1), bottom=dict(dims=cfg["bottom"]["dims"], activation=act),
+        bidir=cfg.get("bidir", True))
     if params is not None:
         rec.set_parameter_values(params)
     return rec
@@ -247,10 +249,14 @@ def bottom_params(cfg, seed, gain=1.0, eos_bias=None):
     return OrderedDict((k, f32(v)) for k, v in p.items())
 
 
-def check_overlap_claims(rec, plan, B, subsample):
+INT_MAX = 2 ** 31 - 1
+
+
+def check_overlap_claims(rec, plan, B, subsample, ndir=2):
     """Every tile the launch beside a scan claimed had all its rows final at the progress it was claimed at: input frame
     f of layer l is the scan's output frame f, stored at scan step f k by the forward direction and at step T - 1 - f k
-    by the backward one, so it is final once forward progress > f k and backward progress >= T - f k."""
+    by the backward one, so it is final once forward progress > f k and backward progress >= T - f k.  A forward-only
+    scan (ndir 1) has no backward progress: its records must hold INT_MAX there, and only the forward rule decides."""
     for l, p in enumerate(plan):
         if not p["overlap"]:
             continue
@@ -262,9 +268,86 @@ def check_overlap_claims(rec, plan, B, subsample):
         r0 = (rec_[:, 0] - 1) * 128
         r1 = np.minimum(r0 + 128, M) - 1
         f_lo, f_hi = r0 // B, r1 // B
-        early = (rec_[:, 1] < f_hi * k + 1) | (rec_[:, 2] < T - f_lo * k)
+        if ndir == 1:
+            assert (rec_[:, 2] == INT_MAX).all(), ("layer %d: backward progress recorded beside a forward-only scan" % l,
+                                                   rec_[rec_[:, 2] != INT_MAX][:5])
+            early = rec_[:, 1] < f_hi * k + 1
+        else:
+            early = (rec_[:, 1] < f_hi * k + 1) | (rec_[:, 2] < T - f_lo * k)
         assert not early.any(), ("layer %d: %d of %d tiles claimed before their rows were final" %
                                  (l, early.sum(), len(rec_)), rec_[early][:5], f_lo[early][:5], f_hi[early][:5])
+
+
+def stream_mid(T, k, B, tiles_m, ndir):
+    """gemm_tc.cu gemm_f16_stream: the m-tile whose rows become final first.  Output frame f is the scan's step f k:
+    final after f k + 1 forward steps and, with two directions, T - f k backward steps; mid is the m-tile of the first
+    frame with the fewest steps max(both) (two directions) or f k + 1 (forward only: frame 0)."""
+    best, fmid = None, 0
+    for f in range(-(-T // k)):
+        ready = f * k + 1 if ndir == 1 else max(f * k + 1, T - f * k)
+        if best is None or ready < best:
+            best, fmid = ready, f
+    return min(fmid * B // 128, tiles_m - 1)
+
+
+def stream_m_tile(i, mid, tiles_m):
+    """gemm_tc.cu stream_m_tile: claim index i (in whole m-tiles) -> m-tile: mid, then alternately one further right
+    and one further left, then the rest of the longer side."""
+    if i == 0:
+        return mid
+    j, left, right = i - 1, mid, tiles_m - 1 - mid
+    both = min(left, right)
+    if j < 2 * both:
+        return mid - 1 - (j >> 1) if j & 1 else mid + 1 + (j >> 1)
+    return mid + 1 + j - both if right > left else mid - 1 - (j - both)
+
+
+def check_overlap_claim_order(rec, plan, B, subsample, widths, ndir):
+    """Claim c beside the scan took m-tile stream_m_tile(c // tiles_n, mid, tiles_m), with tiles_n = ndir 3 D / 128
+    column tiles of the fork projection and mid = stream_mid's.  Returns {layer: (mid, tiles beside)}."""
+    out = {}
+    for l, p in enumerate(plan):
+        if not p["overlap"] or not p["tiles_beside"]:
+            continue
+        T, k, M = plan[l - 1]["T"], subsample[l - 1], p["T"] * B
+        tiles_m, tiles_n = -(-M // 128), ndir * 3 * widths[l] // 128
+        mid = stream_mid(T, k, B, tiles_m, ndir)
+        recs = rec.encoder_overlap_claims(l, p["tiles_beside"] + p["tiles_after"]).astype(np.int64)
+        c = np.flatnonzero(recs[:, 0] > 0)
+        assert np.array_equal(c, np.arange(p["tiles_beside"])), (l, c[:8], p)
+        want = np.array([stream_m_tile(i // tiles_n, mid, tiles_m) for i in c])
+        got = recs[c, 0] - 1
+        bad = np.flatnonzero(got != want)
+        assert not bad.size, ("layer %d: %d of %d claims out of order (mid %d of %d m-tiles)" %
+                              (l, bad.size, c.size, mid, tiles_m), c[bad][:5], got[bad][:5], want[bad][:5])
+        out[l] = (mid, int(c.size))
+    return out
+
+
+def check_unidirectional_grads(cfg, params, batch, tol=1e-4, atol_frac=1e-6):
+    """check_grads' comparison for a forward-only model (net.bidir: False) against the gradient oracle of
+    tests/unidirectional_oracle.py; returns the recognizer."""
+    import unidirectional_oracle as U
+    pkg = package()
+    rec = make_recognizer(cfg, params, bidir=False)
+    algo = pkg.GradientDescent(recognizer=rec, step_rule=pkg.CompositeRule([pkg.RemoveNotFinite(0.0)]))
+    cost, grads = algo.cost_and_gradients(dict(zip(algo.SOURCES, batch)))
+    want_cost, want = U.cost_and_grads(cfg, params, *batch)
+    assert set(grads) == set(want)
+    gmax = max(np.abs(w).max() for w in want.values())
+    bad = {}
+    worst = 0.0
+    for k, w in want.items():
+        e = float(np.abs(grads[k].astype(np.float64) - w).max() / max(np.abs(w).max(), 1e-30))
+        floor = atol_frac * gmax / max(np.abs(w).max(), 1e-30)
+        if w.any():
+            worst = max(worst, e)
+        if e > tol + floor:
+            bad[k] = e
+    print("cost", cost, want_cost, "worst rel grad err %.2e" % worst)
+    assert abs(cost - want_cost) <= 1e-4 * abs(want_cost), (cost, want_cost)
+    assert not bad, bad
+    return rec
 
 
 def bench_recognizer():

@@ -18,6 +18,7 @@ test_gpu_train.py::test_wsj_training_batch_matches_golden_gradients; the gradien
 each of two updates to train_like_the_oracle's bar against the float64 step rules applied to the GPU's own gradients."""
 import importlib.util
 import os
+import re
 from collections import OrderedDict
 
 import numpy as np
@@ -60,7 +61,8 @@ def _bench_recognizer(pkg):
 
 def _family(name):
     if "/encoder/" in name:
-        return "encoder layer " + name.split("/encoder/bidir")[1][0]
+        # bidir<l> (Bidirectional layers) or with_fork<l> (forward-only layers)
+        return "encoder layer " + re.search(r"/encoder/(?:bidir|with_fork)(\d+)/", name).group(1)
     if name.startswith(O._ATT + "/"):
         return "attention"
     if name.startswith(O._TR + "/"):

@@ -5,6 +5,7 @@ asserts through encoder_plan() where the overlap ran and that the two launches t
 import numpy as np
 import pytest
 
+import unidirectional_oracle as U
 from helpers import O, WSJ, check_grads, f32, make_recognizer
 from helpers import check_overlap_claims as _check_claims
 
@@ -23,7 +24,7 @@ def _encode(rec, x, m):
     return att.cpu().numpy(), attm.cpu().numpy(), rec.encoder_plan()
 
 
-def _case(net, B, T, seed, monkeypatch, one_frame=False, spin_limit=None, warm=False, reps=1):
+def _case(net, B, T, seed, monkeypatch, one_frame=False, spin_limit=None, warm=False, reps=1, bidir=True):
     """encode with the overlap on and off: bit-identical outputs; returns the plan of the last run with the overlap on.
 
     The workspace persists across calls at the same offsets in both modes, so before every overlap-on run the test
@@ -31,10 +32,13 @@ def _case(net, B, T, seed, monkeypatch, one_frame=False, spin_limit=None, warm=F
     the streamed projection reads and writes then hold another batch's values, and a tile read before its rows are final
     or never written shows in the output; and each tile claimed beside a scan must have been claimed at a progress that
     makes its rows final (_check_claims).  warm: the first call of all has the overlap on (its launch beside the scan
-    also loads the streamed kernel's module) and is compared too; reps: decoy + overlap-on runs."""
+    also loads the streamed kernel's module) and is compared too; reps: decoy + overlap-on runs; bidir False: the
+    forward-only encoder (tests/unidirectional_oracle.py's parameters), whose projections have 3 D columns."""
     _torch()
-    cfg = O.make_config(**dict(WSJ, **net))
-    rec = make_recognizer(cfg, O.init_params(cfg, seed=seed, scale=10.0))
+    M = O if bidir else U
+    ndir = 2 if bidir else 1
+    cfg = M.make_config(**dict(WSJ, **net))
+    rec = make_recognizer(cfg, M.init_params(cfg, seed=seed, scale=10.0), bidir=bidir)
     x, m, _, _ = O.synthetic_batch(cfg, B=B, T=T, seed=seed + 1)
     decoy = O.synthetic_batch(cfg, B=B, T=T, seed=seed + 2)[0]
     if one_frame:
@@ -42,7 +46,7 @@ def _case(net, B, T, seed, monkeypatch, one_frame=False, spin_limit=None, warm=F
     runs = []
     if warm:
         runs.append(_encode(rec, x, m))
-        _check_claims(rec, runs[-1][2], B, cfg["subsample"])
+        _check_claims(rec, runs[-1][2], B, cfg["subsample"], ndir)
     monkeypatch.setenv("LVSR_ENC_OVERLAP", "0")
     want, wantm, off = _encode(rec, x, m)
     assert not any(p["overlap"] for p in off), off
@@ -53,7 +57,7 @@ def _case(net, B, T, seed, monkeypatch, one_frame=False, spin_limit=None, warm=F
         rec.encode(decoy, m)
         monkeypatch.delenv("LVSR_ENC_OVERLAP")
         runs.append(_encode(rec, x, m))
-        _check_claims(rec, runs[-1][2], B, cfg["subsample"])
+        _check_claims(rec, runs[-1][2], B, cfg["subsample"], ndir)
     dims = cfg["dims_bidir"]
     for got, gotm, plan in runs:
         assert np.array_equal(got.view(np.uint32), want.view(np.uint32)), np.abs(got - want).max()
@@ -61,8 +65,8 @@ def _case(net, B, T, seed, monkeypatch, one_frame=False, spin_limit=None, warm=F
         for l, p in enumerate(plan):
             assert (p["proj"], p["operands"]) == (off[l]["proj"], off[l]["operands"]), (l, p, off[l])
             if p["overlap"]:
-                # 128 x 128 output tiles: ceil(T_l B / 128) row tiles x 6 D_l / 128 column tiles
-                tiles = -(-p["T"] * B // 128) * (6 * dims[l] // 128)
+                # 128 x 128 output tiles: ceil(T_l B / 128) row tiles x 3 ndir D_l / 128 column tiles
+                tiles = -(-p["T"] * B // 128) * (3 * ndir * dims[l] // 128)
                 assert p["tiles_beside"] + p["tiles_after"] == tiles, (l, p, tiles)
             else:
                 assert p["tiles_beside"] == p["tiles_after"] == 0, (l, p)

@@ -21,6 +21,7 @@ import pytest
 
 import unidirectional_oracle as U
 from helpers import O, PYRAMID, check_overlap_claims, elementwise_err, f32, make_recognizer, package, rel_err
+from helpers import check_unidirectional_grads as _grads
 from oracle import lvsr_oracle_grad as G
 
 pytestmark = pytest.mark.gpu
@@ -208,30 +209,6 @@ def test_search_many_matches_oracle(attention):
 
 # ---- training ----------------------------------------------------------------------------------------------------------
 
-def _grads(cfg, params, batch, tol=1e-4, atol_frac=1e-6):
-    """helpers.check_grads' comparison against the unidirectional gradient oracle."""
-    pkg = package()
-    rec = _rec(cfg, params)
-    algo = pkg.GradientDescent(recognizer=rec, step_rule=pkg.CompositeRule([pkg.RemoveNotFinite(0.0)]))
-    cost, grads = algo.cost_and_gradients(dict(zip(algo.SOURCES, batch)))
-    want_cost, want = U.cost_and_grads(cfg, params, *batch)
-    assert set(grads) == set(want)
-    gmax = max(np.abs(w).max() for w in want.values())
-    bad = {}
-    worst = 0.0
-    for k, w in want.items():
-        e = float(np.abs(grads[k].astype(np.float64) - w).max() / max(np.abs(w).max(), 1e-30))
-        floor = atol_frac * gmax / max(np.abs(w).max(), 1e-30)
-        if w.any():
-            worst = max(worst, e)
-        if e > tol + floor:
-            bad[k] = e
-    print("cost", cost, want_cost, "worst rel grad err %.2e" % worst)
-    assert abs(cost - want_cost) <= 1e-4 * abs(want_cost), (cost, want_cost)
-    assert not bad, bad
-    return rec
-
-
 GRADS = {                 # name -> (widths, subsampling, B, T, attention)
     "d256_tc": ([256], [1], 33, 63, "content_and_conv"),
     "d448_ffma": ([448], [1], 4, 40, "content_and_conv"),
@@ -339,7 +316,7 @@ def test_streamed_projection_of_a_forward_only_wsj_encoder():
     plan = rec.encoder_plan()
     print([(p["overlap"], p["tiles_beside"], p["tiles_after"], p["clusters"], p["waves"]) for p in plan])
     assert plan[0]["clusters"] == 16 and plan[0]["waves"] == 1, plan[0]
-    check_overlap_claims(rec, plan, 64, cfg["subsample"])
+    check_overlap_claims(rec, plan, 64, cfg["subsample"], ndir=1)
     os.environ["LVSR_ENC_OVERLAP"] = "0"
     try:
         att0, _ = _rec(cfg, params).encode(x, m)
