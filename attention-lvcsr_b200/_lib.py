@@ -106,6 +106,22 @@ class LvsrLmFusion(C.Structure):
                 ("normalize_tot_weights", C.c_int32)]
 
 
+# window_type of lvsr_fbank_options (LVSR_WINDOW_*)
+WINDOW_TYPES = {"povey": 0, "hamming": 1, "hanning": 2, "rectangular": 3}
+
+
+class LvsrFbankOptions(C.Structure):
+    """Mirror of ``lvsr_fbank_options`` (include/lvsr_b200.h)."""
+    _fields_ = [("sample_frequency", C.c_double), ("frame_length", C.c_double), ("frame_shift", C.c_double),
+                ("dither", C.c_double), ("preemphasis_coefficient", C.c_double), ("low_freq", C.c_double),
+                ("high_freq", C.c_double), ("energy_floor", C.c_double), ("vtln_warp", C.c_double),
+                ("seed", C.c_uint64), ("remove_dc_offset", C.c_int32), ("window_type", C.c_int32),
+                ("round_to_power_of_two", C.c_int32), ("snip_edges", C.c_int32), ("num_mel_bins", C.c_int32),
+                ("use_energy", C.c_int32), ("raw_energy", C.c_int32), ("use_log_fbank", C.c_int32),
+                ("use_power", C.c_int32), ("htk_compat", C.c_int32), ("delta_order", C.c_int32),
+                ("delta_window", C.c_int32)]
+
+
 # name -> (restype, argtypes); every symbol include/lvsr_b200.h declares
 _P = C.c_void_p
 _I = C.c_int32
@@ -170,6 +186,14 @@ SIGNATURES = {
     "lvsr_train_dropout_mask": (C.c_int, [_P, C.c_int64, C.c_int64, _I, _I, _I, _P, _P]),
     "lvsr_train_weight_noise_sample": (C.c_int, [_P, C.c_int64, _P, _P]),
     "lvsr_train_penalty_sum": (C.c_int, [_P, _P, _P]),
+    "lvsr_frontend_create": (C.c_int, [C.POINTER(LvsrFbankOptions), C.POINTER(_P)]),
+    "lvsr_frontend_destroy": (C.c_int, [_P]),
+    "lvsr_frontend_num_frames": (C.c_int64, [_P, C.c_int64]),
+    "lvsr_frontend_feature_dim": (C.c_int, [_P]),
+    "lvsr_frontend_compute": (C.c_int, [_P, _P, C.c_int64, C.POINTER(C.c_int64), _I, _I, _P, _P, _P, _P]),
+    "lvsr_frontend_accumulate_cmvn": (C.c_int, [_P, _P, _P, _I, _I, _P, _P]),
+    "lvsr_frontend_apply_cmvn": (C.c_int, [_P, _P, _P, _I, _I, _P, _P]),
+    "lvsr_frontend_dither_sample": (C.c_int, [_P, _I, _I, _P, _P]),
     "lvsr_launch_count": (C.c_int64, [C.c_int]),
     "lvsr_profile_enable": (C.c_int, [C.c_int]),
     "lvsr_profile_read": (C.c_int, [C.c_char_p, C.POINTER(C.c_double), C.POINTER(C.c_int64)]),

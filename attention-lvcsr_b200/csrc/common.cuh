@@ -65,6 +65,16 @@ static inline int device_sm_count() {
   return sms[dev];
 }
 
+// Two N(0, 1) draws from two 32-bit Philox words, Box-Muller in fp32 (the weight noise's and the front end's dither)
+__device__ __forceinline__ float2 box_muller(unsigned x, unsigned y) {
+  const float u = ((float)(x >> 8) + 0.5f) * (1.f / 16777216.f);    // (0, 1): log(u) is finite
+  const float v = (float)(y >> 8) * (1.f / 16777216.f);
+  const float r = sqrtf(-2.f * logf(u));
+  float s, c;
+  sincospif(2.f * v, &s, &c);
+  return make_float2(r * c, r * s);
+}
+
 // ---- device math: accurate enough for the 1e-4 gate against the float64 oracle ----
 __device__ __forceinline__ float sigmoidf_acc(float x) { return 1.0f / (1.0f + __expf(-x)); }
 

@@ -34,15 +34,6 @@ constexpr int kCtasPerParam = 32;              // grid (kCtasPerParam, parameter
 
 struct Span { long long offset, count; };
 
-__device__ __forceinline__ float2 box_muller(unsigned x, unsigned y) {
-  const float u = ((float)(x >> 8) + 0.5f) * (1.f / 16777216.f);    // (0, 1): log(u) is finite
-  const float v = (float)(y >> 8) * (1.f / 16777216.f);
-  const float r = sqrtf(-2.f * logf(u));
-  float s, c;
-  sincospif(2.f * v, &s, &c);
-  return make_float2(r * c, r * s);
-}
-
 // Stream tags of the draws, in the high byte of the fourth Philox counter word (adaptive noise: 0, so its draws are
 // those of an update counter below 2^24 * 2^32)
 constexpr unsigned kTagDropout = 0xD0u << 24, kTagWeightNoise = 0x57u << 24;

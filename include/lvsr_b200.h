@@ -466,6 +466,74 @@ int lvsr_train_dropout_mask(lvsr_model* m, int64_t update, int64_t utterance_off
 int lvsr_train_weight_noise_sample(lvsr_model* m, int64_t update, float* eps_dev, void* stream);
 int lvsr_train_penalty_sum(lvsr_model* m, float* penalty_dev, void* stream);
 
+/* ---- filterbank front end: Kaldi's compute-fbank-feats | add-deltas | global CMVN (exp/wsj/write_hdf_dataset.sh) ----
+ * Waveforms in, the recognizer's recordings [T, B, D] and recordings_mask [T, B] out (DESIGN §1 (j) states the
+ * definition).  Samples are float32 in int16 units, one mono utterance per row of a [B, row_stride] device buffer.
+ * With W / S the frame length / shift in samples, an utterance of N >= W samples has 1 + (N - W) / S frames
+ * (snip_edges); per frame: dither, DC removal, raw log energy, pre-emphasis, window, |real FFT|^2 of the frame
+ * zero-padded to P (a power of two, at most LVSR_FBANK_MAX_PADDED), triangular mel banks, log; the row is
+ * [log energy, bins] (use_energy) or [bins], D0 wide; delta_order > 0 appends the deltas of add-deltas
+ * (D = D0 (delta_order + 1)); a global CMVN stats matrix, when given, normalises every column.
+ *   - dither draws N(0, 1) per (utterance row, frame, sample of the frame) from Philox-4x32-10 keyed by seed, Box-Muller
+ *     in fp32: a rerun with the same seed is bit-identical; lvsr_frontend_dither_sample writes the draws.
+ *   - CMVN stats are Kaldi's [2, D + 1] float64 matrix: row 0 the column sums and the frame count in its last entry,
+ *     row 1 the sums of squares.  Applying them: x' = (x - mean) / sqrt(max(s1 / n - mean^2, 1e-20)).
+ *   - frames past an utterance's end (up to T) are exactly 0 with mask 0.
+ * lvsr_frontend_create refuses, before any device work, snip_edges 0, vtln_warp != 1, htk_compat 1, use_log_fbank 0,
+ * a frame longer than LVSR_FBANK_MAX_PADDED samples and options outside Kaldi's ranges; lvsr_frontend_compute
+ * refuses an utterance shorter than one frame, naming its row.  The handle is bound to the device current at create,
+ * and to streams as the model handle is (the stream rule at the top of this file); it owns its tables and workspace.
+ * Added within version 104: detect these calls by their symbols. */
+enum { LVSR_WINDOW_POVEY = 0, LVSR_WINDOW_HAMMING = 1, LVSR_WINDOW_HANNING = 2, LVSR_WINDOW_RECTANGULAR = 3 };
+enum { LVSR_FBANK_MAX_PADDED = 512, LVSR_FBANK_MAX_DELTA_ORDER = 3, LVSR_FBANK_MAX_DELTA_WINDOW = 4 };
+typedef struct {                     /* Kaldi's option names; (the recipes' values)                                  */
+  double sample_frequency;           /* Hz (16000)                                                                   */
+  double frame_length;               /* ms (25)                                                                      */
+  double frame_shift;                /* ms (10)                                                                      */
+  double dither;                     /* standard deviation of the dither, int16 units (1.0); 0 = off                 */
+  double preemphasis_coefficient;    /* (0.97)                                                                       */
+  double low_freq;                   /* Hz, lower edge of the mel banks (20)                                         */
+  double high_freq;                  /* Hz, upper edge; <= 0: Nyquist + high_freq (0)                                */
+  double energy_floor;               /* > 0: log energy floored at log(energy_floor) (0)                             */
+  double vtln_warp;                  /* must be 1 (no VTLN)                                                          */
+  uint64_t seed;                     /* key of the dither draws                                                      */
+  int32_t remove_dc_offset;          /* (1)                                                                          */
+  int32_t window_type;               /* LVSR_WINDOW_* (povey)                                                        */
+  int32_t round_to_power_of_two;     /* (1); 0 only for a frame of a power-of-two length                             */
+  int32_t snip_edges;                /* must be 1                                                                    */
+  int32_t num_mel_bins;              /* (40)                                                                         */
+  int32_t use_energy;                /* (1)                                                                          */
+  int32_t raw_energy;                /* 1: energy before pre-emphasis and window (1)                                 */
+  int32_t use_log_fbank;             /* must be 1                                                                    */
+  int32_t use_power;                 /* 1: power spectrum, 0: magnitude (1)                                          */
+  int32_t htk_compat;                /* must be 0                                                                    */
+  int32_t delta_order;               /* add-deltas --delta-order, 0 .. LVSR_FBANK_MAX_DELTA_ORDER (2)                */
+  int32_t delta_window;              /* add-deltas --delta-window, 1 .. LVSR_FBANK_MAX_DELTA_WINDOW (2)              */
+} lvsr_fbank_options;
+typedef struct lvsr_frontend lvsr_frontend;
+int lvsr_frontend_create(const lvsr_fbank_options* opts, lvsr_frontend** out);
+int lvsr_frontend_destroy(lvsr_frontend* f);
+/* frames of an utterance of num_samples samples (0 when shorter than one frame); -1 on a null handle */
+int64_t lvsr_frontend_num_frames(const lvsr_frontend* f, int64_t num_samples);
+/* D, the width of a feature row; -1 on a null handle */
+int lvsr_frontend_feature_dim(const lvsr_frontend* f);
+/* samples_dev [B, row_stride] float32 (16-byte aligned, row_stride a multiple of 4), lengths_host[b] <= row_stride the
+ * samples of row b; T >= every row's frame count.  Writes features_dev [T, B, D] and mask_dev [T, B] (float 0 / 1).
+ * cmvn_stats_dev: [2, D + 1] float64 on the device, or NULL for no CMVN. */
+int lvsr_frontend_compute(lvsr_frontend* f, const float* samples_dev, int64_t row_stride, const int64_t* lengths_host,
+                          int32_t B, int32_t T, float* features_dev, float* mask_dev, const double* cmvn_stats_dev,
+                          void* stream);
+/* Adds the sums of the frames of features_dev [T, B, D] whose mask_dev [T, B] entry is > 0.5 (NULL: every frame) to
+ * stats_dev [2, D + 1] float64: per-CTA float64 partial sums over fixed row ranges, reduced in a fixed order, so
+ * the result depends on the batch alone. */
+int lvsr_frontend_accumulate_cmvn(lvsr_frontend* f, const float* features_dev, const float* mask_dev, int32_t T,
+                                  int32_t B, double* stats_dev, void* stream);
+/* Normalises features_dev [T, B, D] in place by stats_dev, on the frames whose mask is > 0.5 (NULL: every frame). */
+int lvsr_frontend_apply_cmvn(lvsr_frontend* f, float* features_dev, const float* mask_dev, int32_t T, int32_t B,
+                             const double* stats_dev, void* stream);
+/* The dither's N(0, 1) draws for utterance rows 0 .. B-1 and frames 0 .. T-1: draws_dev [B, T, W] (unscaled). */
+int lvsr_frontend_dither_sample(lvsr_frontend* f, int32_t B, int32_t T, float* draws_dev, void* stream);
+
 /* Counters for bench.py: number of kernels this library launched since the last reset. */
 int64_t lvsr_launch_count(int reset);
 
@@ -474,7 +542,8 @@ int64_t lvsr_launch_count(int reset);
  * (libs/Theano/theano/compile/profiling.py:97).  Classes: "gemm", "bigru", "attention",
  * "window", "dense", "readout", "lm", "noise" (adaptive weight noise), "bottom" (the bottom MLP's forward, its
  * GEMMs included), "bottom_bwd" (its backward), "dropout" (the training dropout's forward and backward) and
- * "weight_noise" (the sample of regularization.noise) and "penalty" (the alignment penalty's gradient and sum).  lvsr_profile_read synchronises the device, returns the
+ * "weight_noise" (the sample of regularization.noise) and "penalty" (the alignment penalty's gradient and sum) and
+ * "fbank" (the two kernels of lvsr_frontend_compute).  lvsr_profile_read synchronises the device, returns the
  * summed milliseconds and launch count recorded since the last read of that class. */
 int lvsr_profile_enable(int on);
 int lvsr_profile_read(const char* kernel_class, double* total_ms, int64_t* count);
