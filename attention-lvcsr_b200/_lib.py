@@ -106,6 +106,16 @@ class LvsrLmFusion(C.Structure):
                 ("normalize_tot_weights", C.c_int32)]
 
 
+# name of lvsr_criterion (LVSR_CRITERION_*)
+CRITERIA = {"log_likelihood": 0, "mse_gain": 1, "mse_reward": 2}
+
+
+class LvsrCriterion(C.Structure):
+    """Mirror of ``lvsr_criterion`` (include/lvsr_b200.h)."""
+    _fields_ = [("name", C.c_int32), ("eos_label", C.c_int32), ("initial_output", C.c_int32),
+                ("min_reward", C.c_double)]
+
+
 # window_type of lvsr_fbank_options (LVSR_WINDOW_*)
 WINDOW_TYPES = {"povey": 0, "hamming": 1, "hanning": 2, "rectangular": 3}
 
@@ -153,6 +163,9 @@ SIGNATURES = {
     "lvsr_encoder_forward": (C.c_int, [_P, _P, _P, _I, _I, _P, _P, _P]),
     "lvsr_preprocess": (C.c_int, [_P, _P, _I, _I, _P, _P]),
     "lvsr_cost_matrix": (C.c_int, [_P, _P, _P, _I, _I, _P, _P, _I, _P, _P, _P, _P, _P, _P]),
+    "lvsr_model_set_criterion": (C.c_int, [_P, C.POINTER(LvsrCriterion)]),
+    "lvsr_cost_matrix_groundtruth": (C.c_int, [_P, _P, _P, _I, _I, _P, _P, _I, _P, _I, _P, _P, _P, _P, _P, _P]),
+    "lvsr_tle_matrices": (C.c_int, [_P, _P, _I, _P, _I, _I, _P, _P, _P]),
     "lvsr_initial_states": (C.c_int, [_P, _I, _I, _P, _P, _P, _P, _P, _P, _P]),
     "lvsr_logprobs": (C.c_int, [_P, _P, _P, _P, _I, _I, _P, _I, _P, _P, _P, _P, _P]),
     "lvsr_next_states": (C.c_int, [_P, _P, _P, _P, _I, _I, _P, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),

@@ -256,8 +256,13 @@ def _regularization(reg):
 
 
 def check_trainable_net(net):
-    """Refuse a config['net'] the training step cannot run: a stacked decoder (dec_stack > 1) decodes and scores,
-    but has no backward pass through the RecurrentStack."""
+    """Refuse a config['net'] the training step cannot run: a task-loss criterion (mse_gain / mse_reward) and a
+    stacked decoder (dec_stack > 1) decode and score, but have no backward pass."""
+    name = (net.get("criterion") or {}).get("name", "log_likelihood")
+    if name != "log_likelihood":
+        # the MSE backward and the exploration of RewardRegressionEmitter training are not built
+        raise NotImplementedError("attention-lvcsr_b200: training with criterion %r (task loss estimation scores and "
+                                  "decodes only)" % name)
     if net.get("dec_stack", 1) != 1:
         raise NotImplementedError("attention-lvcsr_b200: training with dec_stack=%d (a stacked decoder is inference "
                                   "only: cost, analyze, beam search and sampling)" % net["dec_stack"])
@@ -305,7 +310,7 @@ class GradientDescent(object):
             # with an LM the reference's emitter is LMEmitter, whose costs are the fused readout's: inference only
             raise NotImplementedError("attention-lvcsr_b200: training with a language model (shallow fusion is "
                                       "inference only)")
-        check_trainable_net(getattr(recognizer, "net", {}))
+        check_trainable_net(dict(getattr(recognizer, "net", {}), criterion=getattr(recognizer, "criterion", None)))
         self.recognizer = recognizer
         self.step_rule = step_rule if step_rule is not None else CompositeRule([Scale(), RemoveNotFinite(0.0)])
         self.adaptive_noise = None

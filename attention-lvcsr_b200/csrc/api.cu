@@ -264,6 +264,7 @@ ReadoutArgs readout_args(lvsr_model* m, int R, const float* merged) {
   r.Wo = m->P(std::string(GEN) + "/readout/post_merge/mlp/linear_0.W");
   r.bo = m->P(std::string(GEN) + "/readout/post_merge/mlp/linear_0.b");
   r.R = R; r.Cpm = c.post_merge_dim; r.pieces = c.maxout_pieces; r.V = c.num_phonemes; r.act = c.post_merge_activation;
+  r.tle = tle_criterion(m) ? 1 : 0;
   return r;
 }
 
@@ -469,6 +470,7 @@ int lvsr_model_destroy(lvsr_model* m) {
   for (const lvsr_model::DecLayer& d : m->dec)
     for (float* p : {d.Wd, d.Wff, d.bff, d.FF}) if (p) cudaFree(p);
   if (m->Wb1) cudaFree(m->Wb1);
+  if (m->tle_status) cudaFree(m->tle_status);
   if (m->stack.mem) cudaFree(m->stack.mem);
   if (m->status) cudaFree(m->status);
   if (m->enc_tiles) cudaFree(m->enc_tiles);
@@ -612,6 +614,7 @@ int lvsr_model_set_lm(lvsr_model* m, int32_t num_states, int32_t start, const in
   LVSR_CHECK(m && off && fusion && num_states > 0 && num_arcs >= 0 && (num_arcs == 0 || (label && next && weight)),
              "set_lm: bad arguments");
   LVSR_CHECK(start >= 0 && start < num_states, "set_lm: start state %d outside [0, %d)", start, num_states);
+  LVSR_CHECK(!tle_criterion(m), "set_lm: a task-loss criterion (mse_gain / mse_reward) takes no language model");
   LVSR_CHECK(off[0] == 0 && off[num_states] == num_arcs, "set_lm: arc offsets must run from 0 to num_arcs");
   const int V = m->cfg.num_phonemes;
   for (int32_t s = 0; s < num_states; ++s) {
@@ -987,7 +990,74 @@ int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int
 }
 }  // namespace lvsr
 
+// Workspace of tle_costs
+static size_t tle_ws_bytes(const lvsr_model* m, int Lg, int L, int B) {
+  return (size_t)3 * L * B * m->cfg.num_phonemes * sizeof(float) + tle_dist_ints(Lg, L, B) * sizeof(int) + 4096;
+}
+
+// RewardOp's matrices of prediction [L, B] against groundtruth [Lg, B] into rewards / gains [L, B, V] (from ws);
+// synchronises st and reports the first utterance whose groundtruth holds no eos.
+static int tle_run_matrices(lvsr_model* m, Arena& ws, const long long* groundtruth, int Lg, const long long* prediction,
+                            int L, int B, float* rewards, float* gains, cudaStream_t st) {
+  int* dist = ws.i32(tle_dist_ints(Lg, L, B));
+  LVSR_CHECK(dist, "out of device memory (task-loss distances)");
+  LVSR_CUDA_OK(cudaMemsetAsync(m->tle_status, 0xff, sizeof(unsigned), st));
+  if (int rc = tle_matrices(groundtruth, Lg, prediction, L, B, m->cfg.num_phonemes, m->criterion.eos_label, dist, rewards,
+                            gains, m->tle_status, st)) return rc;
+  unsigned h = LVSR_TLE_OK;
+  LVSR_CUDA_OK(cudaMemcpyAsync(&h, m->tle_status, sizeof(h), cudaMemcpyDeviceToHost, st));
+  LVSR_CUDA_OK(cudaStreamSynchronize(st));
+  LVSR_CHECK(h == LVSR_TLE_OK, "task loss estimation: the groundtruth of utterance %u does not end in eos (%d)", h,
+             m->criterion.eos_label);
+  return 0;
+}
+
+// The task-loss cost rows [L, B] from the emitter costs neg [L*B, V] of the prediction `labels`
+static int tle_costs(lvsr_model* m, Arena& ws, const long long* groundtruth, int Lg, const long long* labels,
+                     const float* lmask, int L, int B, const float* neg, float* costs, cudaStream_t st) {
+  const size_t n = (size_t)L * B * m->cfg.num_phonemes;
+  float* rewards = ws.f32(n);
+  float* gains = ws.f32(n);
+  LVSR_CHECK(rewards && gains, "out of device memory (task-loss matrices)");
+  if (int rc = tle_run_matrices(m, ws, groundtruth, Lg, labels, L, B, rewards, gains, st)) return rc;
+  const int loss = m->criterion.name == LVSR_CRITERION_MSE_GAIN ? LVSR_TLE_GAIN : LVSR_TLE_REWARD;
+  return tle_loss(loss, neg, rewards, gains, labels, lmask, L, B, m->cfg.num_phonemes, (float)m->criterion.min_reward,
+                  costs, st);
+}
+
 extern "C" {
+
+int lvsr_model_set_criterion(lvsr_model* m, const lvsr_criterion* cr) {
+  DeviceGuard device_guard(m);
+  LVSR_CHECK(m && cr, "set_criterion: bad arguments");
+  const int V = m->cfg.num_phonemes;
+  LVSR_CHECK(cr->name == LVSR_CRITERION_LOG_LIKELIHOOD || cr->name == LVSR_CRITERION_MSE_GAIN ||
+                 cr->name == LVSR_CRITERION_MSE_REWARD, "set_criterion: unknown criterion %d", cr->name);
+  if (cr->name != LVSR_CRITERION_LOG_LIKELIHOOD) {
+    LVSR_CHECK(!lm_attached(m), "set_criterion: a task-loss criterion takes no language model (detach it first)");
+    LVSR_CHECK(cr->eos_label >= 0 && cr->eos_label < V, "set_criterion: eos_label %d outside [0, %d)", cr->eos_label, V);
+    LVSR_CHECK(cr->initial_output >= 0 && cr->initial_output <= V, "set_criterion: initial_output %d outside [0, %d]",
+               cr->initial_output, V);
+    LVSR_CHECK(std::isfinite(cr->min_reward), "set_criterion: min_reward must be finite");
+    if (!m->tle_status) LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->tle_status), sizeof(unsigned)));
+  }
+  LVSR_CUDA_OK(cudaStreamSynchronize(m->stream));   // calls already queued keep the criterion they were issued under
+  m->criterion = *cr;
+  return 0;
+}
+
+int lvsr_tle_matrices(lvsr_model* m, const int64_t* groundtruth, int32_t Lg, const int64_t* prediction, int32_t L,
+                      int32_t B, float* rewards, float* gains, void* stream) {
+  DeviceGuard device_guard(m);
+  if (int rc = bind_stream(m, static_cast<cudaStream_t>(stream))) return rc;
+  LVSR_CHECK(groundtruth && prediction && rewards && gains && Lg > 0 && L > 0 && B > 0, "tle_matrices: bad arguments");
+  LVSR_CHECK(tle_criterion(m), "tle_matrices: the handle's criterion is log_likelihood (lvsr_model_set_criterion)");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  m->ws.reserve(tle_ws_bytes(m, Lg, L, B), st);
+  ArenaScope scope(m, st);
+  return tle_run_matrices(m, m->ws, reinterpret_cast<const long long*>(groundtruth), Lg,
+                          reinterpret_cast<const long long*>(prediction), L, B, rewards, gains, st);
+}
 
 int lvsr_encoded_length(const lvsr_model* m, int32_t T) {
   if (!m) return 0;
@@ -1031,12 +1101,24 @@ int lvsr_preprocess(lvsr_model* m, const float* attended, int32_t Tp, int32_t U,
 int lvsr_cost_matrix(lvsr_model* m, const float* attended, const float* attended_mask, int32_t Tp, int32_t B,
                      const int64_t* labels, const float* labels_mask, int32_t L, float* costs,
                      float* weights_out, float* energies_out, float* states_out, float* wavg_out, void* stream) {
+  return lvsr_cost_matrix_groundtruth(m, attended, attended_mask, Tp, B, labels, labels_mask, L, nullptr, 0, costs,
+                                      weights_out, energies_out, states_out, wavg_out, stream);
+}
+
+int lvsr_cost_matrix_groundtruth(lvsr_model* m, const float* attended, const float* attended_mask, int32_t Tp, int32_t B,
+                                 const int64_t* labels, const float* labels_mask, int32_t L, const int64_t* groundtruth,
+                                 int32_t Lg, float* costs, float* weights_out, float* energies_out, float* states_out,
+                                 float* wavg_out, void* stream) {
   DeviceGuard device_guard(m);
   if (int rc = bind_stream(m, static_cast<cudaStream_t>(stream))) return rc;
   if (int rc = check_ready(m)) return rc;
   LVSR_CHECK(attended && attended_mask && labels && costs && Tp > 0 && B > 0 && L > 0, "cost_matrix: bad arguments");
+  LVSR_CHECK(!groundtruth || Lg > 0, "cost_matrix: groundtruth without rows");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  m->ws.reserve(cost_ws_bytes(m, Tp, B, L) + (lm_attached(m) ? (size_t)L * B * m->cfg.num_phonemes * sizeof(float) : 0), st);
+  const bool tle = tle_criterion(m);
+  if (!groundtruth) { groundtruth = labels; Lg = L; }
+  m->ws.reserve(cost_ws_bytes(m, Tp, B, L) + (lm_attached(m) ? (size_t)L * B * m->cfg.num_phonemes * sizeof(float) : 0) +
+                    (tle ? tle_ws_bytes(m, Lg, L, B) : 0), st);
   ArenaScope scope(m, st);
   const lvsr_config& c = m->cfg;
   Arena& ws = m->ws;
@@ -1118,10 +1200,20 @@ int lvsr_cost_matrix(lvsr_model* m, const float* attended, const float* attended
                            nullptr, merged, acc);
     if (int rc = gemm_bias(b, st)) return rc;
     ReadoutArgs r = readout_args(m, R, merged);
-    r.labels = lab; r.lmask = labels_mask; r.costs_picked = costs;
     r.poison = scanned ? m->status : nullptr;
-    if (lm_add) lm_fuse(m, r, lm_add);
-    if (int rc = readout_costs(r, st)) return rc;
+    if (tle) {
+      // RewardRegressionEmitter.cost over the whole readouts (lvsr/bricks/__init__.py:135-184)
+      float* neg = ws.f32((size_t)R * c.num_phonemes);
+      LVSR_CHECK(neg, "out of device memory (task-loss readouts)");
+      r.costs_all = neg;
+      if (int rc = readout_costs(r, st)) return rc;
+      if (int rc = tle_costs(m, ws, reinterpret_cast<const long long*>(groundtruth), Lg, lab, labels_mask, L, B, neg,
+                             costs, st)) return rc;
+    } else {
+      r.labels = lab; r.lmask = labels_mask; r.costs_picked = costs;
+      if (lm_add) lm_fuse(m, r, lm_add);
+      if (int rc = readout_costs(r, st)) return rc;
+    }
   }
   if (states_out)
     LVSR_CUDA_OK(cudaMemcpyAsync(states_out, s_all, (size_t)L * B * S * sizeof(float), cudaMemcpyDeviceToDevice, st));
@@ -1135,9 +1227,8 @@ int lvsr_initial_states(lvsr_model* m, int32_t Tp, int32_t R, float* states, int
   if (int rc = check_ready(m)) return rc;
   LVSR_CHECK(states && outputs && wavg && weights && energies && step && Tp > 0 && R > 0, "initial_states: bad arguments");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const lvsr_config& c = m->cfg;
   if (int rc = broadcast_rows(states, initial_state_row(m), R, state_dim(m), st)) return rc;
-  if (int rc = fill_i64(reinterpret_cast<long long*>(outputs), R, c.num_phonemes, st)) return rc;   // recognizer.py:286
+  if (int rc = fill_i64(reinterpret_cast<long long*>(outputs), R, initial_output(m), st)) return rc;
   if (int rc = fill_f32(wavg, (long long)R * m->E, 0.f, st)) return rc;
   if (content_attention(m)) {             // B/bricks/attention.py:392-395: zero weights; no energies state
     if (int rc = fill_f32(weights, (long long)R * Tp, 0.f, st)) return rc;

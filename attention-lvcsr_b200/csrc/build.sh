@@ -12,7 +12,7 @@ if [ ! -f $STAMP ] || [ "$(cat $STAMP)" != "$FLAGS $*" ]; then
   echo "$FLAGS $*" > $STAMP
 fi
 OBJS=()
-for f in gemm gemm_tc bigru bigru_bwd attention decoder dec_scan bottom train noise stats search lm fbank api; do
+for f in gemm gemm_tc bigru bigru_bwd attention decoder dec_scan bottom train noise stats search lm fbank tle api; do
   stale=0
   for h in kernels.h common.cuh attention_row.cuh model.h train_kernels.cuh ../../include/lvsr_b200.h; do
     if [ "$h" -nt "$f.o" ]; then stale=1; fi

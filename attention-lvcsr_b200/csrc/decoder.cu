@@ -159,7 +159,8 @@ __device__ __forceinline__ void readout_fused(const ReadoutArgs& a, int r, int l
   }
 }
 
-// One warp per row.
+// One warp per row.  kTle: RewardRegressionEmitter.costs (lvsr/bricks/__init__.py:194-196), the costs are -readouts.
+template <bool kTle>
 __global__ void __launch_bounds__(256) readout_kernel(ReadoutArgs a) {
   extern __shared__ float sh[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -196,6 +197,20 @@ __global__ void __launch_bounds__(256) readout_kernel(ReadoutArgs a) {
     }
     logit[q] = s;
     vmax = fmaxf(vmax, s);
+  }
+  if constexpr (kTle) {
+    const long long lab = a.labels ? a.labels[r] : -1;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int v = lane + q * 32;
+      if (v < a.V) {
+        float cost = -logit[q];
+        if (a.poison && *a.poison != 0u) cost = __int_as_float(0x7fc00000);
+        if (a.costs_all) a.costs_all[(long long)r * a.V + v] = cost;
+        if (a.costs_picked && v == lab) a.costs_picked[r] = cost * (a.lmask ? a.lmask[r] : 1.f);
+      }
+    }
+    return;
   }
   vmax = warp_max(vmax);
   if (a.lm_add) {
@@ -336,7 +351,9 @@ int readout_costs(const ReadoutArgs& a, cudaStream_t stream) {
   LVSR_CHECK(a.pieces >= 1 && a.Cpm % a.pieces == 0, "readout: bad maxout pieces");
   const size_t smem = (size_t)8 * (a.Cpm / a.pieces) * sizeof(float);
   LVSR_CHECK(smem <= 48 * 1024, "readout: post_merge_dim too large");
-  readout_kernel<<<ceil_div(a.R, 8), 256, smem, stream>>>(a);
+  LVSR_CHECK(!(a.tle && a.lm_add), "readout: the task-loss emitter takes no language model");
+  if (a.tle) readout_kernel<true><<<ceil_div(a.R, 8), 256, smem, stream>>>(a);
+  else readout_kernel<false><<<ceil_div(a.R, 8), 256, smem, stream>>>(a);
   LVSR_LAUNCH_CHECK();
   return 0;
 }

@@ -200,8 +200,26 @@ struct ReadoutArgs {
   const float* lm_add;     // [R, V] or nullptr
   float lm_weight, am_beta;
   int norm_am, norm_lm, norm_tot;
+  // RewardRegressionEmitter (lvsr/bricks/__init__.py:119-202): the costs are -readouts, no log-softmax (lm_add unused)
+  int tle;
 };
 int readout_costs(const ReadoutArgs& a, cudaStream_t stream);
+
+// ---- tle.cu: task loss estimation, RewardOp + RewardRegressionEmitter.cost (lvsr/ops.py:236-294,
+// lvsr/error_rate.py:11-112, lvsr/bricks/__init__.py:135-184) --------------------------------------------------------
+// rewards / gains [L, B, V] of prediction [L, B] against groundtruth [Lg, B] (int64, symbols in [0, V)), one CTA per
+// utterance.  dist: tle_dist_ints(Lg, L, B) ints of scratch.  status: the lowest utterance whose groundtruth holds no
+// eos is atomicMin-ed into it (the caller sets it to LVSR_TLE_OK first); that utterance's rows are not written.
+enum : unsigned { LVSR_TLE_OK = 0xffffffffu };
+enum { LVSR_TLE_GAIN = 1, LVSR_TLE_REWARD = 2 };   // the mse_gain / mse_reward losses (LVSR_CRITERION_MSE_*)
+size_t tle_dist_ints(int Lg, int L, int B);
+int tle_matrices(const long long* groundtruth, int Lg, const long long* prediction, int L, int B, int V, int eos,
+                 int* dist, float* rewards, float* gains, unsigned* status, cudaStream_t stream);
+// costs [L, B] of the loss `criterion` (LVSR_TLE_*) from the emitter costs neg_readouts [L*B, V] (= -readouts), the
+// matrices above and prediction [L, B]; multiplied by lmask [L, B] when it is given.  One warp per utterance.
+int tle_loss(int criterion, const float* neg_readouts, const float* rewards, const float* gains,
+             const long long* prediction, const float* lmask, int L, int B, int V, float min_reward, float* costs,
+             cudaStream_t stream);
 
 // ---- lm.cu: FST language model states (float64 weights, at most LVSR_LM_MAX_STATES per hypothesis) --------------
 enum { LVSR_LM_TOO_MANY_STATES = 1, LVSR_LM_CLOSURE_CAP = 2, LVSR_LM_CYCLE = 3 };   // status word codes

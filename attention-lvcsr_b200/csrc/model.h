@@ -162,6 +162,9 @@ struct lvsr_model {
   int lm_start = 0;
   lvsr_lm_fusion lm_fusion = {};
   unsigned* lm_status = nullptr;
+  // ---- criterion (lvsr_model_set_criterion; read through tle_criterion and initial_output) ----
+  lvsr_criterion criterion = {LVSR_CRITERION_LOG_LIKELIHOOD, 0, 0, -1.0};
+  unsigned* tle_status = nullptr;   // device word of tle_matrices, allocated with the first task-loss criterion
   // The stream of the last call that enqueued work on the handle (bind_stream).  Both arenas, the device words above
   // and the parameter and optimizer buffers are only ever touched in this stream's order.
   cudaStream_t stream = nullptr;
@@ -401,6 +404,13 @@ ReadoutArgs readout_args(lvsr_model* m, int R, const float* merged);
 // language model (api.cu): the device view of the attached FST, the fusion fields of a readout, and the LM status
 // word read back after a synchronisation of st (an error return when a kernel reported one; the word is cleared)
 static inline bool lm_attached(const lvsr_model* m) { return m->lm_off != nullptr; }
+// task loss estimation (lvsr_model_set_criterion): RewardRegressionEmitter instead of SoftmaxEmitter
+static inline bool tle_criterion(const lvsr_model* m) { return m->criterion.name != LVSR_CRITERION_LOG_LIKELIHOOD; }
+// the emitter's initial output: num_phonemes for SoftmaxEmitter (lvsr/bricks/recognizer.py:286), the criterion's for
+// RewardRegressionEmitter (0 in the reference, lvsr/bricks/__init__.py:198-201)
+static inline int initial_output(const lvsr_model* m) {
+  return tle_criterion(m) ? m->criterion.initial_output : m->cfg.num_phonemes;
+}
 LmFst lm_fst(lvsr_model* m);
 void lm_fuse(const lvsr_model* m, ReadoutArgs& r, const float* lm_add);
 int lm_report(unsigned status);

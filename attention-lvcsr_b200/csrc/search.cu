@@ -155,7 +155,7 @@ int lvsr_beam_search_many(lvsr_model* m, const float* attended, const float* pre
   std::vector<Utt> utts(U);
   int longest = 0;
   for (int u = 0; u < U; ++u) {
-    utts[u].outs.assign(1, std::vector<int64_t>(1, (int64_t)V));          // initial symbol = num_phonemes (recognizer.py:286)
+    utts[u].outs.assign(1, std::vector<int64_t>(1, (int64_t)initial_output(m)));   // the emitter's initial output
     utts[u].costs.assign(1, std::vector<float>(1, 0.f));
     utts[u].max_length = max_length_host[u];
     longest = std::max(longest, utts[u].max_length);

@@ -621,6 +621,7 @@ int forward_backward(lvsr_model* m, const float* x, const float* mask, const int
   if (int rc = check_ready(m)) return rc;
   LVSR_CHECK(x && labels && cost_out && grads && T > 0 && B > 0 && L > 0, "train_cost_and_grads: bad arguments");
   LVSR_CHECK(!lm_attached(m), "train_cost_and_grads: shallow fusion is inference only (detach the language model)");
+  LVSR_CHECK(!tle_criterion(m), "train_cost_and_grads: the task-loss criteria (mse_gain / mse_reward) are inference only");
   return TrainStep{m, static_cast<cudaStream_t>(stream), labels, lmask, grads, gscale, B, L, lvsr_encoded_length(m, T),
                    drop, m->reg.penalty_coof}
       .run(x, mask, T, cost_out);

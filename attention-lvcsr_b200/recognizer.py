@@ -106,8 +106,12 @@ class SpeechRecognizer(object):
             # RecurrentStack of GatedRecurrent layers (lvsr/bricks/recognizer.py:250-259): one or two; two decode and
             # score only (GradientDescent refuses them)
             unsupported("dec_stack=%r (1 or 2)" % (dec_stack,))
-        if criterion is not None and criterion.get("name", "log_likelihood") != "log_likelihood":
-            unsupported("criterion %r" % criterion.get("name"))
+        criterion = dict(criterion) if criterion else dict(name="log_likelihood")
+        if criterion["name"] not in _lib.CRITERIA:
+            raise ValueError("Unknown criterion {}".format(criterion["name"]))       # recognizer.py:297
+        if lm and criterion["name"] != "log_likelihood":
+            # the reference would fuse the LM into RewardRegressionEmitter's raw readouts
+            unsupported("criterion %r with a language model" % criterion["name"])
         # SpeechBottom (lvsr/bricks/recognizer.py:105-157): an MLP of one Linear + activation per entry of dims, Tanh
         # when the activation is None; Identity when dims is empty
         bottom = dict(bottom or {})
@@ -129,7 +133,7 @@ class SpeechRecognizer(object):
         self.character_map = character_map
         self.lm = lm
         self._lm_tables = _lm.load(lm["path"], character_map, int(num_phonemes)) if lm else None
-        self.criterion = criterion or dict(name="log_likelihood")
+        self.criterion = criterion
         self.max_decoded_length_scale = max_decoded_length_scale
         self.rec_weights_init = None
         self.initial_states_init = None
@@ -281,7 +285,27 @@ class SpeechRecognizer(object):
             self._handle = h
             if self.lm:
                 self._attach_lm(lib, h)
+            if self.tle:
+                self._set_criterion(lib, h)
         return self._handle
+
+    @property
+    def tle(self):
+        """Task loss estimation (criterion mse_gain / mse_reward): RewardRegressionEmitter in place of SoftmaxEmitter."""
+        return self.criterion["name"] != "log_likelihood"
+
+    def _set_criterion(self, lib, h):
+        """RewardRegressionEmitter(criterion, eos_label, num_phonemes, min_reward) (lvsr/bricks/recognizer.py:291-295),
+        whose initial output is 0 (lvsr/bricks/__init__.py:198-201)."""
+        import ctypes as C
+        crit = _lib.LvsrCriterion(name=_lib.CRITERIA[self.criterion["name"]], eos_label=int(self.eos_label),
+                                  initial_output=0, min_reward=float(self.criterion.get("min_reward", -1.0)))
+        try:
+            _lib.check(lib.lvsr_model_set_criterion(h, C.byref(crit)))
+        except Exception:
+            lib.lvsr_model_destroy(h)
+            self._handle = None
+            raise
 
     def _attach_lm(self, lib, h):
         """LanguageModel + ShallowFusionReadout (lvsr/bricks/recognizer.py:322-338) on the handle."""
@@ -621,8 +645,10 @@ class SpeechRecognizer(object):
             if lo < 0 or hi >= self.net["num_phonemes"]:
                 raise ValueError("labels must lie in [0, %d): got %d..%d" % (self.net["num_phonemes"], lo, hi))
 
-    def cost_matrix(self, labels, labels_mask, attended, attended_mask, return_all=False):
-        """generator.cost_matrix (B/bricks/sequence_generators.py:319-326) on device tensors."""
+    def cost_matrix(self, labels, labels_mask, attended, attended_mask, return_all=False, groundtruth=None):
+        """generator.cost_matrix (B/bricks/sequence_generators.py:319-326) on device tensors.  Under task loss
+        estimation the labels are scored against ``groundtruth`` [Lg, B] (None: the labels themselves), as
+        get_cost_graph substitutes it (recognizer.py:423-450); log-likelihood ignores it."""
         torch = self._torch()
         lib, h = _lib.load(), self._require_ready()
         self._check_labels(labels)
@@ -642,6 +668,12 @@ class SpeechRecognizer(object):
             raise ValueError("cost_matrix: attended_mask must be [%d, %d], got %s" % (Tp, B, tuple(attm.shape)))
         if ym is not None and tuple(ym.shape) != (L, B):
             raise ValueError("cost_matrix: labels_mask must be [%d, %d], got %s" % (L, B, tuple(ym.shape)))
+        g = None
+        if groundtruth is not None and self.tle:
+            self._check_labels(groundtruth)
+            g = self._dev(groundtruth, torch.int64)
+            if g.dim() != 2 or g.shape[1] != B or g.shape[0] < 1:
+                raise ValueError("cost_matrix: groundtruth must be [Lg, %d], got %s" % (B, tuple(g.shape)))
         costs = torch.empty((L, B), dtype=torch.float32, device=self.device)
         extra = {}
         if return_all:
@@ -650,9 +682,9 @@ class SpeechRecognizer(object):
                          states=torch.empty((L, B, self.dim_state), dtype=torch.float32, device=self.device),
                          weighted_averages=torch.empty((L, B, self.dim_encoded), dtype=torch.float32,
                                                        device=self.device))
-        _lib.check(lib.lvsr_cost_matrix(
-            h, _ptr(att), _ptr(attm), Tp, B, _ptr(y), _ptr(ym), L, _ptr(costs),
-            _ptr(extra.get("weights")), _ptr(extra.get("energies")), _ptr(extra.get("states")),
+        _lib.check(lib.lvsr_cost_matrix_groundtruth(
+            h, _ptr(att), _ptr(attm), Tp, B, _ptr(y), _ptr(ym), L, _ptr(g), 0 if g is None else g.shape[0],
+            _ptr(costs), _ptr(extra.get("weights")), _ptr(extra.get("energies")), _ptr(extra.get("states")),
             _ptr(extra.get("weighted_averages")), self._stream()))
         if return_all:
             extra["costs"] = costs
@@ -737,11 +769,13 @@ class SpeechRecognizer(object):
         return costs
 
     def analyze(self, inputs, groundtruth, prediction=None):
-        """recognizer.py:452-494: one utterance, mask of ones, no label mask."""
+        """recognizer.py:452-494: one utterance, mask of ones, no label mask.  Under task loss estimation the
+        prediction is scored against the groundtruth."""
         rec = np.asarray(dict(inputs)["recordings"], dtype=np.float32)[:, None, :]
         labels = np.asarray(groundtruth if prediction is None else prediction, dtype=np.int64)[:, None]
         att, attm = self.encode(rec, np.ones(rec.shape[:2], dtype=np.float32))
-        r = self.cost_matrix(labels, None, att, attm, return_all=True)
+        r = self.cost_matrix(labels, None, att, attm, return_all=True,
+                             groundtruth=np.asarray(groundtruth, dtype=np.int64)[:, None])
         return [r["costs"][:, 0].cpu().numpy(), r["weights"][:, 0, :].cpu().numpy(),
                 r["energies"][:, 0, :].cpu().numpy()]
 
@@ -785,7 +819,9 @@ class SpeechRecognizer(object):
         feedback -> next state.  ``sample=True`` emits from the softmax like SoftmaxEmitter.emit
         (sequence_generators.py:772-778; a seeded Philox stream on the device instead of Theano's MRG stream, so
         draws differ from the reference while their distribution does not), ``sample=False`` emits the arg-max.
-        Returns dict(outputs [n,B] int64, costs [n,B] = -log p(emitted), states [n,B,dim_state], weights [n,B,T'])."""
+        Returns dict(outputs [n,B] int64, costs [n,B] = -log p(emitted), states [n,B,dim_state], weights [n,B,T']).
+        Under task loss estimation RewardRegressionEmitter emits the arg-max of the readouts whatever ``sample`` says,
+        and the costs are the emitted readouts (its cost, lvsr/bricks/__init__.py:185-192)."""
         if self.lm:
             # LMEmitter.emit returns zeros in the reference: generating with an LM is not defined there
             raise NotImplementedError("attention-lvcsr_b200: generate / sample with a language model")
@@ -803,11 +839,12 @@ class SpeechRecognizer(object):
         outs, costs, states, weights = [], [], [], []
         for _ in range(int(n_steps)):
             neglogp = self._logprobs(ctx, st)
-            if sample:
+            if sample and not self.tle:
                 y = torch.multinomial(torch.exp(-neglogp), 1, generator=gen)[:, 0]
             else:
                 y = neglogp.argmin(dim=1)
-            costs.append(neglogp.gather(1, y[:, None])[:, 0])
+            picked = neglogp.gather(1, y[:, None])[:, 0]
+            costs.append(-picked if self.tle else picked)
             st = self._next_states(ctx, st, y)
             outs.append(y)
             states.append(st["states"])

@@ -230,6 +230,40 @@ int lvsr_cost_matrix(lvsr_model* m, const float* attended_dev, const float* atte
                      int32_t L, float* costs_dev, float* weights_dev, float* energies_dev,
                      float* states_dev, float* weighted_averages_dev, void* stream);
 
+/* ---- training criterion: log-likelihood or task loss estimation --------------------------------------------------
+ * (lvsr/bricks/recognizer.py:285-297).  A handle starts with log_likelihood (SoftmaxEmitter, initial output
+ * num_phonemes).  mse_gain / mse_reward switch it to RewardRegressionEmitter (lvsr/bricks/__init__.py:119-202):
+ *   - every emitter cost (lvsr_logprobs, the beam search) is -readouts, without a log-softmax;
+ *   - lvsr_cost_matrix returns the loss rows of RewardOp's matrices (lvsr/ops.py:236-294) times the label mask:
+ *       mse_gain    sum_v (r - max(G, min_reward))^2
+ *       mse_reward  sum_v (r + sum_{1<=s<=t} r[s, y_s] - R)^2
+ *     with the labels as their own groundtruth (lvsr_cost_matrix_groundtruth takes another one);
+ *   - lvsr_initial_states and the beam search start from initial_output (the reference's 0).
+ * A groundtruth without eos_label makes the cost call fail naming the utterance; the call synchronises its stream to
+ * find out.  Task loss estimation takes no language model and has no training step: lvsr_model_set_criterion refuses a
+ * handle with an LM attached, lvsr_model_set_lm and lvsr_train_cost_and_grads refuse a handle with this criterion.
+ * Callers that must run on an older library detect the entry point by its symbol. */
+enum { LVSR_CRITERION_LOG_LIKELIHOOD = 0, LVSR_CRITERION_MSE_GAIN = 1, LVSR_CRITERION_MSE_REWARD = 2 };
+typedef struct {
+  int32_t name;                    /* LVSR_CRITERION_*                                           */
+  int32_t eos_label;               /* the groundtruth's end symbol, in [0, num_phonemes)         */
+  int32_t initial_output;          /* first output of generation and search, in [0, num_phonemes] */
+  double min_reward;               /* mse_gain's floor of the gains (reference default -1.0)     */
+} lvsr_criterion;
+int lvsr_model_set_criterion(lvsr_model* m, const lvsr_criterion* criterion);
+/* lvsr_cost_matrix with the prediction `labels` scored against groundtruth_dev [Lg, B] (int64; NULL: the labels) by
+ * the task-loss criterion, as SpeechRecognizer.analyze does (lvsr/bricks/recognizer.py:423-494).  Under
+ * log_likelihood the groundtruth is not read. */
+int lvsr_cost_matrix_groundtruth(lvsr_model* m, const float* attended_dev, const float* attended_mask_dev,
+                                 int32_t Tp, int32_t B, const int64_t* labels_dev, const float* labels_mask_dev,
+                                 int32_t L, const int64_t* groundtruth_dev, int32_t Lg, float* costs_dev,
+                                 float* weights_dev, float* energies_dev, float* states_dev,
+                                 float* weighted_averages_dev, void* stream);
+/* RewardOp alone: rewards_dev and gains_dev [L, B, num_phonemes] (float32, integer values) of prediction_dev [L, B]
+ * against groundtruth_dev [Lg, B], with the eos_label of the handle's criterion.  Synchronises the stream. */
+int lvsr_tle_matrices(lvsr_model* m, const int64_t* groundtruth_dev, int32_t Lg, const int64_t* prediction_dev,
+                      int32_t L, int32_t B, float* rewards_dev, float* gains_dev, void* stream);
+
 /* ---- alignment statistics of validation: weights_entropy and weights_penalty -------------------------------------
  * (lvsr/expressions.py:4-25 as lvsr/main.py:385-388 monitors them) of the weights lvsr_cost_matrix writes,
  * weights [L,B,T'], labels_mask [L,B] (NULL = all ones).  out_dev (float64, device):
