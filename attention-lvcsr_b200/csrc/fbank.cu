@@ -191,8 +191,7 @@ __global__ void __launch_bounds__(kThreads) fbank_frames_kernel(const FrameParam
       row[p.use_energy + m] = logf(fmaxf(acc, FLT_EPSILON));
     }
     if (p.use_energy && lane == 0) {
-      float le = logf(fmaxf(energy, p.raw_energy ? FLT_EPSILON : FLT_MIN));
-      row[0] = fmaxf(le, p.log_energy_floor);
+      row[0] = fmaxf(logf(fmaxf(energy, FLT_EPSILON)), p.log_energy_floor);
     }
     __syncwarp();                                 // fr and z are rewritten by the warp's next frame
   }

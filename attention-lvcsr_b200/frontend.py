@@ -146,6 +146,8 @@ def _device_stats(cmvn, device, D):
     """The stats of a GlobalCmvn (as they are on the device: no wait) or of a [2, D+1] array, on `device`."""
     torch = _torch()
     if isinstance(cmvn, GlobalCmvn):
+        if not cmvn.filled:
+            raise ValueError("cmvn stats: no frames yet (accumulate, or set stats with a frame count >= 1)")
         s = cmvn.device_stats
     else:
         s = np.asarray(cmvn, np.float64)
@@ -159,13 +161,16 @@ def _device_stats(cmvn, device, D):
 
 class GlobalCmvn(object):
     """Kaldi's global CMVN stats [2, D+1] float64 (row 0: column sums | frame count; row 1: sums of squares), kept on
-    the front end's device: accumulated over any number of batches, applied with norm_vars."""
+    the front end's device: accumulated over any number of batches, applied with norm_vars.  As Kaldi refuses a
+    frame count below 1, they are refused until `accumulate` has run or `stats` has been set with a count >= 1
+    (`filled`)."""
 
     def __init__(self, fbank, stats=None):
         torch = _torch()
         self.fbank = fbank
         D = fbank.feature_dim
         self.device_stats = torch.zeros((2, D + 1), dtype=torch.float64, device=fbank.device)
+        self.filled = False
         if stats is not None:
             self.stats = stats
 
@@ -179,6 +184,7 @@ class GlobalCmvn(object):
         if value.shape != tuple(self.device_stats.shape):
             raise ValueError("cmvn stats: %s expected, got %s" % (tuple(self.device_stats.shape), value.shape))
         self.device_stats.copy_(_torch().from_numpy(value))
+        self.filled = bool(value[0, -1] >= 1)
 
     def save(self, path):
         np.save(path, self.stats)
@@ -207,6 +213,7 @@ class GlobalCmvn(object):
             _lib.check(_lib.load().lvsr_frontend_accumulate_cmvn(
                 f._handle, features.data_ptr(), None if mask is None else mask.data_ptr(), T, B,
                 self.device_stats.data_ptr(), f._stream()))
+        self.filled = True
 
     def apply(self, features, mask=None):
         """Normalises features [T, B, D] in place on the frames whose mask is 1; returns them."""

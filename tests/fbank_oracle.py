@@ -6,8 +6,7 @@ GPU used (lvsr_frontend_dither_sample) as `draws` [frames, W], scaled by `dither
 """
 import numpy as np
 
-FLT_EPSILON = float(np.finfo(np.float32).eps)       # floor of the energy before the window and of the mel energies
-FLT_MIN = float(np.finfo(np.float32).tiny)          # floor of the energy after the window (raw_energy false)
+FLT_EPSILON = float(np.finfo(np.float32).eps)       # floor of the log energy (raw or windowed) and of the mel energies
 
 DEFAULTS = dict(sample_frequency=16000.0, frame_length=25.0, frame_shift=10.0, dither=1.0, remove_dc_offset=True,
                 preemphasis_coefficient=0.97, window_type="povey", round_to_power_of_two=True, snip_edges=True,
@@ -98,7 +97,7 @@ def process_frames(x, o, draws=None):
     pre[:, 0] -= p * fr[:, 0]
     win = pre * window(o)[None, :]
     if not o["raw_energy"]:
-        log_e = np.log(np.maximum((win ** 2).sum(1), FLT_MIN))
+        log_e = np.log(np.maximum((win ** 2).sum(1), FLT_EPSILON))
     spec = np.abs(np.fft.rfft(win, n=P, axis=1)) ** 2
     if not o["use_power"]:
         spec = np.sqrt(spec)

@@ -20,69 +20,10 @@ import pytest
 
 import fbank_oracle as F
 from compat_helpers import BASE_YAML, COMPAT
+import fbank_helpers as H
 from helpers import ROOT, O, make_recognizer, package
 
 pytestmark = pytest.mark.gpu
-
-LIN_TOL = 5e-6
-LOG_TOL = 5e-5
-FEAT_TOL = 2e-3
-
-
-def _torch():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("needs a CUDA device")
-    return torch
-
-
-def _signal(rng, n, fs=16000.0):
-    t = np.arange(n) / fs
-    x = rng.normal(0, 300, size=n)
-    for f in rng.uniform(100, 0.45 * fs, size=3):
-        x += rng.uniform(500, 4000) * np.sin(2 * np.pi * f * t + rng.uniform(0, 6.3))
-    return np.clip(np.round(x), -32768, 32767).astype(np.int16)
-
-
-def _waves(rng, lengths, fs=16000.0):
-    return [_signal(rng, n, fs) for n in lengths]
-
-
-def _fb(**kw):
-    pkg = package()
-    o = F.options(**kw)
-    opts = pkg.FbankOptions(**{k: v for k, v in o.items()})
-    return pkg.Fbank(opts), o
-
-
-def _check(feats, mask, waves, o, draws=None, stats=None, errs=None):
-    """The GPU's features [T, B, D] and mask against the oracle's; returns the worst errors."""
-    feats, mask = feats.cpu().numpy().astype(np.float64), mask.cpu().numpy()
-    T = feats.shape[0]
-    want, wmask = F.batch(waves, o, draws, stats, T=T)
-    assert np.array_equal(mask, wmask)
-    assert not feats[mask == 0].any(), "padded frames must be exactly 0"
-    errs = {} if errs is None else errs
-    e = float(np.abs(feats - want)[mask > 0].max())
-    errs["feat"] = max(errs.get("feat", 0.0), e)
-    assert e <= FEAT_TOL, ("features", e)
-    if stats is None:
-        ne = int(o["use_energy"])
-        for b, x in enumerate(waves):
-            st, lin = F.fbank(x, o, None if draws is None else draws[b], linear=True)
-            n = st.shape[0]
-            got = feats[:n, b, :st.shape[1]]
-            peak = lin.max(1, keepdims=True)
-            le = float((np.abs(np.exp(got[:, ne:]) - lin) / peak).max())
-            strong = lin >= 1e-4 * peak
-            ge = float(np.abs(got[:, ne:] - st[:, ne:])[strong].max())
-            errs["lin"] = max(errs.get("lin", 0.0), le)
-            errs["log"] = max(errs.get("log", 0.0), ge)
-            if ne:
-                errs["log"] = max(errs["log"], float(np.abs(got[:, 0] - st[:, 0]).max()))
-        assert errs["lin"] <= LIN_TOL and errs["log"] <= LOG_TOL, errs
-    return errs
-
 
 CONFIGS = [
     dict(),
@@ -101,42 +42,42 @@ CONFIGS = [
 @pytest.mark.parametrize("cmvn", [False, True], ids=["raw", "cmvn"])
 @pytest.mark.parametrize("kw", CONFIGS, ids=lambda kw: "-".join("%s=%s" % i for i in kw.items()) or "recipe")
 def test_features_match_oracle(kw, cmvn):
-    _torch()
-    fb, o = _fb(dither=0.0, **kw)
+    H.torch_or_skip()
+    fb, o = H.make_fb(dither=0.0, **kw)
     W, S, _ = F.frame_sizes(o)
     rng = np.random.RandomState(len(kw) * 7 + int(cmvn))
     lengths = [W, W + S - 1, W + 5 * S, W + 5 * S + 1, W + 17 * S - 1, 3 * W + 11, int(o["sample_frequency"])]
-    waves = _waves(rng, lengths, o["sample_frequency"])
+    waves = H.waves(rng, lengths, o["sample_frequency"])
     assert fb.feature_dim == (o["num_mel_bins"] + o["use_energy"]) * (o["delta_order"] + 1)
     assert [fb.num_frames(n) for n in lengths] == [F.num_frames(n, o) for n in lengths]
     stats = None
     if cmvn:
         stats = F.cmvn_stats([F.features(x, o) for x in waves])
     feats, mask = fb.compute(waves, cmvn=stats)
-    print(kw, cmvn, _check(feats, mask, waves, o, stats=stats))
+    print(kw, cmvn, H.check(feats, mask, waves, o, stats=stats))
 
 
 @pytest.mark.parametrize("B", [1, 7, 64, 129])
 def test_batches(B):
-    _torch()
-    fb, o = _fb(dither=0.0)
+    H.torch_or_skip()
+    fb, o = H.make_fb(dither=0.0)
     rng = np.random.RandomState(B)
     if B == 1:
         lengths = [400 + 1999 * 160]                        # 20 s: 2000 frames
     else:
         edges = [400, 399 + 160, 400 + 160, 401 + 160, 400 + 7 * 160 - 1, 400 + 7 * 160 + 1]
         lengths = (edges + list(rng.randint(400, 16000 * (3 if B < 100 else 1), size=B)))[:B]
-    waves = _waves(rng, lengths)
+    waves = H.waves(rng, lengths)
     feats, mask = fb.compute(waves, T=max(fb.num_frames(n) for n in lengths) + 3)
     assert feats.shape[0] == max(F.num_frames(n, o) for n in lengths) + 3
-    print(B, _check(feats, mask, waves, o))
+    print(B, H.check(feats, mask, waves, o))
 
 
 def test_tensor_input_and_short_utterance_refused():
-    torch = _torch()
-    fb, o = _fb(dither=0.0, delta_order=0)
+    torch = H.torch_or_skip()
+    fb, o = H.make_fb(dither=0.0, delta_order=0)
     rng = np.random.RandomState(3)
-    waves = _waves(rng, [4000, 2500, 3333])
+    waves = H.waves(rng, [4000, 2500, 3333])
     x = torch.zeros((3, 4001), dtype=torch.float32, device="cuda")        # row stride padded to 4004 inside
     for b, w in enumerate(waves):
         x[b, :len(w)] = torch.as_tensor(w.astype(np.float32))
@@ -148,31 +89,31 @@ def test_tensor_input_and_short_utterance_refused():
 
 
 def test_dither_is_replayable_and_keyed_by_seed():
-    torch = _torch()
-    fb, o = _fb(dither=1.0, seed=7)
+    torch = H.torch_or_skip()
+    fb, o = H.make_fb(dither=1.0, seed=7)
     rng = np.random.RandomState(9)
-    waves = _waves(rng, [5000, 400, 3210])
+    waves = H.waves(rng, [5000, 400, 3210])
     a, m = fb.compute(waves)
     b, _ = fb.compute(waves)
     assert torch.equal(a, b)
     draws = fb.dither_sample(len(waves), a.shape[0]).cpu().numpy()
     assert abs(draws.mean()) < 0.05 and abs(draws.std() - 1) < 0.05
-    print(_check(a, m, waves, o, draws=list(draws)))
-    other, _ = _fb(dither=1.0, seed=8)
+    print(H.check(a, m, waves, o, draws=list(draws)))
+    other, _ = H.make_fb(dither=1.0, seed=8)
     c, _ = other.compute(waves)
     assert not torch.equal(a, c)
-    quiet, _ = _fb(dither=0.0)
+    quiet, _ = H.make_fb(dither=0.0)
     d1, _ = quiet.compute(waves)
     d2, _ = quiet.compute(waves)
     assert torch.equal(d1, d2)
 
 
 def test_cmvn_accumulation_and_application():
-    torch = _torch()
+    torch = H.torch_or_skip()
     pkg = package()
-    fb, o = _fb(dither=0.0)
+    fb, o = H.make_fb(dither=0.0)
     rng = np.random.RandomState(11)
-    waves = _waves(rng, [8000, 400, 5000, 12345, 999])
+    waves = H.waves(rng, [8000, 400, 5000, 12345, 999])
     feats, mask = fb.compute(waves)
     cmvn = pkg.GlobalCmvn(fb)
     cmvn.accumulate(feats, mask)
@@ -201,10 +142,10 @@ def test_cmvn_accumulation_and_application():
 
 
 def test_compute_on_a_non_blocking_stream():
-    torch = _torch()
-    fb, o = _fb(dither=1.0, seed=3)
+    torch = H.torch_or_skip()
+    fb, o = H.make_fb(dither=1.0, seed=3)
     rng = np.random.RandomState(12)
-    waves = _waves(rng, [16000, 7000, 401])
+    waves = H.waves(rng, [16000, 7000, 401])
     want, wm = fb.compute(waves)
     cmvn = package().GlobalCmvn(fb)
     s = torch.cuda.Stream()
@@ -220,10 +161,10 @@ def test_compute_on_a_non_blocking_stream():
 
 def test_end_to_end_recognizer_on_gpu_features():
     """The CUDA features go straight into a 123-feature recognizer (wsj_jan_new-shaped, small)."""
-    _torch()
-    fb, o = _fb(dither=0.0)
+    H.torch_or_skip()
+    fb, o = H.make_fb(dither=0.0)
     rng = np.random.RandomState(21)
-    waves = _waves(rng, [16000, 9000, 12000])
+    waves = H.waves(rng, [16000, 9000, 12000])
     raw, _ = fb.compute(waves)
     stats = F.cmvn_stats([F.features(x, o) for x in waves])
     feats, mask = fb.compute(waves, cmvn=stats)
@@ -263,14 +204,14 @@ def _write_wav(path, x, fs=16000):
 
 
 def test_featurize_writes_the_oracle_features_and_compat_searches_them(tmp_path, capsys):
-    _torch()
+    H.torch_or_skip()
     rng = np.random.RandomState(31)
     texts = {"train": ["abc", "bad", "cab", "dab", "a", "ccd"], "valid": ["ab", "dc"]}
     waves = {}
     for part, ts in texts.items():
         lines, waves[part] = [], []
         for i, t in enumerate(ts):
-            x = _signal(rng, int(rng.randint(4000, 9000)))
+            x = H.signal(rng, int(rng.randint(4000, 9000)))
             waves[part].append(x)
             _write_wav(str(tmp_path / ("%s%d.wav" % (part, i))), x)
             lines.append("%s_%d %s%d.wav %s" % (part, i, part, i, t))
@@ -287,7 +228,7 @@ def test_featurize_writes_the_oracle_features_and_compat_searches_them(tmp_path,
     for part in texts:
         want = np.concatenate([F.apply_cmvn(F.features(x, o), stats) for x in waves[part]])
         assert z[part + "_features"].shape == want.shape == (len(want), 123)
-        assert np.abs(z[part + "_features"] - want).max() <= FEAT_TOL
+        assert np.abs(z[part + "_features"] - want).max() <= H.FEAT_TOL
         assert z[part + "_labels"].tolist() == ["abcd".index(c) for t in texts[part] for c in t]
     if COMPAT not in sys.path:
         sys.path.insert(0, COMPAT)
