@@ -208,6 +208,7 @@ SIGNATURES = {
     "lvsr_frontend_apply_cmvn": (C.c_int, [_P, _P, _P, _I, _I, _P, _P]),
     "lvsr_frontend_dither_sample": (C.c_int, [_P, _I, _I, _P, _P]),
     "lvsr_launch_count": (C.c_int64, [C.c_int]),
+    "lvsr_device_bytes": (C.c_int64, []),
     "lvsr_profile_enable": (C.c_int, [C.c_int]),
     "lvsr_profile_read": (C.c_int, [C.c_char_p, C.POINTER(C.c_double), C.POINTER(C.c_int64)]),
 }

@@ -12,6 +12,7 @@
 
 #include <algorithm>
 #include <map>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -21,6 +22,7 @@ namespace lvsr {
 
 thread_local std::string g_last_error;
 long long g_launch_count = 0;
+std::atomic<long long> g_device_bytes{0};
 
 int set_error(const char* fmt, ...) {
   char buf[1024];
@@ -231,10 +233,10 @@ static int transition(lvsr_model* m, int R, const float* states, const float* ct
     const lvsr_model::DecLayer& in = m->dec[l];
     const float* s = states + (size_t)l * C;
     DenseArgs g = {};
-    g.op[0] = {ctx, m->E, m->E, in.Wd, 3 * C};
+    g.op[0] = {ctx, m->E, m->E, in.Wd.get(), 3 * C};
     if (l == 1) g.op[1] = {next_states, C, S, m->stack.F, 3 * C};
     g.op[l + 1] = {s, C, S, m->P(dec_gru(m, l) + ".state_to_gates"), 2 * C};   // the layer's own state comes last
-    g.add = in.FF; g.arow = outputs; g.add_rows = c.num_phonemes + 1; g.R = R; g.N = 3 * C; g.mode = DENSE_GATES;
+    g.add = in.FF.get(); g.arow = outputs; g.add_rows = c.num_phonemes + 1; g.R = R; g.N = 3 * C; g.mode = DENSE_GATES;
     g.s = s; g.ld_s = S; g.z = z; g.hr = hr; g.ai = ai; g.C = C;
     if (int rc = dense_step(g, st)) return rc;
     DenseArgs k = {};
@@ -270,10 +272,10 @@ ReadoutArgs readout_args(lvsr_model* m, int R, const float* merged) {
 
 LmFst lm_fst(lvsr_model* m) {
   LmFst f = {};
-  f.off = m->lm_off; f.label = m->lm_label; f.next = m->lm_next; f.weight = m->lm_weight;
+  f.off = m->lm_off.get(); f.label = m->lm_label.get(); f.next = m->lm_next.get(); f.weight = m->lm_weight.get();
   f.start = m->lm_start; f.V = m->cfg.num_phonemes;
   f.no_transition_cost = (float)m->lm_fusion.no_transition_cost;
-  f.status = m->lm_status;
+  f.status = m->lm_status.get();
   return f;
 }
 
@@ -297,9 +299,9 @@ int lm_report(unsigned status) {
 // Synchronises st and turns the LM status word into an error return (clearing it).
 static int lm_sync_status(lvsr_model* m, cudaStream_t st) {
   unsigned h = 0;
-  LVSR_CUDA_OK(cudaMemcpyAsync(&h, m->lm_status, sizeof(h), cudaMemcpyDeviceToHost, st));
+  LVSR_CUDA_OK(cudaMemcpyAsync(&h, m->lm_status.get(), sizeof(h), cudaMemcpyDeviceToHost, st));
   LVSR_CUDA_OK(cudaStreamSynchronize(st));
-  if (h) LVSR_CUDA_OK(cudaMemsetAsync(m->lm_status, 0, sizeof(unsigned), st));
+  if (h) LVSR_CUDA_OK(cudaMemsetAsync(m->lm_status.get(), 0, sizeof(unsigned), st));
   return lm_report(h);
 }
 
@@ -339,6 +341,7 @@ int64_t lvsr_launch_count(int reset) {
   if (reset) g_launch_count = 0;
   return v;
 }
+int64_t lvsr_device_bytes(void) { return g_device_bytes.load(); }
 
 int lvsr_profile_enable(int on) {
   g_prof_on = on != 0;
@@ -412,7 +415,7 @@ int lvsr_model_create_encoder(const lvsr_config* cfg, const lvsr_bottom_config* 
   int dev_count = 0;
   LVSR_CUDA_OK(cudaGetDeviceCount(&dev_count));
   LVSR_CHECK(dev_count > 0, "no CUDA device: the GPU path has no CPU fallback");
-  lvsr_model* m = new lvsr_model();
+  std::unique_ptr<lvsr_model> m(new lvsr_model());      // deleted with every buffer it holds on a failed return
   m->cfg = *cfg;
   m->ndir = bidir ? 2 : 1;
   if (bottom && bottom->num_layers > 0) m->bottom = *bottom;
@@ -430,8 +433,8 @@ int lvsr_model_create_encoder(const lvsr_config* cfg, const lvsr_bottom_config* 
     c.prior_before = c.prior_after = 0.0;
   }
   LVSR_CUDA_OK(cudaGetDevice(&m->device));
-  m->E = encoder_output_dim(m, cfg->num_layers - 1);
-  build_param_table(m);
+  m->E = encoder_output_dim(m.get(), cfg->num_layers - 1);
+  build_param_table(m.get());
   int64_t total = 0;
   for (auto& p : m->params) {
     p.offset = total;
@@ -439,21 +442,16 @@ int lvsr_model_create_encoder(const lvsr_config* cfg, const lvsr_bottom_config* 
   }
   m->flat_count = total;
   {
-    cudaError_t e = cudaMalloc(reinterpret_cast<void**>(&m->flat), (size_t)total * sizeof(float));
-    if (e != cudaSuccess) {
-      lvsr_model_destroy(m);
+    cudaError_t e = m->flat.alloc((size_t)total * sizeof(float));
+    if (e != cudaSuccess)
       return set_error("cudaMalloc(parameters, %lld floats) failed: %s", (long long)total, cudaGetErrorString(e));
-    }
-    cudaMemset(m->flat, 0, (size_t)total * sizeof(float));
+    cudaMemset(m->flat.get(), 0, (size_t)total * sizeof(float));
   }
-  for (auto& p : m->params) p.dev = m->flat + p.offset;
-  if (cudaMalloc(reinterpret_cast<void**>(&m->status), 64) != cudaSuccess) {
-    lvsr_model_destroy(m);
-    return set_error("cudaMalloc(status) failed");
-  }
-  cudaMemset(m->status, 0, 64);
+  for (auto& p : m->params) p.dev = m->flat.get() + p.offset;
+  if (m->status.alloc(64) != cudaSuccess) return set_error("cudaMalloc(status) failed");
+  cudaMemset(m->status.get(), 0, 64);
   cudaDeviceSynchronize();      // the zeroed buffers are in place before a call on any stream reads them
-  *out = m;
+  *out = m.release();
   return 0;
 }
 
@@ -461,32 +459,6 @@ int lvsr_model_destroy(lvsr_model* m) {
   if (!m) return 0;
   DeviceGuard device_guard(m);
   cudaDeviceSynchronize();
-  if (m->flat) cudaFree(m->flat);
-  for (float* p : m->Wcat) if (p) cudaFree(p);
-  for (float* p : m->bcat) if (p) cudaFree(p);
-  for (TcWeights& t : m->Wcat_tc) if (t.mem) cudaFree(t.mem);
-  for (TcWeights& t : m->bottom_tc) if (t.mem) cudaFree(t.mem);
-  if (m->Wp_tc.mem) cudaFree(m->Wp_tc.mem);
-  for (const lvsr_model::DecLayer& d : m->dec)
-    for (float* p : {d.Wd, d.Wff, d.bff, d.FF}) if (p) cudaFree(p);
-  if (m->Wb1) cudaFree(m->Wb1);
-  if (m->tle_status) cudaFree(m->tle_status);
-  if (m->stack.mem) cudaFree(m->stack.mem);
-  if (m->status) cudaFree(m->status);
-  if (m->enc_tiles) cudaFree(m->enc_tiles);
-  if (m->enc_claims) cudaFree(m->enc_claims);
-  if (m->opt_velocity) cudaFree(m->opt_velocity);
-  if (m->opt_ms_step) cudaFree(m->opt_ms_step);
-  if (m->opt_ms_dx) cudaFree(m->opt_ms_dx);
-  if (m->opt_scratch) cudaFree(m->opt_scratch);
-  if (m->opt_desc) cudaFree(m->opt_desc);
-  if (m->clip) cudaFree(m->clip);
-  if (m->align_mem) cudaFree(m->align_mem);
-  lvsr_model_clear_lm(m);
-  noise_free(m);
-  reg_free(m);
-  m->tws.destroy();
-  m->ws.destroy();
   delete m;
   return 0;
 }
@@ -495,7 +467,7 @@ int lvsr_model_status(lvsr_model* m, int32_t* launch_status, int64_t* stepwise_f
   DeviceGuard device_guard(m);
   LVSR_CHECK(m && launch_status, "null argument");
   unsigned hst = 0;
-  if (int rc = copy_on_handle(m, &hst, m->status, sizeof(hst), cudaMemcpyDeviceToHost)) return rc;   // after the handle's work
+  if (int rc = copy_on_handle(m, &hst, m->status.get(), sizeof(hst), cudaMemcpyDeviceToHost)) return rc;   // after the handle's work
   *launch_status = (int32_t)hst;
   if (stepwise_fallbacks) *stepwise_fallbacks = m->dec_fallbacks;
   return 0;
@@ -529,7 +501,7 @@ int lvsr_model_encoder_overlap(lvsr_model* m, int32_t layer, int32_t out[3]) {
   if (out[0]) {
     int tiles[2];
     LVSR_CUDA_OK(cudaDeviceSynchronize());
-    LVSR_CUDA_OK(cudaMemcpy(tiles, m->enc_tiles + 2 * layer, sizeof(tiles), cudaMemcpyDeviceToHost));
+    LVSR_CUDA_OK(cudaMemcpy(tiles, m->enc_tiles.get() + 2 * layer, sizeof(tiles), cudaMemcpyDeviceToHost));
     out[1] = tiles[0];
     out[2] = tiles[1];
   }
@@ -540,13 +512,13 @@ int lvsr_model_encoder_overlap_claims(lvsr_model* m, int32_t layer, int32_t* out
   LVSR_CHECK(m && out, "null argument");
   LVSR_CHECK(layer >= 1 && layer < m->cfg.num_layers && m->enc_overlap[layer],
              "encoder_overlap_claims: layer %d did not overlap in the last encoder forward", layer);
-  const size_t end = layer + 1 < m->cfg.num_layers ? m->enc_claims_off[layer + 1] : m->enc_claims_cap;
+  const size_t end = layer + 1 < m->cfg.num_layers ? m->enc_claims_off[layer + 1] : m->enc_claims.bytes() / sizeof(int);
   const size_t n = end - m->enc_claims_off[layer];
   LVSR_CHECK(count >= 0 && (size_t)count <= n, "encoder_overlap_claims: %lld ints asked, layer %d has %zu",
              (long long)count, layer, n);
   DeviceGuard device_guard(m);
   LVSR_CUDA_OK(cudaDeviceSynchronize());
-  LVSR_CUDA_OK(cudaMemcpy(out, m->enc_claims + m->enc_claims_off[layer], (size_t)count * sizeof(int), cudaMemcpyDeviceToHost));
+  LVSR_CUDA_OK(cudaMemcpy(out, m->enc_claims.get() + m->enc_claims_off[layer], (size_t)count * sizeof(int), cudaMemcpyDeviceToHost));
   return 0;
 }
 
@@ -569,7 +541,7 @@ int lvsr_model_param_offset(const lvsr_model* m, int i, int64_t* offset, int64_t
   if (count) *count = m->params[i].count;
   return 0;
 }
-float* lvsr_model_flat_params(lvsr_model* m) { return m ? m->flat : nullptr; }
+float* lvsr_model_flat_params(lvsr_model* m) { return m ? m->flat.get() : nullptr; }
 int lvsr_model_set_param(lvsr_model* m, const char* name, const float* host, int64_t count) {
   DeviceGuard device_guard(m);
   LVSR_CHECK(m && name && host, "null argument");
@@ -599,12 +571,8 @@ int lvsr_model_finalize(lvsr_model* m) {
 int lvsr_model_clear_lm(lvsr_model* m) {
   DeviceGuard device_guard(m);
   LVSR_CHECK(m, "null model");
-  if (m->lm_off) {
-    LVSR_CUDA_OK(cudaDeviceSynchronize());       // a search or cost call may still read the tables
-    cudaFree(m->lm_off); cudaFree(m->lm_label); cudaFree(m->lm_next); cudaFree(m->lm_weight);
-  }
-  if (m->lm_status) cudaFree(m->lm_status);
-  m->lm_off = nullptr; m->lm_label = m->lm_next = nullptr; m->lm_weight = nullptr; m->lm_status = nullptr;
+  if (m->lm_off) LVSR_CUDA_OK(cudaDeviceSynchronize());       // a search or cost call may still read the tables
+  m->lm_off.reset(); m->lm_label.reset(); m->lm_next.reset(); m->lm_weight.reset(); m->lm_status.reset();
   return 0;
 }
 
@@ -626,23 +594,33 @@ int lvsr_model_set_lm(lvsr_model* m, int32_t num_states, int32_t start, const in
                  "set_lm: the arcs of state %d are not sorted by (label, next state)", s);
     }
   }
-  if (int rc = lvsr_model_clear_lm(m)) return rc;
+  // the new tables are filled before the attached ones are replaced: a failed call leaves the handle as it was
   const size_t na = (size_t)std::max<int64_t>(num_arcs, 1);
-  LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->lm_status), sizeof(unsigned)));
-  LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->lm_off), (size_t)(num_states + 1) * sizeof(long long)));
-  LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->lm_label), na * sizeof(int)));
-  LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->lm_next), na * sizeof(int)));
-  LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->lm_weight), na * sizeof(float)));
+  DeviceBuffer<unsigned> lm_status;
+  DeviceBuffer<long long> lm_off;
+  DeviceBuffer<int> lm_label, lm_next;
+  DeviceBuffer<float> lm_weight;
+  LVSR_CUDA_OK(lm_status.alloc(sizeof(unsigned)));
+  LVSR_CUDA_OK(lm_off.alloc((size_t)(num_states + 1) * sizeof(long long)));
+  LVSR_CUDA_OK(lm_label.alloc(na * sizeof(int)));
+  LVSR_CUDA_OK(lm_next.alloc(na * sizeof(int)));
+  LVSR_CUDA_OK(lm_weight.alloc(na * sizeof(float)));
   // on the handle's stream, complete before the host tables may go away
   cudaStream_t st = m->stream;
-  LVSR_CUDA_OK(cudaMemsetAsync(m->lm_status, 0, sizeof(unsigned), st));
-  LVSR_CUDA_OK(cudaMemcpyAsync(m->lm_off, off, (size_t)(num_states + 1) * sizeof(long long), cudaMemcpyHostToDevice, st));
+  LVSR_CUDA_OK(cudaMemsetAsync(lm_status.get(), 0, sizeof(unsigned), st));
+  LVSR_CUDA_OK(cudaMemcpyAsync(lm_off.get(), off, (size_t)(num_states + 1) * sizeof(long long), cudaMemcpyHostToDevice, st));
   if (num_arcs > 0) {
-    LVSR_CUDA_OK(cudaMemcpyAsync(m->lm_label, label, (size_t)num_arcs * sizeof(int), cudaMemcpyHostToDevice, st));
-    LVSR_CUDA_OK(cudaMemcpyAsync(m->lm_next, next, (size_t)num_arcs * sizeof(int), cudaMemcpyHostToDevice, st));
-    LVSR_CUDA_OK(cudaMemcpyAsync(m->lm_weight, weight, (size_t)num_arcs * sizeof(float), cudaMemcpyHostToDevice, st));
+    LVSR_CUDA_OK(cudaMemcpyAsync(lm_label.get(), label, (size_t)num_arcs * sizeof(int), cudaMemcpyHostToDevice, st));
+    LVSR_CUDA_OK(cudaMemcpyAsync(lm_next.get(), next, (size_t)num_arcs * sizeof(int), cudaMemcpyHostToDevice, st));
+    LVSR_CUDA_OK(cudaMemcpyAsync(lm_weight.get(), weight, (size_t)num_arcs * sizeof(float), cudaMemcpyHostToDevice, st));
   }
   LVSR_CUDA_OK(cudaStreamSynchronize(st));
+  if (int rc = lvsr_model_clear_lm(m)) return rc;
+  m->lm_status = std::move(lm_status);
+  m->lm_off = std::move(lm_off);
+  m->lm_label = std::move(lm_label);
+  m->lm_next = std::move(lm_next);
+  m->lm_weight = std::move(lm_weight);
   m->lm_start = start;
   m->lm_fusion = *fusion;
   return 0;
@@ -681,14 +659,14 @@ static int pack_tc_weights(TcWeights& tw, const float* W, int K, int N, cudaStre
   if (!tw.mem) {
     if (gemm_f16_supported(128, N, K)) {
       const size_t plane = (size_t)N * K * sizeof(__half);
-      LVSR_CUDA_OK(cudaMalloc(&tw.mem, 2 * plane + (size_t)N * sizeof(int)));
-      tw.head = static_cast<__half*>(tw.mem);
-      tw.tail = reinterpret_cast<__half*>(static_cast<char*>(tw.mem) + plane);
-      tw.ew = reinterpret_cast<int*>(static_cast<char*>(tw.mem) + 2 * plane);
+      LVSR_CUDA_OK(tw.mem.alloc(2 * plane + (size_t)N * sizeof(int)));
+      tw.head = reinterpret_cast<__half*>(tw.mem.get());
+      tw.tail = reinterpret_cast<__half*>(tw.mem.get() + plane);
+      tw.ew = reinterpret_cast<int*>(tw.mem.get() + 2 * plane);
     } else if (gemm_tc_supported(128, N, K)) {
       const size_t plane = (size_t)N * gemm_tc_kpad(K);
-      LVSR_CUDA_OK(cudaMalloc(&tw.mem, 2 * plane * sizeof(float)));
-      tw.hi = static_cast<float*>(tw.mem);
+      LVSR_CUDA_OK(tw.mem.alloc(2 * plane * sizeof(float)));
+      tw.hi = reinterpret_cast<float*>(tw.mem.get());
       tw.lo = tw.hi + plane;
     } else {
       return 0;
@@ -700,39 +678,44 @@ static int pack_tc_weights(TcWeights& tw, const float* W, int K, int N, cudaStre
 
 int finalize_on_stream(lvsr_model* m, cudaStream_t st, bool synchronise) {
   const lvsr_config& c = m->cfg;
-  if (m->Wcat.empty()) {
+  if (m->Wcat.empty()) {       // the first finalize: the whole group, or (on a failed allocation) none of it
+    std::vector<DeviceBuffer<float>> Wcat(c.num_layers), bcat(c.num_layers);
     for (int l = 0; l < c.num_layers; ++l) {
       const ForkLayout f = encoder_fork(m, l, 0);       // Wcat[l] [rows, ld], bcat[l] [ld]
-      float *W = nullptr, *b = nullptr;
-      LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&W), (size_t)f.rows * f.ld * sizeof(float)));
-      LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&b), (size_t)f.ld * sizeof(float)));
-      m->Wcat.push_back(W);
-      m->bcat.push_back(b);
+      LVSR_CUDA_OK(Wcat[l].alloc((size_t)f.rows * f.ld * sizeof(float)));
+      LVSR_CUDA_OK(bcat[l].alloc((size_t)f.ld * sizeof(float)));
     }
     const int C = c.dim_dec;
+    lvsr_model::DecLayer dec[2];
     for (int l = 0; l < c.dec_stack; ++l) {
-      lvsr_model::DecLayer& d = m->dec[l];
-      LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&d.Wd), (size_t)m->E * 3 * C * sizeof(float)));
-      LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&d.Wff), (size_t)c.dim_feedback * 3 * C * sizeof(float)));
-      LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&d.bff), (size_t)3 * C * sizeof(float)));
-      LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&d.FF), (size_t)(c.num_phonemes + 1) * 3 * C * sizeof(float)));
+      lvsr_model::DecLayer& d = dec[l];
+      LVSR_CUDA_OK(d.Wd.alloc((size_t)m->E * 3 * C * sizeof(float)));
+      LVSR_CUDA_OK(d.Wff.alloc((size_t)c.dim_feedback * 3 * C * sizeof(float)));
+      LVSR_CUDA_OK(d.bff.alloc((size_t)3 * C * sizeof(float)));
+      LVSR_CUDA_OK(d.FF.alloc((size_t)(c.num_phonemes + 1) * 3 * C * sizeof(float)));
     }
-    LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->Wb1), (size_t)(m->E + C) * 3 * C * sizeof(float)));
+    DeviceBuffer<float> Wb1;
+    LVSR_CUDA_OK(Wb1.alloc((size_t)(m->E + C) * 3 * C * sizeof(float)));
+    lvsr_model::Stack s;
     if (c.dec_stack == 2) {
-      lvsr_model::Stack& s = m->stack;
       const size_t n[4] = {(size_t)2 * C * c.dim_matcher, (size_t)2 * C * c.post_merge_dim, (size_t)2 * C,
                            (size_t)C * 3 * C};
       size_t total = 0;
       for (size_t k : n) total += (k + 63) & ~(size_t)63;      // 256-byte aligned pieces
-      LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&s.mem), total * sizeof(float)));
+      LVSR_CUDA_OK(s.mem.alloc(total * sizeof(float)));
       float** piece[4] = {&s.Ws, &s.Wm, &s.h0, &s.F};
-      float* p = s.mem;
+      float* p = s.mem.get();
       for (int i = 0; i < 4; ++i) { *piece[i] = p; p += (n[i] + 63) & ~(size_t)63; }
     }
+    m->Wcat = std::move(Wcat);
+    m->bcat = std::move(bcat);
+    for (int l = 0; l < 2; ++l) m->dec[l] = std::move(dec[l]);
+    m->Wb1 = std::move(Wb1);
+    m->stack = std::move(s);
   }
   for (int l = 0; l < c.num_layers; ++l)
     for (int dir = 0; dir < encoder_dirs(m); ++dir)
-      if (int rc = fork_copy(m, encoder_fork(m, l, dir), m->Wcat[l], m->bcat[l], nullptr, st)) return rc;
+      if (int rc = fork_copy(m, encoder_fork(m, l, dir), m->Wcat[l].get(), m->bcat[l].get(), nullptr, st)) return rc;
   const int C = c.dim_dec, Cfb = c.dim_feedback, V = c.num_phonemes;
   const std::string g = GEN, t = TR;
   // decoder-side packing, per layer: gate columns first (update | reset), then the candidate inputs
@@ -740,28 +723,29 @@ int finalize_on_stream(lvsr_model* m, cudaStream_t st, bool synchronise) {
     const lvsr_model::DecLayer& d = m->dec[l];
     const std::string x = layer_suffix(l);
     const std::string dist = t + "/distribute/";
-    if (int rc = copy2d(d.Wd, 3 * C, m->P(dist + "fork_gate_inputs" + x + ".W"), 2 * C, m->E, 2 * C, st)) return rc;
-    if (int rc = copy2d(d.Wd + 2 * C, 3 * C, m->P(dist + "fork_inputs" + x + ".W"), C, m->E, C, st)) return rc;
-    if (int rc = fork_copy(m, feedback_fork(c, l), d.Wff, d.bff, nullptr, st)) return rc;
+    float *Wd = d.Wd.get(), *Wff = d.Wff.get(), *bff = d.bff.get(), *FF = d.FF.get();
+    if (int rc = copy2d(Wd, 3 * C, m->P(dist + "fork_gate_inputs" + x + ".W"), 2 * C, m->E, 2 * C, st)) return rc;
+    if (int rc = copy2d(Wd + 2 * C, 3 * C, m->P(dist + "fork_inputs" + x + ".W"), C, m->E, C, st)) return rc;
+    if (int rc = fork_copy(m, feedback_fork(c, l), Wff, bff, nullptr, st)) return rc;
     // fork(feedback(y)) for every symbol y, once: [(V+1), 3C]
     if (c.one_of_n_feedback) {
       // one-hot feedback: fork(feedback(y)) is row y of the fork weights plus the bias
-      if (int rc = add_bias_rows(d.FF, d.Wff, d.bff, V + 1, 3 * C, st)) return rc;
+      if (int rc = add_bias_rows(FF, Wff, bff, V + 1, 3 * C, st)) return rc;
     } else {
-      GemmArgs ff = make_gemm(m->P(g + "/readout/lookupfeedback/lookuptable.W"), V + 1, Cfb, d.Wff, 3 * C, d.bff, d.FF);
+      GemmArgs ff = make_gemm(m->P(g + "/readout/lookupfeedback/lookuptable.W"), V + 1, Cfb, Wff, 3 * C, bff, FF);
       if (int rc = gemm_bias(ff, st)) return rc;
     }
   }
-  LVSR_CUDA_OK(cudaMemsetAsync(m->Wb1, 0, (size_t)(m->E + C) * 3 * C * sizeof(float), st));
-  if (int rc = copy2d(m->Wb1, 3 * C, m->dec[0].Wd, 3 * C, m->E, 3 * C, st)) return rc;
-  if (int rc = copy2d(m->Wb1 + (size_t)m->E * 3 * C, 3 * C, m->P(dec_gru(m, 0) + ".state_to_gates"), 2 * C, C, 2 * C, st)) return rc;
+  LVSR_CUDA_OK(cudaMemsetAsync(m->Wb1.get(), 0, (size_t)(m->E + C) * 3 * C * sizeof(float), st));
+  if (int rc = copy2d(m->Wb1.get(), 3 * C, m->dec[0].Wd.get(), 3 * C, m->E, 3 * C, st)) return rc;
+  if (int rc = copy2d(m->Wb1.get() + (size_t)m->E * 3 * C, 3 * C, m->P(dec_gru(m, 0) + ".state_to_gates"), 2 * C, C, 2 * C, st)) return rc;
   // tensor-core operands of the fork and preprocess weights (K-major fp16 head/tail planes or tf32 hi/lo pairs)
   m->use_tc = getenv("LVSR_NO_TC_GEMM") == nullptr;
   if (m->use_tc) {
     m->Wcat_tc.resize(c.num_layers);
     for (int l = 0; l < c.num_layers; ++l) {
       const ForkLayout f = encoder_fork(m, l, 0);
-      if (int rc = pack_tc_weights(m->Wcat_tc[l], m->Wcat[l], f.rows, f.ld, st)) return rc;
+      if (int rc = pack_tc_weights(m->Wcat_tc[l], m->Wcat[l].get(), f.rows, f.ld, st)) return rc;
     }
     if (int rc = pack_tc_weights(m->Wp_tc, m->P(att_base(m) + "/preprocess.W"), m->E, c.dim_matcher, st)) return rc;
     m->bottom_tc.resize(m->bottom.num_layers);
@@ -866,22 +850,16 @@ int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int
   const char* sl = getenv("LVSR_ENC_OVERLAP_SPIN_LIMIT");
   const unsigned spin_limit = sl ? (unsigned)strtoul(sl, nullptr, 10) : LVSR_SPIN_LIMIT;
   if (overlap_on && c.num_layers > 1) {
-    if (!m->enc_tiles) LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->enc_tiles), LVSR_MAX_LAYERS * 2 * sizeof(int)));
-    LVSR_CUDA_OK(cudaMemsetAsync(m->enc_tiles, 0, LVSR_MAX_LAYERS * 2 * sizeof(int), st));
+    if (!m->enc_tiles) LVSR_CUDA_OK(m->enc_tiles.alloc(LVSR_MAX_LAYERS * 2 * sizeof(int)));
+    LVSR_CUDA_OK(cudaMemsetAsync(m->enc_tiles.get(), 0, LVSR_MAX_LAYERS * 2 * sizeof(int), st));
     // the claim records of every layer's projection (lvsr_model_encoder_overlap_claims)
     size_t need = 0;
     for (int l = 1, Tp = ceil_div(T, c.subsample[0]); l < c.num_layers; Tp = ceil_div(Tp, c.subsample[l]), ++l) {
       m->enc_claims_off[l] = need;
       need += 3 * (size_t)ceil_div(Tp * B, 128) * (encoder_fork(m, l, 0).ld / 128);
     }
-    if (need > m->enc_claims_cap) {
-      if (m->enc_claims) LVSR_CUDA_OK(cudaFree(m->enc_claims));
-      m->enc_claims = nullptr;
-      m->enc_claims_cap = 0;
-      LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->enc_claims), need * sizeof(int)));
-      m->enc_claims_cap = need;
-    }
-    LVSR_CUDA_OK(cudaMemsetAsync(m->enc_claims, 0, need * sizeof(int), st));
+    LVSR_CUDA_OK(m->enc_claims.grow(need * sizeof(int), st));
+    LVSR_CUDA_OK(cudaMemsetAsync(m->enc_claims.get(), 0, need * sizeof(int), st));
   }
   float* pre_done = nullptr;   // this layer's pre-activations, when they were projected beside the previous scan
   const int nd = encoder_dirs(m);
@@ -896,7 +874,7 @@ int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int
       // finalize splits the fork weights only while the tensor-core GEMM is on (null entry: a shape it refuses)
       ArenaMark mark{ws};      // the split scratch is dead once the GEMM is enqueued (stream order)
       int kpad = 0, operands = 0;
-      if (int rc = projection_gemm(ws, cur, rows, din, m->Wcat[l], m->use_tc ? &m->Wcat_tc[l] : nullptr, N, m->bcat[l],
+      if (int rc = projection_gemm(ws, cur, rows, din, m->Wcat[l].get(), m->use_tc ? &m->Wcat_tc[l] : nullptr, N, m->bcat[l].get(),
                                    pre, st, &kpad, &operands))
         return rc;
       plan[LVSR_ENC_PROJ] = kpad ? LVSR_ENC_PATH_TC : LVSR_ENC_PATH_FFMA;
@@ -945,23 +923,23 @@ int run_encoder(lvsr_model* m, Arena& ws, const float* x, const float* mask, int
       a.progress = gemm_f16_stream_progress(sync);
       __half* a_head = reinterpret_cast<__half*>(a_hi);
       const TcWeights& tw = m->Wcat_tc[l1];
-      ProjStream ps = {sync, a.progress, scan_ctas, bp.cs, nd, Tl, k, B, spin_limit, m->enc_tiles + 2 * l1,
-                       m->enc_claims + m->enc_claims_off[l1]};
+      ProjStream ps = {sync, a.progress, scan_ctas, bp.cs, nd, Tl, k, B, spin_limit, m->enc_tiles.get() + 2 * l1,
+                       m->enc_claims.get() + m->enc_claims_off[l1]};
       {
         // no event between the two launches: the projection must directly follow the scan in the stream.  The
         // profiled "bigru" time therefore covers the scan and the projection tiles done beside it.
         ProfScope prof("bigru", st);
         if (int rc = bigru_layer(a, st, &bp)) return rc;
         if (int rc = gemm_f16_stream(out, a_head, a_head + (size_t)rows1 * K1, reinterpret_cast<int*>(a_lo), rows1, K1,
-                                     tw.head, tw.tail, tw.ew, N1, m->bcat[l1], pre1, N1, ps, free_sms, st))
+                                     tw.head, tw.tail, tw.ew, N1, m->bcat[l1].get(), pre1, N1, ps, free_sms, st))
           return rc;
       }
       {
         ProfScope prof("gemm", st);
         ps.progress = nullptr;
-        ps.tiles_done = m->enc_tiles + 2 * l1 + 1;
+        ps.tiles_done = m->enc_tiles.get() + 2 * l1 + 1;
         if (int rc = gemm_f16_stream(out, a_head, a_head + (size_t)rows1 * K1, reinterpret_cast<int*>(a_lo), rows1, K1,
-                                     tw.head, tw.tail, tw.ew, N1, m->bcat[l1], pre1, N1, ps, device_sm_count(), st))
+                                     tw.head, tw.tail, tw.ew, N1, m->bcat[l1].get(), pre1, N1, ps, device_sm_count(), st))
           return rc;
       }
       int32_t* plan1 = m->enc_plan[l1];
@@ -1001,11 +979,11 @@ static int tle_run_matrices(lvsr_model* m, Arena& ws, const long long* groundtru
                             int L, int B, float* rewards, float* gains, cudaStream_t st) {
   int* dist = ws.i32(tle_dist_ints(Lg, L, B));
   LVSR_CHECK(dist, "out of device memory (task-loss distances)");
-  LVSR_CUDA_OK(cudaMemsetAsync(m->tle_status, 0xff, sizeof(unsigned), st));
+  LVSR_CUDA_OK(cudaMemsetAsync(m->tle_status.get(), 0xff, sizeof(unsigned), st));
   if (int rc = tle_matrices(groundtruth, Lg, prediction, L, B, m->cfg.num_phonemes, m->criterion.eos_label, dist, rewards,
-                            gains, m->tle_status, st)) return rc;
+                            gains, m->tle_status.get(), st)) return rc;
   unsigned h = LVSR_TLE_OK;
-  LVSR_CUDA_OK(cudaMemcpyAsync(&h, m->tle_status, sizeof(h), cudaMemcpyDeviceToHost, st));
+  LVSR_CUDA_OK(cudaMemcpyAsync(&h, m->tle_status.get(), sizeof(h), cudaMemcpyDeviceToHost, st));
   LVSR_CUDA_OK(cudaStreamSynchronize(st));
   LVSR_CHECK(h == LVSR_TLE_OK, "task loss estimation: the groundtruth of utterance %u does not end in eos (%d)", h,
              m->criterion.eos_label);
@@ -1039,7 +1017,7 @@ int lvsr_model_set_criterion(lvsr_model* m, const lvsr_criterion* cr) {
     LVSR_CHECK(cr->initial_output >= 0 && cr->initial_output <= V, "set_criterion: initial_output %d outside [0, %d]",
                cr->initial_output, V);
     LVSR_CHECK(std::isfinite(cr->min_reward), "set_criterion: min_reward must be finite");
-    if (!m->tle_status) LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->tle_status), sizeof(unsigned)));
+    if (!m->tle_status) LVSR_CUDA_OK(m->tle_status.alloc(sizeof(unsigned)));
   }
   LVSR_CUDA_OK(cudaStreamSynchronize(m->stream));   // calls already queued keep the criterion they were issued under
   m->criterion = *cr;
@@ -1142,7 +1120,7 @@ int lvsr_cost_matrix_groundtruth(lvsr_model* m, const float* attended, const flo
 
   bool scanned = false;
   for (int32_t& v : m->dec_plan) v = 0;
-  LVSR_CUDA_OK(cudaMemsetAsync(m->status, 0, sizeof(unsigned), st));
+  LVSR_CUDA_OK(cudaMemsetAsync(m->status.get(), 0, sizeof(unsigned), st));
   // the persistent decoder holds one GRU layer: a stacked decoder runs on the step-wise kernels
   if (getenv("LVSR_NO_DEC_SCAN") == nullptr && !m->force_stepwise && c.dec_stack == 1) {
     DecScanInputs d = {};
@@ -1152,14 +1130,14 @@ int lvsr_cost_matrix_groundtruth(lvsr_model* m, const float* attended, const flo
     d.v = m->P(att_base(m) + "/energy_comp/linear.W");
     d.v_bias = m->v_bias;
     d.prior = prior_of(c);
-    d.Wb1 = m->Wb1;
+    d.Wb1 = m->Wb1.get();
     d.Wstate = m->P(dec_gru(m, 0) + ".state_to_state");
     d.Ws = m->P(att_base(m) + "/state_trans/transform_states.W");
-    d.FF = m->dec[0].FF;
+    d.FF = m->dec[0].FF.get();
     d.labels = lab; d.lmask = labels_mask;
     d.s_all = s_all; d.ctx_all = ctx_all; d.w0 = w0; d.w_all = weights_out;
     d.e_seq = energies_out; d.e_scratch = e_scratch;
-    d.status = m->status;
+    d.status = m->status.get();
     d.Tp = Tp; d.B = B; d.L = L; d.M = M; d.E = E; d.C = C; d.K = c.conv_num_filters; d.n = c.conv_n;
     d.normalizer = c.energy_normalizer;
     d.V = c.num_phonemes;
@@ -1200,7 +1178,7 @@ int lvsr_cost_matrix_groundtruth(lvsr_model* m, const float* attended, const flo
                            nullptr, merged, acc);
     if (int rc = gemm_bias(b, st)) return rc;
     ReadoutArgs r = readout_args(m, R, merged);
-    r.poison = scanned ? m->status : nullptr;
+    r.poison = scanned ? m->status.get() : nullptr;
     if (tle) {
       // RewardRegressionEmitter.cost over the whole readouts (lvsr/bricks/__init__.py:135-184)
       float* neg = ws.f32((size_t)R * c.num_phonemes);
@@ -1406,7 +1384,7 @@ int lvsr_recognizer_cost_host(lvsr_model* m, const float* x_h, const float* mask
     if (!rc) {
       unsigned hst = 0;
       LVSR_CUDA_OK(cudaMemcpyAsync(costs_h, costs, (size_t)L * B * sizeof(float), cudaMemcpyDeviceToHost, st));
-      LVSR_CUDA_OK(cudaMemcpyAsync(&hst, m->status, sizeof(hst), cudaMemcpyDeviceToHost, st));
+      LVSR_CUDA_OK(cudaMemcpyAsync(&hst, m->status.get(), sizeof(hst), cudaMemcpyDeviceToHost, st));
       LVSR_CUDA_OK(cudaStreamSynchronize(st));
       if (hst != 0) {
         // the persistent decoder gave up (status in common.cuh): same math on the step-wise kernels

@@ -4,7 +4,9 @@
 #include <cooperative_groups.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <atomic>
 #include <string>
+#include <utility>
 
 namespace lvsr {
 
@@ -12,6 +14,7 @@ namespace cg = cooperative_groups;
 
 extern thread_local std::string g_last_error;
 extern long long g_launch_count;
+extern std::atomic<long long> g_device_bytes;    // bytes every DeviceBuffer holds (lvsr_device_bytes)
 
 int set_error(const char* fmt, ...);
 
@@ -46,6 +49,88 @@ struct ProfScope {
   } while (0)
 
 static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
+
+// The owner of one cudaMalloc allocation, and the only code that calls cudaMalloc / cudaFree: move-only, freed when it
+// is destroyed, reset or assigned to.  Releasing never waits: code that drops a buffer enqueued work may still read
+// waits for that work first.
+template <class T>
+class DeviceBuffer {
+ public:
+  DeviceBuffer() = default;
+  DeviceBuffer(DeviceBuffer&& o) noexcept : p_(std::exchange(o.p_, nullptr)), bytes_(std::exchange(o.bytes_, 0)) {}
+  DeviceBuffer& operator=(DeviceBuffer&& o) noexcept {
+    if (this != &o) {
+      reset();
+      p_ = std::exchange(o.p_, nullptr);
+      bytes_ = std::exchange(o.bytes_, 0);
+    }
+    return *this;
+  }
+  ~DeviceBuffer() { reset(); }
+
+  // Replaces the buffer by `bytes` of device memory (empty when the allocation fails)
+  cudaError_t alloc(size_t bytes) {
+    reset();
+    void* p = nullptr;
+    const cudaError_t e = cudaMalloc(&p, bytes);
+    if (e != cudaSuccess) return e;
+    p_ = static_cast<T*>(p);
+    bytes_ = bytes;
+    g_device_bytes += (long long)bytes;
+    return cudaSuccess;
+  }
+  // At least `bytes`: a smaller buffer is replaced once `stream`, whose work may still read it, has drained
+  cudaError_t grow(size_t bytes, cudaStream_t stream) {
+    if (bytes <= bytes_) return cudaSuccess;
+    if (p_) {
+      const cudaError_t e = cudaStreamSynchronize(stream);
+      if (e != cudaSuccess) return e;
+    }
+    return alloc(bytes);
+  }
+  void reset() {
+    if (!p_) return;
+    cudaFree(p_);
+    g_device_bytes -= (long long)bytes_;
+    p_ = nullptr;
+    bytes_ = 0;
+  }
+  T* get() const { return p_; }
+  size_t bytes() const { return bytes_; }
+  explicit operator bool() const { return p_ != nullptr; }
+
+ private:
+  T* p_ = nullptr;
+  size_t bytes_ = 0;
+};
+
+// Every entry point runs on its handle's GPU (the device current when the handle was created), whatever device the
+// calling thread has current.  Handle: lvsr_model or lvsr_frontend; a null handle switches nothing.
+struct DeviceGuard {
+  int prev = -1;
+  template <class Handle>
+  explicit DeviceGuard(const Handle* h) {
+    int cur = 0;
+    if (h && cudaGetDevice(&cur) == cudaSuccess && cur != h->device) {
+      prev = cur;
+      cudaSetDevice(h->device);
+    }
+  }
+  ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
+};
+
+// Every entry point that takes a stream binds it first, before it sizes a workspace or touches per-handle device
+// state: a call on another stream than the handle's last one first waits for everything the handle enqueued there, so
+// two streams never share its workspaces, status words or parameters at once.
+template <class Handle>
+static inline int bind_stream(Handle* h, cudaStream_t st) {
+  LVSR_CHECK(h != nullptr, "null model");
+  if (st != h->stream) {
+    LVSR_CUDA_OK(cudaStreamSynchronize(h->stream));
+    h->stream = st;
+  }
+  return 0;
+}
 
 // Function attributes (dynamic shared-memory opt-in), SM counts and occupancy answers are properties
 // of a DEVICE, not of the process: caches are keyed by the current device ordinal.

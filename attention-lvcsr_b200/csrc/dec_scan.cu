@@ -711,15 +711,15 @@ __global__ void count_sentinels_kernel(const unsigned* p, long long n, unsigned 
 
 // *host_count = the words of p[0, n) that still hold the sentinel (synchronises)
 int count_sentinels(const float* p, long long n, long long* host_count, cudaStream_t stream) {
-  unsigned long long* d = nullptr;
-  LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&d), sizeof(*d)));
+  DeviceBuffer<unsigned long long> buf;
+  LVSR_CUDA_OK(buf.alloc(sizeof(unsigned long long)));
+  unsigned long long* d = buf.get();
   cudaMemsetAsync(d, 0, sizeof(*d), stream);
   const int grid = (int)std::min<long long>(2048, (n + 255) / 256);
   if (n > 0) count_sentinels_kernel<<<grid, 256, 0, stream>>>(reinterpret_cast<const unsigned*>(p), n, d);
   unsigned long long h = 0;
   cudaError_t e = cudaMemcpyAsync(&h, d, sizeof(h), cudaMemcpyDeviceToHost, stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
-  cudaFree(d);
   if (e != cudaSuccess) return set_error("count_sentinels failed: %s", cudaGetErrorString(e));
   *host_count = (long long)h;
   return 0;

@@ -13,6 +13,7 @@
 #include <cfloat>
 #include <algorithm>
 #include <cmath>
+#include <memory>
 #include <vector>
 
 #include <curand_kernel.h>
@@ -317,54 +318,14 @@ struct lvsr_frontend {
   cudaStream_t stream = nullptr;
   int W = 0, S = 0, P = 0, log2n = 0, D0 = 0, D = 0;
   DeltaScales scales = {};
-  float* table = nullptr;           // window [W] | twiddles [P / 2] float2 | mel weights
-  MelBin* bins = nullptr;
+  DeviceBuffer<float> table;        // window [W] | twiddles [P / 2] float2 | mel weights
+  DeviceBuffer<MelBin> bins;
   const float2* twiddle = nullptr;
   const float* weights = nullptr;
-  double* part = nullptr;           // [kCmvnCtas][2][D + 1]
-  float* raw = nullptr;             // [T, B, D0]
-  size_t raw_cap = 0;
-  int* frames = nullptr;            // [B]
-  size_t frames_cap = 0;
+  DeviceBuffer<double> part;        // [kCmvnCtas][2][D + 1]
+  DeviceBuffer<float> raw;          // [T, B, D0], grown on demand
+  DeviceBuffer<int> frames;         // [B], grown on demand
 };
-
-namespace {
-
-struct FrontendGuard {
-  int prev = -1;
-  explicit FrontendGuard(const lvsr_frontend* f) {
-    int cur = 0;
-    if (f && cudaGetDevice(&cur) == cudaSuccess && cur != f->device) {
-      prev = cur;
-      cudaSetDevice(f->device);
-    }
-  }
-  ~FrontendGuard() { if (prev >= 0) cudaSetDevice(prev); }
-};
-
-// the model handle's stream rule: a call on another stream first waits for the handle's work on the previous one
-int bind(lvsr_frontend* f, cudaStream_t st) {
-  if (st != f->stream) {
-    LVSR_CUDA_OK(cudaStreamSynchronize(f->stream));
-    f->stream = st;
-  }
-  return 0;
-}
-
-// grows a workspace buffer (waiting for the bound stream, whose work may still read it)
-template <class T>
-int grow(lvsr_frontend* f, T** buf, size_t* cap, size_t need) {
-  if (need <= *cap) return 0;
-  LVSR_CUDA_OK(cudaStreamSynchronize(f->stream));
-  if (*buf) cudaFree(*buf);
-  *buf = nullptr;
-  *cap = 0;
-  LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(buf), need * sizeof(T)));
-  *cap = need;
-  return 0;
-}
-
-}  // namespace
 
 extern "C" {
 
@@ -429,7 +390,7 @@ int lvsr_frontend_create(const lvsr_fbank_options* o, lvsr_frontend** out) {
   LVSR_CUDA_OK(cudaGetDeviceCount(&dev_count));
   LVSR_CHECK(dev_count > 0, "no CUDA device: the front end has no CPU fallback");
 
-  lvsr_frontend* f = new lvsr_frontend();
+  std::unique_ptr<lvsr_frontend> f(new lvsr_frontend());   // deleted with its buffers on a failed return
   f->opt = *o;
   f->W = (int)W;
   f->S = (int)S;
@@ -473,32 +434,25 @@ int lvsr_frontend_create(const lvsr_fbank_options* o, lvsr_frontend** out) {
   }
   const size_t w_off = table.size();
   table.insert(table.end(), weights.begin(), weights.end());
-  int rc = 0;
   cudaError_t e = cudaGetDevice(&f->device);
-  if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void**>(&f->table), table.size() * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void**>(&f->bins), nb * sizeof(MelBin));
-  if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void**>(&f->part), (size_t)kCmvnCtas * 2 * (f->D + 1) * sizeof(double));
-  if (e == cudaSuccess) e = cudaMemcpy(f->table, table.data(), table.size() * sizeof(float), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemcpy(f->bins, bins.data(), nb * sizeof(MelBin), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = f->table.alloc(table.size() * sizeof(float));
+  if (e == cudaSuccess) e = f->bins.alloc(nb * sizeof(MelBin));
+  if (e == cudaSuccess) e = f->part.alloc((size_t)kCmvnCtas * 2 * (f->D + 1) * sizeof(double));
+  if (e == cudaSuccess) e = cudaMemcpy(f->table.get(), table.data(), table.size() * sizeof(float), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(f->bins.get(), bins.data(), nb * sizeof(MelBin), cudaMemcpyHostToDevice);
   if (e == cudaSuccess)
     e = cudaFuncSetAttribute(fbank_frames_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
-  if (e != cudaSuccess) {
-    rc = set_error("frontend_create: %s", cudaGetErrorString(e));
-    lvsr_frontend_destroy(f);
-    return rc;
-  }
-  f->twiddle = reinterpret_cast<const float2*>(f->table + tw_off);
-  f->weights = f->table + w_off;
-  *out = f;
+  if (e != cudaSuccess) return set_error("frontend_create: %s", cudaGetErrorString(e));
+  f->twiddle = reinterpret_cast<const float2*>(f->table.get() + tw_off);
+  f->weights = f->table.get() + w_off;
+  *out = f.release();
   return 0;
 }
 
 int lvsr_frontend_destroy(lvsr_frontend* f) {
   if (!f) return 0;
-  FrontendGuard guard(f);
+  DeviceGuard guard(f);
   cudaStreamSynchronize(f->stream);
-  for (void* p : {(void*)f->table, (void*)f->bins, (void*)f->part, (void*)f->raw, (void*)f->frames})
-    if (p) cudaFree(p);
   delete f;
   return 0;
 }
@@ -528,21 +482,21 @@ int lvsr_frontend_compute(lvsr_frontend* f, const float* samples_dev, int64_t ro
     LVSR_CHECK(nf <= T, "utterance %d has %lld frames, more than T = %d", b, (long long)nf, T);
     frames[b] = (int)nf;
   }
-  FrontendGuard guard(f);
+  DeviceGuard guard(f);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (int rc = bind(f, st)) return rc;
-  if (int rc = grow(f, &f->frames, &f->frames_cap, (size_t)B)) return rc;
-  if (int rc = grow(f, &f->raw, &f->raw_cap, (size_t)T * B * f->D0)) return rc;
-  LVSR_CUDA_OK(cudaMemcpyAsync(f->frames, frames.data(), B * sizeof(int), cudaMemcpyHostToDevice, st));
+  if (int rc = bind_stream(f, st)) return rc;
+  LVSR_CUDA_OK(f->frames.grow((size_t)B * sizeof(int), f->stream));
+  LVSR_CUDA_OK(f->raw.grow((size_t)T * B * f->D0 * sizeof(float), f->stream));
+  LVSR_CUDA_OK(cudaMemcpyAsync(f->frames.get(), frames.data(), B * sizeof(int), cudaMemcpyHostToDevice, st));
   ProfScope prof("fbank", st);
   FrameParams p;
   p.samples = samples_dev;
   p.stride = row_stride;
-  p.frames = f->frames;
-  p.raw = f->raw;
-  p.window = f->table;
+  p.frames = f->frames.get();
+  p.raw = f->raw.get();
+  p.window = f->table.get();
   p.twiddle = f->twiddle;
-  p.bins = f->bins;
+  p.bins = f->bins.get();
   p.weights = f->weights;
   p.B = B;
   p.W = f->W;
@@ -564,7 +518,7 @@ int lvsr_frontend_compute(lvsr_frontend* f, const float* samples_dev, int64_t ro
   LVSR_LAUNCH_CHECK();
   const long long n = (long long)T * B * f->D;
   fbank_finish_kernel<<<elementwise_grid(n), kThreads, cmvn_stats_dev ? 2 * f->D * sizeof(float) : 0, st>>>(
-      f->raw, f->frames, features_dev, mask_dev, cmvn_stats_dev, T, B, f->D0, f->opt.delta_order, f->opt.delta_window,
+      f->raw.get(), f->frames.get(), features_dev, mask_dev, cmvn_stats_dev, T, B, f->D0, f->opt.delta_order, f->opt.delta_window,
       f->scales);
   LVSR_LAUNCH_CHECK();
   return 0;
@@ -573,14 +527,14 @@ int lvsr_frontend_compute(lvsr_frontend* f, const float* samples_dev, int64_t ro
 int lvsr_frontend_accumulate_cmvn(lvsr_frontend* f, const float* features_dev, const float* mask_dev, int32_t T,
                                   int32_t B, double* stats_dev, void* stream) {
   LVSR_CHECK(f && features_dev && stats_dev && T >= 1 && B >= 1, "frontend_accumulate_cmvn: bad arguments");
-  FrontendGuard guard(f);
+  DeviceGuard guard(f);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (int rc = bind(f, st)) return rc;
+  if (int rc = bind_stream(f, st)) return rc;
   const long long rows = (long long)T * B;
   const int nparts = (int)std::min<long long>(kCmvnCtas, rows);
-  cmvn_partial_kernel<<<nparts, kThreads, 0, st>>>(features_dev, mask_dev, rows, f->D, f->part);
+  cmvn_partial_kernel<<<nparts, kThreads, 0, st>>>(features_dev, mask_dev, rows, f->D, f->part.get());
   LVSR_LAUNCH_CHECK();
-  cmvn_reduce_kernel<<<1, kThreads, 0, st>>>(f->part, nparts, f->D, stats_dev);
+  cmvn_reduce_kernel<<<1, kThreads, 0, st>>>(f->part.get(), nparts, f->D, stats_dev);
   LVSR_LAUNCH_CHECK();
   return 0;
 }
@@ -588,9 +542,9 @@ int lvsr_frontend_accumulate_cmvn(lvsr_frontend* f, const float* features_dev, c
 int lvsr_frontend_apply_cmvn(lvsr_frontend* f, float* features_dev, const float* mask_dev, int32_t T, int32_t B,
                              const double* stats_dev, void* stream) {
   LVSR_CHECK(f && features_dev && stats_dev && T >= 1 && B >= 1, "frontend_apply_cmvn: bad arguments");
-  FrontendGuard guard(f);
+  DeviceGuard guard(f);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (int rc = bind(f, st)) return rc;
+  if (int rc = bind_stream(f, st)) return rc;
   const long long rows = (long long)T * B;
   cmvn_apply_kernel<<<elementwise_grid(rows * f->D), kThreads, 2 * f->D * sizeof(float), st>>>(features_dev, mask_dev,
                                                                                              rows, f->D, stats_dev);
@@ -600,9 +554,9 @@ int lvsr_frontend_apply_cmvn(lvsr_frontend* f, float* features_dev, const float*
 
 int lvsr_frontend_dither_sample(lvsr_frontend* f, int32_t B, int32_t T, float* draws_dev, void* stream) {
   LVSR_CHECK(f && draws_dev && B >= 1 && T >= 1, "frontend_dither_sample: bad arguments");
-  FrontendGuard guard(f);
+  DeviceGuard guard(f);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (int rc = bind(f, st)) return rc;
+  if (int rc = bind_stream(f, st)) return rc;
   const long long n = (long long)B * T * ((f->W + 3) >> 2);
   dither_sample_kernel<<<elementwise_grid(n), kThreads, 0, st>>>(draws_dev, B, T, f->W, f->opt.seed);
   LVSR_LAUNCH_CHECK();

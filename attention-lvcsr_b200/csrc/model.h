@@ -14,12 +14,13 @@ namespace lvsr {
 // the block is too small the overflow is served by separate cudaMallocs and the block is
 // regrown at the end of the call, so a steady-state workload never allocates.  The arena is
 // rewound when a call returns while its kernels may still be in flight: safe because every call
-// on the handle runs on the handle's bound stream (bind_stream below).
+// on the handle runs on the handle's bound stream (bind_stream, common.cuh).
 struct Arena {
+  DeviceBuffer<char> block;         // base = block + shift (LVSR_WS_SHIFT_KB, read by reserve: placement experiments)
   char* base = nullptr;
-  size_t cap = 0, off = 0, overflow_bytes = 0;
+  size_t cap = 0, off = 0, overflow_bytes = 0, shift = 0;
   int depth = 0;
-  std::vector<void*> overflow;
+  std::vector<DeviceBuffer<char>> overflow;
 
   void* alloc(size_t bytes) {
     bytes = (bytes + 255) & ~(size_t)255;
@@ -28,11 +29,11 @@ struct Arena {
       off += bytes;
       return p;
     }
-    void* p = nullptr;
-    if (cudaMalloc(&p, bytes) != cudaSuccess) return nullptr;
-    overflow.push_back(p);
+    DeviceBuffer<char> p;
+    if (p.alloc(bytes) != cudaSuccess) return nullptr;
+    overflow.push_back(std::move(p));
     overflow_bytes += bytes;
-    return p;
+    return overflow.back().get();
   }
   float* f32(size_t n) { return static_cast<float*>(alloc(n * sizeof(float))); }
   long long* i64(size_t n) { return static_cast<long long*>(alloc(n * sizeof(long long))); }
@@ -42,14 +43,9 @@ struct Arena {
   void reserve(size_t bytes, cudaStream_t stream) {
     if (off != 0 || bytes <= cap) return;
     if (cudaStreamSynchronize(stream) != cudaSuccess) return;
-    if (base) cudaFree(base - shift);
-    base = nullptr;
-    cap = 0;
-    shift = getenv("LVSR_WS_SHIFT_KB") ? (size_t)atoll(getenv("LVSR_WS_SHIFT_KB")) * 1024 : 0;   // placement experiments
-    if (cudaMalloc(reinterpret_cast<void**>(&base), bytes + shift) == cudaSuccess) { cap = bytes; base += shift; }
-    else cudaGetLastError();
+    shift = getenv("LVSR_WS_SHIFT_KB") ? (size_t)atoll(getenv("LVSR_WS_SHIFT_KB")) * 1024 : 0;
+    replace(bytes);
   }
-  size_t shift = 0;
   void enter() { depth++; }
   // returns non-zero on CUDA failure
   int leave(cudaStream_t stream) {
@@ -59,24 +55,19 @@ struct Arena {
     off = 0;
     if (!overflow.empty()) {
       if (cudaStreamSynchronize(stream) != cudaSuccess) return 1;
-      for (void* p : overflow) cudaFree(p);
       overflow.clear();
-      if (base) cudaFree(base - shift);
-      base = nullptr;
-      const size_t want = (size_t)((used + overflow_bytes) * 1.25) + (1 << 20);
+      replace((size_t)((used + overflow_bytes) * 1.25) + (1 << 20));
       overflow_bytes = 0;
-      cap = 0;
-      if (cudaMalloc(reinterpret_cast<void**>(&base), want + shift) == cudaSuccess) { cap = want; base += shift; }
-      else cudaGetLastError();
     }
     return 0;
   }
-  void destroy() {
-    for (void* p : overflow) cudaFree(p);
-    overflow.clear();
-    if (base) cudaFree(base - shift);
+  // a new block of cap `bytes` (0 when the allocation fails)
+  void replace(size_t bytes) {
+    block.reset();
     base = nullptr;
-    cap = off = 0;
+    cap = 0;
+    if (block.alloc(bytes + shift) == cudaSuccess) { cap = bytes; base = block.get() + shift; }
+    else cudaGetLastError();
   }
 };
 
@@ -84,7 +75,7 @@ struct Arena {
 // exponent of every column (K a multiple of 64), else tf32 hi / lo planes [N, gemm_tc_kpad(K)].  mem == null: the
 // shape has no tensor-core form.
 struct TcWeights {
-  void* mem = nullptr;                              // the one allocation the planes below live in
+  DeviceBuffer<char> mem;                           // the one allocation the planes below live in
   __half *head = nullptr, *tail = nullptr;
   int* ew = nullptr;
   float *hi = nullptr, *lo = nullptr;
@@ -113,23 +104,23 @@ struct lvsr_model {
   std::map<std::string, int> index;
   // ONE allocation for all parameters, each at a 256-byte aligned offset (padding stays zero): the
   // gradient buffer, the optimizer state and the all-reduce of the training step use the same layout
-  float* flat = nullptr;
+  DeviceBuffer<float> flat;
   int64_t flat_count = 0;
   // packed, kernel-side weights (rebuilt by finalize)
-  std::vector<float*> Wcat, bcat;   // per encoder layer: [Din, 3 ndir D], [3 ndir D] (encoder_fork)
+  std::vector<DeviceBuffer<float>> Wcat, bcat;   // per encoder layer: [Din, 3 ndir D], [3 ndir D] (encoder_fork)
   // the packed inputs of decoder layer l < dec_stack (finalize), gate columns first (update | reset), then the
   // candidate inputs; the parameters of layer l > 0 carry the suffix "#l" (layer_suffix)
   struct DecLayer {
-    float* Wd = nullptr;            // [E, 3C]     distribute [fork_gate_inputs | fork_inputs]
-    float* Wff = nullptr;           // [Cfb, 3C]   generator fork (feedback_fork)
-    float* bff = nullptr;           // [3C]
-    float* FF = nullptr;            // [(V+1), 3C] = feedback . Wff + bff
+    DeviceBuffer<float> Wd;         // [E, 3C]     distribute [fork_gate_inputs | fork_inputs]
+    DeviceBuffer<float> Wff;        // [Cfb, 3C]   generator fork (feedback_fork)
+    DeviceBuffer<float> bff;        // [3C]
+    DeviceBuffer<float> FF;         // [(V+1), 3C] = feedback . Wff + bff
   } dec[2];
-  float* Wb1 = nullptr;             // [E+C, 3C] = dec[0].Wd stacked on [state_to_gates | 0] (persistent decoder)
+  DeviceBuffer<float> Wb1;          // [E+C, 3C] = dec[0].Wd stacked on [state_to_gates | 0] (persistent decoder)
   // dec_stack 2 (finalize; all inside mem): the attention and the readout see the wide state [s0 | s1] through
   // row-stacked weights
   struct Stack {
-    float* mem = nullptr;           // the one allocation of the buffers below
+    DeviceBuffer<float> mem;        // the one allocation of the buffers below
     float* Ws = nullptr;            // [2C, M]   state_trans/transform_states.W ; transform_states#1.W
     float* Wm = nullptr;            // [2C, Cpm] readout/merge/transform_states.W ; transform_states#1.W
     float* h0 = nullptr;            // [2C]      initial_state of both layers
@@ -141,7 +132,7 @@ struct lvsr_model {
   TcWeights Wp_tc;
   bool use_tc = true;
   float v_bias = 0.f;               // host copy of energy_comp/linear.b
-  unsigned* status = nullptr;       // device word: launch status of the data-flow decoder (common.cuh LVSR_FLOW_*)
+  DeviceBuffer<unsigned> status;    // device word: launch status of the data-flow decoder (common.cuh LVSR_FLOW_*)
   bool force_stepwise = false;      // set while a failed persistent launch is re-run on the step-wise kernels
   long long dec_fallbacks = 0;      // how often that happened
   int32_t dec_plan[16] = {0};       // plan of the last lvsr_cost_matrix (lvsr_model_decoder_plan, LVSR_PLAN_* slots)
@@ -149,37 +140,35 @@ struct lvsr_model {
   int32_t enc_plan[LVSR_MAX_LAYERS][16] = {};   // per layer: lvsr_model_encoder_plan's LVSR_ENC_* slots
   // per layer: 1 when the last encoder forward streamed its projection behind the previous layer's scan
   int32_t enc_overlap[LVSR_MAX_LAYERS] = {};
-  int* enc_tiles = nullptr;         // device [LVSR_MAX_LAYERS][2]: tiles of those projections done beside / after the scan
-  int* enc_claims = nullptr;        // device: ProjStream::claims of every layer, layer l at enc_claims_off[l]
-  size_t enc_claims_cap = 0;        // ints allocated
+  DeviceBuffer<int> enc_tiles;      // device [LVSR_MAX_LAYERS][2]: tiles of those projections done beside / after the scan
+  DeviceBuffer<int> enc_claims;     // device: ProjStream::claims of every layer, layer l at enc_claims_off[l]
   size_t enc_claims_off[LVSR_MAX_LAYERS] = {};
   int32_t pre_plan[3] = {0, 0, 0};  // last lvsr_preprocess: path (LVSR_ENC_PATH_*), Kpad, operands (LVSR_ENC_OPS_*)
   bool finalized = false;
-  // ---- FST language model (lvsr_model_set_lm); lm_off == nullptr: none attached ----
-  long long* lm_off = nullptr;
-  int *lm_label = nullptr, *lm_next = nullptr;
-  float* lm_weight = nullptr;
+  // ---- FST language model (lvsr_model_set_lm); lm_off empty: none attached ----
+  DeviceBuffer<long long> lm_off;
+  DeviceBuffer<int> lm_label, lm_next;
+  DeviceBuffer<float> lm_weight;
   int lm_start = 0;
   lvsr_lm_fusion lm_fusion = {};
-  unsigned* lm_status = nullptr;
+  DeviceBuffer<unsigned> lm_status;
   // ---- criterion (lvsr_model_set_criterion; read through tle_criterion and initial_output) ----
   lvsr_criterion criterion = {LVSR_CRITERION_LOG_LIKELIHOOD, 0, 0, -1.0};
-  unsigned* tle_status = nullptr;   // device word of tle_matrices, allocated with the first task-loss criterion
+  DeviceBuffer<unsigned> tle_status;   // device word of tle_matrices, allocated with the first task-loss criterion
   // The stream of the last call that enqueued work on the handle (bind_stream).  Both arenas, the device words above
   // and the parameter and optimizer buffers are only ever touched in this stream's order.
   cudaStream_t stream = nullptr;
   Arena ws;
   // ---- training (train.cu) ----
   Arena tws;                        // tape + backward workspace
-  float *opt_velocity = nullptr, *opt_ms_step = nullptr, *opt_ms_dx = nullptr;   // flat layout, allocated on first use
-  float* opt_scratch = nullptr;     // [1024 partial sums | norm]
-  void* opt_desc = nullptr;         // device copy of the per-parameter table (train::ParamDesc)
+  DeviceBuffer<float> opt_velocity, opt_ms_step, opt_ms_dx;   // flat layout, allocated on first use
+  DeviceBuffer<float> opt_scratch;  // [1024 partial sums | norm]
+  DeviceBuffer<void> opt_desc;      // device copy of the per-parameter table (train::ParamDesc)
   long long burn_in_left = -1;      // BurnIn counter (-1: not started)
-  double* clip = nullptr;           // device train::CLIP_* words of adaptive clipping (nullptr: off)
+  DeviceBuffer<double> clip;        // device train::CLIP_* words of adaptive clipping (empty: off)
   double clip_init[8] = {};         // their values after lvsr_train_set_adaptive_clipping / lvsr_train_reset
   // ---- lvsr_alignment_stats (stats.cu): [finished-CTA count | 256-byte pad | 2 doubles per batch row] ----
-  void* align_mem = nullptr;
-  int align_rows = 0;               // batch rows it holds
+  DeviceBuffer<void> align_mem;
   // ---- adaptive weight noise (noise.cu; lvsr_train_set_adaptive_noise) ----
   struct Noise {
     bool on = false;
@@ -188,12 +177,12 @@ struct lvsr_model {
     bool sampled = false;           // a sample pass ran since the last update (its priors feed the gradients)
     bool stale = false;             // an update left the packed weights un-built (the next training forward packs
                                     // its noisy copy; any other entry point first waits for the update, check_ready)
-    float* mem = nullptr;           // the one allocation of the buffers below (flat layout each, padding zero)
+    DeviceBuffer<float> mem;        // the one allocation of the buffers below (flat layout each, padding zero)
     float* ls2 = nullptr;           // log-variance parameters
     float* noisy = nullptr;         // means + eps * sigma of the current step
     float* gls2 = nullptr;          // gradients, then steps, of ls2
     float *velocity = nullptr, *ms_step = nullptr, *ms_dx = nullptr;   // optimizer state of ls2
-    void* aux = nullptr;            // the one allocation of the tables below
+    DeviceBuffer<char> aux;         // the one allocation of the tables below
     void* spans = nullptr;          // device [params]: (offset, count) of every parameter, padding excluded
     double* stats = nullptr;        // device [LVSR_NOISE_*]: model cost, prior mean, prior variance, element count
     double* part = nullptr;         // device partial sums of the sample pass
@@ -206,10 +195,10 @@ struct lvsr_model {
     unsigned long long seed = 1;
     long long update = 0;           // update counter of both draws; advanced by lvsr_train_apply_updates
     long long utt_offset = 0;       // global index of the batch's first utterance (dropout key)
-    float* noisy = nullptr;         // flat layout: the means + level * eps of the current step (padding zero)
-    void* spans = nullptr;          // device [params]: (offset, count, subject): 0 for the attention's parameters
+    DeviceBuffer<float> noisy;      // flat layout: the means + level * eps of the current step (padding zero)
+    DeviceBuffer<void> spans;       // device [params]: (offset, count, subject): 0 for the attention's parameters
     float penalty_coof = 0.f;       // alignment penalty coefficient (0: off)
-    float* penalty = nullptr;       // device: the penalty sum of the last training forward (penalty_coof > 0)
+    DeviceBuffer<float> penalty;    // device: the penalty sum of the last training forward (penalty_coof > 0)
   } reg;
 
   const Param* param(const std::string& n) const {     // null when the model has no such parameter
@@ -265,33 +254,6 @@ static inline PriorParams prior_of(const lvsr_config& c) {
   p.before = c.prior_before;
   p.after = c.prior_after;
   return p;
-}
-
-// Every entry point runs on the handle's own GPU, whatever device the calling thread has current
-// (a handle is bound to the device that was current at lvsr_model_create).
-struct DeviceGuard {
-  int prev = -1;
-  explicit DeviceGuard(const lvsr_model* m) {
-    if (!m) return;
-    int cur = 0;
-    if (cudaGetDevice(&cur) == cudaSuccess && cur != m->device) {
-      prev = cur;
-      cudaSetDevice(m->device);
-    }
-  }
-  ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
-};
-
-// Every entry point that takes a stream binds it first, before it sizes a workspace or touches per-handle device
-// state: a call on another stream than the last one first waits for everything the handle enqueued there, so two
-// streams never share the arenas, the status and claim words or the parameters at once.
-static inline int bind_stream(lvsr_model* m, cudaStream_t st) {
-  LVSR_CHECK(m != nullptr, "null model");
-  if (st != m->stream) {
-    LVSR_CUDA_OK(cudaStreamSynchronize(m->stream));
-    m->stream = st;
-  }
-  return 0;
 }
 
 // Host calls without a stream take effect after all work queued on the handle: they copy on its bound stream and,
@@ -369,17 +331,15 @@ int copy2d(float* dst, int ld_dst, const float* src, int ld_src, int rows, int c
 int fork_copy(lvsr_model* m, const ForkLayout& f, float* W, float* b, float* grads, cudaStream_t st);
 // adaptive weight noise (noise.cu): the sample pass of a training forward (noisy parameters + priors + model cost)
 // and the gradient transform of an update (both gradient groups; *nparts partial sums of squares of their union in
-// noise.norm_part when nparts is not null).  noise_free releases the handle's noise buffers.
+// noise.norm_part when nparts is not null).
 int noise_sample(lvsr_model* m, cudaStream_t st);
 int noise_gradients(lvsr_model* m, float* grads, float gscale, float* gls2, cudaStream_t st, int* nparts);
-void noise_free(lvsr_model* m);
 // dropout and weight noise (noise.cu): out = in * the dropout multiplier of update `update` over a [T, B, F] batch whose
 // first utterance has the global index utt_offset (in null: the multiplier itself; in == out is allowed), and the
-// noisy parameter copy reg.noisy of the handle's current update.  reg_free releases the handle's buffers.
+// noisy parameter copy reg.noisy of the handle's current update.
 struct DropoutKey { unsigned long long seed; long long update, utt_offset; };
 int dropout_apply(const DropoutKey& key, const float* in, float* out, int T, int B, int F, cudaStream_t st);
 int weight_noise_sample(lvsr_model* m, cudaStream_t st);
-void reg_free(lvsr_model* m);
 // Every encoder layer (fork projection + BiGRU scan) and the mask of the encoded frames: attended [Tp, B, E] (the last
 // layer writes it), attended_mask [Tp, B].  Buffers come from `ws`.  Without a tape (inference) the BiGRU runs without
 // the training stores; with one, tape[l] records layer l's buffers (and allocates hext) for the backward pass.
@@ -403,7 +363,7 @@ int readout_merged(lvsr_model* m, int R, const float* states, const float* ctx, 
 ReadoutArgs readout_args(lvsr_model* m, int R, const float* merged);
 // language model (api.cu): the device view of the attached FST, the fusion fields of a readout, and the LM status
 // word read back after a synchronisation of st (an error return when a kernel reported one; the word is cleared)
-static inline bool lm_attached(const lvsr_model* m) { return m->lm_off != nullptr; }
+static inline bool lm_attached(const lvsr_model* m) { return (bool)m->lm_off; }
 // task loss estimation (lvsr_model_set_criterion): RewardRegressionEmitter instead of SoftmaxEmitter
 static inline bool tle_criterion(const lvsr_model* m) { return m->criterion.name != LVSR_CRITERION_LOG_LIKELIHOOD; }
 // the emitter's initial output: num_phonemes for SoftmaxEmitter (lvsr/bricks/recognizer.py:286), the criterion's for

@@ -215,16 +215,10 @@ int check_index(const lvsr_model* m, int index, int64_t count) {
 
 namespace lvsr {
 
-void noise_free(lvsr_model* m) {
-  if (m->noise.mem) cudaFree(m->noise.mem);
-  if (m->noise.aux) cudaFree(m->noise.aux);
-  m->noise = lvsr_model::Noise();
-}
-
 int noise_sample(lvsr_model* m, cudaStream_t st) {
   ProfScope prof("noise", st);
   lvsr_model::Noise& z = m->noise;
-  noise_sample_kernel<<<param_grid(m), kThreads, 0, st>>>(m->flat, z.ls2, z.noisy, spans_of(m), z.cfg.seed,
+  noise_sample_kernel<<<param_grid(m), kThreads, 0, st>>>(m->flat.get(), z.ls2, z.noisy, spans_of(m), z.cfg.seed,
                                                           (unsigned long long)z.update, z.part);
   LVSR_LAUNCH_CHECK();
   double n = 0.0;
@@ -240,7 +234,7 @@ int noise_gradients(lvsr_model* m, float* grads, float gscale, float* gls2, cuda
   lvsr_model::Noise& z = m->noise;
   LVSR_CHECK(z.sampled, "adaptive noise: no training forward since the last update (its priors form the gradients)");
   ProfScope prof("noise", st);
-  noise_grad_kernel<<<param_grid(m), kThreads, 0, st>>>(grads, gls2, m->flat, z.ls2, spans_of(m), z.stats, gscale,
+  noise_grad_kernel<<<param_grid(m), kThreads, 0, st>>>(grads, gls2, m->flat.get(), z.ls2, spans_of(m), z.stats, gscale,
                                                         (float)(z.cfg.model_cost_coefficient / (double)z.cfg.num_examples),
                                                         nparts ? z.norm_part : nullptr);
   LVSR_LAUNCH_CHECK();
@@ -260,17 +254,11 @@ int dropout_apply(const DropoutKey& key, const float* in, float* out, int T, int
 int weight_noise_sample(lvsr_model* m, cudaStream_t st) {
   ProfScope prof("weight_noise", st);
   const lvsr_model::Reg& r = m->reg;
-  weight_noise_kernel<<<param_grid(m), kThreads, 0, st>>>(m->flat, r.noisy, static_cast<const RegSpan*>(r.spans), r.level,
-                                                          r.seed, (unsigned long long)r.update);
+  weight_noise_kernel<<<param_grid(m), kThreads, 0, st>>>(m->flat.get(), r.noisy.get(),
+                                                          static_cast<const RegSpan*>(r.spans.get()), r.level, r.seed,
+                                                          (unsigned long long)r.update);
   LVSR_LAUNCH_CHECK();
   return 0;
-}
-
-void reg_free(lvsr_model* m) {
-  if (m->reg.noisy) cudaFree(m->reg.noisy);
-  if (m->reg.spans) cudaFree(m->reg.spans);
-  if (m->reg.penalty) cudaFree(m->reg.penalty);
-  m->reg = lvsr_model::Reg();
 }
 
 }  // namespace lvsr
@@ -282,7 +270,7 @@ int lvsr_train_set_adaptive_noise(lvsr_model* m, const lvsr_adaptive_noise* cfg)
   DeviceGuard device_guard(m);
   if (!cfg) {
     LVSR_CUDA_OK(cudaDeviceSynchronize());        // a training call may still read the buffers
-    noise_free(m);
+    m->noise = lvsr_model::Noise();
     return 0;
   }
   LVSR_CHECK(cfg->init_sigma > 0.0 && std::isfinite(cfg->init_sigma), "adaptive noise: init_sigma must be > 0");
@@ -293,21 +281,26 @@ int lvsr_train_set_adaptive_noise(lvsr_model* m, const lvsr_adaptive_noise* cfg)
   const size_t n = (size_t)m->flat_count, np = m->params.size();
   const size_t nparts = (size_t)kCtasPerParam * np;
   LVSR_CUDA_OK(cudaDeviceSynchronize());          // after every call queued on the handle, on any stream
-  if (!z.mem) {
-    LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&z.mem), 6 * n * sizeof(float)));
+  if (!z.mem) {                                   // both allocations, or neither
+    DeviceBuffer<float> mem;
+    DeviceBuffer<char> aux;
+    LVSR_CUDA_OK(mem.alloc(6 * n * sizeof(float)));
     const size_t span_bytes = (np * sizeof(Span) + 255) & ~(size_t)255;
-    LVSR_CUDA_OK(cudaMalloc(&z.aux, span_bytes + (4 + 4 * nparts) * sizeof(double) + nparts * sizeof(float)));
-    z.ls2 = z.mem; z.noisy = z.mem + n; z.gls2 = z.mem + 2 * n;
-    z.velocity = z.mem + 3 * n; z.ms_step = z.mem + 4 * n; z.ms_dx = z.mem + 5 * n;
-    z.spans = z.aux;
-    z.stats = reinterpret_cast<double*>(static_cast<char*>(z.aux) + span_bytes);
-    z.part = z.stats + 4;
-    z.norm_part = reinterpret_cast<float*>(z.part + 4 * nparts);
+    LVSR_CUDA_OK(aux.alloc(span_bytes + (4 + 4 * nparts) * sizeof(double) + nparts * sizeof(float)));
     std::vector<Span> h(np);
     for (size_t i = 0; i < np; ++i) h[i] = Span{m->params[i].offset, m->params[i].count};
-    LVSR_CUDA_OK(cudaMemcpy(z.spans, h.data(), np * sizeof(Span), cudaMemcpyHostToDevice));
+    LVSR_CUDA_OK(cudaMemcpy(aux.get(), h.data(), np * sizeof(Span), cudaMemcpyHostToDevice));
+    z.mem = std::move(mem);
+    z.aux = std::move(aux);
+    float* p = z.mem.get();
+    z.ls2 = p; z.noisy = p + n; z.gls2 = p + 2 * n;
+    z.velocity = p + 3 * n; z.ms_step = p + 4 * n; z.ms_dx = p + 5 * n;
+    z.spans = z.aux.get();
+    z.stats = reinterpret_cast<double*>(z.aux.get() + span_bytes);
+    z.part = z.stats + 4;
+    z.norm_part = reinterpret_cast<float*>(z.part + 4 * nparts);
   }
-  LVSR_CUDA_OK(cudaMemset(z.mem, 0, 6 * n * sizeof(float)));
+  LVSR_CUDA_OK(cudaMemset(z.mem.get(), 0, 6 * n * sizeof(float)));
   LVSR_CUDA_OK(cudaMemset(z.stats, 0, 4 * sizeof(double)));
   // graph.py:173-175: ls2 = log(init_sigma) * 2 / log_sigma_scale, in float32
   noise_fill_kernel<<<param_grid(m), kThreads>>>(z.ls2, spans_of(m), (float)(log(cfg->init_sigma) * 2.0 / kLogSigmaScale));
@@ -390,16 +383,19 @@ int lvsr_train_set_regularization(lvsr_model* m, const lvsr_regularization* cfg)
     LVSR_CHECK(cfg->penalty_coof >= 0.0 && std::isfinite(cfg->penalty_coof), "regularization: penalty_coof must be >= 0");
   }
   if (m->reg.spans || m->reg.penalty) LVSR_CUDA_OK(cudaDeviceSynchronize());     // a training call may still read the buffers
-  reg_free(m);
-  if (!cfg) return 0;
-  lvsr_model::Reg& r = m->reg;
+  // the new settings and buffers replace the handle's only once every allocation succeeded
+  lvsr_model::Reg r;
+  if (!cfg) {
+    m->reg = std::move(r);
+    return 0;
+  }
   r.dropout = cfg->dropout != 0;
   r.level = (float)cfg->noise_level;
   r.seed = cfg->seed ? cfg->seed : 1;
   r.penalty_coof = (float)cfg->penalty_coof;
   if (r.penalty_coof > 0.f) {
-    LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&r.penalty), sizeof(float)));
-    LVSR_CUDA_OK(cudaMemset(r.penalty, 0, sizeof(float)));
+    LVSR_CUDA_OK(r.penalty.alloc(sizeof(float)));
+    LVSR_CUDA_OK(cudaMemset(r.penalty.get(), 0, sizeof(float)));
   }
   if (r.level > 0.f) {
     // Blocks' apply_noise subjects: every parameter outside Selector(generator.transition.attention) (lvsr/main.py:297)
@@ -410,11 +406,12 @@ int lvsr_train_set_regularization(lvsr_model* m, const lvsr_regularization* cfg)
       const bool attention = name.rfind(std::string(ATT) + "/", 0) == 0 || name.rfind(std::string(CONT) + "/", 0) == 0;
       h[i] = RegSpan{m->params[i].offset, m->params[i].count, attention ? 0 : 1};
     }
-    LVSR_CUDA_OK(cudaMalloc(&r.spans, np * sizeof(RegSpan)));
-    LVSR_CUDA_OK(cudaMemcpy(r.spans, h.data(), np * sizeof(RegSpan), cudaMemcpyHostToDevice));
-    LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&r.noisy), (size_t)m->flat_count * sizeof(float)));
-    LVSR_CUDA_OK(cudaMemset(r.noisy, 0, (size_t)m->flat_count * sizeof(float)));
+    LVSR_CUDA_OK(r.spans.alloc(np * sizeof(RegSpan)));
+    LVSR_CUDA_OK(cudaMemcpy(r.spans.get(), h.data(), np * sizeof(RegSpan), cudaMemcpyHostToDevice));
+    LVSR_CUDA_OK(r.noisy.alloc((size_t)m->flat_count * sizeof(float)));
+    LVSR_CUDA_OK(cudaMemset(r.noisy.get(), 0, (size_t)m->flat_count * sizeof(float)));
   }
+  m->reg = std::move(r);
   return 0;
 }
 
@@ -424,7 +421,7 @@ int lvsr_train_penalty_sum(lvsr_model* m, float* penalty_dev, void* stream) {
   DeviceGuard device_guard(m);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (int rc = bind_stream(m, st)) return rc;
-  LVSR_CUDA_OK(cudaMemcpyAsync(penalty_dev, m->reg.penalty, sizeof(float), cudaMemcpyDeviceToDevice, st));
+  LVSR_CUDA_OK(cudaMemcpyAsync(penalty_dev, m->reg.penalty.get(), sizeof(float), cudaMemcpyDeviceToDevice, st));
   return 0;
 }
 
@@ -452,7 +449,7 @@ int lvsr_train_weight_noise_sample(lvsr_model* m, int64_t update, float* eps_dev
   if (int rc = bind_stream(m, st)) return rc;
   ProfScope prof("weight_noise", st);
   LVSR_CUDA_OK(cudaMemsetAsync(eps_dev, 0, (size_t)m->flat_count * sizeof(float), st));
-  weight_noise_kernel<<<param_grid(m), kThreads, 0, st>>>(nullptr, eps_dev, static_cast<const RegSpan*>(m->reg.spans),
+  weight_noise_kernel<<<param_grid(m), kThreads, 0, st>>>(nullptr, eps_dev, static_cast<const RegSpan*>(m->reg.spans.get()),
                                                           0.f, m->reg.seed, (unsigned long long)update);
   LVSR_LAUNCH_CHECK();
   return 0;

@@ -135,13 +135,13 @@ int lvsr_beam_search_many(lvsr_model* m, const float* attended, const float* pre
   struct FreeLm { char* p; cudaStream_t s; ~FreeLm() { if (p) cudaFreeAsync(p, s); } } free_lm{lm_dev, st};
   // the LM status word travels with the step's own copies and is checked after its synchronisations
   auto lm_fetch = [&]() -> int {
-    if (lm) LVSR_CUDA_OK(cudaMemcpyAsync(h_lm, m->lm_status, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+    if (lm) LVSR_CUDA_OK(cudaMemcpyAsync(h_lm, m->lm_status.get(), sizeof(unsigned), cudaMemcpyDeviceToHost, st));
     return 0;
   };
   auto lm_check = [&]() -> int {
     if (!lm || *h_lm == 0) return 0;
     const unsigned s = *h_lm;
-    LVSR_CUDA_OK(cudaMemsetAsync(m->lm_status, 0, sizeof(unsigned), st));
+    LVSR_CUDA_OK(cudaMemsetAsync(m->lm_status.get(), 0, sizeof(unsigned), st));
     return lm_report(s);
   };
 

@@ -99,21 +99,19 @@ extern "C" int lvsr_alignment_stats(lvsr_model* m, const float* weights_dev, con
   LVSR_CUDA_OK(cudaDeviceGetAttribute(&smem_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
   LVSR_CHECK(smem + 1024 <= (size_t)smem_max, "alignment_stats: T' = %d exceeds the %d positions a CTA holds", Tp,
              (int)((smem_max - 1024) / sizeof(double)));
-  if (B > m->align_rows) {                        // regrown: the previous call may still use the partials
-    if (m->align_mem) {
-      LVSR_CUDA_OK(cudaStreamSynchronize(st));
-      cudaFree(m->align_mem);
-      m->align_mem = nullptr;
-      m->align_rows = 0;
+  const size_t need = 256 + 2 * (size_t)B * sizeof(double);
+  if (need > m->align_mem.bytes()) {              // regrown: the previous call may still use the partials
+    LVSR_CUDA_OK(m->align_mem.grow(need, st));    // a failed allocation leaves it empty: the next call regrows it
+    const cudaError_t e = cudaMemsetAsync(m->align_mem.get(), 0, 256, st);
+    if (e != cudaSuccess) {
+      m->align_mem.reset();                       // so does a counter that was not zeroed
+      return set_error("cudaMemsetAsync(alignment_stats counter) failed: %s", cudaGetErrorString(e));
     }
-    LVSR_CUDA_OK(cudaMalloc(&m->align_mem, 256 + 2 * (size_t)B * sizeof(double)));
-    LVSR_CUDA_OK(cudaMemsetAsync(m->align_mem, 0, 256, st));
-    m->align_rows = B;
   }
   if (smem > 48 * 1024)
     LVSR_CUDA_OK(cudaFuncSetAttribute(alignment_stats_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  unsigned* done = static_cast<unsigned*>(m->align_mem);
-  double* part = reinterpret_cast<double*>(static_cast<char*>(m->align_mem) + 256);
+  unsigned* done = static_cast<unsigned*>(m->align_mem.get());
+  double* part = reinterpret_cast<double*>(static_cast<char*>(m->align_mem.get()) + 256);
   alignment_stats_kernel<<<B, AS_THREADS, smem, st>>>(weights_dev, labels_mask_dev, L, B, Tp, part, done, out_dev);
   LVSR_LAUNCH_CHECK();
   return 0;

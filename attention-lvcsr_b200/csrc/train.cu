@@ -218,7 +218,7 @@ struct TrainStep {
     if (int rc = transpose(m->P(g + "/readout/merge/transform_weighted_averages.W"), WmcT, E, Cpm, st)) return rc;
     if (int rc = transpose(m->P(t + "/transition.state_to_state"), WstateT, C, C, st)) return rc;
     if (int rc = transpose(m->P(t + "/transition.state_to_gates"), WgT, C, 2 * C, st)) return rc;
-    if (int rc = transpose(m->dec[0].Wd, WdcatT, E, 3 * C, st)) return rc;
+    if (int rc = transpose(m->dec[0].Wd.get(), WdcatT, E, 3 * C, st)) return rc;
     // [dG (3C)] . WcombT [3C, C + E] = [ grad of s_{i-1} through the gates | grad of the glimpse ]: one product per step
     float* WcombT = ws.f32((size_t)3 * C * (C + E));
     LVSR_CHECK(WcombT, "out of device memory (transposed weights)");
@@ -317,9 +317,9 @@ struct TrainStep {
                    win && lohi,
                "out of device memory (decoder backward)");
     if (int rc = lvsr_preprocess(m, d.Hatt, Tp, B, P, st)) return rc;
-    if (int rc = gemm_nn(d.CTX, R, E, E, m->dec[0].Wd, 3 * C, 3 * C, nullptr, G, 3 * C, false, st)) return rc;
+    if (int rc = gemm_nn(d.CTX, R, E, E, m->dec[0].Wd.get(), 3 * C, 3 * C, nullptr, G, 3 * C, false, st)) return rc;
     if (int rc = gemm_nn(d.S_prev, R, C, C, m->P(t + "/transition.state_to_gates"), 2 * C, 2 * C, nullptr, G, 3 * C, true, st)) return rc;
-    dec_gates_kernel<<<grid1d((long long)R * 3 * C), 256, 0, st>>>(G, m->dec[0].FF, lab, d.S_prev, R, C, Z, Rg, HR);
+    dec_gates_kernel<<<grid1d((long long)R * 3 * C), 256, 0, st>>>(G, m->dec[0].FF.get(), lab, d.S_prev, R, C, Z, Rg, HR);
     LVSR_LAUNCH_CHECK();
     {
       ArenaMark mark{ws};
@@ -348,7 +348,7 @@ struct TrainStep {
       LVSR_CHECK(pen && rows, "out of device memory (alignment penalty)");
       penalty_grad_kernel<<<ceil_div(R, 256), 256, 0, st>>>(d.W_all, lmask, L, B, Tp, penalty_coof * gscale, pen, rows);
       LVSR_LAUNCH_CHECK();
-      sum_all_kernel<<<1, 1024, 0, st>>>(rows, R, m->reg.penalty, 1.f);
+      sum_all_kernel<<<1, 1024, 0, st>>>(rows, R, m->reg.penalty.get(), 1.f);
       LVSR_LAUNCH_CHECK();
     }
     void (*att_bwd)(AttBwdArgs, int) = att_bwd_content_kernel;
@@ -440,7 +440,7 @@ struct TrainStep {
       // FF[y] = W_fork[y, :] + b: the gradient of the fork weights IS dFF
       LVSR_CUDA_OK(cudaMemcpyAsync(dWff, dFF, (size_t)(V + 1) * 3 * C * sizeof(float), cudaMemcpyDeviceToDevice, st));
     } else {
-      if (int rc = transpose(m->dec[0].Wff, WffT, Cfb, 3 * C, st)) return rc;
+      if (int rc = transpose(m->dec[0].Wff.get(), WffT, Cfb, 3 * C, st)) return rc;
       const float* look = m->P(g + "/readout/lookupfeedback/lookuptable.W");
       if (int rc = gemm_nn(dFF, V + 1, 3 * C, 3 * C, WffT, Cfb, Cfb, nullptr, grad(g + "/readout/lookupfeedback/lookuptable.W"), Cfb, false, st)) return rc;
       if (int rc = gemm_tn(ws, look, Cfb, dFF, 3 * C, V + 1, Cfb, 3 * C, dWff, 3 * C, false, st)) return rc;
@@ -603,7 +603,7 @@ struct TrainStep {
         float* dX = ws.f32((size_t)rows * tp.Din);
         LVSR_CHECK(dX, "out of device memory (dX)");
         // dX = dPre . Wcat^T: the K-major form of the right-hand side [N = Din, K = 3 nd D] is Wcat itself
-        if (int rc = input_grad(tp.pre, rows, N, m->Wcat[l], tp.Din, dX, &plan[LVSR_ENC_DX])) return rc;
+        if (int rc = input_grad(tp.pre, rows, N, m->Wcat[l].get(), tp.Din, dX, &plan[LVSR_ENC_DX])) return rc;
         dout = dX0 = dX;
       }
     }
@@ -636,7 +636,7 @@ int forward_backward_on(lvsr_model* m, const float* copy, const float* x, const 
   struct Restore {
     lvsr_model* m;
     ~Restore() {
-      for (Param& p : m->params) p.dev = m->flat + p.offset;
+      for (Param& p : m->params) p.dev = m->flat.get() + p.offset;
       m->finalized = false;
       m->noise.stale = true;         // the step may still read the noisy packing on its own stream (check_ready)
     }
@@ -673,7 +673,7 @@ int lvsr_train_cost_and_grads(lvsr_model* m, const float* x, const float* mask, 
   if (weight_noise) {
     // weight noise (noise.cu): the step runs on p + level eps, the attention's parameters as they are
     if (int rc = weight_noise_sample(m, st)) return rc;
-    return forward_backward_on(m, r.noisy, x, mask, labels, lmask, T, B, L, gscale, cost_out, grads, stream, drop);
+    return forward_backward_on(m, r.noisy.get(), x, mask, labels, lmask, T, B, L, gscale, cost_out, grads, stream, drop);
   }
   return forward_backward(m, x, mask, labels, lmask, T, B, L, gscale, cost_out, grads, stream, drop);
 }
@@ -704,45 +704,51 @@ int lvsr_train_apply_updates(lvsr_model* m, float* grads, float gscale, const lv
       h[i].cols = (int)(m->params[i].ndim == 2 ? m->params[i].shape[1] : 1);
       h[i].is_weight = is_weight_name(m->params[i].name) ? 1 : 0;
     }
-    LVSR_CUDA_OK(cudaMalloc(&m->opt_desc, sizeof(ParamDesc) * np));
-    LVSR_CUDA_OK(cudaMemcpyAsync(m->opt_desc, h.data(), sizeof(ParamDesc) * np, cudaMemcpyHostToDevice, st));
+    DeviceBuffer<void> opt_desc;
+    DeviceBuffer<float> opt_scratch;
+    LVSR_CUDA_OK(opt_desc.alloc(sizeof(ParamDesc) * np));
+    LVSR_CUDA_OK(cudaMemcpyAsync(opt_desc.get(), h.data(), sizeof(ParamDesc) * np, cudaMemcpyHostToDevice, st));
     LVSR_CUDA_OK(cudaStreamSynchronize(st));         // h goes away on return (once per handle)
-    LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->opt_scratch), 1032 * sizeof(float)));
+    LVSR_CUDA_OK(opt_scratch.alloc(1032 * sizeof(float)));
+    m->opt_desc = std::move(opt_desc);               // both tables, or neither
+    m->opt_scratch = std::move(opt_scratch);
   }
-  auto lazy = [&](float** p) -> int {
-    if (*p) return 0;
-    LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(p), (size_t)n * sizeof(float)));
-    LVSR_CUDA_OK(cudaMemsetAsync(*p, 0, (size_t)n * sizeof(float), st));
+  auto lazy = [&](DeviceBuffer<float>& p) -> int {
+    if (p) return 0;
+    LVSR_CUDA_OK(p.alloc((size_t)n * sizeof(float)));
+    LVSR_CUDA_OK(cudaMemsetAsync(p.get(), 0, (size_t)n * sizeof(float), st));
     return 0;
   };
-  if (tc->use_momentum) if (int rc = lazy(&m->opt_velocity)) return rc;
-  if (tc->use_adadelta) { if (int rc = lazy(&m->opt_ms_step)) return rc; if (int rc = lazy(&m->opt_ms_dx)) return rc; }
-  const ParamDesc* desc = static_cast<const ParamDesc*>(m->opt_desc);
+  if (tc->use_momentum) if (int rc = lazy(m->opt_velocity)) return rc;
+  if (tc->use_adadelta) { if (int rc = lazy(m->opt_ms_step)) return rc; if (int rc = lazy(m->opt_ms_dx)) return rc; }
+  const ParamDesc* desc = static_cast<const ParamDesc*>(m->opt_desc.get());
+  float* flat = m->flat.get();
   if (tc->decay > 0.f) {
     dim3 grid(64, np);
-    add_decay_kernel<<<grid, 256, 0, st>>>(grads, m->flat, desc, np, 2.f * tc->decay / gscale);
+    add_decay_kernel<<<grid, 256, 0, st>>>(grads, flat, desc, np, 2.f * tc->decay / gscale);
     LVSR_LAUNCH_CHECK();
   }
-  float* part = m->opt_scratch;
-  float* norm = m->opt_scratch + 1024;
+  float* part = m->opt_scratch.get();
+  float* norm = part + 1024;
   if (z.on) {
     // both gradient groups of adaptive noise (noise.cu), already multiplied by gscale; one clipping norm over both
     int nparts = 0;
     if (int rc = noise_gradients(m, grads, gscale, z.gls2, st, &nparts)) return rc;
-    sqnorm_final_kernel<<<1, 32, 0, st>>>(z.norm_part, nparts, 1.f, norm, m->clip);
+    sqnorm_final_kernel<<<1, 32, 0, st>>>(z.norm_part, nparts, 1.f, norm, m->clip.get());
     LVSR_LAUNCH_CHECK();
     gscale = 1.f;
   } else {
     const int nparts = (int)std::min<long long>(1024, std::max<long long>(1, n / 4096));
     sqnorm_partial_kernel<<<nparts, 256, 0, st>>>(grads, n, part);
     LVSR_LAUNCH_CHECK();
-    sqnorm_final_kernel<<<1, 32, 0, st>>>(part, nparts, gscale, norm, m->clip);
+    sqnorm_final_kernel<<<1, 32, 0, st>>>(part, nparts, gscale, norm, m->clip.get());
     LVSR_LAUNCH_CHECK();
   }
   StepArgs a = {};
-  a.grads = grads; a.params = m->flat; a.velocity = m->opt_velocity; a.ms_step = m->opt_ms_step; a.ms_dx = m->opt_ms_dx;
+  a.grads = grads; a.params = flat; a.velocity = m->opt_velocity.get(); a.ms_step = m->opt_ms_step.get();
+  a.ms_dx = m->opt_ms_dx.get();
   a.norm = norm; a.n = n; a.gscale = gscale; a.decay = tc->decay; a.threshold = tc->gradient_threshold;
-  a.clip = m->clip;
+  a.clip = m->clip.get();
   a.use_momentum = tc->use_momentum; a.learning_rate = tc->scale; a.momentum = tc->momentum;
   a.use_adadelta = tc->use_adadelta; a.decay_rate = tc->decay_rate; a.epsilon = tc->epsilon;
   step_rules_kernel<<<grid1d(n, 256, 1184), 256, 0, st>>>(a);
@@ -755,7 +761,7 @@ int lvsr_train_apply_updates(lvsr_model* m, float* grads, float gscale, const lv
   }
   if (tc->max_norm > 0.f) {
     dim3 grid(32, np);
-    max_norm_kernel<<<grid, 256, 0, st>>>(grads, m->flat, desc, tc->max_norm);
+    max_norm_kernel<<<grid, 256, 0, st>>>(grads, flat, desc, tc->max_norm);
     LVSR_LAUNCH_CHECK();
   }
   float burn_mult = 1.f;
@@ -766,7 +772,7 @@ int lvsr_train_apply_updates(lvsr_model* m, float* grads, float gscale, const lv
   }
   m->reg.update++;     // the next step draws a fresh dropout mask and weight noise
   if (z.on) {          // RemoveNotFinite per tensor: every ls2 is a tensor of its own; no max-norm (PARAMETER role only)
-    apply_update_pair_kernel<<<2 * np, 256, 0, st>>>(m->flat, grads, z.ls2, z.gls2, desc, np, burn_mult);
+    apply_update_pair_kernel<<<2 * np, 256, 0, st>>>(flat, grads, z.ls2, z.gls2, desc, np, burn_mult);
     LVSR_LAUNCH_CHECK();
     z.update++;
     z.sampled = false;
@@ -776,7 +782,7 @@ int lvsr_train_apply_updates(lvsr_model* m, float* grads, float gscale, const lv
     m->finalized = false;
     return 0;
   }
-  apply_update_kernel<<<np, 256, 0, st>>>(m->flat, grads, desc, burn_mult);
+  apply_update_kernel<<<np, 256, 0, st>>>(flat, grads, desc, burn_mult);
   LVSR_LAUNCH_CHECK();
   if (m->reg.level > 0.f) {
     // as under adaptive noise: the next training forward packs its noisy copy, other entry points pack the means
@@ -790,7 +796,7 @@ int lvsr_train_apply_updates(lvsr_model* m, float* grads, float gscale, const lv
 int lvsr_train_gradient_norm(lvsr_model* m, float* norm_host) {
   LVSR_CHECK(m && norm_host && m->opt_scratch, "train_gradient_norm: no update has run yet");
   DeviceGuard device_guard(m);
-  return copy_on_handle(m, norm_host, m->opt_scratch + 1024, sizeof(float), cudaMemcpyDeviceToHost);   // after the update
+  return copy_on_handle(m, norm_host, m->opt_scratch.get() + 1024, sizeof(float), cudaMemcpyDeviceToHost);   // after the update
 }
 
 int lvsr_train_reset(lvsr_model* m) {
@@ -798,11 +804,11 @@ int lvsr_train_reset(lvsr_model* m) {
   DeviceGuard device_guard(m);
   const size_t bytes = (size_t)m->flat_count * sizeof(float);
   cudaStream_t st = m->stream;     // after every update queued on the handle, before the next one
-  if (m->opt_velocity) LVSR_CUDA_OK(cudaMemsetAsync(m->opt_velocity, 0, bytes, st));
-  if (m->opt_ms_step) LVSR_CUDA_OK(cudaMemsetAsync(m->opt_ms_step, 0, bytes, st));
-  if (m->opt_ms_dx) LVSR_CUDA_OK(cudaMemsetAsync(m->opt_ms_dx, 0, bytes, st));
+  if (m->opt_velocity) LVSR_CUDA_OK(cudaMemsetAsync(m->opt_velocity.get(), 0, bytes, st));
+  if (m->opt_ms_step) LVSR_CUDA_OK(cudaMemsetAsync(m->opt_ms_step.get(), 0, bytes, st));
+  if (m->opt_ms_dx) LVSR_CUDA_OK(cudaMemsetAsync(m->opt_ms_dx.get(), 0, bytes, st));
   if (m->noise.on) LVSR_CUDA_OK(cudaMemsetAsync(m->noise.velocity, 0, 3 * bytes, st));     // velocity | ms_step | ms_dx of ls2
-  if (m->clip) LVSR_CUDA_OK(cudaMemcpyAsync(m->clip, m->clip_init, sizeof(m->clip_init), cudaMemcpyHostToDevice, st));
+  if (m->clip) LVSR_CUDA_OK(cudaMemcpyAsync(m->clip.get(), m->clip_init, sizeof(m->clip_init), cudaMemcpyHostToDevice, st));
   m->burn_in_left = -1;
   m->reg.update = 0;
   return 0;
@@ -815,8 +821,7 @@ int lvsr_train_set_adaptive_clipping(lvsr_model* m, const lvsr_adaptive_clipping
   if (!cfg) {
     if (m->clip) {
       LVSR_CUDA_OK(cudaStreamSynchronize(m->stream));     // an update queued on the handle may still read the state
-      cudaFree(m->clip);
-      m->clip = nullptr;
+      m->clip.reset();
     }
     return 0;
   }
@@ -829,9 +834,9 @@ int lvsr_train_set_adaptive_clipping(lvsr_model* m, const lvsr_adaptive_clipping
   c[CLIP_THR] = c[CLIP_NEXT] = c[CLIP_THR0] = cfg->initial_threshold;
   c[CLIP_DECAY] = cfg->decay_rate;
   c[CLIP_BURNIN] = (double)cfg->burnin_period;
-  if (!m->clip) LVSR_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&m->clip), sizeof(m->clip_init)));
+  if (!m->clip) LVSR_CUDA_OK(m->clip.alloc(sizeof(m->clip_init)));
   // after every update queued on the handle; the host image lives in the handle, so the copy needs no wait
-  LVSR_CUDA_OK(cudaMemcpyAsync(m->clip, c, sizeof(m->clip_init), cudaMemcpyHostToDevice, m->stream));
+  LVSR_CUDA_OK(cudaMemcpyAsync(m->clip.get(), c, sizeof(m->clip_init), cudaMemcpyHostToDevice, m->stream));
   return 0;
 }
 
@@ -839,7 +844,7 @@ int lvsr_train_clipping_threshold(lvsr_model* m, double* threshold_host) {
   LVSR_CHECK(m && threshold_host, "null argument");
   LVSR_CHECK(m->clip, "adaptive clipping is off (lvsr_train_set_adaptive_clipping)");
   DeviceGuard device_guard(m);
-  return copy_on_handle(m, threshold_host, m->clip + CLIP_NEXT, sizeof(double), cudaMemcpyDeviceToHost);
+  return copy_on_handle(m, threshold_host, m->clip.get() + CLIP_NEXT, sizeof(double), cudaMemcpyDeviceToHost);
 }
 
 }  // extern "C"

@@ -570,6 +570,8 @@ int lvsr_frontend_dither_sample(lvsr_frontend* f, int32_t B, int32_t T, float* d
 
 /* Counters for bench.py: number of kernels this library launched since the last reset. */
 int64_t lvsr_launch_count(int reset);
+/* Bytes of device memory the library's model and front-end handles hold (their workspaces included), process-wide. */
+int64_t lvsr_device_bytes(void);
 
 /* Per-kernel-class device timing (CUDA events recorded on the launching stream around every
  * launch of that class) -- the analogue of the reference's Theano ProfileStats
