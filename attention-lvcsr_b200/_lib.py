@@ -60,6 +60,13 @@ class LvsrConfig(C.Structure):
 
 
 LVSR_MAX_BOTTOM = 4
+LVSR_MAX_READOUT = 4
+
+
+class LvsrReadoutConfig(C.Structure):
+    """Mirror of ``lvsr_readout_config`` (include/lvsr_b200.h)."""
+    _fields_ = [("num_layers", C.c_int32), ("dims", C.c_int32 * LVSR_MAX_READOUT)]
+
 LVSR_MAX_BOTTOM_DIM = 4096
 # activations of the bottom MLP (LVSR_ACT_* values of lvsr_bottom_config.activation)
 BOTTOM_ACTIVATIONS = {"relu": 1, "tanh": 2}
@@ -143,6 +150,9 @@ SIGNATURES = {
     "lvsr_model_create": (C.c_int, [C.POINTER(LvsrConfig), C.POINTER(_P)]),
     "lvsr_model_create_bottom": (C.c_int, [C.POINTER(LvsrConfig), C.POINTER(LvsrBottomConfig), C.POINTER(_P)]),
     "lvsr_model_create_encoder": (C.c_int, [C.POINTER(LvsrConfig), C.POINTER(LvsrBottomConfig), C.c_int32, C.POINTER(_P)]),
+    "lvsr_readout_max_width": (C.c_int, []),
+    "lvsr_model_create_readout": (C.c_int, [C.POINTER(LvsrConfig), C.POINTER(LvsrBottomConfig), C.c_int32,
+                                            C.POINTER(LvsrReadoutConfig), C.POINTER(_P)]),
     "lvsr_model_destroy": (C.c_int, [_P]),
     "lvsr_model_num_params": (C.c_int, [_P]),
     "lvsr_model_param_name": (C.c_char_p, [_P, C.c_int]),

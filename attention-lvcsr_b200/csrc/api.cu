@@ -108,8 +108,12 @@ void build_param_table(lvsr_model* m) {
   }
   add_param(m, g + "/readout/merge/transform_weighted_averages.W", E, Cpm);
   add_param(m, g + "/readout/post_merge/bias.b", Cpm);
-  add_param(m, g + "/readout/post_merge/mlp/linear_0.b", V);
-  add_param(m, g + "/readout/post_merge/mlp/linear_0.W", Cpm / c.maxout_pieces, V);
+  // MLP.children = [linear_0 .. linear_{k-1}]; Linear._initialize draws b before W (B/bricks/interfaces.py:195-200)
+  for (int j = 0, k = readout_depth(m); j < k; ++j) {
+    const int din = j ? readout_dim(m, j) : Cpm / c.maxout_pieces, dout = j + 1 < k ? readout_dim(m, j + 1) : V;
+    add_param(m, readout_linear(j) + ".b", dout);
+    add_param(m, readout_linear(j) + ".W", din, dout);
+  }
   add_param(m, g + "/fork/fork_inputs.b", C);
   add_param(m, g + "/fork/fork_inputs.W", Cfb, C);
   add_param(m, g + "/fork/fork_gate_inputs.b", 2 * C);
@@ -248,24 +252,69 @@ static int transition(lvsr_model* m, int R, const float* states, const float* ct
   return 0;
 }
 
-int readout_merged(lvsr_model* m, int R, const float* states, const float* ctx, float* merged, cudaStream_t st) {
+int readout_merged(lvsr_model* m, int R, const float* states, const float* ctx, float* merged, const float** tail,
+                   cudaStream_t st) {
   const lvsr_config& c = m->cfg;
+  const bool deep = readout_depth(m) > 1;
   DenseArgs d = {};
   const int S = state_dim(m), N = c.post_merge_dim;
   d.op[0] = {ctx, m->E, m->E, m->P(std::string(GEN) + "/readout/merge/transform_weighted_averages.W"), N};
   if (c.use_states_for_readout) d.op[1] = {states, S, S, readout_state_weights(m), N};
   d.R = R; d.N = N; d.mode = DENSE_PLAIN; d.out = merged;
-  return dense_step(d, st);
+  if (deep) {                      // h_0 = act(merge + post_merge/bias.b) in the merge's epilogue
+    d.mode = DENSE_ACT;
+    d.bias = m->P(std::string(GEN) + "/readout/post_merge/bias.b");
+    d.act = c.post_merge_activation;
+  }
+  if (int rc = dense_step(d, st)) return rc;
+  return readout_body(m, m->ws, R, merged, false, tail, nullptr, st);
 }
 
-ReadoutArgs readout_args(lvsr_model* m, int R, const float* merged) {
+int readout_body(lvsr_model* m, Arena& ws, int R, const float* h0, bool bulk, const float** tail, const float** hidden,
+                 cudaStream_t st) {
+  const int k = readout_depth(m);
+  *tail = h0;
+  if (k == 1) return 0;
+  ProfScope prof("readout_body", st);
+  const int act = m->cfg.post_merge_activation;
+  const float* h = h0;
+  if (hidden) hidden[0] = h0;
+  for (int j = 0; j + 1 < k; ++j) {
+    const int din = readout_dim(m, j), dout = readout_dim(m, j + 1);
+    const bool last = j + 2 == k;
+    float* out = ws.f32((size_t)R * dout);
+    LVSR_CHECK(out, "out of device memory (readout hidden layer)");
+    const float* W = m->P(readout_linear(j) + ".W");
+    const float* b = m->P(readout_linear(j) + ".b");
+    if (bulk) {
+      GemmArgs g = make_gemm(h, R, din, W, dout, last ? nullptr : b, out);
+      if (!last) g.act = act;
+      if (int rc = gemm_bias(g, st)) return rc;
+    } else {
+      DenseArgs d = {};
+      d.op[0] = {h, din, din, W, dout};
+      d.R = R; d.N = dout; d.out = out; d.mode = last ? DENSE_PLAIN : DENSE_ACT; d.bias = b; d.act = act;
+      if (int rc = dense_step(d, st)) return rc;
+    }
+    if (last) {
+      *tail = out;
+    } else {
+      h = out;
+      if (hidden) hidden[j + 1] = out;
+    }
+  }
+  return 0;
+}
+
+ReadoutArgs readout_args(lvsr_model* m, int R, const float* tail) {
   const lvsr_config& c = m->cfg;
+  const int k = readout_depth(m);
   ReadoutArgs r = {};
-  r.merged = merged;
-  r.b_pm = m->P(std::string(GEN) + "/readout/post_merge/bias.b");
-  r.Wo = m->P(std::string(GEN) + "/readout/post_merge/mlp/linear_0.W");
-  r.bo = m->P(std::string(GEN) + "/readout/post_merge/mlp/linear_0.b");
-  r.R = R; r.Cpm = c.post_merge_dim; r.pieces = c.maxout_pieces; r.V = c.num_phonemes; r.act = c.post_merge_activation;
+  r.merged = tail;
+  r.b_pm = m->P(k == 1 ? std::string(GEN) + "/readout/post_merge/bias.b" : readout_linear(k - 2) + ".b");
+  r.Wo = m->P(readout_linear(k - 1) + ".W");
+  r.bo = m->P(readout_linear(k - 1) + ".b");
+  r.R = R; r.Cpm = readout_dim(m, k - 1); r.pieces = c.maxout_pieces; r.V = c.num_phonemes; r.act = c.post_merge_activation;
   r.tle = tle_criterion(m) ? 1 : 0;
   return r;
 }
@@ -324,7 +373,7 @@ size_t cost_ws_bytes(const lvsr_model* m, int Tp, int B, int L) {
   size_t f = (size_t)Tp * B * c.dim_matcher + (size_t)2 * Tp * B * m->E + (size_t)(L + 1) * B * S + (size_t)L * B * m->E +
              (size_t)4 * B * Tp + (size_t)L * B * c.post_merge_dim + (size_t)B * c.dim_matcher +
              (size_t)L * B * (Tp + c.dim_matcher + S + 1) +
-             (size_t)3 * B * c.dim_dec + 4 * B + 64;
+             (size_t)3 * B * c.dim_dec + 4 * B + 64 + (size_t)L * B * readout_hidden_floats(m);
   return f * sizeof(float) + (1 << 16);
 }
 
@@ -375,7 +424,18 @@ int lvsr_model_create_bottom(const lvsr_config* cfg, const lvsr_bottom_config* b
   return lvsr_model_create_encoder(cfg, bottom, 1, out);
 }
 
+int lvsr_readout_max_width(void) {
+  int H = 0;
+  while (readout_smem_bytes(H + 8) <= READOUT_SMEM_LIMIT && readout_bwd_smem_bytes(H + 8) <= READOUT_SMEM_LIMIT) H += 8;
+  return H;
+}
+
 int lvsr_model_create_encoder(const lvsr_config* cfg, const lvsr_bottom_config* bottom, int32_t bidir, lvsr_model** out) {
+  return lvsr_model_create_readout(cfg, bottom, bidir, nullptr, out);
+}
+
+int lvsr_model_create_readout(const lvsr_config* cfg, const lvsr_bottom_config* bottom, int32_t bidir,
+                              const lvsr_readout_config* readout, lvsr_model** out) {
   LVSR_CHECK(cfg && out, "null argument");
   LVSR_CHECK(bidir == 0 || bidir == 1, "bidir %d unsupported (1: bidirectional encoder, 0: forward-only encoder)", bidir);
   if (bottom) {
@@ -412,6 +472,24 @@ int lvsr_model_create_encoder(const lvsr_config* cfg, const lvsr_bottom_config* 
   LVSR_CHECK(content || cfg->conv_n >= 1, "conv_n must be >= 1 (got %d)", cfg->conv_n);
   LVSR_CHECK(cfg->num_phonemes >= 1 && cfg->num_phonemes <= 128, "num_phonemes out of range");
   LVSR_CHECK(cfg->dec_stack >= 0 && cfg->dec_stack <= 2, "dec_stack %d unsupported (1 or 2)", cfg->dec_stack);
+  lvsr_readout_config ro = {1, {cfg->post_merge_dim}};
+  if (readout) {
+    const int k = readout->num_layers;
+    LVSR_CHECK(k >= 1 && k <= LVSR_MAX_READOUT, "post_merge_dims: %d layers (1 .. %d)", k, (int)LVSR_MAX_READOUT);
+    LVSR_CHECK(readout->dims[0] == cfg->post_merge_dim, "post_merge_dims[0] = %d must equal post_merge_dim %d",
+               readout->dims[0], cfg->post_merge_dim);
+    for (int j = 1; j < k; ++j)
+      LVSR_CHECK(readout->dims[j] >= 8 && readout->dims[j] % 8 == 0,
+                 "post_merge_dims: width %d of layer %d must be a positive multiple of 8", readout->dims[j], j);
+    LVSR_CHECK(k == 1 || cfg->post_merge_activation != LVSR_ACT_MAXOUT || cfg->maxout_pieces == 1,
+               "post_merge_dims: %d layers under Maxout(%d): a Maxout of more than one piece takes one post-merge layer "
+               "only (the reference's MLP takes d_j / pieces inputs that its Maxout divides again)", k,
+               cfg->maxout_pieces);
+    LVSR_CHECK(k == 1 || readout->dims[k - 1] <= lvsr_readout_max_width(),
+               "post_merge_dims: last width %d above %d, the widest the readout kernels stage in shared memory",
+               readout->dims[k - 1], lvsr_readout_max_width());
+    ro = *readout;
+  }
   int dev_count = 0;
   LVSR_CUDA_OK(cudaGetDeviceCount(&dev_count));
   LVSR_CHECK(dev_count > 0, "no CUDA device: the GPU path has no CPU fallback");
@@ -419,6 +497,7 @@ int lvsr_model_create_encoder(const lvsr_config* cfg, const lvsr_bottom_config* 
   m->cfg = *cfg;
   m->ndir = bidir ? 2 : 1;
   if (bottom && bottom->num_layers > 0) m->bottom = *bottom;
+  m->readout = ro;
   if (m->cfg.dec_stack == 0) m->cfg.dec_stack = 1;     // callers that predate the field zero-fill it
   if (content) {
     // SequenceContentAttention takes none of these (lvsr/bricks/recognizer.py:261-265): softmax weights over every
@@ -1176,8 +1255,14 @@ int lvsr_cost_matrix_groundtruth(lvsr_model* m, const float* attended, const flo
     }
     GemmArgs b = make_gemm(ctx_all, R, E, m->P(g + "/readout/merge/transform_weighted_averages.W"), c.post_merge_dim,
                            nullptr, merged, acc);
+    if (readout_depth(m) > 1) {          // h_0 = act(merge + post_merge/bias.b) in the merge's epilogue
+      b.bias = m->P(g + "/readout/post_merge/bias.b");
+      b.act = c.post_merge_activation;
+    }
     if (int rc = gemm_bias(b, st)) return rc;
-    ReadoutArgs r = readout_args(m, R, merged);
+    const float* tail = nullptr;
+    if (int rc = readout_body(m, ws, R, merged, true, &tail, nullptr, st)) return rc;
+    ReadoutArgs r = readout_args(m, R, tail);
     r.poison = scanned ? m->status.get() : nullptr;
     if (tle) {
       // RewardRegressionEmitter.cost over the whole readouts (lvsr/bricks/__init__.py:135-184)
@@ -1245,8 +1330,9 @@ int lvsr_logprobs(lvsr_model* m, const float* attended, const float* preprocesse
   LVSR_CHECK(w_tmp && e_tmp && ctx && merged, "out of device memory (logprobs workspace)");
   if (int rc = glimpses(m, attended, P, attended_mask, Tp, U, row_utt, R, states, weights,
                         reinterpret_cast<const long long*>(step), 0, w_tmp, e_tmp, ctx, st)) return rc;
-  if (int rc = readout_merged(m, R, states, ctx, merged, st)) return rc;
-  ReadoutArgs r = readout_args(m, R, merged);
+  const float* tail = nullptr;
+  if (int rc = readout_merged(m, R, states, ctx, merged, &tail, st)) return rc;
+  ReadoutArgs r = readout_args(m, R, tail);
   r.costs_all = out;
   return readout_costs(r, st);
 }
@@ -1301,8 +1387,9 @@ int search_expand(lvsr_model* m, const float* attended, const float* preprocesse
   // surviving parents, the state update (next_state_computer) -- B/search.py:109-142 computes it twice
   if (int rc = glimpses(m, attended, preprocessed, attended_mask, Tp, U, row_utt, R, states, weights, step, 0,
                         new_weights, new_energies, wavg, st, sg)) return rc;
-  if (int rc = readout_merged(m, R, states, wavg, merged, st)) return rc;
-  ReadoutArgs r = readout_args(m, R, merged);
+  const float* tail = nullptr;
+  if (int rc = readout_merged(m, R, states, wavg, merged, &tail, st)) return rc;
+  ReadoutArgs r = readout_args(m, R, tail);
   r.costs_all = neglogp;
   if (lm_add) lm_fuse(m, r, lm_add);
   if (int rc = readout_costs(r, st)) return rc;

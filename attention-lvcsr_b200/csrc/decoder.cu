@@ -25,6 +25,16 @@ namespace {
 constexpr int DR = 64;   // rows per CTA
 constexpr int DN = 8;    // columns per CTA
 
+// post_merge activation of the readout's hidden layers (LVSR_ACT_*; Maxout is accepted there with one piece only, which
+// is the identity): the same expressions as readout_kernel's
+__device__ __forceinline__ float readout_act(float v, int act) {
+  if (act == LVSR_ACT_RELU) return fmaxf(v, 0.f);
+  if (act == LVSR_ACT_TANH) return tanhf(v);
+  return v;
+}
+
+// kAct: the DENSE_ACT epilogue; the other modes are the kAct = false instantiation
+template <bool kAct>
 __global__ void __launch_bounds__(256) dense_kernel(DenseArgs a) {
   __shared__ __align__(16) float red[8][DR * DN];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -90,7 +100,9 @@ __global__ void __launch_bounds__(256) dense_kernel(DenseArgs a) {
       if (a.arow && a.add_rows > 0) ar = ar < 0 ? 0 : (ar > a.add_rows - 1 ? a.add_rows - 1 : ar);
       v += a.add[ar * a.N + c];
     }
-    if (a.mode == DENSE_PLAIN) {
+    if constexpr (kAct) {
+      a.out[(long long)r * a.N + c] = readout_act(v + a.bias[c], a.act);
+    } else if (a.mode == DENSE_PLAIN) {
       a.out[(long long)r * a.N + c] = v;
     } else if (a.mode == DENSE_GATES) {
       const int C = a.C;
@@ -338,8 +350,10 @@ int dense_step(const DenseArgs& a, cudaStream_t stream) {
   for (const DenseOperand& p : a.op)
     LVSR_CHECK(!p.X || (p.K % 4 == 0 && p.ldx % 4 == 0 && p.ncols % 4 == 0),
                "dense_step: dimensions and strides must be multiples of 4 (K=%d ldx=%d ncols=%d)", p.K, p.ldx, p.ncols);
+  LVSR_CHECK(a.mode != DENSE_ACT || a.bias, "dense_step: DENSE_ACT without a bias");
   dim3 grid(ceil_div(a.N, DN), ceil_div(a.R, DR));
-  dense_kernel<<<grid, 256, 0, stream>>>(a);
+  if (a.mode == DENSE_ACT) dense_kernel<true><<<grid, 256, 0, stream>>>(a);
+  else dense_kernel<false><<<grid, 256, 0, stream>>>(a);
   LVSR_LAUNCH_CHECK();
   return 0;
 }
@@ -349,8 +363,8 @@ int readout_costs(const ReadoutArgs& a, cudaStream_t stream) {
   if (a.R <= 0) return 0;
   LVSR_CHECK(a.V <= 128, "readout: num_phonemes %d > 128 unsupported", a.V);
   LVSR_CHECK(a.pieces >= 1 && a.Cpm % a.pieces == 0, "readout: bad maxout pieces");
-  const size_t smem = (size_t)8 * (a.Cpm / a.pieces) * sizeof(float);
-  LVSR_CHECK(smem <= 48 * 1024, "readout: post_merge_dim too large");
+  const size_t smem = readout_smem_bytes(a.Cpm / a.pieces);
+  LVSR_CHECK(smem <= READOUT_SMEM_LIMIT, "readout: post_merge_dim too large");
   LVSR_CHECK(!(a.tle && a.lm_add), "readout: the task-loss emitter takes no language model");
   if (a.tle) readout_kernel<true><<<ceil_div(a.R, 8), 256, smem, stream>>>(a);
   else readout_kernel<false><<<ceil_div(a.R, 8), 256, smem, stream>>>(a);

@@ -4,6 +4,7 @@
 //   Fork(Linear) of RecurrentWithFork  (lvsr/bricks/__init__.py:39-43, B/bricks/simple.py:73-76)
 //   attention.preprocess               (lvsr/bricks/attention.py:228-230)
 //   Readout merge                      (B/bricks/sequence_generators.py:614-619)
+//   post_merge MLP hidden layers       (lvsr/bricks/recognizer.py:305-320; act(. + b) in the epilogue)
 //
 // fp32 FFMA tiles (128x128x8, 8x8 per thread, double-buffered shared memory): the
 // 1e-4 parity gate against the float64 oracle rules out single-pass bf16/tf32 here.
@@ -17,7 +18,16 @@ namespace {
 constexpr int BM = 128, BN = 128, BK = 8;
 constexpr int APAD = 4;
 
-template <bool VEC>
+// the readout hidden layers' activations (readout_act in decoder.cu): Rectifier as fmaxf, Tanh
+template <int ACT>
+__device__ __forceinline__ float epilogue_act(float v) {
+  if (ACT == LVSR_ACT_RELU) return fmaxf(v, 0.f);
+  if (ACT == LVSR_ACT_TANH) return tanhf(v);
+  return v;
+}
+
+// ACT: GemmArgs::act as a template argument (LVSR_ACT_IDENTITY: no activation)
+template <bool VEC, int ACT>
 __global__ void __launch_bounds__(256)
 gemm_kernel(GemmArgs g) {
   __shared__ __align__(16) float As[2][BK][BM + APAD];
@@ -128,6 +138,8 @@ gemm_kernel(GemmArgs g) {
           const float4 o = *cp;
           v[0] += o.x; v[1] += o.y; v[2] += o.z; v[3] += o.w;
         }
+#pragma unroll
+        for (int q = 0; q < 4; ++q) v[q] = epilogue_act<ACT>(v[q]);
         *cp = make_float4(v[0], v[1], v[2], v[3]);
       } else {
 #pragma unroll
@@ -135,12 +147,19 @@ gemm_kernel(GemmArgs g) {
           if (c + q < g.N) {
             float o = v[q] + (g.bias ? g.bias[c + q] : 0.f);
             if (g.accumulate) o += crow[c + q];
-            crow[c + q] = o;
+            crow[c + q] = epilogue_act<ACT>(o);
           }
         }
       }
     }
   }
+}
+
+template <bool VEC>
+void launch_gemm(const GemmArgs& g, dim3 grid, cudaStream_t stream) {
+  if (g.act == LVSR_ACT_RELU) gemm_kernel<VEC, LVSR_ACT_RELU><<<grid, 256, 0, stream>>>(g);
+  else if (g.act == LVSR_ACT_TANH) gemm_kernel<VEC, LVSR_ACT_TANH><<<grid, 256, 0, stream>>>(g);
+  else gemm_kernel<VEC, LVSR_ACT_IDENTITY><<<grid, 256, 0, stream>>>(g);
 }
 
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
@@ -156,9 +175,9 @@ int gemm_bias(const GemmArgs& g, cudaStream_t stream) {
                    aligned16(g.W) && aligned16(g.C) && (g.bias == nullptr || aligned16(g.bias));
   dim3 grid(ceil_div(g.N, BN), ceil_div(g.M, BM));
   if (vec)
-    gemm_kernel<true><<<grid, 256, 0, stream>>>(g);
+    launch_gemm<true>(g, grid, stream);
   else
-    gemm_kernel<false><<<grid, 256, 0, stream>>>(g);
+    launch_gemm<false>(g, grid, stream);
   LVSR_LAUNCH_CHECK();
   return 0;
 }

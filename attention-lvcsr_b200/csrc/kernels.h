@@ -3,6 +3,7 @@
 #include <cuda_fp16.h>
 
 #include "common.cuh"
+#include "lvsr_b200.h"
 
 namespace lvsr {
 
@@ -19,6 +20,7 @@ struct GemmArgs {
   float* C;                // [M, N], leading dimension ldc
   int ldc;
   int accumulate;          // C += ... instead of C = ...
+  int act;                 // LVSR_ACT_RELU / LVSR_ACT_TANH: C = act(...) after the bias and the accumulation; other: none
 };
 int gemm_bias(const GemmArgs& g, cudaStream_t stream);
 
@@ -27,6 +29,7 @@ inline GemmArgs make_gemm(const float* A, int M, int K, const float* W, int N, c
   GemmArgs g;
   g.A = A; g.M = M; g.K = K; g.rows_per_block = M > 0 ? M : 1; g.block_stride = 0; g.lda = K;
   g.W = W; g.N = N; g.ldw = N; g.bias = bias; g.C = C; g.ldc = N; g.accumulate = accumulate ? 1 : 0;
+  g.act = LVSR_ACT_IDENTITY;
   return g;
 }
 
@@ -159,7 +162,7 @@ int attention_max_cluster();
 
 // ---- decoder.cu ---------------------------------------------------------------------
 // out[R,N] = epilogue( sum over the operands, in order, of X[R,K].W[K,ncols] (columns < ncols only) + add[arow[r]] )
-enum { DENSE_PLAIN = 0, DENSE_GATES = 1, DENSE_CAND = 2 };
+enum { DENSE_PLAIN = 0, DENSE_GATES = 1, DENSE_CAND = 2, DENSE_ACT = 3 };
 struct DenseOperand {
   const float* X; int K, ldx;   // X [R, K], row stride ldx; null: no operand
   const float* W; int ncols;    // W [K, ncols], ncols <= N
@@ -170,8 +173,9 @@ struct DenseArgs {
   const long long* arow;   // [R] row index into add (labels) or nullptr (identity)
   long long add_rows;      // rows of `add` when arow is given (0 = unknown): indices are clamped into the table
   int R, N, mode;
-  // DENSE_PLAIN: out[R,N]
+  // DENSE_PLAIN: out[R,N]; DENSE_ACT: out[R,N] = act(acc + bias) (a readout hidden layer, act LVSR_ACT_*)
   float* out;
+  const float* bias; int act;
   // DENSE_GATES (N = 3C): cols [0,C) update -> z[R,C]; [C,2C) reset -> hr[R,C] = s*r; [2C,3C) -> ai[R,C]
   // DENSE_CAND  (N = C):  c = tanh(acc + ai); s' = c*z + s*(1-z); optional row mask blend -> out[R,C], row stride ld_out
   const float* s; int ld_s;   // [R, C] current states, row stride ld_s
@@ -204,6 +208,11 @@ struct ReadoutArgs {
   int tle;
 };
 int readout_costs(const ReadoutArgs& a, cudaStream_t stream);
+// Shared memory the readout kernels stage per CTA of 8 rows for a last hidden width H: readout_kernel (decoder.cu) and
+// the training step's readout_bwd_kernel (train_kernels.cuh), each at most READOUT_SMEM_LIMIT
+constexpr size_t READOUT_SMEM_LIMIT = 48 * 1024;
+constexpr size_t readout_smem_bytes(int H) { return (size_t)8 * H * sizeof(float); }
+constexpr size_t readout_bwd_smem_bytes(int H) { return (size_t)8 * (H + 128) * sizeof(float); }
 
 // ---- tle.cu: task loss estimation, RewardOp + RewardRegressionEmitter.cost (lvsr/ops.py:236-294,
 // lvsr/error_rate.py:11-112, lvsr/bricks/__init__.py:135-184) --------------------------------------------------------

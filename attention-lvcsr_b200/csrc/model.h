@@ -97,6 +97,7 @@ using namespace lvsr;
 struct lvsr_model {
   lvsr_config cfg;
   lvsr_bottom_config bottom = {};   // the bottom MLP in front of the encoder (num_layers 0: none)
+  lvsr_readout_config readout = {}; // the readout's post-merge depth and widths (read through readout_depth / _dim)
   int device = 0;                   // the GPU this handle lives on (current device at lvsr_model_create)
   int ndir = 2;                     // encoder directions: 2 bidirectional, 1 forward only (read through encoder_dirs)
   int E;
@@ -229,6 +230,19 @@ static inline std::string dec_gru(const lvsr_model* m, int level) {
   return std::string(TR) + "/recurrentstack/transition_" + std::to_string(level) + "#" + std::to_string(level);
 }
 
+// The readout's post-merge MLP (lvsr_readout_config): depth k, width d_{j+1} of hidden layer j (readout_dim(m, 0) is
+// post_merge_dim), the Blocks path of its Linear j, and the floats per row of the hidden layers above h_0
+static inline int readout_depth(const lvsr_model* m) { return m->readout.num_layers; }
+static inline int readout_dim(const lvsr_model* m, int j) { return m->readout.dims[j]; }
+static inline std::string readout_linear(int j) {
+  return std::string(GEN) + "/readout/post_merge/mlp/linear_" + std::to_string(j);
+}
+static inline size_t readout_hidden_floats(const lvsr_model* m) {
+  size_t n = 0;
+  for (int j = 1; j < readout_depth(m); ++j) n += readout_dim(m, j);
+  return n;
+}
+
 // Directions of every encoder layer: 2 for Bidirectional, 1 for a forward-only RecurrentWithFork (net.bidir False,
 // lvsr/bricks/__init__.py:54-78).  Layer l's output, and layer l + 1's input, is encoder_dirs(m) * dims_bidir[l] wide.
 static inline int encoder_dirs(const lvsr_model* m) { return m->ndir; }
@@ -359,8 +373,20 @@ size_t bottom_ws_bytes(const lvsr_model* m, int rows);
 // LVSR_ENC_OPS_* of the kernel that ran
 int projection_gemm(Arena& ws, const float* A, int M, int K, const float* W, const TcWeights* tw, int N,
                     const float* bias, float* out, cudaStream_t st, int* kpad = nullptr, int* operands = nullptr);
-int readout_merged(lvsr_model* m, int R, const float* states, const float* ctx, float* merged, cudaStream_t st);
-ReadoutArgs readout_args(lvsr_model* m, int R, const float* merged);
+// Readout.merge of R step-wise rows into merged [R, post_merge_dim], then the post-merge body: *tail = the input of
+// the readout tail (readout_args).  Depth 1: merged itself; deeper: merged holds h_0 = act(merge + post_merge/bias.b)
+// and the body runs on buffers from m->ws.
+int readout_merged(lvsr_model* m, int R, const float* states, const float* ctx, float* merged, const float** tail,
+                   cudaStream_t st);
+// The post-merge body above h_0 [R, d_1] at depth k > 1: h_j = act(h_{j-1} W_{j-1} + b_{j-1}) for j = 1 .. k-2 (the bias
+// and the activation in the product's epilogue) and *tail = z = h_{k-2} W_{k-2}, whose bias and activation the tail
+// applies.  bulk: the tile GEMM (L*B teacher-forced rows), else dense_step.  Buffers from ws; hidden (null: not kept)
+// receives h_0 .. h_{k-2}.  Depth 1: *tail = h0, nothing runs.
+int readout_body(lvsr_model* m, Arena& ws, int R, const float* h0, bool bulk, const float** tail, const float** hidden,
+                 cudaStream_t st);
+// The readout tail (readout_costs) on `tail`: bias + activation + the last Linear + emitter.  Depth 1: post_merge/bias.b
+// and linear_0; deeper: linear_{k-2}.b and linear_{k-1}.
+ReadoutArgs readout_args(lvsr_model* m, int R, const float* tail);
 // language model (api.cu): the device view of the attached FST, the fusion fields of a readout, and the LM status
 // word read back after a synchronisation of st (an error return when a kernel reported one; the word is cleared)
 static inline bool lm_attached(const lvsr_model* m) { return (bool)m->lm_off; }

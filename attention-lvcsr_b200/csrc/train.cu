@@ -156,19 +156,21 @@ struct TrainStep {
   Arena& ws = m->tws;
   const long long* lab = reinterpret_cast<const long long*>(labels);
   const int C = c.dim_dec, E = m->E, M = c.dim_matcher, K = c.conv_num_filters, n = c.conv_n, w = 2 * n + 1;
-  const int V = c.num_phonemes, Cfb = c.dim_feedback, Cpm = c.post_merge_dim, Hd = Cpm / c.maxout_pieces;
+  // Hd: the readout tail's hidden width, d_k / pieces (pieces is 1 above depth 1)
+  const int V = c.num_phonemes, Cfb = c.dim_feedback, Cpm = c.post_merge_dim, Kro = readout_depth(m);
+  const int Hd = readout_dim(m, Kro - 1) / c.maxout_pieces;
   const int R = L * B, nct = AB_CS * B, tc_cap = ceil_div(Tp, AB_CS);
   const bool content = content_attention(m);
   // the logistic and relu energy gradients read the step's energies, which the softmax one does not need
   const bool keep_energies = c.energy_normalizer != LVSR_NORM_SOFTMAX;
-  const size_t ro_smem = (size_t)8 * (Hd + 128) * sizeof(float);
+  const size_t ro_smem = readout_bwd_smem_bytes(Hd);
   const size_t ab_smem = (content ? att_bwd_content_smem_floats(E, tc_cap) : att_bwd_smem_floats(M, E, K, n, tc_cap)) * sizeof(float);
   const std::string g = GEN, t = TR, at = att_base(m);
   float* grad(const std::string& name) const { const Param* p = m->param(name); return p ? grads + p->offset : nullptr; }
 
   int run(const float* x, const float* mask, int T, float* cost_out) const {
     // shapes the backward kernels cannot take are refused before any work is enqueued
-    LVSR_CHECK(ro_smem <= 48 * 1024 && V <= 128, "readout backward: post_merge_dim / num_phonemes too large");
+    LVSR_CHECK(ro_smem <= READOUT_SMEM_LIMIT && V <= 128, "readout backward: post_merge_dim / num_phonemes too large");
     LVSR_CHECK(ab_smem <= 227 * 1024 && M <= AB_NT && M % 128 == 0 && K <= 16 && E % 4 == 0,
                "attention backward: shape unsupported (Tp=%d M=%d)", Tp, M);
     LVSR_CHECK(E <= 1024, "encoded dim %d > 1024 unsupported in training", E);
@@ -193,6 +195,8 @@ struct TrainStep {
     bytes += ((size_t)Tp * B * (2 * M + 2 * E) + (size_t)R * (Tp + 8 * C + 3 * E + 2 * M + 3 * Cpm + V + 16) + (size_t)4 * B * Tp +
               (size_t)2 * B * (M + (size_t)K * M + (size_t)K * w) + (size_t)4 * (E + C) * 3 * C + (size_t)80 * E * M) * sizeof(float);
     if (keep_energies) bytes += ((size_t)R * Tp + (size_t)AB_CS * B) * sizeof(float);
+    for (int j = 1; j < Kro; ++j)         // the readout body: h_j, dh_j, z's gradient, W_{j-1}^T and TN partials
+      bytes += ((size_t)3 * R * readout_dim(m, j) + (size_t)81 * readout_dim(m, j - 1) * readout_dim(m, j) + 1024) * sizeof(float);
     if (drop) bytes += (size_t)T * B * encoder_input_dim(m) * sizeof(float);      // the dropped encoder input
     if (penalty_coof > 0.f) bytes += (size_t)R * (Tp + 1) * sizeof(float);      // penalty gradient and row sums
     ws.reserve(bytes, st);
@@ -253,28 +257,61 @@ struct TrainStep {
     LVSR_LAUNCH_CHECK();
     return 0;
   }
-  // Readout + emitter backward, all steps at once; dS_ro / dCtx_ro: its gradients of the states and the glimpses
+  // Readout + emitter backward, all steps at once; dS_ro / dCtx_ro: its gradients of the states and the glimpses.  Above
+  // depth 1 the merge's epilogue makes h_0, the body the hidden layers up to the tail's input, and after the tail's
+  // backward the body is walked top-down to the gradient of the merge.
   int readout_backward(const DecTape& d, const float* WmsT, const float* WmcT, float*& dS_ro, float*& dCtx_ro) const {
+    const int Clast = readout_dim(m, Kro - 1);
     float* merged = ws.f32((size_t)R * Cpm);
     float* hid = ws.f32((size_t)R * Hd);
     float* dlogits = ws.f32((size_t)R * V);
-    float* dmerged = ws.f32((size_t)R * Cpm);
+    float* dmerged = ws.f32((size_t)R * Clast);
     dS_ro = ws.f32((size_t)R * C);
     dCtx_ro = ws.f32((size_t)R * E);
     LVSR_CHECK(merged && hid && dlogits && dmerged && dS_ro && dCtx_ro, "out of device memory (readout backward)");
     if (c.use_states_for_readout)
       if (int rc = gemm_nn(d.S_prev, R, C, C, m->P(g + "/readout/merge/transform_states.W"), Cpm, Cpm, nullptr, merged, Cpm, false, st)) return rc;
-    if (int rc = gemm_nn(d.CTX, R, E, E, m->P(g + "/readout/merge/transform_weighted_averages.W"), Cpm, Cpm, nullptr, merged, Cpm,
-                         c.use_states_for_readout, st)) return rc;
+    {
+      GemmArgs mc = make_gemm(d.CTX, R, E, m->P(g + "/readout/merge/transform_weighted_averages.W"), Cpm, nullptr, merged,
+                              c.use_states_for_readout);
+      if (Kro > 1) {
+        mc.bias = m->P(g + "/readout/post_merge/bias.b");
+        mc.act = c.post_merge_activation;
+      }
+      if (int rc = gemm_bias(mc, st)) return rc;
+    }
+    const float* h[LVSR_MAX_READOUT] = {};
+    const float* tail = nullptr;
+    if (int rc = readout_body(m, ws, R, merged, true, &tail, h, st)) return rc;
+    const std::string top = readout_linear(Kro - 1);
     ReadoutBwdArgs rb = {};
-    rb.merged = merged; rb.b_pm = m->P(g + "/readout/post_merge/bias.b"); rb.Wo = m->P(g + "/readout/post_merge/mlp/linear_0.W");
-    rb.bo = m->P(g + "/readout/post_merge/mlp/linear_0.b");
-    rb.R = R; rb.Cpm = Cpm; rb.pieces = c.maxout_pieces; rb.V = V; rb.act = c.post_merge_activation;
+    rb.merged = tail; rb.b_pm = m->P(Kro == 1 ? g + "/readout/post_merge/bias.b" : readout_linear(Kro - 2) + ".b");
+    rb.Wo = m->P(top + ".W"); rb.bo = m->P(top + ".b");
+    rb.R = R; rb.Cpm = Clast; rb.pieces = c.maxout_pieces; rb.V = V; rb.act = c.post_merge_activation;
     rb.labels = lab; rb.lmask = lmask; rb.gscale = gscale; rb.hid = hid; rb.dlogits = dlogits; rb.dmerged = dmerged;
     readout_bwd_kernel<<<ceil_div(R, 8), 256, ro_smem, st>>>(rb);
     LVSR_LAUNCH_CHECK();
-    if (int rc = gemm_tn(ws, hid, Hd, dlogits, V, R, Hd, V, grad(g + "/readout/post_merge/mlp/linear_0.W"), V, false, st)) return rc;
-    if (int rc = colsum(dlogits, R, V, V, grad(g + "/readout/post_merge/mlp/linear_0.b"), false, st)) return rc;
+    if (int rc = gemm_tn(ws, hid, Hd, dlogits, V, R, Hd, V, grad(top + ".W"), V, false, st)) return rc;
+    if (int rc = colsum(dlogits, R, V, V, grad(top + ".b"), false, st)) return rc;
+    // dz: the gradient of the pre-activation of h_j, from j = k-1 down to 0 (h_0's is the merge's, dmerged [R, Cpm])
+    float* dz = dmerged;
+    for (int j = Kro - 2; j >= 0; --j) {
+      ProfScope prof("readout_body_bwd", st);
+      const int din = readout_dim(m, j), dout = readout_dim(m, j + 1);
+      const std::string lin = readout_linear(j);
+      if (int rc = colsum(dz, R, dout, dout, grad(lin + ".b"), false, st)) return rc;
+      if (int rc = gemm_tn(ws, h[j], din, dz, dout, R, din, dout, grad(lin + ".W"), dout, false, st)) return rc;
+      float* WT = ws.f32((size_t)dout * din);
+      float* dh = ws.f32((size_t)R * din);
+      LVSR_CHECK(WT && dh, "out of device memory (readout body backward)");
+      if (int rc = transpose(m->P(lin + ".W"), WT, din, dout, st)) return rc;
+      if (int rc = gemm_nn(dz, R, dout, dout, WT, din, din, nullptr, dh, din, false, st)) return rc;
+      // Rectifier and Tanh from the stored output; Identity and Maxout(1) pass the gradient as it is
+      if (c.post_merge_activation == LVSR_ACT_RELU || c.post_merge_activation == LVSR_ACT_TANH)
+        if (int rc = bottom_act_backward(dh, h[j], (long long)R * din, c.post_merge_activation, st)) return rc;
+      dz = dh;
+    }
+    dmerged = dz;
     if (int rc = colsum(dmerged, R, Cpm, Cpm, grad(g + "/readout/post_merge/bias.b"), false, st)) return rc;
     if (int rc = gemm_tn(ws, d.CTX, E, dmerged, Cpm, R, E, Cpm, grad(g + "/readout/merge/transform_weighted_averages.W"), Cpm, false, st)) return rc;
     if (int rc = gemm_nn(dmerged, R, Cpm, Cpm, WmcT, E, E, nullptr, dCtx_ro, E, false, st)) return rc;

@@ -124,8 +124,6 @@ class SpeechRecognizer(object):
         for tr in (enc_transition, dec_transition):
             if tr is not None and getattr(tr, "__name__", type(tr).__name__) != "GatedRecurrent":
                 unsupported("transition %r" % tr)
-        if post_merge_dims is not None and len(post_merge_dims) != 1:
-            unsupported("deep post_merge")
 
         self.name = name
         self.eos_label = eos_label
@@ -142,6 +140,23 @@ class SpeechRecognizer(object):
         self._brick_schemes = OrderedDict()          # {brick path below /recognizer: {scheme: value}}
 
         act = post_merge_activation if post_merge_activation is not None else _bricks.Tanh()
+        post_merge_dims = [int(d) for d in post_merge_dims] if post_merge_dims else []
+        if len(post_merge_dims) > 1:
+            # Bias(d_1) -> act -> MLP([act] * (k-1) + [Identity()], [d_j // pieces] + [V]) (recognizer.py:305-320)
+            k, pieces = len(post_merge_dims), int(getattr(act, "num_pieces", 1))
+            if k > _lib.LVSR_MAX_READOUT:
+                unsupported("a post-merge MLP of %d layers (post_merge_dims of at most %d entries)"
+                            % (k, _lib.LVSR_MAX_READOUT))
+            if any(d < 8 or d % 8 for d in post_merge_dims):
+                raise ValueError("post_merge_dims %r: every width must be a positive multiple of 8" % (post_merge_dims,))
+            if pieces > 1:
+                # the reference's MLP takes d_j // pieces inputs and its Maxout divides them again: the graph fails
+                raise ValueError("post_merge_dims %r under Maxout(%d): a Maxout of more than one piece takes one "
+                                 "post-merge layer only" % (post_merge_dims, pieces))
+            widest = _lib.load().lvsr_readout_max_width()
+            if post_merge_dims[-1] > widest:
+                unsupported("a last post-merge width of %d (at most %d: the widest the readout kernels stage in "
+                            "shared memory)" % (post_merge_dims[-1], widest))
         if dim_matcher is None:
             dim_matcher = dim_dec                                  # recognizer.py:225-226
         content = attention_type == "content"
@@ -162,7 +177,8 @@ class SpeechRecognizer(object):
             dim_feedback=(int(dim_dec if dim_output_embedding is None else dim_output_embedding) if embed_outputs
                           else int(num_phonemes) + 1),
             embed_outputs=bool(embed_outputs),
-            post_merge_dim=int(post_merge_dims[0]) if post_merge_dims else int(num_phonemes),
+            post_merge_dim=post_merge_dims[0] if post_merge_dims else int(num_phonemes),
+            post_merge_dims=post_merge_dims,
             post_merge_activation=act.kind, maxout_pieces=int(getattr(act, "num_pieces", 1)),
             use_states_for_readout=bool(use_states_for_readout),
             energy_normalizer=energy_normalizer or "softmax", prior=prior, attention_type=attention_type,
@@ -266,6 +282,17 @@ class SpeechRecognizer(object):
         out.activation = _lib.BOTTOM_ACTIVATIONS[b["activation"]]
         return out
 
+    def _make_readout_config(self):
+        """lvsr_readout_config of a post-merge MLP deeper than one layer, None otherwise."""
+        dims = self.net.get("post_merge_dims") or []
+        if len(dims) <= 1:
+            return None
+        out = _lib.LvsrReadoutConfig()
+        out.num_layers = len(dims)
+        for i, d in enumerate(dims):
+            out.dims[i] = d
+        return out
+
     def _require_ready(self):
         if self._handle is None:
             import ctypes as C
@@ -275,7 +302,11 @@ class SpeechRecognizer(object):
                 h = C.c_void_p()
                 cfg = self._make_config()
                 bottom = self._make_bottom_config()
-                if not self.bidir:
+                readout = self._make_readout_config()
+                if readout is not None:
+                    _lib.check(lib.lvsr_model_create_readout(C.byref(cfg), None if bottom is None else C.byref(bottom),
+                                                             int(self.bidir), C.byref(readout), C.byref(h)))
+                elif not self.bidir:
                     _lib.check(lib.lvsr_model_create_encoder(C.byref(cfg), None if bottom is None else C.byref(bottom),
                                                              0, C.byref(h)))
                 elif bottom is None:

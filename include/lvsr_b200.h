@@ -113,6 +113,27 @@ int lvsr_model_create_bottom(const lvsr_config* cfg, const lvsr_bottom_config* b
  * dims_bidir[num_layers - 1].  Any other value is refused before any device work.  Added within version 104: detect it
  * by its symbol. */
 int lvsr_model_create_encoder(const lvsr_config* cfg, const lvsr_bottom_config* bottom, int32_t bidir, lvsr_model** out);
+
+/* The readout's post-merge MLP of config['net']['post_merge_dims'] = [d_1 .. d_k] (lvsr/bricks/recognizer.py:305-320):
+ * Bias(d_1) -> act -> MLP([act] * (k-1) + [Identity], [d_1 .. d_k, V]), act = cfg->post_merge_activation.  With
+ * h_0 = act(merged + post_merge/bias.b), h_j = act(h_{j-1} W_{j-1} + b_{j-1}) for j = 1 .. k-1 and the logits
+ * h_{k-1} W_{k-1} + b_{k-1}; W_j = "/recognizer/generator/readout/post_merge/mlp/linear_<j>.W" [d_{j+1}, d_{j+2}] (the
+ * last [d_k, V]), each Linear's .b before its .W in the parameter table, as Blocks initialises them.  num_layers = k:
+ * 1 .. LVSR_MAX_READOUT; dims[0] must equal cfg->post_merge_dim.  Above depth 1 every width is a multiple of 8, the
+ * activation is not Maxout with more than one piece (the reference's MLP takes d_j / pieces inputs and its Maxout
+ * divides them again), and d_k is at most lvsr_readout_max_width(). */
+enum { LVSR_MAX_READOUT = 4 };
+typedef struct {
+  int32_t num_layers;              /* k = len(post_merge_dims), 1 .. LVSR_MAX_READOUT                            */
+  int32_t dims[LVSR_MAX_READOUT];  /* d_1 .. d_k                                                                 */
+} lvsr_readout_config;
+/* The widest last hidden layer the readout kernels (forward and training backward) stage in shared memory. */
+int lvsr_readout_max_width(void);
+/* lvsr_model_create_encoder with the readout's post-merge depth: readout NULL (or num_layers 1) is depth 1, which is
+ * lvsr_model_create_encoder itself.  A readout outside the rules above is refused before any device work.  Added within
+ * version 104: detect it by its symbol. */
+int lvsr_model_create_readout(const lvsr_config* cfg, const lvsr_bottom_config* bottom, int32_t bidir,
+                              const lvsr_readout_config* readout, lvsr_model** out);
 int lvsr_model_destroy(lvsr_model* m);
 
 /* Parameter table in Blocks order/names ("/recognizer/encoder/bidir0/forward/fork/fork_inputs.W"
