@@ -175,8 +175,27 @@ def beam_search(cfg, params, recordings, beam_size, **kw):
 # --------------------------------------------------------------------------
 
 
-def _cost_matrix_torch(cfg, p, attended, attended_mask, labels, labels_mask):
-    """mirror of cost_matrix above, in the style of G._cost_matrix."""
+def _readout_torch(cfg, p, states, weighted_averages):
+    """mirror of O.readout: the single-layer post_merge."""
+    import torch
+    r = weighted_averages @ p[O._GEN + "/readout/merge/transform_weighted_averages.W"]
+    if cfg["use_states_for_readout"]:
+        r = r + states @ p[O._GEN + "/readout/merge/transform_states.W"]
+    r = r + p[O._GEN + "/readout/post_merge/bias.b"]
+    act = cfg["post_merge_activation"]
+    if act == "maxout":
+        pieces = cfg["maxout_pieces"]
+        r = r.reshape(r.shape[:-1] + (r.shape[-1] // pieces, pieces)).max(dim=-1).values
+    elif act == "relu":
+        r = torch.clamp(r, min=0)
+    elif act == "tanh":
+        r = torch.tanh(r)
+    return r @ p[O._GEN + "/readout/post_merge/mlp/linear_0.W"] + p[O._GEN + "/readout/post_merge/mlp/linear_0.b"]
+
+
+def _cost_matrix_torch(cfg, p, attended, attended_mask, labels, labels_mask, readout=_readout_torch):
+    """mirror of cost_matrix above, in the style of G._cost_matrix; `readout(cfg, p, states, weighted_averages)` gives
+    the logits of every step (readout_oracle.readout_torch for a deep readout)."""
     import torch
     L, B = labels.shape
     P = attended @ p[CONT + "/preprocess.W"] + p[CONT + "/preprocess.b"]
@@ -199,21 +218,7 @@ def _cost_matrix_torch(cfg, p, attended, attended_mask, labels, labels_mask):
         s = G._gru_step(s, a, g, p[O._TR + "/transition.state_to_state"], p[O._TR + "/transition.state_to_gates"],
                         None if labels_mask is None else labels_mask[i])
         ctxs.append(wavg)
-    prev, ctx = torch.stack(prev), torch.stack(ctxs)
-    r = ctx @ p[O._GEN + "/readout/merge/transform_weighted_averages.W"]
-    if cfg["use_states_for_readout"]:
-        r = r + prev @ p[O._GEN + "/readout/merge/transform_states.W"]
-    r = r + p[O._GEN + "/readout/post_merge/bias.b"]
-    act = cfg["post_merge_activation"]
-    if act == "maxout":
-        pieces = cfg["maxout_pieces"]
-        r = r.reshape(r.shape[:-1] + (r.shape[-1] // pieces, pieces)).max(dim=-1).values
-    elif act == "relu":
-        r = torch.clamp(r, min=0)
-    elif act == "tanh":
-        r = torch.tanh(r)
-    r = r @ p[O._GEN + "/readout/post_merge/mlp/linear_0.W"] + p[O._GEN + "/readout/post_merge/mlp/linear_0.b"]
-    logp = torch.log_softmax(r, dim=-1)
+    logp = torch.log_softmax(readout(cfg, p, torch.stack(prev), torch.stack(ctxs)), dim=-1)
     costs = -torch.gather(logp, 2, torch.as_tensor(labels)[..., None])[..., 0]
     if labels_mask is not None:
         costs = costs * labels_mask

@@ -14,15 +14,19 @@ Everything else is oracle/lvsr_oracle.py's (O.make_config asserts one post-merge
 builds the single-layer config and widens its post_merge_dims).  The decoder's recurrence never reads the readout,
 so the teacher-forced cost takes the oracle's states and glimpses (O.cost_matrix on parameters whose readout is
 depth 1, shallow_params) and applies the deep readout to them.  The torch float64 mirror (cost_and_grads, train_step)
-restates G._cost_matrix's loop with the deep readout on top and takes G's step rules.
+restates G._cost_matrix's loop (content_oracle's for content attention) with the deep readout on top and takes G's
+step rules.  relu_kinks screens every Rectifier layer for pre-activations on the derivative's jump, and clear_kinks
+moves those units' biases off it.
 
 tests/test_readout_depth_cpu.py pins this module: depth 1 is O.readout, the body is Blocks' MLP restated, known
-answers for a 2-layer Tanh and a 3-layer Rectifier readout, the mirror against numpy and central differences.
+answers for a 2-layer Tanh and a 3-layer Rectifier readout, both mirrors against numpy and central differences, the
+kink screen on a hand-built readout.
 """
 from collections import OrderedDict
 
 import numpy as np
 
+from helpers import KINK_EPS
 from oracle import lvsr_oracle as O
 from oracle import lvsr_oracle_grad as G
 
@@ -92,15 +96,25 @@ def activation(cfg, x):
     return x
 
 
-def hidden(cfg, params, states, weighted_averages):
-    """[h_0 .. h_{k-1}] of the readout."""
+def bias_name(j):
+    """The bias added to the pre-activation of h_j: post_merge/bias.b for h_0, linear_{j-1}.b above it."""
+    return PM + "/bias.b" if j == 0 else linear_name(j - 1) + ".b"
+
+
+def pre_activations(cfg, params, states, weighted_averages):
+    """[z_0 .. z_{k-1}] of the readout, h_j = act(z_j)."""
     r = weighted_averages.dot(params[O._GEN + "/readout/merge/transform_weighted_averages.W"])
     if cfg["use_states_for_readout"]:
         r = r + states.dot(params[O._GEN + "/readout/merge/transform_states.W"])
-    h = [activation(cfg, r + params[PM + "/bias.b"])]
+    z = [r + params[PM + "/bias.b"]]
     for j in range(len(cfg["post_merge_dims"]) - 1):
-        h.append(activation(cfg, O.linear(h[-1], params[linear_name(j) + ".W"], params[linear_name(j) + ".b"])))
-    return h
+        z.append(O.linear(activation(cfg, z[-1]), params[linear_name(j) + ".W"], params[linear_name(j) + ".b"]))
+    return z
+
+
+def hidden(cfg, params, states, weighted_averages):
+    """[h_0 .. h_{k-1}] of the readout."""
+    return [activation(cfg, z) for z in pre_activations(cfg, params, states, weighted_averages)]
 
 
 def readout(cfg, params, states, weighted_averages):
@@ -118,6 +132,45 @@ def shallow_params(cfg, params):
     for leaf in (".b", ".W"):
         p[linear_name(0) + leaf] = np.zeros(shapes[linear_name(0) + leaf])
     return p
+
+
+def relu_kinks(cfg, params, states, weighted_averages, live=None, eps=KINK_EPS):
+    """(j, step, utterance, unit) of every Rectifier pre-activation z_j of h_0 .. h_{k-1} within eps of 0 on a live row
+    (live: [L, B] bool, None for every row).  The derivative jumps at 0, and a float32 forward may land on either side of
+    it, which changes that row's backward through the unit.  [] for the other activations."""
+    if cfg["post_merge_activation"] != "relu":
+        return []
+    out = []
+    for j, z in enumerate(pre_activations(cfg, params, states, weighted_averages)):
+        near = np.abs(z) < eps
+        if live is not None:
+            near &= np.asarray(live, bool)[..., None]
+        out += [(j,) + tuple(int(v) for v in i) for i in np.argwhere(near)]
+    return out
+
+
+def clear_kinks(cfg, params, states, weighted_averages, live=None, eps=KINK_EPS):
+    """params with the bias of every unit relu_kinks finds moved off the kink, h_0 first (a move in h_j moves every layer
+    above it): by the smallest of +-3 eps, +-4 eps, .. that leaves every live row of the unit at least 2 eps from 0.
+    Both sides of a comparison take the result, so the float32 forward and the float64 one take the same side of every
+    unit.  Returns (params, [(j, unit, shift)]); asserts that the screen of the result is empty."""
+    p = OrderedDict(params)
+    moved = []
+    for j in range(len(cfg["post_merge_dims"]) if cfg["post_merge_activation"] == "relu" else 0):
+        z = pre_activations(cfg, p, states, weighted_averages)[j]
+        rows = z.reshape(-1, z.shape[-1]) if live is None else z[np.asarray(live, bool)]
+        units = np.flatnonzero((np.abs(rows) < eps).any(axis=0))
+        if not units.size:
+            continue
+        b = np.array(p[bias_name(j)], dtype=np.float64)
+        for u in units:
+            shift = next(s * n * eps for n in range(3, 1000) for s in (1, -1)
+                         if (np.abs(rows[:, u] + s * n * eps) >= 2 * eps).all())
+            b[u] += shift
+            moved.append((j, int(u), shift))
+        p[bias_name(j)] = b.astype(np.asarray(params[bias_name(j)]).dtype)
+    assert not relu_kinks(cfg, p, states, weighted_averages, live, eps)
+    return p, moved
 
 
 def cost_matrix(cfg, params, attended, attended_mask, labels, labels_mask=None, return_all=False, emitter="softmax"):
@@ -244,8 +297,16 @@ def _cost_matrix_torch(cfg, p, attended, attended_mask, labels, labels_mask):
     return costs
 
 
+def _content_cost_matrix_torch(cfg, p, attended, attended_mask, labels, labels_mask):
+    """mirror of cost_matrix above over content attention (attention_type: content): content_oracle's loop, then the
+    deep readout."""
+    import content_oracle as CO
+    return CO._cost_matrix_torch(cfg, p, attended, attended_mask, labels, labels_mask, readout=readout_torch)
+
+
 def cost_and_grads(cfg, params, recordings, recordings_mask, labels, labels_mask, decay=0.0, return_costs=False):
-    """G.cost_and_grads for the deep readout: sum(costs) / B (+ decay * ||WEIGHT||^2) and its float64 gradient."""
+    """G.cost_and_grads for the deep readout: sum(costs) / B (+ decay * ||WEIGHT||^2) and its float64 gradient.  A
+    content-attention config (content_oracle.make_config) runs the content mirror."""
     import torch
     p = OrderedDict((k, torch.tensor(np.asarray(v, dtype=np.float64), requires_grad=True)) for k, v in params.items())
     x = torch.as_tensor(np.asarray(recordings, dtype=np.float64))
@@ -253,7 +314,8 @@ def cost_and_grads(cfg, params, recordings, recordings_mask, labels, labels_mask
     lm = None if labels_mask is None else torch.as_tensor(np.asarray(labels_mask, dtype=np.float64))
     labels = np.asarray(labels, dtype=np.int64)
     attended, amask = G._encoder(cfg, p, x, m)
-    costs = _cost_matrix_torch(cfg, p, attended, amask, labels, lm)
+    mirror = _content_cost_matrix_torch if cfg.get("attention_type") == "content" else _cost_matrix_torch
+    costs = mirror(cfg, p, attended, amask, labels, lm)
     cost = costs.sum() / labels.shape[1]
     if decay > 0:
         cost = cost + decay * sum((v ** 2).sum() for k, v in p.items() if G.is_weight(k))

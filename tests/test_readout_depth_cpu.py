@@ -220,3 +220,91 @@ def test_config_keeps_dec_stack_last_and_version():
     ro = re.search(r"typedef struct \{([^}]*)\} lvsr_readout_config;", header, re.S).group(1)
     assert [f for f, _ in pkg._lib.LvsrReadoutConfig._fields_] == \
         re.findall(r"\b(\w+)(?:\[\w+\])?;", re.sub(r"/\*.*?\*/", "", ro, flags=re.S))
+
+
+def _content_costs(cfg, params, batch):
+    """The content model's cost matrix with the deep readout, from content_oracle's numpy decoder and RO.readout."""
+    import content_oracle as CO
+    x, m, labels, lm = batch
+    r = CO.recognizer_cost(cfg, RO.shallow_params(cfg, params), x, m, labels, lm, return_all=True)
+    logits = RO.readout(cfg, params, r["states"], r["weighted_averages"])
+    return -np.take_along_axis(O.log_softmax(logits), labels[..., None], axis=-1)[..., 0] * lm
+
+
+@pytest.mark.parametrize("dims,act,use_states", [([16, 24], "tanh", True), ([16, 8, 16], "relu", False)])
+def test_content_mirror_and_its_gradient(dims, act, use_states):
+    """The deep readout over content attention: RO.cost_and_grads on a content config runs content_oracle's loop with
+    the deep readout; its costs equal content_oracle's decoder plus RO.readout, its gradients central differences."""
+    pytest.importorskip("torch")
+    import content_oracle as CO
+    cfg = CO.make_config(num_features=6, dims_bidir=[8], dim_dec=8, dim_matcher=8, num_phonemes=5,
+                         post_merge_dims=dims[:1], post_merge_activation=act, maxout_pieces=1,
+                         use_states_for_readout=use_states)
+    cfg["post_merge_dims"] = list(dims)
+    deep = RO.init_params(small_cfg(dims, act, use_states), seed=2, scale=20.0)
+    params = {}
+    for k, v in CO.init_params(dict(cfg, post_merge_dims=dims[:1]), seed=2, scale=20.0).items():
+        params[k] = deep[k] if k.startswith(RO.PM + "/") else v
+    params.update((k, v) for k, v in deep.items() if k.startswith(RO.PM + "/mlp/"))
+    batch = O.synthetic_batch(cfg, B=2, T=10, seed=4)
+    cost, grads, costs = RO.cost_and_grads(cfg, params, *batch, return_costs=True)
+    assert set(grads) == set(params)
+    want = _content_costs(cfg, params, batch)
+    assert_allclose(costs, want, rtol=1e-11, atol=1e-11)
+    assert abs(cost - want.sum() / batch[2].shape[1]) < 1e-11
+    # a deep readout changes the costs: the mirror does not fall back to the single-layer readout
+    assert np.abs(want - CO.recognizer_cost(cfg, RO.shallow_params(cfg, params), *batch)).max() > 1e-3
+    rng = np.random.RandomState(0)
+    eps = 1e-6
+    names = [RO.PM + "/bias.b", CO.CONT + "/energy_comp/linear.W", CO.CONT + "/state_trans/transform_states.W"] + \
+        [RO.linear_name(j) + leaf for j in range(len(dims)) for leaf in (".W", ".b")]
+    for name in names:
+        assert grads[name].any(), name
+        for _ in range(3):
+            idx = tuple(rng.randint(n) for n in params[name].shape)
+            plus, minus = dict(params), dict(params)
+            plus[name], minus[name] = params[name].copy(), params[name].copy()
+            plus[name][idx] += eps
+            minus[name][idx] -= eps
+            fd = (_content_costs(cfg, plus, batch).sum() - _content_costs(cfg, minus, batch).sum()) / (
+                2 * eps * batch[2].shape[1])
+            assert abs(fd - grads[name][idx]) <= 1e-6 * max(1.0, abs(fd)), (name, idx, fd, grads[name][idx])
+
+
+def test_kink_screen_finds_every_rectifier_layer():
+    """relu_kinks reports the pre-activations of h_0, h_1 and h_2 within eps of 0 on live rows, and nothing else;
+    clear_kinks moves exactly those units' biases, the way that keeps the unit's other rows off the kink."""
+    cfg = small_cfg([8, 8, 8], "relu", use_states=False)
+    eps = 1e-5
+    p = {k: np.zeros(v) for k, v in RO.param_shapes(cfg).items()}
+    Wc = p[O._GEN + "/readout/merge/transform_weighted_averages.W"]
+    for u in range(8):
+        Wc[u, u] = 1.0                                              # z_0 = ctx[:8] + b
+    p[RO.PM + "/bias.b"][:] = 0.5
+    p[RO.linear_name(0) + ".W"][:] = np.eye(8)
+    p[RO.linear_name(0) + ".b"][:] = -1.0                           # z_1 = h_0 - 1
+    p[RO.linear_name(1) + ".W"][:] = np.eye(8)
+    p[RO.linear_name(1) + ".b"][:] = 0.25                           # z_2 = relu(z_1) + 0.25
+    p[RO.linear_name(1) + ".b"][5] = -2.0                           # z_2[5] = relu(z_1[5]) - 2
+    ctx = np.ones((3, 2, 16))                                       # z_0 = 1.5, z_1 = 0.5 everywhere
+    ctx[0, 1, 2] = -0.5 + 3e-6                                      # z_0[2] = 3e-6: h_0 kink
+    ctx[2, 0, 4] = 0.5 - 4e-6                                       # z_1[4] = -4e-6: h_1 kink
+    ctx[1, 1, 5] = 2.5 + 2e-6                                       # z_2[5] = 2e-6: h_2 kink
+    ctx[1, 0, 6] = -0.5                                             # z_0[6] = 0 exactly, on a masked row
+    ctx[2, 1, 2] = -0.5 - 2e-5                                      # z_0[2] = -2e-5: near, not within eps
+    live = np.ones((3, 2), bool)
+    live[1, 0] = False
+    assert sorted(RO.relu_kinks(cfg, p, None, ctx, live, eps)) == [(0, 0, 1, 2), (1, 2, 0, 4), (2, 1, 1, 5)]
+    assert (1, 1, 0, 6) not in RO.relu_kinks(cfg, p, None, ctx, None, eps) and \
+        (0, 1, 0, 6) in RO.relu_kinks(cfg, p, None, ctx, None, eps)
+    assert RO.relu_kinks(dict(cfg, post_merge_activation="tanh"), p, None, ctx, live, eps) == []
+    cleared, moved = RO.clear_kinks(cfg, p, None, ctx, live, eps)
+    # h_0 unit 2 has rows at 3e-6 and -2e-5: +3 eps leaves -2e-5 + 3e-5 = 1e-5 < 2 eps, -3 eps clears both
+    assert [(j, u) for j, u, _ in moved] == [(0, 2), (1, 4), (2, 5)]
+    assert_allclose([s for _, _, s in moved], [-3 * eps, 3 * eps, 3 * eps], rtol=1e-12)
+    for k, v in p.items():
+        changed = np.flatnonzero(np.asarray(cleared[k]).ravel() != v.ravel())
+        want = {RO.PM + "/bias.b": [2], RO.linear_name(0) + ".b": [4], RO.linear_name(1) + ".b": [5]}.get(k, [])
+        assert list(changed) == want, k
+    assert RO.relu_kinks(cfg, cleared, None, ctx, live, eps) == []
+    assert RO.clear_kinks(cfg, cleared, None, ctx, live, eps)[1] == []
