@@ -84,8 +84,9 @@ def _kper_ok(k):
     return k % 128 == 0 and k // 32 in (4, 8, 12, 16, 24)
 
 
-def _derive(E, C, M, Tp, cs, ncg, loc, K=10, n=8):
-    """derive() with the padded handler copy: (nc1, nc2, nc3, dynamic shared memory in bytes); None: no tile fits."""
+def _derive(E, C, M, Tp, cs, ncg, loc, K=10, n=8, wh_rows=16):
+    """derive() with a handler copy of wh_rows rows (16: padded, K: compact): (nc1, nc2, nc3, dynamic shared memory in
+    bytes, red_alias); None: no tile fits."""
     r8 = lambda x: (x + 7) // 8 * 8
     nc2 = r8(-(-C // ncg))
     nc1, nc3 = 3 * nc2, r8(-(-M // ncg))
@@ -94,10 +95,10 @@ def _derive(E, C, M, Tp, cs, ncg, loc, K=10, n=8):
     tc = -(-Tp // cs)
     red_f = DS_WARPS * DS_ROWS * max(nc1, nc2, nc3)
     red_alias = max(8 * E, ATT_NW * (tc + 16)) >= red_f
-    f = _smem_bytes(Tp, cs, loc, M=M, E=E, K=K, n=n) // 4
+    f = _smem_bytes(Tp, cs, loc, M=M, E=E, K=K, n=n, wh_rows=wh_rows) // 4
     f = (f + 3) // 4 * 4 + (E + C) * (nc1 + 4) + C * (nc2 + 4) + C * (nc3 + 4)
     f = (f + 3) // 4 * 4 + 3 * DS_ROWS * nc2 + 4 + (0 if red_alias else red_f)
-    return nc1, nc2, nc3, 4 * f + 64
+    return nc1, nc2, nc3, 4 * f + 64, red_alias
 
 
 def _one_wave_cs(R, Tp):

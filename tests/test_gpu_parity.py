@@ -252,33 +252,6 @@ def test_config3_wsj_beam10_identical_tokens():
     assert np.allclose(got_costs, want_costs, rtol=1e-3, atol=5e-3)
 
 
-def test_config5_timit_long_utterance_properties():
-    """configs[4] per GPU: 16 utterances x 2000 frames, 3x BiGRU(256) without subsampling
-    (T' = 2000), 63 output symbols, window_around_median prior."""
-    torch = _torch()
-    cfg = O.make_config(num_features=40, dims_bidir=[256, 256, 256], subsample=[1, 1, 1], dim_dec=256,
-                        dim_matcher=512, conv_n=100, conv_num_filters=10, num_phonemes=63,
-                        post_merge_dims=[256], maxout_pieces=2,
-                        prior=dict(type="window_around_median", before=100, after=100))
-    params = O.init_params(cfg, seed=2, scale=10.0)
-    x, m, labels, lm = O.synthetic_batch(cfg, B=16, T=2000, seed=5, dtype=np.float32, label_div=32)
-    rec = make_recognizer(cfg, params)
-    att, attm = rec.encode(x, m)
-    assert tuple(att.shape) == (2000, 16, 512)
-    r = rec.cost_matrix(labels, lm, att, attm, return_all=True)
-    plan = rec.decoder_plan()
-    assert plan["ran"] and plan["kernel"] == "dec_scan<COMPACT>", plan      # the padded handler copy does not fit
-    w = r["weights"]
-    assert bool(torch.isfinite(r["costs"]).all())
-    assert torch.allclose(w.sum(dim=2), torch.ones_like(w.sum(dim=2)), atol=1e-4)
-    assert int((w > 0).sum(dim=2).max()) <= 201                      # the median window: at most before+after+1 positions
-    # one short utterance of the same architecture against the oracle
-    xs, ms, ls, lms = O.synthetic_batch(cfg, B=2, T=96, seed=6)
-    want = O.recognizer_cost(cfg, params, xs, ms, ls, lms)
-    got = rec.cost(xs, ms, ls, lms)
-    assert rel_err(got, want) < TOL
-
-
 def test_persistent_decoder_equals_stepwise_kernels(monkeypatch):
     _torch()
     cfg = O.make_config(prior=dict(type="window_around_mean", before=9, after=9), **PYRAMID)

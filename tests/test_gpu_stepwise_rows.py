@@ -50,12 +50,13 @@ SMEM_MAX = 227 * 1024        # dynamic shared memory one CTA may opt in to
 ATT_NW = 16                  # warps of an attention CTA (ATT_NT = 512 threads)
 
 
-def _smem_bytes(Tp, cs, loc=True, M=512, E=512, K=10, n=100):
-    """att_smem_floats (wh_rows = 16) in bytes for a chunk of ceil(T'/cs) positions."""
+def _smem_bytes(Tp, cs, loc=True, M=512, E=512, K=10, n=100, wh_rows=16):
+    """att_smem_floats in bytes for a chunk of ceil(T'/cs) positions, with a handler copy of wh_rows rows (16: padded,
+    K: compact)."""
     tc = -(-Tp // cs)
     f = 2 * M                                                        # sq, sv
     if loc:
-        f += 16 * M + (2 * n + 1) * (12 if K <= 12 else 16)            # sWh, sfiltT
+        f += wh_rows * M + (2 * n + 1) * (12 if K <= 12 else 16)       # sWh, sfiltT
         f += tc + 2 * n + 8 + (tc + 16) * 16                         # salpha, sF
     f += 2 * (tc + 16) + 96                                          # se, su, block scratch
     f += max(8 * E, ATT_NW * (tc + 16))                              # sred (att_red_floats)
