@@ -940,6 +940,10 @@ class SpeechRecognizer(object):
         y = self._dev(outputs, torch.int64)
         s, w = self._dev(st["lm_states"], torch.int32), self._dev(st["lm_weights"], torch.float64)
         R = s.shape[0]
+        # the C ABI takes R rows of every array and no lengths: a short one would be read past its end
+        if s.dim() != 2 or s.shape[1] != _lib.LM_MAX_STATES or tuple(w.shape) != tuple(s.shape) or tuple(y.shape) != (R,):
+            raise ValueError("lm_next_states: states %s and weights %s must be [R, %d] and outputs %s [R]"
+                             % (tuple(s.shape), tuple(w.shape), _lib.LM_MAX_STATES, tuple(y.shape)))
         nxt = OrderedDict(lm_states=torch.empty_like(s), lm_weights=torch.empty_like(w),
                           lm_add=torch.empty((R, self.net["num_phonemes"]), dtype=torch.float32, device=self.device))
         _lib.check(lib.lvsr_lm_next_states(h, R, _ptr(s), _ptr(w), _ptr(y), _ptr(nxt["lm_states"]),
