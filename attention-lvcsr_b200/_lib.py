@@ -191,6 +191,7 @@ SIGNATURES = {
     "lvsr_lm_next_states": (C.c_int, [_P, _I, _P, _P, _P, _P, _P, _P, _P]),
     "lvsr_recognizer_cost_host": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _P, _P]),
     "lvsr_train_cost_and_grads": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _I, C.c_float, _P, _P, _P]),
+    "lvsr_train_cost_and_grads_greedy": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, C.c_float, _P, _P, _P, _P, _P]),
     "lvsr_train_apply_updates": (C.c_int, [_P, _P, C.c_float, C.POINTER(LvsrTrainConfig), _P]),
     "lvsr_train_gradient_norm": (C.c_int, [_P, C.POINTER(C.c_float)]),
     "lvsr_train_reset": (C.c_int, [_P]),

@@ -31,6 +31,7 @@ NOISE_BRICK = "adaptive_noise"
 ADAPTIVE_NOISE_DEFAULTS = dict(init_sigma=1e-6, model_cost_coefficient=1.0, seed=None)   # graph.py:71-80
 # regularization.dropout / noise / penalty_coof (lvsr/main.py:400-417); seed None or 0 is Blocks' default_seed, 1
 REGULARIZATION_DEFAULTS = dict(dropout=False, noise=0.0, penalty_coof=0.0, seed=None)
+GREEDY_EXTRA_STEPS = 10       # LVSR_GREEDY_EXTRA_STEPS: greedy exploration generates L + 10 steps (lvsr/main.py:251)
 ADAPTIVE_NOISE_ERROR = "using  adaptive noise with alignment weight panalty or weight decay is probably stupid"
 
 
@@ -256,16 +257,42 @@ def _regularization(reg):
 
 
 def check_trainable_net(net):
-    """Refuse a config['net'] the training step cannot run: a task-loss criterion (mse_gain / mse_reward) and a
-    stacked decoder (dec_stack > 1) decode and score, but have no backward pass."""
-    name = (net.get("criterion") or {}).get("name", "log_likelihood")
-    if name != "log_likelihood":
-        # the MSE backward and the exploration of RewardRegressionEmitter training are not built
-        raise NotImplementedError("attention-lvcsr_b200: training with criterion %r (task loss estimation scores and "
-                                  "decodes only)" % name)
+    """Refuse a config['net'] the training step cannot run: a stacked decoder (dec_stack > 1) decodes and scores, but
+    has no backward pass."""
     if net.get("dec_stack", 1) != 1:
         raise NotImplementedError("attention-lvcsr_b200: training with dec_stack=%d (a stacked decoder is inference "
                                   "only: cost, analyze, beam search and sampling)" % net["dec_stack"])
+
+
+# config['training']['exploration'] values the training step runs (lvsr/main.py:245-283); 'mixed' also draws, per
+# utterance, whether to train on the labels or on the greedy prediction
+EXPLORATIONS = ("imitative", "greedy")
+
+
+def check_exploration(net, exploration, regularization=None):
+    """The exploration a training step of `net` (config['net'] with its criterion) runs for config['training']'s
+    `exploration` (None: the reference's default, imitative), refused before any device work when the step cannot run
+    it.  Only a task-loss criterion (mse_gain / mse_reward) reads the key: a log-likelihood model trains on its labels
+    whatever it says.  `regularization`: the dropout / noise / penalty_coof the step applies (None: none, as under
+    adaptive noise, which drops them)."""
+    if (net.get("criterion") or {}).get("name", "log_likelihood") == "log_likelihood":
+        return "imitative"
+    exploration = exploration or "imitative"
+    if exploration == "mixed":
+        raise NotImplementedError("attention-lvcsr_b200: exploration 'mixed' (lvsr/main.py:262-276) is not built: "
+                                  "use 'imitative' or 'greedy'")
+    if exploration not in EXPLORATIONS:
+        raise ValueError("unknown exploration %r (lvsr/main.py:279-280 accepts imitative, greedy and mixed)"
+                         % (exploration,))
+    reg = _regularization(regularization or {})
+    if exploration == "greedy" and reg:
+        if reg["penalty_coof"] > 0:
+            raise ValueError("greedy exploration with penalty_coof > 0: the alignment penalty pairs the L + 10 "
+                             "generated steps with the L-row labels mask (lvsr/main.py:411-417)")
+        if reg["dropout"]:
+            raise NotImplementedError("greedy exploration with dropout: the reference's dropout graph holds two "
+                                      "applications of the bottom, in no defined order (lvsr/main.py:400-408)")
+    return exploration
 
 
 class GradientDescent(object):
@@ -300,17 +327,26 @@ class GradientDescent(object):
     Under adaptive noise the reference trains on the clean graph, so all three are dropped with a logged error.
     Data-parallel dropout needs equal shards: rank r's first utterance is utterance r * B of the global batch.
     ``last_cost`` stays the task cost of the regularised forward; ``last_penalty`` is weights_penalty / B of the
-    last update (a device scalar; None when the penalty is off), all-reduced with the gradient."""
+    last update (a device scalar; None when the penalty is off), all-reduced with the gradient.
+
+    exploration: config['training']['exploration'] (check_exploration), read under a task-loss criterion only.
+    'imitative' trains on the labels; 'greedy' generates L + 10 steps of the model's own arg-max output on the device
+    with the parameters the step runs on, and trains on that prediction scored against the labels (lvsr/main.py:
+    245-283).  ``last_prediction`` is then (prediction [L + 10, B] int64, its mask [L + 10, B] float32), device tensors
+    of the last step; None otherwise.  Each data-parallel rank explores its own shard."""
 
     def __init__(self, recognizer=None, step_rule=None, decay=0.0, cost=None, parameters=None, gradients=None,
-                 on_unused_sources="warn", adaptive_noise=None, regularization=None, **kwargs):
+                 on_unused_sources="warn", adaptive_noise=None, regularization=None, exploration="imitative",
+                 **kwargs):
         if recognizer is None:
             raise ValueError("GradientDescent needs the recognizer (no symbolic cost exists in the CUDA path)")
         if getattr(recognizer, "lm", None):
             # with an LM the reference's emitter is LMEmitter, whose costs are the fused readout's: inference only
             raise NotImplementedError("attention-lvcsr_b200: training with a language model (shallow fusion is "
                                       "inference only)")
-        check_trainable_net(dict(getattr(recognizer, "net", {}), criterion=getattr(recognizer, "criterion", None)))
+        net = dict(getattr(recognizer, "net", {}), criterion=getattr(recognizer, "criterion", None))
+        check_trainable_net(net)
+        self.exploration = check_exploration(net, exploration, None if adaptive_noise else regularization)
         self.recognizer = recognizer
         self.step_rule = step_rule if step_rule is not None else CompositeRule([Scale(), RemoveNotFinite(0.0)])
         self.adaptive_noise = None
@@ -344,6 +380,7 @@ class GradientDescent(object):
         self.last_cost = None
         self.last_penalty = None
         self.last_batch_size = None
+        self.last_prediction = None
 
     SOURCES = ("recordings", "recordings_mask", "labels", "labels_mask")
 
@@ -497,9 +534,18 @@ class GradientDescent(object):
         gs = (1.0 / B) if gscale is None else gscale
         if self.regularization and self.regularization["dropout"]:
             _lib.check(lib.lvsr_train_set_utterance_offset(h, int(utterance_offset)))
-        _lib.check(lib.lvsr_train_cost_and_grads(
-            h, x.data_ptr(), None if m is None else m.data_ptr(), y.data_ptr(), None if ym is None else ym.data_ptr(),
-            T, B, L, float(gs), self._cost.data_ptr(), self._buf.data_ptr(), rec._stream()))
+        if self.exploration == "greedy":
+            n = L + GREEDY_EXTRA_STEPS
+            pred = torch.empty((n, B), dtype=torch.int64, device=rec.device)
+            pmask = torch.empty((n, B), dtype=torch.float32, device=rec.device)
+            _lib.check(lib.lvsr_train_cost_and_grads_greedy(
+                h, x.data_ptr(), None if m is None else m.data_ptr(), y.data_ptr(), T, B, L, float(gs),
+                self._cost.data_ptr(), self._buf.data_ptr(), pred.data_ptr(), pmask.data_ptr(), rec._stream()))
+            self.last_prediction = (pred, pmask)
+        else:
+            _lib.check(lib.lvsr_train_cost_and_grads(
+                h, x.data_ptr(), None if m is None else m.data_ptr(), y.data_ptr(), None if ym is None else ym.data_ptr(),
+                T, B, L, float(gs), self._cost.data_ptr(), self._buf.data_ptr(), rec._stream()))
         if self._penalty_on():
             # the penalty sum rides in the step buffer's padding: the data-parallel step stays one all-reduce
             _lib.check(lib.lvsr_train_penalty_sum(h, self._buf.data_ptr() + 4 * (self._n + 2), rec._stream()))

@@ -1052,15 +1052,7 @@ static size_t tle_ws_bytes(const lvsr_model* m, int Lg, int L, int B) {
   return (size_t)3 * L * B * m->cfg.num_phonemes * sizeof(float) + tle_dist_ints(Lg, L, B) * sizeof(int) + 4096;
 }
 
-// RewardOp's matrices of prediction [L, B] against groundtruth [Lg, B] into rewards / gains [L, B, V] (from ws);
-// synchronises st and reports the first utterance whose groundtruth holds no eos.
-static int tle_run_matrices(lvsr_model* m, Arena& ws, const long long* groundtruth, int Lg, const long long* prediction,
-                            int L, int B, float* rewards, float* gains, cudaStream_t st) {
-  int* dist = ws.i32(tle_dist_ints(Lg, L, B));
-  LVSR_CHECK(dist, "out of device memory (task-loss distances)");
-  LVSR_CUDA_OK(cudaMemsetAsync(m->tle_status.get(), 0xff, sizeof(unsigned), st));
-  if (int rc = tle_matrices(groundtruth, Lg, prediction, L, B, m->cfg.num_phonemes, m->criterion.eos_label, dist, rewards,
-                            gains, m->tle_status.get(), st)) return rc;
+int lvsr::tle_check_status(lvsr_model* m, cudaStream_t st) {
   unsigned h = LVSR_TLE_OK;
   LVSR_CUDA_OK(cudaMemcpyAsync(&h, m->tle_status.get(), sizeof(h), cudaMemcpyDeviceToHost, st));
   LVSR_CUDA_OK(cudaStreamSynchronize(st));
@@ -1069,14 +1061,28 @@ static int tle_run_matrices(lvsr_model* m, Arena& ws, const long long* groundtru
   return 0;
 }
 
-// The task-loss cost rows [L, B] from the emitter costs neg [L*B, V] of the prediction `labels`
+// RewardOp's matrices of prediction [L, B] against groundtruth [Lg, B] into rewards / gains [L, B, V] (from ws); with
+// `wait`, synchronises st and reports the first utterance whose groundtruth holds no eos (else tle_check_status does)
+static int tle_run_matrices(lvsr_model* m, Arena& ws, const long long* groundtruth, int Lg, const long long* prediction,
+                            int L, int B, float* rewards, float* gains, bool wait, cudaStream_t st) {
+  int* dist = ws.i32(tle_dist_ints(Lg, L, B));
+  LVSR_CHECK(dist, "out of device memory (task-loss distances)");
+  LVSR_CUDA_OK(cudaMemsetAsync(m->tle_status.get(), 0xff, sizeof(unsigned), st));
+  if (int rc = tle_matrices(groundtruth, Lg, prediction, L, B, m->cfg.num_phonemes, m->criterion.eos_label, dist, rewards,
+                            gains, m->tle_status.get(), st)) return rc;
+  return wait ? tle_check_status(m, st) : 0;
+}
+
+// The task-loss cost rows [L, B] from the emitter costs neg [L*B, V] of the prediction `labels`; the matrices go to
+// keep's buffers when it is given
 static int tle_costs(lvsr_model* m, Arena& ws, const long long* groundtruth, int Lg, const long long* labels,
-                     const float* lmask, int L, int B, const float* neg, float* costs, cudaStream_t st) {
+                     const float* lmask, int L, int B, const float* neg, float* costs, const TleTape* keep,
+                     cudaStream_t st) {
   const size_t n = (size_t)L * B * m->cfg.num_phonemes;
-  float* rewards = ws.f32(n);
-  float* gains = ws.f32(n);
+  float* rewards = keep ? keep->rewards : ws.f32(n);
+  float* gains = keep ? keep->gains : ws.f32(n);
   LVSR_CHECK(rewards && gains, "out of device memory (task-loss matrices)");
-  if (int rc = tle_run_matrices(m, ws, groundtruth, Lg, labels, L, B, rewards, gains, st)) return rc;
+  if (int rc = tle_run_matrices(m, ws, groundtruth, Lg, labels, L, B, rewards, gains, !keep, st)) return rc;
   const int loss = m->criterion.name == LVSR_CRITERION_MSE_GAIN ? LVSR_TLE_GAIN : LVSR_TLE_REWARD;
   return tle_loss(loss, neg, rewards, gains, labels, lmask, L, B, m->cfg.num_phonemes, (float)m->criterion.min_reward,
                   costs, st);
@@ -1113,7 +1119,7 @@ int lvsr_tle_matrices(lvsr_model* m, const int64_t* groundtruth, int32_t Lg, con
   m->ws.reserve(tle_ws_bytes(m, Lg, L, B), st);
   ArenaScope scope(m, st);
   return tle_run_matrices(m, m->ws, reinterpret_cast<const long long*>(groundtruth), Lg,
-                          reinterpret_cast<const long long*>(prediction), L, B, rewards, gains, st);
+                          reinterpret_cast<const long long*>(prediction), L, B, rewards, gains, true, st);
 }
 
 int lvsr_encoded_length(const lvsr_model* m, int32_t T) {
@@ -1166,12 +1172,21 @@ int lvsr_cost_matrix_groundtruth(lvsr_model* m, const float* attended, const flo
                                  const int64_t* labels, const float* labels_mask, int32_t L, const int64_t* groundtruth,
                                  int32_t Lg, float* costs, float* weights_out, float* energies_out, float* states_out,
                                  float* wavg_out, void* stream) {
+  return cost_matrix(m, attended, attended_mask, Tp, B, labels, labels_mask, L, groundtruth, Lg, costs, weights_out,
+                     energies_out, states_out, wavg_out, nullptr, static_cast<cudaStream_t>(stream));
+}
+
+}  // extern "C"
+
+int lvsr::cost_matrix(lvsr_model* m, const float* attended, const float* attended_mask, int Tp, int B,
+                      const int64_t* labels, const float* labels_mask, int L, const int64_t* groundtruth, int Lg,
+                      float* costs, float* weights_out, float* energies_out, float* states_out, float* wavg_out,
+                      const TleTape* keep, cudaStream_t st) {
   DeviceGuard device_guard(m);
-  if (int rc = bind_stream(m, static_cast<cudaStream_t>(stream))) return rc;
+  if (int rc = bind_stream(m, st)) return rc;
   if (int rc = check_ready(m)) return rc;
   LVSR_CHECK(attended && attended_mask && labels && costs && Tp > 0 && B > 0 && L > 0, "cost_matrix: bad arguments");
   LVSR_CHECK(!groundtruth || Lg > 0, "cost_matrix: groundtruth without rows");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
   const bool tle = tle_criterion(m);
   if (!groundtruth) { groundtruth = labels; Lg = L; }
   m->ws.reserve(cost_ws_bytes(m, Tp, B, L) + (lm_attached(m) ? (size_t)L * B * m->cfg.num_phonemes * sizeof(float) : 0) +
@@ -1192,7 +1207,7 @@ int lvsr_cost_matrix_groundtruth(lvsr_model* m, const float* attended, const flo
   LVSR_CHECK(P && s_all && ctx_all && w0 && merged && wpp[0] && wpp[1] && (energies_out || e_scratch),
              "out of device memory (decoder workspace)");
 
-  if (int rc = lvsr_preprocess(m, attended, Tp, B, P, stream)) return rc;          // hoisted: B/bricks/attention.py:733-738
+  if (int rc = lvsr_preprocess(m, attended, Tp, B, P, st)) return rc;              // hoisted: B/bricks/attention.py:733-738
   if (int rc = broadcast_rows(s_all, initial_state_row(m), B, S, st)) return rc;
   if (int rc = onehot_rows(w0, B, Tp, st)) return rc;                               // lvsr/bricks/attention.py:215-222
   if (int rc = fill_f32(costs, (long long)L * B, 0.f, st)) return rc;
@@ -1266,12 +1281,12 @@ int lvsr_cost_matrix_groundtruth(lvsr_model* m, const float* attended, const flo
     r.poison = scanned ? m->status.get() : nullptr;
     if (tle) {
       // RewardRegressionEmitter.cost over the whole readouts (lvsr/bricks/__init__.py:135-184)
-      float* neg = ws.f32((size_t)R * c.num_phonemes);
+      float* neg = keep ? keep->neg : ws.f32((size_t)R * c.num_phonemes);
       LVSR_CHECK(neg, "out of device memory (task-loss readouts)");
       r.costs_all = neg;
       if (int rc = readout_costs(r, st)) return rc;
       if (int rc = tle_costs(m, ws, reinterpret_cast<const long long*>(groundtruth), Lg, lab, labels_mask, L, B, neg,
-                             costs, st)) return rc;
+                             costs, keep, st)) return rc;
     } else {
       r.labels = lab; r.lmask = labels_mask; r.costs_picked = costs;
       if (lm_add) lm_fuse(m, r, lm_add);
@@ -1282,6 +1297,47 @@ int lvsr_cost_matrix_groundtruth(lvsr_model* m, const float* attended, const flo
     LVSR_CUDA_OK(cudaMemcpyAsync(states_out, s_all, (size_t)L * B * S * sizeof(float), cudaMemcpyDeviceToDevice, st));
   return 0;
 }
+
+int lvsr::tle_generate_greedy(lvsr_model* m, const float* attended, const float* attended_mask, int Tp, int B, int n,
+                              long long* prediction, float* prediction_mask, cudaStream_t st) {
+  ProfScope prof("tle_generate", st);
+  const lvsr_config& c = m->cfg;
+  const int E = m->E, S = state_dim(m), V = c.num_phonemes;
+  m->ws.reserve(cost_ws_bytes(m, Tp, B, 1), st);
+  ArenaScope scope(m, st);
+  Arena& ws = m->ws;
+  float* P = ws.f32((size_t)Tp * B * c.dim_matcher);
+  float* s[2] = {ws.f32((size_t)B * S), ws.f32((size_t)B * S)};
+  float* w[2] = {ws.f32((size_t)B * Tp), ws.f32((size_t)B * Tp)};
+  float* e = ws.f32((size_t)B * Tp);
+  float* ctx = ws.f32((size_t)B * E);
+  float* merged = ws.f32((size_t)B * c.post_merge_dim);
+  float* neg = ws.f32((size_t)B * V);
+  float* alive = ws.f32((size_t)B);
+  LVSR_CHECK(P && s[0] && s[1] && w[0] && w[1] && e && ctx && merged && neg && alive,
+             "out of device memory (greedy generation)");
+  if (int rc = lvsr_preprocess(m, attended, Tp, B, P, st)) return rc;
+  if (int rc = broadcast_rows(s[0], initial_state_row(m), B, S, st)) return rc;
+  if (int rc = onehot_rows(w[0], B, Tp, st)) return rc;
+  if (int rc = fill_f32(alive, B, 1.f, st)) return rc;
+  for (int i = 0; i < n; ++i) {
+    ArenaMark mark{ws};
+    const float* s_i = s[i & 1];
+    if (int rc = glimpses(m, attended, P, attended_mask, Tp, B, nullptr, B, s_i, w[i & 1], nullptr, i, w[(i + 1) & 1], e,
+                          ctx, st)) return rc;
+    const float* tail = nullptr;
+    if (int rc = readout_merged(m, B, s_i, ctx, merged, &tail, st)) return rc;
+    ReadoutArgs r = readout_args(m, B, tail);
+    r.costs_all = neg;
+    if (int rc = readout_costs(r, st)) return rc;
+    long long* y_i = prediction + (size_t)i * B;
+    if (int rc = tle_greedy_pick(neg, B, V, m->criterion.eos_label, alive, y_i, prediction_mask + (size_t)i * B, st)) return rc;
+    if (int rc = transition(m, B, s_i, ctx, y_i, nullptr, s[(i + 1) & 1], st)) return rc;
+  }
+  return 0;
+}
+
+extern "C" {
 
 int lvsr_initial_states(lvsr_model* m, int32_t Tp, int32_t R, float* states, int64_t* outputs, float* wavg,
                         float* weights, float* energies, int64_t* step, void* stream) {

@@ -229,6 +229,14 @@ int tle_matrices(const long long* groundtruth, int Lg, const long long* predicti
 int tle_loss(int criterion, const float* neg_readouts, const float* rewards, const float* gains,
              const long long* prediction, const float* lmask, int L, int B, int V, float min_reward, float* costs,
              cudaStream_t stream);
+// dlogits [L*B, V] = gscale * d sum(tle_loss costs) / d readouts, from the same inputs; row_sum: L*B doubles of scratch
+int tle_loss_grad(int criterion, const float* neg_readouts, const float* rewards, const float* gains,
+                  const long long* prediction, const float* lmask, int L, int B, int V, float min_reward, float gscale,
+                  double* row_sum, float* dlogits, cudaStream_t stream);
+// One greedy step from the emitter costs neg_readouts [B, V]: out [B] = the arg-max of the readouts, out_mask [B] =
+// alive [B] (1 until eos has been emitted), then alive is cleared where out is eos
+int tle_greedy_pick(const float* neg_readouts, int B, int V, int eos, float* alive, long long* out, float* out_mask,
+                    cudaStream_t stream);
 
 // ---- lm.cu: FST language model states (float64 weights, at most LVSR_LM_MAX_STATES per hypothesis) --------------
 enum { LVSR_LM_TOO_MANY_STATES = 1, LVSR_LM_CLOSURE_CAP = 2, LVSR_LM_CYCLE = 3 };   // status word codes

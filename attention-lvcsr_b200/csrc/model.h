@@ -402,6 +402,20 @@ void lm_fuse(const lvsr_model* m, ReadoutArgs& r, const float* lm_add);
 int lm_report(unsigned status);
 size_t encoder_ws_bytes(const lvsr_model* m, int T, int B);
 size_t cost_ws_bytes(const lvsr_model* m, int Tp, int B, int L);
+// lvsr_cost_matrix_groundtruth, which under a task-loss criterion keeps what the loss was formed from in `tle` (null:
+// workspace scratch): the emitter costs (-readouts), rewards and gains, each [L*B, num_phonemes].  With `tle` given the
+// call does not wait for the groundtruth's eos check: the caller runs tle_check_status once its own work is enqueued.
+struct TleTape { float *neg, *rewards, *gains; };
+// Synchronises st, then reports the first utterance of the last reward launch whose groundtruth holds no eos
+int tle_check_status(lvsr_model* m, cudaStream_t st);
+int cost_matrix(lvsr_model* m, const float* attended, const float* attended_mask, int Tp, int B, const int64_t* labels,
+                const float* labels_mask, int L, const int64_t* groundtruth, int Lg, float* costs, float* weights_out,
+                float* energies_out, float* states_out, float* wavg_out, const TleTape* tle, cudaStream_t st);
+// generate() under RewardRegressionEmitter for n steps on the device (glimpses, readout, arg-max, transition per step,
+// no host round trip): prediction [n, B] and its mask [n, B] (1 up to and including the first eos), as
+// lvsr/main.py:245-283 builds them for greedy exploration.  Buffers from m->ws.
+int tle_generate_greedy(lvsr_model* m, const float* attended, const float* attended_mask, int Tp, int B, int n,
+                        long long* prediction, float* prediction_mask, cudaStream_t st);
 
 // The two device steps of lvsr_beam_search_many (search.cu), which holds the device guard and has finalized the
 // model.  The hypotheses (rows) of utterance s are the contiguous rows [seg_start[s], seg_start[s+1]) -- one segment

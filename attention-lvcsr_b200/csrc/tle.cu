@@ -139,6 +139,77 @@ __global__ void __launch_bounds__(256) tle_loss_kernel(int criterion, const floa
   }
 }
 
+// gscale times the gradient of tle_loss_kernel's costs with respect to the readouts r = -neg_readouts, one warp per
+// utterance.  mse_gain: 2 m_t (r - max(G, min_reward)).  mse_reward: with d_t = r_t + cum_t - R_t, 2 m_t d_t, and the
+// picked readout r[t, y_t] (t >= 1) sits in cum_{t'} of every step t' >= t, so it also receives sum_{t' >= t} 2 m_t'
+// sum_v d_t': a second, reverse-time walk over the per-step sums the first one leaves in row_sum [L, B].
+__global__ void __launch_bounds__(256) tle_grad_kernel(int criterion, const float* neg_readouts, const float* rewards,
+                                                       const float* gains, const long long* y, const float* lmask,
+                                                       int L, int B, int V, float min_reward, float gscale,
+                                                       double* row_sum, float* dlogits) {
+  const int lane = threadIdx.x & 31, b = blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (b >= B) return;
+  float cum = 0.f;                     // as tle_loss_kernel forms it
+  for (int t = 0; t < L; ++t) {
+    const long long r = (long long)t * B + b;
+    const float* x = neg_readouts + r * V;
+    if (criterion == LVSR_TLE_REWARD && t > 0) {
+      const long long s = y[r];
+      cum += (s >= 0 && s < V) ? -x[s] : 0.f;
+    }
+    const double w = 2.0 * (lmask ? lmask[r] : 1.f);
+    double sum = 0.0;
+    for (int v = lane; v < V; v += 32) {
+      double d;
+      if (criterion == LVSR_TLE_GAIN) d = (double)(-x[v]) - fmax((double)gains[r * V + v], (double)min_reward);
+      else d = (double)(-x[v] + cum) - (double)rewards[r * V + v];
+      dlogits[r * V + v] = (float)(w * d * gscale);
+      sum += d;
+    }
+    if (criterion == LVSR_TLE_REWARD) {
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+      if (lane == 0) row_sum[r] = w * sum;
+    }
+  }
+  if (criterion != LVSR_TLE_REWARD) return;
+  __syncwarp();                        // the picked entries lane 0 adds to were written by any lane
+  if (lane != 0) return;
+  double acc = 0.0;
+  for (int t = L - 1; t >= 1; --t) {
+    const long long r = (long long)t * B + b, s = y[r];
+    acc += row_sum[r];
+    if (s >= 0 && s < V) dlogits[r * V + s] = (float)((double)dlogits[r * V + s] + acc * gscale);
+  }
+}
+
+// One greedy step of RewardRegressionEmitter.emit (the arg-max of the readouts, the first on ties), one warp per row:
+// out[b] = the pick, out_mask[b] = alive[b] (1 until the row has emitted eos), then alive[b] drops to 0 on an eos.
+__global__ void __launch_bounds__(256) tle_greedy_pick_kernel(const float* neg_readouts, int B, int V, int eos,
+                                                              float* alive, long long* out, float* out_mask) {
+  const int lane = threadIdx.x & 31, b = blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (b >= B) return;
+  float bv = INFINITY;
+  int bi = 0x7fffffff;
+  for (int v = lane; v < V; v += 32) {
+    const float x = neg_readouts[(long long)b * V + v];
+    if (x < bv) { bv = x; bi = v; }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+    if (ov < bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+  }
+  if (lane == 0) {
+    if (bi == 0x7fffffff) bi = 0;      // a row of NaN
+    const float a = alive[b];
+    out[b] = bi;
+    out_mask[b] = a;
+    alive[b] = bi == eos ? 0.f : a;
+  }
+}
+
 size_t tle_smem_bytes(int Lg, int L) { return (size_t)(Lg + 2 * L + 3 * (Lg + 1) + TLE_WARPS * TLE_VMAX) * sizeof(int); }
 
 }  // namespace
@@ -172,6 +243,26 @@ int tle_loss(int criterion, const float* neg_readouts, const float* rewards, con
   LVSR_CHECK(criterion == LVSR_TLE_GAIN || criterion == LVSR_TLE_REWARD, "tle: unknown loss %d", criterion);
   tle_loss_kernel<<<ceil_div(B, 8), 256, 0, stream>>>(criterion, neg_readouts, rewards, gains, prediction, lmask, L, B,
                                                       V, min_reward, costs);
+  LVSR_LAUNCH_CHECK();
+  return 0;
+}
+
+int tle_loss_grad(int criterion, const float* neg_readouts, const float* rewards, const float* gains,
+                  const long long* prediction, const float* lmask, int L, int B, int V, float min_reward, float gscale,
+                  double* row_sum, float* dlogits, cudaStream_t stream) {
+  ProfScope prof("tle_grad", stream);
+  if (B <= 0 || L <= 0) return 0;
+  LVSR_CHECK(criterion == LVSR_TLE_GAIN || criterion == LVSR_TLE_REWARD, "tle: unknown loss %d", criterion);
+  tle_grad_kernel<<<ceil_div(B, 8), 256, 0, stream>>>(criterion, neg_readouts, rewards, gains, prediction, lmask, L, B,
+                                                      V, min_reward, gscale, row_sum, dlogits);
+  LVSR_LAUNCH_CHECK();
+  return 0;
+}
+
+int tle_greedy_pick(const float* neg_readouts, int B, int V, int eos, float* alive, long long* out, float* out_mask,
+                    cudaStream_t stream) {
+  if (B <= 0) return 0;
+  tle_greedy_pick_kernel<<<ceil_div(B, 8), 256, 0, stream>>>(neg_readouts, B, V, eos, alive, out, out_mask);
   LVSR_LAUNCH_CHECK();
   return 0;
 }

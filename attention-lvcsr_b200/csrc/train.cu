@@ -136,8 +136,12 @@ int gemm_tn_tc(Arena& ws, const TcOperand& A, int a0, int Mo, const TcOperand& B
   return 0;
 }
 
-// The decoder's tape: attended sequence and mask, per step costs, alignments, energies (softmax: null), s_{i-1}, glimpses
-struct DecTape { float *Hatt, *attm, *costs, *W_all, *E_all, *S_prev, *CTX; };
+// The decoder's tape: attended sequence and mask, per step costs, alignments, energies (softmax: null), s_{i-1}, glimpses,
+// and under a task-loss criterion what its loss was formed from (log-likelihood: null)
+struct DecTape { float *Hatt, *attm, *costs, *W_all, *E_all, *S_prev, *CTX; TleTape tle; };
+// Greedy exploration (lvsr/main.py:245-283): the step generates its own `labels` (prediction) and `lmask` (the
+// prediction's mask) into these buffers after the encoder, and the task-loss rewards compare them with `groundtruth`
+struct Greedy { const int64_t* groundtruth; int Lg; long long* prediction; float* prediction_mask; };
 // Decoder backward's results: [dGz|dGr|dA], re-computed HR, dCTX, dq partials [L][2][B][M], dP, attention-constant partials
 struct DecGrads { float *dG, *HR, *dCTX, *dQp, *dP, *acc_v, *acc_Wh, *acc_filt, *acc_b; };
 
@@ -152,6 +156,7 @@ struct TrainStep {
   int B, L, Tp;
   const DropoutKey* drop;          // dropout on the encoder's input (null: off)
   float penalty_coof;              // alignment penalty coefficient (0: off)
+  const Greedy* greedy = nullptr;  // greedy exploration (null: the labels are the decoder's outputs)
   const lvsr_config& c = m->cfg;
   Arena& ws = m->tws;
   const long long* lab = reinterpret_cast<const long long*>(labels);
@@ -161,6 +166,7 @@ struct TrainStep {
   const int Hd = readout_dim(m, Kro - 1) / c.maxout_pieces;
   const int R = L * B, nct = AB_CS * B, tc_cap = ceil_div(Tp, AB_CS);
   const bool content = content_attention(m);
+  const bool tle = tle_criterion(m);
   // the logistic and relu energy gradients read the step's energies, which the softmax one does not need
   const bool keep_energies = c.energy_normalizer != LVSR_NORM_SOFTMAX;
   const size_t ro_smem = readout_bwd_smem_bytes(Hd);
@@ -199,6 +205,7 @@ struct TrainStep {
       bytes += ((size_t)3 * R * readout_dim(m, j) + (size_t)81 * readout_dim(m, j - 1) * readout_dim(m, j) + 1024) * sizeof(float);
     if (drop) bytes += (size_t)T * B * encoder_input_dim(m) * sizeof(float);      // the dropped encoder input
     if (penalty_coof > 0.f) bytes += (size_t)R * (Tp + 1) * sizeof(float);      // penalty gradient and row sums
+    if (tle) bytes += (size_t)3 * R * V * sizeof(float) + (size_t)R * sizeof(double);   // the loss's inputs, its row sums
     ws.reserve(bytes, st);
     ArenaScope scope(ws, st);
     for (int l = 0; l < c.num_layers; ++l)
@@ -237,7 +244,9 @@ struct TrainStep {
     if (int rc = decoder_backward(d, WstateT, WcombT, WsT, dS_ro, dCtx_ro, dg)) return rc;
     if (int rc = decoder_weight_grads(d, dg)) return rc;
     if (int rc = attended_grad(d, dg, WpT, dH)) return rc;
-    return encoder_backward(tape.data(), mask, dH, x, bottom_out);
+    if (int rc = encoder_backward(tape.data(), mask, dH, x, bottom_out)) return rc;
+    // the groundtruth's eos check of the task-loss rewards waits for the whole step, not for its forward alone
+    return tle ? tle_check_status(m, st) : 0;
   }
   // Taped forward: the encoder keeping its tape, then the teacher-forced decoder; *cost_out = sum(costs) * gscale
   int taped_forward(const float* x, const float* mask, int T, LayerTape* tape, const float** bottom_out, float* cost_out,
@@ -246,13 +255,22 @@ struct TrainStep {
     d.attm = ws.f32((size_t)Tp * B);
     LVSR_CHECK(d.Hatt && d.attm, "out of device memory (encoder output)");
     if (int rc = run_encoder(m, ws, x, mask, T, B, d.Hatt, d.attm, tape, st, bottom_out, drop)) return rc;
+    if (greedy)
+      if (int rc = tle_generate_greedy(m, d.Hatt, d.attm, Tp, B, L, greedy->prediction, greedy->prediction_mask, st)) return rc;
+    d.tle = {};
+    if (tle) {
+      d.tle = {ws.f32((size_t)R * V), ws.f32((size_t)R * V), ws.f32((size_t)R * V)};
+      LVSR_CHECK(d.tle.neg && d.tle.rewards && d.tle.gains, "out of device memory (task-loss tape)");
+    }
     d.costs = ws.f32((size_t)R);
     d.W_all = ws.f32((size_t)R * Tp);        // alignments alpha_i
     d.S_prev = ws.f32((size_t)R * C);        // s_{i-1}
     d.CTX = ws.f32((size_t)R * E);           // weighted averages
     d.E_all = keep_energies ? ws.f32((size_t)R * Tp) : nullptr;     // energies e_i, bias included
     LVSR_CHECK(d.costs && d.W_all && d.S_prev && d.CTX && (d.E_all || !keep_energies), "out of device memory (decoder tape)");
-    if (int rc = lvsr_cost_matrix(m, d.Hatt, d.attm, Tp, B, labels, lmask, L, d.costs, d.W_all, d.E_all, d.S_prev, d.CTX, st)) return rc;
+    if (int rc = cost_matrix(m, d.Hatt, d.attm, Tp, B, labels, lmask, L, greedy ? greedy->groundtruth : nullptr,
+                             greedy ? greedy->Lg : 0, d.costs, d.W_all, d.E_all, d.S_prev, d.CTX, tle ? &d.tle : nullptr, st))
+      return rc;
     sum_all_kernel<<<1, 1024, 0, st>>>(d.costs, R, cost_out, gscale);
     LVSR_LAUNCH_CHECK();
     return 0;
@@ -289,7 +307,17 @@ struct TrainStep {
     rb.Wo = m->P(top + ".W"); rb.bo = m->P(top + ".b");
     rb.R = R; rb.Cpm = Clast; rb.pieces = c.maxout_pieces; rb.V = V; rb.act = c.post_merge_activation;
     rb.labels = lab; rb.lmask = lmask; rb.gscale = gscale; rb.hid = hid; rb.dlogits = dlogits; rb.dmerged = dmerged;
-    readout_bwd_kernel<<<ceil_div(R, 8), 256, ro_smem, st>>>(rb);
+    if (tle) {
+      // RewardRegressionEmitter.cost's gradient (lvsr/bricks/__init__.py:135-184) in place of the softmax one
+      double* row_sum = reinterpret_cast<double*>(ws.f32((size_t)2 * R));
+      LVSR_CHECK(row_sum, "out of device memory (task-loss gradient)");
+      const int loss = m->criterion.name == LVSR_CRITERION_MSE_GAIN ? LVSR_TLE_GAIN : LVSR_TLE_REWARD;
+      if (int rc = tle_loss_grad(loss, d.tle.neg, d.tle.rewards, d.tle.gains, lab, lmask, L, B, V,
+                                 (float)m->criterion.min_reward, gscale, row_sum, dlogits, st)) return rc;
+      readout_bwd_kernel<true><<<ceil_div(R, 8), 256, ro_smem, st>>>(rb);
+    } else {
+      readout_bwd_kernel<false><<<ceil_div(R, 8), 256, ro_smem, st>>>(rb);
+    }
     LVSR_LAUNCH_CHECK();
     if (int rc = gemm_tn(ws, hid, Hd, dlogits, V, R, Hd, V, grad(top + ".W"), V, false, st)) return rc;
     if (int rc = colsum(dlogits, R, V, V, grad(top + ".b"), false, st)) return rc;
@@ -654,13 +682,12 @@ struct TrainStep {
 // forward + backward of one batch on the parameters Param::dev points at and the weights packed from them
 int forward_backward(lvsr_model* m, const float* x, const float* mask, const int64_t* labels, const float* lmask,
                      int32_t T, int32_t B, int32_t L, float gscale, float* cost_out, float* grads, void* stream,
-                     const DropoutKey* drop) {
+                     const DropoutKey* drop, const Greedy* greedy) {
   if (int rc = check_ready(m)) return rc;
   LVSR_CHECK(x && labels && cost_out && grads && T > 0 && B > 0 && L > 0, "train_cost_and_grads: bad arguments");
   LVSR_CHECK(!lm_attached(m), "train_cost_and_grads: shallow fusion is inference only (detach the language model)");
-  LVSR_CHECK(!tle_criterion(m), "train_cost_and_grads: the task-loss criteria (mse_gain / mse_reward) are inference only");
   return TrainStep{m, static_cast<cudaStream_t>(stream), labels, lmask, grads, gscale, B, L, lvsr_encoded_length(m, T),
-                   drop, m->reg.penalty_coof}
+                   drop, m->reg.penalty_coof, greedy}
       .run(x, mask, T, cost_out);
 }
 
@@ -669,7 +696,7 @@ int forward_backward(lvsr_model* m, const float* x, const float* mask, const int
 // marked un-finalized, so any other entry point re-packs from the means first.
 int forward_backward_on(lvsr_model* m, const float* copy, const float* x, const float* mask, const int64_t* labels,
                         const float* lmask, int32_t T, int32_t B, int32_t L, float gscale, float* cost_out, float* grads,
-                        void* stream, const DropoutKey* drop) {
+                        void* stream, const DropoutKey* drop, const Greedy* greedy) {
   struct Restore {
     lvsr_model* m;
     ~Restore() {
@@ -680,16 +707,14 @@ int forward_backward_on(lvsr_model* m, const float* copy, const float* x, const 
   } restore{m};
   for (Param& p : m->params) p.dev = const_cast<float*>(copy) + p.offset;
   if (int rc = finalize_on_stream(m, static_cast<cudaStream_t>(stream), false)) return rc;
-  return forward_backward(m, x, mask, labels, lmask, T, B, L, gscale, cost_out, grads, stream, drop);
+  return forward_backward(m, x, mask, labels, lmask, T, B, L, gscale, cost_out, grads, stream, drop, greedy);
 }
 
-}  // namespace
-
-extern "C" {
-
-int lvsr_train_cost_and_grads(lvsr_model* m, const float* x, const float* mask, const int64_t* labels, const float* lmask,
-                              int32_t T, int32_t B, int32_t L, float gscale, float* cost_out, float* grads, void* stream) {
-  DeviceGuard device_guard(m);
+// lvsr_train_cost_and_grads, and with `greedy` its greedy-exploration form: the regularisation in force, then the step
+// on the parameters it perturbs
+int train_cost_and_grads(lvsr_model* m, const float* x, const float* mask, const int64_t* labels, const float* lmask,
+                         int32_t T, int32_t B, int32_t L, float gscale, float* cost_out, float* grads, void* stream,
+                         const Greedy* greedy) {
   LVSR_CHECK(!m || m->cfg.dec_stack == 1,
              "train_cost_and_grads: a stacked decoder (dec_stack %d) is inference only: no backward pass through the "
              "RecurrentStack", m ? m->cfg.dec_stack : 0);
@@ -705,14 +730,43 @@ int lvsr_train_cost_and_grads(lvsr_model* m, const float* x, const float* mask, 
   if (m->noise.on) {
     // adaptive weight noise (noise.cu): the step runs on p + eps sqrt(s2)
     if (int rc = noise_sample(m, st)) return rc;
-    return forward_backward_on(m, m->noise.noisy, x, mask, labels, lmask, T, B, L, gscale, cost_out, grads, stream, drop);
+    return forward_backward_on(m, m->noise.noisy, x, mask, labels, lmask, T, B, L, gscale, cost_out, grads, stream, drop,
+                               greedy);
   }
   if (weight_noise) {
     // weight noise (noise.cu): the step runs on p + level eps, the attention's parameters as they are
     if (int rc = weight_noise_sample(m, st)) return rc;
-    return forward_backward_on(m, r.noisy.get(), x, mask, labels, lmask, T, B, L, gscale, cost_out, grads, stream, drop);
+    return forward_backward_on(m, r.noisy.get(), x, mask, labels, lmask, T, B, L, gscale, cost_out, grads, stream, drop,
+                               greedy);
   }
-  return forward_backward(m, x, mask, labels, lmask, T, B, L, gscale, cost_out, grads, stream, drop);
+  return forward_backward(m, x, mask, labels, lmask, T, B, L, gscale, cost_out, grads, stream, drop, greedy);
+}
+
+}  // namespace
+
+extern "C" {
+
+int lvsr_train_cost_and_grads(lvsr_model* m, const float* x, const float* mask, const int64_t* labels, const float* lmask,
+                              int32_t T, int32_t B, int32_t L, float gscale, float* cost_out, float* grads, void* stream) {
+  DeviceGuard device_guard(m);
+  return train_cost_and_grads(m, x, mask, labels, lmask, T, B, L, gscale, cost_out, grads, stream, nullptr);
+}
+
+int lvsr_train_cost_and_grads_greedy(lvsr_model* m, const float* x, const float* mask, const int64_t* groundtruth,
+                                     int32_t T, int32_t B, int32_t L, float gscale, float* cost_out, float* grads,
+                                     int64_t* prediction, float* prediction_mask, void* stream) {
+  DeviceGuard device_guard(m);
+  LVSR_CHECK(m && groundtruth && prediction && prediction_mask && L > 0, "train_cost_and_grads_greedy: bad arguments");
+  LVSR_CHECK(tle_criterion(m), "train_cost_and_grads_greedy: greedy exploration trains a task-loss criterion "
+             "(mse_gain / mse_reward; lvsr_model_set_criterion)");
+  LVSR_CHECK(m->reg.penalty_coof <= 0.f, "train_cost_and_grads_greedy: the alignment penalty pairs the L + %d generated "
+             "steps with the L-row label mask (lvsr/main.py:411-417): it is undefined under greedy exploration",
+             LVSR_GREEDY_EXTRA_STEPS);
+  LVSR_CHECK(!m->reg.dropout, "train_cost_and_grads_greedy: dropout under greedy exploration picks one of two encoder "
+             "applications in no defined order (lvsr/main.py:400-408)");
+  const Greedy g{groundtruth, L, reinterpret_cast<long long*>(prediction), prediction_mask};
+  return train_cost_and_grads(m, x, mask, prediction, prediction_mask, T, B, L + LVSR_GREEDY_EXTRA_STEPS, gscale,
+                              cost_out, grads, stream, &g);
 }
 
 // Parameters with the WEIGHT role, the subjects of weight decay and max-norm (lvsr/main.py:418-420,493): Linear and

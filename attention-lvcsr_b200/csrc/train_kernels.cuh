@@ -248,9 +248,10 @@ __global__ void __launch_bounds__(SK_WARPS * 32) skinny_kernel(SkinnyArgs a) {
 }
 
 // ------------------------------------------------------------------------------------------
-// Readout + SoftmaxEmitter backward, one warp per (step, row): recomputes the forward of readout_kernel
-// (decoder.cu) and emits  dlogits = (softmax - onehot(label)) * mask * gscale,  hid (post-activation) and
-// dmerged (through Linear^T and Maxout / ReLU / Tanh / Identity and the Bias).
+// Readout + emitter backward, one warp per (step, row): recomputes the forward of readout_kernel (decoder.cu) and
+// emits hid (post-activation) and dmerged (through Linear^T and Maxout / ReLU / Tanh / Identity and the Bias) from
+// dlogits.  SoftmaxEmitter (kTle false) forms dlogits = (softmax - onehot(label)) * mask * gscale itself;
+// RewardRegressionEmitter (kTle true) reads the dlogits tle_loss_grad wrote.
 // ------------------------------------------------------------------------------------------
 struct ReadoutBwdArgs {
   const float* merged;     // [R, Cpm]  states.W_ms + ctx.W_mc
@@ -259,10 +260,11 @@ struct ReadoutBwdArgs {
   const long long* labels; const float* lmask;
   float gscale;
   float* hid;              // [R, Cpm/pieces]
-  float* dlogits;          // [R, V]
+  float* dlogits;          // [R, V]: written (kTle false) or read (kTle true)
   float* dmerged;          // [R, Cpm]
 };
 
+template <bool kTle>
 __global__ void __launch_bounds__(256) readout_bwd_kernel(ReadoutBwdArgs a) {
   extern __shared__ float sh[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -286,33 +288,37 @@ __global__ void __launch_bounds__(256) readout_bwd_kernel(ReadoutBwdArgs a) {
     a.hid[(long long)r * H + j] = v;
   }
   __syncwarp();
-  float logit[4], vmax = -INFINITY;
+  if constexpr (kTle) {
+    for (int v = lane; v < a.V; v += 32) dl[v] = a.dlogits[(long long)r * a.V + v];
+  } else {
+    float logit[4], vmax = -INFINITY;
 #pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    const int v = lane + q * 32;
-    float s = -INFINITY;
-    if (v < a.V) {
-      s = a.bo[v];
-      for (int j = 0; j < H; ++j) s = fmaf(hid[j], __ldg(a.Wo + (long long)j * a.V + v), s);
+    for (int q = 0; q < 4; ++q) {
+      const int v = lane + q * 32;
+      float s = -INFINITY;
+      if (v < a.V) {
+        s = a.bo[v];
+        for (int j = 0; j < H; ++j) s = fmaf(hid[j], __ldg(a.Wo + (long long)j * a.V + v), s);
+      }
+      logit[q] = s;
+      vmax = fmaxf(vmax, s);
     }
-    logit[q] = s;
-    vmax = fmaxf(vmax, s);
-  }
-  vmax = warp_max(vmax);
-  float se = 0.f;
+    vmax = warp_max(vmax);
+    float se = 0.f;
 #pragma unroll
-  for (int q = 0; q < 4; ++q)
-    if (lane + q * 32 < a.V) se += expf(logit[q] - vmax);
-  se = warp_sum(se);
-  const long long lab = a.labels[r];
-  const float w = (a.lmask ? a.lmask[r] : 1.f) * a.gscale;
+    for (int q = 0; q < 4; ++q)
+      if (lane + q * 32 < a.V) se += expf(logit[q] - vmax);
+    se = warp_sum(se);
+    const long long lab = a.labels[r];
+    const float w = (a.lmask ? a.lmask[r] : 1.f) * a.gscale;
 #pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    const int v = lane + q * 32;
-    if (v < a.V) {
-      const float g = (expf(logit[q] - vmax) / se - (v == lab ? 1.f : 0.f)) * w;
-      dl[v] = g;
-      a.dlogits[(long long)r * a.V + v] = g;
+    for (int q = 0; q < 4; ++q) {
+      const int v = lane + q * 32;
+      if (v < a.V) {
+        const float g = (expf(logit[q] - vmax) / se - (v == lab ? 1.f : 0.f)) * w;
+        dl[v] = g;
+        a.dlogits[(long long)r * a.V + v] = g;
+      }
     }
   }
   __syncwarp();

@@ -183,10 +183,15 @@ def train(config, save_path, bokeh_name="", params=None, bokeh_server=None, boke
     `_best_ll` checkpoints, Patience.  Monitoring runs only when config['monitoring'] has validate_every_* /
     search_every_* keys.  Parameters are saved in Blocks checkpoint format."""
     pkg.algorithms.check_trainable_net(config["net"])     # before the model and the data are built
-    data = Data(**config["data"])
-    recognizer = create_model(config, data, params)
     train_conf = config["training"]
     reg_conf = config.get("regularization", {})
+    # lvsr/main.py:245-283; read under a task-loss criterion only, and refused before any device work
+    exploration = pkg.algorithms.check_exploration(
+        config["net"], train_conf.get("exploration", "imitative"),
+        None if reg_conf.get("adaptive_noise") else {k: reg_conf[k] for k in ("dropout", "noise", "penalty_coof")
+                                                     if k in reg_conf})
+    data = Data(**config["data"])
+    recognizer = create_model(config, data, params)
     mon_conf = config.get("monitoring", {})
     adaptive_noise = None
     if reg_conf.get("adaptive_noise"):
@@ -202,6 +207,8 @@ def train(config, save_path, bokeh_name="", params=None, bokeh_server=None, boke
         logger.info("apply noise")
     if reg_conf.get("dropout") or reg_conf.get("noise") or reg_conf.get("penalty_coof", 0.0) > 0:
         extra["regularization"] = {k: reg_conf[k] for k in ("dropout", "noise", "penalty_coof") if k in reg_conf}
+    if exploration != "imitative":
+        extra["exploration"] = exploration
     step_rule = pkg.step_rule_from_config(train_conf, reg_conf)
     if train_conf.get("gradient_threshold"):
         pkg.adaptive_clipping(step_rule, burnin_period=CLIPPING_BURNIN_PERIOD, decay_rate=CLIPPING_DECAY_RATE)

@@ -261,8 +261,9 @@ int lvsr_cost_matrix(lvsr_model* m, const float* attended_dev, const float* atte
  *     with the labels as their own groundtruth (lvsr_cost_matrix_groundtruth takes another one);
  *   - lvsr_initial_states and the beam search start from initial_output (the reference's 0).
  * A groundtruth without eos_label makes the cost call fail naming the utterance; the call synchronises its stream to
- * find out.  Task loss estimation takes no language model and has no training step: lvsr_model_set_criterion refuses a
- * handle with an LM attached, lvsr_model_set_lm and lvsr_train_cost_and_grads refuse a handle with this criterion.
+ * find out.  Task loss estimation takes no language model: lvsr_model_set_criterion refuses a handle with an LM
+ * attached, lvsr_model_set_lm a handle with this criterion.  lvsr_train_cost_and_grads trains it with imitative
+ * exploration (the labels are the prediction), lvsr_train_cost_and_grads_greedy with greedy exploration.
  * Callers that must run on an older library detect the entry point by its symbol. */
 enum { LVSR_CRITERION_LOG_LIKELIHOOD = 0, LVSR_CRITERION_MSE_GAIN = 1, LVSR_CRITERION_MSE_REWARD = 2 };
 typedef struct {
@@ -416,6 +417,26 @@ int lvsr_train_cost_and_grads(lvsr_model* m, const float* recordings_dev, const 
                               int32_t L, float gscale, float* cost_dev, float* grads_dev, void* stream);
 int lvsr_train_apply_updates(lvsr_model* m, float* grads_dev, float gscale, const lvsr_train_config* tc,
                              void* stream);
+/* Under a task-loss criterion (lvsr_model_set_criterion) the cost lvsr_train_cost_and_grads differentiates is the
+ * mse_gain / mse_reward rows of the labels scored against themselves: imitative exploration (lvsr/main.py:245-283).
+ * Such a step synchronises its stream once, after all of its work is enqueued, to report a groundtruth that holds no
+ * eos_label (naming the utterance; the gradient buffer is then undefined).
+ * lvsr_train_cost_and_grads_greedy is the same step under greedy exploration (exploration: greedy):
+ *   1. after the encoder, n = L + LVSR_GREEDY_EXTRA_STEPS steps of generate() on the device with the parameters the
+ *      step runs on (under adaptive noise or weight noise, the noisy ones): prediction_dev [n, B] (int64) is the
+ *      arg-max of the readouts at every step (the first on ties), from the state the previous pick fed;
+ *   2. prediction_mask_dev [n, B] = 1 at step 0 and wherever no eos_label occurs in the earlier steps of the row;
+ *   3. the step of lvsr_train_cost_and_grads on labels = the prediction, labels mask = its mask, with the rewards and
+ *      gains of the prediction against groundtruth_dev [L, B] (every utterance of which must hold eos_label).
+ * No gradient flows through the generation.  The groundtruth's mask plays no part: the prediction's own mask weights
+ * the cost, as in the reference.  Refused: a log-likelihood handle; dropout and the alignment penalty, which the
+ * reference leaves undefined under greedy exploration (its dropout graph holds two encoder applications, and its
+ * penalty pairs n rows of alignments with the L-row label mask).  Detected by symbol. */
+enum { LVSR_GREEDY_EXTRA_STEPS = 10 };
+int lvsr_train_cost_and_grads_greedy(lvsr_model* m, const float* recordings_dev, const float* mask_dev,
+                                     const int64_t* groundtruth_dev, int32_t T, int32_t B, int32_t L, float gscale,
+                                     float* cost_dev, float* grads_dev, int64_t* prediction_dev,
+                                     float* prediction_mask_dev, void* stream);
 int lvsr_train_gradient_norm(lvsr_model* m, float* norm_host);   /* total_gradient_norm of the last update (synchronises
                                                                     the handle's stream) */
 int lvsr_train_reset(lvsr_model* m);     /* zero the optimizer state, enqueued on the handle's stream after its updates */
