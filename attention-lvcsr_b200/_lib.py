@@ -178,6 +178,7 @@ SIGNATURES = {
     "lvsr_tle_matrices": (C.c_int, [_P, _P, _I, _P, _I, _I, _P, _P, _P]),
     "lvsr_initial_states": (C.c_int, [_P, _I, _I, _P, _P, _P, _P, _P, _P, _P]),
     "lvsr_logprobs": (C.c_int, [_P, _P, _P, _P, _I, _I, _P, _I, _P, _P, _P, _P, _P]),
+    "lvsr_logprobs_lm": (C.c_int, [_P, _P, _P, _P, _I, _I, _P, _I, _P, _P, _P, _P, _P, _P]),
     "lvsr_next_states": (C.c_int, [_P, _P, _P, _P, _I, _I, _P, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "lvsr_beam_search_many": (C.c_int, [_P, _P, _P, _P, _I, _I, _P, _P, _I, _I, _I, C.c_double, C.c_double, _I, VALIDATE_FN,
                                         _P, C.POINTER(_P), _P]),

@@ -661,7 +661,6 @@ int lvsr_model_set_lm(lvsr_model* m, int32_t num_states, int32_t start, const in
   LVSR_CHECK(m && off && fusion && num_states > 0 && num_arcs >= 0 && (num_arcs == 0 || (label && next && weight)),
              "set_lm: bad arguments");
   LVSR_CHECK(start >= 0 && start < num_states, "set_lm: start state %d outside [0, %d)", start, num_states);
-  LVSR_CHECK(!tle_criterion(m), "set_lm: a task-loss criterion (mse_gain / mse_reward) takes no language model");
   LVSR_CHECK(off[0] == 0 && off[num_states] == num_arcs, "set_lm: arc offsets must run from 0 to num_arcs");
   const int V = m->cfg.num_phonemes;
   for (int32_t s = 0; s < num_states; ++s) {
@@ -1097,7 +1096,6 @@ int lvsr_model_set_criterion(lvsr_model* m, const lvsr_criterion* cr) {
   LVSR_CHECK(cr->name == LVSR_CRITERION_LOG_LIKELIHOOD || cr->name == LVSR_CRITERION_MSE_GAIN ||
                  cr->name == LVSR_CRITERION_MSE_REWARD, "set_criterion: unknown criterion %d", cr->name);
   if (cr->name != LVSR_CRITERION_LOG_LIKELIHOOD) {
-    LVSR_CHECK(!lm_attached(m), "set_criterion: a task-loss criterion takes no language model (detach it first)");
     LVSR_CHECK(cr->eos_label >= 0 && cr->eos_label < V, "set_criterion: eos_label %d outside [0, %d)", cr->eos_label, V);
     LVSR_CHECK(cr->initial_output >= 0 && cr->initial_output <= V, "set_criterion: initial_output %d outside [0, %d]",
                cr->initial_output, V);
@@ -1279,8 +1277,10 @@ int lvsr::cost_matrix(lvsr_model* m, const float* attended, const float* attende
     if (int rc = readout_body(m, ws, R, merged, true, &tail, nullptr, st)) return rc;
     ReadoutArgs r = readout_args(m, R, tail);
     r.poison = scanned ? m->status.get() : nullptr;
+    if (lm_add) lm_fuse(m, r, lm_add);
     if (tle) {
-      // RewardRegressionEmitter.cost over the whole readouts (lvsr/bricks/__init__.py:135-184)
+      // RewardRegressionEmitter.cost over the whole readouts (lvsr/bricks/__init__.py:135-184); with a language model
+      // these are the fused readouts x, whose LM rows follow the labels (the prediction), not the groundtruth
       float* neg = keep ? keep->neg : ws.f32((size_t)R * c.num_phonemes);
       LVSR_CHECK(neg, "out of device memory (task-loss readouts)");
       r.costs_all = neg;
@@ -1289,7 +1289,6 @@ int lvsr::cost_matrix(lvsr_model* m, const float* attended, const float* attende
                              costs, keep, st)) return rc;
     } else {
       r.labels = lab; r.lmask = labels_mask; r.costs_picked = costs;
-      if (lm_add) lm_fuse(m, r, lm_add);
       if (int rc = readout_costs(r, st)) return rc;
     }
   }
@@ -1362,12 +1361,20 @@ int lvsr_initial_states(lvsr_model* m, int32_t Tp, int32_t R, float* states, int
 int lvsr_logprobs(lvsr_model* m, const float* attended, const float* preprocessed, const float* attended_mask,
                   int32_t Tp, int32_t U, const int32_t* row_utt, int32_t R, const float* states,
                   const float* weights, const int64_t* step, float* out, void* stream) {
+  return lvsr_logprobs_lm(m, attended, preprocessed, attended_mask, Tp, U, row_utt, R, states, weights, step, nullptr,
+                          out, stream);
+}
+
+int lvsr_logprobs_lm(lvsr_model* m, const float* attended, const float* preprocessed, const float* attended_mask,
+                     int32_t Tp, int32_t U, const int32_t* row_utt, int32_t R, const float* states,
+                     const float* weights, const int64_t* step, const float* lm_add, float* out, void* stream) {
   DeviceGuard device_guard(m);
   if (int rc = bind_stream(m, static_cast<cudaStream_t>(stream))) return rc;
   if (int rc = check_ready(m)) return rc;
   LVSR_CHECK(attended && attended_mask && states && weights && step && out && Tp > 0 && U > 0 && R > 0,
              "logprobs: bad arguments");
   LVSR_CHECK(row_utt || U == R, "logprobs: without row_utt the contexts must be replicated (U == R)");
+  LVSR_CHECK(!lm_add || lm_attached(m), "logprobs: language-model cost rows given but no language model attached");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   ArenaScope scope(m, st);
   const lvsr_config& c = m->cfg;
@@ -1390,6 +1397,7 @@ int lvsr_logprobs(lvsr_model* m, const float* attended, const float* preprocesse
   if (int rc = readout_merged(m, R, states, ctx, merged, &tail, st)) return rc;
   ReadoutArgs r = readout_args(m, R, tail);
   r.costs_all = out;
+  if (lm_add) lm_fuse(m, r, lm_add);
   return readout_costs(r, st);
 }
 

@@ -172,7 +172,11 @@ __device__ __forceinline__ void readout_fused(const ReadoutArgs& a, int r, int l
 }
 
 // One warp per row.  kTle: RewardRegressionEmitter.costs (lvsr/bricks/__init__.py:194-196), the costs are -readouts.
-template <bool kTle>
+// kTleLm (with kTle, a.lm_add set): those readouts go through ShallowFusionReadout first, as the log-likelihood
+// instantiation's fused rows do (lvsr/bricks/recognizer.py:285-297, 323-338: only the SoftmaxEmitter is swapped for
+// LMEmitter, so the task-loss emitter's costs are -x of the fused x).  An instantiation of its own, so that the two
+// emitters' paths without a language model keep their code.
+template <bool kTle, bool kTleLm = false>
 __global__ void __launch_bounds__(256) readout_kernel(ReadoutArgs a) {
   extern __shared__ float sh[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -209,6 +213,10 @@ __global__ void __launch_bounds__(256) readout_kernel(ReadoutArgs a) {
     }
     logit[q] = s;
     vmax = fmaxf(vmax, s);
+  }
+  if constexpr (kTleLm) {
+    readout_fused(a, r, lane, logit);
+    return;
   }
   if constexpr (kTle) {
     const long long lab = a.labels ? a.labels[r] : -1;
@@ -365,8 +373,8 @@ int readout_costs(const ReadoutArgs& a, cudaStream_t stream) {
   LVSR_CHECK(a.pieces >= 1 && a.Cpm % a.pieces == 0, "readout: bad maxout pieces");
   const size_t smem = readout_smem_bytes(a.Cpm / a.pieces);
   LVSR_CHECK(smem <= READOUT_SMEM_LIMIT, "readout: post_merge_dim too large");
-  LVSR_CHECK(!(a.tle && a.lm_add), "readout: the task-loss emitter takes no language model");
-  if (a.tle) readout_kernel<true><<<ceil_div(a.R, 8), 256, smem, stream>>>(a);
+  if (a.tle && a.lm_add) readout_kernel<true, true><<<ceil_div(a.R, 8), 256, smem, stream>>>(a);
+  else if (a.tle) readout_kernel<true><<<ceil_div(a.R, 8), 256, smem, stream>>>(a);
   else readout_kernel<false><<<ceil_div(a.R, 8), 256, smem, stream>>>(a);
   LVSR_LAUNCH_CHECK();
   return 0;

@@ -204,7 +204,8 @@ struct ReadoutArgs {
   const float* lm_add;     // [R, V] or nullptr
   float lm_weight, am_beta;
   int norm_am, norm_lm, norm_tot;
-  // RewardRegressionEmitter (lvsr/bricks/__init__.py:119-202): the costs are -readouts, no log-softmax (lm_add unused)
+  // RewardRegressionEmitter (lvsr/bricks/__init__.py:119-202): the costs are -readouts, no log-softmax; with lm_add the
+  // readouts are the fused x above, so the costs are -x as under the SoftmaxEmitter
   int tle;
 };
 int readout_costs(const ReadoutArgs& a, cudaStream_t stream);

@@ -718,6 +718,9 @@ int train_cost_and_grads(lvsr_model* m, const float* x, const float* mask, const
   LVSR_CHECK(!m || m->cfg.dec_stack == 1,
              "train_cost_and_grads: a stacked decoder (dec_stack %d) is inference only: no backward pass through the "
              "RecurrentStack", m ? m->cfg.dec_stack : 0);
+  LVSR_CHECK(!m || !(tle_criterion(m) && lm_attached(m)),
+             "train_cost_and_grads: shallow fusion is inference only: a task-loss handle with a language model decodes "
+             "and scores (detach the language model)");
   if (int rc = bind_stream(m, static_cast<cudaStream_t>(stream))) return rc;
   const lvsr_model::Reg& r = m->reg;
   const bool weight_noise = r.level > 0.f;

@@ -109,9 +109,8 @@ class SpeechRecognizer(object):
         criterion = dict(criterion) if criterion else dict(name="log_likelihood")
         if criterion["name"] not in _lib.CRITERIA:
             raise ValueError("Unknown criterion {}".format(criterion["name"]))       # recognizer.py:297
-        if lm and criterion["name"] != "log_likelihood":
-            # the reference would fuse the LM into RewardRegressionEmitter's raw readouts
-            unsupported("criterion %r with a language model" % criterion["name"])
+        # with a task-loss criterion and an LM, RewardRegressionEmitter stays and reads the fused readouts
+        # (lvsr/bricks/recognizer.py:285-297, 323-338): only SoftmaxEmitter is swapped for LMEmitter
         # SpeechBottom (lvsr/bricks/recognizer.py:105-157): an MLP of one Linear + activation per entry of dims, Tanh
         # when the activation is None; Identity when dims is empty
         bottom = dict(bottom or {})
@@ -852,8 +851,9 @@ class SpeechRecognizer(object):
         draws differ from the reference while their distribution does not), ``sample=False`` emits the arg-max.
         Returns dict(outputs [n,B] int64, costs [n,B] = -log p(emitted), states [n,B,dim_state], weights [n,B,T']).
         Under task loss estimation RewardRegressionEmitter emits the arg-max of the readouts whatever ``sample`` says,
-        and the costs are the emitted readouts (its cost, lvsr/bricks/__init__.py:185-192)."""
-        if self.lm:
+        and the costs are the emitted readouts (its cost, lvsr/bricks/__init__.py:185-192); with a language model
+        these are the fused readouts, and the LM state of every row advances by its emitted symbol."""
+        if self.lm and not self.tle:
             # LMEmitter.emit returns zeros in the reference: generating with an LM is not defined there
             raise NotImplementedError("attention-lvcsr_b200: generate / sample with a language model")
         torch = self._torch()
@@ -863,6 +863,8 @@ class SpeechRecognizer(object):
             n_steps = int(np.asarray(recordings).shape[0] / self.max_decoded_length_scale)
         ctx = dict(attended=att, attended_mask=attm, preprocessed=self.preprocess(att))
         st = self._initial_states(Tp, B)
+        if self.lm:
+            st.update(self._lm_initial_states(B))
         gen = None
         if sample:
             gen = torch.Generator(device=self.device)
@@ -876,7 +878,9 @@ class SpeechRecognizer(object):
                 y = neglogp.argmin(dim=1)
             picked = neglogp.gather(1, y[:, None])[:, 0]
             costs.append(-picked if self.tle else picked)
+            lm_st = self._lm_next_states(st, y) if self.lm else {}
             st = self._next_states(ctx, st, y)
+            st.update(lm_st)
             outs.append(y)
             states.append(st["states"])
             weights.append(st["weights"])
@@ -963,17 +967,25 @@ class SpeechRecognizer(object):
         return self._dev(ru, torch.int32)
 
     def _logprobs(self, contexts, st):
+        """The emitter costs [R, V] of the rows of st; fused with the language model when st carries its cost rows
+        (``lm_add``, from _lm_initial_states / _lm_next_states)."""
         torch = self._torch()
         lib, h = _lib.load(), self._require_ready()
         att = contexts["attended"]
         Tp, U, _ = att.shape
         R = st["states"].shape[0]
         ru = self._row_utt(contexts, R)
-        out = torch.empty((R, self.net["num_phonemes"]), dtype=torch.float32, device=self.device)
-        _lib.check(lib.lvsr_logprobs(h, _ptr(att), _ptr(contexts.get("preprocessed")), _ptr(contexts["attended_mask"]),
-                                     Tp, U, _ptr(ru), R, _ptr(st["states"].contiguous()),
-                                     _ptr(st["weights"].contiguous()), _ptr(st["step"].contiguous()), _ptr(out),
-                                     self._stream()))
+        V = self.net["num_phonemes"]
+        out = torch.empty((R, V), dtype=torch.float32, device=self.device)
+        lm_add = st.get("lm_add")
+        if lm_add is not None:
+            lm_add = self._dev(lm_add, torch.float32)
+            if tuple(lm_add.shape) != (R, V):      # the C ABI reads R rows of V
+                raise ValueError("logprobs: lm_add must be [%d, %d], got %s" % (R, V, tuple(lm_add.shape)))
+        _lib.check(lib.lvsr_logprobs_lm(h, _ptr(att), _ptr(contexts.get("preprocessed")), _ptr(contexts["attended_mask"]),
+                                        Tp, U, _ptr(ru), R, _ptr(st["states"].contiguous()),
+                                        _ptr(st["weights"].contiguous()), _ptr(st["step"].contiguous()), _ptr(lm_add),
+                                        _ptr(out), self._stream()))
         return out
 
     def _next_states(self, contexts, st, outputs):

@@ -261,9 +261,12 @@ int lvsr_cost_matrix(lvsr_model* m, const float* attended_dev, const float* atte
  *     with the labels as their own groundtruth (lvsr_cost_matrix_groundtruth takes another one);
  *   - lvsr_initial_states and the beam search start from initial_output (the reference's 0).
  * A groundtruth without eos_label makes the cost call fail naming the utterance; the call synchronises its stream to
- * find out.  Task loss estimation takes no language model: lvsr_model_set_criterion refuses a handle with an LM
- * attached, lvsr_model_set_lm a handle with this criterion.  lvsr_train_cost_and_grads trains it with imitative
- * exploration (the labels are the prediction), lvsr_train_cost_and_grads_greedy with greedy exploration.
+ * find out.  lvsr_train_cost_and_grads trains it with imitative exploration (the labels are the prediction),
+ * lvsr_train_cost_and_grads_greedy with greedy exploration.
+ * With a language model attached (in either order with lvsr_model_set_lm) the readouts r become the fused readouts x
+ * of shallow fusion (below): every emitter cost is -x, the same row the log-likelihood emitter writes under fusion,
+ * and the losses above take x in place of r, with the LM rows along the labels (the prediction).  Both training entry
+ * points refuse such a handle before any device work.
  * Callers that must run on an older library detect the entry point by its symbol. */
 enum { LVSR_CRITERION_LOG_LIKELIHOOD = 0, LVSR_CRITERION_MSE_GAIN = 1, LVSR_CRITERION_MSE_REWARD = 2 };
 typedef struct {
@@ -311,6 +314,13 @@ int lvsr_logprobs(lvsr_model* m, const float* attended_dev, const float* preproc
                   const float* attended_mask_dev, int32_t Tp, int32_t U, const int32_t* row_utt_dev,
                   int32_t R, const float* states_dev, const float* weights_dev, const int64_t* step_dev,
                   float* neg_logprobs_dev, void* stream);
+/* lvsr_logprobs fused with the language model: lm_add_dev [R, V] is each row's LM cost row (lvsr_lm_initial_states /
+ * lvsr_lm_next_states), and the output is the emitter cost -x of the fused readouts x, the row lvsr_beam_search_many
+ * selects on.  lm_add_dev NULL: lvsr_logprobs.  lvsr_logprobs itself never fuses. */
+int lvsr_logprobs_lm(lvsr_model* m, const float* attended_dev, const float* preprocessed_dev,
+                     const float* attended_mask_dev, int32_t Tp, int32_t U, const int32_t* row_utt_dev,
+                     int32_t R, const float* states_dev, const float* weights_dev, const int64_t* step_dev,
+                     const float* lm_add_dev, float* neg_logprobs_dev, void* stream);
 int lvsr_next_states(lvsr_model* m, const float* attended_dev, const float* preprocessed_dev,
                      const float* attended_mask_dev, int32_t Tp, int32_t U, const int32_t* row_utt_dev,
                      int32_t R, const float* states_dev, const float* weights_dev, const int64_t* step_dev,
@@ -350,7 +360,8 @@ int lvsr_search_result_destroy(lvsr_search_result* r);
  * [arc_offsets[s], arc_offsets[s+1]) (arc_offsets has num_states + 1 entries), arc_label = NN symbol + 1 with
  * 0 = epsilon, each state's arcs sorted by (label, next state); arc weights are costs (negative log).  While it is
  * attached, lvsr_cost_matrix (and so lvsr_recognizer_cost_host) and lvsr_beam_search_many return the costs of
- * ShallowFusionReadout + LMEmitter instead of -log softmax, and lvsr_train_cost_and_grads refuses to run.
+ * ShallowFusionReadout + LMEmitter instead of -log softmax (under task loss estimation: the loss of the fused readouts),
+ * and lvsr_train_cost_and_grads refuses to run.
  * lvsr_cost_matrix then synchronises its stream once, to report an LM error.  lvsr_model_clear_lm detaches it.
  *
  * The LM state of a row is a set of at most LVSR_LM_MAX_STATES (fst state int32, weight float64) pairs padded with
